@@ -710,8 +710,10 @@ int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, in
 
 // Sine-mode tile batch (tile_t::create_zvals / create_texture in force_sine_mode): tables once per distinct tile column / row, then ONE grid launch per
 // <= 65535 tiles. h_org = ntiles (mx0, my0) pairs (HOST; mx0 = dx*float(x1 - MESH_X_SIZE/2) as build_arrays computes it).
+size_t twi_sine_tiles_stage_bytes(uint32_t ntiles) {return (size_t)ntiles*(2*sizeof(float) + sizeof(uint2) + sizeof(float2));} // distinct origins (<= 2 per tile), table indices, origins
+
 int twi_heightgen_sine_tiles(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin, const float2 *h_org, uint32_t ntiles,
-                             float *d_out, unsigned *d_mm_ord)
+                             float *d_out, unsigned *d_mm_ord, void *h_stage)
 {
 	if (!ctx->have_sine_params) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sine_params() has not been called");
 	unsigned const nx = g->nx, ny = g->ny;
@@ -742,9 +744,16 @@ int twi_heightgen_sine_tiles(tw_ctx *ctx, const tw_grid2d *g, const tw_height_pa
 	uint2 *d_tabs = (uint2 *)sp; sp += tt_bytes;
 	float2 *d_torg = (float2 *)sp;
 	std::vector<float> uorg(ux); uorg.insert(uorg.end(), uy.begin(), uy.end());
-	TW_CUDA(ctx, cudaMemcpyAsync(d_uorg, uorg.data(), uorg.size()*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(d_tabs, tabs.data(), (size_t)ntiles*sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(d_torg, h_org, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+	const void *src_uorg = uorg.data(), *src_tabs = tabs.data(), *src_org = h_org;
+	if (h_stage) { // pinned copies that outlive this call: nothing below has to wait for the uploads
+		char *hs = (char *)h_stage;
+		memcpy(hs, uorg.data(), uorg.size()*sizeof(float)); src_uorg = hs; hs += (size_t)2*ntiles*sizeof(float);
+		memcpy(hs, tabs.data(), (size_t)ntiles*sizeof(uint2)); src_tabs = hs; hs += (size_t)ntiles*sizeof(uint2);
+		memcpy(hs, h_org, (size_t)ntiles*sizeof(float2)); src_org = hs;
+	}
+	TW_CUDA(ctx, cudaMemcpyAsync(d_uorg, src_uorg, uorg.size()*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+	TW_CUDA(ctx, cudaMemcpyAsync(d_tabs, src_tabs, (size_t)ntiles*sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
+	TW_CUDA(ctx, cudaMemcpyAsync(d_torg, src_org, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
 	SineTabParams S;
 	memset(&S, 0, sizeof(S));
 	S.msx = p->mesh_scale*p->dx_val_inv; S.msy = p->mesh_scale*p->dy_val_inv; S.ms2 = (float)(0.5*p->mesh_scale);
@@ -767,7 +776,7 @@ int twi_heightgen_sine_tiles(tw_ctx *ctx, const tw_grid2d *g, const tw_height_pa
 			ctx->d_sin_table, d_mm_ord ? d_mm_ord + 2*(size_t)t0 : nullptr, 0, d_tabs + t0, d_torg + t0, xstride, ystride);
 		TW_LAUNCH_CHECK(ctx);
 	}
-	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the host vectors above are read by the async copies
+	if (!h_stage) {TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));} // the host vectors above are read by the async copies
 	return TW_OK;
 }
 

@@ -7,12 +7,23 @@
 #include <string.h>
 #include "../../include/tw3d.h"
 
+// The one asynchronous job a context may have in flight (tw_heightgen_2d_launch or tw_create_tiles_launch). `done` is recorded on ctx->stream
+// after everything the job enqueued (the tile pipeline's other streams are joined into ctx->stream first); the small per-tile results are staged
+// in ctx->h_pinned at the offsets below and unpacked into the caller's host arrays by the poll that reports completion.
 struct tw_async_state {
 	bool pending = false;
+	bool tiles = false;             // the pending job is a tile job (else a 2-D grid)
 	cudaEvent_t done = nullptr;
 	float *host_out = nullptr;      // user host buffer (nullptr => result stays on device)
 	tw_minmax *host_mm = nullptr;
 	uint32_t n_mm = 0;
+	// tile job: where the staged results go and what the bounds combination needs
+	tw_tile_bounds *host_bounds = nullptr;
+	float *host_min_nz = nullptr;
+	bool steps = false;             // an erosion step counter is staged
+	float dx = 0.0f, dy = 0.0f;
+	uint32_t size = 0;
+	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0; // byte offsets into ctx->h_pinned
 };
 
 struct tw_ctx {
@@ -46,6 +57,7 @@ struct tw_ctx {
 };
 
 int  tw_set_error(tw_ctx *ctx, int status, const char *fmt, ...);
+int  twi_finish_pending(tw_ctx *ctx);                           // completes the context's pending asynchronous job (if any) before other work reuses its scratch
 int  tw_reserve(tw_ctx *ctx, int slot, size_t bytes);           // grow d_scratch[slot]; returns TW_OK / TW_ERR_CUDA
 int  tw_reserve_pinned(tw_ctx *ctx, size_t bytes);
 bool tw_is_device_ptr(const void *p);
@@ -91,13 +103,19 @@ __host__ __device__ inline float tw_ord2f(unsigned u) {
 int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin,
                   const float2 *d_tile_origins, uint32_t ntiles, float *d_out, unsigned *d_mm_ord, float *h_out_bands = nullptr);
 int twi_tile_weights(tw_ctx *ctx, const float *d_zvals, const float *d_rand, uint32_t ntiles, uint32_t zvsize, const float *d_tile_params, const tw_weight_params *W, uint8_t *d_out, uint8_t *d_flags);
+// h_stage (optional): pinned host staging of twi_sine_tiles_stage_bytes(ntiles) bytes that stays untouched until the enqueued work is done; without it
+// the call synchronises ctx->stream before it returns (its host-side index tables are locals)
 int twi_heightgen_sine_tiles(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin, const float2 *h_org, uint32_t ntiles,
-                             float *d_out, unsigned *d_mm_ord);
+                             float *d_out, unsigned *d_mm_ord, void *h_stage = nullptr);
+size_t twi_sine_tiles_stage_bytes(uint32_t ntiles);
 int twi_ensure_aux_streams(tw_ctx *ctx);
 int twi_erode(tw_ctx *ctx, float *d_maps, uint32_t ntiles, int xsize, int ysize, const float *d_min_zvals, float min_zval_all,
               uint32_t num_iters, const tw_erosion_params *p);
 int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const void *d_origins, uint32_t ntiles, uint32_t zvsize, float *d_out);
-int twi_tile_normals(tw_ctx *ctx, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float dx_val, float dy_val, unsigned char *d_rgba, unsigned *d_min_nz_ord);
+// d_perm (optional): launch tile z handles tile d_perm[z] of d_zvals and of the outputs (the tile pipeline's schedule order)
+int twi_tile_normals(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float dx_val, float dy_val, unsigned char *d_rgba, unsigned *d_min_nz_ord,
+                     const unsigned *d_perm = nullptr);
+int twi_fill_u32(tw_ctx *ctx, cudaStream_t st, unsigned *d_vals, size_t n, unsigned value);
 int twi_tile_ao(tw_ctx *ctx, const float *d_zvals, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float half_dxy, bool ctx_inside, unsigned char *d_ao);
 int twi_tile_cut(tw_ctx *ctx, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float *d_zvals);
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
@@ -115,7 +133,7 @@ int twi_sweep_walk(tw_ctx *ctx, float *P, long long *D, int xsize, int ysize, in
 int twi_sweep_add(tw_ctx *ctx, long long *D, const long long *R, size_t n);
 int twi_sweep_apply(tw_ctx *ctx, float *P, long long *D, size_t n);
 int twi_sweep_unpad(tw_ctx *ctx, const float *P, int E0, int xsize, int y0, int y1, float min_zval, float *out);
-int twi_tile_bounds(tw_ctx *ctx, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float wpz_max, void *d_sub);
+int twi_tile_bounds(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float wpz_max, void *d_sub, const unsigned *d_perm = nullptr);
 int twi_glaciate_mesh(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, unsigned *d_mm);
 int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out);
 int twi_from_floats_u16(tw_ctx *ctx, const float *d_vals, size_t n, float val_mult, float val_add, uint8_t *d_out, unsigned *d_bad);

@@ -121,6 +121,7 @@ extern "C" int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int3
 {
 	if (!ctx || !zvals || !tile_xy || !sp || !smask || ntiles == 0 || zvsize < 2) return TW_ERR_ARG;
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
 	int const n = (int)zvsize;
 	size_t const cells = (size_t)ntiles*n*n, edge = (size_t)ntiles*n;

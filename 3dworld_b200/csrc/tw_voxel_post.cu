@@ -251,6 +251,7 @@ unsigned stream_grid(const tw_ctx *ctx, size_t n) {size_t const b = (n + 255)/25
 extern "C" int tw_voxel_outside(tw_ctx *ctx, const float *vals, const tw_voxel_post_params *vp, const uint32_t *zix_xy, uint8_t *outside) {
 	if (!ctx || !vals || !outside) return TW_ERR_ARG;
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
 	int rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz, nxy = (size_t)vp->nx*vp->ny;
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_z = (zix_xy && tw_is_device_ptr(zix_xy));
@@ -288,6 +289,7 @@ static int run_flood(tw_ctx *ctx, unsigned char *d_o, const tw_voxel_post_params
 extern "C" int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *outside, const tw_voxel_post_params *vp, uint64_t *changed) {
 	if (!ctx || !vals || !outside) return TW_ERR_ARG;
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
 	int rc = validate(ctx, vp); if (rc) return rc;
 	if (changed) *changed = 0;
 	if (vp->remove_unconnected <= 0) return TW_OK;
@@ -339,6 +341,7 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 {
 	if (!ctx || !vals || !outside || !edge_table256 || !tri_table256x16 || !edge_to_vals12x2 || !ntris || (capacity && !tris)) return TW_ERR_ARG;
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
 	int rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);

@@ -5,6 +5,7 @@
 //   tw3d::noise_gen_3d           <->  noise_gen_3d::{set_rand_seeds,gen_sines}        src/upsurface.h:39-50
 //   tw3d::create_procedural      <->  voxel_manager::create_procedural               src/voxels.h:196, src/voxels.cpp:278-346
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
+//   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //
 // The reference reads ~20 globals on this path (SURVEY.md 8b); here they are one explicit struct (scene_globals) set once per scene
 // with set_globals(). Same names, argument meaning and error behaviour as the reference: argument errors assert/abort like the
@@ -12,6 +13,7 @@
 // No CPU fallback: all grid evaluation happens on the GPU through the C ABI; without a device ctx() fails.
 #pragma once
 #include <tw3d.h>
+#include <atomic>
 #include <cassert>
 #include <cmath>
 #include <cstdio>
@@ -64,13 +66,15 @@ namespace detail {
 	inline state_t &state() {static state_t s; return s;}
 	struct tls_ctx {
 		tw_ctx *c = nullptr; unsigned generation = ~0u;
+		std::atomic<uint64_t> tile_jobs{0}; // create_tiles_async launches on c: a job whose number is no longer the latest was completed by the next launch
 		~tls_ctx() {if (c) tw_destroy(c);}
 	};
+	inline tls_ctx &tls() {static thread_local tls_ctx t; return t;}
 }
 
 // thread-local context (a tw_ctx is not re-entrant); device from $TW3D_DEVICE (default 0)
 inline tw_ctx *ctx() {
-	static thread_local detail::tls_ctx t;
+	detail::tls_ctx &t = detail::tls();
 	detail::state_t &s = detail::state();
 	if (!t.c) {
 		const char *dev = getenv("TW3D_DEVICE");
@@ -258,6 +262,50 @@ inline void create_zvals_batch(const int32_t *origins_xy, unsigned ntiles, unsig
 	// apply_erosion(zvals.data(), zvsize, zvsize, zmin, erosion_iters_tt): min_zval is the global zmin (src/tiled_mesh.cpp:515)
 	int const rc = tw_create_zvals_batch(c, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, zvals_out, mm);
 	if (rc != TW_OK) {detail::fail(rc, "create_zvals_batch", c);}
+}
+
+// A frame's new tiles without stalling the frame - the per-frame pattern of tile_draw_t::update (src/tiled_mesh.cpp:2367-2417, build_arrays(..., no_wait=1)):
+// create_tiles_async() enqueues heights, erosion and the tile tail (tile_bounds, normal map) and returns at once; call ready() on later frames and use the
+// outputs once it returns true (wait() blocks instead). The outputs named in `out` (tw_tile_outputs, include/tw3d.h) must stay valid until then; zvals and
+// normals_rgba may be device memory, or page-locked host memory for a launch that never blocks. One job per context: any other call on this thread's
+// context completes the job first. Not copyable; a handle that is destroyed while its job runs waits for it.
+class tiles_job {
+	tw_ctx *c = nullptr;
+	std::atomic<uint64_t> const *latest = nullptr; // the launch count of c's thread
+	uint64_t number = 0;
+	bool done = true;
+	bool poll(bool wait) {
+		if (done) return true;
+		if (latest->load() != number) {done = true; return true;} // a later launch on the same context completed this job before it started
+		int const rc = tw_create_tiles_poll(c, wait ? 1 : 0);
+		if (rc == TW_ERR_NOT_READY) return false;
+		done = true;
+		if (rc != TW_OK) {detail::fail(rc, "create_tiles_async", c);}
+		return true;
+	}
+public:
+	tiles_job() = default;
+	tiles_job(tw_ctx *ctx_, std::atomic<uint64_t> const *latest_, uint64_t number_) : c(ctx_), latest(latest_), number(number_), done(false) {}
+	tiles_job(tiles_job &&o) noexcept : c(o.c), latest(o.latest), number(o.number), done(o.done) {o.done = true;}
+	tiles_job &operator=(tiles_job &&o) {if (this != &o) {wait(); c = o.c; latest = o.latest; number = o.number; done = o.done; o.done = true;} return *this;}
+	tiles_job(tiles_job const &) = delete;
+	tiles_job &operator=(tiles_job const &) = delete;
+	~tiles_job() {try {wait();} catch (...) {}}
+	bool ready() {return poll(false);}
+	void wait() {poll(true);}
+};
+// wpz_max / size: the water level and tile size of the bounds (tile_t::create_zvals, src/tiled_mesh.cpp:517-541); dx, dy also scale the normals (get_norm)
+inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
+                                    tw_tile_outputs const &out) {
+	scene_globals const &g = globals();
+	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
+	tw_erosion_params const e = erosion_params_from_globals();
+	tw_ctx *c = ctx();
+	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+	uint64_t const number = ++jobs;
+	int const rc = tw_create_tiles_launch(c, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out);
+	if (rc != TW_OK) {detail::fail(rc, "create_tiles_async", c);}
+	return tiles_job(c, &jobs, number);
 }
 
 // heightmap-texture mode of tile_t::create_zvals (src/tiled_mesh.cpp:498-501): zvals[y*zvsize + x] = terrain_hmap_manager.get_clamped_height(x1 + x, y1 + y)

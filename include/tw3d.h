@@ -35,7 +35,7 @@ typedef enum tw_status {
 	TW_ERR_CUDA      = -2,   /* a CUDA runtime call failed; see tw_last_error() */
 	TW_ERR_ARG       = -3,   /* invalid argument (the reference would assert) */
 	TW_ERR_STATE     = -4,   /* tables not set (tw_set_sin_table / tw_set_sine_params) */
-	TW_ERR_NOT_READY = -5    /* tw_heightgen_2d_poll: result not available yet (mirrors build_arrays() returning 0 with no_wait) */
+	TW_ERR_NOT_READY = -5    /* tw_heightgen_2d_poll / tw_create_tiles_poll: result not available yet (mirrors build_arrays() returning 0 with no_wait) */
 } tw_status;
 
 /* mesh_gen_mode values, src/3DWorld.h:1399 */
@@ -115,8 +115,10 @@ typedef struct tw_voxel_params {
  * the GL compute shader of mesh_xy_grid_cache_t src/mesh.h:33). One context = one device, one CUDA stream, its scratch buffers and the
  * uploaded tables; not re-entrant (use one per thread). tw_create fails with TW_ERR_NO_DEVICE when there is no GPU - there is no CPU fallback.
  * Every call makes the context's device the calling thread's current CUDA device (cudaSetDevice) and leaves it so.
- * Host output buffers: asynchronous entry points (tw_heightgen_2d_launch) overlap the device->host copy with compute only when the buffer is
- * page-locked (cudaHostAlloc / cudaHostRegister / tw_multi_alloc_host); with pageable memory the copy - and therefore the launch call - blocks. */
+ * Host output buffers: asynchronous entry points (tw_heightgen_2d_launch, tw_create_tiles_launch) overlap the device->host copy with compute only when
+ * the buffer is page-locked (cudaHostAlloc / cudaHostRegister / tw_multi_alloc_host); with pageable memory the copy - and therefore the launch call - blocks.
+ * A context has at most one asynchronous job in flight: every other call on it (including the next launch) first completes the pending job, exactly
+ * as a poll with wait = 1 would, and either poll function completes whichever job is pending. */
 TW_API int  tw_abi_version(void);
 TW_API int  tw_create(int device, tw_ctx **out);
 TW_API void tw_destroy(tw_ctx *ctx);
@@ -248,10 +250,36 @@ TW_API int tw_erode_tiles(tw_ctx *ctx, float *heightmaps, uint32_t ntiles, int x
  * exactly tw_heightgen_tiles followed by tw_erode_tiles(min_zval_all = min_zval) in one call (one upload of the origins, one download of
  * the result, per-tile z range fused). When memory forces several chunks, generation of chunk k+1 is issued on a separate stream and
  * overlaps the droplet walk of chunk k. mm (optional, HOST, ntiles entries) receives
- * the per-tile z range AFTER erosion (mzmin/mzmax). erosion_iters == 0 or erode_amount <= 0 => height fill only. */
+ * the per-tile z range AFTER erosion (mzmin/mzmax). erosion_iters == 0 or erode_amount <= 0 => height fill only.
+ * Blocks until the result is complete: it is tw_create_tiles_launch (below) with zvals and mm only, followed by tw_create_tiles_poll(wait = 1). */
 TW_API int tw_create_zvals_batch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
                           uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
                           float *out, tw_minmax *mm);
+/* Asynchronous form of a frame's new tiles (tile_draw_t::update creates them with build_arrays(..., no_wait=1) and collects them on a later frame,
+ * src/tiled_mesh.cpp:2367-2417): tw_create_tiles_launch enqueues tw_create_zvals_batch AND the tile tail - tw_tile_bounds_batch(wpz_max, dx, dy, size)
+ * and tw_tile_normals_batch(dx, dy) - on the context's streams and returns without waiting for the device; tw_create_tiles_poll(wait = 0) only
+ * queries an event and returns TW_ERR_NOT_READY until every requested output is complete (wait = 1 blocks until then); TW_OK when no job is pending.
+ * Every output is bit-identical to the three synchronous calls with the same arguments, and tw_last_erosion_steps() after the completing poll equals
+ * its value after tw_create_zvals_batch. The sub-block bounds and the normal map of a chunk of tiles are computed on the stream that eroded it, right
+ * after its erosion, so they run under the generation and erosion of the other chunks. origins_xy and the parameter structs are copied during the
+ * launch (they may be reused as soon as it returns). Outputs must stay valid until the completing poll:
+ *   zvals         required, ntiles*zvsize^2 floats, host or device
+ *   mm            optional HOST array of ntiles: per-tile z range after erosion (as tw_create_zvals_batch)
+ *   bounds        optional HOST array of ntiles (as tw_tile_bounds_batch; needs zvsize >= 4 with 4*(zvsize/4) < zvsize)
+ *   normals_rgba  optional, ntiles*(zvsize-1)^2*4 bytes, host or device (as tw_tile_normals_batch)
+ *   min_normal_z  optional HOST array of ntiles (needs normals_rgba)
+ * The host arrays mm / bounds / min_normal_z are filled by the poll that reports completion. */
+typedef struct tw_tile_outputs {
+	float          *zvals;
+	tw_minmax      *mm;
+	tw_tile_bounds *bounds;
+	uint8_t        *normals_rgba;
+	float          *min_normal_z;
+} tw_tile_outputs;
+TW_API int tw_create_tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                           uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                           float wpz_max, uint32_t size, const tw_tile_outputs *out);
+TW_API int tw_create_tiles_poll(tw_ctx *ctx, int wait);
 /* droplet steps executed by the last tw_erode/tw_erode_tiles call (sum over droplets; for roofline byte accounting) */
 TW_API uint64_t tw_last_erosion_steps(const tw_ctx *ctx);
 

@@ -87,6 +87,11 @@ class TileOutputs(C.Structure):
     _fields_ = [("zvals", C.c_void_p), ("mm", C.c_void_p), ("bounds", C.c_void_p), ("normals_rgba", C.c_void_p), ("min_normal_z", C.c_void_p)]
 
 
+class TileShading(C.Structure):
+    """tw_tile_shading (include/tw3d.h): the AO map and terrain weights texture tw_create_tiles_launch_ex adds to the tile job (NULL = not requested)."""
+    _fields_ = [("half_dxy", C.c_float), ("wp", C.c_void_p), ("tile_params", C.c_void_p), ("ao", C.c_void_p), ("weights", C.c_void_p), ("has_any_grass", C.c_void_p)]
+
+
 class PointQuery(C.Structure):
     _fields_ = [("kind", C.c_int), ("xy_scale", C.c_float), ("mesh_x_size", C.c_int), ("mesh_y_size", C.c_int), ("x_scene_size", C.c_float),
                 ("y_scene_size", C.c_float), ("xoff2", C.c_int), ("yoff2", C.c_int), ("no_xyoff", C.c_int)]
@@ -118,7 +123,7 @@ def hmap_params(**kw):
 ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_destroy", "tw_last_error", "tw_sync", "tw_stream", "tw_launch_count",
                "tw_build_sin_table", "tw_compute_scale", "tw_gen_sine_params", "tw_gen_rx_ry", "tw_noise3d_gen_sines",
                "tw_water_z_height", "tw_set_sin_table", "tw_set_sine_params", "tw_heightgen_2d", "tw_heightgen_2d_launch",
-               "tw_heightgen_2d_poll", "tw_heightgen_tiles", "tw_create_zvals_batch", "tw_create_tiles_launch", "tw_create_tiles_poll", "tw_tile_bounds_batch", "tw_tile_normals_batch", "tw_tile_ao_batch", "tw_create_zvals_ao_batch", "tw_glaciate_mesh", "tw_eval_points", "tw_erode", "tw_erode_parallel", "tw_erode_tiles", "tw_last_erosion_steps", "tw_voxel_fill",
+               "tw_heightgen_2d_poll", "tw_heightgen_tiles", "tw_create_zvals_batch", "tw_create_tiles_launch", "tw_create_tiles_launch_ex", "tw_create_tiles_poll", "tw_tile_bounds_batch", "tw_tile_normals_batch", "tw_tile_ao_batch", "tw_create_zvals_ao_batch", "tw_glaciate_mesh", "tw_eval_points", "tw_erode", "tw_erode_parallel", "tw_erode_tiles", "tw_last_erosion_steps", "tw_voxel_fill",
                "tw_heightmap_from_floats_u16", "tw_heightmap_to_floats_u16", "tw_proc_gen_heightmap", "tw_heightmap_sample_tiles", "tw_minmax_f32",
                "tw_multi_create", "tw_multi_destroy", "tw_multi_size", "tw_multi_ctx", "tw_multi_last_error", "tw_multi_set_sine_params", "tw_multi_range",
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
@@ -164,6 +169,7 @@ def _load():
                                         C.POINTER(ErosionParams), C.c_float, vp, vp]
     L.tw_create_tiles_launch.argtypes = [vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint32, C.POINTER(HeightParams), C.c_uint32,
                                          C.POINTER(ErosionParams), C.c_float, C.c_float, C.c_uint32, C.POINTER(TileOutputs)]
+    L.tw_create_tiles_launch_ex.argtypes = L.tw_create_tiles_launch.argtypes + [C.POINTER(TileShading)]
     L.tw_create_tiles_poll.argtypes = [vp, C.c_int]
     L.tw_tile_bounds_batch.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_uint32, vp]
     L.tw_glaciate_mesh.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(HeightParams), C.POINTER(MinMax)]
@@ -452,17 +458,32 @@ class Context:
         return (out, mm) if want_minmax else out
 
     def create_tiles_launch(self, origins_xy, mesh_size, dx, dy, zvsize, hp, erosion_iters, ep, min_zval, zvals, mm=None, bounds=None, normals=None,
-                            min_normal_z=None, wpz_max=0.0, size=0):
-        """tw_create_tiles_launch: a frame's new tiles (heights, erosion, z range, sub-block bounds, normal map) enqueued without waiting for the GPU.
-        zvals [nt, zv, zv] float32 and normals [nt, zv-1, zv-1, 4] uint8: numpy arrays (pinned for a launch that does not block) or CUDA tensors;
-        mm [nt, 2] float32, bounds (TileBounds * nt) and min_normal_z [nt] float32 are host arrays that the completing create_tiles_poll fills.
-        The origins are copied during the launch; the outputs are kept referenced here until the job completes."""
+                            min_normal_z=None, wpz_max=0.0, size=0, ao=None, weights=None, has_any_grass=None, half_dxy=None, wp=None, tile_params=None):
+        """tw_create_tiles_launch(_ex): a frame's new tiles (heights, erosion, z range, sub-block bounds, normal map, and on request the AO map and the
+        terrain weights texture) enqueued without waiting for the GPU.
+        zvals [nt, zv, zv] float32, normals [nt, zv-1, zv-1, 4] uint8, ao [nt, zv-1, zv-1] uint8 and weights [nt, zv-1, zv-1, 4] uint8: numpy arrays
+        (pinned for a launch that does not block) or CUDA tensors; mm [nt, 2] float32, bounds (TileBounds * nt) and min_normal_z [nt] float32 are host
+        arrays that the completing create_tiles_poll fills, has_any_grass [nt] uint8 is either. weights needs wp (WeightParams) and tile_params
+        ([nt, 8] float32, host or CUDA); ao takes the ray step half_dxy. In GPU gen modes (3/4) requesting ao makes the zvals those of
+        create_zvals_ao_batch (see tw3d.h). The origins and host tile_params are copied during the launch; the outputs and device inputs are kept
+        referenced here until the job completes."""
         org = np.ascontiguousarray(origins_xy, np.int32).reshape(-1, 2)
         nt = org.shape[0]
         outs = TileOutputs(_ptr(zvals), _ptr(mm), C.cast(bounds, C.c_void_p) if bounds is not None else None, _ptr(normals), _ptr(min_normal_z))
-        self._check(lib.tw_create_tiles_launch(self._h, _ptr(org), nt, mesh_size[0], mesh_size[1], dx, dy, zvsize, C.byref(hp), erosion_iters,
-                                               C.byref(ep) if ep is not None else None, min_zval, wpz_max, size, C.byref(outs)))
-        self._tiles_job = (zvals, mm, bounds, normals, min_normal_z)
+        args = [self._h, _ptr(org), nt, mesh_size[0], mesh_size[1], dx, dy, zvsize, C.byref(hp), erosion_iters, C.byref(ep) if ep is not None else None,
+                min_zval, wpz_max, size, C.byref(outs)]
+        shading = None
+        if ao is not None and half_dxy is None:
+            raise ValueError("create_tiles_launch: ao needs half_dxy (the ray's z step, HALF_DXY)")
+        if ao is not None or weights is not None or has_any_grass is not None:
+            if tile_params is not None and not hasattr(tile_params, "data_ptr"):
+                tile_params = np.ascontiguousarray(tile_params, np.float32)
+            shading = TileShading(0.0 if half_dxy is None else half_dxy, C.cast(C.pointer(wp), C.c_void_p) if wp is not None else None, _ptr(tile_params),
+                                  _ptr(ao), _ptr(weights), _ptr(has_any_grass))
+            self._check(lib.tw_create_tiles_launch_ex(*args, C.byref(shading)))
+        else:
+            self._check(lib.tw_create_tiles_launch(*args))
+        self._tiles_job = (zvals, mm, bounds, normals, min_normal_z, ao, weights, has_any_grass, wp, tile_params, shading)
 
     def create_tiles_poll(self, wait=False):
         """True once the job of create_tiles_launch (or any pending job of this context) is complete, False while it runs (wait=False)."""

@@ -20,10 +20,11 @@ struct tw_async_state {
 	// tile job: where the staged results go and what the bounds combination needs
 	tw_tile_bounds *host_bounds = nullptr;
 	float *host_min_nz = nullptr;
+	uint8_t *host_flags = nullptr;  // has_any_grass
 	bool steps = false;             // an erosion step counter is staged
 	float dx = 0.0f, dy = 0.0f;
 	uint32_t size = 0;
-	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0; // byte offsets into ctx->h_pinned
+	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0, off_flags = 0; // byte offsets into ctx->h_pinned
 };
 
 struct tw_ctx {
@@ -102,12 +103,26 @@ __host__ __device__ inline float tw_ord2f(unsigned u) {
 // entry points implemented in the individual .cu files (called from tw_api.cu)
 int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin,
                   const float2 *d_tile_origins, uint32_t ntiles, float *d_out, unsigned *d_mm_ord, float *h_out_bands = nullptr);
-int twi_tile_weights(tw_ctx *ctx, const float *d_zvals, const float *d_rand, uint32_t ntiles, uint32_t zvsize, const float *d_tile_params, const tw_weight_params *W, uint8_t *d_out, uint8_t *d_flags);
 // h_stage (optional): pinned host staging of twi_sine_tiles_stage_bytes(ntiles) bytes that stays untouched until the enqueued work is done; without it
-// the call synchronises ctx->stream before it returns (its host-side index tables are locals)
+// the call synchronises ctx->stream after the uploads (its host-side index tables are locals)
 int twi_heightgen_sine_tiles(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin, const float2 *h_org, uint32_t ntiles,
                              float *d_out, unsigned *d_mm_ord, void *h_stage = nullptr);
 size_t twi_sine_tiles_stage_bytes(uint32_t ntiles);
+// The same in three steps, for a pipeline that generates the batch chunk by chunk. twi_sine_tiles_plan (host only) finds the batch's distinct tile columns /
+// rows and returns the device memory the tables need; twi_sine_tiles_setup uploads the planned batch (staged in h_stage as above, or synchronously read from
+// h_org and b until the work is done) and builds the tables in d_mem (nullptr: scratch slot 1); twi_sine_tiles_grid generates batch tiles [t0, t0 + nt) -
+// or d_perm[t0 .. t0 + nt) - into consecutive slots of d_out. Setup and grid enqueue on ctx->stream.
+#include <vector>
+struct twi_sine_batch {
+	std::vector<float> uorg; std::vector<uint2> tabs; unsigned nux = 0, nuy = 0; // plan: distinct x then y origins, per-tile table indices
+	tw_grid2d g; tw_height_params p; int enable_glaciate, min_start_sin;
+	float *Xt, *Yt; const uint2 *d_tabs; const float2 *d_torg;
+	size_t xstride, ystride; unsigned xpitch, ypitch;
+};
+size_t twi_sine_tiles_plan(const tw_grid2d *g, const float2 *h_org, uint32_t ntiles, twi_sine_batch *b);
+int twi_sine_tiles_setup(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin, const float2 *h_org, uint32_t ntiles,
+                         void *d_mem, void *h_stage, twi_sine_batch *b);
+int twi_sine_tiles_grid(tw_ctx *ctx, const twi_sine_batch *b, uint32_t t0, uint32_t nt, const unsigned *d_perm, float *d_out, unsigned *d_mm_ord);
 int twi_ensure_aux_streams(tw_ctx *ctx);
 int twi_erode(tw_ctx *ctx, float *d_maps, uint32_t ntiles, int xsize, int ysize, const float *d_min_zvals, float min_zval_all,
               uint32_t num_iters, const tw_erosion_params *p);
@@ -116,8 +131,11 @@ int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sa
 int twi_tile_normals(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float dx_val, float dy_val, unsigned char *d_rgba, unsigned *d_min_nz_ord,
                      const unsigned *d_perm = nullptr);
 int twi_fill_u32(tw_ctx *ctx, cudaStream_t st, unsigned *d_vals, size_t n, unsigned value);
-int twi_tile_ao(tw_ctx *ctx, const float *d_zvals, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float half_dxy, bool ctx_inside, unsigned char *d_ao);
-int twi_tile_cut(tw_ctx *ctx, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float *d_zvals);
+int twi_tile_ao(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float half_dxy, bool ctx_inside, unsigned char *d_ao,
+                const unsigned *d_perm = nullptr);   // d_czv: context grids in launch order
+int twi_tile_cut(tw_ctx *ctx, cudaStream_t st, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float *d_zvals, const unsigned *d_perm = nullptr);
+int twi_tile_weights(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, const float *d_rand, uint32_t ntiles, uint32_t zvsize, const float *d_tile_params, const tw_weight_params *W,
+                     uint8_t *d_out, uint8_t *d_flags, const unsigned *d_perm = nullptr); // d_rand: jitter grids in launch order
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
 int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads);
 size_t   twi_erode_scratch_bytes(const tw_ctx *ctx, uint32_t chunk, int xsize, int ysize);

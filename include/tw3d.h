@@ -193,7 +193,11 @@ TW_API int tw_tile_bounds_batch(tw_ctx *ctx, const float *zvals, uint32_t ntiles
  * tw_create_zvals_ao_batch = tile_t::create_zvals + calc_mesh_ao_lighting with enable_tiled_mesh_ao: heights, per-tile erosion and the AO map
  *   of a batch in one call. GPU gen modes: ONE (stride + 72)^2 generation per tile, zvals cut out of it (:505) - 1.4x less noise work than
  *   tw_create_zvals_batch + tw_tile_ao_batch for 128-tiles - and bit-identical to the reference, whose zvals ARE the context's interior there.
- *   CPU gen modes: zvals generated directly (as the reference does), context generated only outside the tile. zvals/ao host or device, mm optional HOST. */
+ *   CPU gen modes: zvals generated directly (as the reference does), context generated only outside the tile. zvals/ao host or device, mm optional HOST.
+ *   Blocks until the result is complete: it is tw_create_tiles_launch_ex (below) with zvals, mm and ao, followed by tw_create_tiles_poll(wait = 1).
+ *   So it needs the device memory that job needs, as tw_create_zvals_batch does: host zvals / ao are staged whole on the device (n*zvsize^2*4 +
+ *   n*(zvsize-1)^2 bytes) besides about 2 GB of context grids, and in sine mode (gen_mode 0) one batch may hold at most 65535 distinct tile
+ *   columns + rows (TW_ERR_ARG beyond). Split larger batches into several calls. */
 TW_API int tw_tile_normals_batch(tw_ctx *ctx, const float *zvals, uint32_t ntiles, uint32_t zvsize, float dx_val, float dy_val, uint8_t *rgba,
                           float *min_normal_z);
 TW_API int tw_tile_ao_batch(tw_ctx *ctx, const float *zvals, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size,
@@ -279,6 +283,34 @@ typedef struct tw_tile_outputs {
 TW_API int tw_create_tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
                            uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
                            float wpz_max, uint32_t size, const tw_tile_outputs *out);
+/* The same job with the two other per-tile products the reference makes for every new tile; tw_create_tiles_launch(...) is
+ * tw_create_tiles_launch_ex(..., NULL), and tw_create_tiles_poll completes both. shading (optional) adds:
+ *   ao             optional, ntiles*(zvsize-1)^2 bytes, host or device: tile_t::calc_mesh_ao_lighting with the ray z step half_dxy, as tw_tile_ao_batch
+ *   weights        optional, ntiles*(zvsize-1)^2*4 bytes, host or device: the terrain weights texture of tile_t::create_texture, as tw_tile_weights_batch
+ *                  (needs wp, tile_params and tw_set_sine_params; wp is validated and copied during the launch)
+ *   has_any_grass  optional, needs weights, ntiles bytes: HOST (filled by the completing poll) or device
+ *   tile_params    with weights: ntiles*8 floats as for tw_tile_weights_batch; HOST (copied during the launch) or device (read until the completing poll)
+ * Each chunk's AO map and weights texture are computed on the stream that eroded it, after its erosion, like the bounds and the normal map.
+ * AO follows the reference's two flows, exactly as tw_create_zvals_ao_batch:
+ *   CPU gen modes (0-2): the zvals are generated directly; the (stride + 72)^2 context is generated outside the tile only, and the rays read the
+ *     eroded zvals inside the tile. Every output equals the synchronous calls'.
+ *   GPU gen modes (3/4): the context is generated once and the zvals are cut from its interior BEFORE erosion; the un-eroded context is the ray
+ *     source everywhere, only the ray origin is the eroded zval. So in these modes requesting AO CHANGES THE ZVALS: they equal
+ *     tw_create_zvals_ao_batch's, not tw_create_zvals_batch's (the reference does the same). The z range, bounds, normal map and weights are then
+ *     derived from those zvals, and tw_last_erosion_steps() after the completing poll equals its value after tw_create_zvals_ao_batch.
+ * Errors: TW_ERR_ARG for weights without wp or tile_params, has_any_grass without weights, a tex_class that does not name each class once, or
+ * zmax <= zmin; TW_ERR_STATE for weights before tw_set_sine_params. The layout of tw_tile_outputs is unchanged (ABI 1). */
+typedef struct tw_tile_shading {
+	float                   half_dxy;      /* HALF_DXY: the AO ray's z step, as tw_tile_ao_batch */
+	const struct tw_weight_params *wp;     /* required with weights (declared below) */
+	const float            *tile_params;   /* required with weights: ntiles*8 biome corners */
+	uint8_t                *ao;            /* optional: ntiles*(zvsize-1)^2 bytes */
+	uint8_t                *weights;       /* optional: ntiles*(zvsize-1)^2*4 bytes */
+	uint8_t                *has_any_grass; /* optional, needs weights: ntiles bytes */
+} tw_tile_shading;
+TW_API int tw_create_tiles_launch_ex(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                           uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                           float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading);
 TW_API int tw_create_tiles_poll(tw_ctx *ctx, int wait);
 /* droplet steps executed by the last tw_erode/tw_erode_tiles call (sum over droplets; for roofline byte accounting) */
 TW_API uint64_t tw_last_erosion_steps(const tw_ctx *ctx);

@@ -1,8 +1,9 @@
 """A frame's worth of new tiles the way an engine creates them (tile_draw_t::update): the asynchronous path (tw_create_tiles_launch, then
 tw_create_tiles_poll(wait=0) until ready) against the three synchronous calls it replaces (tw_create_zvals_batch, tw_tile_bounds_batch,
 tw_tile_normals_batch), alternated in one process. Default: 16 tiles of 130^2, BASELINE terrain (mode 4, 8 octaves), 1000 droplets per tile, z range +
-sub-block bounds + normal map into pinned host memory; medians over --reps rounds after 3 warm-up rounds. Prints one JSON line with the GPU's name and
-power limit; writes nothing."""
+sub-block bounds + normal map into pinned host memory; medians over --reps rounds after 3 warm-up rounds. --ao adds the AO map (the synchronous side
+then calls tw_create_zvals_ao_batch instead of tw_create_zvals_batch), --weights the terrain weights texture and has_any_grass (tw_tile_weights_batch):
+the asynchronous job is then tw_create_tiles_launch_ex. Prints one JSON line with the GPU's name and power limit; writes nothing."""
 import argparse
 import importlib
 import json
@@ -24,6 +25,8 @@ ap.add_argument("--tiles", type=int, default=16)
 ap.add_argument("--zvsize", type=int, default=130)
 ap.add_argument("--droplets", type=int, default=1000)
 ap.add_argument("--reps", type=int, default=20)
+ap.add_argument("--ao", action="store_true")
+ap.add_argument("--weights", action="store_true")
 a = ap.parse_args()
 
 nt, zv, iters, size = a.tiles, a.zvsize, a.droplets, a.zvsize - 2
@@ -35,19 +38,40 @@ dx, dy, wpz_max = float(cfg.dx_val), float(cfg.dy_val), float(cfg.erosion_params
 z = torch.empty((nt, zv, zv), dtype=torch.float32).pin_memory()
 nrm = torch.empty((nt, zv - 1, zv - 1, 4), dtype=torch.uint8).pin_memory()
 mm, mnz, bounds = np.empty((nt, 2), np.float32), np.empty(nt, np.float32), (tw.TileBounds * nt)()
+hd = 0.5 * (dx + dy)
+ao = torch.empty((nt, zv - 1, zv - 1), dtype=torch.uint8).pin_memory() if a.ao else None
+wts = torch.empty((nt, zv - 1, zv - 1, 4), dtype=torch.uint8).pin_memory() if a.weights else None
+grass = np.empty(nt, np.uint8) if a.weights else None
+wp, corners = None, None
+if a.weights:
+    ctx.set_sine_params(cfg.sine_params())
+    wp = tw.WeightParams()
+    for i, h in enumerate((0.40, 0.44, 0.60, 0.75, 1.0)):
+        wp.h_dirt[i], wp.tex_class[i] = h, i
+    wp.sthresh[0][0], wp.sthresh[0][1], wp.sthresh[1][0], wp.sthresh[1][1] = 0.68, 0.86, 0.48, 0.72
+    wp.zmin, wp.zmax, wp.water_level = -2.3, 2.3, float(ep.water_plane_z)
+    wp.noise_scale, wp.vnz_scale, wp.vegetation = 0.003, float(np.float32(np.sqrt(2.0))), 1.0
+    wp.dx_val, wp.dy_val, wp.dxdy, wp.xy_mult = dx, dy, dx * dy, 1.0 / size
+    corners = np.random.default_rng(1).uniform(-0.2, 1.3, (nt, 8)).astype(np.float32)
+shading = dict(ao=ao, weights=wts, has_any_grass=grass, half_dxy=hd, wp=wp, tile_params=corners) if (a.ao or a.weights) else {}
 launch_ms, ready_ms, sync_ms = [], [], []
 for r in range(a.reps + 3):
     origins = [((r * 5 + t % 4) * size, (t // 4 + r) * size) for t in range(nt)]   # new tiles every frame
     t0 = time.perf_counter()
     ctx.create_tiles_launch(origins, cfg.mesh_size, dx, dy, zv, hp, iters, ep, ep.zmin, z, mm=mm, bounds=bounds, normals=nrm, min_normal_z=mnz,
-                            wpz_max=wpz_max, size=size)
+                            wpz_max=wpz_max, size=size, **shading)
     t1 = time.perf_counter()
     while not ctx.create_tiles_poll(wait=False):
         pass
     t2 = time.perf_counter()
-    ctx.create_zvals_batch(origins, cfg.mesh_size, dx, dy, zv, hp, iters, ep, ep.zmin, out=z, want_minmax=True)
+    if a.ao:
+        ctx.create_zvals_ao_batch(origins, cfg.mesh_size, dx, dy, zv, hp, iters, ep, ep.zmin, hd, out=z, ao=ao, want_minmax=True)
+    else:
+        ctx.create_zvals_batch(origins, cfg.mesh_size, dx, dy, zv, hp, iters, ep, ep.zmin, out=z, want_minmax=True)
     ctx.tile_bounds(z, wpz_max, dx, dy, size)
     ctx.tile_normals(z, dx, dy, out=nrm)
+    if a.weights:
+        ctx.tile_weights(z, origins, cfg.mesh_size, dx, dy, hp, wp, corners, out=wts)
     t3 = time.perf_counter()
     if r >= 3:
         launch_ms.append(1e3 * (t1 - t0))
@@ -58,6 +82,7 @@ try:
                                                     capture_output=True, text=True, timeout=30).stdout.split(",")[:2]]
 except Exception:   # noqa: BLE001 - descriptive only
     name, plim = None, None
-print(json.dumps({"workload": "%d tiles of %d^2, mode 4 8-octave + %d droplets per tile, z range + bounds + normal map, pinned host outputs" % (nt, zv, iters),
+extra = "".join(s for s, on in ((" + AO map", a.ao), (" + weights texture", a.weights)) if on)
+print(json.dumps({"workload": "%d tiles of %d^2, mode 4 8-octave + %d droplets per tile, z range + bounds + normal map%s, pinned host outputs" % (nt, zv, iters, extra),
                   "launch_host_ms": float(np.median(launch_ms)), "launch_host_ms_max": max(launch_ms), "launch_to_ready_ms": float(np.median(ready_ms)),
-                  "sync_three_calls_ms": float(np.median(sync_ms)), "rounds": a.reps, "gpu": name, "power_limit_w": plim}))
+                  ("sync_calls_ms" if extra else "sync_three_calls_ms"): float(np.median(sync_ms)), "rounds": a.reps, "gpu": name, "power_limit_w": plim}))

@@ -92,6 +92,16 @@ class TileShading(C.Structure):
     _fields_ = [("half_dxy", C.c_float), ("wp", C.c_void_p), ("tile_params", C.c_void_p), ("ao", C.c_void_p), ("weights", C.c_void_p), ("has_any_grass", C.c_void_p)]
 
 
+class TileLight(C.Structure):
+    """tw_tile_light (include/tw3d.h): one light's mesh shadows in the tile job (smask required; sh_in_* / sh_out_* optional)."""
+    _fields_ = [("sp", ShadowParams), ("sh_in_x", C.c_void_p), ("sh_in_y", C.c_void_p), ("smask", C.c_void_p), ("sh_out_x", C.c_void_p), ("sh_out_y", C.c_void_p)]
+
+
+class TileShadows(C.Structure):
+    """tw_tile_shadows (include/tw3d.h): the tiles' grid coordinates and the lights whose mesh shadows tw_create_tiles_launch_shadows adds to the job."""
+    _fields_ = [("tile_xy", C.c_void_p), ("nlights", C.c_uint32), ("lights", C.c_void_p)]
+
+
 class PointQuery(C.Structure):
     _fields_ = [("kind", C.c_int), ("xy_scale", C.c_float), ("mesh_x_size", C.c_int), ("mesh_y_size", C.c_int), ("x_scene_size", C.c_float),
                 ("y_scene_size", C.c_float), ("xoff2", C.c_int), ("yoff2", C.c_int), ("no_xyoff", C.c_int)]
@@ -127,7 +137,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_destroy", "tw_last_error", "tw
                "tw_heightmap_from_floats_u16", "tw_heightmap_to_floats_u16", "tw_proc_gen_heightmap", "tw_heightmap_sample_tiles", "tw_minmax_f32",
                "tw_multi_create", "tw_multi_destroy", "tw_multi_size", "tw_multi_ctx", "tw_multi_last_error", "tw_multi_set_sine_params", "tw_multi_range",
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
-               "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_weights_batch", "tw_gen_tex_height_tables"]
+               "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables"]
 
 
 def _load():
@@ -170,6 +180,7 @@ def _load():
     L.tw_create_tiles_launch.argtypes = [vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint32, C.POINTER(HeightParams), C.c_uint32,
                                          C.POINTER(ErosionParams), C.c_float, C.c_float, C.c_uint32, C.POINTER(TileOutputs)]
     L.tw_create_tiles_launch_ex.argtypes = L.tw_create_tiles_launch.argtypes + [C.POINTER(TileShading)]
+    L.tw_create_tiles_launch_shadows.argtypes = L.tw_create_tiles_launch_ex.argtypes + [C.POINTER(TileShadows)]
     L.tw_create_tiles_poll.argtypes = [vp, C.c_int]
     L.tw_tile_bounds_batch.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_uint32, vp]
     L.tw_glaciate_mesh.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(HeightParams), C.POINTER(MinMax)]
@@ -215,6 +226,7 @@ def _load():
     L.tw_voxel_remove_unconnected.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), C.POINTER(C.c_uint64)]
     L.tw_voxel_triangles.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, vp, C.c_uint64, C.POINTER(C.c_uint64)]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
+    L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_weights_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint32, C.POINTER(HeightParams), C.POINTER(WeightParams), vp, vp, vp]
     L.tw_gen_tex_height_tables.argtypes = [C.c_float, C.c_float, C.c_float, vp, vp, vp]
     L.tw_gen_tex_height_tables.restype = None
@@ -241,6 +253,19 @@ def _ptr(a):
         assert a.is_contiguous()
         return C.c_void_p(a.data_ptr())
     raise TypeError(type(a))
+
+
+def _edge(a):
+    """An optional incoming shadow edge: a CUDA tensor as it is, anything else as a contiguous float32 numpy array."""
+    return a if a is None or hasattr(a, "data_ptr") else np.ascontiguousarray(a, np.float32)
+
+
+class Light:
+    """One light of Context.create_tiles_launch(lights=...): its ShadowParams, the required smask [nt, zv, zv] uint8 and the optional sh_out_x, sh_out_y,
+    sh_in_x, sh_in_y ([nt, zv] float32), numpy arrays (pinned for a launch that does not block) or CUDA tensors."""
+
+    def __init__(self, sp, smask, sh_out_x=None, sh_out_y=None, sh_in_x=None, sh_in_y=None):
+        self.sp, self.smask, self.sh_out_x, self.sh_out_y, self.sh_in_x, self.sh_in_y = sp, smask, sh_out_x, sh_out_y, sh_in_x, sh_in_y
 
 
 # ---- host-side helpers (no GPU needed) ----
@@ -458,15 +483,18 @@ class Context:
         return (out, mm) if want_minmax else out
 
     def create_tiles_launch(self, origins_xy, mesh_size, dx, dy, zvsize, hp, erosion_iters, ep, min_zval, zvals, mm=None, bounds=None, normals=None,
-                            min_normal_z=None, wpz_max=0.0, size=0, ao=None, weights=None, has_any_grass=None, half_dxy=None, wp=None, tile_params=None):
+                            min_normal_z=None, wpz_max=0.0, size=0, ao=None, weights=None, has_any_grass=None, half_dxy=None, wp=None, tile_params=None,
+                            tile_xy=None, lights=None):
         """tw_create_tiles_launch(_ex): a frame's new tiles (heights, erosion, z range, sub-block bounds, normal map, and on request the AO map and the
         terrain weights texture) enqueued without waiting for the GPU.
         zvals [nt, zv, zv] float32, normals [nt, zv-1, zv-1, 4] uint8, ao [nt, zv-1, zv-1] uint8 and weights [nt, zv-1, zv-1, 4] uint8: numpy arrays
         (pinned for a launch that does not block) or CUDA tensors; mm [nt, 2] float32, bounds (TileBounds * nt) and min_normal_z [nt] float32 are host
         arrays that the completing create_tiles_poll fills, has_any_grass [nt] uint8 is either. weights needs wp (WeightParams) and tile_params
         ([nt, 8] float32, host or CUDA); ao takes the ray step half_dxy. In GPU gen modes (3/4) requesting ao makes the zvals those of
-        create_zvals_ao_batch (see tw3d.h). The origins and host tile_params are copied during the launch; the outputs and device inputs are kept
-        referenced here until the job completes."""
+        create_zvals_ao_batch (see tw3d.h). lights adds the mesh shadows of these tiles (tw_create_tiles_launch_shadows): a list of Light records or
+        (ShadowParams, smask, sh_out_x, sh_out_y, sh_in_x, sh_in_y) tuples - smask [nt, zv, zv] uint8 required, the rest [nt, zv] float32 or None - and
+        needs tile_xy [nt, 2] (x1/size, y1/size). The origins, tile_xy, host tile_params and host sh_in rows are copied during the launch; the outputs and
+        device inputs are kept referenced here until the job completes."""
         org = np.ascontiguousarray(origins_xy, np.int32).reshape(-1, 2)
         nt = org.shape[0]
         outs = TileOutputs(_ptr(zvals), _ptr(mm), C.cast(bounds, C.c_void_p) if bounds is not None else None, _ptr(normals), _ptr(min_normal_z))
@@ -480,10 +508,25 @@ class Context:
                 tile_params = np.ascontiguousarray(tile_params, np.float32)
             shading = TileShading(0.0 if half_dxy is None else half_dxy, C.cast(C.pointer(wp), C.c_void_p) if wp is not None else None, _ptr(tile_params),
                                   _ptr(ao), _ptr(weights), _ptr(has_any_grass))
+        shadows, keep = None, []
+        if lights is not None:
+            if tile_xy is None:
+                raise ValueError("create_tiles_launch: lights need tile_xy (the tiles' grid coordinates)")
+            tile_xy = np.ascontiguousarray(tile_xy, np.int32).reshape(-1, 2)
+            recs = [lt if isinstance(lt, Light) else Light(*lt) for lt in lights]
+            keep = [[r.smask, r.sh_out_x, r.sh_out_y, _edge(r.sh_in_x), _edge(r.sh_in_y)] for r in recs]
+            arr = (TileLight * max(1, len(recs)))()
+            for i, (r, k) in enumerate(zip(recs, keep)):
+                arr[i] = TileLight(r.sp, _ptr(k[3]), _ptr(k[4]), _ptr(k[0]), _ptr(k[1]), _ptr(k[2]))
+            shadows = TileShadows(_ptr(tile_xy), len(recs), C.cast(arr, C.c_void_p))
+            keep.append(arr)
+        if shadows is not None:
+            self._check(lib.tw_create_tiles_launch_shadows(*args, C.byref(shading) if shading is not None else None, C.byref(shadows)))
+        elif shading is not None:
             self._check(lib.tw_create_tiles_launch_ex(*args, C.byref(shading)))
         else:
             self._check(lib.tw_create_tiles_launch(*args))
-        self._tiles_job = (zvals, mm, bounds, normals, min_normal_z, ao, weights, has_any_grass, wp, tile_params, shading)
+        self._tiles_job = (zvals, mm, bounds, normals, min_normal_z, ao, weights, has_any_grass, wp, tile_params, shading, tile_xy, keep, shadows)
 
     def create_tiles_poll(self, wait=False):
         """True once the job of create_tiles_launch (or any pending job of this context) is complete, False while it runs (wait=False)."""
@@ -599,14 +642,19 @@ class Context:
         self._check(lib.tw_voxel_fill(self._h, C.byref(vp), _ptr(rd), _ptr(out)))
         return out
 
-    def tile_shadows(self, tiles, tile_xy, sp, out=None):
-        """calc_mesh_shadows for a batch of tiles with neighbour chaining: returns (smask [nt, zv, zv] uint8, sh_out_x [nt, zv], sh_out_y [nt, zv])."""
+    def tile_shadows(self, tiles, tile_xy, sp, out=None, sh_in_x=None, sh_in_y=None):
+        """calc_mesh_shadows for a batch of tiles with neighbour chaining: returns (smask [nt, zv, zv] uint8, sh_out_x [nt, zv], sh_out_y [nt, zv]).
+        sh_in_x / sh_in_y ([nt, zv] float32, numpy or CUDA): incoming heights from neighbours outside the batch (tw_tile_shadows_batch_ex)."""
         nt, zv = int(tiles.shape[0]), int(tiles.shape[1])
         txy = np.ascontiguousarray(tile_xy, np.int32).reshape(-1, 2)
         if out is None:
             out = np.empty((nt, zv, zv), np.uint8)
         ox, oy = np.empty((nt, zv), np.float32), np.empty((nt, zv), np.float32)
-        self._check(lib.tw_tile_shadows_batch(self._h, _ptr(tiles), _ptr(txy), nt, zv, C.byref(sp), _ptr(out), _ptr(ox), _ptr(oy)))
+        if sh_in_x is None and sh_in_y is None:
+            self._check(lib.tw_tile_shadows_batch(self._h, _ptr(tiles), _ptr(txy), nt, zv, C.byref(sp), _ptr(out), _ptr(ox), _ptr(oy)))
+        else:
+            ix, iy = _edge(sh_in_x), _edge(sh_in_y)
+            self._check(lib.tw_tile_shadows_batch_ex(self._h, _ptr(tiles), _ptr(txy), nt, zv, C.byref(sp), _ptr(ix), _ptr(iy), _ptr(out), _ptr(ox), _ptr(oy)))
         return out, ox, oy
 
     def tile_weights(self, tiles, origins_xy, mesh_size, dx, dy, hp, wp, tile_params, out=None, want_grass_flags=True):

@@ -445,11 +445,12 @@ int tw_erode_tiles(tw_ctx *ctx, float *maps, uint32_t ntiles, int xsize, int ysi
 	return TW_OK;
 }
 
-// The tile pipeline behind tw_create_zvals_batch, tw_create_zvals_ao_batch and tw_create_tiles_launch(_ex): enqueues everything and returns without
-// waiting for the device; the job completes through poll_job (check_ctx and finish_pending have run). sh (optional): AO map and weights texture.
+// The tile pipeline behind tw_create_zvals_batch, tw_create_zvals_ao_batch and tw_create_tiles_launch(_ex, _shadows): enqueues everything and returns
+// without waiting for the device; the job completes through poll_job (check_ctx and finish_pending have run). sh (optional): AO map and weights texture;
+// shs (optional): per-light mesh shadows.
 static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy, uint32_t zvsize,
                         const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
-                        const tw_tile_outputs *o, const tw_tile_shading *sh)
+                        const tw_tile_outputs *o, const tw_tile_shading *sh, const tw_tile_shadows *shs)
 {
 	if (!origins_xy || ntiles == 0 || !p || !o || !o->zvals) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	bool const want_mm = (o->mm != nullptr), want_bounds = (o->bounds != nullptr), want_normals = (o->normals_rgba != nullptr), want_mnz = (o->min_normal_z != nullptr);
@@ -463,6 +464,25 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		if (!sh->wp || !sh->tile_params) return tw_set_error(ctx, TW_ERR_ARG, "the weights texture needs wp and tile_params");
 		if (zvsize < 3) return tw_set_error(ctx, TW_ERR_ARG, "the weights texture needs zvsize >= 3");
 		int const rc = validate_weights(ctx, sh->wp, W); if (rc) return rc;
+	}
+	// mesh shadows: the lights and their plans (neighbours, waves, light direction) are taken from the caller's arrays here, during the launch
+	uint32_t const nl = shs ? shs->nlights : 0;
+	std::vector<tw_tile_light> lights;
+	std::vector<twi_shadow_plan> splan;
+	std::vector<char> sdev_m, sdev_ix, sdev_iy; // smask / sh_in_x / sh_in_y are device memory
+	if (shs) {
+		if (!shs->tile_xy || shs->nlights == 0 || !shs->lights) return tw_set_error(ctx, TW_ERR_ARG, "mesh shadows need tile_xy and at least one light");
+		if (zvsize < 2) return tw_set_error(ctx, TW_ERR_ARG, "mesh shadows need zvsize >= 2");
+		lights.assign(shs->lights, shs->lights + nl);
+		splan.resize(nl); sdev_m.resize(nl); sdev_ix.resize(nl); sdev_iy.resize(nl);
+		for (uint32_t l = 0; l < nl; ++l) {
+			tw_tile_light const &L = lights[l];
+			if (!L.smask) return tw_set_error(ctx, TW_ERR_ARG, "light %u: smask is required", l);
+			sdev_m[l] = tw_is_device_ptr(L.smask);
+			if (sdev_m[l] && ((size_t)L.smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "light %u: a device smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)", l);
+			sdev_ix[l] = L.sh_in_x && tw_is_device_ptr(L.sh_in_x); sdev_iy[l] = L.sh_in_y && tw_is_device_ptr(L.sh_in_y);
+			if (!twi_shadow_plan_make(shs->tile_xy, ntiles, &L.sp, L.sh_in_x != nullptr, L.sh_in_y != nullptr, &splan[l])) return tw_set_error(ctx, TW_ERR_ARG, "tile_xy names a tile twice");
+		}
 	}
 	tw_grid2d g; g.x0 = 0; g.y0 = 0; g.dx = dx; g.dy = dy; g.nx = zvsize; g.ny = zvsize;
 	int rc = validate_height(ctx, &g, p, o->zvals); if (rc) return rc;
@@ -504,7 +524,14 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	size_t const z_bytes = dev_out ? 0 : al(n*sizeof(float)), nrm_bytes = (want_normals && !dev_nrm) ? al(ntiles*nrm_elems*4) : 0;
 	size_t const ao_bytes = (want_ao && !dev_ao) ? al(ntiles*nrm_elems) : 0, w_bytes = (want_w && !dev_w) ? al(ntiles*nrm_elems*4) : 0, f_bytes = (want_f && !dev_f) ? al(ntiles) : 0;
 	size_t const tp_bytes = (want_w && !dev_tp) ? al((size_t)ntiles*8*sizeof(float)) : 0;
-	size_t const fixed_bytes = z_bytes + nrm_bytes + ao_bytes + w_bytes + f_bytes + tp_bytes + ctab_bytes + jtab_bytes;
+	// mesh shadows, reused light after light: [mask staging (host smask) | 64-bit keys | x edges | y edges (outputs, then caller rows) | plan of every light]
+	size_t const edge = (size_t)ntiles*zvsize, plan_bytes = al(twi_shadow_plan_ints(ntiles)*sizeof(int));
+	bool sh_host_m = false, sh_in_x = false, sh_in_y = false;
+	for (uint32_t l = 0; l < nl; ++l) {sh_host_m |= !sdev_m[l]; sh_in_x |= (lights[l].sh_in_x != nullptr); sh_in_y |= (lights[l].sh_in_y != nullptr);}
+	size_t const shm_bytes = sh_host_m ? al(n + 4) : 0, shk_bytes = nl ? al(2*edge*sizeof(unsigned long long)) : 0;
+	size_t const shx_bytes = nl ? al((sh_in_x ? 2 : 1)*edge*sizeof(float)) : 0, shy_bytes = nl ? al((sh_in_y ? 2 : 1)*edge*sizeof(float)) : 0;
+	size_t const sh_bytes = shm_bytes + shk_bytes + shx_bytes + shy_bytes + nl*plan_bytes;
+	size_t const fixed_bytes = z_bytes + nrm_bytes + ao_bytes + w_bytes + f_bytes + tp_bytes + ctab_bytes + jtab_bytes + sh_bytes;
 	if (fixed_bytes) {rc = tw_reserve(ctx, 0, fixed_bytes); if (rc) return rc;}
 	// AO context grids and weights jitter grids are per chunk (schedule order): written on the main stream, read on the chunk's erosion stream. The buffers
 	// hold about 2 GB of context grids (or jitter grids without AO) in all, the bound tw_tile_ao_batch keeps; a chunk holds at most a third of that. When
@@ -553,6 +580,11 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	const float *d_tp = !want_w ? nullptr : (dev_tp ? sh->tile_params : (const float *)s0); s0 += tp_bytes;
 	char *d_ctab = s0; s0 += ctab_bytes;
 	char *d_jtab = s0; s0 += jtab_bytes;
+	unsigned char *d_shm = (unsigned char *)s0; s0 += shm_bytes;
+	unsigned long long *d_shk = (unsigned long long *)s0; s0 += shk_bytes;
+	float *d_shx = (float *)s0; s0 += shx_bytes;
+	float *d_shy = (float *)s0; s0 += shy_bytes;
+	char *d_shp = s0; s0 += nl*plan_bytes;
 	char *d_ring = s0;
 	if (erode) {
 		sbytes = al(twi_erode_scratch_bytes(ctx, chunk, (int)zvsize, (int)zvsize));
@@ -579,13 +611,19 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	float2 *d_corg = (float2 *)s2; s2 += corg_bytes;
 	float2 *d_corg_sorted = (float2 *)s2;
 	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
-	// pinned staging: inputs [origins | sine-mode index tables | context origins or their sine tables | jitter sine tables | tile_params], then the small results
-	// [steps | min/max | sub-block bounds | min_normal_z | has_any_grass] that the completing poll unpacks. Every sine batch has its own region, and the caller's
-	// origins and tile_params may be reused as soon as this function returns.
+	// pinned staging: inputs [origins | sine-mode index tables | context origins or their sine tables | jitter sine tables | tile_params | per light: shadow plan,
+	// host sh_in_x, host sh_in_y], then the small results [steps | min/max | sub-block bounds | min_normal_z | has_any_grass] that the completing poll unpacks.
+	// Every sine batch has its own region, and the caller's origins, tile_params, tile_xy and host sh_in rows may be reused as soon as this function returns.
 	size_t const in_org = al((size_t)ntiles*sizeof(float2)), in_sine = sine ? al(twi_sine_tiles_stage_bytes(ntiles)) : 0;
 	size_t const in_ctx = !want_ao ? 0 : (sine ? al(twi_sine_tiles_stage_bytes(ntiles)) : in_org), in_jit = want_w ? al(twi_sine_tiles_stage_bytes(ntiles)) : 0;
-	size_t const in_tp = tp_bytes, off_ctx = in_org + in_sine, off_jit = off_ctx + in_ctx, off_tp = off_jit + in_jit;
-	size_t const off_steps = off_tp + in_tp, off_mm = off_steps + 256, off_sub = off_mm + (want_mm ? mm_bytes : 0), off_mnz = off_sub + sub_bytes, off_f = off_mnz + mnz_bytes;
+	size_t const in_tp = tp_bytes, off_ctx = in_org + in_sine, off_jit = off_ctx + in_ctx, off_tp = off_jit + in_jit, off_sh = off_tp + in_tp;
+	std::vector<size_t> off_six(nl), off_siy(nl);
+	size_t in_sh = nl*plan_bytes;
+	for (uint32_t l = 0; l < nl; ++l) {
+		off_six[l] = off_sh + in_sh; in_sh += (lights[l].sh_in_x && !sdev_ix[l]) ? al(edge*sizeof(float)) : 0;
+		off_siy[l] = off_sh + in_sh; in_sh += (lights[l].sh_in_y && !sdev_iy[l]) ? al(edge*sizeof(float)) : 0;
+	}
+	size_t const off_steps = off_sh + in_sh, off_mm = off_steps + 256, off_sub = off_mm + (want_mm ? mm_bytes : 0), off_mnz = off_sub + sub_bytes, off_f = off_mnz + mnz_bytes;
 	rc = tw_reserve_pinned(ctx, off_f + (want_f ? al(ntiles) : 0)); if (rc) return rc;
 	char *h_stage = (char *)ctx->h_pinned;
 	float2 *h_org = (float2 *)h_stage;
@@ -601,6 +639,12 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	if (tp_bytes) {
 		memcpy(h_stage + off_tp, sh->tile_params, (size_t)ntiles*8*sizeof(float));
 		TW_CUDA(ctx, cudaMemcpyAsync((void *)d_tp, h_stage + off_tp, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+	}
+	for (uint32_t l = 0; l < nl; ++l) { // the plans go up now; host sh_in rows wait in the staging until their light's pass copies them into the edge buffers
+		twi_shadow_plan_pack(splan[l], (int *)(h_stage + off_sh + l*plan_bytes));
+		TW_CUDA(ctx, cudaMemcpyAsync(d_shp + l*plan_bytes, h_stage + off_sh + l*plan_bytes, twi_shadow_plan_ints(ntiles)*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+		if (lights[l].sh_in_x && !sdev_ix[l]) {memcpy(h_stage + off_six[l], lights[l].sh_in_x, edge*sizeof(float));}
+		if (lights[l].sh_in_y && !sdev_iy[l]) {memcpy(h_stage + off_siy[l], lights[l].sh_in_y, edge*sizeof(float));}
 	}
 	if (want_f) {TW_CUDA(ctx, cudaMemsetAsync(d_f, 0, ntiles, ctx->stream));}
 	if (erode) {TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, sizeof(unsigned long long), ctx->stream));} // the aux streams see it through the chunk events
@@ -696,6 +740,17 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		for (int l = 0; l < 3; ++l) {cudaStreamSynchronize(ctx->aux_stream[l]);}
 		return status;
 	}
+	// mesh shadows on ctx->stream, light after light through the same buffers: every tile's neighbours have their final heights once the chunks are joined
+	for (uint32_t l = 0; l < nl; ++l) {
+		tw_tile_light const &L = lights[l];
+		unsigned char *d_m = sdev_m[l] ? L.smask : d_shm;
+		if (L.sh_in_x) {TW_CUDA(ctx, cudaMemcpyAsync(d_shx + edge, sdev_ix[l] ? (const void *)L.sh_in_x : h_stage + off_six[l], edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+		if (L.sh_in_y) {TW_CUDA(ctx, cudaMemcpyAsync(d_shy + edge, sdev_iy[l] ? (const void *)L.sh_in_y : h_stage + off_siy[l], edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+		rc = twi_shadow_enqueue(ctx, ctx->stream, splan[l], d_out, ntiles, zvsize, d_m, d_shk, d_shx, d_shy, (const int *)(d_shp + l*plan_bytes), true); if (rc) return rc;
+		if (!sdev_m[l]) {TW_CUDA(ctx, cudaMemcpyAsync(L.smask, d_m, n, cudaMemcpyDeviceToHost, ctx->stream));}
+		if (L.sh_out_x) {TW_CUDA(ctx, cudaMemcpyAsync(L.sh_out_x, d_shx, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+		if (L.sh_out_y) {TW_CUDA(ctx, cudaMemcpyAsync(L.sh_out_y, d_shy, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+	}
 	// every host-bound result is copied once, at the end: the schedule order scatters a chunk over the whole batch
 	if (!dev_out && d_perm) {TW_CUDA(ctx, cudaMemcpyAsync(o->zvals, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 	if (want_normals && !dev_nrm) {TW_CUDA(ctx, cudaMemcpyAsync(o->normals_rgba, d_rgba, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
@@ -715,14 +770,21 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	return TW_OK;
 }
 
-int tw_create_tiles_launch_ex(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
-                              uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
-                              float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading)
+int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                                   uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                                   float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows)
 {
 	int rc = check_ctx(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
 	ctx->last_erosion_steps = 0;
-	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading);
+	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, shadows);
+}
+
+int tw_create_tiles_launch_ex(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                              uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                              float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading)
+{
+	return tw_create_tiles_launch_shadows(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, nullptr);
 }
 
 int tw_create_tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,

@@ -136,6 +136,29 @@ int twi_tile_ao(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, const float 
 int twi_tile_cut(tw_ctx *ctx, cudaStream_t st, const float *d_czv, uint32_t ntiles, uint32_t zvsize, float *d_zvals, const unsigned *d_perm = nullptr);
 int twi_tile_weights(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, const float *d_rand, uint32_t ntiles, uint32_t zvsize, const float *d_tile_params, const tw_weight_params *W,
                      uint8_t *d_out, uint8_t *d_flags, const unsigned *d_perm = nullptr); // d_rand: jitter grids in launch order
+// Mesh shadows of a batch of tiles (tw_shadows.cu) in two steps, so the tile job can run them after its chunks. twi_shadow_plan_make (host only) finds each
+// tile's neighbours toward the light, the dependency waves and the light direction; a tile whose neighbour is not in the batch reads the caller's row
+// ntiles + t of the edge buffers instead when has_in_x / has_in_y say one exists. It returns false when tile_xy holds a tile twice (the plan is then the one
+// tw_tile_shadows_batch has always made: the later entry owns the position). twi_shadow_enqueue runs one light on `st` into buffers reserved by the caller:
+//   d_m     ntiles*n^2 bytes, 4-byte aligned        d_keys  2*ntiles*n 64-bit keys
+//   d_ox    ntiles*n floats (outputs), then ntiles*n caller rows when has_in_x (resp. d_oy, has_in_y)
+//   d_plan  twi_shadow_plan_ints(ntiles) ints of device memory holding twi_shadow_plan_pack's output
+// use_graph: more than 32 waves go to the stream as one CUDA graph (for a caller that must not block behind a full launch queue)
+struct twi_shadow_dev {
+	float xs, ys, dx, dy, dxi, dyi, zmin, zmax; // X/Y_SCENE_SIZE, DX/DY_VAL, their inverses, clip z range
+	float dirx, diry, dirz, dist;
+	int dim; double dir_ratio;
+};
+struct twi_shadow_plan {
+	std::vector<int> nbx, nby, wave_tiles, wave_start; // wave l = wave_tiles[wave_start[l] .. wave_start[l + 1])
+	twi_shadow_dev S;
+	bool trace = false, all_shadowed = false;
+};
+bool   twi_shadow_plan_make(const int32_t *tile_xy, uint32_t ntiles, const tw_shadow_params *sp, bool has_in_x, bool has_in_y, twi_shadow_plan *P);
+size_t twi_shadow_plan_ints(uint32_t ntiles);
+void   twi_shadow_plan_pack(const twi_shadow_plan &P, int *out); // [wave_tiles | nbx | nby]
+int    twi_shadow_enqueue(tw_ctx *ctx, cudaStream_t st, const twi_shadow_plan &P, const float *d_z, uint32_t ntiles, uint32_t n, unsigned char *d_m,
+                          unsigned long long *d_keys, float *d_ox, float *d_oy, const int *d_plan, bool use_graph);
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
 int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads);
 size_t   twi_erode_scratch_bytes(const tw_ctx *ctx, uint32_t chunk, int xsize, int ysize);

@@ -15,11 +15,7 @@
 
 namespace {
 
-struct ShadowDev {
-	float xs, ys, dx, dy, dxi, dyi, zmin, zmax; // X/Y_SCENE_SIZE, DX/DY_VAL, their inverses, clip z range
-	float dirx, diry, dirz, dist;
-	int dim; double dir_ratio;
-};
+typedef twi_shadow_dev ShadowDev; // tw_internal.h: the plan carries it
 struct Pt {float x, y, z;};
 
 __device__ __forceinline__ int region_of(Pt v, const float (&d)[3][2]) { // get_region, src/inlines.h:522-528
@@ -116,21 +112,17 @@ __global__ void shadow_unpack_kernel(const unsigned long long *__restrict__ kx, 
 
 } // namespace
 
-extern "C" int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp,
-                                     uint8_t *smask, float *sh_out_x, float *sh_out_y)
-{
-	if (!ctx || !zvals || !tile_xy || !sp || !smask || ntiles == 0 || zvsize < 2) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
-	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
-	int const n = (int)zvsize;
-	size_t const cells = (size_t)ntiles*n*n, edge = (size_t)ntiles*n;
-	if ((cells & 3) && ntiles > 1) {/* tiles of odd cell count straddle flag words: still correct, the atomics are per word */}
+bool twi_shadow_plan_make(const int32_t *tile_xy, uint32_t ntiles, const tw_shadow_params *sp, bool has_in_x, bool has_in_y, twi_shadow_plan *P) {
 	// neighbours toward the light, dependency waves
 	int const sx = (sp->lpos[0] < 0.0f) ? -1 : 1, sy = (sp->lpos[1] < 0.0f) ? -1 : 1;
 	std::map<std::pair<int, int>, int> where;
-	for (uint32_t t = 0; t < ntiles; ++t) {where[std::make_pair(tile_xy[2*t], tile_xy[2*t+1])] = (int)t;}
-	std::vector<int> nbx(ntiles, -1), nby(ntiles, -1), level(ntiles, -1);
+	bool unique = true;
+	for (uint32_t t = 0; t < ntiles; ++t) {
+		auto const r = where.insert(std::make_pair(std::make_pair(tile_xy[2*t], tile_xy[2*t+1]), (int)t));
+		if (!r.second) {r.first->second = (int)t; unique = false;} // a duplicate: the later entry owns the position
+	}
+	std::vector<int> &nbx = P->nbx, &nby = P->nby, level(ntiles, -1);
+	nbx.assign(ntiles, -1); nby.assign(ntiles, -1);
 	for (uint32_t t = 0; t < ntiles; ++t) {
 		auto a = where.find(std::make_pair(tile_xy[2*t] + sx, tile_xy[2*t+1])); if (a != where.end()) nbx[t] = a->second;
 		auto b = where.find(std::make_pair(tile_xy[2*t], tile_xy[2*t+1] + sy)); if (b != where.end()) nby[t] = b->second;
@@ -147,15 +139,23 @@ extern "C" int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int3
 			level[t] = l; nlevels = std::max(nlevels, l + 1);
 		}
 	}
-	std::vector<int> wave_tiles; std::vector<int> wave_start(nlevels + 1, 0);
-	for (int l = 0; l < nlevels; ++l) {for (uint32_t t = 0; t < ntiles; ++t) {if (level[t] == l) wave_tiles.push_back((int)t);} wave_start[l + 1] = (int)wave_tiles.size();}
+	for (uint32_t t = 0; t < ntiles; ++t) { // a missing neighbour: the caller's row of that edge, where there is one (row ntiles + t of the edge buffer)
+		if (nbx[t] < 0 && has_in_y) nbx[t] = (int)(ntiles + t);
+		if (nby[t] < 0 && has_in_x) nby[t] = (int)(ntiles + t);
+	}
+	P->wave_start.assign(nlevels + 1, 0); // tiles grouped by level, ascending index within a level
+	for (uint32_t t = 0; t < ntiles; ++t) {P->wave_start[level[t] + 1]++;}
+	for (int l = 0; l < nlevels; ++l) {P->wave_start[l + 1] += P->wave_start[l];}
+	P->wave_tiles.resize(ntiles);
+	std::vector<int> fill(P->wave_start.begin(), P->wave_start.end() - 1);
+	for (uint32_t t = 0; t < ntiles; ++t) {P->wave_tiles[fill[level[t]]++] = (int)t;}
 	// light direction and ray length (mesh_shadow_gen::run, :492-496), on the host with the reference's operations
-	ShadowDev S;
+	ShadowDev &S = P->S;
 	memset(&S, 0, sizeof(S));
 	S.xs = sp->x_scene_size; S.ys = sp->y_scene_size; S.dx = sp->dx_val; S.dy = sp->dy_val; S.dxi = sp->dx_val_inv; S.dyi = sp->dy_val_inv; S.zmin = sp->zmin; S.zmax = sp->zmax;
-	bool const all_shadowed = (!sp->no_shadow && sp->lpos[2] < sp->zmin);
-	bool const trace = !(sp->no_shadow || (sp->lpos[0] == 0.0f && sp->lpos[1] == 0.0f));
-	if (trace) {
+	P->all_shadowed = (!sp->no_shadow && sp->lpos[2] < sp->zmin);
+	P->trace = !(sp->no_shadow || (sp->lpos[0] == 0.0f && sp->lpos[1] == 0.0f));
+	if (P->trace) {
 		volatile float m2 = sp->lpos[0]*sp->lpos[0]; volatile float m2b = sp->lpos[1]*sp->lpos[1]; volatile float m2c = sp->lpos[2]*sp->lpos[2];
 		volatile float ms = m2 + m2b; ms = ms + m2c;
 		float const vmag = sqrtf(ms);
@@ -167,39 +167,107 @@ extern "C" int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int3
 		S.dim = (fabsf(S.dirx) < fabsf(S.diry)) ? 1 : 0;
 		S.dir_ratio = (double)(S.dirz/(S.dim ? S.diry : S.dirx));
 	}
+	return unique;
+}
+
+size_t twi_shadow_plan_ints(uint32_t ntiles) {return (size_t)3*ntiles;}
+
+void twi_shadow_plan_pack(const twi_shadow_plan &P, int *out) {
+	size_t const nt = P.nbx.size();
+	memcpy(out, P.wave_tiles.data(), nt*sizeof(int));
+	memcpy(out + nt, P.nbx.data(), nt*sizeof(int));
+	memcpy(out + 2*nt, P.nby.data(), nt*sizeof(int));
+}
+
+int twi_shadow_enqueue(tw_ctx *ctx, cudaStream_t st, const twi_shadow_plan &P, const float *d_z, uint32_t ntiles, uint32_t zvsize, unsigned char *d_m,
+                       unsigned long long *d_keys, float *d_ox, float *d_oy, const int *d_plan, bool use_graph)
+{
+	int const n = (int)zvsize;
+	size_t const cells = (size_t)ntiles*n*n, edge = (size_t)ntiles*n;
+	const int *d_wave = d_plan, *d_nbx = d_plan + ntiles, *d_nby = d_plan + 2*(size_t)ntiles;
+	unsigned long long *d_kx = d_keys, *d_ky = d_keys + edge;
+	shadow_init_kernel<<<ctx->num_sms*8, 256, 0, st>>>(d_m, d_keys, cells, 2*edge, P.all_shadowed ? (unsigned char)TW_MESH_SHADOW : (unsigned char)0);
+	TW_LAUNCH_CHECK(ctx);
+	int const nlevels = (int)P.wave_start.size() - 1, YMAX = 65535; // a wave of more tiles than gridDim.y takes runs in pieces
+	auto waves = [&](cudaStream_t s) -> int {
+		for (int l = 0; l < nlevels; ++l) {
+			int const w1 = P.wave_start[l + 1];
+			for (int w0 = P.wave_start[l]; P.trace && w0 < w1; w0 += YMAX) {
+				shadow_rays_kernel<<<dim3((4*n + 127)/128, std::min(YMAX, w1 - w0)), 128, 0, s>>>(d_z, d_m, n, P.S, d_wave + w0, d_nbx, d_nby, d_ox, d_oy, d_kx, d_ky);
+				TW_LAUNCH_CHECK(ctx);
+			}
+			for (int w0 = P.wave_start[l]; w0 < w1; w0 += YMAX) {
+				shadow_unpack_kernel<<<dim3((n + 127)/128, std::min(YMAX, w1 - w0)), 128, 0, s>>>(d_kx, d_ky, d_ox, d_oy, n, d_wave + w0);
+				TW_LAUNCH_CHECK(ctx);
+			}
+		}
+		return TW_OK;
+	};
+	if (!use_graph || nlevels <= 32) return waves(st);
+	// Many waves behind other work (a long strip of tiles along the light, in the tile job): their launches go into one CUDA graph, launched once. Thousands
+	// of kernel launches would fill the launch queue and block the host until the device had worked through the work queued before them - the whole job.
+	cudaStream_t cs = nullptr;
+	cudaGraph_t graph = nullptr;
+	cudaGraphExec_t exec = nullptr;
+	TW_CUDA(ctx, cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+	bool const began = (cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal) == cudaSuccess);
+	int const rc = began ? waves(cs) : TW_OK;
+	bool const captured = began && cudaStreamEndCapture(cs, &graph) == cudaSuccess && graph != nullptr; // ends the capture whatever happened inside it
+	bool const launched = (rc == TW_OK && captured && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess && cudaGraphLaunch(exec, st) == cudaSuccess);
+	if (exec) cudaGraphExecDestroy(exec); // a launched graph is released once it has run
+	if (graph) cudaGraphDestroy(graph);
+	cudaStreamDestroy(cs);
+	if (rc) return rc;
+	if (!launched) {cudaError_t const e = cudaGetLastError(); return tw_set_error(ctx, TW_ERR_CUDA, "mesh shadow waves (CUDA graph): %s", cudaGetErrorString(e));}
+	return TW_OK;
+}
+
+// tw_tile_shadows_batch (ex = false: at most 65535 tiles, duplicates allowed) and tw_tile_shadows_batch_ex (any tile count, duplicates refused, caller edges)
+static int tile_shadows(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp, const float *sh_in_x,
+                        const float *sh_in_y, uint8_t *smask, float *sh_out_x, float *sh_out_y, bool ex)
+{
+	if (!ctx || !zvals || !tile_xy || !sp || !smask || ntiles == 0 || zvsize < 2) return TW_ERR_ARG;
+	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	if (!ex && ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
+	size_t const cells = (size_t)ntiles*zvsize*zvsize, edge = (size_t)ntiles*zvsize;
+	twi_shadow_plan P;
+	if (!twi_shadow_plan_make(tile_xy, ntiles, sp, sh_in_x != nullptr, sh_in_y != nullptr, &P) && ex) return tw_set_error(ctx, TW_ERR_ARG, "tile_xy names a tile twice");
 	bool const dev_z = tw_is_device_ptr(zvals), dev_m = tw_is_device_ptr(smask);
 	if (dev_m && ((size_t)smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)");
-	size_t const zb = (cells*sizeof(float) + 255) & ~(size_t)255, mb = (cells + 259) & ~(size_t)255, kb = (edge*sizeof(unsigned long long) + 255) & ~(size_t)255;
-	size_t const fb = (edge*sizeof(float) + 255) & ~(size_t)255, ib = ((size_t)ntiles*sizeof(int) + 255) & ~(size_t)255;
-	int rc = tw_reserve(ctx, 0, (dev_z ? 0 : zb) + (dev_m ? 0 : mb) + 2*kb + 2*fb + 3*ib + 256); if (rc) return rc;
+	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
+	size_t const zb = al(cells*sizeof(float)), mb = al(cells + 4), kb = al(2*edge*sizeof(unsigned long long));
+	size_t const fbx = al((sh_in_x ? 2 : 1)*edge*sizeof(float)), fby = al((sh_in_y ? 2 : 1)*edge*sizeof(float)), ib = al(twi_shadow_plan_ints(ntiles)*sizeof(int));
+	int rc = tw_reserve(ctx, 0, (dev_z ? 0 : zb) + (dev_m ? 0 : mb) + kb + fbx + fby + ib + 256); if (rc) return rc;
 	char *p = (char *)ctx->d_scratch[0];
 	const float *d_z = zvals; unsigned char *d_m = smask;
 	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(p, zvals, cells*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const float *)p; p += zb;}
 	if (!dev_m) {d_m = (unsigned char *)p; p += mb;}
-	unsigned long long *d_kx = (unsigned long long *)p; p += kb;
-	unsigned long long *d_ky = (unsigned long long *)p; p += kb;
-	float *d_ox = (float *)p; p += fb;
-	float *d_oy = (float *)p; p += fb;
-	int *d_wave = (int *)p; p += ib;
-	int *d_nbx = (int *)p; p += ib;
-	int *d_nby = (int *)p;
-	TW_CUDA(ctx, cudaMemcpyAsync(d_wave, wave_tiles.data(), (size_t)ntiles*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(d_nbx, nbx.data(), (size_t)ntiles*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(d_nby, nby.data(), (size_t)ntiles*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-	shadow_init_kernel<<<ctx->num_sms*8, 256, 0, ctx->stream>>>(d_m, d_kx, cells, 2*(kb/sizeof(unsigned long long)), all_shadowed ? (unsigned char)TW_MESH_SHADOW : (unsigned char)0);
-	TW_LAUNCH_CHECK(ctx);
-	for (int l = 0; l < nlevels; ++l) {
-		int const nw = wave_start[l + 1] - wave_start[l];
-		if (trace) {
-			shadow_rays_kernel<<<dim3((4*n + 127)/128, nw), 128, 0, ctx->stream>>>(d_z, d_m, n, S, d_wave + wave_start[l], d_nbx, d_nby, d_ox, d_oy, d_kx, d_ky);
-			TW_LAUNCH_CHECK(ctx);
-		}
-		shadow_unpack_kernel<<<dim3((n + 127)/128, nw), 128, 0, ctx->stream>>>(d_kx, d_ky, d_ox, d_oy, n, d_wave + wave_start[l]);
-		TW_LAUNCH_CHECK(ctx);
-	}
+	unsigned long long *d_keys = (unsigned long long *)p; p += kb;
+	float *d_ox = (float *)p; p += fbx;
+	float *d_oy = (float *)p; p += fby;
+	int *d_plan = (int *)p;
+	std::vector<int> plan(twi_shadow_plan_ints(ntiles));
+	twi_shadow_plan_pack(P, plan.data());
+	TW_CUDA(ctx, cudaMemcpyAsync(d_plan, plan.data(), plan.size()*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+	if (sh_in_x) {TW_CUDA(ctx, cudaMemcpyAsync(d_ox + edge, sh_in_x, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+	if (sh_in_y) {TW_CUDA(ctx, cudaMemcpyAsync(d_oy + edge, sh_in_y, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+	rc = twi_shadow_enqueue(ctx, ctx->stream, P, d_z, ntiles, zvsize, d_m, d_keys, d_ox, d_oy, d_plan, false); if (rc) return rc; // the call blocks anyway
 	if (!dev_m) {TW_CUDA(ctx, cudaMemcpyAsync(smask, d_m, cells, cudaMemcpyDeviceToHost, ctx->stream));}
 	if (sh_out_x) {TW_CUDA(ctx, cudaMemcpyAsync(sh_out_x, d_ox, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	if (sh_out_y) {TW_CUDA(ctx, cudaMemcpyAsync(sh_out_y, d_oy, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
+}
+
+extern "C" int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp,
+                                     uint8_t *smask, float *sh_out_x, float *sh_out_y)
+{
+	return tile_shadows(ctx, zvals, tile_xy, ntiles, zvsize, sp, nullptr, nullptr, smask, sh_out_x, sh_out_y, false);
+}
+
+extern "C" int tw_tile_shadows_batch_ex(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp,
+                                        const float *sh_in_x, const float *sh_in_y, uint8_t *smask, float *sh_out_x, float *sh_out_y)
+{
+	return tile_shadows(ctx, zvals, tile_xy, ntiles, zvsize, sp, sh_in_x, sh_in_y, smask, sh_out_x, sh_out_y, true);
 }

@@ -297,17 +297,26 @@ public:
 // wpz_max / size: the water level and tile size of the bounds (tile_t::create_zvals, src/tiled_mesh.cpp:517-541); dx, dy also scale the normals (get_norm).
 // The overload with `shading` (tw_tile_shading, include/tw3d.h) adds the AO map (calc_mesh_ao_lighting) and the terrain weights texture (create_texture's terrain
 // part) to the same job; its outputs and device tile_params must stay valid until the job is ready. In the GPU gen modes AO makes the zvals those of create_zvals_with_ao.
+// The overload with `shadows` (tw_tile_shadows, include/tw3d.h) also computes every light's mesh shadows of the new tiles in the job, as calc_mesh_shadows (below) would
+// on the job's zvals: smask and sh_out_* must stay valid until the job is ready; tile_xy, the lights and host sh_in rows are copied during the launch. Build each
+// light's tw_shadow_params with shadow_params().
 inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
-                                    tw_tile_outputs const &out, tw_tile_shading const &shading) {
+                                    tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows) {
 	scene_globals const &g = globals();
 	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
 	tw_erosion_params const e = erosion_params_from_globals();
 	tw_ctx *c = ctx();
 	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
 	uint64_t const number = ++jobs;
-	int const rc = tw_create_tiles_launch_ex(c, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out, &shading);
+	int const rc = tw_create_tiles_launch_shadows(c, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out, &shading,
+	                                              shadows.nlights ? &shadows : nullptr);
 	if (rc != TW_OK) {detail::fail(rc, "create_tiles_async", c);}
 	return tiles_job(c, &jobs, number);
+}
+inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
+                                    tw_tile_outputs const &out, tw_tile_shading const &shading) {
+	tw_tile_shadows const none = {nullptr, 0, nullptr}; // no lights: the job of tw_create_tiles_launch_ex
+	return create_tiles_async(origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, none);
 }
 inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
                                     tw_tile_outputs const &out) {
@@ -356,9 +365,8 @@ inline void tile_ao_lighting(const float *zvals, const int32_t *origins_xy, unsi
 // calc_mesh_shadows(l, lpos, mh, smask, xsize, ysize, sh_in_x, sh_in_y, sh_out_x, sh_out_y) (src/visibility.cpp:508-517) for ALL tiles a light change dirties, in
 // one call: tile_t::calc_shadows_for_light's chain (src/tiled_mesh.cpp:664-692: each tile starts from the sh_out of its neighbours toward the light) becomes dependency
 // waves on the device. tile_xy = (x1/size, y1/size) per tile; smask = ntiles*zvsize^2 bytes (0 / MESH_SHADOW); sh_out_* optional (ntiles*zvsize floats each).
-// no_shadow = (l == LIGHT_MOON && combined_gu). Globals read: X/Y_SCENE_SIZE, DX/DY_VAL(+_INV), XY_SUM_SIZE = MESH_X_SIZE + MESH_Y_SIZE, zmin, zmax.
-inline void calc_mesh_shadows(const float lpos[3], const float *zvals, const int32_t *tile_xy, unsigned ntiles, unsigned zvsize, float dx_val, float dy_val,
-                              unsigned char *smask, float *sh_out_x = nullptr, float *sh_out_y = nullptr, bool no_shadow = false) {
+// no_shadow = (l == LIGHT_MOON && combined_gu). Globals read (shadow_params): X/Y_SCENE_SIZE, DX/DY_VAL(+_INV), XY_SUM_SIZE = MESH_X_SIZE + MESH_Y_SIZE, zmin, zmax.
+inline tw_shadow_params shadow_params(const float lpos[3], float dx_val, float dy_val, bool no_shadow = false) {
 	scene_globals const &g = globals();
 	tw_shadow_params sp;
 	for (int d = 0; d < 3; ++d) {sp.lpos[d] = lpos[d];}
@@ -366,8 +374,23 @@ inline void calc_mesh_shadows(const float lpos[3], const float *zvals, const int
 	sp.dx_val = dx_val; sp.dy_val = dy_val; sp.dx_val_inv = 1.0f/dx_val; sp.dy_val_inv = 1.0f/dy_val; // set_scene_constants: DX_VAL_INV = 1.0/DX_VAL
 	sp.xy_sum_size = g.MESH_X_SIZE + g.MESH_Y_SIZE;
 	sp.zmin = g.zmin; sp.zmax = g.zmax; sp.no_shadow = no_shadow ? 1 : 0;
+	return sp;
+}
+inline void calc_mesh_shadows(const float lpos[3], const float *zvals, const int32_t *tile_xy, unsigned ntiles, unsigned zvsize, float dx_val, float dy_val,
+                              unsigned char *smask, float *sh_out_x = nullptr, float *sh_out_y = nullptr, bool no_shadow = false) {
+	tw_shadow_params const sp = shadow_params(lpos, dx_val, dy_val, no_shadow);
 	tw_ctx *c = ctx();
 	int const rc = tw_tile_shadows_batch(c, zvals, tile_xy, ntiles, zvsize, &sp, smask, sh_out_x, sh_out_y);
+	if (rc != TW_OK) {detail::fail(rc, "calc_mesh_shadows", c);}
+}
+// The same for new tiles next to existing ones (tw_tile_shadows_batch_ex): sh_in_x / sh_in_y (ntiles*zvsize floats each, either may be null) hold, per tile, the sh_out
+// of its neighbour toward the light where that neighbour is an existing tile outside the batch (what calc_shadows_for_light reads from the tile map); rows of tiles
+// whose neighbour is in the batch are ignored. Also the way to re-shadow existing tiles once new tiles appear on their light side: pass the new tiles' sh_out.
+inline void calc_mesh_shadows(const float lpos[3], const float *zvals, const int32_t *tile_xy, unsigned ntiles, unsigned zvsize, float dx_val, float dy_val,
+                              const float *sh_in_x, const float *sh_in_y, unsigned char *smask, float *sh_out_x = nullptr, float *sh_out_y = nullptr, bool no_shadow = false) {
+	tw_shadow_params const sp = shadow_params(lpos, dx_val, dy_val, no_shadow);
+	tw_ctx *c = ctx();
+	int const rc = tw_tile_shadows_batch_ex(c, zvals, tile_xy, ntiles, zvsize, &sp, sh_in_x, sh_in_y, smask, sh_out_x, sh_out_y);
 	if (rc != TW_OK) {detail::fail(rc, "calc_mesh_shadows", c);}
 }
 

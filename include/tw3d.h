@@ -299,7 +299,8 @@ TW_API int tw_create_tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32
  *     tw_create_zvals_ao_batch's, not tw_create_zvals_batch's (the reference does the same). The z range, bounds, normal map and weights are then
  *     derived from those zvals, and tw_last_erosion_steps() after the completing poll equals its value after tw_create_zvals_ao_batch.
  * Errors: TW_ERR_ARG for weights without wp or tile_params, has_any_grass without weights, a tex_class that does not name each class once, or
- * zmax <= zmin; TW_ERR_STATE for weights before tw_set_sine_params. The layout of tw_tile_outputs is unchanged (ABI 1). */
+ * zmax <= zmin; TW_ERR_STATE for weights before tw_set_sine_params. The layout of tw_tile_outputs is unchanged (ABI 1).
+ * The per-light mesh shadows of the same tiles join the job through tw_create_tiles_launch_shadows (below, with tw_tile_shadows_batch). */
 typedef struct tw_tile_shading {
 	float                   half_dxy;      /* HALF_DXY: the AO ray's z step, as tw_tile_ao_batch */
 	const struct tw_weight_params *wp;     /* required with weights (declared below) */
@@ -416,6 +417,39 @@ typedef struct tw_shadow_params {
  * 1-thread order is reproduced. zvals / smask: host or device. */
 TW_API int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp,
                           uint8_t *smask, float *sh_out_x, float *sh_out_y);
+/* The same with incoming shadow heights from tiles OUTSIDE the batch - what calc_shadows_for_light reads from the tile map when a frame's new tiles border
+ * existing ones. With sx = (lpos.x < 0 ? -1 : 1), sy = (lpos.y < 0 ? -1 : 1), tile t at (tx, ty):
+ *   sh_in_x   optional, ntiles*zvsize floats, host or device: row t = the sh_out_x of its neighbour (tx, ty + sy)
+ *   sh_in_y   optional, ntiles*zvsize floats, host or device: row t = the sh_out_y of its neighbour (tx + sx, ty)
+ * A caller row is read only where that neighbour is NOT in the batch; an in-batch neighbour's sh_out, computed in this call, always wins. Entries
+ * <= TW_MESH_MIN_Z mean "no incoming height". With both NULL the results equal tw_tile_shadows_batch's. Unlike it, this call takes any number of tiles and
+ * returns TW_ERR_ARG when tile_xy names a tile twice.
+ * What stays the caller's job: when new tiles appear, existing tiles on their far side from the light may need new shadows, because their neighbour toward
+ * the light now exists. Which of them to redo is engine policy; redo them with this call, passing the new tiles' sh_out as their sh_in. */
+TW_API int tw_tile_shadows_batch_ex(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp,
+                          const float *sh_in_x, const float *sh_in_y, uint8_t *smask, float *sh_out_x, float *sh_out_y);
+/* Mesh shadows of a frame's new tiles inside the asynchronous tile job: tw_create_tiles_launch_shadows(..., shading, shadows) is tw_create_tiles_launch_ex
+ * (..., shading) plus, for every light, the results of tw_tile_shadows_batch_ex on the job's own final zvals (in GPU gen modes with AO: the zvals of
+ * tw_create_zvals_ao_batch, as documented above) with the same tile_xy, sp and sh_in - bit for bit. Every other output is the job's without shadows, and
+ * tw_create_tiles_launch_ex(...) is tw_create_tiles_launch_shadows(..., NULL). The shadow pass runs after every chunk's erosion (a tile's rays read its
+ * neighbours' final heights), light after light; tw_create_tiles_poll completes it with the rest. tile_xy, the lights array, each sp and HOST sh_in rows are
+ * copied during the launch; device sh_in rows are read until the completing poll; smask and sh_out_* must stay valid until then (pinned host memory or device
+ * memory for a launch that does not block). Errors (TW_ERR_ARG, nothing enqueued): no tile_xy, nlights == 0 or no lights, a light without smask, a device
+ * smask that is not 4-byte aligned, a tile named twice in tile_xy, zvsize < 2. */
+typedef struct tw_tile_light {
+	tw_shadow_params sp;               /* one light: lpos, scene sizes, zmin/zmax, no_shadow (moon with combined_gu) */
+	const float *sh_in_x, *sh_in_y;    /* optional: incoming edges from tiles outside the batch, as tw_tile_shadows_batch_ex */
+	uint8_t     *smask;                /* required: ntiles*zvsize^2 bytes, host or device (device: 4-byte aligned) */
+	float       *sh_out_x, *sh_out_y;  /* optional: ntiles*zvsize floats each, host or device */
+} tw_tile_light;
+typedef struct tw_tile_shadows {
+	const int32_t       *tile_xy;      /* required: (x1/size, y1/size) per tile, caller order */
+	uint32_t             nlights;      /* >= 1; the reference has sun and moon */
+	const tw_tile_light *lights;
+} tw_tile_shadows;
+TW_API int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                          uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                          float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows);
 
 /* ---- terrain weights texture of tiles (SURVEY.md 8f row N4): tile_t::create_texture (src/tiled_mesh.cpp:1071-1248), the terrain part ----
  * RGBA texel (x, y) of a tile, x, y < stride = zvsize - 1: the weights {sand, dirt, grass, rock} (snow = the rest) of the ground textures from the cell's relative

@@ -114,7 +114,8 @@ __device__ __forceinline__ void block_minmax(float vmin, float vmax, unsigned *m
 struct NoiseParams {
 	int   octaves;               // NUM_FREQ_COMP - start_eval_sin/N_RAND_SIN2
 	int   gen_shape;
-	float freq[9], mag[9], rx[9], ry[9]; // per-octave constants of gen_noise's loop (mag*=0.5, freq*=1.92, rx*=1.5, ry*=1.5), host-computed
+	float4 oct[9];               // per-octave constants of gen_noise's loop {freq, rx, ry, mag} (freq*=1.92, rx*=1.5, ry*=1.5, mag*=0.5), host-computed;
+	                             // packed so that an octave reads them from the constant bank with two 64-bit loads instead of four 32-bit ones
 	float xy_scale;              // MESH_SCALE_FACTOR*mesh_scale
 	float hmap_scale;            // get_hmap_scale(mode)
 	float freq_last, rsum_last;  // freq / (rx+ry) of the last octave: bound of the lattice coordinates (paired-path range guard)
@@ -125,11 +126,12 @@ __device__ __forceinline__ float gen_noise(float xv, float yv, const NoiseParams
 	float zval = 0.0f;
 #pragma unroll 1
 	for (int i = 0; i < N.octaves; ++i) {
-		float const px = N.freq[i]*xv + N.rx[i], py = N.freq[i]*yv + N.ry[i];
+		float4 const o = N.oct[i];
+		float const px = o.x*xv + o.y, py = o.x*yv + o.z;
 		float noise = SIMPLEX ? twn::simplex2(px, py) : twn::perlin2(px, py);
 		if (SHAPE == 1) {noise = (float)((double)fabsf(noise) - 0.40);}
 		if (SHAPE == 2) {noise = (float)(0.45 - (double)fabsf(noise));}
-		zval = __fmaf_rn(N.mag[i], noise, zval); // mag is a power of two: mag*noise is exact, so fused == mul-then-add
+		zval = __fmaf_rn(o.w, noise, zval); // mag is a power of two: mag*noise is exact, so fused == mul-then-add
 	}
 	return zval;
 }
@@ -177,14 +179,24 @@ noise_grid_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y_
 }
 
 #ifndef TW_NOISE2_MIN_BLOCKS
-#define TW_NOISE2_MIN_BLOCKS 3   // 74 KB of table per block (tw_noise2.cuh, level 3) => 3 blocks per SM
+#define TW_NOISE2_MIN_BLOCKS 2   // 74 KB of table per block (111 KB with the hash table of the domain-warp kernel, tw_noise2.cuh): 2 blocks of 512 threads
+                                 // = 32 warps per SM, which caps the kernel at 64 registers
 #endif
 #ifndef TW_NOISE2_PERSISTENT
-#define TW_NOISE2_PERSISTENT 0   // k > 0: single grids launch at most k waves of resident blocks, each striding over the chunk groups (table staged once per block)
+#define TW_NOISE2_PERSISTENT 1   // k > 0: single grids launch at most k waves of resident blocks, each striding over the chunk groups (table staged once per block).
+                                 // One H100, against 0: headline step 0.5 % shorter, plain simplex / Perlin 8192^2 5 % / 4 % more cells/s, e2e unchanged
+                                 // (results/h100/launch_shape.txt); tile batches launch one block per chunk group either way
 #endif
 #ifndef TW_NOISE2_THREADS
-#define TW_NOISE2_THREADS 256    // threads per block; (512, 2 blocks) = 32 warps per SM at 64 registers is the next experiment (DESIGN.md section 9)
+#define TW_NOISE2_THREADS 512    // threads per block (256 x 3 blocks = 24 warps per SM at 80 registers: 0.7 % slower on the headline, results/h100/launch_shape.txt)
 #endif
+#ifndef TW_NOISE2_BLOCK_CELLS
+// Cells per block in every mode, walked as chunks of 2*TW_NOISE2_THREADS cells: the 74 KB table fill is paid once per block (the plain modes run
+// only 8 evaluations per cell), and a 258^2 tile (66564 cells) leaves 1.5 % of the cells of its last block idle. One H100, 8192^2 headline at
+// 256 threads: 512 -> 9.76 ms, 1024 -> 9.31, 2048 -> 9.13, 4096 -> 9.15 (results/h100/warp_chunks.txt)
+#define TW_NOISE2_BLOCK_CELLS 2048
+#endif
+static_assert(TW_NOISE2_BLOCK_CELLS % (2*TW_NOISE2_THREADS) == 0, "a block walks whole chunks of 2 cells per thread");
 // ---- paired variant: two horizontally adjacent cells per thread (see tw_noise2.cuh) ----
 // |lattice coordinate| < 2^22 for every octave of this fBm call (needed by the division-free mod); NaN-safe
 __device__ __forceinline__ bool noise_lattice_in_range(float2 xv, float2 yv, const NoiseParams &N) {
@@ -192,48 +204,54 @@ __device__ __forceinline__ bool noise_lattice_in_range(float2 xv, float2 yv, con
 	return (bx < 2097152.0f && by < 2097152.0f); // |p + s| <= 1.37*(|px|+|py|) < 2^22, and floor(p)+1 stays in range for Perlin
 }
 
-template<bool SIMPLEX, int SHAPE>
+// The domain-warp simplex kernel also stages the simplex hash table (tw_noise2.cuh): 4 adds fewer per cell pair and octave. Its 37 KB fill is
+// repaid by the 40 evaluations per cell of that mode; plain simplex, 8 evaluations per cell, measured 8 % slower with it at one block per
+// 2048 cells (as tile batches launch).
+template<bool SIMPLEX, bool WARP> __host__ __device__ constexpr bool noise2_hash() {return SIMPLEX && WARP && TW_SIMPLEX_HASH_TABLE;}
+// entries of the table a block stages: the gradient table, and the hash table behind it
+template<bool HASH> __host__ __device__ constexpr int lut_entries() {return twn2::SIMPLEX_LUT_N + (HASH ? twn2::SIMPLEX_HASH_N : 0);}
+
+template<bool SIMPLEX, int SHAPE, bool HASH>
 __device__ __forceinline__ float2 gen_noise2(float2 xv, float2 yv, const NoiseParams &N, unsigned L) { // gen_noise (src/mesh_gen.cpp:706-730) for two cells; L: simplex table base (twn2::simplex_lut_base) or 0
 	float2 zval = make_float2(0.0f, 0.0f);
 	if (noise_lattice_in_range(xv, yv, N)) {
 #pragma unroll 1
 		for (int i = 0; i < N.octaves; ++i) {
-			float2 const px = twn2::add2(twn2::mul2(xv, N.freq[i]), N.rx[i]), py = twn2::add2(twn2::mul2(yv, N.freq[i]), N.ry[i]);
-			float2 noise = SIMPLEX ? ((TW_SIMPLEX_LUT > 0) ? twn2::simplex2_lut(px, py, L) : twn2::simplex2(px, py)) : ((TW_SIMPLEX_LUT > 0) ? twn2::perlin2_lut(px, py, L) : twn2::perlin2(px, py));
+			float4 const o = N.oct[i]; // {freq, rx, ry, mag}
+			float2 const px = twn2::add2(twn2::mul2(xv, o.x), o.y), py = twn2::add2(twn2::mul2(yv, o.x), o.z);
+			float2 noise = SIMPLEX ? ((TW_SIMPLEX_LUT > 0) ? twn2::simplex2_lut<HASH>(px, py, L) : twn2::simplex2(px, py)) : ((TW_SIMPLEX_LUT > 0) ? twn2::perlin2_lut(px, py, L) : twn2::perlin2(px, py));
 			if (SHAPE == 1) {noise = make_float2((float)((double)fabsf(noise.x) - 0.40), (float)((double)fabsf(noise.y) - 0.40));}
 			if (SHAPE == 2) {noise = make_float2((float)(0.45 - (double)fabsf(noise.x)), (float)(0.45 - (double)fabsf(noise.y)));}
-			zval = twn2::fma2(noise, N.mag[i], zval); // mag is a power of two: exact product
+			zval = twn2::fma2(noise, o.w, zval); // mag is a power of two: exact product
 		}
 	}
 	else {zval = make_float2(gen_noise<SIMPLEX, SHAPE>(xv.x, yv.x, N), gen_noise<SIMPLEX, SHAPE>(xv.y, yv.y, N));} // astronomically far out: scalar path with the literal division
 	return zval;
 }
 
-#ifndef TW_NOISE2_WARP_CHUNKS
-#define TW_NOISE2_WARP_CHUNKS 4 // 512-cell chunks a block of the domain-warp kernel walks per 74 KB table fill. One H100, 8192^2 headline: 1 -> 9.76 ms, 2 -> 9.31, 4 -> 9.13, 8 -> 9.15
-#endif
 #ifndef TW_NOISE2_DUAL
 #define TW_NOISE2_DUAL 0   // 1: the two independent fBm evaluations of each domain-warp stage (dx1|dy1, dx2|dy2) share one octave loop (2x the ILP per thread)
 #endif
 // two independent gen_noise2 evaluations in one octave loop: same operations per evaluation, interleaved by the compiler
-template<bool SIMPLEX, int SHAPE>
+template<bool SIMPLEX, int SHAPE, bool HASH>
 __device__ __forceinline__ void gen_noise2_dual(float2 xa, float2 ya, float2 xb, float2 yb, const NoiseParams &N, unsigned L, float2 &za, float2 &zb) {
 	if (TW_SIMPLEX_LUT > 0 && noise_lattice_in_range(xa, ya, N) && noise_lattice_in_range(xb, yb, N)) {
 		float2 zva = make_float2(0.0f, 0.0f), zvb = make_float2(0.0f, 0.0f);
 #pragma unroll 1
 		for (int i = 0; i < N.octaves; ++i) {
-			float const f = N.freq[i], rx = N.rx[i], ry = N.ry[i], mag = N.mag[i];
+			float4 const o = N.oct[i];
+			float const f = o.x, rx = o.y, ry = o.z, mag = o.w;
 			float2 const pxa = twn2::add2(twn2::mul2(xa, f), rx), pya = twn2::add2(twn2::mul2(ya, f), ry);
 			float2 const pxb = twn2::add2(twn2::mul2(xb, f), rx), pyb = twn2::add2(twn2::mul2(yb, f), ry);
-			float2 na = SIMPLEX ? twn2::simplex2_lut(pxa, pya, L) : twn2::perlin2_lut(pxa, pya, L);
-			float2 nb = SIMPLEX ? twn2::simplex2_lut(pxb, pyb, L) : twn2::perlin2_lut(pxb, pyb, L);
+			float2 na = SIMPLEX ? twn2::simplex2_lut<HASH>(pxa, pya, L) : twn2::perlin2_lut(pxa, pya, L);
+			float2 nb = SIMPLEX ? twn2::simplex2_lut<HASH>(pxb, pyb, L) : twn2::perlin2_lut(pxb, pyb, L);
 			if (SHAPE == 1) {na = make_float2((float)((double)fabsf(na.x) - 0.40), (float)((double)fabsf(na.y) - 0.40)); nb = make_float2((float)((double)fabsf(nb.x) - 0.40), (float)((double)fabsf(nb.y) - 0.40));}
 			if (SHAPE == 2) {na = make_float2((float)(0.45 - (double)fabsf(na.x)), (float)(0.45 - (double)fabsf(na.y))); nb = make_float2((float)(0.45 - (double)fabsf(nb.x)), (float)(0.45 - (double)fabsf(nb.y)));}
 			zva = twn2::fma2(na, mag, zva); zvb = twn2::fma2(nb, mag, zvb);
 		}
 		za = zva; zb = zvb;
 	}
-	else {za = gen_noise2<SIMPLEX, SHAPE>(xa, ya, N, L); zb = gen_noise2<SIMPLEX, SHAPE>(xb, yb, N, L);}
+	else {za = gen_noise2<SIMPLEX, SHAPE, HASH>(xa, ya, N, L); zb = gen_noise2<SIMPLEX, SHAPE, HASH>(xb, yb, N, L);}
 }
 
 __device__ __forceinline__ float dadd(float a, double b) {return (float)((double)a + b);} // float + double literal, rounded back (src/mesh_gen.cpp:742-745)
@@ -243,24 +261,24 @@ __global__ void __launch_bounds__(TW_NOISE2_THREADS, TW_NOISE2_MIN_BLOCKS)
 noise_grid2_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y_off, unsigned y_end, float mx0_single, float my0_single, const float2 *__restrict__ tile_origins,
 	NoiseParams N, PostParams P, const float *__restrict__ sin_tab, unsigned *__restrict__ mm, const float4 *__restrict__ simplex_lut)
 {
+	constexpr bool HASH = noise2_hash<SIMPLEX, WARP>();
 	unsigned L = 0;
 	if (TW_SIMPLEX_LUT > 0) { // hash/gradient table (simplex or Perlin flavour) -> shared memory, 8 interleaved copies (see tw_noise2.cuh)
-		extern __shared__ float4 lut_s[]; // SIMPLEX_LUT_N*SIMPLEX_LUT_COPIES entries (dynamic: 74 KB at level 3)
-		for (int e = threadIdx.x; e < twn2::SIMPLEX_LUT_N*twn2::SIMPLEX_LUT_COPIES; e += blockDim.x) {lut_s[e] = __ldg(simplex_lut + e/twn2::SIMPLEX_LUT_COPIES);}
+		extern __shared__ float4 lut_s[]; // lut_entries<HASH>()*SIMPLEX_LUT_COPIES entries (dynamic: 74 KB at level 3, + 37 KB of hash table)
+		for (int e = threadIdx.x; e < lut_entries<HASH>()*twn2::SIMPLEX_LUT_COPIES; e += blockDim.x) {lut_s[e] = __ldg(simplex_lut + e/twn2::SIMPLEX_LUT_COPIES);}
 		__syncthreads();
 		L = twn2::simplex_lut_base(lut_s, threadIdx.x);
 		asm volatile("" : "+r"(L) :: "memory"); // every table load depends on L, and L is defined after the barrier
 	}
 	// cells are numbered row-major over the band [y_off, y_end) of the grid and dealt out in pairs (2t, 2t+1): no lanes idle on widths that are
 	// not a multiple of the block width (258-wide tiles wasted 27 % of a 64x8-cell block grid); a pair may straddle a row end when nx is odd
-	// A block walks NOISE2_CHUNKS consecutive 512-cell chunks, so the table is staged once per chunk group (4 for the plain modes, whose 8
-	// evaluations per cell would otherwise be rivalled by the 74 KB fill; 1 for the 40-evaluation warp mode).
+	// A block walks NCH consecutive chunks of 2*blockDim cells (TW_NOISE2_BLOCK_CELLS in all), so the table is staged once per chunk group.
 	unsigned const tile = blockIdx.z;
 	float mx0 = mx0_single, my0 = my0_single;
 	if (tile_origins) {float2 const o = __ldg(tile_origins + tile); mx0 = o.x; my0 = o.y;}
 	size_t const c_end = (size_t)y_end*nx;
 	float lo = INFINITY, hi = -INFINITY;
-	constexpr unsigned NCH = WARP ? TW_NOISE2_WARP_CHUNKS : 4;
+	constexpr unsigned NCH = TW_NOISE2_BLOCK_CELLS/(2*TW_NOISE2_THREADS);
 	// blocks stride over the chunk groups of the band: with gridDim.x == number of groups every block does exactly one (the default); a smaller
 	// grid (TW_NOISE2_PERSISTENT: one wave of resident blocks) keeps the staged table for many chunks
 	// P.ngroups = chunk groups of this band (host-computed: a 64-bit division per thread here cost 2.5 % of the whole kernel)
@@ -285,22 +303,22 @@ noise_grid2_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y
 		if (WARP) { // domain warping, src/mesh_gen.cpp:740-747
 			float const scale = 0.2f;
 			float2 dx1, dy1, dx2, dy2;
-			if (TW_NOISE2_DUAL) {gen_noise2_dual<SIMPLEX, SHAPE>(make_float2(dadd(xv.x, 0.0), dadd(xv.y, 0.0)), make_float2(dadd(yv.x, 0.0), dadd(yv.y, 0.0)),
+			if (TW_NOISE2_DUAL) {gen_noise2_dual<SIMPLEX, SHAPE, HASH>(make_float2(dadd(xv.x, 0.0), dadd(xv.y, 0.0)), make_float2(dadd(yv.x, 0.0), dadd(yv.y, 0.0)),
 			                                                     make_float2(dadd(xv.x, 5.2), dadd(xv.y, 5.2)), make_float2(dadd(yv.x, 1.3), dadd(yv.y, 1.3)), N, L, dx1, dy1);}
 			else {
-				dx1 = gen_noise2<SIMPLEX, SHAPE>(make_float2(dadd(xv.x, 0.0), dadd(xv.y, 0.0)), make_float2(dadd(yv.x, 0.0), dadd(yv.y, 0.0)), N, L);
-				dy1 = gen_noise2<SIMPLEX, SHAPE>(make_float2(dadd(xv.x, 5.2), dadd(xv.y, 5.2)), make_float2(dadd(yv.x, 1.3), dadd(yv.y, 1.3)), N, L);
+				dx1 = gen_noise2<SIMPLEX, SHAPE, HASH>(make_float2(dadd(xv.x, 0.0), dadd(xv.y, 0.0)), make_float2(dadd(yv.x, 0.0), dadd(yv.y, 0.0)), N, L);
+				dy1 = gen_noise2<SIMPLEX, SHAPE, HASH>(make_float2(dadd(xv.x, 5.2), dadd(xv.y, 5.2)), make_float2(dadd(yv.x, 1.3), dadd(yv.y, 1.3)), N, L);
 			}
 			float2 const wx = add2(xv, mul2(dx1, scale)), wy = add2(yv, mul2(dy1, scale));
-			if (TW_NOISE2_DUAL) {gen_noise2_dual<SIMPLEX, SHAPE>(make_float2(dadd(wx.x, 1.7), dadd(wx.y, 1.7)), make_float2(dadd(wy.x, 9.2), dadd(wy.y, 9.2)),
+			if (TW_NOISE2_DUAL) {gen_noise2_dual<SIMPLEX, SHAPE, HASH>(make_float2(dadd(wx.x, 1.7), dadd(wx.y, 1.7)), make_float2(dadd(wy.x, 9.2), dadd(wy.y, 9.2)),
 			                                                     make_float2(dadd(wx.x, 8.3), dadd(wx.y, 8.3)), make_float2(dadd(wy.x, 2.8), dadd(wy.y, 2.8)), N, L, dx2, dy2);}
 			else {
-				dx2 = gen_noise2<SIMPLEX, SHAPE>(make_float2(dadd(wx.x, 1.7), dadd(wx.y, 1.7)), make_float2(dadd(wy.x, 9.2), dadd(wy.y, 9.2)), N, L);
-				dy2 = gen_noise2<SIMPLEX, SHAPE>(make_float2(dadd(wx.x, 8.3), dadd(wx.y, 8.3)), make_float2(dadd(wy.x, 2.8), dadd(wy.y, 2.8)), N, L);
+				dx2 = gen_noise2<SIMPLEX, SHAPE, HASH>(make_float2(dadd(wx.x, 1.7), dadd(wx.y, 1.7)), make_float2(dadd(wy.x, 9.2), dadd(wy.y, 9.2)), N, L);
+				dy2 = gen_noise2<SIMPLEX, SHAPE, HASH>(make_float2(dadd(wx.x, 8.3), dadd(wx.y, 8.3)), make_float2(dadd(wy.x, 2.8), dadd(wy.y, 2.8)), N, L);
 			}
 			xv = add2(xv, mul2(dx2, scale)); yv = add2(yv, mul2(dy2, scale));
 		}
-		float2 const zz = gen_noise2<SIMPLEX, SHAPE>(xv, yv, N, L);
+		float2 const zz = gen_noise2<SIMPLEX, SHAPE, HASH>(xv, yv, N, L);
 		z0 = zz.x; z1 = zz.y;
 		if (P.need_postproc) {z0 = postproc_noise_zval(z0, P.h); z1 = postproc_noise_zval(z1, P.h);}
 		z0 = z0*N.hmap_scale; z1 = z1*N.hmap_scale;
@@ -327,7 +345,7 @@ template<bool SIMPLEX, bool WARP>
 void launch_noise2(int shape, dim3 grid, dim3 block, cudaStream_t st, float *out, unsigned nx, unsigned ny, unsigned y_off, unsigned y_end, float mx0, float my0,
 	const float2 *origins, const NoiseParams &N, const PostParams &P, const float *tab, unsigned *mm, const float4 *lut)
 {
-	size_t const lut_bytes = (TW_SIMPLEX_LUT > 0) ? (size_t)twn2::SIMPLEX_LUT_N*twn2::SIMPLEX_LUT_COPIES*sizeof(float4) : 0;
+	size_t const lut_bytes = (TW_SIMPLEX_LUT > 0) ? (size_t)lut_entries<noise2_hash<SIMPLEX, WARP>()>()*twn2::SIMPLEX_LUT_COPIES*sizeof(float4) : 0;
 	// more than 48 KB of dynamic shared memory needs the opt-in; set per launch (a few hundred ns) rather than cached in a static, so that
 	// contexts on several devices in one process all get it
 	if (lut_bytes > 48*1024) {
@@ -344,13 +362,16 @@ void launch_noise2(int shape, dim3 grid, dim3 block, cudaStream_t st, float *out
 	}
 }
 
-__global__ void simplex_lut_kernel(float4 *__restrict__ lut) { // [0, N): simplex table, [N, 2N): Perlin table
+constexpr int PERLIN_LUT_OFFSET = lut_entries<true>();
+__global__ void simplex_lut_kernel(float4 *__restrict__ lut) { // [0, N): simplex table, [N, N + H): simplex hash table, [N + H, 2N + H): Perlin table
 	int const k = blockIdx.x*blockDim.x + threadIdx.x;
-	if (k < twn2::SIMPLEX_LUT_N) {lut[k] = twn2::simplex_lut_entry((float)k); lut[twn2::SIMPLEX_LUT_N + k] = twn2::perlin_lut_entry((float)k);}
+	if (k < twn2::SIMPLEX_LUT_N) {lut[k] = twn2::simplex_lut_entry((float)k); lut[PERLIN_LUT_OFFSET + k] = twn2::perlin_lut_entry((float)k);}
+	if (k < twn2::SIMPLEX_HASH_N) {lut[twn2::SIMPLEX_LUT_N + k] = twn2::simplex_hash_entry((float)k);}
 }
 static int ensure_simplex_lut(tw_ctx *ctx) {
 	if (ctx->d_simplex_lut) return TW_OK;
-	TW_CUDA(ctx, cudaMalloc(&ctx->d_simplex_lut, 2*twn2::SIMPLEX_LUT_N*sizeof(float4)));
+	static_assert(twn2::SIMPLEX_HASH_N <= twn2::SIMPLEX_LUT_N, "simplex_lut_kernel's grid covers the gradient tables");
+	TW_CUDA(ctx, cudaMalloc(&ctx->d_simplex_lut, (PERLIN_LUT_OFFSET + twn2::SIMPLEX_LUT_N)*sizeof(float4)));
 	simplex_lut_kernel<<<(twn2::SIMPLEX_LUT_N + 127)/128, 128, 0, ctx->stream>>>((float4 *)ctx->d_simplex_lut);
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
@@ -616,10 +637,11 @@ static bool make_noise_params(const tw_height_params *p, NoiseParams &N, bool &s
 	N.gen_shape = p->gen_shape;
 	float mag = 1.0f, freq = 1.0f, rx = p->rx, ry = p->ry;
 	for (int i = 0; i < 9; ++i) { // loop-carried constants of gen_noise, src/mesh_gen.cpp:725-728
-		N.mag[i] = mag; N.freq[i] = freq; N.rx[i] = rx; N.ry[i] = ry;
+		N.oct[i] = make_float4(freq, rx, ry, mag);
 		mag *= 0.5f; freq *= 1.92f; rx *= 1.5f; ry *= 1.5f;
 	}
-	N.freq_last = N.freq[N.octaves > 0 ? N.octaves - 1 : 0]; N.rsum_last = N.rx[N.octaves > 0 ? N.octaves - 1 : 0] + N.ry[N.octaves > 0 ? N.octaves - 1 : 0];
+	float4 const last = N.oct[N.octaves > 0 ? N.octaves - 1 : 0];
+	N.freq_last = last.x; N.rsum_last = last.y + last.z;
 	N.xy_scale = 0.0007f*p->mesh_scale; // MESH_SCALE_FACTOR, src/mesh_gen.cpp:23,737
 	simplex = (p->gen_mode == TW_MGEN_SIMPLEX || p->gen_mode == TW_MGEN_SIMPLEX_GPU || p->gen_mode == TW_MGEN_DWARP_GPU);
 	N.hmap_scale = (simplex ? 16.0f : 32.0f)*p->mesh_height*p->mesh_height_scale*p->mesh_scale_z_inv; // get_hmap_scale, :550-553
@@ -645,15 +667,14 @@ int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, in
 		if (!make_noise_params(p, N, simplex)) return tw_set_error(ctx, TW_ERR_ARG, "start_eval_sin %d out of range", p->start_eval_sin);
 		bool const warp = (p->gen_mode == TW_MGEN_DWARP_GPU);
 		{int const rc = ensure_simplex_lut(ctx); if (rc) return rc;}
-		const float4 *lut = (const float4 *)ctx->d_simplex_lut + (simplex ? 0 : twn2::SIMPLEX_LUT_N);
+		const float4 *lut = (const float4 *)ctx->d_simplex_lut + (simplex ? 0 : PERLIN_LUT_OFFSET);
 		unsigned const band_rows = band_rows_for(ctx, ny, nx, h_out_bands != nullptr && ntiles == 1);
 		for (unsigned r0 = 0; r0 < ny; r0 += band_rows) {
 			unsigned const r1 = (ny - r0 < band_rows) ? ny : r0 + band_rows;
 			static bool const use_scalar = (getenv("TW_NOISE_SCALAR") != nullptr); // A/B switch: one cell per thread, scalar FMUL/FADD
 			if (!use_scalar) { // two cells per thread
 				size_t const band_cells = (size_t)(r1 - r0)*nx;
-				size_t const cells_per_block = 2*TW_NOISE2_THREADS*(size_t)((p->gen_mode == TW_MGEN_DWARP_GPU) ? TW_NOISE2_WARP_CHUNKS : 4); // noise_grid2_kernel: NCH chunks of blockDim threads x 2 cells
-				unsigned gx = (unsigned)((band_cells + cells_per_block - 1)/cells_per_block);
+				unsigned gx = (unsigned)((band_cells + TW_NOISE2_BLOCK_CELLS - 1)/TW_NOISE2_BLOCK_CELLS);
 				P.ngroups = gx;
 #if TW_NOISE2_PERSISTENT
 				{unsigned const wave = ctx->num_sms*TW_NOISE2_MIN_BLOCKS*TW_NOISE2_PERSISTENT; if (ntiles == 1 && gx > wave) gx = wave;} // TW_NOISE2_PERSISTENT waves' worth of resident blocks

@@ -41,7 +41,7 @@ struct tw_ctx {
 	// uploaded tables
 	float  *d_sin_table = nullptr;     // [65536]  sin_table (src/sinf.h:11)
 	void   *d_glm3_lut = nullptr;      // float4[2*291]: simplex(vec3) / perlin(vec3) normalised gradient + permute tables (voxel density)
-	void   *d_simplex_lut = nullptr;   // float4[291] {a0, h, norm, permute(k)}: simplex hash/gradient table (tw_noise2.cuh), built on first use
+	void   *d_simplex_lut = nullptr;   // float4 simplex gradient table, simplex hash table, Perlin gradient table (tw_noise2.cuh, tw_heightgen.cu), built on first use
 	float2 *d_dir_table = nullptr;     // [1000000] (cosf(a_k), sinf(a_k)), a_k = float(1e-6*k)*TWO_PI, host libm (src/erosion.cpp:85-86)
 	float  *d_sine_params = nullptr;   // [450] sinTable
 	float   h_sine_params[TW_F_TABLE_SIZE*5];

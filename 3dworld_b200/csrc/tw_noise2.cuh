@@ -34,6 +34,11 @@ __device__ __forceinline__ f2 fma2(f2 a, float b, f2 c) {return raw_fma(a, splat
 __device__ __forceinline__ f2 fma2(f2 a, float b, float c) {return raw_fma(a, splat(b), splat(c));}
 __device__ __forceinline__ f2 abs2(f2 a) {return make_float2(fabsf(a.x), fabsf(a.y));}
 __device__ __forceinline__ f2 max0_2(f2 a) {return make_float2(fmaxf(a.x, 0.0f), fmaxf(a.y, 0.0f));} // see twn::gmax0
+// max(a - d, 0) as one saturating subtract (FADD.SAT) for the simplex falloff terms, d a sum of squares, a = 0.5 or 0.6: the same bits as
+// fmaxf(a - d, 0.0f) for every d. The saturation clamps to [0, 1]; d >= 0 keeps a - d <= a < 1, so only the lower clamp can act, and it is max(., 0).
+// A NaN saturates to +0, as fmaxf(NaN, 0) returns +0; an exact zero difference is +0 under round-to-nearest either way.
+__device__ __forceinline__ float rsub_max0(float a, float d) {float r; asm("sub.rn.sat.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(d)); return r;}
+__device__ __forceinline__ f2 rsub_max0_2(float a, f2 d) {return make_float2(rsub_max0(a, d.x), rsub_max0(a, d.y));}
 __device__ __forceinline__ f2 floor2(f2 x) {return make_float2(floorf(x.x), floorf(x.y));}
 
 __device__ __forceinline__ f2 mod289(f2 x)  {f2 const t = floor2(mul2(x, 1.0f/289.0f)); return fma2(t, -289.0f, x);}
@@ -97,8 +102,8 @@ __device__ __forceinline__ f2 simplex2(f2 vx, f2 vy) {
 // of an LDS.128 then hit 8 different 16-byte bank groups by construction (conflict-free, 4 cycles per warp load).
 // Level 3 folds the second permute into the gradient entries: entry k = {gradient of permute(k), permute(k)} for every reachable argument
 // k = permute(iy') + ix' <= 578, so the gradient is fetched at k directly and the second hash (8 instructions + 4 floors per cell pair and corner)
-// disappears at no extra load; the table grows to 580 entries (74 KB with the 8 copies => 3 blocks of 256 threads per SM, which measured
-// the same as 5 before: the kernel is pipe-bound, not latency-bound).
+// disappears at no extra load; the table grows to 580 entries (74 KB with the 8 copies; 3 blocks of 256 threads per SM measured the same as 5
+// before it: the kernel is bound by instruction issue).
 #ifndef TW_SIMPLEX_LUT
 #define TW_SIMPLEX_LUT 3
 #endif
@@ -134,6 +139,20 @@ __device__ __forceinline__ float4 simplex_lut_entry(float k) { // scalar restate
 #endif
 constexpr unsigned SIMPLEX_LUT_MAGIC_BITS = 0x4B400000u; // bits of 12582912.0f = 1.5*2^23
 constexpr unsigned LUT_ENTRY_BYTES = 16u*SIMPLEX_LUT_COPIES;
+
+// Simplex hash table (level 3 with the denormal addressing): SIMPLEX_HASH_N entries staged right behind the gradient table, in the same 8-copy
+// layout, entry k = {permute(k), permute(k) + 1, permute(k + 1) + 1, 0}. The three second-permute arguments of a cell then cost one add each:
+//   p0 = q0 + ix = [iy].x + ix,   p2 = (q2 + ix) + 1 = [iy].z + ix,
+//   p1 = (q1 + ix) + i1.x = [iy].y + ix (i1.y = 0) or [iy + 1].x + ix (i1.y = 1): the word at entry iy's address + 4 + 124*i1.y.
+// Exact: every operand is an integer below 2^24, so any order of the adds gives the same value. iy comes from mod_int289_lazy (<= 289), so entries
+// up to 290 are read; entry 290 needs permute(291), which the float arithmetic of permute() evaluates exactly (= permute(2)).
+#define TW_SIMPLEX_HASH_TABLE (TW_SIMPLEX_LUT >= 3 && TW_LUT_DENORM && !TW_HASH_Q1_ARITH)
+constexpr int SIMPLEX_HASH_N = TW_SIMPLEX_HASH_TABLE ? 291 : 0;
+constexpr unsigned SIMPLEX_HASH_OFFSET = SIMPLEX_LUT_N*LUT_ENTRY_BYTES; // byte distance from entry k of the gradient table to entry k of the hash table
+__device__ __forceinline__ float4 simplex_hash_entry(float k) {
+	float const pk = twn::permute(k);
+	return make_float4(pk, pk + 1.0f, twn::permute(k + 1.0f) + 1.0f, 0.0f);
+}
 __device__ __forceinline__ unsigned simplex_lut_base(const float4 *lut_s, unsigned lane) {
 	unsigned const a = (unsigned)__cvta_generic_to_shared(lut_s) + (lane & (SIMPLEX_LUT_COPIES - 1))*16u;
 	return TW_LUT_DENORM ? a : a - SIMPLEX_LUT_MAGIC_BITS;
@@ -157,9 +176,26 @@ __device__ __forceinline__ float lut_load_w_addr_next(unsigned addr) { // .w of 
 	return v;
 }
 __device__ __forceinline__ float lut_load_w(unsigned Lb, float off) {return lut_load_w_addr(lut_addr(Lb, off));}
+template<unsigned OFF> __device__ __forceinline__ float lut_load_f32(unsigned addr) { // one word at a constant byte offset (an LDS immediate)
+	float v; asm("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(addr), "n"(OFF));
+	return v;
+}
 
-// glm::simplex(vec2) for two positions with the table; Lb = simplex_lut_base()
+// arguments of the second permute for two cells from the simplex hash table (ix, iy: lattice indices after mod_int289_lazy)
+__device__ __forceinline__ void simplex_hash_args(f2 ix, f2 iy, f2 i1y, unsigned Lb, f2 &p0, f2 &p1, f2 &p2) {
+	constexpr unsigned H = SIMPLEX_HASH_OFFSET;
+	f2 const j0 = lut_offsets(iy, Lb); // address of entry iy of the gradient table; + H: of the hash table
+	f2 const j1 = raw_fma(i1y, splat(__uint_as_float(LUT_ENTRY_BYTES - 4)), j0); // + 124 bytes when i1.y = 1 (see simplex_hash_entry)
+	unsigned const ja = __float_as_uint(j0.x), jb = __float_as_uint(j0.y), j1a = __float_as_uint(j1.x), j1b = __float_as_uint(j1.y);
+	p0 = add2(make_float2(lut_load_f32<H>(ja), lut_load_f32<H>(jb)), ix);
+	p1 = add2(make_float2(lut_load_f32<H + 4>(j1a), lut_load_f32<H + 4>(j1b)), ix);
+	p2 = add2(make_float2(lut_load_f32<H + 8>(ja), lut_load_f32<H + 8>(jb)), ix);
+}
+
+// glm::simplex(vec2) for two positions with the table; Lb = simplex_lut_base(); HASH: the block staged the simplex hash table too
+template<bool HASH>
 __device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
+	static_assert(!HASH || TW_SIMPLEX_HASH_TABLE, "the hash table exists at level 3 with the denormal addressing only");
 	float const Cx = 0.211324865405187f, Cy = 0.366025403784439f, Cz = -0.577350269189626f;
 	f2 const s = sumprod2(vx, Cy, vy, Cy);
 	f2 ix = floor2(add2(vx, s)), iy = floor2(add2(vy, s));
@@ -168,6 +204,9 @@ __device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
 	f2 const i1x = make_float2((x0x.x > x0y.x) ? 1.0f : 0.0f, (x0x.y > x0y.y) ? 1.0f : 0.0f);
 	f2 const i1y = rsub2(1.0f, i1x); // (1,0) or (0,1)
 	f2 const x12x = sub2(add2(x0x, Cx), i1x), x12y = sub2(add2(x0y, Cx), i1y), x12z = add2(x0x, Cz), x12w = add2(x0y, Cz);
+	f2 p0, p1, p2;
+	if constexpr (HASH) {simplex_hash_args(mod_int289_lazy(ix), mod_int289_lazy(iy), i1y, Lb, p0, p1, p2);}
+	else {
 #if TW_SIMPLEX_LUT >= 2
 	ix = mod_int289_lazy(ix); iy = mod_int289_lazy(iy);
 	// permute(iy), permute(iy + i1.y), permute(iy + 1): consecutive table entries, so the second and third addresses are the first plus 0/128/256 bytes
@@ -193,15 +232,16 @@ __device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
 	// All of these are small non-negative integers, exact in fp32 in any order: with d = q2 - q0 and e = p0 + 1, p2 = e + d and p1 = e + i1.y*(d - 1)
 	// (a product by 0 or 1 plus an integer: fused or not, the same number). Two table loads fewer per pair of cells - the shared-memory pipe is the
 	// second-busiest unit of this kernel - for one more FMA per cell.
-	f2 const p0 = add2(q0, ix), dq = sub2(q2, q0), e1 = add2(p0, 1.0f), p2 = add2(e1, dq), p1 = raw_fma(i1y, add2(dq, -1.0f), e1);
+	p0 = add2(q0, ix); f2 const dq = sub2(q2, q0), e1 = add2(p0, 1.0f); p2 = add2(e1, dq); p1 = raw_fma(i1y, add2(dq, -1.0f), e1);
 #elif TW_SIMPLEX_LUT >= 3
-	f2 const p0 = add2(q0, ix), p1 = add2(add2(q1, ix), i1x), p2 = add2(add2(q2, ix), 1.0f); // the table is indexed by the argument of the second permute (q: table values, ix: an fma result)
+	p0 = add2(q0, ix); p1 = add2(add2(q1, ix), i1x); p2 = add2(add2(q2, ix), 1.0f); // the table is indexed by the argument of the second permute (q: table values, ix: an fma result)
 #else
-	f2 const p0 = permute(add2(q0, ix)), p1 = permute(add2(add2(q1, ix), i1x)), p2 = permute(add2(add2(q2, ix), 1.0f));
+	p0 = permute(add2(q0, ix)); p1 = permute(add2(add2(q1, ix), i1x)); p2 = permute(add2(add2(q2, ix), 1.0f));
 #endif
-	f2 m0 = max0_2(rsub2(0.5f, sumprod2(x0x, x0x, x0y, x0y)));
-	f2 m1 = max0_2(rsub2(0.5f, sumprod2(x12x, x12x, x12y, x12y)));
-	f2 m2 = max0_2(rsub2(0.5f, sumprod2(x12z, x12z, x12w, x12w)));
+	}
+	f2 m0 = rsub_max0_2(0.5f, sumprod2(x0x, x0x, x0y, x0y));
+	f2 m1 = rsub_max0_2(0.5f, sumprod2(x12x, x12x, x12y, x12y));
+	f2 m2 = rsub_max0_2(0.5f, sumprod2(x12z, x12z, x12w, x12w));
 	m0 = mul2(m0, m0); m1 = mul2(m1, m1); m2 = mul2(m2, m2);
 	m0 = mul2(m0, m0); m1 = mul2(m1, m1); m2 = mul2(m2, m2);
 	f2 const k0 = lut_offsets(p0, Lb), k1 = lut_offsets(p1, Lb), k2 = lut_offsets(p2, Lb);
@@ -329,8 +369,8 @@ __device__ __forceinline__ float simplex3_lut(float vx, float vy, float vz, unsi
 	float const p2 = twn::permute(q2 + i1_ + i2y)  + i0 + i2x;
 	float const p3 = twn::permute(q3 + i1_ + 1.0f) + i0 + 1.0f;
 	float4 const P0 = lut_load4(Lb, lut_offset1(p0, Lb)), P1 = lut_load4(Lb, lut_offset1(p1, Lb)), P2 = lut_load4(Lb, lut_offset1(p2, Lb)), P3 = lut_load4(Lb, lut_offset1(p3, Lb));
-	float m0 = twn::gmax0(0.6f - (x0x*x0x + x0y*x0y + x0z*x0z)), m1 = twn::gmax0(0.6f - (x1x*x1x + x1y*x1y + x1z*x1z));
-	float m2 = twn::gmax0(0.6f - (x2x*x2x + x2y*x2y + x2z*x2z)), m3 = twn::gmax0(0.6f - (x3x*x3x + x3y*x3y + x3z*x3z));
+	float m0 = rsub_max0(0.6f, x0x*x0x + x0y*x0y + x0z*x0z), m1 = rsub_max0(0.6f, x1x*x1x + x1y*x1y + x1z*x1z);
+	float m2 = rsub_max0(0.6f, x2x*x2x + x2y*x2y + x2z*x2z), m3 = rsub_max0(0.6f, x3x*x3x + x3y*x3y + x3z*x3z);
 	m0 = m0*m0; m1 = m1*m1; m2 = m2*m2; m3 = m3*m3;
 	float const d0 = P0.x*x0x + P0.y*x0y + P0.z*x0z, d1 = P1.x*x1x + P1.y*x1y + P1.z*x1z;
 	float const d2 = P2.x*x2x + P2.y*x2y + P2.z*x2z, d3 = P3.x*x3x + P3.y*x3y + P3.z*x3z;

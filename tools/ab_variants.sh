@@ -1,9 +1,9 @@
 #!/bin/bash
 # A/B helper for kernel experiments: builds one library per set of extra nvcc flags into tools/ab/ (git-ignored),
 # then prints the command that runs the parity tests once and the kernel-only bench for every variant, to be run on the GPU machine.
-#   tools/ab_variants.sh base "" t512 "-DTW_NOISE2_THREADS=512 -DTW_NOISE2_MIN_BLOCKS=2" lut2 "-DTW_SIMPLEX_LUT=2 -DTW_NOISE2_MIN_BLOCKS=5"
+#   tools/ab_variants.sh base "" t256 "-DTW_NOISE2_THREADS=256 -DTW_NOISE2_MIN_BLOCKS=3" lut2 "-DTW_SIMPLEX_LUT=2 -DTW_NOISE2_THREADS=256 -DTW_NOISE2_MIN_BLOCKS=5"
 # Knobs that exist today: TW_SIMPLEX_LUT (0 no table, 1 gradient, 2 + first hash, 3 + second hash folded = shipped), TW_NOISE2_MIN_BLOCKS,
-# TW_NOISE2_THREADS (tw_heightgen.cu); run-time: TW_NOISE_SCALAR=1 (scalar kernel), TW_EROSION_LANES, TW_PIPE_CHUNKS.
+# TW_NOISE2_THREADS, TW_NOISE2_BLOCK_CELLS, TW_NOISE2_PERSISTENT (tw_heightgen.cu); run-time: TW_NOISE_SCALAR=1 (scalar kernel), TW_EROSION_LANES, TW_PIPE_CHUNKS.
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p tools/ab

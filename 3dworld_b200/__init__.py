@@ -134,7 +134,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_destroy", "tw_last_error", "tw
                "tw_build_sin_table", "tw_compute_scale", "tw_gen_sine_params", "tw_gen_rx_ry", "tw_noise3d_gen_sines",
                "tw_water_z_height", "tw_set_sin_table", "tw_set_sine_params", "tw_heightgen_2d", "tw_heightgen_2d_launch",
                "tw_heightgen_2d_poll", "tw_heightgen_tiles", "tw_create_zvals_batch", "tw_create_tiles_launch", "tw_create_tiles_launch_ex", "tw_create_tiles_poll", "tw_tile_bounds_batch", "tw_tile_normals_batch", "tw_tile_ao_batch", "tw_create_zvals_ao_batch", "tw_glaciate_mesh", "tw_eval_points", "tw_erode", "tw_erode_parallel", "tw_erode_tiles", "tw_last_erosion_steps", "tw_voxel_fill",
-               "tw_heightmap_from_floats_u16", "tw_heightmap_to_floats_u16", "tw_proc_gen_heightmap", "tw_heightmap_sample_tiles", "tw_minmax_f32",
+               "tw_heightmap_from_floats_u16", "tw_heightmap_to_floats_u16", "tw_proc_gen_heightmap", "tw_heightmap_sample_tiles", "tw_set_heightmap", "tw_create_tiles_launch_hmap", "tw_minmax_f32",
                "tw_multi_create", "tw_multi_destroy", "tw_multi_size", "tw_multi_ctx", "tw_multi_last_error", "tw_multi_set_sine_params", "tw_multi_range",
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables"]
@@ -181,6 +181,7 @@ def _load():
                                          C.POINTER(ErosionParams), C.c_float, C.c_float, C.c_uint32, C.POINTER(TileOutputs)]
     L.tw_create_tiles_launch_ex.argtypes = L.tw_create_tiles_launch.argtypes + [C.POINTER(TileShading)]
     L.tw_create_tiles_launch_shadows.argtypes = L.tw_create_tiles_launch_ex.argtypes + [C.POINTER(TileShadows)]
+    L.tw_create_tiles_launch_hmap.argtypes = [vp, C.POINTER(HmapSampler)] + L.tw_create_tiles_launch_shadows.argtypes[1:]
     L.tw_create_tiles_poll.argtypes = [vp, C.c_int]
     L.tw_tile_bounds_batch.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_uint32, vp]
     L.tw_glaciate_mesh.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(HeightParams), C.POINTER(MinMax)]
@@ -190,6 +191,7 @@ def _load():
     L.tw_create_zvals_ao_batch.argtypes = [vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint32, C.POINTER(HeightParams), C.c_uint32,
                                            C.POINTER(ErosionParams), C.c_float, C.c_float, vp, vp, vp]
     L.tw_heightmap_sample_tiles.argtypes = [vp, vp, C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp]
+    L.tw_set_heightmap.argtypes = [vp, vp, C.c_int, C.c_int]
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_erode_parallel.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_uint32, C.POINTER(ErosionParams), C.c_uint32]
     L.tw_erode_tiles.argtypes = [vp, vp, C.c_uint32, C.c_int, C.c_int, vp, C.c_float, C.c_uint32, C.POINTER(ErosionParams)]
@@ -484,9 +486,10 @@ class Context:
 
     def create_tiles_launch(self, origins_xy, mesh_size, dx, dy, zvsize, hp, erosion_iters, ep, min_zval, zvals, mm=None, bounds=None, normals=None,
                             min_normal_z=None, wpz_max=0.0, size=0, ao=None, weights=None, has_any_grass=None, half_dxy=None, wp=None, tile_params=None,
-                            tile_xy=None, lights=None):
+                            tile_xy=None, lights=None, hmap=None):
         """tw_create_tiles_launch(_ex): a frame's new tiles (heights, erosion, z range, sub-block bounds, normal map, and on request the AO map and the
-        terrain weights texture) enqueued without waiting for the GPU.
+        terrain weights texture) enqueued without waiting for the GPU. hmap (HmapSampler) takes the heights from the image of set_heightmap instead of the
+        height function (tw_create_tiles_launch_hmap): hp may then be None unless weights is given, and ao is refused.
         zvals [nt, zv, zv] float32, normals [nt, zv-1, zv-1, 4] uint8, ao [nt, zv-1, zv-1] uint8 and weights [nt, zv-1, zv-1, 4] uint8: numpy arrays
         (pinned for a launch that does not block) or CUDA tensors; mm [nt, 2] float32, bounds (TileBounds * nt) and min_normal_z [nt] float32 are host
         arrays that the completing create_tiles_poll fills, has_any_grass [nt] uint8 is either. weights needs wp (WeightParams) and tile_params
@@ -498,7 +501,8 @@ class Context:
         org = np.ascontiguousarray(origins_xy, np.int32).reshape(-1, 2)
         nt = org.shape[0]
         outs = TileOutputs(_ptr(zvals), _ptr(mm), C.cast(bounds, C.c_void_p) if bounds is not None else None, _ptr(normals), _ptr(min_normal_z))
-        args = [self._h, _ptr(org), nt, mesh_size[0], mesh_size[1], dx, dy, zvsize, C.byref(hp), erosion_iters, C.byref(ep) if ep is not None else None,
+        args = [self._h, _ptr(org), nt, mesh_size[0], mesh_size[1], dx, dy, zvsize, C.byref(hp) if hp is not None else None, erosion_iters,
+                C.byref(ep) if ep is not None else None,
                 min_zval, wpz_max, size, C.byref(outs)]
         shading = None
         if ao is not None and half_dxy is None:
@@ -520,7 +524,10 @@ class Context:
                 arr[i] = TileLight(r.sp, _ptr(k[3]), _ptr(k[4]), _ptr(k[0]), _ptr(k[1]), _ptr(k[2]))
             shadows = TileShadows(_ptr(tile_xy), len(recs), C.cast(arr, C.c_void_p))
             keep.append(arr)
-        if shadows is not None:
+        if hmap is not None:
+            self._check(lib.tw_create_tiles_launch_hmap(args[0], C.byref(hmap), *args[1:], C.byref(shading) if shading is not None else None,
+                                                        C.byref(shadows) if shadows is not None else None))
+        elif shadows is not None:
             self._check(lib.tw_create_tiles_launch_shadows(*args, C.byref(shading) if shading is not None else None, C.byref(shadows)))
         elif shading is not None:
             self._check(lib.tw_create_tiles_launch_ex(*args, C.byref(shading)))
@@ -552,6 +559,18 @@ class Context:
             out = np.empty((nt, zvsize, zvsize), np.float32)
         self._check(lib.tw_heightmap_sample_tiles(self._h, _ptr(data16), C.byref(hs), _ptr(org), nt, zvsize, _ptr(out)))
         return out
+
+    def set_heightmap(self, data16):
+        """tw_set_heightmap: the image create_tiles_launch(hmap=...) samples, copied to device memory this context owns; data16 = uint8 [h, w, 2]
+        (numpy or CUDA tensor), None releases it."""
+        if data16 is None:
+            self._check(lib.tw_set_heightmap(self._h, None, 0, 0))
+            return
+        if not hasattr(data16, "data_ptr"):
+            data16 = np.ascontiguousarray(data16, np.uint8)
+        if len(data16.shape) != 3 or data16.shape[2] != 2:
+            raise ValueError("set_heightmap: data16 must have shape [h, w, 2]")
+        self._check(lib.tw_set_heightmap(self._h, _ptr(data16), int(data16.shape[1]), int(data16.shape[0])))
 
     def tile_normals(self, tiles, dx_val, dy_val, out=None):
         """tile_t::upload_normal_texture for a batch: returns (rgba [nt, stride, stride, 4] uint8, min_normal_z [nt])."""

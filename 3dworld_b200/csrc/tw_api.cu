@@ -188,6 +188,7 @@ void tw_destroy(tw_ctx *ctx) {
 	if (ctx->d_simplex_lut) cudaFree(ctx->d_simplex_lut);
 	if (ctx->d_glm3_lut) cudaFree(ctx->d_glm3_lut);
 	if (ctx->d_sine_params) cudaFree(ctx->d_sine_params);
+	if (ctx->d_hmap) cudaFree(ctx->d_hmap);
 	if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
 	if (ctx->async.done) cudaEventDestroy(ctx->async.done);
 	for (int i = 0; i < 3; ++i) {if (ctx->aux_stream[i]) cudaStreamDestroy(ctx->aux_stream[i]);}
@@ -447,12 +448,13 @@ int tw_erode_tiles(tw_ctx *ctx, float *maps, uint32_t ntiles, int xsize, int ysi
 
 // The tile pipeline behind tw_create_zvals_batch, tw_create_zvals_ao_batch and tw_create_tiles_launch(_ex, _shadows): enqueues everything and returns
 // without waiting for the device; the job completes through poll_job (check_ctx and finish_pending have run). sh (optional): AO map and weights texture;
-// shs (optional): per-light mesh shadows.
+// shs (optional): per-light mesh shadows. hs: the height source - nullptr = the procedural height function p, else the context's heightmap image under hs
+// (tw_create_tiles_launch_hmap, which has checked hs against the image and refused AO); p is then only read by the weights' jitter noise.
 static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy, uint32_t zvsize,
                         const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
-                        const tw_tile_outputs *o, const tw_tile_shading *sh, const tw_tile_shadows *shs)
+                        const tw_tile_outputs *o, const tw_tile_shading *sh, const tw_tile_shadows *shs, const tw_hmap_sampler *hs)
 {
-	if (!origins_xy || ntiles == 0 || !p || !o || !o->zvals) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
+	if (!origins_xy || ntiles == 0 || (!p && !hs) || !o || !o->zvals) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	bool const want_mm = (o->mm != nullptr), want_bounds = (o->bounds != nullptr), want_normals = (o->normals_rgba != nullptr), want_mnz = (o->min_normal_z != nullptr);
 	bool const want_ao = (sh && sh->ao), want_w = (sh && sh->weights), want_f = (sh && sh->has_any_grass);
 	if (want_mnz && !want_normals) return tw_set_error(ctx, TW_ERR_ARG, "min_normal_z is produced with the normal map: pass normals_rgba too");
@@ -485,10 +487,16 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		}
 	}
 	tw_grid2d g; g.x0 = 0; g.y0 = 0; g.dx = dx; g.dy = dy; g.nx = zvsize; g.ny = zvsize;
-	int rc = validate_height(ctx, &g, p, o->zvals); if (rc) return rc;
+	int rc = TW_OK;
+	if (!hs) {rc = validate_height(ctx, &g, p, o->zvals); if (rc) return rc;}
+	else {
+		if (zvsize == 0) return tw_set_error(ctx, TW_ERR_ARG, "zvsize must be > 0");
+		if (want_w && !p) return tw_set_error(ctx, TW_ERR_ARG, "the weights texture needs p (its jitter noise is the height function's sine mode)");
+		if (want_w && !ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
+	}
 	if (want_w && !ctx->have_sine_params) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sine_params() has not been called (the weights texture's jitter noise is sine mode)");
 	bool const erode = (erosion_iters > 0 && ep && ep->erode_amount > 0.0);
-	bool const sine = (p->gen_mode == TW_MGEN_SINE); // sine tables: one batched generation up front (twi_heightgen_sine_tiles), no schedule order
+	bool const sine = (!hs && p->gen_mode == TW_MGEN_SINE); // sine tables: one batched generation up front (twi_heightgen_sine_tiles), no schedule order
 	// AO with a GPU gen mode: the context is generated once and the zvals are cut from it before erosion (src/tiled_mesh.cpp:479-487,505); rays read the un-eroded context
 	bool const ctx_mode = want_ao && p->gen_mode >= TW_MGEN_SIMPLEX_GPU;
 	uint32_t const stride = zvsize - 1, ray = 36, csz = stride + 2*ray; // AO_RAY_LEN, context_sz (src/tiled_mesh.cpp:43,601)
@@ -627,9 +635,12 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	rc = tw_reserve_pinned(ctx, off_f + (want_f ? al(ntiles) : 0)); if (rc) return rc;
 	char *h_stage = (char *)ctx->h_pinned;
 	float2 *h_org = (float2 *)h_stage;
-	for (uint32_t t = 0; t < ntiles; ++t) { // build_arrays((x1 - MESH_X_SIZE/2), (y1 - MESH_Y_SIZE/2), ...): int -> float, mx0 = dx*x0 (src/tiled_mesh.cpp:461, src/mesh_gen.cpp:591)
-		float const x0 = (float)(origins_xy[2*t] - mesh_x_size/2), y0 = (float)(origins_xy[2*t+1] - mesh_y_size/2);
-		h_org[t] = make_float2(dx*x0, dy*y0);
+	if (hs) {memcpy(h_stage, origins_xy, (size_t)ntiles*2*sizeof(int32_t));} // the sampler reads the int (x1, y1) origins (d_org then holds int2)
+	else {
+		for (uint32_t t = 0; t < ntiles; ++t) { // build_arrays((x1 - MESH_X_SIZE/2), (y1 - MESH_Y_SIZE/2), ...): int -> float, mx0 = dx*x0 (src/tiled_mesh.cpp:461, src/mesh_gen.cpp:591)
+			float const x0 = (float)(origins_xy[2*t] - mesh_x_size/2), y0 = (float)(origins_xy[2*t+1] - mesh_y_size/2);
+			h_org[t] = make_float2(dx*x0, dy*y0);
+		}
 	}
 	if (!sine) {TW_CUDA(ctx, cudaMemcpyAsync(d_org, h_org, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));}
 	if (ctx_org) {
@@ -652,15 +663,18 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	const float2 *d_gen_org = d_org, *d_gen_corg = d_corg;
 	const unsigned *d_perm = nullptr;
 	if (reorder) { // (1) + (2): coarse estimate, heaviest-first order of the WHOLE batch
-		tw_grid2d gcs = g; gcs.dx = dx*(float)cstep; gcs.dy = dy*(float)cstep; gcs.nx = CS; gcs.ny = CS;
-		for (uint32_t t0 = 0; t0 < ntiles; t0 += 65535) {
-			uint32_t const nt = (ntiles - t0 < 65535) ? ntiles - t0 : 65535;
-			rc = twi_heightgen(ctx, &gcs, p, 1, 0, d_org + t0, nt, d_coarse + (size_t)t0*CS*CS, nullptr); if (rc) return rc;
+		if (hs) {rc = twi_hmap_sample_tiles(ctx, ctx->d_hmap, hs, d_org, ntiles, CS, d_coarse, ctx->stream, nullptr, cstep); if (rc) return rc;}
+		else {
+			tw_grid2d gcs = g; gcs.dx = dx*(float)cstep; gcs.dy = dy*(float)cstep; gcs.nx = CS; gcs.ny = CS;
+			for (uint32_t t0 = 0; t0 < ntiles; t0 += 65535) {
+				uint32_t const nt = (ntiles - t0 < 65535) ? ntiles - t0 : 65535;
+				rc = twi_heightgen(ctx, &gcs, p, 1, 0, d_org + t0, nt, d_coarse + (size_t)t0*CS*CS, nullptr); if (rc) return rc;
+			}
 		}
 		rc = twi_coarse_work(ctx, d_coarse, CS*CS, ntiles, ep->water_plane_z - ep->half_dxy, d_work); if (rc) return rc;
 		TW_CUDA(ctx, cudaMemsetAsync(d_hist, 0, 1024, ctx->stream));
 		rc = twi_order_by_work(ctx, ctx->stream, d_work, ntiles, CS*CS, d_hist, d_order); if (rc) return rc;
-		rc = twi_gather_origins(ctx, d_org, d_order, ntiles, d_org_sorted); if (rc) return rc;
+		if (!hs) {rc = twi_gather_origins(ctx, d_org, d_order, ntiles, d_org_sorted); if (rc) return rc;} // the sampler reads its origins through the permutation
 		if (ctx_org) {rc = twi_gather_origins(ctx, d_corg, d_order, ntiles, d_corg_sorted); if (rc) return rc; d_gen_corg = d_corg_sorted;}
 		d_gen_org = d_org_sorted; d_perm = d_order;
 	}
@@ -694,6 +708,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 			status = twi_heightgen(ctx, &gc, p, 1, 0, d_gen_corg + t0, nt, d_cz, nullptr); if (status) break;
 			status = twi_tile_cut(ctx, ctx->stream, d_cz, nt, zvsize, maps, perm_k); if (status) break;
 		}
+		else if (hs) {status = twi_hmap_sample_tiles(ctx, ctx->d_hmap, hs, d_perm ? (const void *)d_org : (const void *)(d_org + t0), nt, zvsize, maps, ctx->stream, perm_k); if (status) break;}
 		else if (!sine) {
 			ctx->tile_perm = perm_k;
 			status = twi_heightgen(ctx, &g, p, 1, 0, d_gen_org + t0, nt, maps, nullptr);           // generation on ctx->stream
@@ -777,7 +792,37 @@ int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy, uint3
 	int rc = check_ctx(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
 	ctx->last_erosion_steps = 0;
-	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, shadows);
+	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, shadows, nullptr);
+}
+
+int tw_set_heightmap(tw_ctx *ctx, const uint8_t *data16, int width, int height) {
+	int rc = check_ctx(ctx); if (rc) return rc;
+	rc = finish_pending(ctx); if (rc) return rc;
+	if (data16 && (width <= 0 || height <= 0)) return tw_set_error(ctx, TW_ERR_ARG, "heightmap size %d x %d", width, height);
+	size_t const bytes = (size_t)2*width*height, had = (size_t)2*ctx->hmap_w*ctx->hmap_h;
+	if (ctx->d_hmap && (!data16 || bytes != had)) {TW_CUDA(ctx, cudaFree(ctx->d_hmap)); ctx->d_hmap = nullptr;}
+	ctx->hmap_w = ctx->hmap_h = 0;
+	if (!data16) return TW_OK;
+	if (!ctx->d_hmap) {TW_CUDA(ctx, cudaMalloc(&ctx->d_hmap, bytes));}
+	TW_CUDA(ctx, cudaMemcpyAsync(ctx->d_hmap, data16, bytes, cudaMemcpyDefault, ctx->stream));
+	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // data16 is the caller's buffer
+	ctx->hmap_w = width; ctx->hmap_h = height;
+	return TW_OK;
+}
+
+int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                                uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                                float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows)
+{
+	int rc = check_ctx(ctx); if (rc) return rc;
+	rc = finish_pending(ctx); if (rc) return rc;
+	if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_heightmap() has not been called");
+	if (!hs) return tw_set_error(ctx, TW_ERR_ARG, "null heightmap sampler");
+	if (hs->width != ctx->hmap_w || hs->height != ctx->hmap_h) return tw_set_error(ctx, TW_ERR_ARG, "sampler size %d x %d differs from the heightmap's %d x %d", hs->width, hs->height, ctx->hmap_w, ctx->hmap_h);
+	if (hs->edge_mode < 0 || hs->edge_mode > 2) return tw_set_error(ctx, TW_ERR_ARG, "bad edge_mode %d", hs->edge_mode);
+	if (shading && shading->ao) return tw_set_error(ctx, TW_ERR_ARG, "the AO map is not available for heightmap tiles (its context outside the tile is not defined in this mode)");
+	ctx->last_erosion_steps = 0;
+	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, shadows, hs);
 }
 
 int tw_create_tiles_launch_ex(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,

@@ -49,6 +49,9 @@ struct tw_ctx {
 	// growable device scratch
 	void  *d_scratch[3] = {nullptr, nullptr, nullptr}; // 0: generic output staging, 1: tables / padded heightmaps, 2: small (minmax, counters, origins)
 	size_t scratch_bytes[3] = {0, 0, 0};
+	// tw_set_heightmap's 16-bit image (its own allocation: tw_reserve may re-allocate the scratch slots while a tile job still reads the image)
+	uint8_t *d_hmap = nullptr;
+	int hmap_w = 0, hmap_h = 0;
 	// pinned host staging for small results
 	void  *h_pinned = nullptr;
 	size_t pinned_bytes = 0;
@@ -126,7 +129,9 @@ int twi_sine_tiles_grid(tw_ctx *ctx, const twi_sine_batch *b, uint32_t t0, uint3
 int twi_ensure_aux_streams(tw_ctx *ctx);
 int twi_erode(tw_ctx *ctx, float *d_maps, uint32_t ntiles, int xsize, int ysize, const float *d_min_zvals, float min_zval_all,
               uint32_t num_iters, const tw_erosion_params *p);
-int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const void *d_origins, uint32_t ntiles, uint32_t zvsize, float *d_out);
+// st: nullptr = ctx->stream; d_perm (optional): launch tile z handles tile d_perm[z] of d_origins and d_out; cstep: tile cell (i, j) samples (x1 + i*cstep, y1 + j*cstep)
+int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const void *d_origins, uint32_t ntiles, uint32_t zvsize, float *d_out,
+                          cudaStream_t st = nullptr, const unsigned *d_perm = nullptr, uint32_t cstep = 1);
 // d_perm (optional): launch tile z handles tile d_perm[z] of d_zvals and of the outputs (the tile pipeline's schedule order)
 int twi_tile_normals(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float dx_val, float dy_val, unsigned char *d_rgba, unsigned *d_min_nz_ord,
                      const unsigned *d_perm = nullptr);

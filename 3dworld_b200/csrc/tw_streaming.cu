@@ -89,11 +89,13 @@ __device__ __forceinline__ float hmap_raw_height(const uint8_t *__restrict__ d, 
 }
 
 __global__ void __launch_bounds__(256)
-hmap_sample_tiles_kernel(const uint8_t *__restrict__ data16, tw_hmap_sampler H, const int2 *__restrict__ origins, unsigned zvsize, float *__restrict__ out) {
-	unsigned const tile = blockIdx.y, i = blockIdx.x*blockDim.x + threadIdx.x;
+hmap_sample_tiles_kernel(const uint8_t *__restrict__ data16, tw_hmap_sampler H, const int2 *__restrict__ origins, unsigned zvsize, float *__restrict__ out,
+                         const unsigned *__restrict__ perm, int cstep) {
+	unsigned const i = blockIdx.x*blockDim.x + threadIdx.x;
 	if (i >= zvsize*zvsize) return;
+	unsigned const tile = perm ? __ldg(perm + blockIdx.y) : blockIdx.y;
 	int2 const o = __ldg(origins + tile);
-	int x = o.x + (int)(i % zvsize), y = o.y + (int)(i / zvsize);
+	int x = o.x + cstep*(int)(i % zvsize), y = o.y + cstep*(int)(i / zvsize);
 	float z;
 	if (H.mesh_scale < 1.0f) { // interpolate_height(float(x), float(y)), src/heightmap.cpp:394-402
 		float const sx = H.mesh_scale*(float)x, sy = H.mesh_scale*(float)y;
@@ -115,8 +117,15 @@ hmap_sample_tiles_kernel(const uint8_t *__restrict__ data16, tw_hmap_sampler H, 
 }
 } // namespace
 
-int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const void *d_origins, uint32_t ntiles, uint32_t zvsize, float *d_out) {
-	hmap_sample_tiles_kernel<<<dim3((zvsize*zvsize + 255)/256, ntiles), 256, 0, ctx->stream>>>(d_data16, *hs, (const int2 *)d_origins, zvsize, d_out);
-	TW_LAUNCH_CHECK(ctx);
+int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const void *d_origins, uint32_t ntiles, uint32_t zvsize, float *d_out,
+                          cudaStream_t st, const unsigned *d_perm, uint32_t cstep) {
+	size_t const tile_elems = (size_t)zvsize*zvsize;
+	for (uint32_t t0 = 0; t0 < ntiles; t0 += 65535) { // gridDim.y limit
+		uint32_t const nt = (ntiles - t0 < 65535) ? ntiles - t0 : 65535;
+		const int2 *org = (const int2 *)d_origins + (d_perm ? 0 : t0);
+		float *out = d_out + (d_perm ? 0 : (size_t)t0*tile_elems);
+		hmap_sample_tiles_kernel<<<dim3((zvsize*zvsize + 255)/256, nt), 256, 0, st ? st : ctx->stream>>>(d_data16, *hs, org, zvsize, out, d_perm ? d_perm + t0 : nullptr, (int)cstep);
+		TW_LAUNCH_CHECK(ctx);
+	}
 	return TW_OK;
 }

@@ -6,6 +6,7 @@
 //   tw3d::create_procedural      <->  voxel_manager::create_procedural               src/voxels.h:196, src/voxels.cpp:278-346
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
+//   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //
 // The reference reads ~20 globals on this path (SURVEY.md 8b); here they are one explicit struct (scene_globals) set once per scene
 // with set_globals(). Same names, argument meaning and error behaviour as the reference: argument errors assert/abort like the
@@ -67,6 +68,7 @@ namespace detail {
 	struct tls_ctx {
 		tw_ctx *c = nullptr; unsigned generation = ~0u;
 		std::atomic<uint64_t> tile_jobs{0}; // create_tiles_async launches on c: a job whose number is no longer the latest was completed by the next launch
+		int hmap_w = 0, hmap_h = 0;         // size of the image set_heightmap gave c
 		~tls_ctx() {if (c) tw_destroy(c);}
 	};
 	inline tls_ctx &tls() {static thread_local tls_ctx t; return t;}
@@ -326,15 +328,43 @@ inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, 
 
 // heightmap-texture mode of tile_t::create_zvals (src/tiled_mesh.cpp:498-501): zvals[y*zvsize + x] = terrain_hmap_manager.get_clamped_height(x1 + x, y1 + y)
 // for a batch of tiles, from the 16-bit image hmap16 (width*height*2 bytes, the layout heightmap_t keeps); TEX_EDGE_MODE 2 = mirror as compiled in the reference
-inline void create_zvals_from_heightmap(const uint8_t *hmap16, int width, int height, const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float *zvals_out, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+inline tw_hmap_sampler hmap_sampler(int width, int height, int tex_edge_mode) {
 	scene_globals const &g = globals();
 	tw_hmap_sampler hs;
 	hs.width = width; hs.height = height; hs.edge_mode = tex_edge_mode; hs.mesh_scale = g.mesh_scale;
 	hs.h_scale = 0.0008f*g.mesh_height_scale; // READ_MESH_H_SCALE*mesh_height_scale (src/mesh_gen.cpp:22,120)
 	hs.mesh_file_scale = g.mesh_file_scale; hs.mesh_file_tz = g.mesh_file_tz; hs.mesh_scale_z_inv = g.mesh_scale_z_inv;
+	return hs;
+}
+inline void create_zvals_from_heightmap(const uint8_t *hmap16, int width, int height, const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float *zvals_out, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	tw_hmap_sampler const hs = hmap_sampler(width, height, tex_edge_mode);
 	tw_ctx *c = ctx();
 	int const rc = tw_heightmap_sample_tiles(c, hmap16, &hs, origins_xy, ntiles, zvsize, zvals_out);
 	if (rc != TW_OK) {detail::fail(rc, "create_zvals_from_heightmap", c);}
+}
+// The same heightmap mode as a frame's asynchronous tile job: set_heightmap() keeps the image on this thread's device once (host or device hmap16, as above;
+// call it again when the map changes), and create_tiles_async_from_heightmap() is create_tiles_async() with zvals = create_zvals_from_heightmap()'s.
+// erosion_iters_tt: whether heightmap tiles are eroded is the engine's choice (0 = not). shading.ao is refused (tw_create_tiles_launch_hmap in tw3d.h).
+inline void set_heightmap(const uint8_t *hmap16, int width, int height) {
+	tw_ctx *c = ctx();
+	int const rc = tw_set_heightmap(c, hmap16, width, height);
+	if (rc != TW_OK) {detail::fail(rc, "set_heightmap", c);}
+	detail::tls().hmap_w = hmap16 ? width : 0; detail::tls().hmap_h = hmap16 ? height : 0;
+}
+inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max,
+                                                   unsigned size, tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows,
+                                                   int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	scene_globals const &g = globals();
+	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape); // the weights' jitter noise
+	tw_erosion_params const e = erosion_params_from_globals();
+	tw_ctx *c = ctx();
+	tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
+	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+	uint64_t const number = ++jobs;
+	int const rc = tw_create_tiles_launch_hmap(c, &hs, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out,
+	                                           &shading, shadows.nlights ? &shadows : nullptr);
+	if (rc != TW_OK) {detail::fail(rc, "create_tiles_async_from_heightmap", c);}
+	return tiles_job(c, &jobs, number);
 }
 
 // tile_t::upload_normal_texture (src/tiled_mesh.cpp:865-880, minus the GL upload) and tile_t::calc_mesh_ao_lighting (:586-662) for a batch of

@@ -355,6 +355,10 @@ typedef struct tw_hmap_sampler {
 #define TW_HMAP_EDGE_MIRROR 2
 TW_API int tw_heightmap_sample_tiles(tw_ctx *ctx, const uint8_t *data16, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles,
                               uint32_t zvsize, float *out);
+/* The context's heightmap image for tw_create_tiles_launch_hmap: copies data16 (2*width*height bytes in the layout of tw_heightmap_from_floats_u16, host or
+ * device) into device memory the context owns, so a frame's tiles do not upload the image again. Completes a pending job first. data16 == NULL releases the
+ * image; width or height <= 0 with an image is TW_ERR_ARG. Changing the map (brushes, a new file) means calling it again; tw_destroy frees the image. */
+TW_API int tw_set_heightmap(tw_ctx *ctx, const uint8_t *data16, int width, int height);
 /* min/max over a float array (get_heightmap_z_range, src/map_view.cpp:399-407) */
 TW_API int tw_minmax_f32(tw_ctx *ctx, const float *vals, size_t n, tw_minmax *mm);
 
@@ -449,6 +453,21 @@ typedef struct tw_tile_shadows {
 } tw_tile_shadows;
 TW_API int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
                           uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                          float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows);
+/* The asynchronous tile job (tw_create_tiles_launch_shadows, above) with heights from the context's heightmap image instead of the height function: tile t's
+ * zvals are get_clamped_height(x1 + x, y1 + y) of the image under hs - exactly what tw_heightmap_sample_tiles returns for the same origins. Everything after
+ * that is the job's: erosion when erosion_iters > 0 && erode_amount > 0, per-tile z range, bounds, normal map and min_normal_z, the weights texture with
+ * has_any_grass, and the per-light mesh shadows with sh_in. Every output is bit-identical to tw_heightmap_sample_tiles, then tw_erode_tiles(min_zval_all =
+ * min_zval) when eroding, then tw_tile_bounds_batch(wpz_max, dx, dy, size), tw_tile_normals_batch(dx, dy), tw_tile_weights_batch(origins, mesh size, dx, dy, p,
+ * wp, tile_params) and tw_tile_shadows_batch_ex per light; tw_last_erosion_steps() after the completing poll equals its value after that tw_erode_tiles.
+ * Whether heightmap tiles are eroded is the caller's choice (erosion_iters_tt or 0): this library does not pin the reference's (its test harness cannot reach the heightmap branch of create_zvals, see
+ * oracle/refbuild/ref_tiled_harness.inc). tw_create_tiles_poll
+ * completes the job; the image must not be replaced before then (tw_set_heightmap completes the job first). p is read only by the weights' jitter noise and
+ * may be NULL without weights. No tile limit. Not done: the AO map (calc_mesh_ao_lighting reads a (stride + 72)^2 context around the tile, and what the
+ * reference reads outside the tile in this mode is not pinned here). Errors, nothing enqueued: TW_ERR_STATE without tw_set_heightmap; TW_ERR_ARG for hs NULL
+ * or sized unlike the image, edge_mode outside 0..2, shading->ao, weights without p, and every error of tw_create_tiles_launch_shadows. */
+TW_API int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size,
+                          float dx, float dy, uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
                           float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows);
 
 /* ---- terrain weights texture of tiles (SURVEY.md 8f row N4): tile_t::create_texture (src/tiled_mesh.cpp:1071-1248), the terrain part ----

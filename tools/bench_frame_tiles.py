@@ -4,8 +4,11 @@ tw_tile_normals_batch), alternated in one process. Default: 16 tiles of 130^2, B
 sub-block bounds + normal map into pinned host memory; medians over --reps rounds after 3 warm-up rounds. --ao adds the AO map (the synchronous side
 then calls tw_create_zvals_ao_batch instead of tw_create_zvals_batch), --weights the terrain weights texture and has_any_grass (tw_tile_weights_batch):
 the asynchronous job is then tw_create_tiles_launch_ex. --shadows adds the mesh shadows of two lights (sun and moon, masks and outgoing edges into pinned
-memory) through tw_create_tiles_launch_shadows; the synchronous side then also calls tw_tile_shadows_batch once per light on the zvals it made. Prints one
-JSON line with the GPU's name and power limit; writes nothing."""
+memory) through tw_create_tiles_launch_shadows; the synchronous side then also calls tw_tile_shadows_batch once per light on the zvals it made. --hmap takes
+the heights from a 7168^2 terrain image built with tw_proc_gen_heightmap and kept in host memory, as an engine keeps a loaded heightmap: the job is
+tw_create_tiles_launch_hmap on the image tw_set_heightmap uploaded once (its time is reported), the synchronous side the chain an engine uses without it,
+tw_heightmap_sample_tiles on the host image (which uploads the whole image every call) and tw_erode_tiles, then the same tail. Prints one JSON line with the
+GPU's name and power limit; writes nothing."""
 import argparse
 import importlib
 import json
@@ -30,7 +33,10 @@ ap.add_argument("--reps", type=int, default=20)
 ap.add_argument("--ao", action="store_true")
 ap.add_argument("--weights", action="store_true")
 ap.add_argument("--shadows", action="store_true")
+ap.add_argument("--hmap", action="store_true")
 a = ap.parse_args()
+if a.hmap and a.ao:
+    ap.error("--hmap: the tile job makes no AO map for heightmap tiles")
 
 nt, zv, iters, size = a.tiles, a.zvsize, a.droplets, a.zvsize - 2
 ctx = tw.Context(0)
@@ -67,6 +73,16 @@ if a.shadows:
         sp.lpos[0], sp.lpos[1], sp.lpos[2] = lp
         lights.append(tw.Light(sp, torch.empty((nt, zv, zv), dtype=torch.uint8).pin_memory(), torch.empty((nt, zv)).pin_memory(), torch.empty((nt, zv)).pin_memory()))
     shading.update(lights=lights)
+hmap, img, upload_ms = None, None, None
+if a.hmap:
+    N = 7168
+    img, info, _ = ctx.proc_gen_heightmap(N, N, dx, dy, hp, 0, ep)
+    img = img.reshape(N, N, 2)
+    hmap = tw.HmapSampler(N, N, 2, 1.0, float(np.float32(0.0008) * np.float32(hp.mesh_height_scale)), info.mesh_file_scale, info.mesh_file_tz, hp.mesh_scale_z_inv)
+    t0 = time.perf_counter()
+    ctx.set_heightmap(img)
+    upload_ms = 1e3 * (time.perf_counter() - t0)
+    shading.update(hmap=hmap)
 launch_ms, ready_ms, sync_ms = [], [], []
 for r in range(a.reps + 3):
     origins = [((r * 5 + t % 4) * size, (t // 4 + r) * size) for t in range(nt)]   # new tiles every frame
@@ -77,7 +93,12 @@ for r in range(a.reps + 3):
     while not ctx.create_tiles_poll(wait=False):
         pass
     t2 = time.perf_counter()
-    if a.ao:
+    if a.hmap:
+        ctx.heightmap_sample_tiles(img, hmap, origins, zv, out=z)
+        ctx.erode_tiles(z, iters, ep, min_zval_all=ep.zmin)
+        zn = z.numpy().reshape(nt, -1)
+        mm[:, 0], mm[:, 1] = zn.min(1), zn.max(1)
+    elif a.ao:
         ctx.create_zvals_ao_batch(origins, cfg.mesh_size, dx, dy, zv, hp, iters, ep, ep.zmin, hd, out=z, ao=ao, want_minmax=True)
     else:
         ctx.create_zvals_batch(origins, cfg.mesh_size, dx, dy, zv, hp, iters, ep, ep.zmin, out=z, want_minmax=True)
@@ -98,6 +119,10 @@ try:
 except Exception:   # noqa: BLE001 - descriptive only
     name, plim = None, None
 extra = "".join(s for s, on in ((" + AO map", a.ao), (" + weights texture", a.weights), (" + mesh shadows of 2 lights", a.shadows)) if on)
-print(json.dumps({"workload": "%d tiles of %d^2, mode 4 8-octave + %d droplets per tile, z range + bounds + normal map%s, pinned host outputs" % (nt, zv, iters, extra),
-                  "launch_host_ms": float(np.median(launch_ms)), "launch_host_ms_max": max(launch_ms), "launch_to_ready_ms": float(np.median(ready_ms)),
-                  ("sync_calls_ms" if extra else "sync_three_calls_ms"): float(np.median(sync_ms)), "rounds": a.reps, "gpu": name, "power_limit_w": plim}))
+src = "heights from a 7168^2 host heightmap image (mode 4 8-octave terrain)" if a.hmap else "mode 4 8-octave"
+res = {"workload": "%d tiles of %d^2, %s + %d droplets per tile, z range + bounds + normal map%s, pinned host outputs" % (nt, zv, src, iters, extra),
+       "launch_host_ms": float(np.median(launch_ms)), "launch_host_ms_max": max(launch_ms), "launch_to_ready_ms": float(np.median(ready_ms)),
+       ("sync_calls_ms" if extra or a.hmap else "sync_three_calls_ms"): float(np.median(sync_ms)), "rounds": a.reps, "gpu": name, "power_limit_w": plim}
+if a.hmap:
+    res["set_heightmap_once_ms"] = upload_ms
+print(json.dumps(res))

@@ -140,18 +140,28 @@ __device__ __forceinline__ float4 simplex_lut_entry(float k) { // scalar restate
 constexpr unsigned SIMPLEX_LUT_MAGIC_BITS = 0x4B400000u; // bits of 12582912.0f = 1.5*2^23
 constexpr unsigned LUT_ENTRY_BYTES = 16u*SIMPLEX_LUT_COPIES;
 
-// Simplex hash table (level 3 with the denormal addressing): SIMPLEX_HASH_N entries staged right behind the gradient table, in the same 8-copy
-// layout, entry k = {permute(k), permute(k) + 1, permute(k + 1) + 1, 0}. The three second-permute arguments of a cell then cost one add each:
-//   p0 = q0 + ix = [iy].x + ix,   p2 = (q2 + ix) + 1 = [iy].z + ix,
-//   p1 = (q1 + ix) + i1.x = [iy].y + ix (i1.y = 0) or [iy + 1].x + ix (i1.y = 1): the word at entry iy's address + 4 + 124*i1.y.
-// Exact: every operand is an integer below 2^24, so any order of the adds gives the same value. iy comes from mod_int289_lazy (<= 289), so entries
-// up to 290 are read; entry 290 needs permute(291), which the float arithmetic of permute() evaluates exactly (= permute(2)).
+// Simplex hash table (level 3 with the denormal addressing): SIMPLEX_HASH_N entries staged right behind the 8 copies of the gradient table. Its
+// entries are the second-permute arguments already turned into gradient-table byte offsets: with P = permute and B(v) = the float whose bit
+// pattern is the integer v (a denormal, v*2^-149),
+//   entry k = {B(128*P(k)), B(128*(P(k) + 1)), B(128*(P(k + 1) + 1)), 0}.
+// With bx = lut_offsets(ix) (bits 128*ix + Lb), the three gradient addresses of a cell are one add each:
+//   k0 = [iy].x + bx = lut_offsets(P(iy) + ix)              (p0 = q0 + ix)
+//   k2 = [iy].z + bx = lut_offsets(P(iy + 1) + ix + 1)      (p2 = q2 + ix + 1)
+//   k1 = [iy].y + bx (i1.y = 0) or [iy + 1].x + bx (i1.y = 1) = lut_offsets(P(iy + i1.y) + ix + i1.x)   (p1 = q1 + ix + i1.x, i1.x = 1 - i1.y):
+//        the word at entry iy's address + 4 + (pitch - 4)*i1.y.
+// Exact, bit for bit: every operand is a non-negative integer multiple of 2^-149 below 2^23*2^-149, where float adds are exact (denormals are
+// fixed point; nothing here is compiled with -ftz). ix, iy come from mod_int289_lazy (<= 289) and P <= 288, so the largest offset is
+// 128*578 + Lb < 2^19. Entries up to 290 are read; entry 290 needs permute(291), which the float arithmetic of permute() evaluates exactly
+// (= permute(2)). Against the hash values of the table's earlier form this saves the three address FMAs of lut_offsets per cell for one (bx).
 #define TW_SIMPLEX_HASH_TABLE (TW_SIMPLEX_LUT >= 3 && TW_LUT_DENORM && !TW_HASH_Q1_ARITH)
 constexpr int SIMPLEX_HASH_N = TW_SIMPLEX_HASH_TABLE ? 291 : 0;
-constexpr unsigned SIMPLEX_HASH_OFFSET = SIMPLEX_LUT_N*LUT_ENTRY_BYTES; // byte distance from entry k of the gradient table to entry k of the hash table
+// The hash table is ONE copy (16-byte pitch), not 8 interleaved ones like the gradient table: the lattice row iy is nearly uniform across a warp, so
+// its look-ups mostly broadcast, and the block stages 4.6 KB instead of 37 KB (headline 0.7 % faster than 8 copies, results/h100/octave_body.txt).
+constexpr int SIMPLEX_HASH_COPIES = 1;
+constexpr unsigned SIMPLEX_HASH_OFFSET = SIMPLEX_LUT_N*LUT_ENTRY_BYTES; // byte distance from the start of the gradient table to the hash table
 __device__ __forceinline__ float4 simplex_hash_entry(float k) {
-	float const pk = twn::permute(k);
-	return make_float4(pk, pk + 1.0f, twn::permute(k + 1.0f) + 1.0f, 0.0f);
+	unsigned const p0 = (unsigned)twn::permute(k), p1 = (unsigned)twn::permute(k + 1.0f);
+	return make_float4(__uint_as_float(LUT_ENTRY_BYTES*p0), __uint_as_float(LUT_ENTRY_BYTES*(p0 + 1)), __uint_as_float(LUT_ENTRY_BYTES*(p1 + 1)), 0.0f);
 }
 __device__ __forceinline__ unsigned simplex_lut_base(const float4 *lut_s, unsigned lane) {
 	unsigned const a = (unsigned)__cvta_generic_to_shared(lut_s) + (lane & (SIMPLEX_LUT_COPIES - 1))*16u;
@@ -181,15 +191,17 @@ template<unsigned OFF> __device__ __forceinline__ float lut_load_f32(unsigned ad
 	return v;
 }
 
-// arguments of the second permute for two cells from the simplex hash table (ix, iy: lattice indices after mod_int289_lazy)
-__device__ __forceinline__ void simplex_hash_args(f2 ix, f2 iy, f2 i1y, unsigned Lb, f2 &p0, f2 &p1, f2 &p2) {
-	constexpr unsigned H = SIMPLEX_HASH_OFFSET;
-	f2 const j0 = lut_offsets(iy, Lb); // address of entry iy of the gradient table; + H: of the hash table
-	f2 const j1 = raw_fma(i1y, splat(__uint_as_float(LUT_ENTRY_BYTES - 4)), j0); // + 124 bytes when i1.y = 1 (see simplex_hash_entry)
+// gradient-table offsets of the three corners of two cells from the simplex hash table (ix, iy: lattice indices after mod_int289_lazy)
+__device__ __forceinline__ void simplex_hash_offsets(f2 ix, f2 iy, f2 i1y, unsigned Lb, f2 &k0, f2 &k1, f2 &k2) {
+	constexpr unsigned H = SIMPLEX_HASH_OFFSET, PITCH = 16u*SIMPLEX_HASH_COPIES;
+	unsigned const base = Lb - (threadIdx.x & (SIMPLEX_LUT_COPIES - 1))*16u; // Lb without the lane's copy offset: the hash table's one copy
+	f2 const j0 = raw_fma(iy, splat(__uint_as_float(PITCH)), splat(__uint_as_float(base))); // address of entry iy of the hash table, less H (exact, as lut_offsets)
+	f2 const j1 = raw_fma(i1y, splat(__uint_as_float(PITCH - 4)), j0);                       // + pitch - 4 bytes when i1.y = 1 (see simplex_hash_entry)
 	unsigned const ja = __float_as_uint(j0.x), jb = __float_as_uint(j0.y), j1a = __float_as_uint(j1.x), j1b = __float_as_uint(j1.y);
-	p0 = add2(make_float2(lut_load_f32<H>(ja), lut_load_f32<H>(jb)), ix);
-	p1 = add2(make_float2(lut_load_f32<H + 4>(j1a), lut_load_f32<H + 4>(j1b)), ix);
-	p2 = add2(make_float2(lut_load_f32<H + 8>(ja), lut_load_f32<H + 8>(jb)), ix);
+	f2 const bx = lut_offsets(ix, Lb);
+	k0 = add2(make_float2(lut_load_f32<H>(ja), lut_load_f32<H>(jb)), bx);
+	k1 = add2(make_float2(lut_load_f32<H + 4>(j1a), lut_load_f32<H + 4>(j1b)), bx);
+	k2 = add2(make_float2(lut_load_f32<H + 8>(ja), lut_load_f32<H + 8>(jb)), bx);
 }
 
 // glm::simplex(vec2) for two positions with the table; Lb = simplex_lut_base(); HASH: the block staged the simplex hash table too
@@ -204,9 +216,10 @@ __device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
 	f2 const i1x = make_float2((x0x.x > x0y.x) ? 1.0f : 0.0f, (x0x.y > x0y.y) ? 1.0f : 0.0f);
 	f2 const i1y = rsub2(1.0f, i1x); // (1,0) or (0,1)
 	f2 const x12x = sub2(add2(x0x, Cx), i1x), x12y = sub2(add2(x0y, Cx), i1y), x12z = add2(x0x, Cz), x12w = add2(x0y, Cz);
-	f2 p0, p1, p2;
-	if constexpr (HASH) {simplex_hash_args(mod_int289_lazy(ix), mod_int289_lazy(iy), i1y, Lb, p0, p1, p2);}
+	f2 k0, k1, k2;
+	if constexpr (HASH) {simplex_hash_offsets(mod_int289_lazy(ix), mod_int289_lazy(iy), i1y, Lb, k0, k1, k2);}
 	else {
+	f2 p0, p1, p2;
 #if TW_SIMPLEX_LUT >= 2
 	ix = mod_int289_lazy(ix); iy = mod_int289_lazy(iy);
 	// permute(iy), permute(iy + i1.y), permute(iy + 1): consecutive table entries, so the second and third addresses are the first plus 0/128/256 bytes
@@ -238,13 +251,13 @@ __device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
 #else
 	p0 = permute(add2(q0, ix)); p1 = permute(add2(add2(q1, ix), i1x)); p2 = permute(add2(add2(q2, ix), 1.0f));
 #endif
+	k0 = lut_offsets(p0, Lb); k1 = lut_offsets(p1, Lb); k2 = lut_offsets(p2, Lb);
 	}
 	f2 m0 = rsub_max0_2(0.5f, sumprod2(x0x, x0x, x0y, x0y));
 	f2 m1 = rsub_max0_2(0.5f, sumprod2(x12x, x12x, x12y, x12y));
 	f2 m2 = rsub_max0_2(0.5f, sumprod2(x12z, x12z, x12w, x12w));
 	m0 = mul2(m0, m0); m1 = mul2(m1, m1); m2 = mul2(m2, m2);
 	m0 = mul2(m0, m0); m1 = mul2(m1, m1); m2 = mul2(m2, m2);
-	f2 const k0 = lut_offsets(p0, Lb), k1 = lut_offsets(p1, Lb), k2 = lut_offsets(p2, Lb);
 	float4 const g0a = lut_load4(Lb, k0.x), g0b = lut_load4(Lb, k0.y), g1a = lut_load4(Lb, k1.x), g1b = lut_load4(Lb, k1.y), g2a = lut_load4(Lb, k2.x), g2b = lut_load4(Lb, k2.y);
 	// the table values arrive one cell per register quad (same IEEE operations; the file is compiled with -fmad=false)
 	m0 = make_float2(m0.x*g0a.z, m0.y*g0b.z); m1 = make_float2(m1.x*g1a.z, m1.y*g1b.z); m2 = make_float2(m2.x*g2a.z, m2.y*g2b.z);

@@ -130,7 +130,7 @@ def hmap_params(**kw):
 
 
 # every symbol include/tw3d.h declares (tests check the library exports exactly these)
-ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_destroy", "tw_last_error", "tw_sync", "tw_stream", "tw_launch_count",
+ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", "tw_last_error", "tw_sync", "tw_stream", "tw_launch_count",
                "tw_build_sin_table", "tw_compute_scale", "tw_gen_sine_params", "tw_gen_rx_ry", "tw_noise3d_gen_sines",
                "tw_water_z_height", "tw_set_sin_table", "tw_set_sine_params", "tw_heightgen_2d", "tw_heightgen_2d_launch",
                "tw_heightgen_2d_poll", "tw_heightgen_tiles", "tw_create_zvals_batch", "tw_create_tiles_launch", "tw_create_tiles_launch_ex", "tw_create_tiles_poll", "tw_tile_bounds_batch", "tw_tile_normals_batch", "tw_tile_ao_batch", "tw_create_zvals_ao_batch", "tw_glaciate_mesh", "tw_eval_points", "tw_erode", "tw_erode_parallel", "tw_erode_tiles", "tw_last_erosion_steps", "tw_voxel_fill",
@@ -147,6 +147,7 @@ def _load():
     L = C.CDLL(LIB_PATH)
     vp, fp = C.c_void_p, C.POINTER(C.c_float)
     L.tw_create.argtypes = [C.c_int, C.POINTER(vp)]
+    L.tw_create_shared.argtypes = [vp, C.POINTER(vp)]
     L.tw_destroy.argtypes = [vp]
     L.tw_destroy.restype = None
     L.tw_last_error.argtypes = [vp]
@@ -402,11 +403,27 @@ class Context:
             raise TwError(rc, "tw_create failed (no CUDA device? this library has no CPU fallback)")
         self._h = h
         self.device = device
+        self.parent, self._shared = None, []
         self._check(lib.tw_set_sin_table(self._h, _ptr(sin_table)))
+
+    def shared(self):
+        """tw_create_shared: a Context on this one's device that reads this one's tables (sin and direction tables, sine params, LUTs, the set_heightmap
+        image) and has its own stream, scratch and pending job, so its asynchronous job runs beside this context's and the other shared ones'. Tables are
+        set here only: on the shared Context the setters raise. It keeps a reference to this Context; close() here closes it first."""
+        h = C.c_void_p()
+        self._check(lib.tw_create_shared(self._h, C.byref(h)))
+        s = Context.__new__(Context)
+        s._h, s.device, s.parent, s._shared = h, self.device, self, []
+        self._shared.append(s)
+        return s
 
     def close(self):
         if getattr(self, "_h", None) and lib is not None:   # lib can already be gone at interpreter shutdown
+            for s in getattr(self, "_shared", ()):         # tw_destroy(parent) destroys them: their handles must not be destroyed again
+                s._h = None
             lib.tw_destroy(self._h)
+            if getattr(self, "parent", None) is not None and self in self.parent._shared:
+                self.parent._shared.remove(self)
         self._h = None
 
     def __del__(self):

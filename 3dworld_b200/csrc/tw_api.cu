@@ -58,10 +58,12 @@ namespace {
 // slot-2 layout (small device scalars)
 constexpr size_t OFF_MM = 0, OFF_BAD = 64, OFF_TILES = 4096;
 
-int check_ctx(tw_ctx *ctx) { // NOTE: makes ctx->device the calling thread's current CUDA device and leaves it so (documented in tw3d.h: one context per thread)
+int check_ctx(tw_ctx *ctx) { // NOTE: makes ctx->device the calling thread's current CUDA device and leaves it so (documented in tw3d.h: one context per thread);
+                             // a shared context takes its parent's current tables
 	if (!ctx) return TW_ERR_ARG;
 	cudaError_t e = cudaSetDevice(ctx->device);
 	if (e != cudaSuccess) return tw_set_error(ctx, TW_ERR_CUDA, "cudaSetDevice(%d): %s", ctx->device, cudaGetErrorString(e));
+	twi_borrow_tables(ctx);
 	return TW_OK;
 }
 
@@ -121,6 +123,28 @@ int finish_pending(tw_ctx *ctx) { // complete an outstanding tw_heightgen_2d_lau
 	return poll_job(ctx, 1);
 }
 
+// tw_set_sin_table / tw_set_sine_params / tw_set_heightmap: refused on a shared context; on a parent, the job of every shared context completes first,
+// because it may still read the tables about to be replaced
+int begin_table_change(tw_ctx *ctx) {
+	if (ctx->parent) return tw_set_error(ctx, TW_ERR_ARG, "tables are set on the parent context, not on a shared one");
+	for (tw_ctx *s : ctx->shared) {
+		int const rc = finish_pending(s);
+		if (rc) return tw_set_error(ctx, rc, "a shared context's job failed: %s", s->err);
+	}
+	return TW_OK;
+}
+
+// a context with its own stream and completion event on `device` (the caller has made it current)
+tw_ctx *new_ctx(int device) {
+	tw_ctx *ctx = new (std::nothrow) tw_ctx();
+	if (!ctx) return nullptr;
+	ctx->device = device;
+	{int sms = 0; if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && sms > 0) ctx->num_sms = (unsigned)sms; else cudaGetLastError();}
+	if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {delete ctx; cudaGetLastError(); return nullptr;}
+	if (cudaEventCreateWithFlags(&ctx->async.done, cudaEventDisableTiming) != cudaSuccess) {cudaStreamDestroy(ctx->stream); delete ctx; cudaGetLastError(); return nullptr;}
+	return ctx;
+}
+
 int read_minmax(tw_ctx *ctx, const unsigned *d_mm, tw_minmax *mm, uint32_t n) { // synchronous
 	int rc = tw_reserve_pinned(ctx, (size_t)n*2*sizeof(unsigned));
 	if (rc) return rc;
@@ -154,7 +178,17 @@ int validate_weights(tw_ctx *ctx, const tw_weight_params *wp, tw_weight_params &
 
 } // namespace
 
-int twi_finish_pending(tw_ctx *ctx) {return finish_pending(ctx);}
+int twi_finish_pending(tw_ctx *ctx) {twi_borrow_tables(ctx); return finish_pending(ctx);} // the entry points of the other translation units call it first
+
+void twi_borrow_tables(tw_ctx *ctx) {
+	tw_ctx const *p = ctx->parent;
+	if (!p) return;
+	ctx->d_sin_table = p->d_sin_table; ctx->d_dir_table = p->d_dir_table; ctx->have_sin = p->have_sin;
+	ctx->d_sine_params = p->d_sine_params; ctx->have_sine_params = p->have_sine_params;
+	memcpy(ctx->h_sine_params, p->h_sine_params, sizeof(ctx->h_sine_params));
+	ctx->d_simplex_lut = p->d_simplex_lut; ctx->d_glm3_lut = p->d_glm3_lut;
+	ctx->d_hmap = p->d_hmap; ctx->hmap_w = p->hmap_w; ctx->hmap_h = p->hmap_h;
+}
 
 extern "C" {
 
@@ -167,20 +201,42 @@ int tw_create(int device, tw_ctx **out) {
 	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {cudaGetLastError(); return TW_ERR_NO_DEVICE;}
 	if (device < 0 || device >= ndev) return TW_ERR_ARG;
 	if (cudaSetDevice(device) != cudaSuccess) {cudaGetLastError(); return TW_ERR_CUDA;}
-	tw_ctx *ctx = new (std::nothrow) tw_ctx();
+	tw_ctx *ctx = new_ctx(device);
 	if (!ctx) return TW_ERR_CUDA;
-	ctx->device = device;
-	{int sms = 0; if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && sms > 0) ctx->num_sms = (unsigned)sms; else cudaGetLastError();}
-	if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {delete ctx; cudaGetLastError(); return TW_ERR_CUDA;}
-	if (cudaEventCreateWithFlags(&ctx->async.done, cudaEventDisableTiming) != cudaSuccess) {cudaStreamDestroy(ctx->stream); delete ctx; cudaGetLastError(); return TW_ERR_CUDA;}
+	*out = ctx;
+	return TW_OK;
+}
+
+int tw_create_shared(tw_ctx *parent, tw_ctx **out) {
+	if (!out) return tw_set_error(parent, TW_ERR_ARG, "null out");
+	*out = nullptr;
+	if (!parent) return TW_ERR_ARG;
+	if (parent->parent) return tw_set_error(parent, TW_ERR_ARG, "a shared context cannot be the parent of another");
+	int rc = check_ctx(parent); if (rc) return rc;
+	// the parent's LUTs are built once, here: the shared context only ever reads them, on its own stream, once the parent's stream has passed them
+	rc = twi_ensure_simplex_lut(parent); if (rc) return rc;
+	rc = twi_ensure_glm3_lut(parent); if (rc) return rc;
+	TW_CUDA(parent, cudaStreamSynchronize(parent->stream));
+	tw_ctx *ctx = new_ctx(parent->device);
+	if (!ctx) return tw_set_error(parent, TW_ERR_CUDA, "tw_create_shared: no memory for the context, its stream or its event");
+	try {parent->shared.push_back(ctx);} catch (...) {tw_destroy(ctx); return tw_set_error(parent, TW_ERR_CUDA, "tw_create_shared: out of host memory");}
+	ctx->parent = parent;
+	twi_borrow_tables(ctx);
 	*out = ctx;
 	return TW_OK;
 }
 
 void tw_destroy(tw_ctx *ctx) {
 	if (!ctx) return;
+	while (!ctx->shared.empty()) tw_destroy(ctx->shared.back()); // each removes itself from the list
 	if (ctx->dist) tw_dist_finalize(ctx);
 	cudaSetDevice(ctx->device);
+	tw_ctx *const parent = ctx->parent;
+	if (parent) { // its job completes as a poll with wait = 1 would; the tables are the parent's
+		finish_pending(ctx);
+		parent->shared.erase(std::find(parent->shared.begin(), parent->shared.end(), ctx));
+		ctx->d_sin_table = nullptr; ctx->d_dir_table = nullptr; ctx->d_simplex_lut = nullptr; ctx->d_glm3_lut = nullptr; ctx->d_sine_params = nullptr; ctx->d_hmap = nullptr;
+	}
 	cudaStreamSynchronize(ctx->stream);
 	for (int i = 0; i < 3; ++i) {if (ctx->d_scratch[i]) cudaFree(ctx->d_scratch[i]);}
 	if (ctx->d_sin_table) cudaFree(ctx->d_sin_table);
@@ -214,6 +270,7 @@ int tw_sync(tw_ctx *ctx) {
 
 int tw_set_sin_table(tw_ctx *ctx, const float *tab) {
 	int rc = check_ctx(ctx); if (rc) return rc;
+	rc = begin_table_change(ctx); if (rc) return rc;
 	std::vector<float> built;
 	if (!tab) {built.resize(TW_SIN_TABLE_SIZE); tw_build_sin_table(built.data()); tab = built.data();}
 	if (!ctx->d_sin_table) {TW_CUDA(ctx, cudaMalloc(&ctx->d_sin_table, TW_SIN_TABLE_SIZE*sizeof(float)));}
@@ -233,6 +290,7 @@ int tw_set_sin_table(tw_ctx *ctx, const float *tab) {
 int tw_set_sine_params(tw_ctx *ctx, const float *sp) {
 	int rc = check_ctx(ctx); if (rc) return rc;
 	if (!sp) return tw_set_error(ctx, TW_ERR_ARG, "null sine_params");
+	rc = begin_table_change(ctx); if (rc) return rc;
 	if (!ctx->d_sine_params) {TW_CUDA(ctx, cudaMalloc(&ctx->d_sine_params, TW_F_TABLE_SIZE*5*sizeof(float)));}
 	memcpy(ctx->h_sine_params, sp, sizeof(ctx->h_sine_params));
 	TW_CUDA(ctx, cudaMemcpyAsync(ctx->d_sine_params, ctx->h_sine_params, sizeof(ctx->h_sine_params), cudaMemcpyHostToDevice, ctx->stream));
@@ -797,6 +855,7 @@ int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy, uint3
 
 int tw_set_heightmap(tw_ctx *ctx, const uint8_t *data16, int width, int height) {
 	int rc = check_ctx(ctx); if (rc) return rc;
+	rc = begin_table_change(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
 	if (data16 && (width <= 0 || height <= 0)) return tw_set_error(ctx, TW_ERR_ARG, "heightmap size %d x %d", width, height);
 	size_t const bytes = (size_t)2*width*height, had = (size_t)2*ctx->hmap_w*ctx->hmap_h;

@@ -396,7 +396,8 @@ __global__ void simplex_lut_kernel(float4 *__restrict__ lut) { // [0, N): simple
 	if (k < twn2::SIMPLEX_LUT_N) {lut[k] = twn2::simplex_lut_entry((float)k); lut[PERLIN_LUT_OFFSET + k] = twn2::perlin_lut_entry((float)k);}
 	if (k < twn2::SIMPLEX_HASH_N) {lut[twn2::SIMPLEX_LUT_N + k] = twn2::simplex_hash_entry((float)k);}
 }
-static int ensure_simplex_lut(tw_ctx *ctx) {
+} // namespace
+int twi_ensure_simplex_lut(tw_ctx *ctx) {
 	if (ctx->d_simplex_lut) return TW_OK;
 	static_assert(twn2::SIMPLEX_HASH_N <= twn2::SIMPLEX_LUT_N, "simplex_lut_kernel's grid covers the gradient tables");
 	TW_CUDA(ctx, cudaMalloc(&ctx->d_simplex_lut, (PERLIN_LUT_OFFSET + twn2::SIMPLEX_LUT_N)*sizeof(float4)));
@@ -404,6 +405,7 @@ static int ensure_simplex_lut(tw_ctx *ctx) {
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }
+namespace {
 
 // ------------------------------------------------------------------------------------------------ sine-table mode
 struct SineTabParams {
@@ -694,7 +696,7 @@ int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, in
 		bool simplex = false;
 		if (!make_noise_params(p, N, simplex)) return tw_set_error(ctx, TW_ERR_ARG, "start_eval_sin %d out of range", p->start_eval_sin);
 		bool const warp = (p->gen_mode == TW_MGEN_DWARP_GPU);
-		{int const rc = ensure_simplex_lut(ctx); if (rc) return rc;}
+		{int const rc = twi_ensure_simplex_lut(ctx); if (rc) return rc;}
 		const float4 *lut = (const float4 *)ctx->d_simplex_lut + (simplex ? 0 : PERLIN_LUT_OFFSET);
 		unsigned const band_rows = band_rows_for(ctx, ny, nx, h_out_bands != nullptr && ntiles == 1);
 		for (unsigned r0 = 0; r0 < ny; r0 += band_rows) {

@@ -5,6 +5,7 @@
 #include <stddef.h>
 #include <stdio.h>
 #include <string.h>
+#include <vector>
 #include "../../include/tw3d.h"
 
 // The one asynchronous job a context may have in flight (tw_heightgen_2d_launch or tw_create_tiles_launch). `done` is recorded on ctx->stream
@@ -58,10 +59,17 @@ struct tw_ctx {
 	tw_async_state async;
 	void *dist = nullptr;        // tw_dist_state (tw_multi.cu): NCCL communicator of the one-process-per-GPU mode
 	unsigned skip_rect[4] = {0, 0, 0, 0}; // x0, y0, w, h of the cells twi_heightgen's paired noise kernels leave unwritten (set around AO context generation only)
+	// tw_create_shared: a shared context's tables above (sin / direction tables, sine params, both LUTs, the heightmap image) are its parent's, copied
+	// from the parent at the start of every entry point (twi_borrow_tables) and never allocated, built or freed here
+	tw_ctx *parent = nullptr;
+	std::vector<tw_ctx *> shared; // the parent's live shared contexts
 };
 
 int  tw_set_error(tw_ctx *ctx, int status, const char *fmt, ...);
 int  twi_finish_pending(tw_ctx *ctx);                           // completes the context's pending asynchronous job (if any) before other work reuses its scratch
+void twi_borrow_tables(tw_ctx *ctx);                            // a shared context takes its parent's current tables (no-op on any other context)
+int  twi_ensure_simplex_lut(tw_ctx *ctx);                       // builds ctx->d_simplex_lut on ctx->stream if absent (tw_heightgen.cu)
+int  twi_ensure_glm3_lut(tw_ctx *ctx);                          // builds ctx->d_glm3_lut on ctx->stream if absent (tw_voxel.cu)
 int  tw_reserve(tw_ctx *ctx, int slot, size_t bytes);           // grow d_scratch[slot]; returns TW_OK / TW_ERR_CUDA
 int  tw_reserve_pinned(tw_ctx *ctx, size_t bytes);
 bool tw_is_device_ptr(const void *p);
@@ -115,7 +123,6 @@ size_t twi_sine_tiles_stage_bytes(uint32_t ntiles);
 // rows and returns the device memory the tables need; twi_sine_tiles_setup uploads the planned batch (staged in h_stage as above, or synchronously read from
 // h_org and b until the work is done) and builds the tables in d_mem (nullptr: scratch slot 1); twi_sine_tiles_grid generates batch tiles [t0, t0 + nt) -
 // or d_perm[t0 .. t0 + nt) - into consecutive slots of d_out. Setup and grid enqueue on ctx->stream.
-#include <vector>
 struct twi_sine_batch {
 	std::vector<float> uorg; std::vector<uint2> tabs; unsigned nux = 0, nuy = 0; // plan: distinct x then y origins, per-tile table indices
 	tw_grid2d g; tw_height_params p; int enable_glaciate, min_start_sin;

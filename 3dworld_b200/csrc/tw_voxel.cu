@@ -175,6 +175,14 @@ __global__ void glm3_lut_kernel(float4 *__restrict__ lut) { // [0, N): simplex(v
 
 } // namespace
 
+int twi_ensure_glm3_lut(tw_ctx *ctx) {
+	if (ctx->d_glm3_lut) return TW_OK;
+	TW_CUDA(ctx, cudaMalloc(&ctx->d_glm3_lut, 2*twn2::LUT3D_N*sizeof(float4)));
+	glm3_lut_kernel<<<(twn2::LUT3D_N + 127)/128, 128, 0, ctx->stream>>>((float4 *)ctx->d_glm3_lut);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
 int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out)
 {
 	unsigned const nx = vp->nx, ny = vp->ny, nz = vp->nz;
@@ -207,11 +215,7 @@ int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420
 	G.mag = vp->mag; G.nfreq0 = (float)(0.25*vp->freq);
 	G.rx = vp->rx; G.ry = vp->ry; G.rz = vp->rx - vp->ry;
 	G.octaves = vp->octaves; G.perlin = (vp->gen_mode == TW_MGEN_PERLIN);
-	if (!ctx->d_glm3_lut) {
-		TW_CUDA(ctx, cudaMalloc(&ctx->d_glm3_lut, 2*twn2::LUT3D_N*sizeof(float4)));
-		glm3_lut_kernel<<<(twn2::LUT3D_N + 127)/128, 128, 0, ctx->stream>>>((float4 *)ctx->d_glm3_lut);
-		TW_LAUNCH_CHECK(ctx);
-	}
+	{int const rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
 	unsigned const bz = (nz > 128) ? 256 : 128;
 	dim3 const grid((nz + bz - 1)/bz, (nx + VGX - 1)/VGX, ny);
 	size_t const lut_bytes = (size_t)twn2::LUT3D_N*twn2::SIMPLEX_LUT_COPIES*sizeof(float4);

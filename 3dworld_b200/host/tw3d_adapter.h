@@ -7,6 +7,7 @@
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
+//   tw3d::set_deferred_gens, tw3d::tile_job_pool  <->  several of them in flight at once, as tile_draw_t::update keeps up to 8   src/tiled_mesh.cpp:2367-2417
 //
 // The reference reads ~20 globals on this path (SURVEY.md 8b); here they are one explicit struct (scene_globals) set once per scene
 // with set_globals(). Same names, argument meaning and error behaviour as the reference: argument errors assert/abort like the
@@ -20,6 +21,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
@@ -63,12 +65,16 @@ namespace detail {
 		scene_globals g;
 		std::vector<float> sin_table, sine_params;
 		unsigned generation = 0; // bumped by set_globals WHEN IT IS GIVEN A TABLE, so that thread-local contexts re-upload the tables (scalars are read per call)
+		std::atomic<unsigned> deferred_gens{1}; // set_deferred_gens
 	};
 	inline state_t &state() {static state_t s; return s;}
 	struct tls_ctx {
 		tw_ctx *c = nullptr; unsigned generation = ~0u;
 		std::atomic<uint64_t> tile_jobs{0}; // create_tiles_async launches on c: a job whose number is no longer the latest was completed by the next launch
 		int hmap_w = 0, hmap_h = 0;         // size of the image set_heightmap gave c
+		std::vector<tw_ctx *> gens;         // shared contexts of c for deferred height generations (set_deferred_gens), destroyed with c
+		std::vector<uint64_t> gen_launch;   // launch order on each of them
+		uint64_t gen_clock = 0;
 		~tls_ctx() {if (c) tw_destroy(c);}
 	};
 	inline tls_ctx &tls() {static thread_local tls_ctx t; return t;}
@@ -101,6 +107,38 @@ inline void set_globals(scene_globals const &g, const float *sin_table = nullptr
 	if (sin_table || sinTable) {++s.generation;}
 }
 inline scene_globals const &globals() {return detail::state().g;}
+
+// How many asynchronous height generations (mesh_xy_grid_cache_t::build_arrays(..., no_wait=1) + enable_glaciate()) a thread keeps in flight at once;
+// tile_draw_t::update keeps up to 8 (src/tiled_mesh.cpp:2367-2417). n > 1: each thread launches them on up to n shared contexts of its ctx()
+// (tw_create_shared: the same tables, own streams and scratch), picking one with nothing in flight, else the one launched on longest ago, whose
+// generation that launch completes first. n = 1 (the default): every generation goes to ctx(), one in flight at a time. The contexts, once created,
+// live as long as the thread's ctx(). The grid is copied into the object's pageable host vector, which the launch waits for: the generations stay
+// independent of each other, but only the tile jobs of tile_job_pool (outputs in pinned memory) overlap on the device.
+inline void set_deferred_gens(unsigned n) {detail::state().deferred_gens = n ? n : 1;}
+
+namespace detail {
+	inline tw_ctx *gen_ctx() { // the context of the next asynchronous height generation
+		tw_ctx *c = ctx();
+		unsigned const n = state().deferred_gens;
+		if (n <= 1) return c;
+		tls_ctx &t = tls();
+		while (t.gens.size() < n) {
+			tw_ctx *s = nullptr;
+			int const rc = tw_create_shared(c, &s);
+			if (rc != TW_OK) {fail(rc, "set_deferred_gens: tw_create_shared", c);}
+			t.gens.push_back(s); t.gen_launch.push_back(0);
+		}
+		size_t pick = n;
+		for (size_t i = 0; i < n && pick == n; ++i) {
+			int const rc = tw_heightgen_2d_poll(t.gens[i], 0); // TW_OK: nothing in flight (a finished generation's host copy is already complete)
+			if (rc == TW_OK) {pick = i;}
+			else if (rc != TW_ERR_NOT_READY) {fail(rc, "build_arrays", t.gens[i]);}
+		}
+		if (pick == n) {pick = 0; for (size_t i = 1; i < n; ++i) {if (t.gen_launch[i] < t.gen_launch[pick]) pick = i;}}
+		t.gen_launch[pick] = ++t.gen_clock;
+		return t.gens[pick];
+	}
+}
 
 inline tw_height_params height_params_from_globals(int gen_mode, int gen_shape) {
 	scene_globals const &g = globals();
@@ -138,7 +176,7 @@ class mesh_xy_grid_cache_t {
 	void launch(bool glaciate, int min_start_sin, bool wait) const {
 		tw_height_params const p = height_params_from_globals(gen_mode, gen_shape);
 		vals.resize((size_t)grid.nx*grid.ny);
-		tw_ctx *c = ctx();
+		tw_ctx *c = wait ? ctx() : detail::gen_ctx();
 		int rc = tw_heightgen_2d_launch(c, &grid, &p, glaciate, min_start_sin, vals.data(), nullptr);
 		if (rc != TW_OK) {detail::fail(rc, "build_arrays", c);}
 		job_running = true; job_ctx = c; vals_glaciate = glaciate; vals_min_start = min_start_sin;
@@ -270,7 +308,7 @@ inline void create_zvals_batch(const int32_t *origins_xy, unsigned ntiles, unsig
 // create_tiles_async() enqueues heights, erosion and the tile tail (tile_bounds, normal map) and returns at once; call ready() on later frames and use the
 // outputs once it returns true (wait() blocks instead). The outputs named in `out` (tw_tile_outputs, include/tw3d.h) must stay valid until then; zvals and
 // normals_rgba may be device memory, or page-locked host memory for a launch that never blocks. One job per context: any other call on this thread's
-// context completes the job first. Not copyable; a handle that is destroyed while its job runs waits for it.
+// context completes the job first (tile_job_pool, below, keeps several in flight). Not copyable; a handle that is destroyed while its job runs waits for it.
 class tiles_job {
 	tw_ctx *c = nullptr;
 	std::atomic<uint64_t> const *latest = nullptr; // the launch count of c's thread
@@ -302,18 +340,26 @@ public:
 // The overload with `shadows` (tw_tile_shadows, include/tw3d.h) also computes every light's mesh shadows of the new tiles in the job, as calc_mesh_shadows (below) would
 // on the job's zvals: smask and sh_out_* must stay valid until the job is ready; tile_xy, the lights and host sh_in rows are copied during the launch. Build each
 // light's tw_shadow_params with shadow_params().
+namespace detail {
+	// the launch behind every create_tiles_async(_from_heightmap): on context c, whose launches jobs counts; hs = nullptr: heights from the height function
+	inline tiles_job launch_tiles(tw_ctx *c, std::atomic<uint64_t> &jobs, const tw_hmap_sampler *hs, const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy,
+	                              unsigned erosion_iters_tt, float wpz_max, unsigned size, tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows) {
+		scene_globals const &g = globals();
+		tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape); // with hs: the weights' jitter noise
+		tw_erosion_params const e = erosion_params_from_globals();
+		uint64_t const number = ++jobs;
+		int const rc = hs ? tw_create_tiles_launch_hmap(c, hs, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out,
+		                                                &shading, shadows.nlights ? &shadows : nullptr)
+		                  : tw_create_tiles_launch_shadows(c, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out,
+		                                                   &shading, shadows.nlights ? &shadows : nullptr);
+		if (rc != TW_OK) {fail(rc, hs ? "create_tiles_async_from_heightmap" : "create_tiles_async", c);}
+		return tiles_job(c, &jobs, number);
+	}
+}
 inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
                                     tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows) {
-	scene_globals const &g = globals();
-	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
-	tw_erosion_params const e = erosion_params_from_globals();
 	tw_ctx *c = ctx();
-	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
-	uint64_t const number = ++jobs;
-	int const rc = tw_create_tiles_launch_shadows(c, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out, &shading,
-	                                              shadows.nlights ? &shadows : nullptr);
-	if (rc != TW_OK) {detail::fail(rc, "create_tiles_async", c);}
-	return tiles_job(c, &jobs, number);
+	return detail::launch_tiles(c, detail::tls().tile_jobs, nullptr, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
 }
 inline tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
                                     tw_tile_outputs const &out, tw_tile_shading const &shading) {
@@ -354,18 +400,69 @@ inline void set_heightmap(const uint8_t *hmap16, int width, int height) {
 inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max,
                                                    unsigned size, tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows,
                                                    int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
-	scene_globals const &g = globals();
-	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape); // the weights' jitter noise
-	tw_erosion_params const e = erosion_params_from_globals();
 	tw_ctx *c = ctx();
 	tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
-	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
-	uint64_t const number = ++jobs;
-	int const rc = tw_create_tiles_launch_hmap(c, &hs, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, zvsize, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size, &out,
-	                                           &shading, shadows.nlights ? &shadows : nullptr);
-	if (rc != TW_OK) {detail::fail(rc, "create_tiles_async_from_heightmap", c);}
-	return tiles_job(c, &jobs, number);
+	return detail::launch_tiles(c, detail::tls().tile_jobs, &hs, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
 }
+
+// Several frames' tile jobs in flight at once: a pool of n shared contexts of this thread's ctx() (tw_create_shared - the same tables and heightmap
+// image, own streams and scratch). pool.create_tiles_async(...) takes the arguments of the free functions above and launches on a slot with no job in
+// flight; when every slot is busy, on the slot launched on longest ago, whose job that launch completes first (its tiles_job then reports ready).
+// A launch never waits for another slot's job. Create and use the pool on one thread, let it outlive the jobs it returned, and destroy it before the
+// thread ends (its contexts are shared contexts of the thread's context); destroying it completes its jobs.
+class tile_job_pool {
+	struct slot {tw_ctx *c = nullptr; std::atomic<uint64_t> jobs{0}; uint64_t launched = 0;};
+	std::vector<std::unique_ptr<slot>> slots; // stable addresses: a tiles_job keeps a pointer to its slot's launch count
+	uint64_t clock = 0;
+	slot &next() {
+		ctx(); // the thread's context takes new tables first (set_globals), completing the slots' jobs if it does
+		slot *pick = nullptr;
+		for (auto &s : slots) {
+			int const rc = tw_create_tiles_poll(s->c, 0);   // TW_OK: nothing in flight (a finished job is unpacked into its outputs here)
+			if (rc == TW_OK) {pick = s.get(); break;}
+			if (rc != TW_ERR_NOT_READY) {detail::fail(rc, "create_tiles_async", s->c);}
+		}
+		if (!pick) {pick = slots[0].get(); for (auto &s : slots) {if (s->launched < pick->launched) pick = s.get();}}
+		pick->launched = ++clock;
+		return *pick;
+	}
+public:
+	explicit tile_job_pool(unsigned n) {
+		tw_ctx *c = ctx();
+		for (unsigned i = 0; i < (n ? n : 1); ++i) {
+			slots.emplace_back(new slot());
+			int const rc = tw_create_shared(c, &slots.back()->c);
+			if (rc != TW_OK) {slots.pop_back(); for (auto &s : slots) {tw_destroy(s->c);} detail::fail(rc, "tile_job_pool: tw_create_shared", c);}
+		}
+	}
+	~tile_job_pool() {for (auto &s : slots) {tw_destroy(s->c);}}
+	tile_job_pool(tile_job_pool const &) = delete;
+	tile_job_pool &operator=(tile_job_pool const &) = delete;
+	unsigned size() const {return (unsigned)slots.size();}
+	tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
+	                             tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows) {
+		slot &s = next();
+		return detail::launch_tiles(s.c, s.jobs, nullptr, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
+	}
+	tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
+	                             tw_tile_outputs const &out, tw_tile_shading const &shading) {
+		tw_tile_shadows const none = {nullptr, 0, nullptr};
+		return create_tiles_async(origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, none);
+	}
+	tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
+	                             tw_tile_outputs const &out) {
+		tw_tile_shading const none = {0.0f, nullptr, nullptr, nullptr, nullptr, nullptr};
+		return create_tiles_async(origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, none);
+	}
+	// heightmap-texture tiles from the image set_heightmap() gave this thread's context
+	tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max,
+	                                            unsigned size, tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows,
+	                                            int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+		slot &s = next();
+		tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
+		return detail::launch_tiles(s.c, s.jobs, &hs, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
+	}
+};
 
 // tile_t::upload_normal_texture (src/tiled_mesh.cpp:865-880, minus the GL upload) and tile_t::calc_mesh_ao_lighting (:586-662) for a batch of
 // finished tiles: normal_data = ntiles*stride^2*4 bytes (RGBA, alpha 0), ao_lighting = ntiles*stride^2 bytes, stride = zvsize-1

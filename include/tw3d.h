@@ -46,7 +46,7 @@ enum { TW_MGEN_SINE = 0, TW_MGEN_SIMPLEX = 1, TW_MGEN_PERLIN = 2, TW_MGEN_SIMPLE
 #define TW_N3D_RDATA      420     /* SINE_DATA_SIZE, src/upsurface.h:14-16 */
 #define TW_N3D_SINES      60      /* TOT_NUM_SINES */
 
-typedef struct tw_ctx tw_ctx;   /* one per (thread, device): owns a CUDA stream, the uploaded tables and scratch buffers */
+typedef struct tw_ctx tw_ctx;   /* one per (thread, device): owns a CUDA stream, the uploaded tables (or reads its parent's: tw_create_shared) and scratch buffers */
 
 /* hmap_params_t, src/mesh.h:85-89 (same field order) */
 typedef struct tw_hmap_params {
@@ -118,9 +118,25 @@ typedef struct tw_voxel_params {
  * Host output buffers: asynchronous entry points (tw_heightgen_2d_launch, tw_create_tiles_launch) overlap the device->host copy with compute only when
  * the buffer is page-locked (cudaHostAlloc / cudaHostRegister / tw_multi_alloc_host); with pageable memory the copy - and therefore the launch call - blocks.
  * A context has at most one asynchronous job in flight: every other call on it (including the next launch) first completes the pending job, exactly
- * as a poll with wait = 1 would, and either poll function completes whichever job is pending. */
+ * as a poll with wait = 1 would, and either poll function completes whichever job is pending. The rule is per context: to keep several jobs in flight
+ * on one device, give each its own shared context (tw_create_shared); a call on one context never completes another context's job, except the three
+ * table setters on a parent (below).
+ * Threads: one thread at a time per context. A parent's tw_set_sin_table, tw_set_sine_params and tw_set_heightmap must not run while another thread is
+ * inside a call on one of its shared contexts. */
 TW_API int  tw_abi_version(void);
 TW_API int  tw_create(int device, tw_ctx **out);
+/* A context on parent's device that uses parent's tables instead of its own: sin table, direction table, sine params, the simplex/Perlin
+ * and 3-D noise LUTs, and the tw_set_heightmap image. It has its own streams, scratch, pinned staging, pending job, launch count and
+ * erosion step count, so its asynchronous job runs beside the parent's and the other shared contexts' jobs. Every entry point accepts it, with the
+ * results the same call on the parent gives, bit for bit.
+ * - Tables are set on the parent only: tw_set_sin_table, tw_set_sine_params and tw_set_heightmap on a shared context return TW_ERR_ARG and change
+ *   nothing. On the parent they first complete the pending job of every shared context (as a poll with wait = 1 would), then replace the table; the
+ *   next call on a shared context uses the new tables. Before the parent has a table, a shared context gets TW_ERR_STATE where the parent would.
+ * - The parent's LUTs are built here if absent (one synchronisation of the parent's stream); a shared context never allocates or builds a table.
+ * - TW_ERR_ARG for a NULL parent and for a parent that is itself a shared context (one level only).
+ * - tw_destroy(shared) completes its job as a poll with wait = 1 would and frees only what it owns. tw_destroy(parent) first destroys the shared
+ *   contexts still alive the same way; their handles are invalid afterwards. */
+TW_API int  tw_create_shared(tw_ctx *parent, tw_ctx **out);
 TW_API void tw_destroy(tw_ctx *ctx);
 TW_API const char *tw_last_error(const tw_ctx *ctx);
 TW_API int  tw_sync(tw_ctx *ctx);                         /* cudaStreamSynchronize on the context stream */

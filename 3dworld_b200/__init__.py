@@ -102,6 +102,16 @@ class TileShadows(C.Structure):
     _fields_ = [("tile_xy", C.c_void_p), ("nlights", C.c_uint32), ("lights", C.c_void_p)]
 
 
+class TileSetLight(C.Structure):
+    """tw_tile_set_light (include/tw3d.h): one light of a tile set relight (smask required; sh_out_* optional)."""
+    _fields_ = [("sp", ShadowParams), ("smask", C.c_void_p), ("sh_out_x", C.c_void_p), ("sh_out_y", C.c_void_p)]
+
+
+class TileSetRequest(C.Structure):
+    """tw_tile_set_request (include/tw3d.h): the resident tiles a relight outputs, its lights, and the optional host recomputed flags."""
+    _fields_ = [("tile_xy", C.c_void_p), ("n", C.c_uint32), ("nlights", C.c_uint32), ("lights", C.c_void_p), ("recomputed", C.c_void_p)]
+
+
 class PointQuery(C.Structure):
     _fields_ = [("kind", C.c_int), ("xy_scale", C.c_float), ("mesh_x_size", C.c_int), ("mesh_y_size", C.c_int), ("x_scene_size", C.c_float),
                 ("y_scene_size", C.c_float), ("xoff2", C.c_int), ("yoff2", C.c_int), ("no_xyoff", C.c_int)]
@@ -137,7 +147,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_heightmap_from_floats_u16", "tw_heightmap_to_floats_u16", "tw_proc_gen_heightmap", "tw_heightmap_sample_tiles", "tw_set_heightmap", "tw_create_tiles_launch_hmap", "tw_minmax_f32",
                "tw_multi_create", "tw_multi_destroy", "tw_multi_size", "tw_multi_ctx", "tw_multi_last_error", "tw_multi_set_sine_params", "tw_multi_range",
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
-               "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables"]
+               "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
+               "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch"]
 
 
 def _load():
@@ -230,6 +241,13 @@ def _load():
     L.tw_voxel_triangles.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, vp, C.c_uint64, C.POINTER(C.c_uint64)]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
+    L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
+    L.tw_tile_set_destroy.argtypes = [vp]
+    L.tw_tile_set_destroy.restype = None
+    L.tw_tile_set_put.argtypes = [vp, vp, C.c_uint32, vp]
+    L.tw_tile_set_remove.argtypes = [vp, vp, C.c_uint32]
+    L.tw_tile_set_stale.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(C.c_uint32)]
+    L.tw_tile_set_shadows_launch.argtypes = [vp, C.POINTER(TileSetRequest)]
     L.tw_tile_weights_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint32, C.POINTER(HeightParams), C.POINTER(WeightParams), vp, vp, vp]
     L.tw_gen_tex_height_tables.argtypes = [C.c_float, C.c_float, C.c_float, vp, vp, vp]
     L.tw_gen_tex_height_tables.restype = None
@@ -403,7 +421,7 @@ class Context:
             raise TwError(rc, "tw_create failed (no CUDA device? this library has no CPU fallback)")
         self._h = h
         self.device = device
-        self.parent, self._shared = None, []
+        self.parent, self._shared, self._sets = None, [], []
         self._check(lib.tw_set_sin_table(self._h, _ptr(sin_table)))
 
     def shared(self):
@@ -413,14 +431,22 @@ class Context:
         h = C.c_void_p()
         self._check(lib.tw_create_shared(self._h, C.byref(h)))
         s = Context.__new__(Context)
-        s._h, s.device, s.parent, s._shared = h, self.device, self, []
+        s._h, s.device, s.parent, s._shared, s._sets = h, self.device, self, [], []
         self._shared.append(s)
         return s
+
+    def tile_set(self, zvsize, nlights):
+        """tw_tile_set_create: a TileSet of this context - the live tiles' zvals on the device and each light slot's cached mesh shadows."""
+        return TileSet(self, zvsize, nlights)
 
     def close(self):
         if getattr(self, "_h", None) and lib is not None:   # lib can already be gone at interpreter shutdown
             for s in getattr(self, "_shared", ()):         # tw_destroy(parent) destroys them: their handles must not be destroyed again
+                for ts in getattr(s, "_sets", ()):
+                    ts._h = None
                 s._h = None
+            for ts in getattr(self, "_sets", ()):           # and this context's tile sets
+                ts._h = None
             lib.tw_destroy(self._h)
             if getattr(self, "parent", None) is not None and self in self.parent._shared:
                 self.parent._shared.remove(self)
@@ -758,6 +784,74 @@ class Context:
         mm = MinMax()
         self._check(lib.tw_minmax_f32(self._h, _ptr(vals), int(np.prod(vals.shape)), C.byref(mm)))
         return mm.zmin, mm.zmax
+
+
+class TileSet:
+    """tw_tile_set (include/tw3d.h): resident tiles keyed by their grid coordinates (x1/size, y1/size), with per light slot the mesh shadows each tile was
+    last computed with. A relight (shadows_launch) is the context's asynchronous job, completed by Context.create_tiles_poll; its outputs equal
+    tw_tile_shadows_batch_ex over all resident tiles, bit for bit. Context.close() destroys the set with the context."""
+
+    def __init__(self, ctx, zvsize, nlights):
+        h = C.c_void_p()
+        ctx._check(lib.tw_tile_set_create(ctx._h, int(zvsize), int(nlights), C.byref(h)))
+        self._h, self.ctx, self.zvsize, self.nlights = h, ctx, int(zvsize), int(nlights)
+        ctx._sets.append(self)
+
+    def close(self):
+        if getattr(self, "_h", None) and lib is not None:
+            lib.tw_tile_set_destroy(self._h)
+            if self in self.ctx._sets:
+                self.ctx._sets.remove(self)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _xy(tile_xy):
+        return np.ascontiguousarray(tile_xy, np.int32).reshape(-1, 2)
+
+    def put(self, tile_xy, zvals):
+        """Inserts or replaces tiles: zvals [n, zv, zv] float32, numpy or CUDA tensor (read before the call returns)."""
+        txy = self._xy(tile_xy)
+        if not hasattr(zvals, "data_ptr"):
+            zvals = np.ascontiguousarray(zvals, np.float32)
+        self.ctx._check(lib.tw_tile_set_put(self._h, _ptr(txy), len(txy), _ptr(zvals)))
+
+    def remove(self, tile_xy):
+        txy = self._xy(tile_xy)
+        self.ctx._check(lib.tw_tile_set_remove(self._h, _ptr(txy), len(txy)))
+
+    def stale(self, sps):
+        """The resident tiles a relight of every tile with these ShadowParams (light l = slot l) would recompute: [k, 2] int32 in (x, y) order."""
+        arr = (ShadowParams * len(sps))(*sps)
+        k = C.c_uint32()
+        self.ctx._check(lib.tw_tile_set_stale(self._h, C.cast(arr, C.c_void_p), len(sps), None, 0, C.byref(k)))
+        out = np.empty((k.value, 2), np.int32)
+        if k.value:
+            self.ctx._check(lib.tw_tile_set_stale(self._h, C.cast(arr, C.c_void_p), len(sps), _ptr(out), k.value, C.byref(k)))
+        return out
+
+    def shadows_launch(self, tile_xy, lights):
+        """tw_tile_set_shadows_launch: enqueues the relight of the resident tiles tile_xy [n, 2] and returns the host recomputed flags [n] uint8 (1 = this job
+        computes the tile for at least one light). lights: Light records or (ShadowParams, smask, sh_out_x, sh_out_y) tuples - smask [n, zv, zv] uint8
+        required, sh_out_* [n, zv] float32 or None - numpy arrays (pinned for a launch that does not block) or CUDA tensors, kept referenced here until
+        Context.create_tiles_poll completes the job."""
+        txy = self._xy(tile_xy)
+        recs = [lt if isinstance(lt, Light) else Light(*lt) for lt in lights]
+        if any(r.sh_in_x is not None or r.sh_in_y is not None for r in recs):
+            raise ValueError("shadows_launch: a tile set takes its incoming rows from its own tiles (no sh_in)")
+        arr = (TileSetLight * max(1, len(recs)))()
+        for i, r in enumerate(recs):
+            arr[i] = TileSetLight(r.sp, _ptr(r.smask), _ptr(r.sh_out_x), _ptr(r.sh_out_y))
+        recomputed = np.zeros(len(txy), np.uint8)
+        req = TileSetRequest(_ptr(txy), len(txy), len(recs), C.cast(arr, C.c_void_p), _ptr(recomputed))
+        self.ctx._check(lib.tw_tile_set_shadows_launch(self._h, C.byref(req)))
+        self.ctx._tiles_job = ([(r.smask, r.sh_out_x, r.sh_out_y) for r in recs], arr)
+        return recomputed
 
 
 def gen_tex_height_tables(water_h_off_rel=0.0, temperature=20.0, glaciate_exp=3.0):

@@ -228,6 +228,7 @@ int tw_create_shared(tw_ctx *parent, tw_ctx **out) {
 
 void tw_destroy(tw_ctx *ctx) {
 	if (!ctx) return;
+	while (!ctx->sets.empty()) tw_tile_set_destroy(ctx->sets.back()); // each completes the pending job and removes itself from the list
 	while (!ctx->shared.empty()) tw_destroy(ctx->shared.back()); // each removes itself from the list
 	if (ctx->dist) tw_dist_finalize(ctx);
 	cudaSetDevice(ctx->device);

@@ -63,6 +63,7 @@ struct tw_ctx {
 	// from the parent at the start of every entry point (twi_borrow_tables) and never allocated, built or freed here
 	tw_ctx *parent = nullptr;
 	std::vector<tw_ctx *> shared; // the parent's live shared contexts
+	std::vector<tw_tile_set *> sets; // live tile sets (tw_tileset.cu), destroyed with the context
 };
 
 int  tw_set_error(tw_ctx *ctx, int status, const char *fmt, ...);

@@ -8,6 +8,7 @@
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //   tw3d::set_deferred_gens, tw3d::tile_job_pool  <->  several of them in flight at once, as tile_draw_t::update keeps up to 8   src/tiled_mesh.cpp:2367-2417
+//   tw3d::tile_set               <->  the live tiles' calc_shadows_for_light when the light moves or new tiles appear   src/tiled_mesh.cpp:664-692
 //
 // The reference reads ~20 globals on this path (SURVEY.md 8b); here they are one explicit struct (scene_globals) set once per scene
 // with set_globals(). Same names, argument meaning and error behaviour as the reference: argument errors assert/abort like the
@@ -520,6 +521,50 @@ inline void calc_mesh_shadows(const float lpos[3], const float *zvals, const int
 	int const rc = tw_tile_shadows_batch_ex(c, zvals, tile_xy, ntiles, zvsize, &sp, sh_in_x, sh_in_y, smask, sh_out_x, sh_out_y);
 	if (rc != TW_OK) {detail::fail(rc, "calc_mesh_shadows", c);}
 }
+
+// The live tiles of tile_draw_t on the device (tw_tile_set, include/tw3d.h), for the two relights of calc_shadows_for_light the engine otherwise does itself
+// (src/tiled_mesh.cpp:664-692): when the light moves, relight_async() every live tile; when new tiles appear, put() them (a tile job's device zvals cost one
+// copy on the device), ask stale() which shadow textures change, and relight_async() those. Each relight equals calc_mesh_shadows over all resident tiles, bit
+// for bit, and recomputes only the tiles whose result can have changed. relight_async returns the tiles_job of create_tiles_async: outputs (smask, sh_out_*
+// of every tw_tile_set_light, in request order) are complete once it is ready. Lives on this thread's ctx(); destroy it before the thread ends.
+class tile_set {
+	tw_ctx *c = nullptr;
+	tw_tile_set *s = nullptr;
+public:
+	tile_set(unsigned zvsize, unsigned nlights) : c(ctx()) {
+		int const rc = tw_tile_set_create(c, zvsize, nlights, &s);
+		if (rc != TW_OK) {s = nullptr; detail::fail(rc, "tile_set", c);}
+	}
+	~tile_set() {if (s) tw_tile_set_destroy(s);}
+	tile_set(tile_set const &) = delete;
+	tile_set &operator=(tile_set const &) = delete;
+	tw_tile_set *handle() const {return s;}
+	void put(const int32_t *tile_xy, unsigned n, const float *zvals) {
+		int const rc = tw_tile_set_put(s, tile_xy, n, zvals);
+		if (rc != TW_OK) {detail::fail(rc, "tile_set::put", c);}
+	}
+	void remove(const int32_t *tile_xy, unsigned n) {
+		int const rc = tw_tile_set_remove(s, tile_xy, n);
+		if (rc != TW_OK) {detail::fail(rc, "tile_set::remove", c);}
+	}
+	// (x, y) pairs of the tiles a relight of every resident tile with these lights recomputes
+	std::vector<int32_t> stale(const tw_shadow_params *sps, unsigned nlights) const {
+		uint32_t k = 0;
+		int rc = tw_tile_set_stale(s, sps, nlights, nullptr, 0, &k);
+		std::vector<int32_t> out(2*(size_t)k);
+		if (rc == TW_OK && k) {rc = tw_tile_set_stale(s, sps, nlights, out.data(), k, &k);}
+		if (rc != TW_OK) {detail::fail(rc, "tile_set::stale", c);}
+		return out;
+	}
+	tiles_job relight_async(const int32_t *tile_xy, unsigned n, const tw_tile_set_light *lights, unsigned nlights, uint8_t *recomputed = nullptr) {
+		std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+		uint64_t const number = ++jobs;
+		tw_tile_set_request const req = {tile_xy, n, nlights, lights, recomputed};
+		int const rc = tw_tile_set_shadows_launch(s, &req);
+		if (rc != TW_OK) {detail::fail(rc, "tile_set::relight_async", c);}
+		return tiles_job(c, &jobs, number);
+	}
+};
 
 // tile_t::create_texture's terrain part (src/tiled_mesh.cpp:1071-1248) for a batch of tiles: mesh_weight_data (RGBA = {sand, dirt, grass, rock}, stride^2 texels per
 // tile) and has_any_grass. The caller passes what the reference reads from engine tables: h_dirt[] and lttex_dirt[].id (as TW_TEX_* classes), sthresh, the biome corners

@@ -444,8 +444,8 @@ TW_API int tw_tile_shadows_batch(tw_ctx *ctx, const float *zvals, const int32_t 
  * A caller row is read only where that neighbour is NOT in the batch; an in-batch neighbour's sh_out, computed in this call, always wins. Entries
  * <= TW_MESH_MIN_Z mean "no incoming height". With both NULL the results equal tw_tile_shadows_batch's. Unlike it, this call takes any number of tiles and
  * returns TW_ERR_ARG when tile_xy names a tile twice.
- * What stays the caller's job: when new tiles appear, existing tiles on their far side from the light may need new shadows, because their neighbour toward
- * the light now exists. Which of them to redo is engine policy; redo them with this call, passing the new tiles' sh_out as their sh_in. */
+ * When new tiles appear, existing tiles on their far side from the light may need new shadows, because their neighbour toward the light now exists; and when
+ * the light moves, every live tile does. A tile set (tw_tile_set_*, below) keeps the live tiles on the device and works out which tiles those are. */
 TW_API int tw_tile_shadows_batch_ex(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy, uint32_t ntiles, uint32_t zvsize, const tw_shadow_params *sp,
                           const float *sh_in_x, const float *sh_in_y, uint8_t *smask, float *sh_out_x, float *sh_out_y);
 /* Mesh shadows of a frame's new tiles inside the asynchronous tile job: tw_create_tiles_launch_shadows(..., shading, shadows) is tw_create_tiles_launch_ex
@@ -485,6 +485,53 @@ TW_API int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy
 TW_API int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size,
                           float dx, float dy, uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
                           float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows);
+
+/* ---- tile sets: the live tiles kept on the device, relit with cached, chained mesh shadows ----
+ * What tile_draw_t::update does for every live tile when the light moves, and for the existing tiles behind new ones (src/tiled_mesh.cpp:664-692): a tile set
+ * holds the zvals of the resident tiles in device memory the set owns, keyed by their grid coordinates (x1/size, y1/size), and per light slot the mesh shadows
+ * (smask, sh_out_x, sh_out_y) each tile was last computed with. tw_tile_set_shadows_launch enqueues a relight as the context's asynchronous job:
+ *   every output equals tw_tile_shadows_batch_ex on ALL tiles resident at launch time, with no caller rows, bit for bit;
+ * the cache only skips tiles whose result cannot have changed. With sx = (lpos.x < 0 ? -1 : 1), sy = (lpos.y < 0 ? -1 : 1), the tiles DOWNSTREAM of (tx, ty)
+ * are the resident (tx, ty - sy) and (tx - sx, ty), transitively (the walk stops at a tile that is not resident): exactly the tiles whose incoming rows come
+ * from it. A light slot keeps the tw_shadow_params it was last computed with and one valid bit per resident tile:
+ *   - a request whose params differ byte for byte from the slot's invalidates the whole slot;
+ *   - tw_tile_set_put of a tile invalidates it and its downstream closure in every slot; tw_tile_set_remove invalidates its downstream closure;
+ *   - a relight recomputes the invalid requested tiles plus their invalid upstream closure, reading the cached sh_out of valid resident neighbours as
+ *     incoming rows and "no incoming height" where a neighbour is not resident.
+ * The cache promises equality with the full recompute, not the fewest recomputed tiles: sh_out is written only for light from +x / +y (DESIGN.md §4b), so a
+ * closure can recompute tiles whose inputs did not change.
+ * A set belongs to its context (a shared context is fine) and follows the context's rules: put, remove, destroy and a new launch complete the context's
+ * pending job first, and tw_create_tiles_poll completes the relight. tw_destroy(ctx) destroys the context's live sets first; their handles are invalid after. */
+typedef struct tw_tile_set tw_tile_set;
+/* zvsize >= 2 and nlights >= 1 (the number of light slots), else TW_ERR_ARG. */
+TW_API int  tw_tile_set_create(tw_ctx *ctx, uint32_t zvsize, uint32_t nlights, tw_tile_set **out);
+TW_API void tw_tile_set_destroy(tw_tile_set *set);
+/* Inserts or replaces n tiles: tile_xy = n (x1/size, y1/size) pairs, zvals = n*zvsize^2 floats, host or device (a tile job's device zvals cost one copy on the
+ * device). Returns once zvals has been read. TW_ERR_ARG (nothing changes) for a tile named twice or n == 0. */
+TW_API int  tw_tile_set_put(tw_tile_set *set, const int32_t *tile_xy, uint32_t n, const float *zvals);
+/* Removes n resident tiles. TW_ERR_ARG (nothing changes) for a tile that is not resident or is named twice. */
+TW_API int  tw_tile_set_remove(tw_tile_set *set, const int32_t *tile_xy, uint32_t n);
+/* Host only: the resident tiles a relight of every resident tile with these nlights lights (light l = slot l) would recompute for at least one light - the
+ * shadow textures the engine has to refresh - in (x, y) order. Writes min(capacity, count) pairs to tile_xy_out (may be NULL with capacity 0); *nstale =
+ * count, which may exceed capacity. */
+TW_API int  tw_tile_set_stale(tw_tile_set *set, const tw_shadow_params *sps, uint32_t nlights, int32_t *tile_xy_out, uint32_t capacity, uint32_t *nstale);
+/* One light of a relight request: all arrays in request order, host or device; smask and sh_out_* must stay valid until the completing poll (pinned host or
+ * device memory for a launch that does not block). */
+typedef struct tw_tile_set_light {
+	tw_shadow_params sp;
+	uint8_t *smask;                    /* required: n*zvsize^2 bytes (device: 4-byte aligned) */
+	float   *sh_out_x, *sh_out_y;      /* optional: n*zvsize floats each */
+} tw_tile_set_light;
+typedef struct tw_tile_set_request {
+	const int32_t           *tile_xy;     /* required: the n tiles to output, each resident and named once */
+	uint32_t                 n;
+	uint32_t                 nlights;     /* 1 .. the set's nlights; light l uses slot l */
+	const tw_tile_set_light *lights;
+	uint8_t                 *recomputed;  /* optional HOST, n bytes, filled before the launch returns: 1 = this job computes tile i for at least one light */
+} tw_tile_set_request;
+/* Enqueues the relight and returns; tw_create_tiles_poll completes it. The request, its lights array and tile_xy are read during the launch. Errors return
+ * TW_ERR_ARG before anything is enqueued or cached state changes. */
+TW_API int  tw_tile_set_shadows_launch(tw_tile_set *set, const tw_tile_set_request *req);
 
 /* ---- terrain weights texture of tiles (SURVEY.md 8f row N4): tile_t::create_texture (src/tiled_mesh.cpp:1071-1248), the terrain part ----
  * RGBA texel (x, y) of a tile, x, y < stride = zvsize - 1: the weights {sand, dirt, grass, rock} (snow = the rest) of the ground textures from the cell's relative

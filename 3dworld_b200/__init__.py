@@ -112,6 +112,11 @@ class TileSetRequest(C.Structure):
     _fields_ = [("tile_xy", C.c_void_p), ("n", C.c_uint32), ("nlights", C.c_uint32), ("lights", C.c_void_p), ("recomputed", C.c_void_p)]
 
 
+class TileSetFrame(C.Structure):
+    """tw_tile_set_frame (include/tw3d.h): a frame launch's removes, the new tiles' grid coordinates, the optional heightmap sampler and relight request."""
+    _fields_ = [("remove_xy", C.c_void_p), ("nremove", C.c_uint32), ("tile_xy", C.c_void_p), ("hs", C.c_void_p), ("relight", C.c_void_p)]
+
+
 class PointQuery(C.Structure):
     _fields_ = [("kind", C.c_int), ("xy_scale", C.c_float), ("mesh_x_size", C.c_int), ("mesh_y_size", C.c_int), ("x_scene_size", C.c_float),
                 ("y_scene_size", C.c_float), ("xoff2", C.c_int), ("yoff2", C.c_int), ("no_xyoff", C.c_int)]
@@ -148,7 +153,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_multi_create", "tw_multi_destroy", "tw_multi_size", "tw_multi_ctx", "tw_multi_last_error", "tw_multi_set_sine_params", "tw_multi_range",
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
-               "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch"]
+               "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
+               "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after"]
 
 
 def _load():
@@ -248,6 +254,10 @@ def _load():
     L.tw_tile_set_remove.argtypes = [vp, vp, C.c_uint32]
     L.tw_tile_set_stale.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(C.c_uint32)]
     L.tw_tile_set_shadows_launch.argtypes = [vp, C.POINTER(TileSetRequest)]
+    L.tw_tile_set_create_tiles_launch.argtypes = [vp, vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.POINTER(HeightParams), C.c_uint32,
+                                                  C.POINTER(ErosionParams), C.c_float, C.c_float, C.c_uint32, C.POINTER(TileOutputs), C.POINTER(TileShading),
+                                                  C.POINTER(TileSetFrame)]
+    L.tw_tile_set_stale_after.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(C.c_uint32)]
     L.tw_tile_weights_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint32, C.POINTER(HeightParams), C.POINTER(WeightParams), vp, vp, vp]
     L.tw_gen_tex_height_tables.argtypes = [C.c_float, C.c_float, C.c_float, vp, vp, vp]
     L.tw_gen_tex_height_tables.restype = None
@@ -851,6 +861,65 @@ class TileSet:
         req = TileSetRequest(_ptr(txy), len(txy), len(recs), C.cast(arr, C.c_void_p), _ptr(recomputed))
         self.ctx._check(lib.tw_tile_set_shadows_launch(self._h, C.byref(req)))
         self.ctx._tiles_job = ([(r.smask, r.sh_out_x, r.sh_out_y) for r in recs], arr)
+        return recomputed
+
+    def stale_after(self, sps, remove_xy=None, put_xy=None):
+        """tw_tile_set_stale_after: what stale(sps) would return after remove(remove_xy) and put(put_xy), without changing the set - the tiles to name in
+        a frame's relight (create_tiles_launch(relight_xy=...))."""
+        arr = (ShadowParams * len(sps))(*sps)
+        rem = self._xy(remove_xy if remove_xy is not None else np.empty((0, 2)))
+        put = self._xy(put_xy if put_xy is not None else np.empty((0, 2)))
+        k = C.c_uint32()
+        args = [self._h, C.cast(arr, C.c_void_p), len(sps), _ptr(rem) if len(rem) else None, len(rem), _ptr(put) if len(put) else None, len(put)]
+        self.ctx._check(lib.tw_tile_set_stale_after(*args, None, 0, C.byref(k)))
+        out = np.empty((k.value, 2), np.int32)
+        if k.value:
+            self.ctx._check(lib.tw_tile_set_stale_after(*args, _ptr(out), k.value, C.byref(k)))
+        return out
+
+    def create_tiles_launch(self, origins_xy, mesh_size, dx, dy, hp, erosion_iters, ep, min_zval, tile_xy, zvals=None, mm=None, bounds=None, normals=None,
+                            min_normal_z=None, wpz_max=0.0, size=0, ao=None, weights=None, has_any_grass=None, half_dxy=None, wp=None, tile_params=None,
+                            remove_xy=None, relight_xy=None, lights=None, hmap=None, ctx=None):
+        """tw_tile_set_create_tiles_launch: one frame in one asynchronous job - remove remove_xy, create the tiles of origins_xy (grid coordinates tile_xy
+        [nt, 2]) as Context.create_tiles_launch would, put them into this set, and relight relight_xy with lights (Light records or (ShadowParams, smask,
+        sh_out_x, sh_out_y) tuples sized for relight_xy, as shadows_launch). The job runs on ctx: this set's Context (None), its parent or a shared Context of
+        that parent, so frames on several shared Contexts are in flight at once; ctx.create_tiles_poll completes it. zvals may be None (the zvals then stay in
+        the set only); the other outputs are those of Context.create_tiles_launch. Returns the relight's recomputed flags [len(relight_xy)] uint8, or None
+        without lights."""
+        c = self.ctx if ctx is None else ctx
+        org = np.ascontiguousarray(origins_xy, np.int32).reshape(-1, 2)
+        nt = org.shape[0]
+        txy = self._xy(tile_xy)
+        outs = TileOutputs(_ptr(zvals), _ptr(mm), C.cast(bounds, C.c_void_p) if bounds is not None else None, _ptr(normals), _ptr(min_normal_z))
+        shading = None
+        if ao is not None and half_dxy is None:
+            raise ValueError("create_tiles_launch: ao needs half_dxy (the ray's z step, HALF_DXY)")
+        if ao is not None or weights is not None or has_any_grass is not None:
+            if tile_params is not None and not hasattr(tile_params, "data_ptr"):
+                tile_params = np.ascontiguousarray(tile_params, np.float32)
+            shading = TileShading(0.0 if half_dxy is None else half_dxy, C.cast(C.pointer(wp), C.c_void_p) if wp is not None else None, _ptr(tile_params),
+                                  _ptr(ao), _ptr(weights), _ptr(has_any_grass))
+        rem = self._xy(remove_xy) if remove_xy is not None else None
+        req, arr, recs, recomputed = None, None, [], None
+        if (lights is None) != (relight_xy is None):
+            raise ValueError("create_tiles_launch: a relight needs both relight_xy (the resident tiles to relight) and lights")
+        if lights is not None:
+            rxy = self._xy(relight_xy)
+            recs = [lt if isinstance(lt, Light) else Light(*lt) for lt in lights]
+            if any(r.sh_in_x is not None or r.sh_in_y is not None for r in recs):
+                raise ValueError("create_tiles_launch: a tile set takes its incoming rows from its own tiles (no sh_in)")
+            arr = (TileSetLight * max(1, len(recs)))()
+            for i, r in enumerate(recs):
+                arr[i] = TileSetLight(r.sp, _ptr(r.smask), _ptr(r.sh_out_x), _ptr(r.sh_out_y))
+            recomputed = np.zeros(len(rxy), np.uint8)
+            req = TileSetRequest(_ptr(rxy), len(rxy), len(recs), C.cast(arr, C.c_void_p), _ptr(recomputed))
+        frame = TileSetFrame(_ptr(rem), 0 if rem is None else len(rem), _ptr(txy), C.cast(C.pointer(hmap), C.c_void_p) if hmap is not None else None,
+                             C.cast(C.pointer(req), C.c_void_p) if req is not None else None)
+        c._check(lib.tw_tile_set_create_tiles_launch(c._h, self._h, _ptr(org), nt, mesh_size[0], mesh_size[1], dx, dy, C.byref(hp) if hp is not None else None,
+                                                     erosion_iters, C.byref(ep) if ep is not None else None, min_zval, wpz_max, size, C.byref(outs),
+                                                     C.byref(shading) if shading is not None else None, C.byref(frame)))
+        c._tiles_job = (zvals, mm, bounds, normals, min_normal_z, ao, weights, has_any_grass, wp, tile_params, shading,
+                        [(r.smask, r.sh_out_x, r.sh_out_y) for r in recs], arr, req, frame)
         return recomputed
 
 

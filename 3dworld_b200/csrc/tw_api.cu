@@ -155,12 +155,27 @@ int read_minmax(tw_ctx *ctx, const unsigned *d_mm, tw_minmax *mm, uint32_t n) { 
 	return TW_OK;
 }
 
-int validate_height(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, const float *out) {
-	if (!g || !p || !out) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+int validate_gen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p) { // the grid and height params of a generation
+	if (!g || !p) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
 	if (g->nx == 0 || g->ny == 0) return tw_set_error(ctx, TW_ERR_ARG, "nx, ny must be > 0 (reference asserts, src/mesh_gen.cpp:589)");
 	if (p->gen_mode < 0 || p->gen_mode > TW_MGEN_DWARP_GPU) return tw_set_error(ctx, TW_ERR_ARG, "bad gen_mode %d", p->gen_mode);
 	if (p->start_eval_sin < 0 || p->start_eval_sin > TW_F_TABLE_SIZE) return tw_set_error(ctx, TW_ERR_ARG, "start_eval_sin out of range (src/mesh_gen.cpp:590)");
 	if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
+	return TW_OK;
+}
+
+int validate_height(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, const float *out) {
+	if (!out) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+	return validate_gen(ctx, g, p);
+}
+
+// tw_create_tiles_launch_hmap's checks of the sampler against the context's image (after check_ctx and finish_pending)
+int validate_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const tw_tile_shading *shading) {
+	if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_heightmap() has not been called");
+	if (!hs) return tw_set_error(ctx, TW_ERR_ARG, "null heightmap sampler");
+	if (hs->width != ctx->hmap_w || hs->height != ctx->hmap_h) return tw_set_error(ctx, TW_ERR_ARG, "sampler size %d x %d differs from the heightmap's %d x %d", hs->width, hs->height, ctx->hmap_w, ctx->hmap_h);
+	if (hs->edge_mode < 0 || hs->edge_mode > 2) return tw_set_error(ctx, TW_ERR_ARG, "bad edge_mode %d", hs->edge_mode);
+	if (shading && shading->ao) return tw_set_error(ctx, TW_ERR_ARG, "the AO map is not available for heightmap tiles (its context outside the tile is not defined in this mode)");
 	return TW_OK;
 }
 
@@ -509,11 +524,12 @@ int tw_erode_tiles(tw_ctx *ctx, float *maps, uint32_t ntiles, int xsize, int ysi
 // without waiting for the device; the job completes through poll_job (check_ctx and finish_pending have run). sh (optional): AO map and weights texture;
 // shs (optional): per-light mesh shadows. hs: the height source - nullptr = the procedural height function p, else the context's heightmap image under hs
 // (tw_create_tiles_launch_hmap, which has checked hs against the image and refused AO); p is then only read by the weights' jitter noise.
+// tail (optional, twi_job_tail): work appended after the chunk join; with it o->zvals may be NULL.
 static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy, uint32_t zvsize,
                         const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
-                        const tw_tile_outputs *o, const tw_tile_shading *sh, const tw_tile_shadows *shs, const tw_hmap_sampler *hs)
+                        const tw_tile_outputs *o, const tw_tile_shading *sh, const tw_tile_shadows *shs, const tw_hmap_sampler *hs, twi_job_tail *tail = nullptr)
 {
-	if (!origins_xy || ntiles == 0 || (!p && !hs) || !o || !o->zvals) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
+	if (!origins_xy || ntiles == 0 || (!p && !hs) || !o || (!o->zvals && !tail)) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	bool const want_mm = (o->mm != nullptr), want_bounds = (o->bounds != nullptr), want_normals = (o->normals_rgba != nullptr), want_mnz = (o->min_normal_z != nullptr);
 	bool const want_ao = (sh && sh->ao), want_w = (sh && sh->weights), want_f = (sh && sh->has_any_grass);
 	if (want_mnz && !want_normals) return tw_set_error(ctx, TW_ERR_ARG, "min_normal_z is produced with the normal map: pass normals_rgba too");
@@ -547,7 +563,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	}
 	tw_grid2d g; g.x0 = 0; g.y0 = 0; g.dx = dx; g.dy = dy; g.nx = zvsize; g.ny = zvsize;
 	int rc = TW_OK;
-	if (!hs) {rc = validate_height(ctx, &g, p, o->zvals); if (rc) return rc;}
+	if (!hs) {rc = validate_gen(ctx, &g, p); if (rc) return rc;}
 	else {
 		if (zvsize == 0) return tw_set_error(ctx, TW_ERR_ARG, "zvsize must be > 0");
 		if (want_w && !p) return tw_set_error(ctx, TW_ERR_ARG, "the weights texture needs p (its jitter noise is the height function's sine mode)");
@@ -560,10 +576,11 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	bool const ctx_mode = want_ao && p->gen_mode >= TW_MGEN_SIMPLEX_GPU;
 	uint32_t const stride = zvsize - 1, ray = 36, csz = stride + 2*ray; // AO_RAY_LEN, context_sz (src/tiled_mesh.cpp:43,601)
 	size_t const tile_elems = (size_t)zvsize*zvsize, n = tile_elems*ntiles, nrm_elems = (size_t)stride*stride, ctx_elems = (size_t)csz*csz;
-	bool const dev_out = tw_is_device_ptr(o->zvals), dev_nrm = want_normals && tw_is_device_ptr(o->normals_rgba);
+	bool const dev_out = o->zvals && tw_is_device_ptr(o->zvals), host_out = o->zvals && !dev_out, dev_nrm = want_normals && tw_is_device_ptr(o->normals_rgba);
 	bool const dev_ao = want_ao && tw_is_device_ptr(sh->ao), dev_w = want_w && tw_is_device_ptr(sh->weights), dev_f = want_f && tw_is_device_ptr(sh->has_any_grass);
 	bool const dev_tp = want_w && tw_is_device_ptr(sh->tile_params);
 	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
+	if (tail) {rc = tail->prepare(ctx); if (rc) return rc;}
 	rc = twi_ensure_aux_streams(ctx); if (rc) return rc;
 	// The pipeline. Work per tile is heavy-tailed (ocean tiles: 1000 droplets x 1 move; mountain tiles: 1e5 moves in one serial chain), and a chain
 	// cannot be sped up (csrc/tw_erosion.cu, plan_heavy), so the chains must START EARLY: (1) a coarse pre-pass evaluates the height function on an
@@ -597,8 +614,8 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	for (uint32_t l = 0; l < nl; ++l) {sh_host_m |= !sdev_m[l]; sh_in_x |= (lights[l].sh_in_x != nullptr); sh_in_y |= (lights[l].sh_in_y != nullptr);}
 	size_t const shm_bytes = sh_host_m ? al(n + 4) : 0, shk_bytes = nl ? al(2*edge*sizeof(unsigned long long)) : 0;
 	size_t const shx_bytes = nl ? al((sh_in_x ? 2 : 1)*edge*sizeof(float)) : 0, shy_bytes = nl ? al((sh_in_y ? 2 : 1)*edge*sizeof(float)) : 0;
-	size_t const sh_bytes = shm_bytes + shk_bytes + shx_bytes + shy_bytes + nl*plan_bytes;
-	size_t const fixed_bytes = z_bytes + nrm_bytes + ao_bytes + w_bytes + f_bytes + tp_bytes + ctab_bytes + jtab_bytes + sh_bytes;
+	size_t const sh_bytes = shm_bytes + shk_bytes + shx_bytes + shy_bytes + nl*plan_bytes, tail_bytes = tail ? al(tail->dev_bytes) : 0;
+	size_t const fixed_bytes = z_bytes + nrm_bytes + ao_bytes + w_bytes + f_bytes + tp_bytes + ctab_bytes + jtab_bytes + sh_bytes + tail_bytes;
 	if (fixed_bytes) {rc = tw_reserve(ctx, 0, fixed_bytes); if (rc) return rc;}
 	// AO context grids and weights jitter grids are per chunk (schedule order): written on the main stream, read on the chunk's erosion stream. The buffers
 	// hold about 2 GB of context grids (or jitter grids without AO) in all, the bound tw_tile_ao_batch keeps; a chunk holds at most a third of that. When
@@ -652,6 +669,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	float *d_shx = (float *)s0; s0 += shx_bytes;
 	float *d_shy = (float *)s0; s0 += shy_bytes;
 	char *d_shp = s0; s0 += nl*plan_bytes;
+	char *d_tail = s0; s0 += tail_bytes;
 	char *d_ring = s0;
 	if (erode) {
 		sbytes = al(twi_erode_scratch_bytes(ctx, chunk, (int)zvsize, (int)zvsize));
@@ -691,7 +709,8 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		off_siy[l] = off_sh + in_sh; in_sh += (lights[l].sh_in_y && !sdev_iy[l]) ? al(edge*sizeof(float)) : 0;
 	}
 	size_t const off_steps = off_sh + in_sh, off_mm = off_steps + 256, off_sub = off_mm + (want_mm ? mm_bytes : 0), off_mnz = off_sub + sub_bytes, off_f = off_mnz + mnz_bytes;
-	rc = tw_reserve_pinned(ctx, off_f + (want_f ? al(ntiles) : 0)); if (rc) return rc;
+	size_t const off_tail = off_f + (want_f ? al(ntiles) : 0);
+	rc = tw_reserve_pinned(ctx, off_tail + (tail ? tail->pin_bytes : 0)); if (rc) return rc;
 	char *h_stage = (char *)ctx->h_pinned;
 	float2 *h_org = (float2 *)h_stage;
 	if (hs) {memcpy(h_stage, origins_xy, (size_t)ntiles*2*sizeof(int32_t));} // the sampler reads the int (x1, y1) origins (d_org then holds int2)
@@ -801,7 +820,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 			if (!ring_ev[b] && cudaEventCreateWithFlags(&ring_ev[b], cudaEventDisableTiming) != cudaSuccess) {ring_ev[b] = nullptr; status = tw_set_error(ctx, TW_ERR_CUDA, "ring event"); break;}
 			if (cudaEventRecord(ring_ev[b], es) != cudaSuccess) {status = tw_set_error(ctx, TW_ERR_CUDA, "ring event"); break;}
 		}
-		if (!dev_out && !d_perm && cudaMemcpyAsync(o->zvals + (size_t)t0*tile_elems, maps, (size_t)nt*tile_elems*sizeof(float), cudaMemcpyDeviceToHost, es) != cudaSuccess) {status = tw_set_error(ctx, TW_ERR_CUDA, "D2H");}
+		if (host_out && !d_perm && cudaMemcpyAsync(o->zvals + (size_t)t0*tile_elems, maps, (size_t)nt*tile_elems*sizeof(float), cudaMemcpyDeviceToHost, es) != cudaSuccess) {status = tw_set_error(ctx, TW_ERR_CUDA, "D2H");}
 	}
 	ctx->tile_perm = nullptr;
 	ctx->skip_rect[0] = ctx->skip_rect[1] = ctx->skip_rect[2] = ctx->skip_rect[3] = 0;
@@ -825,8 +844,12 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		if (L.sh_out_x) {TW_CUDA(ctx, cudaMemcpyAsync(L.sh_out_x, d_shx, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 		if (L.sh_out_y) {TW_CUDA(ctx, cudaMemcpyAsync(L.sh_out_y, d_shy, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	}
+	if (tail) { // the tail's work reads the final zvals; like the chunks', none of it may still run on the scratch when an error is returned
+		rc = tail->enqueue(ctx, d_out, d_tail, h_stage + off_tail);
+		if (rc) {cudaStreamSynchronize(ctx->stream); return rc;}
+	}
 	// every host-bound result is copied once, at the end: the schedule order scatters a chunk over the whole batch
-	if (!dev_out && d_perm) {TW_CUDA(ctx, cudaMemcpyAsync(o->zvals, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	if (host_out && d_perm) {TW_CUDA(ctx, cudaMemcpyAsync(o->zvals, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 	if (want_normals && !dev_nrm) {TW_CUDA(ctx, cudaMemcpyAsync(o->normals_rgba, d_rgba, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
 	if (want_ao && !dev_ao) {TW_CUDA(ctx, cudaMemcpyAsync(sh->ao, d_ao, (size_t)ntiles*nrm_elems, cudaMemcpyDeviceToHost, ctx->stream));}
 	if (want_w && !dev_w) {TW_CUDA(ctx, cudaMemcpyAsync(sh->weights, d_w, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
@@ -876,14 +899,25 @@ int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const in
 {
 	int rc = check_ctx(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
-	if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_heightmap() has not been called");
-	if (!hs) return tw_set_error(ctx, TW_ERR_ARG, "null heightmap sampler");
-	if (hs->width != ctx->hmap_w || hs->height != ctx->hmap_h) return tw_set_error(ctx, TW_ERR_ARG, "sampler size %d x %d differs from the heightmap's %d x %d", hs->width, hs->height, ctx->hmap_w, ctx->hmap_h);
-	if (hs->edge_mode < 0 || hs->edge_mode > 2) return tw_set_error(ctx, TW_ERR_ARG, "bad edge_mode %d", hs->edge_mode);
-	if (shading && shading->ao) return tw_set_error(ctx, TW_ERR_ARG, "the AO map is not available for heightmap tiles (its context outside the tile is not defined in this mode)");
+	rc = validate_hmap(ctx, hs, shading); if (rc) return rc;
 	ctx->last_erosion_steps = 0;
 	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, shadows, hs);
 }
+
+} // extern "C"
+
+int twi_create_tiles_launch(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                            uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
+                            const tw_tile_outputs *out, const tw_tile_shading *shading, twi_job_tail *tail)
+{
+	int rc = check_ctx(ctx); if (rc) return rc;
+	rc = finish_pending(ctx); if (rc) return rc;
+	if (hs) {rc = validate_hmap(ctx, hs, shading); if (rc) return rc;}
+	ctx->last_erosion_steps = 0;
+	return tiles_launch(ctx, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, erosion_iters, ep, min_zval, wpz_max, size, out, shading, nullptr, hs, tail);
+}
+
+extern "C" {
 
 int tw_create_tiles_launch_ex(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
                               uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,

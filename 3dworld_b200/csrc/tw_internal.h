@@ -172,6 +172,20 @@ size_t twi_shadow_plan_ints(uint32_t ntiles);
 void   twi_shadow_plan_pack(const twi_shadow_plan &P, int *out); // [wave_tiles | nbx | nby]
 int    twi_shadow_enqueue(tw_ctx *ctx, cudaStream_t st, const twi_shadow_plan &P, const float *d_z, uint32_t ntiles, uint32_t n, unsigned char *d_m,
                           unsigned long long *d_keys, float *d_ox, float *d_oy, const int *d_plan, bool use_graph);
+// Work a caller adds to the end of the asynchronous tile job (tw_tile_set_create_tiles_launch: the tile set's put and relight). The job validates its
+// arguments, then calls prepare (nothing of the job is enqueued yet), reserves dev_bytes of slot-0 scratch and pin_bytes of pinned staging for the tail
+// together with its own (before the erosion budget is taken), and after the chunk join calls enqueue on ctx->stream with the job's caller-order zvals, the
+// tail's scratch and its staging; the end-of-job copies and the job's event follow.
+struct twi_job_tail {
+	size_t dev_bytes = 0, pin_bytes = 0;
+	virtual int prepare(tw_ctx *ctx) = 0;
+	virtual int enqueue(tw_ctx *ctx, const float *d_zvals, char *d_mem, char *h_mem) = 0;
+	virtual ~twi_job_tail() {}
+};
+// tw_create_tiles_launch_ex (hs == nullptr) or tw_create_tiles_launch_hmap without shadows, with a tail; out->zvals may be NULL with a tail (zvals are then only staged on the device)
+int twi_create_tiles_launch(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                            uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
+                            const tw_tile_outputs *out, const tw_tile_shading *shading, twi_job_tail *tail);
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
 int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads);
 size_t   twi_erode_scratch_bytes(const tw_ctx *ctx, uint32_t chunk, int xsize, int ysize);

@@ -3,25 +3,26 @@
 // are in tw_tileset_rules.h) through the unchanged mesh-shadow plan and kernels of tw_shadows.cu, with the cached sh_out rows of valid neighbours as caller
 // rows, so every output equals tw_tile_shadows_batch_ex on all resident tiles. The kernels here only move tiles: gather a batch's zvals and caller rows out
 // of the slabs, scatter its results back, gather the requested outputs - one launch each per light, 16-byte accesses where the sizes and pointers allow.
+// A frame launch (tw_tile_set_create_tiles_launch) appends the put and the relight to a tile job on any context of the set's family; the set's event orders
+// the device work on its slabs across those contexts, while the host state is committed at launch, in launch order.
 #include "tw_internal.h"
 #include "tw_tileset_rules.h"
 #include <algorithm>
 #include <new>
 
 struct tw_tile_set {
-	struct slot_t {                                  // one light slot
+	struct slot_t {                                  // one light slot (its valid bits are st.valid[l])
 		bool have = false;                           // sp holds the params the valid tiles were computed with
 		tw_shadow_params sp;
-		std::vector<uint8_t> valid;                  // per slab slot
 		unsigned char *d_m = nullptr;                // capacity*zvsize^2 bytes: each tile's smask
 		float *d_ox = nullptr, *d_oy = nullptr;      // capacity*zvsize floats each: each tile's sh_out_x / sh_out_y
 	};
 	tw_ctx *ctx = nullptr;
 	uint32_t zvsize = 0, nlights = 0;
-	twts::index_map where;                           // resident tile -> slab slot
-	std::vector<uint32_t> free_slots;                // slots of removed tiles, reused first
-	uint32_t used = 0, capacity = 0;                 // slots handed out so far, slots allocated
+	twts::state st;                                  // resident tile -> slab slot, free slots, per light slot the valid bits
+	uint32_t capacity = 0;                           // slots allocated
 	float *d_z = nullptr;                            // capacity*zvsize^2 floats: the zvals slab (the set's own memory: tw_reserve may re-allocate scratch under a job)
+	cudaEvent_t ev = nullptr;                        // recorded after the last device work that touched the slabs, on whichever context of the family enqueued it
 	std::vector<slot_t> L;
 };
 
@@ -74,11 +75,11 @@ bool read_keys(const int32_t *tile_xy, uint32_t n, std::vector<twts::key> &keys)
 	return std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end();
 }
 
-// slabs for at least `need` tiles: geometric growth, the old contents copied over on the context's stream (nothing of the set's is in flight: put has completed
-// the pending job); nothing changes when an allocation fails
-int grow(tw_tile_set *s, uint32_t need) {
+// slabs for at least `need` tiles: geometric growth, the old contents copied over on ctx's stream once the set's device work on any context is done (it holds
+// the old slab pointers); nothing changes when an allocation fails
+int grow(tw_tile_set *s, uint32_t need, tw_ctx *ctx) {
 	if (need <= s->capacity) return TW_OK;
-	tw_ctx *ctx = s->ctx;
+	TW_CUDA(ctx, cudaEventSynchronize(s->ev));
 	uint32_t const cap = std::max(need, std::max<uint32_t>(16, 2*s->capacity));
 	size_t const zt = (size_t)s->zvsize*s->zvsize, edge = (size_t)s->zvsize*sizeof(float);
 	std::vector<void *> fresh; // zvals, then smask / sh_out_x / sh_out_y of every slot
@@ -108,15 +109,220 @@ int grow(tw_tile_set *s, uint32_t need) {
 		tw_tile_set::slot_t &S = s->L[l];
 		cudaFree(S.d_m); cudaFree(S.d_ox); cudaFree(S.d_oy);
 		S.d_m = (unsigned char *)fresh[1 + 3*l]; S.d_ox = (float *)fresh[2 + 3*l]; S.d_oy = (float *)fresh[3 + 3*l];
-		S.valid.resize(cap, 0);
+		s->st.valid[l].resize(cap, 0);
 	}
 	s->capacity = cap;
 	return TW_OK;
 }
 
-void slot_signs(tw_tile_set::slot_t const &S, int &sx, int &sy) {
-	sx = S.have ? twts::light_sign(S.sp.lpos[0]) : 1; sy = S.have ? twts::light_sign(S.sp.lpos[1]) : 1;
+std::vector<twts::signs> slot_signs(const tw_tile_set *s) {
+	std::vector<twts::signs> sg(s->nlights);
+	for (uint32_t l = 0; l < s->nlights; ++l) {
+		tw_tile_set::slot_t const &S = s->L[l];
+		sg[l].sx = S.have ? twts::light_sign(S.sp.lpos[0]) : 1; sg[l].sy = S.have ? twts::light_sign(S.sp.lpos[1]) : 1;
+	}
+	return sg;
 }
+
+// per asked light: the slot's params differ from sps[l] (or it has none), so a relight recomputes all of it
+std::vector<uint8_t> slot_resets(const tw_tile_set *s, const tw_shadow_params *sps, uint32_t nlights) {
+	std::vector<uint8_t> reset(nlights);
+	for (uint32_t l = 0; l < nlights; ++l) {reset[l] = !s->L[l].have || memcmp(&s->L[l].sp, &sps[l], sizeof(tw_shadow_params)) != 0;}
+	return reset;
+}
+
+// the removes and puts of a frame (tw_tile_set_create_tiles_launch, tw_tile_set_stale_after): each list names a tile once, every removed tile is resident and
+// no tile is both removed and put
+int frame_keys(tw_ctx *ctx, const tw_tile_set *s, const int32_t *remove_xy, uint32_t nremove, const int32_t *put_xy, uint32_t nput,
+               std::vector<twts::key> &rk, std::vector<twts::key> &pk) {
+	if ((nremove && !remove_xy) || (nput && !put_xy)) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: null remove_xy or tile_xy with a count > 0");
+	if (!read_keys(remove_xy, nremove, rk)) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: remove_xy names a tile twice");
+	for (twts::key const &k : rk) {if (!s->st.where.count(k)) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: removed tile (%d, %d) is not resident", k.first, k.second);}
+	if (!read_keys(put_xy, nput, pk)) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: tile_xy names a tile twice");
+	std::vector<twts::key> sorted(rk);
+	std::sort(sorted.begin(), sorted.end());
+	for (twts::key const &k : pk) {
+		if (std::binary_search(sorted.begin(), sorted.end(), k)) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: tile (%d, %d) is both removed and put", k.first, k.second);
+	}
+	return TW_OK;
+}
+
+// A relight planned on the host against a set state: per light the batch B (invalid requested tiles + their invalid upstream closure), its plan, and the
+// slab slots it reads and writes. Its scratch is [B's zvals | mask | 64-bit keys | x edges (outputs, then caller rows) | y edges | host-bound output staging |
+// int region], the int region ([requested tiles' slots | per light: plan, B's slots, x and y caller-row sources]) staged in pinned memory.
+struct relight_t {
+	struct batch_t {
+		bool reset = false;                      // the slot's params differ: every tile of it is invalid
+		std::vector<twts::key> B;
+		twi_shadow_plan P;
+		std::vector<int> ints;                   // [plan (3*nB) | B's slots | x caller-row sources | y caller-row sources]
+		size_t off_ints = 0, off_out = 0;        // byte offsets into the int region / the output staging
+	};
+	uint32_t n = 0, nl = 0;
+	std::vector<tw_tile_set_light> lights;
+	std::vector<int> req_slot;
+	std::vector<char> dev_m, dev_x, dev_y;
+	std::vector<batch_t> jobs;
+	size_t zb = 0, mb = 0, kb = 0, fb = 0, off_out = 0, off_ints = 0, ints_bytes = 0;
+	size_t dev_bytes() const {return off_ints + ints_bytes;}
+};
+
+// validates req against st (TW_ERR_ARG on ctx; nothing changes) and plans it
+int relight_plan(tw_ctx *ctx, const tw_tile_set *s, twts::state const &st, const tw_tile_set_request *req, relight_t &R) {
+	if (!req || !req->tile_xy || req->n == 0 || !req->lights || req->nlights == 0 || req->nlights > s->nlights)
+		return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: needs tile_xy, n >= 1 and 1 .. %u lights", s->nlights);
+	uint32_t const n = req->n, nl = req->nlights, zv = s->zvsize;
+	size_t const zt = (size_t)zv*zv, eb = (size_t)zv*sizeof(float);
+	R.n = n; R.nl = nl;
+	R.lights.assign(req->lights, req->lights + nl);
+	std::vector<twts::key> keys;
+	if (!read_keys(req->tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: tile_xy names a tile twice");
+	R.req_slot.resize(n);
+	for (uint32_t i = 0; i < n; ++i) {
+		auto const it = st.where.find(keys[i]);
+		if (it == st.where.end()) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: tile (%d, %d) is not resident", keys[i].first, keys[i].second);
+		R.req_slot[i] = (int)it->second;
+	}
+	R.dev_m.assign(nl, 0); R.dev_x.assign(nl, 0); R.dev_y.assign(nl, 0);
+	for (uint32_t l = 0; l < nl; ++l) {
+		tw_tile_set_light const &Lr = R.lights[l];
+		if (!Lr.smask) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: light %u has no smask", l);
+		R.dev_m[l] = tw_is_device_ptr(Lr.smask);
+		if (R.dev_m[l] && ((size_t)Lr.smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: light %u: a device smask must be 4-byte aligned", l);
+		R.dev_x[l] = Lr.sh_out_x && tw_is_device_ptr(Lr.sh_out_x); R.dev_y[l] = Lr.sh_out_y && tw_is_device_ptr(Lr.sh_out_y);
+	}
+	R.jobs.resize(nl);
+	uint32_t maxB = 0;
+	size_t ints_bytes = al(n*sizeof(int)), out_bytes = 0;    // the int region starts with the requested tiles' slots
+	for (uint32_t l = 0; l < nl; ++l) {
+		tw_tile_set::slot_t const &S = s->L[l];
+		relight_t::batch_t &J = R.jobs[l];
+		tw_shadow_params const &sp = R.lights[l].sp;
+		J.reset = !S.have || memcmp(&S.sp, &sp, sizeof(sp)) != 0;
+		int const sx = twts::light_sign(sp.lpos[0]), sy = twts::light_sign(sp.lpos[1]);
+		std::vector<uint8_t> const none(J.reset ? st.valid[l].size() : 0, 0);
+		std::vector<uint8_t> const &valid = J.reset ? none : st.valid[l];
+		J.B = twts::recompute_batch(st.where, valid, keys, sx, sy);
+		uint32_t const nB = (uint32_t)J.B.size();
+		maxB = std::max(maxB, nB);
+		if (nB) {
+			std::vector<int32_t> bxy(2*(size_t)nB);
+			for (uint32_t t = 0; t < nB; ++t) {bxy[2*t] = J.B[t].first; bxy[2*t+1] = J.B[t].second;}
+			twi_shadow_plan_make(bxy.data(), nB, &sp, true, true, &J.P);
+			J.ints.resize(twi_shadow_plan_ints(nB) + 3*(size_t)nB);
+			twi_shadow_plan_pack(J.P, J.ints.data());
+			int *bs = J.ints.data() + twi_shadow_plan_ints(nB), *rx = bs + nB, *ry = rx + nB;
+			auto cached = [&](twts::key const &k) {auto const it = st.where.find(k); return (it != st.where.end() && valid[it->second]) ? (int)it->second : -1;};
+			for (uint32_t t = 0; t < nB; ++t) {
+				bs[t] = (int)st.where.find(J.B[t])->second;
+				rx[t] = cached(twts::key(J.B[t].first, J.B[t].second + sy)); // sh_in_x row: the sh_out_x of (tx, ty + sy); not resident -> MESH_MIN_Z
+				ry[t] = cached(twts::key(J.B[t].first + sx, J.B[t].second)); // sh_in_y row: the sh_out_y of (tx + sx, ty)
+			}
+		}
+		J.off_ints = ints_bytes; ints_bytes += al(J.ints.size()*sizeof(int));
+		J.off_out = out_bytes;
+		out_bytes += (R.dev_m[l] ? 0 : al(n*zt)) + ((R.lights[l].sh_out_x && !R.dev_x[l]) ? al(n*eb) : 0) + ((R.lights[l].sh_out_y && !R.dev_y[l]) ? al(n*eb) : 0);
+	}
+	R.zb = al((size_t)maxB*zt*sizeof(float)); R.mb = al((size_t)maxB*zt + 4); R.kb = al(2*(size_t)maxB*eb*2); R.fb = al(2*(size_t)maxB*eb);
+	R.off_out = R.zb + R.mb + R.kb + 2*R.fb; R.off_ints = R.off_out + out_bytes; R.ints_bytes = ints_bytes;
+	return TW_OK;
+}
+
+// Enqueues R on ctx->stream into R.dev_bytes() of device scratch at d, its int region staged at h (R.ints_bytes of pinned memory that stays untouched until the
+// work is done); records the set's event once the slabs are no longer read or written, then copies the host outputs. The caller has made the stream wait on the
+// set's event.
+int relight_enqueue(tw_ctx *ctx, tw_tile_set *s, relight_t const &R, char *d, char *h) {
+	uint32_t const n = R.n, zv = s->zvsize;
+	size_t const zt = (size_t)zv*zv, eb = (size_t)zv*sizeof(float);
+	float *d_zB = (float *)d;
+	unsigned char *d_mB = (unsigned char *)(d + R.zb);
+	unsigned long long *d_keys = (unsigned long long *)(d + R.zb + R.mb);
+	float *d_ox = (float *)(d + R.zb + R.mb + R.kb), *d_oy = (float *)(d + R.zb + R.mb + R.kb + R.fb);
+	char *d_ints = d + R.off_ints;
+	memcpy(h, R.req_slot.data(), n*sizeof(int));
+	for (relight_t::batch_t const &J : R.jobs) {memcpy(h + J.off_ints, J.ints.data(), J.ints.size()*sizeof(int));}
+	uint32_t minz_bits; {float const m = TW_MESH_MIN_Z; memcpy(&minz_bits, &m, 4);}
+	TW_CUDA(ctx, cudaMemcpyAsync(d_ints, h, R.ints_bytes, cudaMemcpyHostToDevice, ctx->stream));
+	const int *d_req = (const int *)d_ints;
+	for (uint32_t l = 0; l < R.nl; ++l) {
+		tw_tile_set::slot_t &S = s->L[l];
+		relight_t::batch_t const &J = R.jobs[l];
+		uint32_t const nB = (uint32_t)J.B.size();
+		tw_tile_set_light const &Lr = R.lights[l];
+		if (nB) {
+			const int *d_plan = (const int *)(d_ints + J.off_ints), *d_bs = d_plan + twi_shadow_plan_ints(nB), *d_rx = d_bs + nB, *d_ry = d_rx + nB;
+			int r = copy_tiles(ctx, d_zB, nullptr, s->d_z, d_bs, zt*sizeof(float), nB); if (r) return r;            // B's zvals
+			r = copy_tiles(ctx, d_ox + (size_t)nB*zv, nullptr, S.d_ox, d_rx, eb, nB, minz_bits); if (r) return r;  // caller rows: cached sh_out of valid neighbours
+			r = copy_tiles(ctx, d_oy + (size_t)nB*zv, nullptr, S.d_oy, d_ry, eb, nB, minz_bits); if (r) return r;
+			r = twi_shadow_enqueue(ctx, ctx->stream, J.P, d_zB, nB, zv, d_mB, d_keys, d_ox, d_oy, d_plan, true); if (r) return r;
+			r = copy_tiles(ctx, S.d_m, d_bs, d_mB, nullptr, zt, nB); if (r) return r;                                 // results into the slot
+			r = copy_tiles(ctx, S.d_ox, d_bs, d_ox, nullptr, eb, nB); if (r) return r;
+			r = copy_tiles(ctx, S.d_oy, d_bs, d_oy, nullptr, eb, nB); if (r) return r;
+		}
+		char *st = d + R.off_out + J.off_out; // the requested tiles' outputs, in request order
+		unsigned char *om = R.dev_m[l] ? Lr.smask : (unsigned char *)st; st += R.dev_m[l] ? 0 : al(n*zt);
+		float *ox = !Lr.sh_out_x ? nullptr : (R.dev_x[l] ? Lr.sh_out_x : (float *)st); st += (Lr.sh_out_x && !R.dev_x[l]) ? al(n*eb) : 0;
+		float *oy = !Lr.sh_out_y ? nullptr : (R.dev_y[l] ? Lr.sh_out_y : (float *)st);
+		int r = copy_tiles(ctx, om, nullptr, S.d_m, d_req, zt, n); if (r) return r;
+		if (ox) {r = copy_tiles(ctx, ox, nullptr, S.d_ox, d_req, eb, n); if (r) return r;}
+		if (oy) {r = copy_tiles(ctx, oy, nullptr, S.d_oy, d_req, eb, n); if (r) return r;}
+	}
+	TW_CUDA(ctx, cudaEventRecord(s->ev, ctx->stream));
+	for (uint32_t l = 0; l < R.nl; ++l) { // host outputs: one copy each, at the end
+		tw_tile_set_light const &Lr = R.lights[l];
+		char *st = d + R.off_out + R.jobs[l].off_out;
+		if (!R.dev_m[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.smask, st, n*zt, cudaMemcpyDeviceToHost, ctx->stream)); st += al(n*zt);}
+		if (Lr.sh_out_x && !R.dev_x[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_x, st, n*eb, cudaMemcpyDeviceToHost, ctx->stream)); st += al(n*eb);}
+		if (Lr.sh_out_y && !R.dev_y[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_y, st, n*eb, cudaMemcpyDeviceToHost, ctx->stream));}
+	}
+	return TW_OK;
+}
+
+// after an enqueued relight: each slot holds the request's params, and B is valid in it
+void relight_commit(tw_tile_set *s, relight_t const &R, uint8_t *recomputed) {
+	std::vector<uint8_t> computed(s->capacity, 0);
+	for (uint32_t l = 0; l < R.nl; ++l) {
+		tw_tile_set::slot_t &S = s->L[l];
+		relight_t::batch_t const &J = R.jobs[l];
+		std::vector<uint8_t> &valid = s->st.valid[l];
+		if (J.reset) {std::fill(valid.begin(), valid.end(), 0);}
+		S.have = true; S.sp = R.lights[l].sp;
+		for (twts::key const &k : J.B) {uint32_t const slot = s->st.where.find(k)->second; valid[slot] = 1; computed[slot] = 1;}
+	}
+	if (recomputed) {for (uint32_t i = 0; i < R.n; ++i) {recomputed[i] = computed[R.req_slot[i]];}}
+}
+
+void invalidate_all(tw_tile_set *s) { // what the slots hold is unknown: everything is recomputed next time
+	for (uint32_t l = 0; l < s->nlights; ++l) {s->L[l].have = false; std::fill(s->st.valid[l].begin(), s->st.valid[l].end(), 0);}
+}
+
+// The set's part of a frame's tile job: prepare grows the slabs before the job enqueues anything; enqueue, after the chunk join, waits for the set's earlier
+// device work, scatters the job's zvals into the put tiles' slots and runs the relight (or records the set's event itself).
+struct frame_tail : twi_job_tail {
+	tw_tile_set *s = nullptr;
+	twts::state post;                // the set's host state after the frame's removes and puts
+	std::vector<int> idx;            // the put tiles' slab slots, in tile_xy order
+	uint32_t ntiles = 0;
+	size_t idx_bytes = 0;
+	bool relight = false;
+	relight_t R;
+	int prepare(tw_ctx *ctx) override {return grow(s, post.used, ctx);}
+	// once this starts the slabs may be partly written, so every failure from here on is reported as TW_ERR_CUDA (the code that selects the error state)
+	int enqueue(tw_ctx *ctx, const float *d_zvals, char *d, char *h) override {
+		int const rc = enqueue_tail(ctx, d_zvals, d, h);
+		return (rc && rc != TW_ERR_CUDA) ? TW_ERR_CUDA : rc;
+	}
+	int enqueue_tail(tw_ctx *ctx, const float *d_zvals, char *d, char *h) {
+		memcpy(h, idx.data(), ntiles*sizeof(int));
+		int *d_idx = (int *)d;
+		TW_CUDA(ctx, cudaMemcpyAsync(d_idx, h, ntiles*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+		TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0));
+		int rc = copy_tiles(ctx, s->d_z, d_idx, d_zvals, nullptr, (size_t)s->zvsize*s->zvsize*sizeof(float), ntiles); if (rc) return rc;
+		if (relight) return relight_enqueue(ctx, s, R, d + idx_bytes, h + idx_bytes);
+		TW_CUDA(ctx, cudaEventRecord(s->ev, ctx->stream));
+		return TW_OK;
+	}
+};
 
 } // namespace
 
@@ -129,7 +335,10 @@ int tw_tile_set_create(tw_ctx *ctx, uint32_t zvsize, uint32_t nlights, tw_tile_s
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
 	tw_tile_set *s = new (std::nothrow) tw_tile_set();
 	if (!s) return tw_set_error(ctx, TW_ERR_CUDA, "tile set: out of host memory");
-	try {s->L.resize(nlights); ctx->sets.push_back(s);} catch (...) {delete s; return tw_set_error(ctx, TW_ERR_CUDA, "tile set: out of host memory");}
+	try {s->L.resize(nlights); s->st.valid.resize(nlights);} catch (...) {delete s; return tw_set_error(ctx, TW_ERR_CUDA, "tile set: out of host memory");}
+	cudaError_t const e = cudaEventCreateWithFlags(&s->ev, cudaEventDisableTiming);
+	if (e != cudaSuccess) {delete s; return tw_set_error(ctx, TW_ERR_CUDA, "tile set: event: %s", cudaGetErrorString(e));}
+	try {ctx->sets.push_back(s);} catch (...) {cudaEventDestroy(s->ev); delete s; return tw_set_error(ctx, TW_ERR_CUDA, "tile set: out of host memory");}
 	s->ctx = ctx; s->zvsize = zvsize; s->nlights = nlights;
 	*out = s;
 	return TW_OK;
@@ -140,7 +349,9 @@ void tw_tile_set_destroy(tw_tile_set *s) {
 	tw_ctx *ctx = s->ctx;
 	cudaSetDevice(ctx->device);
 	twi_finish_pending(ctx); // a relight may still read the slabs
+	cudaEventSynchronize(s->ev); // and so may a frame's job on another context of the family
 	cudaStreamSynchronize(ctx->stream);
+	cudaEventDestroy(s->ev);
 	cudaFree(s->d_z);
 	for (tw_tile_set::slot_t &S : s->L) {cudaFree(S.d_m); cudaFree(S.d_ox); cudaFree(S.d_oy);}
 	ctx->sets.erase(std::find(ctx->sets.begin(), ctx->sets.end(), s));
@@ -154,17 +365,10 @@ int tw_tile_set_put(tw_tile_set *s, const int32_t *tile_xy, uint32_t n, const fl
 	std::vector<twts::key> keys;
 	if (!read_keys(tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set put: tile_xy names a tile twice");
 	int rc = begin_call(s); if (rc) return rc;
-	// slots: a resident tile keeps its own, new tiles take freed slots first, then fresh ones
-	std::vector<uint32_t> free_left(s->free_slots);
-	uint32_t next = s->used;
-	std::vector<int> idx(n);
-	for (uint32_t i = 0; i < n; ++i) {
-		auto const it = s->where.find(keys[i]);
-		if (it != s->where.end()) {idx[i] = (int)it->second;}
-		else if (!free_left.empty()) {idx[i] = (int)free_left.back(); free_left.pop_back();}
-		else {idx[i] = (int)next++;}
-	}
-	rc = grow(s, next); if (rc) return rc;
+	std::vector<uint32_t> free_left;
+	std::vector<int> idx;
+	uint32_t const next = twts::put_slots(s->st, keys, free_left, idx);
+	rc = grow(s, next, ctx); if (rc) return rc;
 	size_t const tb = (size_t)s->zvsize*s->zvsize*sizeof(float);
 	bool const dev = tw_is_device_ptr(zvals);
 	size_t const zb = dev ? 0 : al(n*tb);
@@ -173,15 +377,11 @@ int tw_tile_set_put(tw_tile_set *s, const int32_t *tile_xy, uint32_t n, const fl
 	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(p, zvals, n*tb, cudaMemcpyHostToDevice, ctx->stream));}
 	int *d_idx = (int *)(p + zb);
 	TW_CUDA(ctx, cudaMemcpyAsync(d_idx, idx.data(), n*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+	TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0)); // a frame's job on another context may still read these slots
 	rc = copy_tiles(ctx, s->d_z, d_idx, dev ? (const void *)zvals : (const void *)p, nullptr, tb, n); if (rc) return rc;
+	TW_CUDA(ctx, cudaEventRecord(s->ev, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // zvals (and idx) have been read
-	// commit: the new tiles are resident; each put tile and its downstream closure are invalid in every slot
-	for (uint32_t i = 0; i < n; ++i) {s->where.emplace(keys[i], (uint32_t)idx[i]);}
-	s->free_slots.swap(free_left); s->used = next;
-	for (tw_tile_set::slot_t &S : s->L) {
-		int sx, sy; slot_signs(S, sx, sy);
-		twts::invalidate_downstream(s->where, keys, sx, sy, S.valid);
-	}
+	twts::put_tiles(s->st, keys, idx, free_left, next, slot_signs(s));
 	return TW_OK;
 }
 
@@ -191,20 +391,10 @@ int tw_tile_set_remove(tw_tile_set *s, const int32_t *tile_xy, uint32_t n) {
 	if (!tile_xy || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "tile set remove: null or empty argument");
 	std::vector<twts::key> keys;
 	if (!read_keys(tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set remove: tile_xy names a tile twice");
-	for (twts::key const &k : keys) {if (!s->where.count(k)) return tw_set_error(ctx, TW_ERR_ARG, "tile set remove: tile (%d, %d) is not resident", k.first, k.second);}
+	for (twts::key const &k : keys) {if (!s->st.where.count(k)) return tw_set_error(ctx, TW_ERR_ARG, "tile set remove: tile (%d, %d) is not resident", k.first, k.second);}
 	int rc = begin_call(s); if (rc) return rc;
-	for (twts::key const &k : keys) {
-		uint32_t const slot = s->where[k];
-		s->where.erase(k);
-		s->free_slots.push_back(slot);
-		for (tw_tile_set::slot_t &S : s->L) {S.valid[slot] = 0;}
-	}
-	for (tw_tile_set::slot_t &S : s->L) { // the removed tiles' downstream neighbours lose an incoming row
-		int sx, sy; slot_signs(S, sx, sy);
-		std::vector<twts::key> seeds;
-		for (twts::key const &k : keys) {seeds.push_back(twts::key(k.first - sx, k.second)); seeds.push_back(twts::key(k.first, k.second - sy));}
-		twts::invalidate_downstream(s->where, seeds, sx, sy, S.valid);
-	}
+	// host state only: the next writer of a freed slot waits on the set's event
+	twts::remove_tiles(s->st, keys, slot_signs(s));
 	return TW_OK;
 }
 
@@ -212,157 +402,96 @@ int tw_tile_set_stale(tw_tile_set *s, const tw_shadow_params *sps, uint32_t nlig
 	if (!s) return TW_ERR_ARG;
 	if (!sps || !nstale || nlights == 0 || nlights > s->nlights || (capacity && !tile_xy_out))
 		return tw_set_error(s->ctx, TW_ERR_ARG, "tile set stale: needs sps, nstale, 1 .. %u lights and tile_xy_out when capacity > 0", s->nlights);
-	uint32_t count = 0;
-	for (auto const &kv : s->where) { // a relight of every resident tile recomputes exactly the invalid ones (their upstream closure is invalid too)
-		bool stale = false;
-		for (uint32_t l = 0; l < nlights && !stale; ++l) {
-			tw_tile_set::slot_t const &S = s->L[l];
-			stale = !S.have || memcmp(&S.sp, &sps[l], sizeof(tw_shadow_params)) != 0 || !S.valid[kv.second];
-		}
-		if (!stale) continue;
-		if (count < capacity) {tile_xy_out[2*count] = kv.first.first; tile_xy_out[2*count+1] = kv.first.second;}
-		++count;
-	}
-	*nstale = count;
+	std::vector<twts::key> const stale = twts::stale_tiles(s->st, slot_resets(s, sps, nlights));
+	for (size_t i = 0; i < stale.size() && i < capacity; ++i) {tile_xy_out[2*i] = stale[i].first; tile_xy_out[2*i+1] = stale[i].second;}
+	*nstale = (uint32_t)stale.size();
+	return TW_OK;
+}
+
+int tw_tile_set_stale_after(tw_tile_set *s, const tw_shadow_params *sps, uint32_t nlights, const int32_t *remove_xy, uint32_t nremove, const int32_t *put_xy,
+                            uint32_t nput, int32_t *tile_xy_out, uint32_t capacity, uint32_t *nstale) {
+	if (!s) return TW_ERR_ARG;
+	if (!sps || !nstale || nlights == 0 || nlights > s->nlights || (capacity && !tile_xy_out))
+		return tw_set_error(s->ctx, TW_ERR_ARG, "tile set stale_after: needs sps, nstale, 1 .. %u lights and tile_xy_out when capacity > 0", s->nlights);
+	std::vector<twts::key> rk, pk;
+	int const rc = frame_keys(s->ctx, s, remove_xy, nremove, put_xy, nput, rk, pk); if (rc) return rc;
+	std::vector<twts::key> const stale = twts::stale_after(s->st, rk, pk, slot_signs(s), slot_resets(s, sps, nlights));
+	for (size_t i = 0; i < stale.size() && i < capacity; ++i) {tile_xy_out[2*i] = stale[i].first; tile_xy_out[2*i+1] = stale[i].second;}
+	*nstale = (uint32_t)stale.size();
 	return TW_OK;
 }
 
 int tw_tile_set_shadows_launch(tw_tile_set *s, const tw_tile_set_request *req) {
 	if (!s) return TW_ERR_ARG;
 	tw_ctx *ctx = s->ctx;
-	if (!req || !req->tile_xy || req->n == 0 || !req->lights || req->nlights == 0 || req->nlights > s->nlights)
-		return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: needs tile_xy, n >= 1 and 1 .. %u lights", s->nlights);
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	uint32_t const n = req->n, nl = req->nlights, zv = s->zvsize;
-	size_t const zt = (size_t)zv*zv, eb = (size_t)zv*sizeof(float);
-	std::vector<tw_tile_set_light> const lights(req->lights, req->lights + nl);
-	std::vector<twts::key> keys;
-	if (!read_keys(req->tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: tile_xy names a tile twice");
-	std::vector<int> req_slot(n);
-	for (uint32_t i = 0; i < n; ++i) {
-		auto const it = s->where.find(keys[i]);
-		if (it == s->where.end()) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: tile (%d, %d) is not resident", keys[i].first, keys[i].second);
-		req_slot[i] = (int)it->second;
-	}
-	std::vector<char> dev_m(nl), dev_x(nl), dev_y(nl);
-	for (uint32_t l = 0; l < nl; ++l) {
-		tw_tile_set_light const &Lr = lights[l];
-		if (!Lr.smask) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: light %u has no smask", l);
-		dev_m[l] = tw_is_device_ptr(Lr.smask);
-		if (dev_m[l] && ((size_t)Lr.smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: light %u: a device smask must be 4-byte aligned", l);
-		dev_x[l] = Lr.sh_out_x && tw_is_device_ptr(Lr.sh_out_x); dev_y[l] = Lr.sh_out_y && tw_is_device_ptr(Lr.sh_out_y);
-	}
-	int rc = twi_finish_pending(ctx); if (rc) return rc;
-	// per light: the batch B (invalid requested tiles + their invalid upstream closure), its plan, and the slab slots it reads and writes
-	struct batch_t {
-		bool reset = false;                      // the slot's params differ: every tile of it is invalid
-		std::vector<twts::key> B;
-		twi_shadow_plan P;
-		std::vector<int> ints;                   // [plan (3*nB) | B's slots | x caller-row sources | y caller-row sources]
-		size_t off_ints = 0, off_out = 0;        // byte offsets into the int region / the output staging
-	};
-	std::vector<batch_t> jobs(nl);
-	uint32_t maxB = 0;
-	size_t ints_bytes = al(n*sizeof(int)), out_bytes = 0;    // the int region starts with the requested tiles' slots
-	for (uint32_t l = 0; l < nl; ++l) {
-		tw_tile_set::slot_t const &S = s->L[l];
-		batch_t &J = jobs[l];
-		tw_shadow_params const &sp = lights[l].sp;
-		J.reset = !S.have || memcmp(&S.sp, &sp, sizeof(sp)) != 0;
-		int const sx = twts::light_sign(sp.lpos[0]), sy = twts::light_sign(sp.lpos[1]);
-		std::vector<uint8_t> const none(J.reset ? s->capacity : 0, 0);
-		std::vector<uint8_t> const &valid = J.reset ? none : S.valid;
-		J.B = twts::recompute_batch(s->where, valid, keys, sx, sy);
-		uint32_t const nB = (uint32_t)J.B.size();
-		maxB = std::max(maxB, nB);
-		if (nB) {
-			std::vector<int32_t> bxy(2*(size_t)nB);
-			for (uint32_t t = 0; t < nB; ++t) {bxy[2*t] = J.B[t].first; bxy[2*t+1] = J.B[t].second;}
-			twi_shadow_plan_make(bxy.data(), nB, &sp, true, true, &J.P);
-			J.ints.resize(twi_shadow_plan_ints(nB) + 3*(size_t)nB);
-			twi_shadow_plan_pack(J.P, J.ints.data());
-			int *bs = J.ints.data() + twi_shadow_plan_ints(nB), *rx = bs + nB, *ry = rx + nB;
-			auto cached = [&](twts::key const &k) {auto const it = s->where.find(k); return (it != s->where.end() && valid[it->second]) ? (int)it->second : -1;};
-			for (uint32_t t = 0; t < nB; ++t) {
-				bs[t] = (int)s->where.find(J.B[t])->second;
-				rx[t] = cached(twts::key(J.B[t].first, J.B[t].second + sy)); // sh_in_x row: the sh_out_x of (tx, ty + sy); not resident -> MESH_MIN_Z
-				ry[t] = cached(twts::key(J.B[t].first + sx, J.B[t].second)); // sh_in_y row: the sh_out_y of (tx + sx, ty)
-			}
-		}
-		J.off_ints = ints_bytes; ints_bytes += al(J.ints.size()*sizeof(int));
-		J.off_out = out_bytes;
-		out_bytes += (dev_m[l] ? 0 : al(n*zt)) + ((lights[l].sh_out_x && !dev_x[l]) ? al(n*eb) : 0) + ((lights[l].sh_out_y && !dev_y[l]) ? al(n*eb) : 0);
-	}
-	// everything is reserved before anything is enqueued (tw_reserve synchronises the stream and may re-allocate): slot 0 = [B's zvals | mask | 64-bit keys |
-	// x edges (outputs, then caller rows) | y edges | host-bound output staging | int region], the int region staged in pinned memory
-	size_t const zb = al((size_t)maxB*zt*sizeof(float)), mb = al((size_t)maxB*zt + 4), kb = al(2*(size_t)maxB*eb*2), fb = al(2*(size_t)maxB*eb);
-	size_t const off_out = zb + mb + kb + 2*fb, off_ints = off_out + out_bytes;
-	rc = tw_reserve(ctx, 0, off_ints + ints_bytes); if (rc) return rc;
-	rc = tw_reserve_pinned(ctx, ints_bytes); if (rc) return rc;
-	char *const s0 = (char *)ctx->d_scratch[0], *const h = (char *)ctx->h_pinned;
-	float *d_zB = (float *)s0;
-	unsigned char *d_mB = (unsigned char *)(s0 + zb);
-	unsigned long long *d_keys = (unsigned long long *)(s0 + zb + mb);
-	float *d_ox = (float *)(s0 + zb + mb + kb), *d_oy = (float *)(s0 + zb + mb + kb + fb);
-	char *d_ints = s0 + off_ints;
-	memcpy(h, req_slot.data(), n*sizeof(int));
-	for (batch_t const &J : jobs) {memcpy(h + J.off_ints, J.ints.data(), J.ints.size()*sizeof(int));}
-	uint32_t minz_bits; {float const m = TW_MESH_MIN_Z; memcpy(&minz_bits, &m, 4);}
+	relight_t R;
+	int rc = relight_plan(ctx, s, s->st, req, R); if (rc) return rc;
+	rc = twi_finish_pending(ctx); if (rc) return rc;
+	// everything is reserved before anything is enqueued (tw_reserve synchronises the stream and may re-allocate)
+	rc = tw_reserve(ctx, 0, R.dev_bytes()); if (rc) return rc;
+	rc = tw_reserve_pinned(ctx, R.ints_bytes); if (rc) return rc;
 	auto enqueue = [&]() -> int {
-		TW_CUDA(ctx, cudaMemcpyAsync(d_ints, h, ints_bytes, cudaMemcpyHostToDevice, ctx->stream));
-		const int *d_req = (const int *)d_ints;
-		for (uint32_t l = 0; l < nl; ++l) {
-			tw_tile_set::slot_t &S = s->L[l];
-			batch_t const &J = jobs[l];
-			uint32_t const nB = (uint32_t)J.B.size();
-			tw_tile_set_light const &Lr = lights[l];
-			if (nB) {
-				const int *d_plan = (const int *)(d_ints + J.off_ints), *d_bs = d_plan + twi_shadow_plan_ints(nB), *d_rx = d_bs + nB, *d_ry = d_rx + nB;
-				int r = copy_tiles(ctx, d_zB, nullptr, s->d_z, d_bs, zt*sizeof(float), nB); if (r) return r;            // B's zvals
-				r = copy_tiles(ctx, d_ox + (size_t)nB*zv, nullptr, S.d_ox, d_rx, eb, nB, minz_bits); if (r) return r;  // caller rows: cached sh_out of valid neighbours
-				r = copy_tiles(ctx, d_oy + (size_t)nB*zv, nullptr, S.d_oy, d_ry, eb, nB, minz_bits); if (r) return r;
-				r = twi_shadow_enqueue(ctx, ctx->stream, J.P, d_zB, nB, zv, d_mB, d_keys, d_ox, d_oy, d_plan, true); if (r) return r;
-				r = copy_tiles(ctx, S.d_m, d_bs, d_mB, nullptr, zt, nB); if (r) return r;                                 // results into the slot
-				r = copy_tiles(ctx, S.d_ox, d_bs, d_ox, nullptr, eb, nB); if (r) return r;
-				r = copy_tiles(ctx, S.d_oy, d_bs, d_oy, nullptr, eb, nB); if (r) return r;
-			}
-			char *st = s0 + off_out + J.off_out; // the requested tiles' outputs, in request order
-			unsigned char *om = dev_m[l] ? Lr.smask : (unsigned char *)st; st += dev_m[l] ? 0 : al(n*zt);
-			float *ox = !Lr.sh_out_x ? nullptr : (dev_x[l] ? Lr.sh_out_x : (float *)st); st += (Lr.sh_out_x && !dev_x[l]) ? al(n*eb) : 0;
-			float *oy = !Lr.sh_out_y ? nullptr : (dev_y[l] ? Lr.sh_out_y : (float *)st);
-			int r = copy_tiles(ctx, om, nullptr, S.d_m, d_req, zt, n); if (r) return r;
-			if (ox) {r = copy_tiles(ctx, ox, nullptr, S.d_ox, d_req, eb, n); if (r) return r;}
-			if (oy) {r = copy_tiles(ctx, oy, nullptr, S.d_oy, d_req, eb, n); if (r) return r;}
-		}
-		for (uint32_t l = 0; l < nl; ++l) { // host outputs: one copy each, at the end
-			tw_tile_set_light const &Lr = lights[l];
-			char *st = s0 + off_out + jobs[l].off_out;
-			if (!dev_m[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.smask, st, n*zt, cudaMemcpyDeviceToHost, ctx->stream)); st += al(n*zt);}
-			if (Lr.sh_out_x && !dev_x[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_x, st, n*eb, cudaMemcpyDeviceToHost, ctx->stream)); st += al(n*eb);}
-			if (Lr.sh_out_y && !dev_y[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_y, st, n*eb, cudaMemcpyDeviceToHost, ctx->stream));}
-		}
+		TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0)); // a frame's job on another context may still use the slabs
+		int const r = relight_enqueue(ctx, s, R, (char *)ctx->d_scratch[0], (char *)ctx->h_pinned); if (r) return r;
 		TW_CUDA(ctx, cudaEventRecord(ctx->async.done, ctx->stream));
 		return TW_OK;
 	};
 	rc = enqueue();
 	if (rc) { // nothing may still run on the scratch; what the slots hold is unknown now, so they are recomputed next time
 		cudaStreamSynchronize(ctx->stream);
-		for (tw_tile_set::slot_t &S : s->L) {S.have = false; std::fill(S.valid.begin(), S.valid.end(), 0);}
+		invalidate_all(s);
 		return rc;
 	}
-	// commit: each slot holds this request's params, and B is valid in it
-	std::vector<uint8_t> computed(s->capacity, 0);
-	for (uint32_t l = 0; l < nl; ++l) {
-		tw_tile_set::slot_t &S = s->L[l];
-		batch_t const &J = jobs[l];
-		if (J.reset) {std::fill(S.valid.begin(), S.valid.end(), 0);}
-		S.have = true; S.sp = lights[l].sp;
-		for (twts::key const &k : J.B) {uint32_t const slot = s->where.find(k)->second; S.valid[slot] = 1; computed[slot] = 1;}
-	}
-	if (req->recomputed) {for (uint32_t i = 0; i < n; ++i) {req->recomputed[i] = computed[req_slot[i]];}}
+	relight_commit(s, R, req->recomputed);
 	tw_async_state &a = ctx->async;
 	a.pending = true; a.tiles = true; a.steps = false; a.n_mm = 0;
 	a.host_mm = nullptr; a.host_bounds = nullptr; a.host_min_nz = nullptr; a.host_flags = nullptr;
+	return TW_OK;
+}
+
+int tw_tile_set_create_tiles_launch(tw_ctx *ctx, tw_tile_set *s, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
+                                    const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
+                                    const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_set_frame *frame) {
+	if (!ctx || !s) return TW_ERR_ARG;
+	tw_ctx const *root = ctx->parent ? ctx->parent : ctx, *set_root = s->ctx->parent ? s->ctx->parent : s->ctx;
+	if (root != set_root || ctx->device != s->ctx->device) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: ctx is neither the set's context, its parent nor a shared context of that parent");
+	if (!frame || !frame->tile_xy) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: needs frame and frame->tile_xy");
+	if (frame->hs && shading && shading->ao) return tw_set_error(ctx, TW_ERR_ARG, "tile set frame: the AO map is not available for heightmap tiles");
+	frame_tail T;
+	T.s = s;
+	std::vector<twts::key> rk, pk;
+	int rc = frame_keys(ctx, s, frame->remove_xy, frame->nremove, frame->tile_xy, ntiles, rk, pk); if (rc) return rc;
+	// the state the sequential calls would leave: remove, then put (the job's zvals), then the relight planned against that
+	std::vector<twts::signs> const sg = slot_signs(s);
+	T.post = s->st;
+	if (!rk.empty()) twts::remove_tiles(T.post, rk, sg);
+	if (!pk.empty()) {
+		std::vector<uint32_t> free_left;
+		uint32_t const used = twts::put_slots(T.post, pk, free_left, T.idx);
+		twts::put_tiles(T.post, pk, T.idx, free_left, used, sg);
+	}
+	if (frame->relight) {rc = relight_plan(ctx, s, T.post, frame->relight, T.R); if (rc) return rc; T.relight = true;}
+	T.ntiles = ntiles; T.idx_bytes = al((size_t)ntiles*sizeof(int));
+	T.dev_bytes = T.idx_bytes + (T.relight ? T.R.dev_bytes() : 0);
+	T.pin_bytes = T.idx_bytes + (T.relight ? T.R.ints_bytes : 0);
+	tw_tile_outputs const none = {nullptr, nullptr, nullptr, nullptr, nullptr};
+	rc = twi_create_tiles_launch(ctx, frame->hs, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, s->zvsize, p, erosion_iters, ep, min_zval, wpz_max, size,
+	                             out ? out : &none, shading, &T);
+	if (rc) {
+		if (rc == TW_ERR_CUDA) { // what reached the slabs is unknown: the removes have happened, no put tile is resident, every slot is invalid
+			if (!rk.empty()) twts::remove_tiles(s->st, rk, sg);
+			std::vector<twts::key> dropped;
+			for (twts::key const &k : pk) {if (s->st.where.count(k)) dropped.push_back(k);}
+			if (!dropped.empty()) twts::remove_tiles(s->st, dropped, sg);
+			invalidate_all(s);
+		}
+		return rc;
+	}
+	// commit at launch: later launches plan against this state, and the set's event orders their device work after this job's
+	s->st = std::move(T.post);
+	for (uint32_t l = 0; l < s->nlights; ++l) {if (s->st.valid[l].size() < s->capacity) s->st.valid[l].resize(s->capacity, 0);}
+	if (T.relight) relight_commit(s, T.R, frame->relight->recomputed);
 	return TW_OK;
 }
 

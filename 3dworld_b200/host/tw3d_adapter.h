@@ -412,6 +412,7 @@ inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, un
 // A launch never waits for another slot's job. Create and use the pool on one thread, let it outlive the jobs it returned, and destroy it before the
 // thread ends (its contexts are shared contexts of the thread's context); destroying it completes its jobs.
 class tile_job_pool {
+	friend class tile_set; // its frame launches take a slot too
 	struct slot {tw_ctx *c = nullptr; std::atomic<uint64_t> jobs{0}; uint64_t launched = 0;};
 	std::vector<std::unique_ptr<slot>> slots; // stable addresses: a tiles_job keeps a pointer to its slot's launch count
 	uint64_t clock = 0;
@@ -563,6 +564,34 @@ public:
 		int const rc = tw_tile_set_shadows_launch(s, &req);
 		if (rc != TW_OK) {detail::fail(rc, "tile_set::relight_async", c);}
 		return tiles_job(c, &jobs, number);
+	}
+	// stale() as it would be after remove(remove_xy) and put(put_xy), without changing the set: the tiles a frame's relight should name
+	std::vector<int32_t> stale_after(const tw_shadow_params *sps, unsigned nlights, const int32_t *remove_xy, unsigned nremove, const int32_t *put_xy, unsigned nput) const {
+		uint32_t k = 0;
+		int rc = tw_tile_set_stale_after(s, sps, nlights, remove_xy, nremove, put_xy, nput, nullptr, 0, &k);
+		std::vector<int32_t> out(2*(size_t)k);
+		if (rc == TW_OK && k) {rc = tw_tile_set_stale_after(s, sps, nlights, remove_xy, nremove, put_xy, nput, out.data(), k, &k);}
+		if (rc != TW_OK) {detail::fail(rc, "tile_set::stale_after", c);}
+		return out;
+	}
+	// A frame in one job (tw_tile_set_create_tiles_launch): frame.remove_xy removed, the new tiles created as create_tiles_async() would (frame.hs: from the
+	// heightmap, as create_tiles_async_from_heightmap()) and put into the set at frame.tile_xy, and frame.relight relit - with no blocking put in between.
+	// out.zvals may be null (the zvals then stay in the set). Launched on this set's context, or on a slot of `pool` (shared contexts of the same thread's
+	// context) so that several frames are in flight at once; only their set-touching tails are ordered on the device. The returned job is ready once every
+	// output of the tile job and of the relight is complete.
+	tiles_job create_tiles_async(const int32_t *origins_xy, unsigned ntiles, float dx, float dy, unsigned erosion_iters_tt, float wpz_max, unsigned size,
+	                             tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_set_frame const &frame, tile_job_pool *pool = nullptr) {
+		scene_globals const &g = globals();
+		tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
+		tw_erosion_params const e = erosion_params_from_globals();
+		tw_ctx *lc = c;
+		std::atomic<uint64_t> *jobs = &detail::tls().tile_jobs;
+		if (pool) {tile_job_pool::slot &sl = pool->next(); lc = sl.c; jobs = &sl.jobs;}
+		uint64_t const number = ++*jobs;
+		int const rc = tw_tile_set_create_tiles_launch(lc, s, origins_xy, ntiles, g.MESH_X_SIZE, g.MESH_Y_SIZE, dx, dy, &p, erosion_iters_tt, &e, g.zmin, wpz_max, size,
+		                                               &out, &shading, &frame);
+		if (rc != TW_OK) {detail::fail(rc, "tile_set::create_tiles_async", lc);}
+		return tiles_job(lc, jobs, number);
 	}
 };
 

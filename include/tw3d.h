@@ -532,6 +532,43 @@ typedef struct tw_tile_set_request {
 /* Enqueues the relight and returns; tw_create_tiles_poll completes it. The request, its lights array and tile_xy are read during the launch. Errors return
  * TW_ERR_ARG before anything is enqueued or cached state changes. */
 TW_API int  tw_tile_set_shadows_launch(tw_tile_set *set, const tw_tile_set_request *req);
+/* A frame's new tiles created straight into a set and relit in the same asynchronous job - tile_draw_t::update's per-frame step in one launch:
+ *   tw_tile_set_create_tiles_launch(ctx, set, origins_xy, ntiles, ..., out, shading, frame) followed by its completing tw_create_tiles_poll(ctx) gives, bit for
+ *   bit, every output and the set state that this sequence gives on a set in the same state, on one context:
+ *     tw_tile_set_remove(frame->remove_xy) when nremove > 0; tw_create_tiles_launch_ex (frame->hs == NULL) or tw_create_tiles_launch_hmap(frame->hs) with the
+ *     same arguments and zvsize = the set's; a completing poll; tw_tile_set_put(frame->tile_xy, the job's zvals); tw_tile_set_shadows_launch(frame->relight)
+ *     when relight != NULL, and its poll.
+ *   That covers the job's outputs (zvals, mm, bounds, normals, min_normal_z, AO, weights, has_any_grass), the relight's (smask, sh_out_*, recomputed),
+ *   tw_last_erosion_steps() and what tw_tile_set_stale and later relights see. In GPU gen modes with AO the put zvals are the AO flow's, as documented for the job.
+ * Arguments: ctx is the set's context or any context of its family (the parent of a shared context, or a shared context of that parent): frames launched on
+ * several shared contexts are in flight at once. out and shading are optional, and out->zvals may be NULL (the zvals then live only in the set). The relight
+ * may name tiles this launch puts, not tiles it removes; its recomputed flags are filled before the launch returns.
+ * Ordering: the host-side set state (residency, slots, valid bits, light params) is committed at launch, in launch order. On the device, generation and erosion
+ * never wait for other frames; only the tail that touches the set's slabs (the zvals scatter into the slabs and the relight) waits on the set's event, the last
+ * device work on the slabs of any context, and records it again. tw_tile_set_put, tw_tile_set_shadows_launch and tw_tile_set_destroy wait on that event as well.
+ * Blocking: the launch returns without waiting for the device, except when the set needs larger slabs: it then first waits for every frame in flight on the
+ * set (they hold the old slab pointers) and copies the slabs. Size the set early (a first put or frame with every tile) to avoid it.
+ * Errors: the return code tells which state the set is in.
+ *   TW_ERR_ARG and TW_ERR_STATE: the set is unchanged. TW_ERR_ARG comes before anything is enqueued for every error of the job, of put, remove and the
+ *     relight request, a tile both removed and put, a tile_xy that names a tile twice, a ctx of another family or device, and hs together with shading->ao;
+ *     TW_ERR_STATE for the job's missing tables or heightmap image.
+ *   TW_ERR_CUDA (whether the launch failed, or completing the context's earlier job reported its failure): the set is left with the removes done, none of
+ *     tile_xy resident (a re-put tile is removed too) and every light slot invalid, so later relights recompute what is then resident and still equal the
+ *     full recompute. A failure after the set's slabs may have been written is always reported as TW_ERR_CUDA. */
+typedef struct tw_tile_set_frame {
+	const int32_t              *remove_xy;  /* optional: nremove resident tiles removed first, as tw_tile_set_remove */
+	uint32_t                    nremove;
+	const int32_t              *tile_xy;    /* required: (x1/size, y1/size) of each new tile, in origins_xy order */
+	const tw_hmap_sampler      *hs;         /* NULL: the height function p; else the context's heightmap image, as tw_create_tiles_launch_hmap */
+	const tw_tile_set_request  *relight;    /* optional: relight after the put, as tw_tile_set_shadows_launch */
+} tw_tile_set_frame;
+TW_API int  tw_tile_set_create_tiles_launch(tw_ctx *ctx, tw_tile_set *set, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size,
+                          float dx, float dy, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
+                          float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_set_frame *frame);
+/* Host only, changes nothing: what tw_tile_set_stale would return after tw_tile_set_remove(remove_xy) (nremove > 0) and tw_tile_set_put(put_xy) (nput > 0) - the
+ * tiles to name in a frame's relight request. TW_ERR_ARG for what stale, remove and put refuse, and a tile both removed and put. */
+TW_API int  tw_tile_set_stale_after(tw_tile_set *set, const tw_shadow_params *sps, uint32_t nlights, const int32_t *remove_xy, uint32_t nremove,
+                          const int32_t *put_xy, uint32_t nput, int32_t *tile_xy_out, uint32_t capacity, uint32_t *nstale);
 
 /* ---- terrain weights texture of tiles (SURVEY.md 8f row N4): tile_t::create_texture (src/tiled_mesh.cpp:1071-1248), the terrain part ----
  * RGBA texel (x, y) of a tile, x, y < stride = zvsize - 1: the weights {sand, dirt, grass, rock} (snow = the rest) of the ground textures from the cell's relative

@@ -296,12 +296,14 @@ extern "C" int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *ou
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside);
 	if (dev_o && ((size_t)outside & 3)) return tw_set_error(ctx, TW_ERR_ARG, "outside must be 4-byte aligned (flag bytes are claimed with 32-bit atomics)");
+	// the 32-bit word that holds the last flag byte reaches up to 3 bytes past a buffer of n % 4 != 0 bytes: such a device buffer is staged like a host one
+	bool const stage_o = !dev_o || (n & 3);
 	size_t const vb = (n*sizeof(float) + 255) & ~(size_t)255, ob = (n + 255 + 4) & ~(size_t)255, fb = ((n + 16)*sizeof(unsigned) + 255) & ~(size_t)255;
-	rc = tw_reserve(ctx, 0, (dev_v ? 0 : vb) + (dev_o ? 0 : ob) + 2*fb + 512); if (rc) return rc;
+	rc = tw_reserve(ctx, 0, (dev_v ? 0 : vb) + (stage_o ? ob : 0) + 2*fb + 512); if (rc) return rc;
 	char *sp = (char *)ctx->d_scratch[0];
 	float *d_v = vals; unsigned char *d_o = outside;
 	if (!dev_v) {d_v = (float *)sp; sp += vb; TW_CUDA(ctx, cudaMemcpyAsync(d_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (!dev_o) {d_o = (unsigned char *)sp; sp += ob; TW_CUDA(ctx, cudaMemcpyAsync(d_o, outside, n, cudaMemcpyHostToDevice, ctx->stream));}
+	if (stage_o) {d_o = (unsigned char *)sp; sp += ob; TW_CUDA(ctx, cudaMemcpyAsync(d_o, outside, n, dev_o ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));}
 	unsigned *f[2] = {(unsigned *)sp, (unsigned *)(sp + fb)}; sp += 2*fb;
 	unsigned *cnt = (unsigned *)sp;
 	unsigned long long *d_changed = (unsigned long long *)(sp + 64);
@@ -330,7 +332,7 @@ extern "C" int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *ou
 	unsigned long long hc = 0;
 	TW_CUDA(ctx, cudaMemcpyAsync(&hc, d_changed, sizeof(hc), cudaMemcpyDeviceToHost, ctx->stream));
 	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(vals, d_v, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
-	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(outside, d_o, n, cudaMemcpyDeviceToHost, ctx->stream));}
+	if (stage_o) {TW_CUDA(ctx, cudaMemcpyAsync(outside, d_o, n, dev_o ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	if (changed) *changed = hc;
 	return TW_OK;

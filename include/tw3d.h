@@ -403,8 +403,8 @@ TW_API int tw_voxel_outside(tw_ctx *ctx, const float *vals, const tw_voxel_post_
 /* remove_unconnected_outside (+ remove_interior_holes when remove_unconnected > 2), src/voxels.cpp:606-610,739-868: flood fill of the inside voxels from the
  * anchors (voxels under the mesh / the centre voxel / the scene-edge columns), every inside voxel not reached becomes outside (make_voxel_outside:
  * val = isolevel -+ TOLERANCE); then the outside space is flood-filled from the top plane and unreached pockets become inside. The set of reached voxels does
- * not depend on the fill order, so the result is identical to the reference's stack-based fill. vals / outside modified in place (host or device);
- * changed (optional) = number of voxels flipped. */
+ * not depend on the fill order, so the result is identical to the reference's stack-based fill. vals / outside modified in place (host or device;
+ * a device outside must be 4-byte aligned, and is worked on in a padded copy when nx*ny*nz is not a multiple of 4); changed (optional) = number of voxels flipped. */
 TW_API int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *outside, const tw_voxel_post_params *vp, uint64_t *changed);
 /* Marching cubes: voxel_manager::add_triangles_for_voxel at LOD 0 for every cube of the grid in the order of voxel_model::create_block (y, x, z),
  * src/voxels.cpp:485-566,1077-1108, as an UNWELDED triangle soup: tris[t] = 3 vertices x (x, y, z), each cube's vertices interpolated by that cube

@@ -65,6 +65,13 @@ class VoxelPostParams(C.Structure):
                 ("skip_under_mesh", C.c_int)]
 
 
+class VoxelBuild(C.Structure):
+    """tw_voxel_build (include/tw3d.h): one asynchronous voxel build - optional fill, outside flags, remove_unconnected and marching cubes."""
+    _fields_ = [("fill", C.c_void_p), ("rdata420", C.c_void_p), ("post", C.c_void_p), ("zix_xy", C.c_void_p), ("edge_table256", C.c_void_p),
+                ("tri_table256x16", C.c_void_p), ("edge_to_vals12x2", C.c_void_p), ("vals", C.c_void_p), ("outside", C.c_void_p), ("tris", C.c_void_p),
+                ("capacity", C.c_uint64), ("ntris", C.c_void_p), ("changed", C.c_void_p)]
+
+
 class WeightParams(C.Structure):
     """tw_weight_params (include/tw3d.h): the terrain weights texture's tables and scene scalars."""
     _fields_ = [("h_dirt", C.c_float * 5), ("tex_class", C.c_int * 5), ("class_ix", C.c_int * 5), ("sthresh", (C.c_float * 2) * 2), ("zmin", C.c_float), ("zmax", C.c_float),
@@ -154,7 +161,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
-               "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after"]
+               "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch"]
 
 
 def _load():
@@ -245,6 +252,7 @@ def _load():
     L.tw_voxel_outside.argtypes = [vp, vp, C.POINTER(VoxelPostParams), vp, vp]
     L.tw_voxel_remove_unconnected.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), C.POINTER(C.c_uint64)]
     L.tw_voxel_triangles.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, vp, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.tw_voxel_build_launch.argtypes = [vp, C.POINTER(VoxelBuild)]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
@@ -419,6 +427,21 @@ class Multi:
         zr = MinMax()
         self._check(lib.tw_heightgen_2d_sharded(self._h, C.byref(grid), C.byref(hp), int(enable_glaciate), C.cast(self._bands(out_bands), C.c_void_p), C.byref(zr)))
         return zr.zmin, zr.zmax
+
+
+class VoxelBuildJob:
+    """The host results of Context.voxel_build_launch, filled by the poll that completes the job."""
+
+    def __init__(self):
+        self._ntris, self._changed = C.c_uint64(0), C.c_uint64(0)
+
+    @property
+    def ntris(self):
+        return int(self._ntris.value)
+
+    @property
+    def changed(self):
+        return int(self._changed.value)
 
 
 class Context:
@@ -767,6 +790,28 @@ class Context:
         cap = int(out.shape[0])
         self._check(lib.tw_voxel_triangles(self._h, _ptr(vals), _ptr(outside), C.byref(vpp), _ptr(e), _ptr(t), _ptr(v), _ptr(out), cap, C.byref(n)))
         return out if isinstance(out, np.ndarray) else (out, n.value)
+
+    def voxel_build_launch(self, vpp, vals=None, outside=None, tris=None, fill=None, rdata=None, zix_xy=None, tables=None, capacity=None):
+        """tw_voxel_build_launch: fill (VoxelParams, optional) -> voxel_outside -> voxel_remove_unconnected -> voxel_triangles as one asynchronous job on
+        this context; create_tiles_poll completes it. vals [ny, nx, nz] float32 is the input field without fill, else an optional output; outside
+        [ny, nx, nz] uint8 optional output; tris: triangles out, a CUDA tensor or a page-locked numpy / torch buffer of capacity*9 floats (capacity defaults
+        to its size // 9). numpy arrays, torch tensors or None. tables (edge_table, tri_table, edge_to_vals) or None = no triangles. Returns a VoxelBuildJob
+        whose ntris / changed are valid once the job is complete. The outputs and device inputs stay referenced here until then."""
+        job = VoxelBuildJob()
+        keep = [vals, outside, tris]
+        tabs = (None, None, None)
+        if tables is not None:
+            tabs = tuple(t if hasattr(t, "data_ptr") else np.ascontiguousarray(t, dt) for t, dt in zip(tables, (np.uint32, np.int32, np.uint32)))
+        z = None if zix_xy is None else (zix_xy if hasattr(zix_xy, "data_ptr") else np.ascontiguousarray(zix_xy, np.uint32))
+        rd = None if rdata is None else np.ascontiguousarray(rdata, np.float32)
+        if capacity is None:
+            capacity = 0 if tris is None else (int(tris.numel()) if hasattr(tris, "numel") else int(tris.size)) // 9
+        b = VoxelBuild(C.cast(C.pointer(fill), C.c_void_p) if fill is not None else None, _ptr(rd), C.cast(C.pointer(vpp), C.c_void_p), _ptr(z),
+                       _ptr(tabs[0]), _ptr(tabs[1]), _ptr(tabs[2]), _ptr(vals), _ptr(outside), _ptr(tris), int(capacity),
+                       C.cast(C.pointer(job._ntris), C.c_void_p) if tables is not None else None, C.cast(C.pointer(job._changed), C.c_void_p))
+        self._check(lib.tw_voxel_build_launch(self._h, C.byref(b)))
+        self._tiles_job = (keep, tabs, z, job)
+        return job
 
     def from_floats_u16(self, vals, val_mult, val_add, out=None):
         n = int(np.prod(vals.shape))

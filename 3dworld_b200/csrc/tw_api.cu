@@ -98,9 +98,16 @@ int poll_job(tw_ctx *ctx, int wait) {
 	cudaError_t const ev = wait ? cudaEventSynchronize(a.done) : cudaEventQuery(a.done);
 	if (ev == cudaErrorNotReady) return TW_ERR_NOT_READY;
 	a.pending = false;
-	if (ev != cudaSuccess) {a.host_mm = nullptr; a.host_bounds = nullptr; a.host_min_nz = nullptr; a.host_flags = nullptr; return tw_set_error(ctx, TW_ERR_CUDA, "asynchronous job failed: %s", cudaGetErrorString(ev));}
+	if (ev != cudaSuccess) {
+		a.host_mm = nullptr; a.host_bounds = nullptr; a.host_min_nz = nullptr; a.host_flags = nullptr; a.host_ntris = nullptr; a.host_changed = nullptr; a.voxel = false;
+		return tw_set_error(ctx, TW_ERR_CUDA, "asynchronous job failed: %s", cudaGetErrorString(ev));
+	}
 	const char *h = (const char *)ctx->h_pinned;
-	if (!a.tiles) {
+	if (a.voxel) {
+		if (a.host_ntris) {memcpy(a.host_ntris, h, sizeof(uint64_t));}
+		if (a.host_changed) {memcpy(a.host_changed, h + 8, sizeof(uint64_t));}
+	}
+	else if (!a.tiles) {
 		if (a.host_mm) {unsigned const *u = (unsigned const *)h; a.host_mm->zmin = tw_ord2f(u[0]); a.host_mm->zmax = tw_ord2f(u[1]);}
 	}
 	else {
@@ -114,12 +121,13 @@ int poll_job(tw_ctx *ctx, int wait) {
 		if (a.host_flags) {memcpy(a.host_flags, h + a.off_flags, a.n_mm);}
 	}
 	a.host_mm = nullptr; a.host_bounds = nullptr; a.host_min_nz = nullptr; a.host_flags = nullptr; a.tiles = false; a.steps = false;
+	a.host_ntris = nullptr; a.host_changed = nullptr; a.voxel = false;
 	cudaError_t const e = cudaGetLastError();
 	if (e != cudaSuccess) return tw_set_error(ctx, TW_ERR_CUDA, "asynchronous job failed: %s", cudaGetErrorString(e));
 	return TW_OK;
 }
 
-int finish_pending(tw_ctx *ctx) { // complete an outstanding tw_heightgen_2d_launch / tw_create_tiles_launch before other work reuses the scratch buffers
+int finish_pending(tw_ctx *ctx) { // complete an outstanding tw_heightgen_2d_launch / tw_create_tiles_launch / tw_voxel_build_launch before other work reuses the scratch buffers
 	return poll_job(ctx, 1);
 }
 
@@ -247,9 +255,9 @@ void tw_destroy(tw_ctx *ctx) {
 	while (!ctx->shared.empty()) tw_destroy(ctx->shared.back()); // each removes itself from the list
 	if (ctx->dist) tw_dist_finalize(ctx);
 	cudaSetDevice(ctx->device);
+	finish_pending(ctx); // the job completes as a poll with wait = 1 would
 	tw_ctx *const parent = ctx->parent;
-	if (parent) { // its job completes as a poll with wait = 1 would; the tables are the parent's
-		finish_pending(ctx);
+	if (parent) { // the tables are the parent's
 		parent->shared.erase(std::find(parent->shared.begin(), parent->shared.end(), ctx));
 		ctx->d_sin_table = nullptr; ctx->d_dir_table = nullptr; ctx->d_simplex_lut = nullptr; ctx->d_glm3_lut = nullptr; ctx->d_sine_params = nullptr; ctx->d_hmap = nullptr;
 	}
@@ -1117,8 +1125,8 @@ int tw_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420,
 	int rc = check_ctx(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
 	if (!vp || !out) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
-	if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
-	if (vp->gen_mode < 0 || vp->gen_mode > TW_MGEN_DWARP_GPU) return tw_set_error(ctx, TW_ERR_ARG, "bad gen_mode");
+	size_t tab_bytes = 0;
+	rc = twi_voxel_fill_check(ctx, vp, &tab_bytes); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	bool const dev_out = tw_is_device_ptr(out);
 	float *d_out = out;

@@ -8,12 +8,14 @@
 #include <vector>
 #include "../../include/tw3d.h"
 
-// The one asynchronous job a context may have in flight (tw_heightgen_2d_launch or tw_create_tiles_launch). `done` is recorded on ctx->stream
-// after everything the job enqueued (the tile pipeline's other streams are joined into ctx->stream first); the small per-tile results are staged
+// The one asynchronous job a context may have in flight (tw_heightgen_2d_launch, tw_create_tiles_launch or tw_voxel_build_launch). `done` is recorded on
+// ctx->stream after everything the job enqueued (the tile pipeline's other streams are joined into ctx->stream first); the small per-tile results are staged
 // in ctx->h_pinned at the offsets below and unpacked into the caller's host arrays by the poll that reports completion.
 struct tw_async_state {
 	bool pending = false;
-	bool tiles = false;             // the pending job is a tile job (else a 2-D grid)
+	bool tiles = false;             // the pending job is a tile job (else a 2-D grid or a voxel build)
+	bool voxel = false;             // the pending job is a voxel build: triangle count and flipped voxels staged at ctx->h_pinned + 0 / + 8 (uint64 each)
+	uint64_t *host_ntris = nullptr, *host_changed = nullptr;
 	cudaEvent_t done = nullptr;
 	float *host_out = nullptr;      // user host buffer (nullptr => result stays on device)
 	tw_minmax *host_mm = nullptr;
@@ -203,7 +205,12 @@ int twi_sweep_apply(tw_ctx *ctx, float *P, long long *D, size_t n);
 int twi_sweep_unpad(tw_ctx *ctx, const float *P, int E0, int xsize, int y0, int y1, float min_zval, float *out);
 int twi_tile_bounds(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float wpz_max, void *d_sub, const unsigned *d_perm = nullptr);
 int twi_glaciate_mesh(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, unsigned *d_mm);
-int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out);
+// the checks of tw_voxel_fill after its null-argument check (TW_ERR_STATE without the sin table, TW_ERR_ARG for a bad gen_mode or size); *tab_bytes = the
+// scratch slot 1 bytes twi_voxel_fill uses for this grid (reserve them first and it never re-allocates)
+int twi_voxel_fill_check(tw_ctx *ctx, const tw_voxel_params *vp, size_t *tab_bytes);
+// h_stage (optional): TW_N3D_RDATA floats of pinned staging left untouched until the enqueued work is done; without it the sine mode synchronises ctx->stream
+// after uploading its coefficients (a stack buffer)
+int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out, void *h_stage = nullptr);
 int twi_from_floats_u16(tw_ctx *ctx, const float *d_vals, size_t n, float val_mult, float val_add, uint8_t *d_out, unsigned *d_bad);
 int twi_to_floats_u16(tw_ctx *ctx, const uint8_t *d_data, size_t n, float val_mult, float val_add, float *d_vals);
 int twi_minmax(tw_ctx *ctx, const float *d_vals, size_t n, unsigned *d_mm_ord);

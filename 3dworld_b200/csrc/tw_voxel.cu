@@ -183,7 +183,19 @@ int twi_ensure_glm3_lut(tw_ctx *ctx) {
 	return TW_OK;
 }
 
-int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out)
+int twi_voxel_fill_check(tw_ctx *ctx, const tw_voxel_params *vp, size_t *tab_bytes)
+{
+	if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
+	if (vp->gen_mode < 0 || vp->gen_mode > TW_MGEN_DWARP_GPU) return tw_set_error(ctx, TW_ERR_ARG, "bad gen_mode");
+	unsigned const nx = vp->nx, ny = vp->ny, nz = vp->nz;
+	if (nx == 0 || ny == 0 || nz == 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_fill: empty grid");
+	if (ny > 65535 || (vp->gen_mode != TW_MGEN_SINE && nx > 65535)) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_fill: nx/ny > 65535 not supported");
+	unsigned const xp = (nx + 31) & ~31u, yp = (ny + 31) & ~31u, zp = (nz + 31) & ~31u;
+	*tab_bytes = (vp->gen_mode == TW_MGEN_SINE) ? (size_t)NS*(xp + yp + zp)*sizeof(float) + TW_N3D_RDATA*sizeof(float) : 0;
+	return TW_OK;
+}
+
+int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out, void *h_stage)
 {
 	unsigned const nx = vp->nx, ny = vp->ny, nz = vp->nz;
 	if (nx == 0 || ny == 0 || nz == 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_fill: empty grid");
@@ -198,10 +210,11 @@ int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420
 		int rc = tw_reserve(ctx, 1, tab_bytes);
 		if (rc) return rc;
 		float *xt = (float *)ctx->d_scratch[1], *yt = xt + (size_t)NS*xp, *zt = yt + (size_t)NS*yp, *d_rdata = zt + (size_t)NS*zp;
-		float rdata[TW_N3D_RDATA];
-		if (rdata420) {memcpy(rdata, rdata420, sizeof(rdata));} else {tw_noise3d_gen_sines(vp->rseed1, vp->rseed2, vp->mag, vp->freq, rdata);}
-		TW_CUDA(ctx, cudaMemcpyAsync(d_rdata, rdata, sizeof(rdata), cudaMemcpyHostToDevice, ctx->stream));
-		TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // rdata is a stack buffer
+		float stack_rdata[TW_N3D_RDATA];
+		float *const rdata = h_stage ? (float *)h_stage : stack_rdata;
+		if (rdata420) {memcpy(rdata, rdata420, sizeof(stack_rdata));} else {tw_noise3d_gen_sines(vp->rseed1, vp->rseed2, vp->mag, vp->freq, rdata);}
+		TW_CUDA(ctx, cudaMemcpyAsync(d_rdata, rdata, sizeof(stack_rdata), cudaMemcpyHostToDevice, ctx->stream));
+		if (!h_stage) {TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));} // rdata is a stack buffer
 		float const sx = vp->lo_pos[0] + vp->offset[0], sy = vp->lo_pos[1] + vp->offset[1], sz = vp->lo_pos[2] + vp->offset[2]; // (lo_pos + offset), src/voxels.cpp:289
 		xyz_tables_kernel<<<3, 64, 0, ctx->stream>>>(xt, yt, zt, xp, yp, zp, nx, ny, nz, sx, sy, sz, vp->vsz[0], vp->vsz[1], vp->vsz[2], d_rdata, ctx->d_sin_table);
 		TW_LAUNCH_CHECK(ctx);

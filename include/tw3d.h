@@ -415,6 +415,32 @@ TW_API int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *outsid
  * device (NULL with capacity 0 to only count); ntris = triangles the grid produces (may exceed capacity: nothing is written beyond it). */
 TW_API int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t *outside, const tw_voxel_post_params *vp, const uint32_t *edge_table256,
                        const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, float *tris, uint64_t capacity, uint64_t *ntris);
+/* voxel_manager::create_procedural + voxel_model::build as ONE asynchronous job: the fill (optional), tw_voxel_outside, tw_voxel_remove_unconnected and
+ * tw_voxel_triangles enqueued on the context's stream without the host reading anything back in between (the flood fills end on the device). After the
+ * completing poll every output is bit-identical to that sequence of synchronous calls on one context: tw_voxel_fill(fill, rdata420) if fill is set, then
+ * tw_voxel_outside(zix_xy), tw_voxel_remove_unconnected, tw_voxel_triangles(capacity); nothing of tris beyond min(ntris, capacity) triangles is written.
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it (wait = 0 returns TW_ERR_NOT_READY while it runs), every
+ *   other entry point and tw_destroy complete it first. On a shared context it runs beside the other contexts' jobs.
+ * - Lifetimes: the struct, *fill, *post, rdata420, host tables and host zix_xy are copied during the launch; vals and device zix_xy / tables are read until the
+ *   completing poll; the outputs are written until then.
+ * - The launch never waits for the device, except that copies to or from PAGEABLE host vals / outside block it (see "Host output buffers" above).
+ * - Errors, nothing enqueued and nothing changed: TW_ERR_ARG for what the four synchronous calls refuse (empty grid, 2^32 voxels or more, the fill's size
+ *   limits and gen_mode), a fill grid that differs from post's, vals == NULL without fill, some but not all three tables, tables without ntris,
+ *   capacity > 0 without tris, tris in pageable host memory; TW_ERR_STATE where tw_voxel_fill returns it. */
+typedef struct tw_voxel_build {
+	const tw_voxel_params      *fill;      /* optional: fill vals first, exactly as tw_voxel_fill(fill, rdata420); nx/ny/nz must equal post's */
+	const float                *rdata420;  /* optional, sine-mode fill only, as tw_voxel_fill; copied during the launch */
+	const tw_voxel_post_params *post;      /* required */
+	const uint32_t             *zix_xy;    /* optional, as tw_voxel_outside */
+	const uint32_t *edge_table256; const int32_t *tri_table256x16; const uint32_t *edge_to_vals12x2; /* all three, or none = no triangles */
+	float    *vals;      /* n floats, host or device: the input field when fill == NULL, else an optional output; after the job = vals after remove_unconnected */
+	uint8_t  *outside;   /* optional output: n flag bytes after remove_unconnected, host or device (no alignment requirement) */
+	float    *tris;      /* optional: capacity*9 floats, device or page-locked host memory (written by the device through its mapping) */
+	uint64_t  capacity;
+	uint64_t *ntris;     /* HOST, required with the tables: filled by the completing poll (may exceed capacity) */
+	uint64_t *changed;   /* optional HOST: voxels flipped by remove_unconnected, filled by the completing poll */
+} tw_voxel_build;
+TW_API int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b);
 
 /* ---- mesh shadows of tiles (SURVEY.md 8f row N4): calc_mesh_shadows (src/visibility.cpp:411-517) for a batch of tiles with the neighbour chaining of
  * tile_t::calc_shadows_for_light (src/tiled_mesh.cpp:664-692) ---- */

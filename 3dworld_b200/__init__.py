@@ -139,6 +139,12 @@ class HeightmapInfo(C.Structure):
                 ("mesh_file_tz", C.c_float), ("erosion_moves", C.c_uint64)]
 
 
+class HeightmapOutputs(C.Structure):
+    """tw_heightmap_outputs (include/tw3d.h): where tw_proc_gen_heightmap_launch puts the image, the eroded heights and the info, and whether the image
+    becomes the context's set_heightmap image."""
+    _fields_ = [("data16", C.c_void_p), ("vals", C.c_void_p), ("info", C.c_void_p), ("set_image", C.c_int)]
+
+
 class Rng(C.Structure):
     _fields_ = [("rseed1", C.c_int64), ("rseed2", C.c_int64)]
 
@@ -161,7 +167,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_multi_alloc_host", "tw_multi_free_host", "tw_create_zvals_sharded", "tw_heightgen_2d_sharded", "tw_dist_unique_id", "tw_dist_init",
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
-               "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch"]
+               "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
+               "tw_proc_gen_heightmap_launch"]
 
 
 def _load():
@@ -227,6 +234,8 @@ def _load():
     L.tw_heightmap_to_floats_u16.argtypes = [vp, vp, C.c_size_t, C.c_float, C.c_float, vp]
     L.tw_proc_gen_heightmap.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.POINTER(HeightParams), C.c_uint32, C.POINTER(ErosionParams), vp, vp,
                                         C.POINTER(HeightmapInfo)]
+    L.tw_proc_gen_heightmap_launch.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.POINTER(HeightParams), C.c_uint32, C.POINTER(ErosionParams),
+                                               C.POINTER(HeightmapOutputs)]
     L.tw_minmax_f32.argtypes = [vp, vp, C.c_size_t, C.POINTER(MinMax)]
     # multi-GPU
     L.tw_multi_create.argtypes = [vp, C.c_int, C.POINTER(vp)]
@@ -442,6 +451,13 @@ class VoxelBuildJob:
     @property
     def changed(self):
         return int(self._changed.value)
+
+
+class HeightmapJob:
+    """The host result of Context.proc_gen_heightmap_launch: info (HeightmapInfo) is filled by the poll that completes the job."""
+
+    def __init__(self):
+        self.info = HeightmapInfo()
 
 
 class Context:
@@ -834,6 +850,16 @@ class Context:
         info = HeightmapInfo()
         self._check(lib.tw_proc_gen_heightmap(self._h, width, height, dx_val, dy_val, C.byref(hp), erosion_iters, C.byref(ep), _ptr(data16), _ptr(vals), C.byref(info)))
         return data16, info, vals
+
+    def proc_gen_heightmap_launch(self, width, height, dx_val, dy_val, hp, erosion_iters, ep, data16=None, vals=None, set_image=False):
+        """tw_proc_gen_heightmap_launch: proc_gen_heightmap as one asynchronous job on this context; create_tiles_poll completes it. data16 (2*w*h bytes)
+        and vals (w*h floats) are optional outputs - numpy arrays or CUDA tensors - but data16 or set_image is required; set_image makes the image this
+        context's set_heightmap image once the job completes. Returns a HeightmapJob whose info is valid then. The outputs stay referenced here until then."""
+        job = HeightmapJob()
+        o = HeightmapOutputs(_ptr(data16), _ptr(vals), C.cast(C.pointer(job.info), C.c_void_p), 1 if set_image else 0)
+        self._check(lib.tw_proc_gen_heightmap_launch(self._h, width, height, dx_val, dy_val, C.byref(hp), erosion_iters, C.byref(ep), C.byref(o)))
+        self._tiles_job = (data16, vals, job)
+        return job
 
     def minmax(self, vals):
         mm = MinMax()

@@ -149,6 +149,7 @@ constexpr unsigned SP_STATE_WORDS = 32; // saved registers of a suspended walk
 constexpr int SP_TILE_SHIFT = TW_SPEC_TILE_SHIFT; // conflict tiles of (1 << shift)^2 cells, >= 4x4 (a move's 4 x 4 footprint then spans at most 2 x 2 tiles)
 static_assert(SP_TILE_SHIFT >= 2, "a move may touch at most 2 x 2 tiles");
 constexpr unsigned SP_NONE = 0xffffffffu;
+constexpr unsigned SP_CTL_ROUND = 16; // ctl word of the round counter: the round kernel advances it, so one graph body serves every round
 struct SpecArgs { // M_SPEC: the window of in-flight droplets (slot = droplet index % B)
 	unsigned B, W, T, R;            // slots, log entries / tile ids / view segments per slot
 	unsigned *it, *status, *nlog, *ntiles, *nseg, *minw, *steps; // [B]
@@ -157,8 +158,8 @@ struct SpecArgs { // M_SPEC: the window of in-flight droplets (slot = droplet in
 	unsigned *seg;                  // [B][R][3] per flush segment: its end in the log, the bounding box of its cells (a cell appears at most once per segment; later segments win)
 	unsigned *stamps;               // [tile] lowest droplet index that touched the tile this round (SP_NONE: none)
 	unsigned *state;                // [B][SP_STATE_WORDS] registers of a walk suspended after `cap` moves in one round (a round must not wait for a 900-move droplet)
-	unsigned *ctl;                  // {lo[0], lo[1], first conflict, done, in-place round, statistics ...}
-	unsigned round, cap;
+	unsigned *ctl;                  // {lo[0], lo[1], first conflict, done, in-place round, statistics ..., [SP_CTL_ROUND] rounds run}
+	unsigned cap;
 	int TNX;                        // tiles per row
 };
 constexpr int TW_SWEEP_VIEW = 32; // M_FROZEN: side of a droplet's private view (part of the algorithm's definition, see tw3d.h)
@@ -232,7 +233,7 @@ droplet_kernel(DArgs const A)
 	unsigned *sp_cells = nullptr, *sp_tiles = nullptr, *sp_seg = nullptr; float *sp_vals = nullptr;
 	bool sp_inplace = false; // M_SPEC: this warp walks the window's HEAD directly on the map (nothing earlier is uncommitted, so its writes are final as they happen)
 	if (SPEC) {
-		unsigned const lo = A.S.ctl[A.S.round & 1u];
+		unsigned const lo = A.S.ctl[A.S.ctl[SP_CTL_ROUND] & 1u];
 		unsigned const st0 = active ? A.S.status[gslot] : SP_EMPTY;
 		if (!active || A.S.it[gslot] >= num_iters) return;
 		iter = A.S.it[gslot];
@@ -905,7 +906,7 @@ __global__ void spec_init_kernel(SpecArgs S, unsigned num_iters, size_t ntile_st
 		S.it[s] = s; S.status[s] = (s < num_iters) ? SP_DIRTY : SP_EMPTY; // slot s starts with droplet s
 		S.nlog[s] = 0; S.ntiles[s] = 0; S.nseg[s] = 0; S.minw[s] = SP_NONE; S.steps[s] = 0;
 	}
-	if (i == 0) {S.ctl[0] = 0; S.ctl[1] = 0; S.ctl[2] = SP_NONE; S.ctl[3] = 0; S.ctl[4] = 0; for (int k = 5; k < 16; ++k) {S.ctl[k] = 0;}}
+	if (i == 0) {S.ctl[0] = 0; S.ctl[1] = 0; S.ctl[2] = SP_NONE; S.ctl[3] = 0; S.ctl[4] = 0; for (int k = 5; k <= (int)SP_CTL_ROUND; ++k) {S.ctl[k] = 0;}}
 }
 // The bookkeeping of one round: ONE thread-block cluster of 8 x 1024 threads = 256 warps, one warp per slot, cluster.sync() between the phases (a hardware
 // barrier: the blocks of a cluster are co-scheduled, so unlike a grid-wide barrier it cannot dead-lock). Every slot's chain of dependent loads runs beside
@@ -914,12 +915,16 @@ __global__ void spec_init_kernel(SpecArgs S, unsigned num_iters, size_t ntile_st
 //   validate  a droplet conflicts if a lower-indexed droplet of the window touched one of its tiles; f = the first droplet that cannot be committed
 //   commit    the prefix [lo, f): the logs go into the map (disjoint tiles: any order), the slots get their next droplets; behind f, droplets whose tiles a
 //             committed droplet touched are walked again from the start; every stamping droplet takes its stamps back
+// The kernel advances the round counter. In the graph form (spec_loop_graph: the body of a conditional WHILE node) it also ends the loop once every droplet is
+// committed, or - with *fail = the rounds run - after max_rounds + 1 rounds without finishing; the host-driven form passes max_rounds = UINT_MAX.
 constexpr unsigned SPEC_CLUSTER = 8, SPEC_MAX_SLOTS = SPEC_CLUSTER*32;
-__global__ void __cluster_dims__(SPEC_CLUSTER, 1, 1) __launch_bounds__(1024) spec_round_kernel(SpecArgs S, unsigned num_iters, float *__restrict__ padded, int NX, unsigned long long *__restrict__ steps_total) {
+__global__ void __cluster_dims__(SPEC_CLUSTER, 1, 1) __launch_bounds__(1024) spec_round_kernel(SpecArgs S, unsigned num_iters, float *__restrict__ padded, int NX, unsigned long long *__restrict__ steps_total,
+                                                                                               unsigned max_rounds, unsigned *__restrict__ fail, cudaGraphConditionalHandle loop, bool in_graph) {
 	namespace cg = cooperative_groups;
 	cg::cluster_group cluster = cg::this_cluster();
 	unsigned const s = (blockIdx.x*blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-	unsigned const lo = S.ctl[S.round & 1u], hi = (num_iters - lo < S.B) ? num_iters : lo + S.B, hs = lo % S.B;
+	unsigned const round = S.ctl[SP_CTL_ROUND]; // written below only after the last cluster.sync(), when every thread has read it
+	unsigned const lo = S.ctl[round & 1u], hi = (num_iters - lo < S.B) ? num_iters : lo + S.B, hs = lo % S.B;
 	bool const mine = (s < S.B);
 	unsigned const st = mine ? S.status[s] : SP_EMPTY, it = mine ? S.it[s] : SP_NONE, nt = mine ? S.ntiles[s] : 0u;
 	bool const live = mine && st != SP_EMPTY && it < num_iters, stamps = live && (st == SP_VALID || st == SP_WALKING);
@@ -961,7 +966,13 @@ __global__ void __cluster_dims__(SPEC_CLUSTER, 1, 1) __launch_bounds__(1024) spe
 		else if (stamps && lane == 0 && (inplace_round || m < f)) {S.status[s] = SP_DIRTY;} // finished or not: walked again from the start
 	}
 	cluster.sync(); // everybody has read ctl[2] and the head's header
-	if (s == 0 && lane == 0) {S.ctl[(S.round + 1u) & 1u] = f; S.ctl[2] = SP_NONE; if (f >= num_iters) {S.ctl[3] = 1u;}}
+	if (s == 0 && lane == 0) {
+		S.ctl[(round + 1u) & 1u] = f; S.ctl[2] = SP_NONE; S.ctl[SP_CTL_ROUND] = round + 1u;
+		bool const done = (f >= num_iters);
+		if (done) {S.ctl[3] = 1u;}
+		else if (round >= max_rounds) {*fail = round + 1u;}
+		if (in_graph && (done || round >= max_rounds)) {cudaGraphSetConditional(loop, 0u);}
+	}
 }
 
 bool spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters) {
@@ -976,26 +987,23 @@ bool spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters) {
 }
 } // namespace
 
-// One heightmap, the reference's serial droplet order, bit for bit (see M_SPEC at the top). Synchronises: the host polls the window's "done" flag.
-int twi_erode_spec(tw_ctx *ctx, float *d_map, int xsize, int ysize, const float *d_min_zvals, float min_zval, uint32_t num_iters, const tw_erosion_params *p, unsigned long long *d_steps) {
-	cudaStream_t const st = ctx->stream;
+// M_SPEC's window: sizes from the TW_SPEC_* overrides, arrays carved from `scratch` (nullptr: sizes only); returns the scratch bytes
+static size_t spec_layout(int xsize, int ysize, void *scratch, SpecArgs &S, float *&d_pad, size_t &ntile) {
 	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
-	SpecArgs S;
 	memset(&S, 0, sizeof(S));
 	S.B = (unsigned)std::max(32, std::min(env_int("TW_SPEC_WINDOW", 256), (int)SPEC_MAX_SLOTS)); S.B &= ~31u; // <= 256: the round kernel is one cluster with a warp per slot
 	S.W = (unsigned)std::max(64, env_int("TW_SPEC_LOG", 8192));
 	S.T = (unsigned)std::max(16, env_int("TW_SPEC_TILES", 4096)) & ~3u;
 	S.R = (unsigned)std::max(2, env_int("TW_SPEC_VIEWS", 256));
 	S.TNX = ((NX - 1) >> SP_TILE_SHIFT) + 1;
-	size_t const ntile = (size_t)S.TNX*(((NY - 1) >> SP_TILE_SHIFT) + 1);
+	S.cap = (unsigned)std::max(1, env_int("TW_SPEC_MOVES", 64));
+	ntile = (size_t)S.TNX*(((NY - 1) >> SP_TILE_SHIFT) + 1);
 	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
 	size_t const pad_b = al((size_t)NX*NY*sizeof(float)), slot_b = al((size_t)S.B*sizeof(unsigned));
-	S.cap = (unsigned)std::max(1, env_int("TW_SPEC_MOVES", 64));
 	size_t const total = pad_b + 7*slot_b + 2*al((size_t)S.B*S.W*4) + al((size_t)S.B*S.T*4) + al((size_t)S.B*S.R*12) + al((size_t)S.B*SP_STATE_WORDS*4) + al(ntile*4) + 256;
-	int rc = tw_reserve(ctx, 1, total);
-	if (rc) return rc;
-	char *q = (char *)ctx->d_scratch[1];
-	float *d_pad = (float *)q; q += pad_b;
+	if (!scratch) return total;
+	char *q = (char *)scratch;
+	d_pad = (float *)q; q += pad_b;
 	unsigned **slot_arrays[7] = {&S.it, &S.status, &S.nlog, &S.ntiles, &S.nseg, &S.minw, &S.steps};
 	for (auto a : slot_arrays) {*a = (unsigned *)q; q += slot_b;}
 	S.cells = (unsigned *)q; q += al((size_t)S.B*S.W*4);
@@ -1004,11 +1012,68 @@ int twi_erode_spec(tw_ctx *ctx, float *d_map, int xsize, int ysize, const float 
 	S.seg = (unsigned *)q; q += al((size_t)S.B*S.R*12);
 	S.state = (unsigned *)q; q += al((size_t)S.B*SP_STATE_WORDS*4);
 	S.stamps = (unsigned *)q; q += al(ntile*4);
-	S.ctl = (unsigned *)q;
-	rc = tw_reserve_pinned(ctx, 64);
-	if (rc) return rc;
-	volatile unsigned *h_done = (volatile unsigned *)ctx->h_pinned;
+	S.ctl = (unsigned *)q; // 256 bytes
+	return total;
+}
 
+// The rounds as one CUDA graph: a conditional WHILE node whose body is the walker launch and the round kernel, which clears the condition. The graph's kernel
+// arguments are fixed, so it is kept in the context and rebuilt only when they change (another map size, scratch address or droplet count).
+static int spec_loop_graph(tw_ctx *ctx, cudaStream_t st, DArgs const &W, unsigned num_iters, float *d_pad, int NX, unsigned long long *d_steps, unsigned max_rounds, unsigned *d_fail) {
+	struct Key {DArgs W; unsigned num_iters, max_rounds; int NX; float *pad; unsigned long long *steps; unsigned *fail;} k;
+	memset(&k, 0, sizeof(k));
+	k.W = W; k.num_iters = num_iters; k.max_rounds = max_rounds; k.NX = NX; k.pad = d_pad; k.steps = d_steps; k.fail = d_fail;
+	if (ctx->spec_graph && ctx->spec_key.size() == sizeof(k) && !memcmp(ctx->spec_key.data(), &k, sizeof(k))) return TW_OK;
+	if (ctx->spec_graph) {cudaGraphExecDestroy(ctx->spec_graph); ctx->spec_graph = nullptr; ctx->spec_key.clear();} // a launch still in flight keeps its copy until it ends
+	cudaGraph_t g = nullptr;
+	cudaGraphExec_t ex = nullptr;
+	cudaGraphConditionalHandle h = 0;
+	cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
+	cudaError_t e = cudaGraphCreate(&g, 0);
+	if (e == cudaSuccess) {e = cudaGraphConditionalHandleCreate(&h, g, 1u, cudaGraphCondAssignDefault);}
+	if (e == cudaSuccess) {
+		cudaGraphNode_t node;
+		np.conditional.handle = h; np.conditional.type = cudaGraphCondTypeWhile; np.conditional.size = 1;
+		e = cudaGraphAddNode(&node, g, nullptr, 0, &np);
+	}
+	if (e == cudaSuccess) {e = cudaStreamBeginCaptureToGraph(st, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed);}
+	if (e == cudaSuccess) {
+		launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));
+		spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(W.S, num_iters, d_pad, NX, d_steps, max_rounds, d_fail, h, true);
+		cudaError_t const le = cudaGetLastError();
+		cudaGraph_t body = nullptr;
+		e = cudaStreamEndCapture(st, &body);
+		if (e == cudaSuccess) {e = le;}
+	}
+	if (e == cudaSuccess) {e = cudaGraphInstantiate(&ex, g, 0);}
+	if (g) {cudaGraphDestroy(g);}
+	if (e != cudaSuccess) {cudaGetLastError(); return tw_set_error(ctx, TW_ERR_CUDA, "speculative erosion graph: %s", cudaGetErrorString(e));}
+	ctx->spec_graph = ex;
+	ctx->spec_key.assign((const unsigned char *)&k, (const unsigned char *)&k + sizeof(k));
+	return TW_OK;
+}
+
+bool twi_erode_spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters) {return spec_eligible(nt, xsize, ysize, num_iters);}
+
+size_t twi_erode_spec_scratch_bytes(int xsize, int ysize) {
+	SpecArgs S; float *d_pad; size_t ntile;
+	return spec_layout(xsize, ysize, nullptr, S, d_pad, ntile);
+}
+
+// One heightmap, the reference's serial droplet order, bit for bit (see M_SPEC at the top), on ctx->stream: pad, window set-up, the rounds, unpad with the lower
+// clamp *d_min_zvals (nullptr: min_zval). scratch: twi_erode_spec_scratch_bytes() bytes. d_steps accumulates the committed moves.
+// host_rounds = false: the rounds are one graph launch that ends on the device and nothing waits; *d_fail becomes the number of rounds run if the window stopped
+// making progress (0 otherwise). host_rounds = true (tw_erode): the rounds are queued from the host, which reads the "done" flag every 8 rounds and returns the
+// no-progress error itself; on the BASELINE 8192^2 map this was 1-2 % faster than the graph with 1000 droplets and equal with 1e5 (DESIGN.md section 4e).
+int twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zvals, float min_zval, uint32_t num_iters,
+                           const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds) {
+	volatile unsigned *h_done = nullptr;
+	if (host_rounds) {int const rc = tw_reserve_pinned(ctx, 64); if (rc) return rc; h_done = (volatile unsigned *)ctx->h_pinned;}
+	cudaStream_t const st = ctx->stream;
+	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
+	SpecArgs S;
+	float *d_pad = nullptr;
+	size_t ntile = 0;
+	spec_layout(xsize, ysize, scratch, S, d_pad, ntile);
 	DArgs A;
 	memset(&A, 0, sizeof(A));
 	A.E = make_eparams(p);
@@ -1019,29 +1084,38 @@ int twi_erode_spec(tw_ctx *ctx, float *d_map, int xsize, int ysize, const float 
 	size_t const init_n = std::max(ntile, (size_t)S.B);
 	spec_init_kernel<<<(unsigned)((init_n + 255)/256), 256, 0, st>>>(S, num_iters, ntile);
 	TW_LAUNCH_CHECK(ctx);
+	TW_CUDA(ctx, cudaMemsetAsync(d_fail, 0, sizeof(unsigned), st));
 	DArgs W = A; // the speculative walkers: one warp per slot, a private 32 x 32 view + 32 words of dirty bits each
-	W.nslots = S.B; W.steps_out = nullptr;
+	W.nslots = S.B; W.steps_out = nullptr; W.S = S;
 	W.WX = std::min(32, NX); W.WY = std::min(32, NY); W.P = whole_pitch(W.WX, W.WY); W.win_elems = (unsigned)(W.P*W.WY + 32);
-	unsigned const min_rounds = (num_iters + S.B - 1)/S.B, max_rounds = 2*num_iters + 64;
-	unsigned spec_rounds = 0;
-	for (unsigned round = 0;; ++round) {
-		if (round > max_rounds) return tw_set_error(ctx, TW_ERR_STATE, "speculative erosion made no progress (%u rounds)", round);
-		S.round = round; W.S = S;
-		launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));
-		spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(S, num_iters, d_pad, NX, d_steps);
-		TW_LAUNCH_CHECK(ctx);
-		if (round + 1 >= min_rounds && (round & 7u) == 7u) { // poll "done" every 8 rounds (not before the window can have covered all droplets): the rounds in between are queued back to back
-			TW_CUDA(ctx, cudaMemcpyAsync((void *)h_done, S.ctl + 3, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-			TW_CUDA(ctx, cudaStreamSynchronize(st));
-			if (*h_done) {spec_rounds = round + 1; break;}
+	unsigned const max_rounds = 2*num_iters + 64;
+	if (host_rounds) {
+		unsigned const min_rounds = (num_iters + S.B - 1)/S.B;
+		for (unsigned round = 0;; ++round) {
+			if (round > max_rounds) return tw_set_error(ctx, TW_ERR_STATE, "speculative erosion made no progress (%u rounds)", round);
+			launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));
+			spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(S, num_iters, d_pad, NX, d_steps, 0xffffffffu, d_fail, 0, false);
+			TW_LAUNCH_CHECK(ctx);
+			if (round + 1 >= min_rounds && (round & 7u) == 7u) { // poll "done" every 8 rounds (not before the window can have covered all droplets): the rounds in between are queued back to back
+				TW_CUDA(ctx, cudaMemcpyAsync((void *)h_done, S.ctl + 3, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+				TW_CUDA(ctx, cudaStreamSynchronize(st));
+				if (*h_done) break;
+			}
 		}
+	}
+	else {
+		int const rc = spec_loop_graph(ctx, st, W, num_iters, d_pad, NX, d_steps, max_rounds, d_fail);
+		if (rc) return rc;
+		TW_CUDA(ctx, cudaGraphLaunch(ctx->spec_graph, st));
+		ctx->launches++;
 	}
 	unpad_kernel<<<dim3((xsize + 255)/256, ysize, 1), 256, 0, st>>>(d_pad, d_map, xsize, ysize, NX, NY, d_min_zvals, min_zval, nullptr);
 	TW_LAUNCH_CHECK(ctx);
 	if (getenv("TW_SPEC_STATS")) {
-		unsigned h[16];
+		unsigned h[SP_CTL_ROUND + 1];
 		TW_CUDA(ctx, cudaMemcpyAsync(h, S.ctl, sizeof(h), cudaMemcpyDeviceToHost, st));
 		TW_CUDA(ctx, cudaStreamSynchronize(st));
+		unsigned const spec_rounds = std::max(1u, h[SP_CTL_ROUND]);
 		fprintf(stderr, "tw spec: %u droplets, window %u: %u rounds (%.1f commits per round), %u walks (%.2f per droplet), %u outgrew their log (log %u, views %u, tiles %u, outside view %u, non-finite at the corner %u), %u walked in place; longest walk %u moves\n",
 		        num_iters, S.B, spec_rounds, (double)num_iters/spec_rounds, h[6], (double)h[6]/num_iters, h[7], h[8], h[9], h[10], h[11], h[12], h[5], h[13]);
 	}
@@ -1060,7 +1134,10 @@ int twi_erode(tw_ctx *ctx, float *d_maps, uint32_t ntiles, int xsize, int ysize,
 	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
 	TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, sizeof(unsigned long long), ctx->stream));
 	if (spec_eligible(ntiles, xsize, ysize, num_iters)) { // one big map: the serial order, walked speculatively in parallel and committed in order (M_SPEC)
-		rc = twi_erode_spec(ctx, d_maps, xsize, ysize, d_min_zvals, min_zval_all, num_iters, p, d_steps);
+		rc = tw_reserve(ctx, 1, twi_erode_spec_scratch_bytes(xsize, ysize));
+		if (rc) return rc;
+		unsigned *d_fail = (unsigned *)(d_steps + 2);
+		rc = twi_erode_spec_enqueue(ctx, ctx->d_scratch[1], d_maps, xsize, ysize, d_min_zvals, min_zval_all, num_iters, p, d_steps, d_fail, true);
 		if (rc) return rc;
 		unsigned long long h_steps = 0;
 		TW_CUDA(ctx, cudaMemcpyAsync(&h_steps, d_steps, sizeof(h_steps), cudaMemcpyDeviceToHost, ctx->stream));

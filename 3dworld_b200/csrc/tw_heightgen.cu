@@ -678,6 +678,12 @@ static bool make_noise_params(const tw_height_params *p, NoiseParams &N, bool &s
 	return true;
 }
 
+size_t twi_heightgen_slot1_bytes(const tw_grid2d *g, const tw_height_params *p) { // the sine-table mode's X / Y tables below
+	if (p->gen_mode != TW_MGEN_SINE) return 0;
+	unsigned const xpitch = (g->nx + 63) & ~63u, ypitch = (g->ny + 63) & ~63u;
+	return (size_t)(F_TABLE + 1)*(xpitch + ypitch)*sizeof(float);
+}
+
 int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin,
                   const float2 *d_tile_origins, uint32_t ntiles, float *d_out, unsigned *d_mm_ord, float *h_out_bands)
 {

@@ -16,6 +16,9 @@ struct tw_async_state {
 	bool tiles = false;             // the pending job is a tile job (else a 2-D grid or a voxel build)
 	bool voxel = false;             // the pending job is a voxel build: triangle count and flipped voxels staged at ctx->h_pinned + 0 / + 8 (uint64 each)
 	uint64_t *host_ntris = nullptr, *host_changed = nullptr;
+	bool hmap = false;              // the pending job is tw_proc_gen_heightmap_launch: a twi_hmap_stage at ctx->h_pinned
+	tw_heightmap_info *host_info = nullptr;
+	int image_w = 0, image_h = 0;   // > 0: the packed image becomes the context's tw_set_heightmap image when the job completes
 	cudaEvent_t done = nullptr;
 	float *host_out = nullptr;      // user host buffer (nullptr => result stays on device)
 	tw_minmax *host_mm = nullptr;
@@ -59,6 +62,8 @@ struct tw_ctx {
 	void  *h_pinned = nullptr;
 	size_t pinned_bytes = 0;
 	tw_async_state async;
+	cudaGraphExec_t spec_graph = nullptr;   // the speculative erosion's round loop (tw_erosion.cu), kept while its kernel arguments stay the same
+	std::vector<unsigned char> spec_key;    // those arguments
 	void *dist = nullptr;        // tw_dist_state (tw_multi.cu): NCCL communicator of the one-process-per-GPU mode
 	unsigned skip_rect[4] = {0, 0, 0, 0}; // x0, y0, w, h of the cells twi_heightgen's paired noise kernels leave unwritten (set around AO context generation only)
 	// tw_create_shared: a shared context's tables above (sin / direction tables, sine params, both LUTs, the heightmap image) are its parent's, copied
@@ -189,6 +194,12 @@ int twi_create_tiles_launch(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_
                             uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
                             const tw_tile_outputs *out, const tw_tile_shading *shading, twi_job_tail *tail);
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
+// M_SPEC (one big map, the reference's serial droplet order) in parts: whether twi_erode takes it, its scratch, and the enqueue - with host_rounds = false
+// one that ends on the device (*d_fail = the rounds run when the window stopped making progress, else 0), with true tw_erode's host-driven rounds
+bool   twi_erode_spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters);
+size_t twi_erode_spec_scratch_bytes(int xsize, int ysize);
+int    twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zvals, float min_zval, uint32_t num_iters,
+                              const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds);
 int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads);
 size_t   twi_erode_scratch_bytes(const tw_ctx *ctx, uint32_t chunk, int xsize, int ysize);
 uint32_t twi_erode_chunk_for(size_t budget, uint32_t ntiles, int xsize, int ysize);
@@ -212,6 +223,13 @@ int twi_voxel_fill_check(tw_ctx *ctx, const tw_voxel_params *vp, size_t *tab_byt
 // after uploading its coefficients (a stack buffer)
 int twi_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *d_out, void *h_stage = nullptr);
 int twi_from_floats_u16(tw_ctx *ctx, const float *d_vals, size_t n, float val_mult, float val_add, uint8_t *d_out, unsigned *d_bad);
+// tw_proc_gen_heightmap's device scalars (tw_streaming.cu): twi_hmap_scales turns the ordered min/max d_mm into a twi_hmap_stage in device memory (the host
+// arithmetic of set_mesh_height_scales_for_zval_range and get_mh_texture_mult/add); twi_from_floats_u16_dev packs with that stage's val_add / val_div
+struct twi_hmap_stage {float min_z, max_z, val_mult, val_add, mesh_file_scale, mesh_file_tz, val_div; unsigned bad, fail, pad_; unsigned long long steps;};
+int twi_hmap_scales(tw_ctx *ctx, const unsigned *d_mm, float mesh_height_scale, float mesh_scale_z_inv, twi_hmap_stage *d_stage);
+int twi_from_floats_u16_dev(tw_ctx *ctx, const float *d_vals, size_t n, const twi_hmap_stage *d_stage, uint8_t *d_out);
+// scratch slot 1 bytes twi_heightgen uses for this grid (the sine mode's tables; 0 otherwise)
+size_t twi_heightgen_slot1_bytes(const tw_grid2d *g, const tw_height_params *p);
 int twi_to_floats_u16(tw_ctx *ctx, const uint8_t *d_data, size_t n, float val_mult, float val_add, float *d_vals);
 int twi_minmax(tw_ctx *ctx, const float *d_vals, size_t n, unsigned *d_mm_ord);
 int twi_minmax_tiles(tw_ctx *ctx, cudaStream_t st, const float *d_vals, size_t tile_elems, uint32_t nt, unsigned *d_mm_ord, const unsigned *d_perm = nullptr);

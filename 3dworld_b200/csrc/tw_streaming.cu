@@ -13,7 +13,10 @@ __device__ __forceinline__ unsigned pack16(float h, float val_add, float val_div
 	return low_bits | (high_bits << 8);                    // data[2i] = low, data[2i+1] = high
 }
 
-__global__ void from_floats_u16_kernel(const float *__restrict__ vals, size_t n, float val_add, float val_div, uint16_t *__restrict__ out, unsigned *__restrict__ bad_count) {
+// stage (optional): val_add / val_div come from the device (tw_proc_gen_heightmap_launch) instead of the arguments
+__global__ void from_floats_u16_kernel(const float *__restrict__ vals, size_t n, float val_add, float val_div, uint16_t *__restrict__ out, unsigned *__restrict__ bad_count,
+                                       const twi_hmap_stage *__restrict__ stage = nullptr) {
+	if (stage) {val_add = stage->val_add; val_div = stage->val_div;}
 	size_t const stride = (size_t)gridDim.x*blockDim.x;
 	unsigned bad = 0;
 	size_t const n4 = n/4;
@@ -42,6 +45,22 @@ __global__ void to_floats_u16_kernel(const uint16_t *__restrict__ data, size_t n
 	}
 }
 
+// the host code of tw_proc_gen_heightmap's scalars, operation for operation (every TU is built with -fmad=false; the _rn intrinsics pin the rest):
+// set_mesh_height_scales_for_zval_range(min_z, dz/255.0) and get_mh_texture_mult/add (src/mesh_gen.cpp:124-131), val_div as twi_from_floats_u16 forms it
+__global__ void hmap_scales_kernel(const unsigned *__restrict__ mm, float mhs, float mszi, twi_hmap_stage *__restrict__ st) {
+	float const TOLERANCE = 1.0E-12, READ_MESH_H_SCALE = 0.0008; // src/3DWorld.h:50, src/mesh_gen.cpp:22
+	float const min_z = tw_ord2f(mm[0]), max_z = tw_ord2f(mm[1]);
+	float const dzr = __fsub_rn(max_z, min_z), dz = (TOLERANCE < dzr) ? dzr : TOLERANCE;
+	float const dz255 = __double2float_rn(__ddiv_rn((double)dz, 255.0));
+	float const rh = __fmul_rn(READ_MESH_H_SCALE, mhs);
+	float const mesh_file_scale = __fdiv_rn(dz255, __fmul_rn(rh, mszi));
+	float const mesh_file_tz = __fdiv_rn(min_z, mszi);
+	float const val_mult = __fmul_rn(__fmul_rn(rh, mesh_file_scale), mszi);
+	st->min_z = min_z; st->max_z = max_z; st->val_mult = val_mult; st->val_add = __fmul_rn(mesh_file_tz, mszi);
+	st->mesh_file_scale = mesh_file_scale; st->mesh_file_tz = mesh_file_tz;
+	st->val_div = __double2float_rn(__ddiv_rn(1.0, (double)val_mult)); // src/heightmap.cpp:206
+}
+
 int grid_for(const tw_ctx *ctx, size_t n) {size_t b = (n + 1023)/1024; if (b > ctx->num_sms*16) b = ctx->num_sms*16; if (b < 1) b = 1; return (int)b;}
 
 } // namespace
@@ -49,6 +68,18 @@ int grid_for(const tw_ctx *ctx, size_t n) {size_t b = (n + 1023)/1024; if (b > c
 int twi_from_floats_u16(tw_ctx *ctx, const float *d_vals, size_t n, float val_mult, float val_add, uint8_t *d_out, unsigned *d_bad) {
 	float const val_div = (float)(1.0/(double)val_mult); // src/heightmap.cpp:206
 	from_floats_u16_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>(d_vals, n, val_add, val_div, reinterpret_cast<uint16_t *>(d_out), d_bad);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+int twi_hmap_scales(tw_ctx *ctx, const unsigned *d_mm, float mesh_height_scale, float mesh_scale_z_inv, twi_hmap_stage *d_stage) {
+	hmap_scales_kernel<<<1, 1, 0, ctx->stream>>>(d_mm, mesh_height_scale, mesh_scale_z_inv, d_stage);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+int twi_from_floats_u16_dev(tw_ctx *ctx, const float *d_vals, size_t n, const twi_hmap_stage *d_stage, uint8_t *d_out) {
+	from_floats_u16_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>(d_vals, n, 0.0f, 0.0f, reinterpret_cast<uint16_t *>(d_out), const_cast<unsigned *>(&d_stage->bad), d_stage);
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }

@@ -406,6 +406,36 @@ inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, un
 	return detail::launch_tiles(c, detail::tls().tile_jobs, &hs, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
 }
 
+// terrain_hmap_manager_t::proc_gen_heightmap (heightmap_t::proc_gen, src/heightmap.cpp:130-215): the globals' height function on a width x height grid
+// (cell size dx, dy), run_erosion with erosion_iters droplets, the z range, the texture scalars (info: get_mh_texture_mult/add, mesh_file_scale / _tz, the
+// droplet moves) and the 16-bit image data16 (2*width*height bytes). data16 and vals (optional, width*height floats) are host or device memory.
+inline void proc_gen_heightmap(unsigned width, unsigned height, float dx, float dy, unsigned erosion_iters, uint8_t *data16, float *vals, tw_heightmap_info *info) {
+	scene_globals const &g = globals();
+	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
+	tw_erosion_params const e = erosion_params_from_globals();
+	tw_ctx *c = ctx();
+	int const rc = tw_proc_gen_heightmap(c, width, height, dx, dy, &p, erosion_iters, &e, data16, vals, info);
+	if (rc != TW_OK) {detail::fail(rc, "proc_gen_heightmap", c);}
+}
+// The same as a job that does not stall the frame (tw_proc_gen_heightmap_launch): returns at once; ready() / wait() on the tiles_job say when data16, vals and
+// *info are complete. set_image: the image also becomes this thread's set_heightmap() image (data16 may then be nullptr), so the frame's
+// create_tiles_async_from_heightmap() samples it once the job is ready - or completes the job first when launched earlier. A pageable host data16 / vals
+// makes the launch wait for its copy.
+inline tiles_job proc_gen_heightmap_async(unsigned width, unsigned height, float dx, float dy, unsigned erosion_iters, uint8_t *data16, float *vals, tw_heightmap_info *info,
+                                          bool set_image = false) {
+	scene_globals const &g = globals();
+	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
+	tw_erosion_params const e = erosion_params_from_globals();
+	tw_heightmap_outputs const out = {data16, vals, info, set_image ? 1 : 0};
+	tw_ctx *c = ctx();
+	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+	uint64_t const number = ++jobs;
+	int const rc = tw_proc_gen_heightmap_launch(c, width, height, dx, dy, &p, erosion_iters, &e, &out);
+	if (rc != TW_OK) {detail::fail(rc, "proc_gen_heightmap_async", c);}
+	if (set_image) {detail::tls().hmap_w = (int)width; detail::tls().hmap_h = (int)height;}
+	return tiles_job(c, &jobs, number);
+}
+
 // Several frames' tile jobs in flight at once: a pool of n shared contexts of this thread's ctx() (tw_create_shared - the same tables and heightmap
 // image, own streams and scratch). pool.create_tiles_async(...) takes the arguments of the free functions above and launches on a slot with no job in
 // flight; when every slot is busy, on the slot launched on longest ago, whose job that launch completes first (its tiles_job then reports ready).

@@ -352,6 +352,28 @@ TW_API int tw_heightmap_to_floats_u16(tw_ctx *ctx, const uint8_t *data2n, size_t
 typedef struct tw_heightmap_info { float min_z, max_z, val_mult, val_add, mesh_file_scale, mesh_file_tz; uint64_t erosion_moves; } tw_heightmap_info;
 TW_API int tw_proc_gen_heightmap(tw_ctx *ctx, uint32_t width, uint32_t height, float dx_val, float dy_val, const tw_height_params *p,
                           uint32_t erosion_iters, const tw_erosion_params *ep, uint8_t *data16, float *vals, tw_heightmap_info *info);
+/* tw_proc_gen_heightmap as the context's ASYNCHRONOUS job: generation, erosion, the z range, the texture scalars and the pack are enqueued without the host
+ * reading anything back (the speculative erosion's rounds end on the device). After the completing poll every output equals tw_proc_gen_heightmap with the same
+ * arguments, bit for bit - data16, vals, every field of info and tw_last_erosion_steps(); a value outside [0,256) makes that poll return TW_ERR_ARG with the
+ * synchronous call's message, after the outputs are written.
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it (wait = 0 returns TW_ERR_NOT_READY while it runs), every
+ *   other entry point and tw_destroy complete it first. On a shared context it runs beside the other contexts' jobs.
+ * - The launch never waits for the device, except that copies to PAGEABLE host data16 / vals block it (see "Host output buffers" above). Every buffer is
+ *   reserved before anything is enqueued.
+ * - set_image = 1 (root context only): the packed image becomes the context's tw_set_heightmap image, written straight into the context's allocation. The
+ *   launch first completes every shared context's job and releases the old image; until the completing poll the context has no image (a shared context's
+ *   tw_create_tiles_launch_hmap gets TW_ERR_STATE; the parent's own completes this job first). After a poll that returns TW_OK the state equals
+ *   tw_set_heightmap(data16, width, height).
+ * - Errors, nothing enqueued and nothing changed: TW_ERR_ARG for a NULL p or out, an empty grid, neither data16 nor set_image, set_image on a shared context,
+ *   and what tw_proc_gen_heightmap refuses; TW_ERR_STATE without the sin table (or, in sine mode, the sine params). */
+typedef struct tw_heightmap_outputs {
+	uint8_t           *data16;    /* optional: 2*width*height bytes, device or host (the layout of tw_heightmap_from_floats_u16) */
+	float             *vals;      /* optional: width*height floats after erosion, device or host */
+	tw_heightmap_info *info;      /* optional HOST: filled by the completing poll */
+	int                set_image; /* 1: the packed image becomes the context's tw_set_heightmap image (root context only) */
+} tw_heightmap_outputs;
+TW_API int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, float dx_val, float dy_val, const tw_height_params *p,
+                                        uint32_t erosion_iters, const tw_erosion_params *ep, const tw_heightmap_outputs *out);
 /* Heightmap-texture mode of tile_t::create_zvals (src/tiled_mesh.cpp:498-501; SURVEY.md 8f row N2): every cell of every tile is
  * terrain_hmap_manager_t::get_clamped_height(x1 + x, y1 + y) (src/heightmap.cpp:385-402) of a 16-bit heightmap image -
  *   mesh_scale < 1: bilinear interpolate_height(); otherwise the nearest texel round_fp(mesh_scale*x) (clamp_xy, :309-313);

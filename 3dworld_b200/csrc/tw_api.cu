@@ -1138,6 +1138,80 @@ int tw_erode_parallel(tw_ctx *ctx, float *heightmap, int xsize, int ysize, float
 	return TW_OK;
 }
 
+// tw_erode / tw_erode_parallel of one map, or of the context's image between its unpack and its pack, as the context's asynchronous job: the work tw_erode
+// (twi_erode's single-map paths) and tw_erode_parallel enqueue, with the step count, the no-progress flag and the pack's error flag staged in a
+// twi_hmap_stage that the completing poll unpacks; the image's lower clamp is its minimum, computed into the stage's min_z on the device
+int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job) {
+	int rc = check_ctx(ctx); if (rc) return rc;
+	rc = finish_pending(ctx); if (rc) return rc;
+	if (!job || !job->ep) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+	bool const image = (job->heightmap == nullptr);
+	if (job->mode != TW_EROSION_SERIAL && job->mode != TW_EROSION_OPENMP) return tw_set_error(ctx, TW_ERR_ARG, "bad erosion mode %d", job->mode);
+	if (job->mode == TW_EROSION_SERIAL && job->num_threads) return tw_set_error(ctx, TW_ERR_ARG, "num_threads is for TW_EROSION_OPENMP only");
+	if (image) {
+		if (job->xsize || job->ysize) return tw_set_error(ctx, TW_ERR_ARG, "the image's size is the tw_set_heightmap image's: xsize and ysize must be 0");
+		if (ctx->parent) return tw_set_error(ctx, TW_ERR_ARG, "tables are set on the parent context, not on a shared one");
+		if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_heightmap() has not been called");
+	}
+	else {
+		if (job->vals) return tw_set_error(ctx, TW_ERR_ARG, "vals is an output of the image's erosion only");
+		if (job->xsize <= 0 || job->ysize <= 0) return tw_set_error(ctx, TW_ERR_ARG, "empty heightmap");
+	}
+	int const xsize = image ? ctx->hmap_w : job->xsize, ysize = image ? ctx->hmap_h : job->ysize;
+	size_t const n = (size_t)xsize*ysize;
+	bool const erode = (job->num_iters > 0 && job->ep->erode_amount > 0.0); // src/erosion.cpp:16
+	if (erode && !ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
+	bool const openmp = (job->mode == TW_EROSION_OPENMP), spec = erode && !openmp && twi_erode_spec_eligible(1, xsize, ysize, job->num_iters);
+	float *const user = image ? job->vals : job->heightmap; // the caller's floats: the map, or the image's optional eroded floats
+	bool const user_dev = (user && tw_is_device_ptr(user));
+	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
+	// slot 0: the floats (unless the caller's are on the device); slot 1: the erosion's scratch; slot 2: [ordered min/max, droplet counter | stage]
+	if (erode && !user_dev) {rc = tw_reserve(ctx, 0, al(n*sizeof(float))); if (rc) return rc;}
+	size_t const ebytes = !erode ? 0 : openmp ? twi_erode_parallel_scratch_bytes(xsize, ysize)
+	                                 : spec ? twi_erode_spec_scratch_bytes(xsize, ysize) : twi_erode_scratch_bytes(ctx, 1, xsize, ysize);
+	if (ebytes) {rc = tw_reserve(ctx, 1, ebytes); if (rc) return rc;}
+	rc = tw_reserve(ctx, 2, OFF_TILES + 64 + al(sizeof(twi_hmap_stage))); if (rc) return rc;
+	rc = tw_reserve_pinned(ctx, sizeof(twi_hmap_stage)); if (rc) return rc;
+	if (image) { // the shared contexts' jobs may read the image; the context has none until the completing poll
+		rc = begin_table_change(ctx); if (rc) return rc;
+		ctx->hmap_w = ctx->hmap_h = 0;
+	}
+	tw_erosion_params const ep = *job->ep;
+	float *const d_vals = user_dev ? user : (float *)ctx->d_scratch[0];
+	unsigned *const d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_TILES);
+	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
+	auto enqueue = [&]() -> int {
+		TW_CUDA(ctx, cudaMemsetAsync(d_st, 0, sizeof(twi_hmap_stage), ctx->stream));
+		if (erode) {
+			const float *d_min = nullptr; // the float map's clamp is job->min_zval
+			if (image) { // tw_heightmap_to_floats_u16, tw_minmax_f32 (run_erosion's min_zval, src/heightmap.cpp:155-156)
+				int r = twi_to_floats_u16(ctx, ctx->d_hmap, n, job->val_mult, job->val_add, d_vals); if (r) return r;
+				r = twi_init_minmax(ctx, d_mm, 1); if (r) return r;
+				r = twi_minmax(ctx, d_vals, n, d_mm); if (r) return r;
+				r = twi_ord_min(ctx, d_mm, &d_st->min_z); if (r) return r;
+				d_min = &d_st->min_z;
+			}
+			else if (!user_dev) {TW_CUDA(ctx, cudaMemcpyAsync(d_vals, user, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+			int r;
+			if (openmp) {r = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, job->num_threads, &d_st->steps, d_mm + 2);}
+			else if (spec) {r = twi_erode_spec_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps, &d_st->fail, false);}
+			else {r = twi_erode_enqueue(ctx, ctx->stream, 0, ctx->d_scratch[1], 1, d_vals, 1, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps);}
+			if (r) return r;
+			if (image) {r = twi_from_floats_u16(ctx, d_vals, n, job->val_mult, job->val_add, ctx->d_hmap, &d_st->bad); if (r) return r;}
+			if (user && !user_dev) {TW_CUDA(ctx, cudaMemcpyAsync(user, d_vals, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+		}
+		TW_CUDA(ctx, cudaMemcpyAsync(ctx->h_pinned, d_st, sizeof(twi_hmap_stage), cudaMemcpyDeviceToHost, ctx->stream));
+		TW_CUDA(ctx, cudaEventRecord(ctx->async.done, ctx->stream));
+		return TW_OK;
+	};
+	rc = enqueue();
+	if (rc) {cudaStreamSynchronize(ctx->stream); return rc;} // nothing may still run on the scratch when the error is returned
+	tw_async_state &a = ctx->async;
+	a.pending = true; a.tiles = false; a.voxel = false; a.hmap = true; a.host_mm = nullptr; a.host_info = nullptr;
+	a.image_w = image ? xsize : 0; a.image_h = image ? ysize : 0;
+	return TW_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ voxels
 int tw_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420, float *out) {
 	int rc = check_ctx(ctx); if (rc) return rc;

@@ -860,22 +860,16 @@ uint32_t twi_erode_chunk_for(size_t budget, uint32_t ntiles, int xsize, int ysiz
 	return (uint32_t)c;
 }
 
-// tw_erode_parallel: `num_threads` droplets of ONE heightmap in flight (0 = as many groups as keep the GPU busy)
-int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads) {
-	ctx->last_erosion_steps = 0;
-	if (num_iters == 0 || p->erode_amount <= 0.0) return TW_OK; // erosion disabled, src/erosion.cpp:16
-	if (xsize <= 0 || ysize <= 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_erode_parallel: empty heightmap");
-	if (!ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
-	int rc = tw_reserve(ctx, 2, 4096);
-	if (rc) return rc;
-	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
-	unsigned *d_next = (unsigned *)(d_steps + 1);
-	TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, 16, ctx->stream));
+size_t twi_erode_parallel_scratch_bytes(int xsize, int ysize) {return (size_t)(xsize + 2*PAD)*(ysize + 2*PAD)*sizeof(float);}
+
+// tw_erode_parallel's work on ctx->stream, nothing waits: pad into `scratch` (twi_erode_parallel_scratch_bytes), the droplets, unpad with the lower clamp
+// *d_min_zval (nullptr: min_zval). d_steps accumulates the droplet moves (the caller zeroes it); d_next is the droplet counter, zeroed here.
+int twi_erode_parallel_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zval, float min_zval, uint32_t num_iters,
+                               const tw_erosion_params *p, uint32_t num_threads, unsigned long long *d_steps, unsigned *d_next) {
 	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
-	rc = tw_reserve(ctx, 1, (size_t)NX*NY*sizeof(float));
-	if (rc) return rc;
-	float *d_pad = (float *)ctx->d_scratch[1];
+	float *d_pad = (float *)scratch;
 	cudaStream_t const st = ctx->stream;
+	TW_CUDA(ctx, cudaMemsetAsync(d_next, 0, sizeof(unsigned), st));
 	DArgs A;
 	memset(&A, 0, sizeof(A));
 	A.E = make_eparams(p);
@@ -887,8 +881,26 @@ int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float mi
 	A.dir_table = ctx->d_dir_table; A.steps_out = d_steps; A.next_droplet = d_next;
 	launch_droplets_g<M_ATOMIC>(pick_group(groups), st, A, 2, 0);
 	TW_LAUNCH_CHECK(ctx);
-	unpad_kernel<<<dim3((xsize + 255)/256, ysize, 1), 256, 0, st>>>(d_pad, d_map, xsize, ysize, NX, NY, nullptr, min_zval);
+	unpad_kernel<<<dim3((xsize + 255)/256, ysize, 1), 256, 0, st>>>(d_pad, d_map, xsize, ysize, NX, NY, d_min_zval, min_zval);
 	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+// tw_erode_parallel: `num_threads` droplets of ONE heightmap in flight (0 = as many groups as keep the GPU busy)
+int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads) {
+	ctx->last_erosion_steps = 0;
+	if (num_iters == 0 || p->erode_amount <= 0.0) return TW_OK; // erosion disabled, src/erosion.cpp:16
+	if (xsize <= 0 || ysize <= 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_erode_parallel: empty heightmap");
+	if (!ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
+	int rc = tw_reserve(ctx, 2, 4096);
+	if (rc) return rc;
+	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
+	TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, sizeof(unsigned long long), ctx->stream));
+	rc = tw_reserve(ctx, 1, twi_erode_parallel_scratch_bytes(xsize, ysize));
+	if (rc) return rc;
+	rc = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_map, xsize, ysize, nullptr, min_zval, num_iters, p, num_threads, d_steps, (unsigned *)(d_steps + 1));
+	if (rc) return rc;
+	cudaStream_t const st = ctx->stream;
 	unsigned long long h_steps = 0;
 	TW_CUDA(ctx, cudaMemcpyAsync(&h_steps, d_steps, sizeof(h_steps), cudaMemcpyDeviceToHost, st));
 	TW_CUDA(ctx, cudaStreamSynchronize(st));

@@ -16,9 +16,10 @@ struct tw_async_state {
 	bool tiles = false;             // the pending job is a tile job (else a 2-D grid or a voxel build)
 	bool voxel = false;             // the pending job is a voxel build: triangle count and flipped voxels staged at ctx->h_pinned + 0 / + 8 (uint64 each)
 	uint64_t *host_ntris = nullptr, *host_changed = nullptr;
-	bool hmap = false;              // the pending job is tw_proc_gen_heightmap_launch: a twi_hmap_stage at ctx->h_pinned
+	bool hmap = false;              // the pending job is tw_proc_gen_heightmap_launch or tw_erode_launch: a twi_hmap_stage at ctx->h_pinned (the erosion job
+	                                // fills only its min_z, bad, fail and steps, and has no host_info)
 	tw_heightmap_info *host_info = nullptr;
-	int image_w = 0, image_h = 0;   // > 0: the packed image becomes the context's tw_set_heightmap image when the job completes
+	int image_w = 0, image_h = 0;   // > 0: the packed image becomes (again) the context's tw_set_heightmap image when the job completes
 	cudaEvent_t done = nullptr;
 	float *host_out = nullptr;      // user host buffer (nullptr => result stays on device)
 	tw_minmax *host_mm = nullptr;
@@ -201,6 +202,10 @@ size_t twi_erode_spec_scratch_bytes(int xsize, int ysize);
 int    twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zvals, float min_zval, uint32_t num_iters,
                               const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds);
 int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads);
+// tw_erode_parallel in parts: its padded scratch, and the enqueue (lower clamp *d_min_zval, or min_zval when it is nullptr; moves added to *d_steps)
+size_t twi_erode_parallel_scratch_bytes(int xsize, int ysize);
+int    twi_erode_parallel_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zval, float min_zval, uint32_t num_iters,
+                                  const tw_erosion_params *p, uint32_t num_threads, unsigned long long *d_steps, unsigned *d_next);
 size_t   twi_erode_scratch_bytes(const tw_ctx *ctx, uint32_t chunk, int xsize, int ysize);
 uint32_t twi_erode_chunk_for(size_t budget, uint32_t ntiles, int xsize, int ysize);
 int twi_erode_enqueue(tw_ctx *ctx, cudaStream_t st, int lane, void *scratch, uint32_t capacity, float *maps, uint32_t nt, int xsize, int ysize,
@@ -228,6 +233,8 @@ int twi_from_floats_u16(tw_ctx *ctx, const float *d_vals, size_t n, float val_mu
 struct twi_hmap_stage {float min_z, max_z, val_mult, val_add, mesh_file_scale, mesh_file_tz, val_div; unsigned bad, fail, pad_; unsigned long long steps;};
 int twi_hmap_scales(tw_ctx *ctx, const unsigned *d_mm, float mesh_height_scale, float mesh_scale_z_inv, twi_hmap_stage *d_stage);
 int twi_from_floats_u16_dev(tw_ctx *ctx, const float *d_vals, size_t n, const twi_hmap_stage *d_stage, uint8_t *d_out);
+// *d_min = the minimum of the ordered min/max d_mm as a float (tw_erode_launch's lower clamp of the image, left on the device)
+int twi_ord_min(tw_ctx *ctx, const unsigned *d_mm, float *d_min);
 // scratch slot 1 bytes twi_heightgen uses for this grid (the sine mode's tables; 0 otherwise)
 size_t twi_heightgen_slot1_bytes(const tw_grid2d *g, const tw_height_params *p);
 int twi_to_floats_u16(tw_ctx *ctx, const uint8_t *d_data, size_t n, float val_mult, float val_add, float *d_vals);

@@ -61,6 +61,8 @@ __global__ void hmap_scales_kernel(const unsigned *__restrict__ mm, float mhs, f
 	st->val_div = __double2float_rn(__ddiv_rn(1.0, (double)val_mult)); // src/heightmap.cpp:206
 }
 
+__global__ void ord_min_kernel(const unsigned *__restrict__ mm, float *__restrict__ out) {*out = tw_ord2f(mm[0]);}
+
 int grid_for(const tw_ctx *ctx, size_t n) {size_t b = (n + 1023)/1024; if (b > ctx->num_sms*16) b = ctx->num_sms*16; if (b < 1) b = 1; return (int)b;}
 
 } // namespace
@@ -80,6 +82,12 @@ int twi_hmap_scales(tw_ctx *ctx, const unsigned *d_mm, float mesh_height_scale, 
 
 int twi_from_floats_u16_dev(tw_ctx *ctx, const float *d_vals, size_t n, const twi_hmap_stage *d_stage, uint8_t *d_out) {
 	from_floats_u16_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>(d_vals, n, 0.0f, 0.0f, reinterpret_cast<uint16_t *>(d_out), const_cast<unsigned *>(&d_stage->bad), d_stage);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+int twi_ord_min(tw_ctx *ctx, const unsigned *d_mm, float *d_min) {
+	ord_min_kernel<<<1, 1, 0, ctx->stream>>>(d_mm, d_min);
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }

@@ -2,6 +2,7 @@
 //
 //   tw3d::mesh_xy_grid_cache_t   <->  mesh_xy_grid_cache_t                    src/mesh.h:22-45, src/mesh_gen.cpp:588-650,754-792
 //   tw3d::apply_erosion          <->  apply_erosion(float*,int,int,float,unsigned)   src/function_registry.h:354, src/erosion.cpp:14
+//   tw3d::erode_heightmap_async  <->  heightmap_t::run_erosion on the set_heightmap image, without stalling the frame   src/heightmap.cpp:153-187
 //   tw3d::noise_gen_3d           <->  noise_gen_3d::{set_rand_seeds,gen_sines}        src/upsurface.h:39-50
 //   tw3d::create_procedural      <->  voxel_manager::create_procedural               src/voxels.h:196, src/voxels.cpp:278-346
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
@@ -434,6 +435,37 @@ inline tiles_job proc_gen_heightmap_async(unsigned width, unsigned height, float
 	if (rc != TW_OK) {detail::fail(rc, "proc_gen_heightmap_async", c);}
 	if (set_image) {detail::tls().hmap_w = (int)width; detail::tls().hmap_h = (int)height;}
 	return tiles_job(c, &jobs, number);
+}
+
+// apply_erosion / apply_erosion_parallel as jobs that do not stall the frame (tw_erode_launch): they return at once, and ready() / wait() on the tiles_job say
+// when heightmap (host or device; pageable host memory makes the launch wait for its copies) holds what the synchronous call would have left there.
+namespace detail {
+	inline tiles_job erode_async(float *heightmap, int xsize, int ysize, float min_zval, float val_mult, float val_add, unsigned num_iters, int num_threads,
+	                             float *vals, const char *what) {
+		tw_erosion_params const e = erosion_params_from_globals();
+		tw_erosion_job const job = {heightmap, xsize, ysize, min_zval, val_mult, val_add, num_iters, &e, num_threads < 0 ? TW_EROSION_SERIAL : TW_EROSION_OPENMP,
+		                            num_threads < 0 ? 0u : (uint32_t)num_threads, vals};
+		tw_ctx *c = ctx();
+		std::atomic<uint64_t> &jobs = tls().tile_jobs;
+		uint64_t const number = ++jobs;
+		int const rc = tw_erode_launch(c, &job);
+		if (rc != TW_OK) {fail(rc, what, c);}
+		return tiles_job(c, &jobs, number);
+	}
+}
+constexpr int serial_order = -1; // erode_heightmap_async: the serial droplet order of apply_erosion instead of apply_erosion_parallel's threads
+inline tiles_job apply_erosion_async(float *heightmap, int xsize, int ysize, float min_zval, unsigned num_iters) {
+	return detail::erode_async(heightmap, xsize, ysize, min_zval, 0.0f, 0.0f, num_iters, serial_order, nullptr, "apply_erosion_async");
+}
+inline tiles_job apply_erosion_parallel_async(float *heightmap, int xsize, int ysize, float min_zval, unsigned num_iters, unsigned num_threads = 0) {
+	return detail::erode_async(heightmap, xsize, ysize, min_zval, 0.0f, 0.0f, num_iters, (int)num_threads, nullptr, "apply_erosion_parallel_async");
+}
+// heightmap_t::run_erosion (src/heightmap.cpp:153-187) on the image set_heightmap() keeps on this thread's device, as one job: to_floats with val_mult /
+// val_add (get_mh_texture_mult / _add), erosion with min_zval = the map's minimum, from_floats back into the image. num_threads: serial_order, or the threads
+// of apply_erosion_parallel (0 = fill the GPU). vals (optional, width*height floats, host or device) receives the eroded floats. The frame's
+// create_tiles_async_from_heightmap() samples the eroded image once the job is ready, or completes the job first when launched earlier.
+inline tiles_job erode_heightmap_async(float val_mult, float val_add, unsigned num_iters, int num_threads = serial_order, float *vals = nullptr) {
+	return detail::erode_async(nullptr, 0, 0, 0.0f, val_mult, val_add, num_iters, num_threads, vals, "erode_heightmap_async");
 }
 
 // Several frames' tile jobs in flight at once: a pool of n shared contexts of this thread's ctx() (tw_create_shared - the same tables and heightmap

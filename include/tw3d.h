@@ -266,6 +266,41 @@ TW_API int tw_erode_parallel(tw_ctx *ctx, float *heightmap, int xsize, int ysize
  * min_zval_all for every tile. */
 TW_API int tw_erode_tiles(tw_ctx *ctx, float *heightmaps, uint32_t ntiles, int xsize, int ysize, const float *min_zvals, float min_zval_all,
                    uint32_t num_iters, const tw_erosion_params *p);
+/* tw_erode / tw_erode_parallel of ONE map as the context's ASYNCHRONOUS job (heightmap_t::run_erosion, src/heightmap.cpp:153-187, without holding the host):
+ * everything is enqueued without the host reading anything back (the speculative erosion's rounds end on the device, the step count is staged) and the
+ * completing poll reports the result.
+ * - heightmap != NULL: xsize*ysize floats eroded in place, device or host. After the completing poll the map and tw_last_erosion_steps() equal
+ *   tw_erode(heightmap, xsize, ysize, min_zval, num_iters, ep) bit for bit in TW_EROSION_SERIAL mode, and tw_erode_parallel(..., num_threads) in
+ *   TW_EROSION_OPENMP mode (bit for bit with num_threads == 1; order-dependent as that call's result otherwise). The serial order's "made no progress" case
+ *   is reported by the poll as TW_ERR_STATE with tw_erode's message.
+ * - heightmap == NULL: the context's tw_set_heightmap image (root context only; xsize = ysize = 0, min_zval unused). After a poll that returns TW_OK the image,
+ *   vals and tw_last_erosion_steps() equal the synchronous chain tw_heightmap_to_floats_u16(image, val_mult, val_add) -> tw_minmax_f32 -> tw_erode (or
+ *   tw_erode_parallel) with min_zval = that minimum (run_erosion's min_zval) -> tw_heightmap_from_floats_u16(val_mult, val_add) back into the image, bit for
+ *   bit. The launch first completes every shared context's job; until a poll returns TW_OK the context has no image (a shared context's
+ *   tw_create_tiles_launch_hmap gets TW_ERR_STATE; the parent's own completes this job first). A packed value outside [0,256) makes the completing poll
+ *   return TW_ERR_ARG with tw_heightmap_from_floats_u16's message; a poll that returns an error leaves the context without an image.
+ * - num_iters == 0 or erode_amount <= 0 (src/erosion.cpp:16): the job does no work and reports 0 steps; the image keeps its bytes and vals is not written.
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it (wait = 0 returns TW_ERR_NOT_READY while it runs), every
+ *   other entry point and tw_destroy complete it first. On a shared context (float maps only) it runs beside the other contexts' jobs.
+ * - The launch never waits for the device, except that copies to or from a PAGEABLE host heightmap / vals block it (see "Host output buffers" above). Every
+ *   buffer is reserved before anything is enqueued. heightmap and vals must stay valid until the completing poll.
+ * - Errors, nothing enqueued and nothing changed: TW_ERR_ARG for a NULL job or ep, an empty map, sizes or vals given with a float map's counterpart (sizes
+ *   with the image, vals with a float map), a bad mode, num_threads != 0 in TW_EROSION_SERIAL mode, the image on a shared context; TW_ERR_STATE for the
+ *   image when none is set, and without the sin table when there is work to do. */
+#define TW_EROSION_SERIAL 0   /* tw_erode: the reference's serial droplet order */
+#define TW_EROSION_OPENMP 1   /* tw_erode_parallel: the reference's `#pragma omp parallel for` mode with num_threads droplets in flight */
+typedef struct tw_erosion_job {
+	float                    *heightmap;        /* xsize*ysize floats, device or host; NULL: the context's tw_set_heightmap image */
+	int                       xsize, ysize;     /* with heightmap; 0 with the image */
+	float                     min_zval;         /* with heightmap: the lower clamp, as tw_erode's */
+	float                     val_mult, val_add;/* with the image: the unpack's and the pack's scalars (get_mh_texture_mult / _add) */
+	uint32_t                  num_iters;
+	const tw_erosion_params  *ep;               /* required; copied during the launch */
+	int                       mode;             /* TW_EROSION_SERIAL or TW_EROSION_OPENMP */
+	uint32_t                  num_threads;      /* TW_EROSION_OPENMP: as tw_erode_parallel's (0 = fill the GPU); must be 0 otherwise */
+	float                    *vals;             /* with the image, optional: the eroded floats before the pack, device or host */
+} tw_erosion_job;
+TW_API int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job);
 /* Fused tile pipeline = the height fill AND the per-tile erosion of tile_t::create_zvals (src/tiled_mesh.cpp:467-515) for a batch of tiles:
  * exactly tw_heightgen_tiles followed by tw_erode_tiles(min_zval_all = min_zval) in one call (one upload of the origins, one download of
  * the result, per-tile z range fused). When memory forces several chunks, generation of chunk k+1 is issued on a separate stream and

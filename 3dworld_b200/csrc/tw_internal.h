@@ -5,33 +5,41 @@
 #include <stddef.h>
 #include <stdio.h>
 #include <string.h>
+#include <utility>
 #include <vector>
 #include "../../include/tw3d.h"
 
-// The one asynchronous job a context may have in flight (tw_heightgen_2d_launch, tw_create_tiles_launch or tw_voxel_build_launch). `done` is recorded on
-// ctx->stream after everything the job enqueued (the tile pipeline's other streams are joined into ctx->stream first); the small per-tile results are staged
-// in ctx->h_pinned at the offsets below and unpacked into the caller's host arrays by the poll that reports completion.
-struct tw_async_state {
-	bool pending = false;
-	bool tiles = false;             // the pending job is a tile job (else a 2-D grid or a voxel build)
-	bool voxel = false;             // the pending job is a voxel build: triangle count and flipped voxels staged at ctx->h_pinned + 0 / + 8 (uint64 each)
-	uint64_t *host_ntris = nullptr, *host_changed = nullptr;
-	bool hmap = false;              // the pending job is tw_proc_gen_heightmap_launch or tw_erode_launch: a twi_hmap_stage at ctx->h_pinned (the erosion job
-	                                // fills only its min_z, bad, fail and steps, and has no host_info)
-	tw_heightmap_info *host_info = nullptr;
-	int image_w = 0, image_h = 0;   // > 0: the packed image becomes (again) the context's tw_set_heightmap image when the job completes
-	cudaEvent_t done = nullptr;
-	float *host_out = nullptr;      // user host buffer (nullptr => result stays on device)
+// A voxel build's counts in ctx->h_pinned (tw_voxel_build_launch)
+struct twi_voxel_stage {unsigned long long ntris, changed;};
+
+// The one asynchronous job a context may have in flight, as the poll that reports its completion unpacks it: which kind it is, what it staged in
+// ctx->h_pinned and where that goes. A job is pending when its kind is not NONE. Only twi_launch_job makes a job pending and only poll_job (tw_api.cu)
+// takes it back.
+struct twi_job {
+	enum kind_t {NONE, TILES, VOXEL, HMAP};
+	kind_t kind = NONE;
+	// TILES (tile jobs and frames; a 2-D grid is n = 1 with its min/max at offset 0; a relight stages nothing): n tiles' results at byte offsets into
+	// ctx->h_pinned, each unpacked only when its destination is set
+	uint32_t n = 0;
+	uint64_t *host_steps = nullptr;       // the erosion step count (&ctx->last_erosion_steps when the job eroded)
 	tw_minmax *host_mm = nullptr;
-	uint32_t n_mm = 0;
-	// tile job: where the staged results go and what the bounds combination needs
 	tw_tile_bounds *host_bounds = nullptr;
 	float *host_min_nz = nullptr;
-	uint8_t *host_flags = nullptr;  // has_any_grass
-	bool steps = false;             // an erosion step counter is staged
-	float dx = 0.0f, dy = 0.0f;
+	uint8_t *host_flags = nullptr;        // has_any_grass
+	float dx = 0.0f, dy = 0.0f;           // what the bounds combination needs
 	uint32_t size = 0;
-	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0, off_flags = 0; // byte offsets into ctx->h_pinned
+	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0, off_flags = 0;
+	// VOXEL: a twi_voxel_stage at ctx->h_pinned
+	uint64_t *host_ntris = nullptr, *host_changed = nullptr;
+	// HMAP (tw_proc_gen_heightmap_launch; tw_erode_launch, which fills only the stage's min_z, bad, fail and steps and has no host_info): a twi_hmap_stage at
+	// ctx->h_pinned
+	tw_heightmap_info *host_info = nullptr;
+	int image_w = 0, image_h = 0;         // > 0: the packed image becomes (again) the context's tw_set_heightmap image when the job completes
+};
+
+struct tw_async_state {
+	twi_job job;
+	cudaEvent_t done = nullptr;           // recorded on ctx->stream after everything the pending job enqueued
 };
 
 struct tw_ctx {
@@ -87,6 +95,25 @@ bool tw_is_device_ptr(const void *p);
 	return tw_set_error((ctx), TW_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
 #define TW_LAUNCH_CHECK(ctx) do { (ctx)->launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { \
 	return tw_set_error((ctx), TW_ERR_CUDA, "%s:%d kernel launch: %s", __FILE__, __LINE__, cudaGetErrorString(e_)); } } while (0)
+
+// Makes `job` the context's pending job (the previous one has been completed): enqueue() puts the job's work on ctx->stream, with every other stream it used
+// joined into ctx->stream, and ctx->async.done is recorded behind it. When either fails, the call waits for every stream of the context, so none of the job
+// still runs on the scratch or the pinned staging when the error is returned, and no job is pending.
+template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, const twi_job &job, Enqueue &&enqueue) {
+	int rc = enqueue();
+	if (rc == TW_OK) {
+		cudaError_t const e = cudaEventRecord(ctx->async.done, ctx->stream);
+		if (e != cudaSuccess) rc = tw_set_error(ctx, TW_ERR_CUDA, "recording the job's event: %s", cudaGetErrorString(e));
+	}
+	if (rc != TW_OK) {
+		cudaStreamSynchronize(ctx->stream);
+		for (cudaStream_t s : ctx->aux_stream) {if (s) cudaStreamSynchronize(s);}
+		for (cudaStream_t s : ctx->heavy_stream) {if (s) cudaStreamSynchronize(s);}
+		return rc;
+	}
+	ctx->async.job = job;
+	return TW_OK;
+}
 
 // ---- constants shared by host and device code (src/3DWorld.h:43,129; src/sinf.h:8-9) ----
 #define TW_TSIZE 32768

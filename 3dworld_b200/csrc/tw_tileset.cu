@@ -431,22 +431,14 @@ int tw_tile_set_shadows_launch(tw_tile_set *s, const tw_tile_set_request *req) {
 	// everything is reserved before anything is enqueued (tw_reserve synchronises the stream and may re-allocate)
 	rc = tw_reserve(ctx, 0, R.dev_bytes()); if (rc) return rc;
 	rc = tw_reserve_pinned(ctx, R.ints_bytes); if (rc) return rc;
-	auto enqueue = [&]() -> int {
+	twi_job pending; // a relight stages nothing for the poll
+	pending.kind = twi_job::TILES;
+	rc = twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0)); // a frame's job on another context may still use the slabs
-		int const r = relight_enqueue(ctx, s, R, (char *)ctx->d_scratch[0], (char *)ctx->h_pinned); if (r) return r;
-		TW_CUDA(ctx, cudaEventRecord(ctx->async.done, ctx->stream));
-		return TW_OK;
-	};
-	rc = enqueue();
-	if (rc) { // nothing may still run on the scratch; what the slots hold is unknown now, so they are recomputed next time
-		cudaStreamSynchronize(ctx->stream);
-		invalidate_all(s);
-		return rc;
-	}
+		return relight_enqueue(ctx, s, R, (char *)ctx->d_scratch[0], (char *)ctx->h_pinned);
+	});
+	if (rc) {invalidate_all(s); return rc;} // what the slots hold is unknown now, so they are recomputed next time
 	relight_commit(s, R, req->recomputed);
-	tw_async_state &a = ctx->async;
-	a.pending = true; a.tiles = true; a.steps = false; a.n_mm = 0;
-	a.host_mm = nullptr; a.host_bounds = nullptr; a.host_min_nz = nullptr; a.host_flags = nullptr;
 	return TW_OK;
 }
 

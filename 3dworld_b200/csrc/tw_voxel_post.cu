@@ -443,7 +443,7 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 // enqueued, so no re-allocation synchronises in the middle.
 //   device slot 0: [counters (256 B) | field (unless vals is device memory) | padded flags | 2 frontiers (remove_unconnected > 0) | tables | block sums | block
 //                  offsets | zix_xy (host input)]
-//   pinned:        [ntris, changed (64 B) | sine coefficients | tables | zix_xy (host input)]
+//   pinned:        [twi_voxel_stage (64 B) | sine coefficients | tables | zix_xy (host input)]
 extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 	if (!ctx) return TW_ERR_ARG;
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -500,8 +500,9 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 	unsigned *d_sums = (unsigned *)sp; sp += sb;
 	unsigned long long *d_offsets = (unsigned long long *)sp; sp += ofb;
 	const unsigned *d_z = dev_z ? b->zix_xy : (b->zix_xy ? (const unsigned *)sp : nullptr);
-	// from here on everything is enqueued; a failure waits for what was, so none of it still runs on the scratch when the error is returned
-	auto enqueue = [&]() -> int {
+	twi_job pending;
+	pending.kind = twi_job::VOXEL; pending.host_ntris = mc ? b->ntris : nullptr; pending.host_changed = b->changed;
+	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(cnt, 0, 256, ctx->stream));
 		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h + off_rdata); if (r) return r;}
 		else if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, b->vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
@@ -531,15 +532,9 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 		}
 		if (b->vals && !dev_v && (fill || rm)) {TW_CUDA(ctx, cudaMemcpyAsync(b->vals, d_v, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 		if (b->outside) {TW_CUDA(ctx, cudaMemcpyAsync(b->outside, d_o, n, cudaMemcpyDefault, ctx->stream));}
-		TW_CUDA(ctx, cudaMemcpyAsync(h, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-		TW_CUDA(ctx, cudaMemcpyAsync(h + 8, d_changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-		TW_CUDA(ctx, cudaEventRecord(ctx->async.done, ctx->stream));
+		twi_voxel_stage *const st = (twi_voxel_stage *)h;
+		TW_CUDA(ctx, cudaMemcpyAsync(&st->ntris, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+		TW_CUDA(ctx, cudaMemcpyAsync(&st->changed, d_changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		return TW_OK;
-	};
-	rc = enqueue();
-	if (rc) {cudaStreamSynchronize(ctx->stream); return rc;}
-	tw_async_state &a = ctx->async;
-	a.pending = true; a.tiles = false; a.voxel = true; a.host_mm = nullptr; a.n_mm = 0;
-	a.host_ntris = mc ? b->ntris : nullptr; a.host_changed = b->changed;
-	return TW_OK;
+	});
 }

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib3dworld_b200.so")
 
 MGEN_SINE, MGEN_SIMPLEX, MGEN_PERLIN, MGEN_SIMPLEX_GPU, MGEN_DWARP_GPU = range(5)
-TW_OK, TW_ERR_NO_DEVICE, TW_ERR_CUDA, TW_ERR_ARG, TW_ERR_STATE, TW_ERR_NOT_READY = 0, -1, -2, -3, -4, -5
+TW_OK, TW_ERR_NO_DEVICE, TW_ERR_CUDA, TW_ERR_ARG, TW_ERR_STATE, TW_ERR_NOT_READY, TW_ERR_CANCELED = 0, -1, -2, -3, -4, -5, -6
 TW_EROSION_SERIAL, TW_EROSION_OPENMP = 0, 1
 PQ_SIN_TERMS, PQ_SIN_TERMS_SCALED, PQ_EXACT_ZVAL = 0, 1, 2   # tw_point_query.kind
 
@@ -25,6 +25,10 @@ class TwError(RuntimeError):
     def __init__(self, status, msg):
         super().__init__("tw3d status %d: %s" % (status, msg))
         self.status = status
+
+
+class TwCanceled(TwError):
+    """A poll completed a job that Context.cancel() cut short (TW_ERR_CANCELED): the job's outputs are unspecified."""
 
 
 # ---- POD mirrors of include/tw3d.h ----
@@ -175,7 +179,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
                "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
-               "tw_proc_gen_heightmap_launch", "tw_erode_launch"]
+               "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel"]
 
 
 def _load():
@@ -195,6 +199,7 @@ def _load():
     L.tw_stream.restype = vp
     L.tw_launch_count.argtypes = [vp]
     L.tw_launch_count.restype = C.c_uint64
+    L.tw_cancel.argtypes = [vp]
     L.tw_build_sin_table.argtypes = [vp]
     L.tw_build_sin_table.restype = None
     L.tw_compute_scale.argtypes = [C.c_float, C.c_int]
@@ -525,7 +530,12 @@ class Context:
 
     def _check(self, rc):
         if rc != TW_OK:
-            raise TwError(rc, lib.tw_last_error(self._h).decode())
+            raise (TwCanceled if rc == TW_ERR_CANCELED else TwError)(rc, lib.tw_last_error(self._h).decode())
+
+    def cancel(self):
+        """tw_cancel: asks this context's pending job to stop and returns at once. The poll that completes a job cut short raises TwCanceled; a job
+        that has already finished, or has nothing left to cut, completes as usual. Raises TwError (TW_ERR_STATE) for a job that touches a TileSet."""
+        self._check(lib.tw_cancel(self._h))
 
     @property
     def stream(self):
@@ -569,6 +579,7 @@ class Context:
         rc = lib.tw_heightgen_2d_poll(self._h, int(wait))
         if rc == TW_ERR_NOT_READY:
             return False
+        self._tiles_job = None
         self._check(rc)
         return True
 

@@ -99,6 +99,12 @@ int poll_job(tw_ctx *ctx, int wait) {
 	if (ev == cudaErrorNotReady) return TW_ERR_NOT_READY;
 	twi_job const j = std::exchange(a.job, twi_job()); // no job is pending from here on, whether it failed or not
 	if (ev != cudaSuccess) return tw_set_error(ctx, TW_ERR_CUDA, "asynchronous job failed: %s", cudaGetErrorString(ev));
+	if (ctx->h_job->stopped) { // a cancellation point acted (tw_cancel): nothing is unpacked, and an image the job would have set stays unset
+		ctx->last_erosion_steps = 0;
+		cudaError_t const e = cudaGetLastError();
+		if (e != cudaSuccess) return tw_set_error(ctx, TW_ERR_CUDA, "asynchronous job failed: %s", cudaGetErrorString(e));
+		return tw_set_error(ctx, TW_ERR_CANCELED, "the job was cancelled (tw_cancel)");
+	}
 	const char *h = (const char *)ctx->h_pinned;
 	int status = TW_OK; // of the completed work (a heightmap job's pack or erosion)
 	switch (j.kind) {
@@ -141,8 +147,12 @@ int poll_job(tw_ctx *ctx, int wait) {
 	return status;
 }
 
-int finish_pending(tw_ctx *ctx) { // complete the pending job before other work reuses the scratch buffers
-	return poll_job(ctx, 1);
+// Completes the pending job before other work reuses the scratch buffers. A job cut short by tw_cancel completes here without an error: the caller threw
+// its outputs away and the entry point goes on with its own work; only the explicit polls report TW_ERR_CANCELED.
+int finish_pending(tw_ctx *ctx) {
+	int const rc = poll_job(ctx, 1);
+	if (rc == TW_ERR_CANCELED) {ctx->err[0] = 0; return TW_OK;}
+	return rc;
 }
 
 // tw_set_sin_table / tw_set_sine_params / tw_set_heightmap: refused on a shared context; on a parent, the job of every shared context completes first,
@@ -164,6 +174,11 @@ tw_ctx *new_ctx(int device) {
 	{int sms = 0; if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && sms > 0) ctx->num_sms = (unsigned)sms; else cudaGetLastError();}
 	if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {delete ctx; cudaGetLastError(); return nullptr;}
 	if (cudaEventCreateWithFlags(&ctx->async.done, cudaEventDisableTiming) != cudaSuccess) {cudaStreamDestroy(ctx->stream); delete ctx; cudaGetLastError(); return nullptr;}
+	bool const ok = (cudaStreamCreateWithFlags(&ctx->cancel_stream, cudaStreamNonBlocking) == cudaSuccess
+	                 && cudaMalloc(&ctx->d_job_words, sizeof(twi_job_words)) == cudaSuccess && cudaMemset(ctx->d_job_words, 0, sizeof(twi_job_words)) == cudaSuccess
+	                 && cudaMallocHost(&ctx->h_job, sizeof(twi_job_host)) == cudaSuccess);
+	if (!ok) {tw_destroy(ctx); cudaGetLastError(); return nullptr;}
+	memset(ctx->h_job, 0, sizeof(twi_job_host));
 	return ctx;
 }
 
@@ -216,6 +231,25 @@ int validate_weights(tw_ctx *ctx, const tw_weight_params *wp, tw_weight_params &
 } // namespace
 
 int twi_finish_pending(tw_ctx *ctx) {twi_borrow_tables(ctx); return finish_pending(ctx);} // the entry points of the other translation units call it first
+
+int twi_job_start(tw_ctx *ctx, unsigned *seq) {
+	if (ctx->cancel_sent) { // the copy of an earlier tw_cancel lands before this job's number is written (it names an older job either way)
+		TW_CUDA(ctx, cudaStreamSynchronize(ctx->cancel_stream));
+		ctx->cancel_sent = false;
+	}
+	if (++ctx->job_seq == 0) ctx->job_seq = 1; // 0 means "no job"
+	*seq = ctx->job_seq;
+	// the previous job has completed, so its copy out of h_job->start is done
+	ctx->h_job->start[0] = ctx->job_seq; ctx->h_job->start[1] = 0u;
+	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->d_job_words->job, ctx->h_job->start, 2*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));
+	return TW_OK;
+}
+
+int twi_job_end(tw_ctx *ctx) {
+	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->h_job->stopped, &ctx->d_job_words->stopped, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+	TW_CUDA(ctx, cudaMemsetAsync(&ctx->d_job_words->job, 0, sizeof(unsigned), ctx->stream));
+	return TW_OK;
+}
 
 void twi_borrow_tables(tw_ctx *ctx) {
 	tw_ctx const *p = ctx->parent;
@@ -276,6 +310,9 @@ void tw_destroy(tw_ctx *ctx) {
 		ctx->d_sin_table = nullptr; ctx->d_dir_table = nullptr; ctx->d_simplex_lut = nullptr; ctx->d_glm3_lut = nullptr; ctx->d_sine_params = nullptr; ctx->d_hmap = nullptr;
 	}
 	cudaStreamSynchronize(ctx->stream);
+	if (ctx->cancel_stream) {cudaStreamSynchronize(ctx->cancel_stream); cudaStreamDestroy(ctx->cancel_stream);}
+	if (ctx->d_job_words) cudaFree(ctx->d_job_words);
+	if (ctx->h_job) cudaFreeHost(ctx->h_job);
 	if (ctx->spec_graph) cudaGraphExecDestroy(ctx->spec_graph);
 	for (int i = 0; i < 3; ++i) {if (ctx->d_scratch[i]) cudaFree(ctx->d_scratch[i]);}
 	if (ctx->d_sin_table) cudaFree(ctx->d_sin_table);
@@ -300,6 +337,18 @@ const char *tw_last_error(const tw_ctx *ctx) {return ctx ? ctx->err : "null cont
 void *tw_stream(tw_ctx *ctx) {return ctx ? (void *)ctx->stream : nullptr;}
 uint64_t tw_launch_count(const tw_ctx *ctx) {return ctx ? ctx->launches : 0;}
 uint64_t tw_last_erosion_steps(const tw_ctx *ctx) {return ctx ? ctx->last_erosion_steps : 0;}
+
+// "cancel job k" into the device words, by a copy on the context's cancel stream: nothing waits, nothing goes to ctx->stream
+int tw_cancel(tw_ctx *ctx) {
+	int rc = check_ctx(ctx); if (rc) return rc;
+	twi_job const &j = ctx->async.job;
+	if (j.kind == twi_job::NONE) return TW_OK;
+	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "a job that touches a tile set cannot be cancelled: the set's state was committed at its launch");
+	ctx->h_job->cancel = j.seq;
+	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->d_job_words->cancel, &ctx->h_job->cancel, sizeof(unsigned), cudaMemcpyHostToDevice, ctx->cancel_stream));
+	ctx->cancel_sent = true;
+	return TW_OK;
+}
 
 int tw_sync(tw_ctx *ctx) {
 	int rc = check_ctx(ctx); if (rc) return rc;
@@ -352,7 +401,7 @@ int tw_heightgen_2d_launch(tw_ctx *ctx, const tw_grid2d *g, const tw_height_para
 	if (!dev_out) {rc = twi_ensure_aux_streams(ctx); if (rc) return rc;}
 	unsigned *d_mm = mm ? (unsigned *)((char *)ctx->d_scratch[2] + OFF_MM) : nullptr;
 	twi_job pending; // the tile unpack of one min/max at offset 0
-	pending.kind = twi_job::TILES; pending.n = 1; pending.host_mm = mm;
+	pending.kind = twi_job::TILES; pending.n = 1; pending.host_mm = mm; pending.cancellable = true;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		if (d_mm) {rc = twi_init_minmax(ctx, d_mm, 1); if (rc) return rc;}
 		rc = twi_heightgen(ctx, g, p, enable_glaciate, min_start_sin, nullptr, 1, d_out, d_mm, dev_out ? nullptr : out); // host out: band-wise D2H overlapped with compute
@@ -745,6 +794,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	}
 	twi_job pending;
 	pending.kind = twi_job::TILES; pending.n = ntiles; pending.host_steps = erode ? &ctx->last_erosion_steps : nullptr;
+	pending.cancellable = (tail == nullptr); // a tail commits a tile set's state
 	pending.host_mm = o->mm; pending.host_bounds = o->bounds; pending.host_min_nz = o->min_normal_z; pending.host_flags = (want_f && !dev_f) ? sh->has_any_grass : nullptr;
 	pending.dx = dx; pending.dy = dy; pending.size = size;
 	pending.off_steps = off_steps; pending.off_mm = off_mm; pending.off_sub = off_sub; pending.off_min_nz = off_mnz; pending.off_flags = off_f;
@@ -1172,7 +1222,7 @@ int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job) {
 	unsigned *const d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_TILES);
 	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
 	twi_job pending;
-	pending.kind = twi_job::HMAP; pending.image_w = image ? xsize : 0; pending.image_h = image ? ysize : 0;
+	pending.kind = twi_job::HMAP; pending.image_w = image ? xsize : 0; pending.image_h = image ? ysize : 0; pending.cancellable = true;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(d_st, 0, sizeof(twi_hmap_stage), ctx->stream));
 		if (erode) {
@@ -1302,6 +1352,7 @@ int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, f
 	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
 	twi_job pending;
 	pending.kind = twi_job::HMAP; pending.host_info = out->info; pending.image_w = out->set_image ? (int)width : 0; pending.image_h = out->set_image ? (int)height : 0;
+	pending.cancellable = true;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(d_st, 0, sizeof(twi_hmap_stage), ctx->stream));
 		int r = twi_init_minmax(ctx, d_mm, 1); if (r) return r;

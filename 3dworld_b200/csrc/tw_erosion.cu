@@ -189,13 +189,17 @@ struct DArgs {
 	int halo_rule;              // a droplet ends when |zi - start row| exceeds this
 	unsigned it0, it1;          // droplets [it0, it1) = this sweep
 	SpecArgs S;                 // M_SPEC; M_GLOBAL with S.ctl != nullptr: walk the window's head in place if it is SP_HUGE
+	twi_job_words *jw;          // in a job: the context's job words (tw_cancel), M_GLOBAL / M_ATOMIC / M_WINDOW / M_WHOLE start no droplet once it is cancelled; nullptr otherwise
 };
 
-template<int G, int MODE>
+// CANCEL: the variant with the cancellation point, for jobs (see launch_droplets); synchronous calls and short latency-mode walks run the one without it, whose
+// code is the same as before tw_cancel existed (the check's branch makes ptxas lay the loop out differently, which costs a serial chain about 4 %)
+template<int G, int MODE, bool CANCEL>
 __global__ void __launch_bounds__(128)
 droplet_kernel(DArgs const A)
 {
 	constexpr bool SHARED = (MODE == M_ATOMIC), FROZEN = (MODE == M_FROZEN), SPEC = (MODE == M_SPEC), WIN = (MODE == M_WINDOW || MODE == M_FROZEN || MODE == M_SPEC), WHOLE = (MODE == M_WHOLE);
+	static_assert(!CANCEL || (!FROZEN && !SPEC), "M_SPEC stops at its round boundary (spec_round_kernel); M_FROZEN is never in a job");
 	static_assert(!SPEC || G == 32, "M_SPEC: one droplet per warp");
 	// M_FROZEN shares M_WINDOW's machinery: the window is the droplet's PRIVATE view (sweep-start heights + its own writes); see hadd
 	constexpr int TPW = 32/G; // heightmaps per warp
@@ -427,6 +431,12 @@ droplet_kernel(DArgs const A)
 				active = false;
 			}
 			else if (iter >= (FROZEN ? A.it1 : num_iters)) {active = false;}
+			// cancelled (tw_cancel): the group stops as if num_iters had been reached. Its leader reads the job words before every 8th droplet only (the
+			// droplet index, group-uniform), which keeps the read's latency off nearly every droplet of the serial chain
+			else if (CANCEL && (iter & 7u) == 0u && __shfl_sync(gmask, (sub == 0 && twi_cancelled(A.jw)) ? 1u : 0u, grp*G)) {
+				if (sub == 0) {twi_mark_stopped(A.jw);}
+				active = false;
+			}
 			else {
 				rgen.s1 = (int)iter + 11; rgen.s2 = 79*(int)iter + 121;
 				xi = PAD + (rgen.rand()%xsize);
@@ -628,12 +638,26 @@ droplet_kernel(DArgs const A)
 
 constexpr size_t SMEM_MAX_BLOCK = 227u*1024u; // sm_90: 227 KB of dynamic shared memory per block
 
-template<int G, int MODE>
-void launch_droplets(cudaStream_t st, DArgs const &A, unsigned warps_per_block, size_t smem_per_group) {
+template<int G, int MODE, bool CANCEL>
+void launch_droplets_c(cudaStream_t st, DArgs const &A, unsigned warps_per_block, size_t smem_per_group) {
 	unsigned const groups_per_block = warps_per_block*(32/G);
 	size_t const smem = smem_per_group*groups_per_block;
-	if (smem > 48*1024) {cudaFuncSetAttribute(droplet_kernel<G, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);}
-	droplet_kernel<G, MODE><<<(A.nslots + groups_per_block - 1)/groups_per_block, 32*warps_per_block, smem, st>>>(A);
+	if (smem > 48*1024) {cudaFuncSetAttribute(droplet_kernel<G, MODE, CANCEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);}
+	droplet_kernel<G, MODE, CANCEL><<<(A.nslots + groups_per_block - 1)/groups_per_block, 32*warps_per_block, smem, st>>>(A);
+}
+
+// The variant with the cancellation point runs for a job's erosion (A.jw set: twi_erode_enqueue / twi_erode_parallel_enqueue inside twi_launch_job) in the
+// throughput mode, and in the latency modes for walks of at least CANCEL_MIN_DROPLETS droplets per map. A shorter latency-mode walk is not worth the
+// check: the checking loop's layout costs a serial chain about 4 % (tools/bench_frame_tiles.py's 16-tile frame, 1000 droplets per tile: ready after
+// 23.0-23.7 ms against 22.1 ms), while the whole walk is over in under 0.1 s (22 ms for 1000 droplets in that frame). In M_GLOBAL the cost hides behind
+// thousands of walks in flight (bench.py's fused 16384-tile row is unchanged). DESIGN §4g.
+constexpr unsigned CANCEL_MIN_DROPLETS = 4096;
+template<int G, int MODE>
+void launch_droplets(cudaStream_t st, DArgs const &A, unsigned warps_per_block, size_t smem_per_group) {
+	if constexpr (MODE != M_SPEC && MODE != M_FROZEN) {
+		if (A.jw && (MODE == M_GLOBAL || A.num_iters >= CANCEL_MIN_DROPLETS)) {launch_droplets_c<G, MODE, true>(st, A, warps_per_block, smem_per_group); return;}
+	}
+	launch_droplets_c<G, MODE, false>(st, A, warps_per_block, smem_per_group);
 }
 
 template<int MODE>
@@ -789,7 +813,7 @@ int twi_erode_enqueue(tw_ctx *ctx, cudaStream_t st, int lane, void *scratch, uin
 	memset(&A, 0, sizeof(A));
 	A.E = make_eparams(p);
 	A.xsize = xsize; A.ysize = ysize; A.num_iters = num_iters; A.dir_table = ctx->d_dir_table; A.steps_out = d_steps;
-	A.min_zvals = d_min_zvals; A.min_zval_all = min_zval_all;
+	A.min_zvals = d_min_zvals; A.min_zval_all = min_zval_all; A.jw = ctx->in_job ? ctx->d_job_words : nullptr;
 	if (plan_whole(ctx->num_sms, nt, xsize, ysize)) { // whole maps in shared memory, straight from / to the caller's tiles
 		A.maps = maps; A.slot0 = 0; A.nslots = nt; A.perm = d_perm;
 		A.WX = NX; A.WY = NY; A.P = whole_pitch(NX, NY); A.win_elems = (unsigned)A.P*NY;
@@ -878,7 +902,7 @@ int twi_erode_parallel_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsi
 	unsigned groups = num_threads ? num_threads : 65536u; // auto: the 65536-map operating point of pick_group() (8 lanes per droplet)
 	if (groups > num_iters) {groups = num_iters;}
 	A.padded = d_pad; A.ntiles = groups; A.slot0 = 0; A.nslots = groups; A.xsize = xsize; A.ysize = ysize; A.num_iters = num_iters;
-	A.dir_table = ctx->d_dir_table; A.steps_out = d_steps; A.next_droplet = d_next;
+	A.dir_table = ctx->d_dir_table; A.steps_out = d_steps; A.next_droplet = d_next; A.jw = ctx->in_job ? ctx->d_job_words : nullptr;
 	launch_droplets_g<M_ATOMIC>(pick_group(groups), st, A, 2, 0);
 	TW_LAUNCH_CHECK(ctx);
 	unpad_kernel<<<dim3((xsize + 255)/256, ysize, 1), 256, 0, st>>>(d_pad, d_map, xsize, ysize, NX, NY, d_min_zval, min_zval);
@@ -928,10 +952,12 @@ __global__ void spec_init_kernel(SpecArgs S, unsigned num_iters, size_t ntile_st
 //   commit    the prefix [lo, f): the logs go into the map (disjoint tiles: any order), the slots get their next droplets; behind f, droplets whose tiles a
 //             committed droplet touched are walked again from the start; every stamping droplet takes its stamps back
 // The kernel advances the round counter. In the graph form (spec_loop_graph: the body of a conditional WHILE node) it also ends the loop once every droplet is
-// committed, or - with *fail = the rounds run - after max_rounds + 1 rounds without finishing; the host-driven form passes max_rounds = UINT_MAX.
+// committed, or - with *fail = the rounds run - after max_rounds + 1 rounds without finishing; the host-driven form passes max_rounds = UINT_MAX. In the graph
+// form a cancelled job (tw_cancel, the job words jw) also ends the loop after the round; the host-driven form (tw_erode) is never cancelled.
 constexpr unsigned SPEC_CLUSTER = 8, SPEC_MAX_SLOTS = SPEC_CLUSTER*32;
 __global__ void __cluster_dims__(SPEC_CLUSTER, 1, 1) __launch_bounds__(1024) spec_round_kernel(SpecArgs S, unsigned num_iters, float *__restrict__ padded, int NX, unsigned long long *__restrict__ steps_total,
-                                                                                               unsigned max_rounds, unsigned *__restrict__ fail, cudaGraphConditionalHandle loop, bool in_graph) {
+                                                                                               unsigned max_rounds, unsigned *__restrict__ fail, cudaGraphConditionalHandle loop, bool in_graph,
+                                                                                               twi_job_words *jw) {
 	namespace cg = cooperative_groups;
 	cg::cluster_group cluster = cg::this_cluster();
 	unsigned const s = (blockIdx.x*blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -983,7 +1009,9 @@ __global__ void __cluster_dims__(SPEC_CLUSTER, 1, 1) __launch_bounds__(1024) spe
 		bool const done = (f >= num_iters);
 		if (done) {S.ctl[3] = 1u;}
 		else if (round >= max_rounds) {*fail = round + 1u;}
-		if (in_graph && (done || round >= max_rounds)) {cudaGraphSetConditional(loop, 0u);}
+		bool const cancel = in_graph && !done && round < max_rounds && twi_cancelled(jw);
+		if (cancel) {twi_mark_stopped(jw);}
+		if (in_graph && (done || round >= max_rounds || cancel)) {cudaGraphSetConditional(loop, 0u);}
 	}
 }
 
@@ -1050,7 +1078,7 @@ static int spec_loop_graph(tw_ctx *ctx, cudaStream_t st, DArgs const &W, unsigne
 	if (e == cudaSuccess) {e = cudaStreamBeginCaptureToGraph(st, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed);}
 	if (e == cudaSuccess) {
 		launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));
-		spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(W.S, num_iters, d_pad, NX, d_steps, max_rounds, d_fail, h, true);
+		spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(W.S, num_iters, d_pad, NX, d_steps, max_rounds, d_fail, h, true, W.jw);
 		cudaError_t const le = cudaGetLastError();
 		cudaGraph_t body = nullptr;
 		e = cudaStreamEndCapture(st, &body);
@@ -1090,7 +1118,7 @@ int twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, 
 	memset(&A, 0, sizeof(A));
 	A.E = make_eparams(p);
 	A.xsize = xsize; A.ysize = ysize; A.num_iters = num_iters; A.dir_table = ctx->d_dir_table;
-	A.padded = d_pad; A.slot0 = 0;
+	A.padded = d_pad; A.slot0 = 0; A.jw = ctx->in_job ? ctx->d_job_words : nullptr; // the graph's round kernel reads them (tw_erode's host rounds never do)
 	pad_kernel<<<dim3((NX + 255)/256, NY, 1), 256, 0, st>>>(d_map, d_pad, xsize, ysize, NX, NY, A.E.wpz_minus_half_dxy, nullptr, nullptr);
 	TW_LAUNCH_CHECK(ctx);
 	size_t const init_n = std::max(ntile, (size_t)S.B);
@@ -1106,7 +1134,7 @@ int twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, 
 		for (unsigned round = 0;; ++round) {
 			if (round > max_rounds) return tw_set_error(ctx, TW_ERR_STATE, "speculative erosion made no progress (%u rounds)", round);
 			launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));
-			spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(S, num_iters, d_pad, NX, d_steps, 0xffffffffu, d_fail, 0, false);
+			spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(S, num_iters, d_pad, NX, d_steps, 0xffffffffu, d_fail, 0, false, nullptr);
 			TW_LAUNCH_CHECK(ctx);
 			if (round + 1 >= min_rounds && (round & 7u) == 7u) { // poll "done" every 8 rounds (not before the window can have covered all droplets): the rounds in between are queued back to back
 				TW_CUDA(ctx, cudaMemcpyAsync((void *)h_done, S.ctl + 3, sizeof(unsigned), cudaMemcpyDeviceToHost, st));

@@ -18,6 +18,8 @@ struct twi_voxel_stage {unsigned long long ntris, changed;};
 struct twi_job {
 	enum kind_t {NONE, TILES, VOXEL, HMAP};
 	kind_t kind = NONE;
+	bool cancellable = false;             // tw_cancel may stop it (set by the launch; a job that touches a tile set is not)
+	unsigned seq = 0;                     // the context's number of the job (twi_launch_job), the one tw_cancel names
 	// TILES (tile jobs and frames; a 2-D grid is n = 1 with its min/max at offset 0; a relight stages nothing): n tiles' results at byte offsets into
 	// ctx->h_pinned, each unpacked only when its destination is set
 	uint32_t n = 0;
@@ -41,6 +43,24 @@ struct tw_async_state {
 	twi_job job;
 	cudaEvent_t done = nullptr;           // recorded on ctx->stream after everything the pending job enqueued
 };
+
+// The device words behind tw_cancel, one set per context at a fixed address. `job` is the number of the job that runs on ctx->stream (0 between jobs:
+// twi_launch_job writes it at the job's start and clears it at its end), `cancel` the number of the last job tw_cancel named. A cancellation point acts
+// only when the two are equal and not 0, so a cancel that lands after its job has ended can never stop the next one, nor a synchronous call. A point that
+// acts sets `stopped`, which the job's end copies to twi_job_host::stopped for the completing poll. Read as one 64-bit word (twi_job_words_load).
+struct twi_job_words {unsigned cancel, job, stopped, pad;};
+// Pinned host side: the source of the job-start copy {job, stopped = 0}, the source of tw_cancel's copy, and the staged `stopped`
+struct twi_job_host {unsigned start[2]; unsigned cancel; unsigned stopped;};
+#ifdef __CUDACC__
+__device__ __forceinline__ unsigned long long twi_job_words_load(const twi_job_words *w) { // past L1: the words change while the kernel runs
+	unsigned long long v;
+	asm volatile("ld.relaxed.gpu.u64 %0, [%1];" : "=l"(v) : "l"(w));
+	return v;
+}
+__device__ __forceinline__ bool twi_job_words_hit(unsigned long long v) {return (unsigned)(v >> 32) != 0u && (unsigned)(v >> 32) == (unsigned)v;}
+__device__ __forceinline__ bool twi_cancelled(const twi_job_words *w) {return twi_job_words_hit(twi_job_words_load(w));}
+__device__ __forceinline__ void twi_mark_stopped(twi_job_words *w) {*(volatile unsigned *)&w->stopped = 1u;}
+#endif
 
 struct tw_ctx {
 	int device = 0;
@@ -71,6 +91,13 @@ struct tw_ctx {
 	void  *h_pinned = nullptr;
 	size_t pinned_bytes = 0;
 	tw_async_state async;
+	// tw_cancel: the words the cancellation points read, their pinned host side, the stream of tw_cancel's copy (never ctx->stream), the last job number
+	twi_job_words *d_job_words = nullptr;
+	twi_job_host *h_job = nullptr;
+	cudaStream_t cancel_stream = nullptr;
+	unsigned job_seq = 0;
+	bool cancel_sent = false;               // a tw_cancel copy may still be in flight: the next job start waits for it
+	bool in_job = false;                    // set while twi_launch_job enqueues: the droplet walks it enqueues check the words, a synchronous call's do not
 	cudaGraphExec_t spec_graph = nullptr;   // the speculative erosion's round loop (tw_erosion.cu), kept while its kernel arguments stay the same
 	std::vector<unsigned char> spec_key;    // those arguments
 	void *dist = nullptr;        // tw_dist_state (tw_multi.cu): NCCL communicator of the one-process-per-GPU mode
@@ -96,11 +123,18 @@ bool tw_is_device_ptr(const void *p);
 #define TW_LAUNCH_CHECK(ctx) do { (ctx)->launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { \
 	return tw_set_error((ctx), TW_ERR_CUDA, "%s:%d kernel launch: %s", __FILE__, __LINE__, cudaGetErrorString(e_)); } } while (0)
 
+// The job's number in the device words, on ctx->stream, before its work (twi_job_start sets *seq) / after it: `stopped` to the pinned staging, `job` cleared
+int twi_job_start(tw_ctx *ctx, unsigned *seq);
+int twi_job_end(tw_ctx *ctx);
+
 // Makes `job` the context's pending job (the previous one has been completed): enqueue() puts the job's work on ctx->stream, with every other stream it used
-// joined into ctx->stream, and ctx->async.done is recorded behind it. When either fails, the call waits for every stream of the context, so none of the job
-// still runs on the scratch or the pinned staging when the error is returned, and no job is pending.
+// joined into ctx->stream, between the job's start and end in the device words, and ctx->async.done is recorded behind it. When any step fails, the call
+// waits for every stream of the context, so none of the job still runs on the scratch or the pinned staging when the error is returned, and no job is pending.
 template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, const twi_job &job, Enqueue &&enqueue) {
-	int rc = enqueue();
+	unsigned seq = 0;
+	int rc = twi_job_start(ctx, &seq);
+	if (rc == TW_OK) {ctx->in_job = true; rc = enqueue(); ctx->in_job = false;}
+	if (rc == TW_OK) {rc = twi_job_end(ctx);}
 	if (rc == TW_OK) {
 		cudaError_t const e = cudaEventRecord(ctx->async.done, ctx->stream);
 		if (e != cudaSuccess) rc = tw_set_error(ctx, TW_ERR_CUDA, "recording the job's event: %s", cudaGetErrorString(e));
@@ -112,6 +146,7 @@ template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, const twi_job &job, 
 		return rc;
 	}
 	ctx->async.job = job;
+	ctx->async.job.seq = seq;
 	return TW_OK;
 }
 

@@ -51,10 +51,12 @@ __global__ void shadow_init_kernel(unsigned char *smask, unsigned long long *key
 	for (size_t k = i; k < ncells; k += stride) {smask[k] = val;}
 	for (size_t k = i; k < nkeys; k += stride) {keys[k] = 0ull;}
 }
-// one thread per ray of one tile of the wave: blockIdx.y = position in the wave's tile list
+// one thread per ray of one tile of the wave: blockIdx.y = position in the wave's tile list. In a cancelled job (tw_cancel) a block returns at entry.
 __global__ void shadow_rays_kernel(const float *__restrict__ zvals, unsigned char *__restrict__ smask, int n, ShadowDev S, const int *__restrict__ wave_tiles,
-	const int *__restrict__ nb_x, const int *__restrict__ nb_y, const float *__restrict__ ox, const float *__restrict__ oy, unsigned long long *__restrict__ kx, unsigned long long *__restrict__ ky)
+	const int *__restrict__ nb_x, const int *__restrict__ nb_y, const float *__restrict__ ox, const float *__restrict__ oy, unsigned long long *__restrict__ kx, unsigned long long *__restrict__ ky,
+	twi_job_words *jw)
 {
+	if (twi_cancelled(jw)) {if (threadIdx.x == 0) {twi_mark_stopped(jw);} return;}
 	int const ray = blockIdx.x*blockDim.x + threadIdx.x;
 	if (ray >= 4*n) return;
 	int const tile = wave_tiles[blockIdx.y];
@@ -193,7 +195,7 @@ int twi_shadow_enqueue(tw_ctx *ctx, cudaStream_t st, const twi_shadow_plan &P, c
 		for (int l = 0; l < nlevels; ++l) {
 			int const w1 = P.wave_start[l + 1];
 			for (int w0 = P.wave_start[l]; P.trace && w0 < w1; w0 += YMAX) {
-				shadow_rays_kernel<<<dim3((4*n + 127)/128, std::min(YMAX, w1 - w0)), 128, 0, s>>>(d_z, d_m, n, P.S, d_wave + w0, d_nbx, d_nby, d_ox, d_oy, d_kx, d_ky);
+				shadow_rays_kernel<<<dim3((4*n + 127)/128, std::min(YMAX, w1 - w0)), 128, 0, s>>>(d_z, d_m, n, P.S, d_wave + w0, d_nbx, d_nby, d_ox, d_oy, d_kx, d_ky, ctx->d_job_words);
 				TW_LAUNCH_CHECK(ctx);
 			}
 			for (int w0 = P.wave_start[l]; w0 < w1; w0 += YMAX) {

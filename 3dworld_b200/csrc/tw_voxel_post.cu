@@ -76,16 +76,24 @@ __global__ void seed_centre_kernel(unsigned char *outside, tw_voxel_post_params 
 // 80GB HBM3 at 400 W (tools/bench_voxel_build.py --remove-only, 512^3 sine / GLM / 20000-generation column): grid.sync() 135 / 138 / 84 ms, 64 ns sleeps
 // 36.8 / 33.0 / 90.5 ms, 128 ns 35.6 / 32.4 / 91.8 ms, 256 ns 35.5 / 32.4 / 91.8 ms, the former launch per generation 35.3 / 32.5 / 157 ms.
 // bar[0]: arrivals, bar[1]: generation; both 0 before the launch.
+// tw_cancel: only the last block to arrive acts on the job words, before it releases the others: in a cancelled job it zeroes the next frontier's count
+// (*next, final once every block has arrived), which every thread reads after the barrier - so all blocks leave in the same generation. (Every block
+// loads the words beside its arrival, so the load adds no latency to the barrier; the others drop the value.)
 #ifndef TW_FLOOD_SLEEP_NS
 #define TW_FLOOD_SLEEP_NS 128
 #endif
-__device__ __forceinline__ void grid_barrier(unsigned *bar) {
+__device__ __forceinline__ void grid_barrier(unsigned *bar, unsigned *next, twi_job_words *jw) {
 	__syncthreads();
 	if (threadIdx.x == 0) {
 		volatile unsigned *gen = bar + 1;
 		unsigned const g0 = *gen; // cannot advance before this block arrives
 		__threadfence();          // this block's frontier, counts and flags before the arrival
-		if (atomicAdd(bar, 1u) == gridDim.x - 1) {bar[0] = 0; __threadfence(); atomicAdd(bar + 1, 1u);}
+		unsigned long long const words = twi_job_words_load(jw);
+		if (atomicAdd(bar, 1u) == gridDim.x - 1) {
+			bar[0] = 0;
+			if (twi_job_words_hit(words) && *(volatile unsigned *)next != 0u) {*next = 0u; twi_mark_stopped(jw);}
+			__threadfence(); atomicAdd(bar + 1, 1u);
+		}
 		else {while (*gen == g0) {__nanosleep(TW_FLOOD_SLEEP_NS);}}
 		__threadfence();
 	}
@@ -98,7 +106,8 @@ __device__ __forceinline__ void grid_barrier(unsigned *bar) {
 // by other blocks are read past L1 (__ldcg); flag bytes are read volatile by claim().
 constexpr int FLOOD_THREADS = 256;
 __global__ void __launch_bounds__(FLOOD_THREADS)
-flood_fill_kernel(unsigned char *outside, unsigned nx, unsigned ny, unsigned nz, unsigned *f0, unsigned *f1, unsigned *cnt, unsigned char fill_val, unsigned char bit)
+flood_fill_kernel(unsigned char *outside, unsigned nx, unsigned ny, unsigned nz, unsigned *f0, unsigned *f1, unsigned *cnt, unsigned char fill_val, unsigned char bit,
+                  twi_job_words *jw)
 {
 	unsigned const nxnz = nx*nz, tid = blockIdx.x*blockDim.x + threadIdx.x, stride = gridDim.x*blockDim.x;
 	if (tid == 0) {cnt[3] = __ldcg(cnt);}
@@ -119,7 +128,7 @@ flood_fill_kernel(unsigned char *outside, unsigned nx, unsigned ny, unsigned nz,
 			TW_FF(z, nz, 1u)
 #undef TW_FF
 		}
-		grid_barrier(cnt + 4);
+		grid_barrier(cnt + 4, n_out, jw);
 	}
 }
 // :808-826 (pass 0) and :847-857 (pass 1); gate (optional): does nothing when *gate == 0 (remove_interior_holes bails out without a seed, :844)
@@ -302,7 +311,8 @@ int flood_blocks(tw_ctx *ctx, unsigned *blocks) {
 int launch_flood(tw_ctx *ctx, unsigned blocks, unsigned char *d_o, const tw_voxel_post_params *vp, unsigned *f0, unsigned *f1, unsigned *cnt, unsigned char fill_val) {
 	unsigned nx = vp->nx, ny = vp->ny, nz = vp->nz;
 	unsigned char bit = TW_VOX_ANCHORED;
-	void *args[] = {&d_o, &nx, &ny, &nz, &f0, &f1, &cnt, &fill_val, &bit};
+	twi_job_words *jw = ctx->d_job_words;
+	void *args[] = {&d_o, &nx, &ny, &nz, &f0, &f1, &cnt, &fill_val, &bit, &jw};
 	TW_CUDA(ctx, cudaLaunchCooperativeKernel((const void *)flood_fill_kernel, dim3(blocks), dim3(FLOOD_THREADS), args, 0, ctx->stream));
 	ctx->launches++;
 	return TW_OK;
@@ -501,7 +511,7 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 	unsigned long long *d_offsets = (unsigned long long *)sp; sp += ofb;
 	const unsigned *d_z = dev_z ? b->zix_xy : (b->zix_xy ? (const unsigned *)sp : nullptr);
 	twi_job pending;
-	pending.kind = twi_job::VOXEL; pending.host_ntris = mc ? b->ntris : nullptr; pending.host_changed = b->changed;
+	pending.kind = twi_job::VOXEL; pending.host_ntris = mc ? b->ntris : nullptr; pending.host_changed = b->changed; pending.cancellable = true;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(cnt, 0, 256, ctx->stream));
 		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h + off_rdata); if (r) return r;}

@@ -311,30 +311,42 @@ inline void create_zvals_batch(const int32_t *origins_xy, unsigned ntiles, unsig
 // outputs once it returns true (wait() blocks instead). The outputs named in `out` (tw_tile_outputs, include/tw3d.h) must stay valid until then; zvals and
 // normals_rgba may be device memory, or page-locked host memory for a launch that never blocks. One job per context: any other call on this thread's
 // context completes the job first (tile_job_pool, below, keeps several in flight). Not copyable; a handle that is destroyed while its job runs waits for it.
+// cancel() asks a job whose outputs are no longer wanted (tiles out of range, a map reloaded, the scene quit) to stop and returns at once (tw_cancel); the job
+// is then ready soon, and cancelled() says whether its outputs are unspecified: true when its poll reports that it was cut short, and also when another
+// call completed it after cancel() (a later launch on the context, or tile_job_pool's slot scan before it relaunches the slot), since this handle cannot
+// tell whether the cancel acted. cancel() on a tile set's job throws (TW_ERR_STATE).
 class tiles_job {
 	tw_ctx *c = nullptr;
 	std::atomic<uint64_t> const *latest = nullptr; // the launch count of c's thread
 	uint64_t number = 0;
-	bool done = true;
+	bool done = true, was_cancelled = false, cancel_asked = false;
 	bool poll(bool wait) {
 		if (done) return true;
-		if (latest->load() != number) {done = true; return true;} // a later launch on the same context completed this job before it started
+		if (latest->load() != number) {done = true; was_cancelled = cancel_asked; return true;} // a later launch on the same context completed this job before it started
 		int const rc = tw_create_tiles_poll(c, wait ? 1 : 0);
 		if (rc == TW_ERR_NOT_READY) return false;
 		done = true;
+		if (rc == TW_ERR_CANCELED) {was_cancelled = true; return true;}
 		if (rc != TW_OK) {detail::fail(rc, "create_tiles_async", c);}
 		return true;
 	}
 public:
 	tiles_job() = default;
 	tiles_job(tw_ctx *ctx_, std::atomic<uint64_t> const *latest_, uint64_t number_) : c(ctx_), latest(latest_), number(number_), done(false) {}
-	tiles_job(tiles_job &&o) noexcept : c(o.c), latest(o.latest), number(o.number), done(o.done) {o.done = true;}
-	tiles_job &operator=(tiles_job &&o) {if (this != &o) {wait(); c = o.c; latest = o.latest; number = o.number; done = o.done; o.done = true;} return *this;}
+	tiles_job(tiles_job &&o) noexcept : c(o.c), latest(o.latest), number(o.number), done(o.done), was_cancelled(o.was_cancelled), cancel_asked(o.cancel_asked) {o.done = true;}
+	tiles_job &operator=(tiles_job &&o) {if (this != &o) {wait(); c = o.c; latest = o.latest; number = o.number; done = o.done; was_cancelled = o.was_cancelled; cancel_asked = o.cancel_asked; o.done = true;} return *this;}
 	tiles_job(tiles_job const &) = delete;
 	tiles_job &operator=(tiles_job const &) = delete;
 	~tiles_job() {try {wait();} catch (...) {}}
 	bool ready() {return poll(false);}
 	void wait() {poll(true);}
+	void cancel() {
+		if (done || latest->load() != number) return; // completed already
+		int const rc = tw_cancel(c);
+		if (rc != TW_OK) {detail::fail(rc, "tiles_job::cancel", c);}
+		cancel_asked = true;
+	}
+	bool cancelled() const {return was_cancelled;} // once the job is ready
 };
 // wpz_max / size: the water level and tile size of the bounds (tile_t::create_zvals, src/tiled_mesh.cpp:517-541); dx, dy also scale the normals (get_norm).
 // The overload with `shading` (tw_tile_shading, include/tw3d.h) adds the AO map (calc_mesh_ao_lighting) and the terrain weights texture (create_texture's terrain
@@ -483,7 +495,7 @@ class tile_job_pool {
 		slot *pick = nullptr;
 		for (auto &s : slots) {
 			int const rc = tw_create_tiles_poll(s->c, 0);   // TW_OK: nothing in flight (a finished job is unpacked into its outputs here)
-			if (rc == TW_OK) {pick = s.get(); break;}
+			if (rc == TW_OK || rc == TW_ERR_CANCELED) {pick = s.get(); break;} // a cancelled job's slot is free again
 			if (rc != TW_ERR_NOT_READY) {detail::fail(rc, "create_tiles_async", s->c);}
 		}
 		if (!pick) {pick = slots[0].get(); for (auto &s : slots) {if (s->launched < pick->launched) pick = s.get();}}

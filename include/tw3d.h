@@ -35,7 +35,8 @@ typedef enum tw_status {
 	TW_ERR_CUDA      = -2,   /* a CUDA runtime call failed; see tw_last_error() */
 	TW_ERR_ARG       = -3,   /* invalid argument (the reference would assert) */
 	TW_ERR_STATE     = -4,   /* tables not set (tw_set_sin_table / tw_set_sine_params) */
-	TW_ERR_NOT_READY = -5    /* tw_heightgen_2d_poll / tw_create_tiles_poll: result not available yet (mirrors build_arrays() returning 0 with no_wait) */
+	TW_ERR_NOT_READY = -5,   /* tw_heightgen_2d_poll / tw_create_tiles_poll: result not available yet (mirrors build_arrays() returning 0 with no_wait) */
+	TW_ERR_CANCELED  = -6    /* tw_heightgen_2d_poll / tw_create_tiles_poll: tw_cancel cut the job short; its outputs are unspecified (see tw_cancel) */
 } tw_status;
 
 /* mesh_gen_mode values, src/3DWorld.h:1399 */
@@ -142,6 +143,28 @@ TW_API const char *tw_last_error(const tw_ctx *ctx);
 TW_API int  tw_sync(tw_ctx *ctx);                         /* cudaStreamSynchronize on the context stream */
 TW_API void *tw_stream(tw_ctx *ctx);                      /* the cudaStream_t all work of this context is issued on */
 TW_API uint64_t tw_launch_count(const tw_ctx *ctx);       /* kernels launched by this context so far (bench.py gpu_launches) */
+/* Asks the context's pending asynchronous job to stop, for work the caller no longer wants (a map reloaded or the scene quit while it is eroded, tiles
+ * that went out of range, a voxel model replaced while its fills run). Returns at once: it never waits for the device and enqueues nothing on the
+ * context's stream. Called by the thread that owns the context, like every other entry point.
+ * - TW_OK whether or not a job is pending; with no job, or a job that has already finished, nothing changes. TW_ERR_ARG for a NULL ctx.
+ * - TW_ERR_STATE for a job that touches a tile set (tw_tile_set_shadows_launch, tw_tile_set_create_tiles_launch), which keeps running unaffected: a set's
+ *   state is committed at launch, in launch order, and frames launched later on other shared contexts already rely on it.
+ * - The job stops at its next cancellation point: a droplet walk within its next 8 droplets (tile erosion, the OpenMP mode; on a batch small enough to be
+ *   walked all at once, only walks of at least 4096 droplets per map - shorter ones take well under 0.1 s and run to their end), the serial order's
+ *   speculative erosion at its next round (a round is at most 64 moves per walker), a voxel flood fill at its next generation, the mesh shadows at their
+ *   next wave.
+ *   What is already enqueued of everything else still runs (generation, the tile tail, marching cubes, the end-of-job copies); a job without a
+ *   cancellation point (a tw_heightgen_2d_launch grid, a heightmap job without erosion) completes as if tw_cancel had not been called.
+ * - The completing poll (tw_create_tiles_poll / tw_heightgen_2d_poll) returns TW_ERR_CANCELED when a cancellation point acted. Every output of the job is
+ *   then unspecified: device and host buffers may be partly written, and the host arrays the poll fills (mm, bounds, info, ntris, ...) are not written.
+ *   tw_last_erosion_steps() is 0, and a job that would have set the context's heightmap image (set_image, erosion of the image) leaves the context without
+ *   one. Nothing else changes: the next job gives what it gives on a fresh context. Otherwise the poll returns what it would have returned, with every
+ *   output bit-identical to the job without tw_cancel.
+ * - Every entry point, tw_set_heightmap and tw_destroy still complete the pending job first; calling tw_cancel before them makes that wait short. A job
+ *   they complete that was cut short counts as completed, not as an error: the call goes on with its own work (a new map is loaded, the next job is
+ *   launched) and returns its own status. Only the two polls report TW_ERR_CANCELED. The same holds for a parent's table setters, which complete the jobs of
+ *   its shared contexts. Synchronous calls are not jobs and are never cancelled. */
+TW_API int  tw_cancel(tw_ctx *ctx);
 
 /* ---- host-side table generation (bit-exact restatements; tiny, run once) ---- */
 /* create_sin_table(), src/mesh_gen.cpp:72-81: tab[i]=sinf(i/sscale), tab[i+32768]=cosf(i/sscale) with the host libm. */

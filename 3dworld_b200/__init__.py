@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, "lib3dworld_b200.so")
 
 MGEN_SINE, MGEN_SIMPLEX, MGEN_PERLIN, MGEN_SIMPLEX_GPU, MGEN_DWARP_GPU = range(5)
 TW_OK, TW_ERR_NO_DEVICE, TW_ERR_CUDA, TW_ERR_ARG, TW_ERR_STATE, TW_ERR_NOT_READY, TW_ERR_CANCELED = 0, -1, -2, -3, -4, -5, -6
-TW_EROSION_SERIAL, TW_EROSION_OPENMP = 0, 1
+TW_EROSION_SERIAL, TW_EROSION_OPENMP, TW_EROSION_SWEEPS = 0, 1, 2
 PQ_SIN_TERMS, PQ_SIN_TERMS_SCALED, PQ_EXACT_ZVAL = 0, 1, 2   # tw_point_query.kind
 
 
@@ -156,6 +156,11 @@ class ErosionJobArgs(C.Structure):
                 ("num_iters", C.c_uint32), ("ep", C.c_void_p), ("mode", C.c_int), ("num_threads", C.c_uint32), ("vals", C.c_void_p)]
 
 
+class SweepParams(C.Structure):
+    """tw_sweep_params (include/tw3d.h): tw_erode_sweeps' sweep and halo for tw_erode_launch_ex's TW_EROSION_SWEEPS mode."""
+    _fields_ = [("sweep", C.c_uint32), ("halo", C.c_int)]
+
+
 class Rng(C.Structure):
     _fields_ = [("rseed1", C.c_int64), ("rseed2", C.c_int64)]
 
@@ -179,7 +184,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
                "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
-               "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel"]
+               "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex"]
 
 
 def _load():
@@ -239,6 +244,7 @@ def _load():
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_erode_parallel.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_uint32, C.POINTER(ErosionParams), C.c_uint32]
     L.tw_erode_launch.argtypes = [vp, C.POINTER(ErosionJobArgs)]
+    L.tw_erode_launch_ex.argtypes = [vp, C.POINTER(ErosionJobArgs), C.POINTER(SweepParams)]
     L.tw_erode_tiles.argtypes = [vp, vp, C.c_uint32, C.c_int, C.c_int, vp, C.c_float, C.c_uint32, C.POINTER(ErosionParams)]
     L.tw_last_erosion_steps.argtypes = [vp]
     L.tw_last_erosion_steps.restype = C.c_uint64
@@ -749,24 +755,30 @@ class Context:
         self._check(lib.tw_erode_parallel(self._h, _ptr(h), xs, ys, min_zval, num_iters, C.byref(ep), num_threads))
         return h
 
-    def _erode_launch(self, job, heightmap, xsize, ysize, min_zval, val_mult, val_add, num_iters, ep, num_threads, vals):
-        mode = TW_EROSION_SERIAL if num_threads is None else TW_EROSION_OPENMP
+    def _erode_launch(self, job, heightmap, xsize, ysize, min_zval, val_mult, val_add, num_iters, ep, num_threads, vals, sweep=None, halo=None):
+        if (sweep is None) != (halo is None):
+            raise ValueError("sweep and halo select the sweeps mode together")
+        sweeps = sweep is not None
+        mode = TW_EROSION_SWEEPS if sweeps else TW_EROSION_SERIAL if num_threads is None else TW_EROSION_OPENMP
         a = ErosionJobArgs(_ptr(heightmap), xsize, ysize, min_zval, val_mult, val_add, num_iters, C.cast(C.pointer(ep), C.c_void_p), mode,
                            0 if num_threads is None else num_threads, _ptr(vals))
-        self._check(lib.tw_erode_launch(self._h, C.byref(a)))
+        sw = SweepParams(sweep, halo) if sweeps else None
+        self._check(lib.tw_erode_launch_ex(self._h, C.byref(a), C.byref(sw) if sweeps else None))
         self._tiles_job = job
         return job
 
-    def erode_launch(self, h, min_zval, num_iters, ep, num_threads=None):
+    def erode_launch(self, h, min_zval, num_iters, ep, num_threads=None, sweep=None, halo=None):
         """tw_erode_launch on h (numpy [ys, xs] or CUDA tensor, in place) as this context's asynchronous job; create_tiles_poll completes it.
-        num_threads=None: the serial order (erode()); an int: the OpenMP mode (erode_parallel(num_threads), 0 = fill the GPU). h stays referenced until then."""
+        num_threads=None: the serial order (erode()); an int: the OpenMP mode (erode_parallel(num_threads), 0 = fill the GPU). sweep and halo (both):
+        the sweeps mode (erode_sweeps(sweep, halo), tw_erode_launch_ex). h stays referenced until then."""
         ys, xs = h.shape
-        return self._erode_launch(ErosionJob(heightmap=h), h, xs, ys, min_zval, 0.0, 0.0, num_iters, ep, num_threads, None)
+        return self._erode_launch(ErosionJob(heightmap=h), h, xs, ys, min_zval, 0.0, 0.0, num_iters, ep, num_threads, None, sweep, halo)
 
-    def erode_image_launch(self, val_mult, val_add, num_iters, ep, num_threads=None, vals=None):
+    def erode_image_launch(self, val_mult, val_add, num_iters, ep, num_threads=None, vals=None, sweep=None, halo=None):
         """tw_erode_launch on this context's set_heightmap image: unpack with val_mult / val_add, erode down to the image's minimum, pack back, as one
-        asynchronous job. vals (optional, w*h floats, numpy array or CUDA tensor) receives the eroded floats before the pack. num_threads as erode_launch."""
-        return self._erode_launch(ErosionJob(vals=vals), None, 0, 0, 0.0, val_mult, val_add, num_iters, ep, num_threads, vals)
+        asynchronous job. vals (optional, w*h floats, numpy array or CUDA tensor) receives the eroded floats before the pack. num_threads, sweep and halo
+        as erode_launch."""
+        return self._erode_launch(ErosionJob(vals=vals), None, 0, 0, 0.0, val_mult, val_add, num_iters, ep, num_threads, vals, sweep, halo)
 
     def erode_sweeps(self, h, min_zval, num_iters, ep, sweep, halo):
         """The coherent batched erosion on one device (see tw_erode_sweeps); in place, returns the droplet moves."""

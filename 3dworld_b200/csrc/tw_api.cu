@@ -314,6 +314,7 @@ void tw_destroy(tw_ctx *ctx) {
 	if (ctx->d_job_words) cudaFree(ctx->d_job_words);
 	if (ctx->h_job) cudaFreeHost(ctx->h_job);
 	if (ctx->spec_graph) cudaGraphExecDestroy(ctx->spec_graph);
+	if (ctx->sweep_graph) cudaGraphExecDestroy(ctx->sweep_graph);
 	for (int i = 0; i < 3; ++i) {if (ctx->d_scratch[i]) cudaFree(ctx->d_scratch[i]);}
 	if (ctx->d_sin_table) cudaFree(ctx->d_sin_table);
 	if (ctx->d_dir_table) cudaFree(ctx->d_dir_table);
@@ -1181,14 +1182,20 @@ int tw_erode_parallel(tw_ctx *ctx, float *heightmap, int xsize, int ysize, float
 
 // tw_erode / tw_erode_parallel of one map, or of the context's image between its unpack and its pack, as the context's asynchronous job: the work tw_erode
 // (twi_erode's single-map paths) and tw_erode_parallel enqueue, with the step count, the no-progress flag and the pack's error flag staged in a
-// twi_hmap_stage that the completing poll unpacks; the image's lower clamp is its minimum, computed into the stage's min_z on the device
-int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job) {
+// twi_hmap_stage that the completing poll unpacks; the image's lower clamp is its minimum, computed into the stage's min_z on the device. The sweeps mode
+// (tw_erode_launch_ex) enqueues tw_erode_sweeps' one-band work the same way (twi_erode_sweeps_enqueue).
+int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job) {return tw_erode_launch_ex(ctx, job, nullptr);}
+
+int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_params *sw) {
 	int rc = check_ctx(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
 	if (!job || !job->ep) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
 	bool const image = (job->heightmap == nullptr);
-	if (job->mode != TW_EROSION_SERIAL && job->mode != TW_EROSION_OPENMP) return tw_set_error(ctx, TW_ERR_ARG, "bad erosion mode %d", job->mode);
-	if (job->mode == TW_EROSION_SERIAL && job->num_threads) return tw_set_error(ctx, TW_ERR_ARG, "num_threads is for TW_EROSION_OPENMP only");
+	if (job->mode != TW_EROSION_SERIAL && job->mode != TW_EROSION_OPENMP && job->mode != TW_EROSION_SWEEPS) return tw_set_error(ctx, TW_ERR_ARG, "bad erosion mode %d", job->mode);
+	if (job->mode != TW_EROSION_OPENMP && job->num_threads) return tw_set_error(ctx, TW_ERR_ARG, "num_threads is for TW_EROSION_OPENMP only");
+	bool const sweeps = (job->mode == TW_EROSION_SWEEPS);
+	if (sweeps != (sw != nullptr)) return tw_set_error(ctx, TW_ERR_ARG, sweeps ? "TW_EROSION_SWEEPS needs its tw_sweep_params" : "tw_sweep_params are for TW_EROSION_SWEEPS only");
+	if (sweeps && (sw->sweep == 0 || sw->halo < twi_sweep_view() + 12)) return tw_set_error(ctx, TW_ERR_ARG, "sweep must be > 0 and halo >= %d (view + 12)", twi_sweep_view() + 12);
 	if (image) {
 		if (job->xsize || job->ysize) return tw_set_error(ctx, TW_ERR_ARG, "the image's size is the tw_set_heightmap image's: xsize and ysize must be 0");
 		if (ctx->parent) return tw_set_error(ctx, TW_ERR_ARG, "tables are set on the parent context, not on a shared one");
@@ -1202,13 +1209,13 @@ int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job) {
 	size_t const n = (size_t)xsize*ysize;
 	bool const erode = (job->num_iters > 0 && job->ep->erode_amount > 0.0); // src/erosion.cpp:16
 	if (erode && !ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
-	bool const openmp = (job->mode == TW_EROSION_OPENMP), spec = erode && !openmp && twi_erode_spec_eligible(1, xsize, ysize, job->num_iters);
+	bool const openmp = (job->mode == TW_EROSION_OPENMP), spec = erode && !openmp && !sweeps && twi_erode_spec_eligible(1, xsize, ysize, job->num_iters);
 	float *const user = image ? job->vals : job->heightmap; // the caller's floats: the map, or the image's optional eroded floats
 	bool const user_dev = (user && tw_is_device_ptr(user));
 	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
 	// slot 0: the floats (unless the caller's are on the device); slot 1: the erosion's scratch; slot 2: [ordered min/max, droplet counter | stage]
 	if (erode && !user_dev) {rc = tw_reserve(ctx, 0, al(n*sizeof(float))); if (rc) return rc;}
-	size_t const ebytes = !erode ? 0 : openmp ? twi_erode_parallel_scratch_bytes(xsize, ysize)
+	size_t const ebytes = !erode ? 0 : openmp ? twi_erode_parallel_scratch_bytes(xsize, ysize) : sweeps ? twi_erode_sweeps_scratch_bytes(xsize, ysize)
 	                                 : spec ? twi_erode_spec_scratch_bytes(xsize, ysize) : twi_erode_scratch_bytes(ctx, 1, xsize, ysize);
 	if (ebytes) {rc = tw_reserve(ctx, 1, ebytes); if (rc) return rc;}
 	rc = tw_reserve(ctx, 2, OFF_TILES + 64 + al(sizeof(twi_hmap_stage))); if (rc) return rc;
@@ -1237,6 +1244,7 @@ int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job) {
 			else if (!user_dev) {TW_CUDA(ctx, cudaMemcpyAsync(d_vals, user, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
 			int r;
 			if (openmp) {r = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, job->num_threads, &d_st->steps, d_mm + 2);}
+			else if (sweeps) {r = twi_erode_sweeps_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, sw->sweep, sw->halo, &d_st->steps);}
 			else if (spec) {r = twi_erode_spec_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps, &d_st->fail, false);}
 			else {r = twi_erode_enqueue(ctx, ctx->stream, 0, ctx->d_scratch[1], 1, d_vals, 1, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps);}
 			if (r) return r;

@@ -85,6 +85,9 @@ __global__ void unpad_kernel(const float *__restrict__ padded, float *__restrict
 	out[dst_tile*xsize*ysize + (size_t)y*xsize + x] = smax(mz, padded[tile*NX*NY + (size_t)(y + PAD)*NX + x + PAD]);
 }
 
+// M_FROZEN in a job: the end of the sweep that starts at droplet it0 (the last sweep of n droplets may be short)
+__device__ __forceinline__ unsigned fz_end(unsigned it0, unsigned sweep, unsigned n) {return (n - it0 < sweep) ? n : it0 + sweep;}
+
 // rand_gen_t core (src/rand_gen.h:22-26) in 32-bit: all intermediates fit (Schrage factorisation), states stay in [0, 2^31)
 struct Rng {
 	int s1, s2;
@@ -190,16 +193,21 @@ struct DArgs {
 	unsigned it0, it1;          // droplets [it0, it1) = this sweep
 	SpecArgs S;                 // M_SPEC; M_GLOBAL with S.ctl != nullptr: walk the window's head in place if it is SP_HUGE
 	twi_job_words *jw;          // in a job: the context's job words (tw_cancel), M_GLOBAL / M_ATOMIC / M_WINDOW / M_WHOLE start no droplet once it is cancelled; nullptr otherwise
+	const unsigned *sweep_it0;  // M_FROZEN in a job (twi_erode_sweeps_enqueue): the device word holding it0; the sweep is [it0, fz_end(it0, sweep, num_iters))
+	unsigned sweep;
 };
 
 // CANCEL: the variant with the cancellation point, for jobs (see launch_droplets); synchronous calls and short latency-mode walks run the one without it, whose
-// code is the same as before tw_cancel existed (the check's branch makes ptxas lay the loop out differently, which costs a serial chain about 4 %)
+// code is the same as before tw_cancel existed (the check's branch makes ptxas lay the loop out differently, which costs a serial chain about 4 %).
+// M_FROZEN's job variant (CANCEL = true) has no check in the walk: it reads its sweep's bounds from A.sweep_it0, so one graph body serves every sweep, and
+// the loop's cancellation point is sweep_advance_kernel. The flags are spelled out in the expressions below rather than named: even an unused constexpr local
+// changes how the front end orders the code, and the SASS of the other instantiations is meant to stay as it was.
 template<int G, int MODE, bool CANCEL>
 __global__ void __launch_bounds__(128)
 droplet_kernel(DArgs const A)
 {
 	constexpr bool SHARED = (MODE == M_ATOMIC), FROZEN = (MODE == M_FROZEN), SPEC = (MODE == M_SPEC), WIN = (MODE == M_WINDOW || MODE == M_FROZEN || MODE == M_SPEC), WHOLE = (MODE == M_WHOLE);
-	static_assert(!CANCEL || (!FROZEN && !SPEC), "M_SPEC stops at its round boundary (spec_round_kernel); M_FROZEN is never in a job");
+	static_assert(!CANCEL || !SPEC, "M_SPEC stops at its round boundary (spec_round_kernel)");
 	static_assert(!SPEC || G == 32, "M_SPEC: one droplet per warp");
 	// M_FROZEN shares M_WINDOW's machinery: the window is the droplet's PRIVATE view (sweep-start heights + its own writes); see hadd
 	constexpr int TPW = 32/G; // heightmaps per warp
@@ -227,7 +235,7 @@ droplet_kernel(DArgs const A)
 	unsigned long long steps = 0;
 	bool const have_tile = active;
 	bool in_droplet = false;
-	unsigned iter = (MODE == M_FROZEN) ? A.it0 + gslot : 0u, numMoves = 0; // M_FROZEN: group g walks droplets it0 + g, it0 + g + groups, ... of the sweep
+	unsigned iter = (MODE == M_FROZEN) ? ((CANCEL && FROZEN) ? *A.sweep_it0 : A.it0) + gslot : 0u, numMoves = 0; // M_FROZEN: group g walks droplets it0 + g, it0 + g + groups, ... of the sweep
 	// M_SPEC: this warp's slot of the window; the log it writes
 	unsigned sp_nlog = 0, sp_nseg = 0, sp_ntiles = 0;
 	int sp_ax = -1, sp_az = -1, sp_bx = -1, sp_bz = -1; // tile rectangle of the previous move (most moves stay inside it)
@@ -430,10 +438,10 @@ droplet_kernel(DArgs const A)
 				}
 				active = false;
 			}
-			else if (iter >= (FROZEN ? A.it1 : num_iters)) {active = false;}
+			else if (iter >= (FROZEN ? ((CANCEL && FROZEN) ? fz_end(*A.sweep_it0, A.sweep, num_iters) : A.it1) : num_iters)) {active = false;}
 			// cancelled (tw_cancel): the group stops as if num_iters had been reached. Its leader reads the job words before every 8th droplet only (the
 			// droplet index, group-uniform), which keeps the read's latency off nearly every droplet of the serial chain
-			else if (CANCEL && (iter & 7u) == 0u && __shfl_sync(gmask, (sub == 0 && twi_cancelled(A.jw)) ? 1u : 0u, grp*G)) {
+			else if (CANCEL && !FROZEN && (iter & 7u) == 0u && __shfl_sync(gmask, (sub == 0 && twi_cancelled(A.jw)) ? 1u : 0u, grp*G)) {
 				if (sub == 0) {twi_mark_stopped(A.jw);}
 				active = false;
 			}
@@ -656,6 +664,9 @@ template<int G, int MODE>
 void launch_droplets(cudaStream_t st, DArgs const &A, unsigned warps_per_block, size_t smem_per_group) {
 	if constexpr (MODE != M_SPEC && MODE != M_FROZEN) {
 		if (A.jw && (MODE == M_GLOBAL || A.num_iters >= CANCEL_MIN_DROPLETS)) {launch_droplets_c<G, MODE, true>(st, A, warps_per_block, smem_per_group); return;}
+	}
+	if constexpr (MODE == M_FROZEN) {
+		if (A.sweep_it0) {launch_droplets_c<G, MODE, true>(st, A, warps_per_block, smem_per_group); return;}
 	}
 	launch_droplets_c<G, MODE, false>(st, A, warps_per_block, smem_per_group);
 }
@@ -1275,6 +1286,97 @@ int twi_sweep_apply(tw_ctx *ctx, float *P, long long *D, size_t n) {
 }
 int twi_sweep_unpad(tw_ctx *ctx, const float *P, int E0, int xsize, int y0, int y1, float min_zval, float *out) {
 	sweep_unpad_kernel<<<dim3((xsize + 255)/256, y1 - y0), 256, 0, ctx->stream>>>(P, E0, xsize + 2*PAD, xsize, y0, y1, min_zval, out);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ tw_erode_sweeps of one map as a job
+namespace {
+// The end of a sweep in the job's loop: the next sweep's first droplet into *it0, or - after the last sweep, or once the job is cancelled (tw_cancel; the
+// job is then marked stopped) - the end of the loop. The walk and the apply of the sweep it follows have finished: this is the loop's cancellation point.
+__global__ void sweep_advance_kernel(unsigned *it0, unsigned sweep, unsigned num_iters, twi_job_words *jw, cudaGraphConditionalHandle loop) {
+	unsigned const a = *it0;
+	bool const last = (num_iters - a <= sweep);
+	if (!last) {*it0 = a + sweep;}
+	bool const cancel = !last && twi_cancelled(jw);
+	if (cancel) {twi_mark_stopped(jw);}
+	if (last || cancel) {cudaGraphSetConditional(loop, 0u);}
+}
+size_t al256(size_t b) {return (b + 255) & ~(size_t)255;}
+} // namespace
+
+size_t twi_erode_sweeps_scratch_bytes(int xsize, int ysize) {
+	size_t const n = (size_t)(xsize + 2*PAD)*(ysize + 2*PAD);
+	return al256(n*sizeof(float)) + al256(n*sizeof(long long)) + 256;
+}
+
+// The sweeps as one CUDA graph: a conditional WHILE node whose body is the walk of a sweep, the apply and sweep_advance_kernel, which clears the condition.
+// Its kernel arguments are fixed, so it is kept in the context and rebuilt only when they change (another map size, scratch address, droplet count, sweep,
+// halo or erosion parameters), as spec_loop_graph does.
+static int sweep_loop_graph(tw_ctx *ctx, cudaStream_t st, DArgs const &W, long long *D, size_t n, unsigned *ctl) {
+	struct Key {DArgs W; long long *D; size_t n; unsigned *ctl;} k;
+	memset(&k, 0, sizeof(k));
+	k.W = W; k.D = D; k.n = n; k.ctl = ctl;
+	if (ctx->sweep_graph && ctx->sweep_key.size() == sizeof(k) && !memcmp(ctx->sweep_key.data(), &k, sizeof(k))) return TW_OK;
+	if (ctx->sweep_graph) {cudaGraphExecDestroy(ctx->sweep_graph); ctx->sweep_graph = nullptr; ctx->sweep_key.clear();} // a launch still in flight keeps its copy until it ends
+	cudaGraph_t g = nullptr;
+	cudaGraphExec_t ex = nullptr;
+	cudaGraphConditionalHandle h = 0;
+	cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
+	cudaError_t e = cudaGraphCreate(&g, 0);
+	if (e == cudaSuccess) {e = cudaGraphConditionalHandleCreate(&h, g, 1u, cudaGraphCondAssignDefault);}
+	if (e == cudaSuccess) {
+		cudaGraphNode_t node;
+		np.conditional.handle = h; np.conditional.type = cudaGraphCondTypeWhile; np.conditional.size = 1;
+		e = cudaGraphAddNode(&node, g, nullptr, 0, &np);
+	}
+	if (e == cudaSuccess) {e = cudaStreamBeginCaptureToGraph(st, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed);}
+	if (e == cudaSuccess) {
+		launch_droplets<8, M_FROZEN>(st, W, 2, (size_t)W.win_elems*sizeof(float));
+		sweep_apply_kernel<<<(unsigned)((n + 255)/256), 256, 0, st>>>(W.padded, D, n);
+		sweep_advance_kernel<<<1, 1, 0, st>>>(ctl, W.sweep, W.num_iters, W.jw, h);
+		cudaError_t const le = cudaGetLastError();
+		cudaGraph_t body = nullptr;
+		e = cudaStreamEndCapture(st, &body);
+		if (e == cudaSuccess) {e = le;}
+	}
+	if (e == cudaSuccess) {e = cudaGraphInstantiate(&ex, g, 0);}
+	if (g) {cudaGraphDestroy(g);}
+	if (e != cudaSuccess) {cudaGetLastError(); return tw_set_error(ctx, TW_ERR_CUDA, "erosion sweeps graph: %s", cudaGetErrorString(e));}
+	ctx->sweep_graph = ex;
+	ctx->sweep_key.assign((const unsigned char *)&k, (const unsigned char *)&k + sizeof(k));
+	return TW_OK;
+}
+
+// tw_erode_sweeps' one-band path on ctx->stream inside a job, nothing waits and nothing is allocated: pad d_map into `scratch`
+// (twi_erode_sweeps_scratch_bytes), zero the deltas and the sweep word, the sweeps as one graph launch that ends on the device, unpad with the lower clamp
+// *d_min_zval (nullptr: min_zval). d_steps accumulates the droplet moves (the caller zeroes it). The caller has checked sweep and halo as tw_erode_sweeps does.
+int twi_erode_sweeps_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zval, float min_zval, uint32_t num_iters,
+                             const tw_erosion_params *p, uint32_t sweep, int halo, unsigned long long *d_steps) {
+	cudaStream_t const st = ctx->stream;
+	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
+	size_t const n = (size_t)NX*NY;
+	float *P = (float *)scratch;
+	long long *D = (long long *)((char *)scratch + al256(n*sizeof(float)));
+	unsigned *ctl = (unsigned *)((char *)D + al256(n*sizeof(long long)));
+	TW_CUDA(ctx, cudaMemsetAsync(D, 0, n*sizeof(long long), st));
+	TW_CUDA(ctx, cudaMemsetAsync(ctl, 0, sizeof(unsigned), st));
+	pad_kernel<<<dim3((NX + 255)/256, NY, 1), 256, 0, st>>>(d_map, P, xsize, ysize, NX, NY, 0.0f, nullptr, nullptr); // = sweep_pad_kernel of the one band
+	TW_LAUNCH_CHECK(ctx);
+	DArgs A; // twi_sweep_walk's arguments for the one band (rows [0, NY) stored and owned), with the sweep's bounds on the device
+	memset(&A, 0, sizeof(A));
+	A.E = make_eparams(p);
+	A.padded = P; A.delta = D; A.row0 = 0; A.own0 = 0; A.own1 = NY; A.halo_rule = halo - TW_SWEEP_VIEW - PAD;
+	A.xsize = xsize; A.ysize = ysize; A.num_iters = num_iters; A.dir_table = ctx->d_dir_table; A.steps_out = d_steps;
+	A.jw = ctx->d_job_words; A.sweep_it0 = ctl; A.sweep = sweep;
+	A.slot0 = 0; A.nslots = std::min(sweep, ctx->num_sms*12u*4u); // twi_sweep_walk's groups of a full sweep; the result does not depend on them
+	A.WX = std::min(TW_SWEEP_VIEW, NX); A.WY = std::min(TW_SWEEP_VIEW, NY);
+	A.P = whole_pitch(A.WX, A.WY); A.win_elems = (unsigned)A.P*A.WY;
+	int const rc = sweep_loop_graph(ctx, st, A, D, n, ctl);
+	if (rc) return rc;
+	TW_CUDA(ctx, cudaGraphLaunch(ctx->sweep_graph, st));
+	ctx->launches++;
+	unpad_kernel<<<dim3((xsize + 255)/256, ysize, 1), 256, 0, st>>>(P, d_map, xsize, ysize, NX, NY, d_min_zval, min_zval, nullptr); // = sweep_unpad_kernel of the one band
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }

@@ -100,6 +100,8 @@ struct tw_ctx {
 	bool in_job = false;                    // set while twi_launch_job enqueues: the droplet walks it enqueues check the words, a synchronous call's do not
 	cudaGraphExec_t spec_graph = nullptr;   // the speculative erosion's round loop (tw_erosion.cu), kept while its kernel arguments stay the same
 	std::vector<unsigned char> spec_key;    // those arguments
+	cudaGraphExec_t sweep_graph = nullptr;  // the sweeps job's loop (twi_erode_sweeps_enqueue), kept the same way
+	std::vector<unsigned char> sweep_key;
 	void *dist = nullptr;        // tw_dist_state (tw_multi.cu): NCCL communicator of the one-process-per-GPU mode
 	unsigned skip_rect[4] = {0, 0, 0, 0}; // x0, y0, w, h of the cells twi_heightgen's paired noise kernels leave unwritten (set around AO context generation only)
 	// tw_create_shared: a shared context's tables above (sin / direction tables, sine params, both LUTs, the heightmap image) are its parent's, copied
@@ -281,6 +283,11 @@ int twi_sweep_walk(tw_ctx *ctx, float *P, long long *D, int xsize, int ysize, in
 int twi_sweep_add(tw_ctx *ctx, long long *D, const long long *R, size_t n);
 int twi_sweep_apply(tw_ctx *ctx, float *P, long long *D, size_t n);
 int twi_sweep_unpad(tw_ctx *ctx, const float *P, int E0, int xsize, int y0, int y1, float min_zval, float *out);
+// tw_erode_sweeps of one map in a job (tw_erode_launch_ex): its scratch (padded map, fixed-point deltas, the sweep word), and the enqueue - pad, the sweeps as
+// one graph that ends on the device (and at a cancel), unpad with the lower clamp *d_min_zval (nullptr: min_zval); moves added to *d_steps
+size_t twi_erode_sweeps_scratch_bytes(int xsize, int ysize);
+int    twi_erode_sweeps_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zval, float min_zval, uint32_t num_iters,
+                                const tw_erosion_params *p, uint32_t sweep, int halo, unsigned long long *d_steps);
 int twi_tile_bounds(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t ntiles, uint32_t zvsize, float wpz_max, void *d_sub, const unsigned *d_perm = nullptr);
 int twi_glaciate_mesh(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, unsigned *d_mm);
 // the checks of tw_voxel_fill after its null-argument check (TW_ERR_STATE without the sin table, TW_ERR_ARG for a bad gen_mode or size); *tab_bytes = the

@@ -151,8 +151,8 @@ TW_API uint64_t tw_launch_count(const tw_ctx *ctx);       /* kernels launched by
  *   state is committed at launch, in launch order, and frames launched later on other shared contexts already rely on it.
  * - The job stops at its next cancellation point: a droplet walk within its next 8 droplets (tile erosion, the OpenMP mode; on a batch small enough to be
  *   walked all at once, only walks of at least 4096 droplets per map - shorter ones take well under 0.1 s and run to their end), the serial order's
- *   speculative erosion at its next round (a round is at most 64 moves per walker), a voxel flood fill at its next generation, the mesh shadows at their
- *   next wave.
+ *   speculative erosion at its next round (a round is at most 64 moves per walker), the TW_EROSION_SWEEPS job after its current sweep, a voxel flood fill
+ *   at its next generation, the mesh shadows at their next wave.
  *   What is already enqueued of everything else still runs (generation, the tile tail, marching cubes, the end-of-job copies); a job without a
  *   cancellation point (a tw_heightgen_2d_launch grid, a heightmap job without erosion) completes as if tw_cancel had not been called.
  * - The completing poll (tw_create_tiles_poll / tw_heightgen_2d_poll) returns TW_ERR_CANCELED when a cancellation point acted. Every output of the job is
@@ -319,11 +319,24 @@ typedef struct tw_erosion_job {
 	float                     val_mult, val_add;/* with the image: the unpack's and the pack's scalars (get_mh_texture_mult / _add) */
 	uint32_t                  num_iters;
 	const tw_erosion_params  *ep;               /* required; copied during the launch */
-	int                       mode;             /* TW_EROSION_SERIAL or TW_EROSION_OPENMP */
+	int                       mode;             /* TW_EROSION_SERIAL or TW_EROSION_OPENMP (TW_EROSION_SWEEPS: tw_erode_launch_ex) */
 	uint32_t                  num_threads;      /* TW_EROSION_OPENMP: as tw_erode_parallel's (0 = fill the GPU); must be 0 otherwise */
 	float                    *vals;             /* with the image, optional: the eroded floats before the pack, device or host */
 } tw_erosion_job;
 TW_API int tw_erode_launch(tw_ctx *ctx, const tw_erosion_job *job);
+/* The same with a third mode, TW_EROSION_SWEEPS: tw_erode_sweeps (below) of the one map as the job - deterministic like the serial order and, on a big map
+ * with many droplets, far faster. tw_erode_launch(ctx, job) is tw_erode_launch_ex(ctx, job, NULL).
+ * - sw is required with TW_EROSION_SWEEPS (TW_ERR_ARG without it) and refused with the other two modes; num_threads must be 0.
+ * - heightmap != NULL: after the completing poll the map and tw_last_erosion_steps() equal tw_erode_sweeps(heightmap, xsize, ysize, min_zval, num_iters, ep,
+ *   sw->sweep, sw->halo, &moves) bit for bit, with the steps equal to moves (device, pinned or pageable host maps).
+ * - heightmap == NULL: as above for the image, with tw_erode_sweeps in the chain (min_zval = the image's minimum); every rule of the image mode holds.
+ * - Errors, nothing enqueued: those of tw_erode_launch, and those of tw_erode_sweeps - sw->sweep == 0 or sw->halo < 44 (view + 12) - checked even when
+ *   num_iters == 0 or erode_amount <= 0 (the job then does no work and reports 0 steps).
+ * - The sweeps run as one graph launch whose loop ends on the device, so a job of thousands of sweeps never fills the launch queue. The device memory is
+ *   the context's scratch: (xsize + 8)*(ysize + 8)*12 bytes besides the floats. tw_cancel stops the job after its current sweep. */
+#define TW_EROSION_SWEEPS 2   /* tw_erode_sweeps: the coherent batched sweeps (tw_sweep_params) */
+typedef struct tw_sweep_params { uint32_t sweep; int halo; } tw_sweep_params; /* tw_erode_sweeps' sweep and halo */
+TW_API int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_params *sw);
 /* Fused tile pipeline = the height fill AND the per-tile erosion of tile_t::create_zvals (src/tiled_mesh.cpp:467-515) for a batch of tiles:
  * exactly tw_heightgen_tiles followed by tw_erode_tiles(min_zval_all = min_zval) in one call (one upload of the origins, one download of
  * the result, per-tile z range fused). When memory forces several chunks, generation of chunk k+1 is issued on a separate stream and

@@ -139,6 +139,11 @@ class HmapSampler(C.Structure):
                 ("mesh_file_scale", C.c_float), ("mesh_file_tz", C.c_float), ("mesh_scale_z_inv", C.c_float)]
 
 
+class HmapRect(C.Structure):
+    """tw_hmap_rect (include/tw3d.h): texels [x, x + w) x [y, y + h) of the heightmap image."""
+    _fields_ = [("x", C.c_int), ("y", C.c_int), ("w", C.c_int), ("h", C.c_int)]
+
+
 class HeightmapInfo(C.Structure):
     _fields_ = [("min_z", C.c_float), ("max_z", C.c_float), ("val_mult", C.c_float), ("val_add", C.c_float), ("mesh_file_scale", C.c_float),
                 ("mesh_file_tz", C.c_float), ("erosion_moves", C.c_uint64)]
@@ -184,7 +189,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_dist_allreduce_minmax", "tw_dist_finalize", "tw_bind_thread_to_device", "tw_erode_sweeps", "tw_erode_sweeps_banded", "tw_erode_sweeps_sharded", "tw_voxel_outside", "tw_voxel_remove_unconnected", "tw_voxel_triangles", "tw_tile_shadows_batch", "tw_tile_shadows_batch_ex", "tw_create_tiles_launch_shadows", "tw_tile_weights_batch", "tw_gen_tex_height_tables",
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
                "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
-               "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex"]
+               "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
+               "tw_update_heightmap", "tw_hmap_tiles_touched"]
 
 
 def _load():
@@ -241,6 +247,8 @@ def _load():
                                            C.POINTER(ErosionParams), C.c_float, C.c_float, vp, vp, vp]
     L.tw_heightmap_sample_tiles.argtypes = [vp, vp, C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp]
     L.tw_set_heightmap.argtypes = [vp, vp, C.c_int, C.c_int]
+    L.tw_update_heightmap.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32]
+    L.tw_hmap_tiles_touched.argtypes = [C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_erode_parallel.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_uint32, C.POINTER(ErosionParams), C.c_uint32]
     L.tw_erode_launch.argtypes = [vp, C.POINTER(ErosionJobArgs)]
@@ -320,6 +328,26 @@ def _ptr(a):
         assert a.is_contiguous()
         return C.c_void_p(a.data_ptr())
     raise TypeError(type(a))
+
+
+def _rects(rects):
+    """[n, 4] (x, y, w, h) as a tw_hmap_rect array (None for n = 0) and n."""
+    r = np.ascontiguousarray(rects, np.int32).reshape(-1, 4)
+    arr = (HmapRect * max(1, len(r)))()
+    C.memmove(arr, r.ctypes.data, r.nbytes)
+    return (arr if len(r) else None), len(r)
+
+
+def hmap_tiles_touched(hs, origins, zvsize, rects):
+    """tw_hmap_tiles_touched (host only): uint8 [nt], 1 where some cell of the heightmap tile at origins[t] (x1, y1) reads, under hs (HmapSampler), a texel
+    inside one of rects ([n, 4] x, y, w, h) - the live tiles an image edit changes."""
+    org = np.ascontiguousarray(origins, np.int32).reshape(-1, 2)
+    arr, n = _rects(rects)
+    out = np.zeros(len(org), np.uint8)
+    rc = lib.tw_hmap_tiles_touched(C.byref(hs), _ptr(org) if len(org) else None, len(org), int(zvsize), arr, n, _ptr(out) if len(org) else None)
+    if rc != TW_OK:
+        raise TwError(rc, "tw_hmap_tiles_touched: bad argument")
+    return out
 
 
 def _edge(a):
@@ -696,6 +724,20 @@ class Context:
         if len(data16.shape) != 3 or data16.shape[2] != 2:
             raise ValueError("set_heightmap: data16 must have shape [h, w, 2]")
         self._check(lib.tw_set_heightmap(self._h, _ptr(data16), int(data16.shape[1]), int(data16.shape[0])))
+
+    def update_heightmap(self, data16, rects):
+        """tw_update_heightmap: texels rects ([n, 4] x, y, w, h) of the set_heightmap image become those of data16 (uint8 [h, w, 2] host array, the whole
+        edited image). Returns without completing any job or waiting for the GPU: jobs launched earlier see the old image, later ones the edited one. The
+        texels are copied before the call returns, so data16 may change at once."""
+        if hasattr(data16, "data_ptr") and data16.is_cuda:
+            ptr, pitch = _ptr(data16), 2 * int(data16.shape[1])          # refused by the library: the source is host memory
+        else:
+            data16 = np.asarray(data16)
+            if data16.dtype != np.uint8 or len(data16.shape) != 3 or data16.shape[2] != 2 or data16.strides[1:] != (2, 1):
+                raise ValueError("update_heightmap: data16 must be uint8 [h, w, 2] with contiguous rows")
+            ptr, pitch = C.c_void_p(data16.ctypes.data), int(data16.strides[0])
+        arr, n = _rects(rects)
+        self._check(lib.tw_update_heightmap(self._h, ptr, pitch, arr, n))
 
     def tile_normals(self, tiles, dx_val, dy_val, out=None):
         """tile_t::upload_normal_texture for a batch: returns (rgba [nt, stride, stride, 4] uint8, min_normal_z [nt])."""

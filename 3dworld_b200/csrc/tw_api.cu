@@ -174,7 +174,8 @@ tw_ctx *new_ctx(int device) {
 	{int sms = 0; if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && sms > 0) ctx->num_sms = (unsigned)sms; else cudaGetLastError();}
 	if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {delete ctx; cudaGetLastError(); return nullptr;}
 	if (cudaEventCreateWithFlags(&ctx->async.done, cudaEventDisableTiming) != cudaSuccess) {cudaStreamDestroy(ctx->stream); delete ctx; cudaGetLastError(); return nullptr;}
-	bool const ok = (cudaStreamCreateWithFlags(&ctx->cancel_stream, cudaStreamNonBlocking) == cudaSuccess
+	bool const ok = (cudaEventCreateWithFlags(&ctx->async.image_free, cudaEventDisableTiming) == cudaSuccess &&
+	                 cudaStreamCreateWithFlags(&ctx->cancel_stream, cudaStreamNonBlocking) == cudaSuccess
 	                 && cudaMalloc(&ctx->d_job_words, sizeof(twi_job_words)) == cudaSuccess && cudaMemset(ctx->d_job_words, 0, sizeof(twi_job_words)) == cudaSuccess
 	                 && cudaMallocHost(&ctx->h_job, sizeof(twi_job_host)) == cudaSuccess);
 	if (!ok) {tw_destroy(ctx); cudaGetLastError(); return nullptr;}
@@ -251,6 +252,23 @@ int twi_job_end(tw_ctx *ctx) {
 	return TW_OK;
 }
 
+int twi_wait_image_edits(tw_ctx *ctx) {
+	tw_ctx const *root = ctx->parent ? ctx->parent : ctx;
+	if (root->img_ev) {TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, root->img_ev, 0));}
+	return TW_OK;
+}
+
+int twi_image_settle(tw_ctx *root) {
+	if (root->img_stream) {TW_CUDA(root, cudaStreamSynchronize(root->img_stream));}
+	for (twi_img_stage &g : root->img_stage) {
+		if (g.h) cudaFreeHost(g.h);
+		if (g.d) cudaFree(g.d);
+		if (g.ev) cudaEventDestroy(g.ev);
+	}
+	root->img_stage.clear();
+	return TW_OK;
+}
+
 void twi_borrow_tables(tw_ctx *ctx) {
 	tw_ctx const *p = ctx->parent;
 	if (!p) return;
@@ -310,6 +328,9 @@ void tw_destroy(tw_ctx *ctx) {
 		ctx->d_sin_table = nullptr; ctx->d_dir_table = nullptr; ctx->d_simplex_lut = nullptr; ctx->d_glm3_lut = nullptr; ctx->d_sine_params = nullptr; ctx->d_hmap = nullptr;
 	}
 	cudaStreamSynchronize(ctx->stream);
+	twi_image_settle(ctx); // the edits of the image: every job they could wait for has completed
+	if (ctx->img_ev) cudaEventDestroy(ctx->img_ev);
+	if (ctx->img_stream) cudaStreamDestroy(ctx->img_stream);
 	if (ctx->cancel_stream) {cudaStreamSynchronize(ctx->cancel_stream); cudaStreamDestroy(ctx->cancel_stream);}
 	if (ctx->d_job_words) cudaFree(ctx->d_job_words);
 	if (ctx->h_job) cudaFreeHost(ctx->h_job);
@@ -324,6 +345,7 @@ void tw_destroy(tw_ctx *ctx) {
 	if (ctx->d_hmap) cudaFree(ctx->d_hmap);
 	if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
 	if (ctx->async.done) cudaEventDestroy(ctx->async.done);
+	if (ctx->async.image_free) cudaEventDestroy(ctx->async.image_free);
 	for (int i = 0; i < 3; ++i) {if (ctx->aux_stream[i]) cudaStreamDestroy(ctx->aux_stream[i]);}
 	for (int i = 0; i < 4; ++i) {
 		if (ctx->heavy_stream[i]) cudaStreamDestroy(ctx->heavy_stream[i]);
@@ -796,6 +818,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	twi_job pending;
 	pending.kind = twi_job::TILES; pending.n = ntiles; pending.host_steps = erode ? &ctx->last_erosion_steps : nullptr;
 	pending.cancellable = (tail == nullptr); // a tail commits a tile set's state
+	pending.reads_image = (hs != nullptr);
 	pending.host_mm = o->mm; pending.host_bounds = o->bounds; pending.host_min_nz = o->min_normal_z; pending.host_flags = (want_f && !dev_f) ? sh->has_any_grass : nullptr;
 	pending.dx = dx; pending.dy = dy; pending.size = size;
 	pending.off_steps = off_steps; pending.off_mm = off_mm; pending.off_sub = off_sub; pending.off_min_nz = off_mnz; pending.off_flags = off_f;
@@ -866,7 +889,14 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 				status = twi_heightgen(ctx, &gc, p, 1, 0, d_gen_corg + t0, nt, d_cz, nullptr); if (status) break;
 				status = twi_tile_cut(ctx, ctx->stream, d_cz, nt, zvsize, maps, perm_k); if (status) break;
 			}
-			else if (hs) {status = twi_hmap_sample_tiles(ctx, ctx->d_hmap, hs, d_perm ? (const void *)d_org : (const void *)(d_org + t0), nt, zvsize, maps, ctx->stream, perm_k); if (status) break;}
+			else if (hs) {
+				status = twi_hmap_sample_tiles(ctx, ctx->d_hmap, hs, d_perm ? (const void *)d_org : (const void *)(d_org + t0), nt, zvsize, maps, ctx->stream, perm_k);
+				if (status) break;
+				// every read of the image so far (the coarse pass, the chunks' sampling) is on ctx->stream, ahead of the chunk's erosion, part of which a small
+				// batch forks onto ctx->stream: after the last chunk this marks the image free (tw_update_heightmap)
+				if (cudaEventRecord(ctx->async.image_free, ctx->stream) != cudaSuccess) {status = tw_set_error(ctx, TW_ERR_CUDA, "image event"); break;}
+				ctx->async.image_free_set = true;
+			}
 			else if (!sine) {
 				ctx->tile_perm = perm_k;
 				status = twi_heightgen(ctx, &g, p, 1, 0, d_gen_org + t0, nt, maps, nullptr);           // generation on ctx->stream
@@ -950,6 +980,7 @@ int tw_set_heightmap(tw_ctx *ctx, const uint8_t *data16, int width, int height) 
 	rc = begin_table_change(ctx); if (rc) return rc;
 	rc = finish_pending(ctx); if (rc) return rc;
 	if (data16 && (width <= 0 || height <= 0)) return tw_set_error(ctx, TW_ERR_ARG, "heightmap size %d x %d", width, height);
+	rc = twi_image_settle(ctx); if (rc) return rc;
 	size_t const bytes = (size_t)2*width*height, had = (size_t)2*ctx->hmap_w*ctx->hmap_h;
 	if (ctx->d_hmap && (!data16 || bytes != had)) {TW_CUDA(ctx, cudaFree(ctx->d_hmap)); ctx->d_hmap = nullptr;}
 	ctx->hmap_w = ctx->hmap_h = 0;
@@ -958,6 +989,80 @@ int tw_set_heightmap(tw_ctx *ctx, const uint8_t *data16, int width, int height) 
 	TW_CUDA(ctx, cudaMemcpyAsync(ctx->d_hmap, data16, bytes, cudaMemcpyDefault, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // data16 is the caller's buffer
 	ctx->hmap_w = width; ctx->hmap_h = height;
+	return TW_OK;
+}
+
+// An edit of the image: the rects' texels packed into pinned staging (row by row, each at its destination's phase modulo 16 bytes), then on the image stream,
+// behind the pending image jobs of the family, one copy of [row table | texels] to the device and one scatter kernel. Completes no job, never waits.
+int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, const tw_hmap_rect *rects, uint32_t nrects) {
+	int rc = check_ctx(ctx); if (rc) return rc;
+	if (ctx->parent) return tw_set_error(ctx, TW_ERR_ARG, "the heightmap image is set on the parent context, not on a shared one");
+	if (nrects && (!src16 || !rects)) return tw_set_error(ctx, TW_ERR_ARG, "null src16 or rects");
+	if (nrects == 0) return TW_OK;
+	if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "the context has no heightmap image (tw_set_heightmap, or a job that sets it is pending)");
+	int const W = ctx->hmap_w, H = ctx->hmap_h;
+	size_t nrows = 0, texels = 0;
+	for (uint32_t r = 0; r < nrects; ++r) {
+		tw_hmap_rect const &R = rects[r];
+		if (R.w <= 0 || R.h <= 0 || R.x < 0 || R.y < 0 || R.x > W - R.w || R.y > H - R.h)
+			return tw_set_error(ctx, TW_ERR_ARG, "rect %u (%d, %d, %d x %d) is empty or reaches outside the %d x %d image", r, R.x, R.y, R.w, R.h, W, H);
+		if (src_pitch < (size_t)2*((size_t)R.x + (size_t)R.w)) return tw_set_error(ctx, TW_ERR_ARG, "src_pitch %zu < 2*(x + w) for rect %u", src_pitch, r);
+		nrows += (size_t)R.h; texels += (size_t)R.w*R.h + 7*(size_t)R.h;
+	}
+	if (tw_is_device_ptr(src16)) return tw_set_error(ctx, TW_ERR_ARG, "src16 must be host memory");
+	if (nrows > 0xffffffffu) return tw_set_error(ctx, TW_ERR_ARG, "too many rows in one edit");
+	size_t const rows_bytes = (nrows*sizeof(twi_hmap_row) + 255) & ~(size_t)255, need = rows_bytes + 2*texels;
+	if (!ctx->img_stream) {
+		TW_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->img_stream, cudaStreamNonBlocking));
+		TW_CUDA(ctx, cudaEventCreateWithFlags(&ctx->img_ev, cudaEventDisableTiming));
+	}
+	// staging: the smallest free buffer that fits (free = its edit has completed on the device); otherwise a new one. Nothing here waits for an edit.
+	twi_img_stage *g = nullptr;
+	for (twi_img_stage &e : ctx->img_stage) {
+		if (e.bytes < need || (g && g->bytes <= e.bytes)) continue;
+		cudaError_t const q = cudaEventQuery(e.ev);
+		if (q == cudaSuccess) g = &e;
+		else if (q != cudaErrorNotReady) return tw_set_error(ctx, TW_ERR_CUDA, "an earlier heightmap edit failed: %s", cudaGetErrorString(q));
+	}
+	if (!g) {
+		twi_img_stage e;
+		e.bytes = std::max<size_t>((size_t)1 << 16, need);
+		cudaError_t err = cudaMallocHost(&e.h, e.bytes);
+		if (err == cudaSuccess) err = cudaMalloc(&e.d, e.bytes);
+		if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e.ev, cudaEventDisableTiming);
+		if (err == cudaSuccess) {try {ctx->img_stage.push_back(e);} catch (...) {err = cudaErrorMemoryAllocation;}}
+		if (err != cudaSuccess) {
+			if (e.h) cudaFreeHost(e.h);
+			if (e.d) cudaFree(e.d);
+			if (e.ev) cudaEventDestroy(e.ev);
+			cudaGetLastError();
+			return tw_set_error(ctx, TW_ERR_CUDA, "heightmap edit staging of %zu bytes: %s", e.bytes, cudaGetErrorString(err));
+		}
+		g = &ctx->img_stage.back();
+	}
+	twi_hmap_row *rows = (twi_hmap_row *)g->h;
+	uint8_t *data = (uint8_t *)g->h + rows_bytes;
+	size_t k = 0, at = 0; // row, next free texel of the packed data
+	for (uint32_t r = 0; r < nrects; ++r) {
+		tw_hmap_rect const &R = rects[r];
+		for (int y = R.y; y < R.y + R.h; ++y, ++k) {
+			size_t const dst = (size_t)y*W + R.x, src = at + ((dst - at) & 7); // src = dst modulo 8 texels (16 bytes)
+			memcpy(data + 2*src, src16 + (size_t)y*src_pitch + 2*(size_t)R.x, 2*(size_t)R.w);
+			rows[k].dst = dst; rows[k].src = src; rows[k].w = (unsigned)R.w; rows[k].pad = 0;
+			at = src + R.w;
+		}
+	}
+	// behind the image work of the family's pending jobs that read or write the image: a heightmap tile job's sampling, the whole of an image erosion or a
+	// set_image job (a job that does not complete before its poll is still pending)
+	std::vector<tw_ctx *> family(1, ctx);
+	family.insert(family.end(), ctx->shared.begin(), ctx->shared.end());
+	for (tw_ctx *c : family) {
+		if (c->async.job.kind != twi_job::NONE && c->async.job.reads_image) {TW_CUDA(ctx, cudaStreamWaitEvent(ctx->img_stream, c->async.image_free, 0));}
+	}
+	TW_CUDA(ctx, cudaMemcpyAsync(g->d, g->h, rows_bytes + 2*at, cudaMemcpyHostToDevice, ctx->img_stream));
+	rc = twi_hmap_scatter(ctx, ctx->img_stream, (const twi_hmap_row *)g->d, (uint32_t)nrows, (const uint8_t *)g->d + rows_bytes, ctx->d_hmap); if (rc) return rc;
+	TW_CUDA(ctx, cudaEventRecord(g->ev, ctx->img_stream));
+	TW_CUDA(ctx, cudaEventRecord(ctx->img_ev, ctx->img_stream));
 	return TW_OK;
 }
 
@@ -1229,7 +1334,7 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 	unsigned *const d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_TILES);
 	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
 	twi_job pending;
-	pending.kind = twi_job::HMAP; pending.image_w = image ? xsize : 0; pending.image_h = image ? ysize : 0; pending.cancellable = true;
+	pending.kind = twi_job::HMAP; pending.image_w = image ? xsize : 0; pending.image_h = image ? ysize : 0; pending.cancellable = true; pending.reads_image = image;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(d_st, 0, sizeof(twi_hmap_stage), ctx->stream));
 		if (erode) {
@@ -1348,6 +1453,7 @@ int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, f
 	rc = tw_reserve_pinned(ctx, sizeof(twi_hmap_stage)); if (rc) return rc;
 	if (out->set_image) { // the old image goes now; the context has none until the completing poll
 		rc = begin_table_change(ctx); if (rc) return rc;
+		rc = twi_image_settle(ctx); if (rc) return rc;
 		size_t const bytes = 2*n, had = (size_t)2*ctx->hmap_w*ctx->hmap_h;
 		if (ctx->d_hmap && bytes != had) {TW_CUDA(ctx, cudaFree(ctx->d_hmap)); ctx->d_hmap = nullptr;}
 		ctx->hmap_w = ctx->hmap_h = 0;
@@ -1360,7 +1466,7 @@ int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, f
 	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
 	twi_job pending;
 	pending.kind = twi_job::HMAP; pending.host_info = out->info; pending.image_w = out->set_image ? (int)width : 0; pending.image_h = out->set_image ? (int)height : 0;
-	pending.cancellable = true;
+	pending.cancellable = true; pending.reads_image = (out->set_image != 0);
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(d_st, 0, sizeof(twi_hmap_stage), ctx->stream));
 		int r = twi_init_minmax(ctx, d_mm, 1); if (r) return r;

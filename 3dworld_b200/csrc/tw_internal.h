@@ -19,6 +19,7 @@ struct twi_job {
 	enum kind_t {NONE, TILES, VOXEL, HMAP};
 	kind_t kind = NONE;
 	bool cancellable = false;             // tw_cancel may stop it (set by the launch; a job that touches a tile set is not)
+	bool reads_image = false;             // it reads or writes the family's heightmap image: its work waits for the edits made before its launch (tw_update_heightmap)
 	unsigned seq = 0;                     // the context's number of the job (twi_launch_job), the one tw_cancel names
 	// TILES (tile jobs and frames; a 2-D grid is n = 1 with its min/max at offset 0; a relight stages nothing): n tiles' results at byte offsets into
 	// ctx->h_pinned, each unpacked only when its destination is set
@@ -39,9 +40,19 @@ struct twi_job {
 	int image_w = 0, image_h = 0;         // > 0: the packed image becomes (again) the context's tw_set_heightmap image when the job completes
 };
 
+// One edit's staging (tw_update_heightmap): pinned host memory and device memory of `bytes` each, holding [row table | packed texels], reused once `ev` (recorded
+// after the edit's scatter kernel) has completed
+struct twi_img_stage {void *h = nullptr; void *d = nullptr; size_t bytes = 0; cudaEvent_t ev = nullptr;};
+// one row of an edit: w texels from texel src of the staging's packed texels to texel dst of the image (src and dst have the same phase modulo 8 texels)
+struct twi_hmap_row {unsigned long long dst, src; unsigned w, pad;};
+
 struct tw_async_state {
 	twi_job job;
 	cudaEvent_t done = nullptr;           // recorded on ctx->stream after everything the pending job enqueued
+	// a job with reads_image: recorded on ctx->stream once the job no longer reads or writes the image, which tw_update_heightmap waits on. A heightmap tile
+	// job records it after its last sampling (image_free_set), so its erosion, shadows and tail overlap a later edit; any other image job records it with done.
+	cudaEvent_t image_free = nullptr;
+	bool image_free_set = false;
 };
 
 // The device words behind tw_cancel, one set per context at a fixed address. `job` is the number of the job that runs on ctx->stream (0 between jobs:
@@ -87,6 +98,11 @@ struct tw_ctx {
 	// tw_set_heightmap's 16-bit image (its own allocation: tw_reserve may re-allocate the scratch slots while a tile job still reads the image)
 	uint8_t *d_hmap = nullptr;
 	int hmap_w = 0, hmap_h = 0;
+	// tw_update_heightmap (root contexts): the image's stream (never ctx->stream, so an edit queued behind one context's long job holds up no other work on
+	// that context), the event recorded after the last edit, which image jobs wait on, and the edits' staging buffers
+	cudaStream_t img_stream = nullptr;
+	cudaEvent_t img_ev = nullptr;
+	std::vector<twi_img_stage> img_stage;
 	// pinned host staging for small results
 	void  *h_pinned = nullptr;
 	size_t pinned_bytes = 0;
@@ -128,17 +144,28 @@ bool tw_is_device_ptr(const void *p);
 // The job's number in the device words, on ctx->stream, before its work (twi_job_start sets *seq) / after it: `stopped` to the pinned staging, `job` cleared
 int twi_job_start(tw_ctx *ctx, unsigned *seq);
 int twi_job_end(tw_ctx *ctx);
+// ctx->stream waits (on the device) for every edit of the family's image so far
+int twi_wait_image_edits(tw_ctx *ctx);
+// Before the root's image is freed or replaced (tw_set_heightmap, a set_image job, tw_destroy): waits for the pending edits (the caller has completed every job
+// of the family they could wait for) and frees their staging
+int twi_image_settle(tw_ctx *root);
+// the scatter kernel of an edit on `st`: nrows rows (d_rows) of packed texels d_data into the image d_img
+int twi_hmap_scatter(tw_ctx *ctx, cudaStream_t st, const twi_hmap_row *d_rows, uint32_t nrows, const uint8_t *d_data, uint8_t *d_img);
 
 // Makes `job` the context's pending job (the previous one has been completed): enqueue() puts the job's work on ctx->stream, with every other stream it used
 // joined into ctx->stream, between the job's start and end in the device words, and ctx->async.done is recorded behind it. When any step fails, the call
 // waits for every stream of the context, so none of the job still runs on the scratch or the pinned staging when the error is returned, and no job is pending.
+// A job that reads or writes the image (job.reads_image) first waits on the device for the edits made before its launch.
 template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, const twi_job &job, Enqueue &&enqueue) {
 	unsigned seq = 0;
-	int rc = twi_job_start(ctx, &seq);
+	int rc = job.reads_image ? twi_wait_image_edits(ctx) : TW_OK;
+	if (rc == TW_OK) {rc = twi_job_start(ctx, &seq);}
+	ctx->async.image_free_set = false;
 	if (rc == TW_OK) {ctx->in_job = true; rc = enqueue(); ctx->in_job = false;}
 	if (rc == TW_OK) {rc = twi_job_end(ctx);}
 	if (rc == TW_OK) {
-		cudaError_t const e = cudaEventRecord(ctx->async.done, ctx->stream);
+		cudaError_t e = cudaEventRecord(ctx->async.done, ctx->stream);
+		if (e == cudaSuccess && job.reads_image && !ctx->async.image_free_set) e = cudaEventRecord(ctx->async.image_free, ctx->stream);
 		if (e != cudaSuccess) rc = tw_set_error(ctx, TW_ERR_CUDA, "recording the job's event: %s", cudaGetErrorString(e));
 	}
 	if (rc != TW_OK) {

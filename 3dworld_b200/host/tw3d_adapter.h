@@ -8,6 +8,7 @@
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
+//   tw3d::update_heightmap, tw3d::hmap_tiles_touched  <->  terrain_hmap_manager_t's brush edits and re-applied modmap, and the tiles they change   src/heightmap.cpp:36-58,243-308
 //   tw3d::set_deferred_gens, tw3d::tile_job_pool  <->  several of them in flight at once, as tile_draw_t::update keeps up to 8   src/tiled_mesh.cpp:2367-2417
 //   tw3d::tile_set               <->  the live tiles' calc_shadows_for_light when the light moves or new tiles appear   src/tiled_mesh.cpp:664-692
 //
@@ -410,6 +411,23 @@ inline void set_heightmap(const uint8_t *hmap16, int width, int height) {
 	int const rc = tw_set_heightmap(c, hmap16, width, height);
 	if (rc != TW_OK) {detail::fail(rc, "set_heightmap", c);}
 	detail::tls().hmap_w = hmap16 ? width : 0; detail::tls().hmap_h = hmap16 ? height : 0;
+}
+// terrain_hmap_manager_t's map edits (src/heightmap.cpp:36-58,243-308): after the engine's brush code has changed its CPU image hmap16 (width x height texels,
+// the layout set_heightmap took) inside rects (the brush's bounding rect, or the saved edits re-applied when a map loads), update_heightmap copies those texels
+// into this thread's context's image without completing or waiting for a frame in flight (tw_update_heightmap): frames launched before it see the old map,
+// frames after it the new one. hmap_tiles_touched names the live tiles (origins x1, y1 of zvsize^2 cells) whose heights the edit changes, for the image
+// set_heightmap gave and the scene's mesh_scale; re-create those in one tile-set frame with them put and the tiles tile_set::stale_after names relit.
+inline void update_heightmap(const uint8_t *hmap16, int width, int height, const tw_hmap_rect *rects, unsigned n) {
+	tw_ctx *c = ctx();
+	if (width != detail::tls().hmap_w || height != detail::tls().hmap_h) {detail::fail(TW_ERR_ARG, "update_heightmap: the image size differs from set_heightmap's", nullptr);}
+	int const rc = tw_update_heightmap(c, hmap16, 2*(size_t)width, rects, n);
+	if (rc != TW_OK) {detail::fail(rc, "update_heightmap", c);}
+}
+inline void hmap_tiles_touched(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const tw_hmap_rect *rects, unsigned n, uint8_t *touched,
+                               int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
+	int const rc = tw_hmap_tiles_touched(&hs, origins_xy, ntiles, zvsize, rects, n, touched);
+	if (rc != TW_OK) {detail::fail(rc, "hmap_tiles_touched: bad argument (no set_heightmap image?)", nullptr);}
 }
 inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max,
                                                    unsigned size, tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows,

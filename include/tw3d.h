@@ -121,9 +121,10 @@ typedef struct tw_voxel_params {
  * A context has at most one asynchronous job in flight: every other call on it (including the next launch) first completes the pending job, exactly
  * as a poll with wait = 1 would, and either poll function completes whichever job is pending. The rule is per context: to keep several jobs in flight
  * on one device, give each its own shared context (tw_create_shared); a call on one context never completes another context's job, except the three
- * table setters on a parent (below).
- * Threads: one thread at a time per context. A parent's tw_set_sin_table, tw_set_sine_params and tw_set_heightmap must not run while another thread is
- * inside a call on one of its shared contexts. */
+ * table setters on a parent (below). Deliberate exceptions to "complete the pending job first": tw_cancel and tw_update_heightmap complete no job and
+ * never wait for the device.
+ * Threads: one thread at a time per context. A parent's tw_set_sin_table, tw_set_sine_params, tw_set_heightmap and tw_update_heightmap must not run while
+ * another thread is inside a call on one of its shared contexts (tw_update_heightmap reads the shared contexts' pending-job state). */
 TW_API int  tw_abi_version(void);
 TW_API int  tw_create(int device, tw_ctx **out);
 /* A context on parent's device that uses parent's tables instead of its own: sin table, direction table, sine params, the simplex/Perlin
@@ -466,8 +467,38 @@ TW_API int tw_heightmap_sample_tiles(tw_ctx *ctx, const uint8_t *data16, const t
                               uint32_t zvsize, float *out);
 /* The context's heightmap image for tw_create_tiles_launch_hmap: copies data16 (2*width*height bytes in the layout of tw_heightmap_from_floats_u16, host or
  * device) into device memory the context owns, so a frame's tiles do not upload the image again. Completes a pending job first. data16 == NULL releases the
- * image; width or height <= 0 with an image is TW_ERR_ARG. Changing the map (brushes, a new file) means calling it again; tw_destroy frees the image. */
+ * image; width or height <= 0 with an image is TW_ERR_ARG. A new map means calling it again; an edit of the map (a brush stroke, the saved edits re-applied
+ * when a map loads) is tw_update_heightmap, which waits for nothing. It first orders after the pending edits, then frees their staging; tw_destroy frees the
+ * image. */
 TW_API int tw_set_heightmap(tw_ctx *ctx, const uint8_t *data16, int width, int height);
+/* A rectangle of the heightmap image: texels [x, x + w) x [y, y + h); image row y is bytes [2*width*y, 2*width*(y + 1)). */
+typedef struct tw_hmap_rect { int x, y, w, h; } tw_hmap_rect;
+/* Edits the context's tw_set_heightmap image in place: for each rect, texel (x, y) becomes the two bytes at src16 + y*src_pitch + 2*x (an engine passes its
+ * whole CPU image, src_pitch = 2*width, after its brush code changed it, with the brush's bounding rect). Rects may overlap; overlapping rects copy the same
+ * source bytes, so their order does not matter.
+ * What each job sees: every job sees the image as it was when its launch returned - every edit made before the launch, none made after it - on the root
+ * context and on every shared context. A job launched before the edit gives, bit for bit, the outputs it gives with the old image; a job launched after it
+ * gives the outputs of the same job after tw_set_heightmap(the edited image).
+ * It completes no job and never waits for the device (an exception to the rule under "context"). The image has its own stream on the root context: the
+ * edit's copy and scatter kernel wait there, on the device, for the image work of the family's pending jobs - the sampling of a heightmap tile job (its
+ * erosion, shadows and tile-set tail run on beside the edit), the whole of an image erosion or a set_image job - and jobs that read or write the image
+ * wait on the device for the edits made before their launch; jobs that do not touch the image wait for nothing. The image is not double-buffered: a job
+ * launched after an edit starts on the device only once the image jobs launched before the edit have sampled it (image erosion, set_image: finished).
+ * A job launched before an edit and cancelled after it leaves the edit in place. The staging is kept for later edits (an edit reuses a free buffer that is large
+ * enough) and freed by tw_set_heightmap, a set_image launch and tw_destroy: freeing pinned memory would synchronise the device, which this call never does.
+ * src16 is host memory (pageable or pinned): the call copies the rects' texels into pinned staging of its own before it returns, so the caller may change
+ * its image at once.
+ * Errors, nothing enqueued: TW_ERR_ARG for a NULL ctx, a shared context (the image is set on the parent), NULL src16 or rects with nrects > 0, a rect with
+ * w <= 0 or h <= 0 or reaching outside the image (no clipping), src_pitch < 2*(x + w) for some rect, and a device src16; TW_ERR_STATE without an image,
+ * which includes the time an erosion of the image or a set_image heightmap job is pending. nrects == 0 is TW_OK and does nothing. */
+TW_API int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, const tw_hmap_rect *rects, uint32_t nrects);
+/* Host only, no context: touched[t] = 1 exactly when some cell of tile t (origin origins_xy[2t], origins_xy[2t + 1], zvsize^2 cells), as the heightmap-texture
+ * tiles sample it under hs, reads a texel inside one of the rects - the live tiles an edit changes. A texel counts as read even where its bilinear weight is 0;
+ * cells that read nothing (off the texture in cliff mode) read no texel. Exact, and O(zvsize) per distinct tile column and row: the sampler's index
+ * arithmetic is separable per axis. TW_ERR_ARG for a NULL hs, a width or height <= 0, edge_mode outside 0..2, a NULL array with a nonzero count, or
+ * zvsize < 2. */
+TW_API int tw_hmap_tiles_touched(const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, uint32_t zvsize, const tw_hmap_rect *rects,
+                                 uint32_t nrects, uint8_t *touched);
 /* min/max over a float array (get_heightmap_z_range, src/map_view.cpp:399-407) */
 TW_API int tw_minmax_f32(tw_ctx *ctx, const float *vals, size_t n, tw_minmax *mm);
 

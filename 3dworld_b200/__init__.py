@@ -77,6 +77,11 @@ class VoxelBuild(C.Structure):
                 ("capacity", C.c_uint64), ("ntris", C.c_void_p), ("changed", C.c_void_p)]
 
 
+class VoxelMesh(C.Structure):
+    """tw_voxel_mesh (include/tw3d.h): the welded mesh's outputs - vertices, triangle indices, and the host counts."""
+    _fields_ = [("verts", C.c_void_p), ("vcapacity", C.c_uint64), ("indices", C.c_void_p), ("tcapacity", C.c_uint64), ("nverts", C.c_void_p), ("ntris", C.c_void_p)]
+
+
 class WeightParams(C.Structure):
     """tw_weight_params (include/tw3d.h): the terrain weights texture's tables and scene scalars."""
     _fields_ = [("h_dirt", C.c_float * 5), ("tex_class", C.c_int * 5), ("class_ix", C.c_int * 5), ("sthresh", (C.c_float * 2) * 2), ("zmin", C.c_float), ("zmax", C.c_float),
@@ -190,7 +195,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
                "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
-               "tw_update_heightmap", "tw_hmap_tiles_touched"]
+               "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex"]
 
 
 def _load():
@@ -289,6 +294,8 @@ def _load():
     L.tw_voxel_remove_unconnected.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), C.POINTER(C.c_uint64)]
     L.tw_voxel_triangles.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, vp, C.c_uint64, C.POINTER(C.c_uint64)]
     L.tw_voxel_build_launch.argtypes = [vp, C.POINTER(VoxelBuild)]
+    L.tw_voxel_mesh_welded.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, C.POINTER(VoxelMesh)]
+    L.tw_voxel_build_launch_ex.argtypes = [vp, C.POINTER(VoxelBuild), C.POINTER(VoxelMesh)]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
@@ -489,11 +496,21 @@ class VoxelBuildJob:
     """The host results of Context.voxel_build_launch, filled by the poll that completes the job."""
 
     def __init__(self):
-        self._ntris, self._changed = C.c_uint64(0), C.c_uint64(0)
+        self._ntris, self._changed, self._nverts, self._mesh_ntris = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
 
     @property
     def ntris(self):
         return int(self._ntris.value)
+
+    @property
+    def nverts(self):
+        """Vertices of the welded mesh (a job launched with mesh outputs)."""
+        return int(self._nverts.value)
+
+    @property
+    def mesh_ntris(self):
+        """Triangles of the welded mesh (a job launched with mesh outputs)."""
+        return int(self._mesh_ntris.value)
 
     @property
     def changed(self):
@@ -907,14 +924,31 @@ class Context:
         self._check(lib.tw_voxel_triangles(self._h, _ptr(vals), _ptr(outside), C.byref(vpp), _ptr(e), _ptr(t), _ptr(v), _ptr(out), cap, C.byref(n)))
         return out if isinstance(out, np.ndarray) else (out, n.value)
 
-    def voxel_build_launch(self, vpp, vals=None, outside=None, tris=None, fill=None, rdata=None, zix_xy=None, tables=None, capacity=None):
+    def voxel_mesh(self, vals, outside, vpp, tables, verts=None, indices=None):
+        """tw_voxel_mesh_welded: create_block's indexed mesh -> (verts [nv, 3] float32, indices [nt, 3] uint32). verts / indices (optional, numpy or torch,
+        host or CUDA) are filled up to their sizes and returned with the counts as (verts, indices, nverts, ntris)."""
+        e, t, v = (np.ascontiguousarray(tables[0], np.uint32), np.ascontiguousarray(tables[1], np.int32), np.ascontiguousarray(tables[2], np.uint32))
+        nv, nt = C.c_uint64(), C.c_uint64()
+        given = verts is not None or indices is not None
+        if not given:
+            m = VoxelMesh(None, 0, None, 0, C.cast(C.pointer(nv), C.c_void_p), C.cast(C.pointer(nt), C.c_void_p))
+            self._check(lib.tw_voxel_mesh_welded(self._h, _ptr(vals), _ptr(outside), C.byref(vpp), _ptr(e), _ptr(t), _ptr(v), C.byref(m)))
+            verts, indices = np.empty((nv.value, 3), np.float32), np.empty((nt.value, 3), np.uint32)
+        size = lambda a: 0 if a is None else (int(a.numel()) if hasattr(a, "numel") else int(a.size)) // 3
+        m = VoxelMesh(_ptr(verts), size(verts), _ptr(indices), size(indices), C.cast(C.pointer(nv), C.c_void_p), C.cast(C.pointer(nt), C.c_void_p))
+        self._check(lib.tw_voxel_mesh_welded(self._h, _ptr(vals), _ptr(outside), C.byref(vpp), _ptr(e), _ptr(t), _ptr(v), C.byref(m)))
+        return (verts, indices, nv.value, nt.value) if given else (verts, indices)
+
+    def voxel_build_launch(self, vpp, vals=None, outside=None, tris=None, fill=None, rdata=None, zix_xy=None, tables=None, capacity=None, mesh=None, soup=True):
         """tw_voxel_build_launch: fill (VoxelParams, optional) -> voxel_outside -> voxel_remove_unconnected -> voxel_triangles as one asynchronous job on
         this context; create_tiles_poll completes it. vals [ny, nx, nz] float32 is the input field without fill, else an optional output; outside
         [ny, nx, nz] uint8 optional output; tris: triangles out, a CUDA tensor or a page-locked numpy / torch buffer of capacity*9 floats (capacity defaults
         to its size // 9). numpy arrays, torch tensors or None. tables (edge_table, tri_table, edge_to_vals) or None = no triangles. Returns a VoxelBuildJob
-        whose ntris / changed are valid once the job is complete. The outputs and device inputs stay referenced here until then."""
+        whose ntris / changed are valid once the job is complete. The outputs and device inputs stay referenced here until then.
+        mesh = (verts, indices): also the welded mesh (tw_voxel_build_launch_ex), into a CUDA tensor or page-locked buffer each (None for none), filled up
+        to their sizes; the job's nverts / mesh_ntris are its counts. soup=False with a mesh: no triangle soup (tris must be None)."""
         job = VoxelBuildJob()
-        keep = [vals, outside, tris]
+        keep = [vals, outside, tris, mesh]
         tabs = (None, None, None)
         if tables is not None:
             tabs = tuple(t if hasattr(t, "data_ptr") else np.ascontiguousarray(t, dt) for t, dt in zip(tables, (np.uint32, np.int32, np.uint32)))
@@ -924,8 +958,15 @@ class Context:
             capacity = 0 if tris is None else (int(tris.numel()) if hasattr(tris, "numel") else int(tris.size)) // 9
         b = VoxelBuild(C.cast(C.pointer(fill), C.c_void_p) if fill is not None else None, _ptr(rd), C.cast(C.pointer(vpp), C.c_void_p), _ptr(z),
                        _ptr(tabs[0]), _ptr(tabs[1]), _ptr(tabs[2]), _ptr(vals), _ptr(outside), _ptr(tris), int(capacity),
-                       C.cast(C.pointer(job._ntris), C.c_void_p) if tables is not None else None, C.cast(C.pointer(job._changed), C.c_void_p))
-        self._check(lib.tw_voxel_build_launch(self._h, C.byref(b)))
+                       C.cast(C.pointer(job._ntris), C.c_void_p) if tables is not None and (soup or mesh is None) else None,
+                       C.cast(C.pointer(job._changed), C.c_void_p))
+        if mesh is None:
+            self._check(lib.tw_voxel_build_launch(self._h, C.byref(b)))
+        else:
+            size = lambda a: 0 if a is None else (int(a.numel()) if hasattr(a, "numel") else int(a.size)) // 3
+            m = VoxelMesh(_ptr(mesh[0]), size(mesh[0]), _ptr(mesh[1]), size(mesh[1]), C.cast(C.pointer(job._nverts), C.c_void_p),
+                          C.cast(C.pointer(job._mesh_ntris), C.c_void_p))
+            self._check(lib.tw_voxel_build_launch_ex(self._h, C.byref(b), C.byref(m)))
         self._tiles_job = (keep, tabs, z, job)
         return job
 

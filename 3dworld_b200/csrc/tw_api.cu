@@ -123,6 +123,7 @@ int poll_job(tw_ctx *ctx, int wait) {
 		memcpy(&st, h, sizeof(st));
 		if (j.host_ntris) {*j.host_ntris = st.ntris;}
 		if (j.host_changed) {*j.host_changed = st.changed;}
+		if (j.host_mesh_nverts) {*j.host_mesh_nverts = st.nverts; *j.host_mesh_ntris = st.mesh_ntris;}
 		break;
 	}
 	case twi_job::HMAP: { // tw_proc_gen_heightmap's order: the step count and info even when the pack fails, the image only when everything succeeded

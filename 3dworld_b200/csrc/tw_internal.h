@@ -10,7 +10,7 @@
 #include "../../include/tw3d.h"
 
 // A voxel build's counts in ctx->h_pinned (tw_voxel_build_launch)
-struct twi_voxel_stage {unsigned long long ntris, changed;};
+struct twi_voxel_stage {unsigned long long ntris, changed, nverts, mesh_ntris;}; // nverts, mesh_ntris: the welded mesh (tw_voxel_build_launch_ex)
 
 // The one asynchronous job a context may have in flight, as the poll that reports its completion unpacks it: which kind it is, what it staged in
 // ctx->h_pinned and where that goes. A job is pending when its kind is not NONE. Only twi_launch_job makes a job pending and only poll_job (tw_api.cu)
@@ -33,7 +33,7 @@ struct twi_job {
 	uint32_t size = 0;
 	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0, off_flags = 0;
 	// VOXEL: a twi_voxel_stage at ctx->h_pinned
-	uint64_t *host_ntris = nullptr, *host_changed = nullptr;
+	uint64_t *host_ntris = nullptr, *host_changed = nullptr, *host_mesh_nverts = nullptr, *host_mesh_ntris = nullptr;
 	// HMAP (tw_proc_gen_heightmap_launch; tw_erode_launch, which fills only the stage's min_z, bad, fail and steps and has no host_info): a twi_hmap_stage at
 	// ctx->h_pinned
 	tw_heightmap_info *host_info = nullptr;

@@ -288,13 +288,214 @@ scan_blocks_kernel(const unsigned *__restrict__ sums, unsigned nblocks, unsigned
 	if (threadIdx.x == 0) {*total = carry;}
 }
 
+// ---- the welded mesh (create_block's shared vertex cache, src/voxels.cpp:1077-1108 + :495-566) ----
+// A grid edge's vertex belongs to its OWNER, the first cube containing it in (y, x, z) order - i.e. the lowest linear index - that is not skipped; the
+// owner's interpolate_pt along its local edge, in its edge_to_vals corner order, is the position every cube on the edge uses. The eager cache of the
+// reference creates vertices in owner order and, per owner, in local edge order, so a vertex's index is the owned-vertex prefix of its owner plus its rank
+// among the owner's owned edges. mesh_kernel<false> counts per cube and stores word[c] = (block-exclusive owned-vertex prefix << 16) | owned-edge mask;
+// mesh_kernel<true> reads the words of the owners it references. Per block <= 12*1024 vertices and 5*1024 triangles: both prefixes fit 16 bits.
+
+// The cube's 12 edges as grid edges, from edge_to_vals: s_edge[i] = axis | ox << 2 | oy << 3 | oz << 4 (axis 0 x, 1 y, 2 z; o = the edge's low corner in
+// the cube); s_look[4*axis + 2*o1 + o2] = the local edge along axis whose low corner is at o1, o2 on the axis' other two (perp() order).
+// edge_to_vals must name each edge of the cube once (Bourke's table does).
+size_t al256(size_t b) {return (b + 255) & ~(size_t)255;}
+__device__ __forceinline__ void perp(unsigned a, unsigned &p1, unsigned &p2) {p1 = (a == 1) ? 0u : 1u; p2 = (a == 2) ? 0u : 2u;} // y > x > z in index weight
+__device__ void mesh_edge_tables(const unsigned *__restrict__ etv, unsigned char *s_edge, unsigned char *s_look) {
+	unsigned const t = threadIdx.x;
+	if (t < 12) {
+		unsigned c[2][3];
+		for (unsigned d = 0; d < 2; ++d) {
+			unsigned const e = __ldg(etv + 2*t + d), yhi = (e & 2) >> 1;
+			c[d][0] = yhi ^ (e & 1); c[d][1] = yhi; c[d][2] = (e >> 2) & 1;
+		}
+		unsigned const a = (c[0][0] != c[1][0]) ? 0u : ((c[0][1] != c[1][1]) ? 1u : 2u);
+		s_edge[t] = (unsigned char)(a | (min(c[0][0], c[1][0]) << 2) | (min(c[0][1], c[1][1]) << 3) | (min(c[0][2], c[1][2]) << 4));
+	}
+	__syncthreads();
+	if (t < 12) {
+		unsigned char look = 0;
+		for (unsigned i = 0; i < 12; ++i) {
+			unsigned const e = s_edge[i], a = e & 3;
+			unsigned p1, p2; perp(a, p1, p2);
+			if (4*a + 2*((e >> (2 + p1)) & 1) + ((e >> (2 + p2)) & 1) == t) {look = (unsigned char)i;}
+		}
+		s_look[t] = look;
+	}
+	__syncthreads();
+}
+
+// cube (c[0], c[1], c[2]) makes triangles: inside the grid, not in the last layer of an axis, and not skip_under_mesh with its 4 low corners under the mesh
+__device__ __forceinline__ bool cube_valid(const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const int *c) {
+	if (c[0] < 0 || c[1] < 0 || c[2] < 0 || (unsigned)c[0] + 1 >= P.nx || (unsigned)c[1] + 1 >= P.ny || (unsigned)c[2] + 1 >= P.nz) return false;
+	if (!P.skip_under_mesh) return true;
+	for (unsigned k = 0; k < 4; ++k) {
+		size_t const ix = (unsigned)c[2] + ((size_t)(c[0] + (k & 1)) + (size_t)(c[1] + (k >> 1))*P.nx)*P.nz;
+		if (!(__ldg(outside + ix) & TW_VOX_UNDER_MESH)) return true;
+	}
+	return false;
+}
+
+// One cube of the welded mesh: the welded position of each of its crossing edges (vlist), each edge's owner (linear index) and local edge there (own, oj),
+// the edges it owns (mask) and the triangles whose welded positions have a nonzero normal (kept, bit k = the k-th triangle of tri_table). Returns the
+// number of kept triangles.
+struct MeshCube {float vlist[12][3]; unsigned own[12]; unsigned char oj[12], tri[5][3]; unsigned mask, kept;};
+template<bool EMIT>
+__device__ unsigned cube_mesh(const float *__restrict__ vals, const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const McTables &T,
+	const unsigned char *s_edge, const unsigned char *s_look, unsigned x, unsigned y, unsigned z, unsigned ci, MeshCube &m)
+{
+	m.mask = 0; m.kept = 0;
+	unsigned const nx = P.nx, ny = P.ny, nz = P.nz;
+	if (x + 1 >= nx || y + 1 >= ny || z + 1 >= nz) return 0; // last layer of an axis
+	unsigned cix = 0;
+	bool all_under_mesh = (P.skip_under_mesh != 0);
+#pragma unroll
+	for (unsigned yhi = 0; yhi < 2; ++yhi) {
+#pragma unroll
+		for (unsigned xhi = 0; xhi < 2; ++xhi) {
+			size_t const ix = z + ((size_t)(x + xhi) + (size_t)(y + yhi)*nx)*nz;
+			if (all_under_mesh) {all_under_mesh = ((__ldg(outside + ix) & TW_VOX_UNDER_MESH) != 0);}
+#pragma unroll
+			for (unsigned zhi = 0; zhi < 2; ++zhi) {if (__ldg(outside + ix + zhi) & 7) {cix |= 1u << ((xhi ^ yhi) + 2*yhi + 4*zhi);}}
+		}
+	}
+	if (all_under_mesh) return 0;
+	unsigned const edge_val = __ldg(T.edge_table + cix);
+	if (edge_val == 0) return 0;
+	for (unsigned i = 0; i < 12; ++i) {
+		if (EMIT) {m.own[i] = ci; m.oj[i] = (unsigned char)i;}
+		if (!(edge_val & (1u << i))) continue;
+		unsigned const e = s_edge[i], a = e & 3;
+		unsigned p1, p2; perp(a, p1, p2);
+		int const g[3] = {(int)(x + ((e >> 2) & 1)), (int)(y + ((e >> 3) & 1)), (int)(z + ((e >> 4) & 1))};
+		int o[3] = {(int)x, (int)y, (int)z};
+		unsigned j = i;
+		for (unsigned k = 0; k < 4; ++k) { // the edge's cubes in increasing index: (d1, d2) = (1, 1), (1, 0), (0, 1), (0, 0) below its low corner
+			unsigned const d1 = (k < 2), d2 = !(k & 1);
+			int c[3] = {g[0], g[1], g[2]};
+			c[p1] -= (int)d1; c[p2] -= (int)d2;
+			if (c[0] == (int)x && c[1] == (int)y && c[2] == (int)z) {m.mask |= 1u << i; break;} // no earlier cube makes triangles: this one owns it
+			if (cube_valid(outside, P, c)) {o[0] = c[0]; o[1] = c[1]; o[2] = c[2]; j = s_look[4*a + 2*d1 + d2]; break;}
+		}
+		if (EMIT) {m.own[i] = (m.mask & (1u << i)) ? ci : (unsigned)o[2] + ((unsigned)o[0] + (unsigned)o[1]*nx)*nz; m.oj[i] = (unsigned char)j;}
+		float v2[2], pts[2][3];
+#pragma unroll
+		for (unsigned d = 0; d < 2; ++d) { // the owner's interpolation: its corners, in its order
+			unsigned const ev = __ldg(T.edge_to_vals + 2*j + d), yhi = (ev & 2) >> 1, xhi = yhi ^ (ev & 1), zhi = (ev >> 2) & 1;
+			unsigned const cx = (unsigned)o[0] + xhi, cy = (unsigned)o[1] + yhi, cz = (unsigned)o[2] + zhi;
+			size_t const ix = cz + ((size_t)cx + (size_t)cy*nx)*nz;
+			v2[d] = ((__ldg(outside + ix) & 7) == TW_VOX_ON_EDGE) ? P.isolevel : __ldg(vals + ix);
+			pts[d][0] = (float)cx*P.vsz[0] + P.lo_pos[0]; pts[d][1] = (float)cy*P.vsz[1] + P.lo_pos[1]; pts[d][2] = (float)cz*P.vsz[2] + P.lo_pos[2];
+		}
+		interpolate_pt(P.isolevel, pts[0], pts[1], v2[0], v2[1], m.vlist[i]);
+	}
+	const int *t = T.tri_table + 16*cix;
+	unsigned count = 0;
+	for (unsigned i = 0, k = 0; i < 15; i += 3, ++k) {
+		int const t0 = __ldg(t + i);
+		if (t0 < 0) break;
+		int const t1 = __ldg(t + i + 1), t2 = __ldg(t + i + 2);
+		const float *p0 = m.vlist[t0], *p1 = m.vlist[t1], *p2 = m.vlist[t2];
+		float const a0 = p1[0] - p0[0], a1 = p1[1] - p0[1], a2 = p1[2] - p0[2], b0 = p2[0] - p1[0], b1 = p2[1] - p1[1], b2 = p2[2] - p1[2]; // get_normal
+		float const cx = a1*b2 - a2*b1, cy = a2*b0 - a0*b2, cz = a0*b1 - a1*b0;
+		if (cx == 0.0f && cy == 0.0f && cz == 0.0f) continue; // degenerate in the welded positions: the reference tests the cached points
+		if (EMIT) {m.tri[count][0] = (unsigned char)t0; m.tri[count][1] = (unsigned char)t1; m.tri[count][2] = (unsigned char)t2;}
+		++count;
+	}
+	return count;
+}
+
+template<bool EMIT>
+__global__ void __launch_bounds__(MC_BLOCK)
+mesh_kernel(const float *__restrict__ vals, const unsigned char *__restrict__ outside, tw_voxel_post_params P, McTables T, size_t n, unsigned *__restrict__ words,
+	unsigned *__restrict__ vsums, unsigned *__restrict__ tsums, const unsigned long long *__restrict__ voff, const unsigned long long *__restrict__ toff,
+	float *__restrict__ verts, unsigned long long vcap, uint32_t *__restrict__ indices, unsigned long long tcap)
+{
+	__shared__ unsigned warp_sums[MC_BLOCK/32];
+	__shared__ unsigned char s_edge[12], s_look[12];
+	mesh_edge_tables(T.edge_to_vals, s_edge, s_look);
+	size_t const i = (size_t)blockIdx.x*MC_BLOCK + threadIdx.x;
+	MeshCube m;
+	m.mask = 0;
+	unsigned cnt = 0; // owned vertices << 16 | kept triangles
+	if (i < n) {
+		unsigned const z = (unsigned)(i % P.nz);
+		size_t const xy = i / P.nz;
+		unsigned const nt = cube_mesh<EMIT>(vals, outside, P, T, s_edge, s_look, (unsigned)(xy % P.nx), (unsigned)(xy / P.nx), z, (unsigned)i, m);
+		cnt = ((unsigned)__popc(m.mask) << 16) | nt;
+	}
+	unsigned const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	unsigned incl = cnt;
+	for (int o = 1; o < 32; o <<= 1) {unsigned const v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= (unsigned)o) incl += v;}
+	if (lane == 31) {warp_sums[warp] = incl;}
+	__syncthreads();
+	if (warp == 0) {
+		unsigned w = warp_sums[lane], wi = w;
+		for (int o = 1; o < 32; o <<= 1) {unsigned const v = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= (unsigned)o) wi += v;}
+		warp_sums[lane] = wi - w;
+		if (!EMIT && lane == 31) {vsums[blockIdx.x] = wi >> 16; tsums[blockIdx.x] = wi & 0xffffu;}
+	}
+	__syncthreads();
+	unsigned const excl = warp_sums[warp] + (incl - cnt);
+	if (!EMIT) {
+		if (i < n) {words[i] = (excl & 0xffff0000u) | m.mask;}
+		return;
+	}
+	if (i >= n) return;
+	unsigned long long const vbase = voff[blockIdx.x] + (excl >> 16);
+	for (unsigned mk = m.mask; mk; mk &= mk - 1) {
+		unsigned const e = __ffs(mk) - 1;
+		unsigned long long const slot = vbase + __popc(m.mask & ((1u << e) - 1));
+		if (slot < vcap) {float *o = verts + 3*slot; o[0] = m.vlist[e][0]; o[1] = m.vlist[e][1]; o[2] = m.vlist[e][2];}
+	}
+	unsigned long long const tbase = toff[blockIdx.x] + (excl & 0xffffu);
+	for (unsigned k = 0; k < (cnt & 0xffffu); ++k) {
+		unsigned long long const slot = tbase + k;
+		if (slot >= tcap) break;
+		for (unsigned v = 0; v < 3; ++v) {
+			unsigned const e = m.tri[k][v], owner = m.own[e], w = __ldg(words + owner);
+			indices[3*slot + v] = (uint32_t)(voff[owner / MC_BLOCK] + (w >> 16) + __popc(w & 0xfffu & ((1u << m.oj[e]) - 1)));
+		}
+	}
+}
+
+// both passes of the welded mesh after the flags are final: count -> two block scans -> emit (when a capacity is > 0). Scratch: words n, vsums / tsums
+// nblocks, voff / toff nblocks, totals[2] = vertices, triangles.
+struct MeshScratch {unsigned *words, *vsums, *tsums; unsigned long long *voff, *toff, *totals;};
+int enqueue_mesh(tw_ctx *ctx, const float *d_v, const unsigned char *d_o, const tw_voxel_post_params &P, const McTables &T, const MeshScratch &S, float *verts,
+                 unsigned long long vcap, uint32_t *indices, unsigned long long tcap)
+{
+	size_t const n = (size_t)P.nx*P.ny*P.nz;
+	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
+	mesh_kernel<false><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, P, T, n, S.words, S.vsums, S.tsums, nullptr, nullptr, nullptr, 0, nullptr, 0);
+	TW_LAUNCH_CHECK(ctx);
+	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(S.vsums, nblocks, S.voff, S.totals);
+	TW_LAUNCH_CHECK(ctx);
+	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(S.tsums, nblocks, S.toff, S.totals + 1);
+	TW_LAUNCH_CHECK(ctx);
+	if (vcap || tcap) {
+		mesh_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, P, T, n, S.words, nullptr, nullptr, S.voff, S.toff, verts, vcap, indices, tcap);
+		TW_LAUNCH_CHECK(ctx);
+	}
+	return TW_OK;
+}
+size_t mesh_scratch_bytes(size_t n, unsigned nblocks) {return al256(n*sizeof(unsigned)) + 2*al256((size_t)nblocks*sizeof(unsigned)) + 2*al256((size_t)nblocks*8) + 256;}
+MeshScratch mesh_scratch(char *sp, size_t n, unsigned nblocks) {
+	MeshScratch S;
+	S.words = (unsigned *)sp; sp += al256(n*sizeof(unsigned));
+	S.vsums = (unsigned *)sp; sp += al256((size_t)nblocks*sizeof(unsigned));
+	S.tsums = (unsigned *)sp; sp += al256((size_t)nblocks*sizeof(unsigned));
+	S.voff = (unsigned long long *)sp; sp += al256((size_t)nblocks*8);
+	S.toff = (unsigned long long *)sp; sp += al256((size_t)nblocks*8);
+	S.totals = (unsigned long long *)sp;
+	return S;
+}
+
 int validate(tw_ctx *ctx, const tw_voxel_post_params *vp) {
 	if (!vp || vp->nx == 0 || vp->ny == 0 || vp->nz == 0) return tw_set_error(ctx, TW_ERR_ARG, "empty voxel grid");
 	if ((unsigned long long)vp->nx*vp->ny*vp->nz >= 0xffffffffull) return tw_set_error(ctx, TW_ERR_ARG, "voxel grids are indexed with 32 bits, as in the reference (src/voxels.h:141)");
 	return TW_OK;
 }
 unsigned stream_grid(const tw_ctx *ctx, size_t n) {size_t const b = (n + 255)/256; return (unsigned)(b < ctx->num_sms*16u ? (b ? b : 1) : ctx->num_sms*16u);}
-size_t al256(size_t b) {return (b + 255) & ~(size_t)255;}
 
 // the flood's grid: 4 blocks per SM, fewer if fewer fit at once (a cooperative launch needs every block resident)
 int flood_blocks(tw_ctx *ctx, unsigned *blocks) {
@@ -447,6 +648,69 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 	return TW_OK;
 }
 
+namespace {
+int validate_mesh(tw_ctx *ctx, const tw_voxel_post_params *vp, const tw_voxel_mesh *m) {
+	if (!m->nverts || !m->ntris) return tw_set_error(ctx, TW_ERR_ARG, "the welded mesh needs nverts and ntris");
+	if ((m->vcapacity && !m->verts) || (m->tcapacity && !m->indices)) return tw_set_error(ctx, TW_ERR_ARG, "a mesh capacity without its buffer");
+	if (3ull*vp->nx*vp->ny*vp->nz >= 0x100000000ull) return tw_set_error(ctx, TW_ERR_ARG, "the welded mesh's indices are 32-bit: 3*nx*ny*nz must be below 2^32");
+	return TW_OK;
+}
+// device or page-locked host memory as the device addresses it (the emit passes of the job write their outputs directly); nullptr for anything else
+void *device_view(void *p) {
+	cudaPointerAttributes a;
+	if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {cudaGetLastError(); return nullptr;}
+	if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) return p;
+	if (a.type == cudaMemoryTypeHost && a.devicePointer) return a.devicePointer;
+	return nullptr;
+}
+} // namespace
+
+extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_t *outside, const tw_voxel_post_params *vp, const uint32_t *edge_table256,
+                                    const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, const tw_voxel_mesh *out)
+{
+	if (!ctx || !vals || !outside || !edge_table256 || !tri_table256x16 || !edge_to_vals12x2 || !out) return TW_ERR_ARG;
+	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int rc = validate(ctx, vp); if (rc) return rc;
+	tw_voxel_mesh const M = *out;
+	rc = validate_mesh(ctx, vp, &M); if (rc) return rc;
+	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
+	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
+	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside);
+	size_t const vb = dev_v ? 0 : al256(n*sizeof(float)), ob = dev_o ? 0 : al256(n), tb = al256(1024 + 16384 + 96);
+	rc = tw_reserve(ctx, 0, vb + ob + tb + mesh_scratch_bytes(n, nblocks)); if (rc) return rc;
+	char *sp = (char *)ctx->d_scratch[0];
+	const float *d_v = vals; const unsigned char *d_o = outside;
+	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(sp, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_v = (const float *)sp; sp += vb;}
+	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(sp, outside, n, cudaMemcpyHostToDevice, ctx->stream)); d_o = (const unsigned char *)sp; sp += ob;}
+	McTables T;
+	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384);
+	TW_CUDA(ctx, cudaMemcpyAsync(sp, edge_table256, 1024, cudaMemcpyDefault, ctx->stream));
+	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024, tri_table256x16, 16384, cudaMemcpyDefault, ctx->stream));
+	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024 + 16384, edge_to_vals12x2, 96, cudaMemcpyDefault, ctx->stream));
+	sp += tb;
+	MeshScratch const S = mesh_scratch(sp, n, nblocks);
+	// count and scan first: the emit pass writes at most min(count, capacity) of each, so host outputs are staged at that size
+	rc = enqueue_mesh(ctx, d_v, d_o, *vp, T, S, nullptr, 0, nullptr, 0); if (rc) return rc;
+	unsigned long long tot[2] = {0, 0};
+	TW_CUDA(ctx, cudaMemcpyAsync(tot, S.totals, sizeof(tot), cudaMemcpyDeviceToHost, ctx->stream));
+	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	*M.nverts = tot[0]; *M.ntris = tot[1];
+	uint64_t const nv = (tot[0] < M.vcapacity) ? tot[0] : M.vcapacity, nt = (tot[1] < M.tcapacity) ? tot[1] : M.tcapacity;
+	if (nv == 0 && nt == 0) return TW_OK;
+	bool const dev_vt = nv && tw_is_device_ptr(M.verts), dev_ix = nt && tw_is_device_ptr(M.indices);
+	size_t const svb = dev_vt ? 0 : al256((size_t)nv*12), sib = dev_ix ? 0 : al256((size_t)nt*12);
+	if (svb + sib) {rc = tw_reserve(ctx, 1, svb + sib); if (rc) return rc;}
+	float *d_vt = dev_vt ? M.verts : (float *)ctx->d_scratch[1];
+	uint32_t *d_ix = dev_ix ? M.indices : (uint32_t *)((char *)ctx->d_scratch[1] + svb);
+	mesh_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, *vp, T, n, S.words, nullptr, nullptr, S.voff, S.toff, d_vt, nv, d_ix, nt);
+	TW_LAUNCH_CHECK(ctx);
+	if (nv && !dev_vt) {TW_CUDA(ctx, cudaMemcpyAsync(M.verts, d_vt, (size_t)nv*12, cudaMemcpyDeviceToHost, ctx->stream));}
+	if (nt && !dev_ix) {TW_CUDA(ctx, cudaMemcpyAsync(M.indices, d_ix, (size_t)nt*12, cudaMemcpyDeviceToHost, ctx->stream));}
+	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return TW_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ the whole build as one asynchronous job
 // fill (optional) -> outside -> remove_unconnected -> marching cubes (count, block scan, emit with the caller's capacity) on ctx->stream; nothing is read back
 // before the end: the triangle count and the flipped voxels go to pinned staging that the completing poll unpacks. Every buffer is reserved before anything is
@@ -454,7 +718,10 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 //   device slot 0: [counters (256 B) | field (unless vals is device memory) | padded flags | 2 frontiers (remove_unconnected > 0) | tables | block sums | block
 //                  offsets | zix_xy (host input)]
 //   pinned:        [twi_voxel_stage (64 B) | sine coefficients | tables | zix_xy (host input)]
-extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
+//   with a welded mesh, device slot 0 ends with the mesh's scratch (mesh_scratch)
+extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {return tw_voxel_build_launch_ex(ctx, b, nullptr);}
+
+extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, const tw_voxel_mesh *mesh) {
 	if (!ctx) return TW_ERR_ARG;
 	TW_CUDA(ctx, cudaSetDevice(ctx->device));
 	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
@@ -472,16 +739,26 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 	else if (!b->vals) return tw_set_error(ctx, TW_ERR_ARG, "vals is the input field when there is no fill");
 	int const ntab = (b->edge_table256 != nullptr) + (b->tri_table256x16 != nullptr) + (b->edge_to_vals12x2 != nullptr);
 	if (ntab != 0 && ntab != 3) return tw_set_error(ctx, TW_ERR_ARG, "pass all three marching-cubes tables or none");
-	bool const mc = (ntab == 3);
+	bool const wm = (mesh != nullptr);
+	if (wm && ntab != 3) return tw_set_error(ctx, TW_ERR_ARG, "the welded mesh needs the three marching-cubes tables");
+	bool const mc = (ntab == 3) && (b->ntris || !wm); // the soup: without a mesh, the tables ask for it
 	if (mc && !b->ntris) return tw_set_error(ctx, TW_ERR_ARG, "the tables need ntris");
 	if (b->capacity && !b->tris) return tw_set_error(ctx, TW_ERR_ARG, "capacity > 0 without tris");
+	if (wm && !mc && b->tris) return tw_set_error(ctx, TW_ERR_ARG, "tris without ntris");
 	float *d_t = nullptr;
 	if (b->tris) { // the emit pass writes tris directly: device memory, or page-locked host memory through its mapping
-		cudaPointerAttributes a;
-		if (cudaPointerGetAttributes(&a, b->tris) != cudaSuccess) {cudaGetLastError(); a.type = cudaMemoryTypeUnregistered;}
-		if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) {d_t = b->tris;}
-		else if (a.type == cudaMemoryTypeHost && a.devicePointer) {d_t = (float *)a.devicePointer;}
-		else return tw_set_error(ctx, TW_ERR_ARG, "tris must be device or page-locked host memory (the emit pass writes it directly)");
+		d_t = (float *)device_view(b->tris);
+		if (!d_t) return tw_set_error(ctx, TW_ERR_ARG, "tris must be device or page-locked host memory (the emit pass writes it directly)");
+	}
+	tw_voxel_mesh M;
+	memset(&M, 0, sizeof(M));
+	float *d_mv = nullptr;
+	uint32_t *d_mi = nullptr;
+	if (wm) {
+		M = *mesh;
+		rc = validate_mesh(ctx, &P, &M); if (rc) return rc;
+		if (M.verts && !(d_mv = (float *)device_view(M.verts))) return tw_set_error(ctx, TW_ERR_ARG, "mesh verts must be device or page-locked host memory");
+		if (M.indices && !(d_mi = (uint32_t *)device_view(M.indices))) return tw_set_error(ctx, TW_ERR_ARG, "mesh indices must be device or page-locked host memory");
 	}
 	bool const rm = (P.remove_unconnected > 0);
 	unsigned blocks = 0;
@@ -490,12 +767,13 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
 	bool const dev_v = b->vals && tw_is_device_ptr(b->vals), dev_z = b->zix_xy && tw_is_device_ptr(b->zix_xy);
 	size_t const TAB = 1024 + 16384 + 96;
-	size_t const vb = dev_v ? 0 : al256(n*sizeof(float)), ob = al256(n + 4), fb = rm ? al256((n + 16)*sizeof(unsigned)) : 0, tb = mc ? al256(TAB) : 0;
+	bool const tabs = (ntab == 3);
+	size_t const vb = dev_v ? 0 : al256(n*sizeof(float)), ob = al256(n + 4), fb = rm ? al256((n + 16)*sizeof(unsigned)) : 0, tb = tabs ? al256(TAB) : 0;
 	size_t const sb = mc ? al256((size_t)nblocks*sizeof(unsigned)) : 0, ofb = mc ? al256((size_t)nblocks*sizeof(unsigned long long)) : 0;
-	size_t const zb = (b->zix_xy && !dev_z) ? al256(nxy*sizeof(unsigned)) : 0;
-	rc = tw_reserve(ctx, 0, 256 + vb + ob + 2*fb + tb + sb + ofb + zb); if (rc) return rc;
+	size_t const zb = (b->zix_xy && !dev_z) ? al256(nxy*sizeof(unsigned)) : 0, mb = wm ? mesh_scratch_bytes(n, nblocks) : 0;
+	rc = tw_reserve(ctx, 0, 256 + vb + ob + 2*fb + tb + sb + ofb + zb + mb); if (rc) return rc;
 	if (tab_bytes) {rc = tw_reserve(ctx, 1, tab_bytes); if (rc) return rc;}
-	size_t const off_rdata = 64, off_tab = off_rdata + al256(TW_N3D_RDATA*sizeof(float)), off_zix = off_tab + (mc ? al256(TAB) : 0);
+	size_t const off_rdata = 64, off_tab = off_rdata + al256(TW_N3D_RDATA*sizeof(float)), off_zix = off_tab + (tabs ? al256(TAB) : 0);
 	rc = tw_reserve_pinned(ctx, off_zix + zb); if (rc) return rc;
 	if (fill && F.gen_mode != TW_MGEN_SINE) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
 	char *sp = (char *)ctx->d_scratch[0], *h = (char *)ctx->h_pinned;
@@ -509,15 +787,18 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384); sp += tb;
 	unsigned *d_sums = (unsigned *)sp; sp += sb;
 	unsigned long long *d_offsets = (unsigned long long *)sp; sp += ofb;
-	const unsigned *d_z = dev_z ? b->zix_xy : (b->zix_xy ? (const unsigned *)sp : nullptr);
+	const unsigned *d_z = dev_z ? b->zix_xy : (b->zix_xy ? (const unsigned *)sp : nullptr); sp += zb;
+	MeshScratch S;
+	if (wm) {S = mesh_scratch(sp, n, nblocks);}
 	twi_job pending;
 	pending.kind = twi_job::VOXEL; pending.host_ntris = mc ? b->ntris : nullptr; pending.host_changed = b->changed; pending.cancellable = true;
+	pending.host_mesh_nverts = M.nverts; pending.host_mesh_ntris = M.ntris;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(cnt, 0, 256, ctx->stream));
 		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h + off_rdata); if (r) return r;}
 		else if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, b->vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
 		if (zb) {memcpy(h + off_zix, b->zix_xy, nxy*sizeof(unsigned)); TW_CUDA(ctx, cudaMemcpyAsync((void *)d_z, h + off_zix, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));}
-		if (mc) {
+		if (tabs) {
 			const void *src[3] = {b->edge_table256, b->tri_table256x16, b->edge_to_vals12x2};
 			size_t const off[3] = {0, 1024, 1024 + 16384}, len[3] = {1024, 16384, 96};
 			for (int k = 0; k < 3; ++k) {
@@ -540,11 +821,13 @@ extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {
 				TW_LAUNCH_CHECK(ctx);
 			}
 		}
+		if (wm) {int const r = enqueue_mesh(ctx, d_v, d_o, P, T, S, d_mv, M.vcapacity, d_mi, M.tcapacity); if (r) return r;}
 		if (b->vals && !dev_v && (fill || rm)) {TW_CUDA(ctx, cudaMemcpyAsync(b->vals, d_v, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 		if (b->outside) {TW_CUDA(ctx, cudaMemcpyAsync(b->outside, d_o, n, cudaMemcpyDefault, ctx->stream));}
 		twi_voxel_stage *const st = (twi_voxel_stage *)h;
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->ntris, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->changed, d_changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+		if (wm) {TW_CUDA(ctx, cudaMemcpyAsync(&st->nverts, S.totals, 2*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));}
 		return TW_OK;
 	});
 }

@@ -5,6 +5,7 @@
 //   tw3d::erode_heightmap_async  <->  heightmap_t::run_erosion on the set_heightmap image, without stalling the frame   src/heightmap.cpp:153-187
 //   tw3d::noise_gen_3d           <->  noise_gen_3d::{set_rand_seeds,gen_sines}        src/upsurface.h:39-50
 //   tw3d::create_procedural      <->  voxel_manager::create_procedural               src/voxels.h:196, src/voxels.cpp:278-346
+//   tw3d::voxel_mesh             <->  voxel_model::create_block's welded tri_verts    src/voxels.cpp:495-566,1077-1108
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
@@ -893,6 +894,31 @@ inline std::vector<float> voxel_build(voxel_grid_view const &v, std::vector<unsi
 	return tris;
 }
 
+// The indexed mesh of create_block (its tri_verts: vertex positions, then three vertex indices per triangle), welded as the reference's vertex cache
+// welds it (tw_voxel_mesh_welded), for the field and flags voxel_build leaves behind.
+struct voxel_mesh_t {std::vector<float> verts; std::vector<uint32_t> indices;}; // 3 floats per vertex, 3 indices per triangle
+inline voxel_mesh_t voxel_mesh(voxel_grid_view const &v, std::vector<unsigned char> const &outside, float isolevel, bool invert, bool make_closed_surface,
+	bool skip_under_mesh, const unsigned *edge_table, const int *tri_table, const unsigned *edge_to_vals)
+{
+	tw_voxel_post_params vp;
+	memset(&vp, 0, sizeof(vp));
+	vp.nx = v.nx; vp.ny = v.ny; vp.nz = v.nz;
+	for (int d = 0; d < 3; ++d) {vp.lo_pos[d] = v.lo_pos[d]; vp.vsz[d] = v.vsz[d];}
+	vp.isolevel = isolevel; vp.invert = invert; vp.make_closed_surface = make_closed_surface; vp.skip_under_mesh = skip_under_mesh;
+	voxel_mesh_t m;
+	uint64_t nv = 0, nt = 0;
+	tw_voxel_mesh out = {nullptr, 0, nullptr, 0, &nv, &nt};
+	tw_ctx *c = ctx();
+	int rc = tw_voxel_mesh_welded(c, v.data->data(), outside.data(), &vp, edge_table, tri_table, edge_to_vals, &out);
+	if (rc == TW_OK && (nv || nt)) {
+		m.verts.resize((size_t)nv*3); m.indices.resize((size_t)nt*3);
+		out.verts = m.verts.data(); out.vcapacity = nv; out.indices = m.indices.data(); out.tcapacity = nt;
+		rc = tw_voxel_mesh_welded(c, v.data->data(), outside.data(), &vp, edge_table, tri_table, edge_to_vals, &out);
+	}
+	if (rc != TW_OK) {detail::fail(rc, "voxel_mesh", c);}
+	return m;
+}
+
 // create_procedural + voxel_build as one job that does not stall the frame (tw_voxel_build_launch): returns at once, and ready() / wait() on the returned
 // tiles_job say when the outputs are complete, as for create_tiles_async. fill (optional, from procedural_params): fill the grid first; v.data is then an
 // optional output (nullptr: only triangles come out), without fill it is the input field. outside (optional, n bytes) receives the flags. tris: capacity*9
@@ -919,6 +945,34 @@ inline tiles_job voxel_build_async(voxel_grid_view const &v, tw_voxel_params con
 	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
 	uint64_t const number = ++jobs;
 	int const rc = tw_voxel_build_launch(c, &b);
+	if (rc != TW_OK) {detail::fail(rc, "voxel_build_async", c);}
+	return tiles_job(c, &jobs, number);
+}
+// the same job with the welded mesh of voxel_mesh as well (tw_voxel_build_launch_ex), or instead of the soup when tris == nullptr: verts (vcapacity*3
+// floats) and indices (tcapacity*3) in device or page-locked host memory, owned by the caller; nverts / ntris_mesh = the mesh's counts once the job is ready
+// (may exceed the capacities: nothing is written beyond them).
+inline tiles_job voxel_build_async(voxel_grid_view const &v, tw_voxel_params const *fill, unsigned char *outside, float isolevel, bool invert, bool make_closed_surface,
+	unsigned remove_unconnected, bool keep_at_edge, bool sphere_mode_or_no_mesh, bool skip_under_mesh, const uint32_t *zix_xy,
+	const unsigned *edge_table, const int *tri_table, const unsigned *edge_to_vals, float *tris, uint64_t capacity, uint64_t *ntris,
+	float *verts, uint64_t vcapacity, uint32_t *indices, uint64_t tcapacity, uint64_t &nverts, uint64_t &ntris_mesh)
+{
+	tw_voxel_post_params vp;
+	memset(&vp, 0, sizeof(vp));
+	vp.nx = v.nx; vp.ny = v.ny; vp.nz = v.nz;
+	for (int d = 0; d < 3; ++d) {vp.lo_pos[d] = v.lo_pos[d]; vp.vsz[d] = v.vsz[d];}
+	vp.isolevel = isolevel; vp.invert = invert; vp.make_closed_surface = make_closed_surface; vp.remove_unconnected = (int)remove_unconnected;
+	vp.keep_at_edge = keep_at_edge; vp.centre_seed = sphere_mode_or_no_mesh; vp.skip_under_mesh = skip_under_mesh;
+	if (fill && v.data) {v.data->resize((size_t)v.nx*v.ny*v.nz);}
+	tw_voxel_build b;
+	memset(&b, 0, sizeof(b));
+	b.fill = fill; b.post = &vp; b.zix_xy = zix_xy;
+	b.edge_table256 = edge_table; b.tri_table256x16 = tri_table; b.edge_to_vals12x2 = edge_to_vals;
+	b.vals = v.data ? v.data->data() : nullptr; b.outside = outside; b.tris = tris; b.capacity = capacity; b.ntris = ntris;
+	tw_voxel_mesh const m = {verts, vcapacity, indices, tcapacity, &nverts, &ntris_mesh};
+	tw_ctx *c = ctx();
+	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+	uint64_t const number = ++jobs;
+	int const rc = tw_voxel_build_launch_ex(c, &b, &m);
 	if (rc != TW_OK) {detail::fail(rc, "voxel_build_async", c);}
 	return tiles_job(c, &jobs, number);
 }

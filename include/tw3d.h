@@ -533,12 +533,33 @@ TW_API int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *outsid
 /* Marching cubes: voxel_manager::add_triangles_for_voxel at LOD 0 for every cube of the grid in the order of voxel_model::create_block (y, x, z),
  * src/voxels.cpp:485-566,1077-1108, as an UNWELDED triangle soup: tris[t] = 3 vertices x (x, y, z), each cube's vertices interpolated by that cube
  * (interpolate_pt); triangles whose normal is the zero vector are dropped as the reference drops them (:550). The reference additionally welds vertices
- * through a per-block index cache (a vertex on a shared edge keeps the position computed by the first cube that used it - at most 1 ulp from this soup's)
- * and averages normals; both stay with the renderer-side caller. The case tables are the caller's voxel_detail::edge_table[256], tri_table[256][16],
+ * through a per-block index cache: a vertex on a shared edge keeps the position computed by the first cube that used it. Neighbouring cubes walk a shared
+ * edge in opposite directions, so this soup's copy of a vertex can differ from the cached one by up to about two ulps of the edge's endpoint coordinate
+ * (many ulps of a coordinate near zero), and welding the soup by position cannot rebuild the reference's mesh: tw_voxel_mesh_welded returns that indexed mesh.
+ * Vertex normals stay with the renderer-side caller. The case tables are the caller's voxel_detail::edge_table[256], tri_table[256][16],
  * edge_to_vals[12][2] (src/marching_cubes.h; Paul Bourke's polygonise tables) - data, passed in like the sin table. tris: capacity*9 floats, host or
  * device (NULL with capacity 0 to only count); ntris = triangles the grid produces (may exceed capacity: nothing is written beyond it). */
 TW_API int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t *outside, const tw_voxel_post_params *vp, const uint32_t *edge_table256,
                        const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, float *tris, uint64_t capacity, uint64_t *ntris);
+/* The indexed (welded) mesh of voxel_model::create_block at LOD 0, one block (src/voxels.cpp:495-566,1077-1108): the cubes of tw_voxel_triangles, with
+ * one vertex per crossing grid edge. The edge's owner is the first cube containing it in (y, x, z) order that is not skipped (last layer of an axis,
+ * skip_under_mesh); its position is the owner's interpolate_pt along its local edge, in its edge_to_vals corner order. Vertices are ordered by owner, then
+ * by the owner's local edge 0..11: the creation order of a vertex cache filled for every crossing edge of a cube (vertices that only degenerate triangles
+ * use are kept, as the reference keeps them). Triangles: per cube in tri_table order, three vertex indices each, dropped when the normal of their WELDED
+ * positions is the zero vector, so their count can differ from the soup's. Flattening indices through verts gives the reference's welded triangles.
+ * edge_to_vals must name each of the cube's 12 edges once (Bourke's table does). */
+typedef struct tw_voxel_mesh {
+	float    *verts;      /* vcapacity*3 floats: x, y, z per vertex (NULL with vcapacity 0) */
+	uint64_t  vcapacity;
+	uint32_t *indices;    /* tcapacity*3 vertex indices (NULL with tcapacity 0) */
+	uint64_t  tcapacity;
+	uint64_t *nverts;     /* HOST, required: vertices / triangles of the mesh (may exceed the capacities: nothing is written beyond them) */
+	uint64_t *ntris;
+} tw_voxel_mesh;
+/* Synchronous. vals / outside / tables / verts / indices: host or device. TW_ERR_ARG: NULL arguments, a capacity without its buffer, an empty grid, or
+ * 3*nx*ny*nz >= 2^32 (the indices are 32-bit). */
+TW_API int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_t *outside, const tw_voxel_post_params *vp, const uint32_t *edge_table256,
+                                const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, const tw_voxel_mesh *out);
 /* voxel_manager::create_procedural + voxel_model::build as ONE asynchronous job: the fill (optional), tw_voxel_outside, tw_voxel_remove_unconnected and
  * tw_voxel_triangles enqueued on the context's stream without the host reading anything back in between (the flood fills end on the device). After the
  * completing poll every output is bit-identical to that sequence of synchronous calls on one context: tw_voxel_fill(fill, rdata420) if fill is set, then
@@ -565,6 +586,12 @@ typedef struct tw_voxel_build {
 	uint64_t *changed;   /* optional HOST: voxels flipped by remove_unconnected, filled by the completing poll */
 } tw_voxel_build;
 TW_API int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b);
+/* tw_voxel_build_launch with the welded mesh of tw_voxel_mesh_welded (on the flags and field after remove_unconnected) as well as, or instead of, the
+ * soup: mesh == NULL is tw_voxel_build_launch(b). With a mesh, the three tables are required, and b->ntris may be NULL for no soup (b->tris and
+ * b->capacity must then be NULL / 0). mesh->verts / indices: device or page-locked host memory, as b->tris; *mesh->nverts / *mesh->ntris are filled by the
+ * completing poll, and not on TW_ERR_CANCELED. The mesh struct is copied during the launch. Every rule of tw_voxel_build_launch applies; TW_ERR_ARG also
+ * for a mesh without tables or counts, a capacity without its buffer, pageable verts / indices and 3*nx*ny*nz >= 2^32. */
+TW_API int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, const tw_voxel_mesh *mesh);
 
 /* ---- mesh shadows of tiles (SURVEY.md 8f row N4): calc_mesh_shadows (src/visibility.cpp:411-517) for a batch of tiles with the neighbour chaining of
  * tile_t::calc_shadows_for_light (src/tiled_mesh.cpp:664-692) ---- */

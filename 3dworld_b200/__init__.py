@@ -82,6 +82,22 @@ class VoxelMesh(C.Structure):
     _fields_ = [("verts", C.c_void_p), ("vcapacity", C.c_uint64), ("indices", C.c_void_p), ("tcapacity", C.c_uint64), ("nverts", C.c_void_p), ("ntris", C.c_void_p)]
 
 
+class VoxelBlockMesh(C.Structure):
+    """tw_voxel_block_mesh (include/tw3d.h): one listed block's vertex and triangle ranges in a voxel model job's outputs."""
+    _fields_ = [("block", C.c_uint32), ("pad", C.c_uint32), ("voff", C.c_uint64), ("nverts", C.c_uint64), ("toff", C.c_uint64), ("ntris", C.c_uint64)]
+
+
+class VoxelBlocksOut(C.Structure):
+    """tw_voxel_blocks_out (include/tw3d.h): a voxel model job's mesh buffers, block table and host counts."""
+    _fields_ = [("verts", C.c_void_p), ("vcapacity", C.c_uint64), ("indices", C.c_void_p), ("tcapacity", C.c_uint64), ("blocks", C.c_void_p),
+                ("nblocks", C.c_void_p), ("nverts", C.c_void_p), ("ntris", C.c_void_p), ("changed", C.c_void_p)]
+
+
+class VoxelBox(C.Structure):
+    """tw_voxel_box (include/tw3d.h): the voxels [x, x+w) x [y, y+h) x [z, z+d)."""
+    _fields_ = [(n, C.c_uint32) for n in ("x", "y", "z", "w", "h", "d")]
+
+
 class WeightParams(C.Structure):
     """tw_weight_params (include/tw3d.h): the terrain weights texture's tables and scene scalars."""
     _fields_ = [("h_dirt", C.c_float * 5), ("tex_class", C.c_int * 5), ("class_ix", C.c_int * 5), ("sthresh", (C.c_float * 2) * 2), ("zmin", C.c_float), ("zmax", C.c_float),
@@ -195,7 +211,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_tile_set_create", "tw_tile_set_destroy", "tw_tile_set_put", "tw_tile_set_remove", "tw_tile_set_stale", "tw_tile_set_shadows_launch",
                "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
-               "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex"]
+               "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
+               "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read"]
 
 
 def _load():
@@ -296,6 +313,12 @@ def _load():
     L.tw_voxel_build_launch.argtypes = [vp, C.POINTER(VoxelBuild)]
     L.tw_voxel_mesh_welded.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, C.POINTER(VoxelMesh)]
     L.tw_voxel_build_launch_ex.argtypes = [vp, C.POINTER(VoxelBuild), C.POINTER(VoxelMesh)]
+    L.tw_voxel_model_create.argtypes = [vp, C.POINTER(VoxelPostParams), vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
+    L.tw_voxel_model_destroy.argtypes = [vp]
+    L.tw_voxel_model_destroy.restype = None
+    L.tw_voxel_model_build_launch.argtypes = [vp, C.POINTER(VoxelParams), vp, vp, C.POINTER(VoxelBlocksOut)]
+    L.tw_voxel_model_edit_launch.argtypes = [vp, vp, C.c_uint32, vp, C.POINTER(VoxelBlocksOut)]
+    L.tw_voxel_model_read.argtypes = [vp, vp, vp, vp]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
@@ -517,6 +540,38 @@ class VoxelBuildJob:
         return int(self._changed.value)
 
 
+class VoxelModelJob:
+    """The host results of a VoxelModel job, filled by the poll that completes it: blocks (numpy structured array of the listed blocks' VoxelBlockMesh
+    rows: block, voff, nverts, toff, ntris), nverts, ntris and changed."""
+
+    def __init__(self, nblocks_max):
+        self._table = (VoxelBlockMesh * max(nblocks_max, 1))()
+        self._nblocks, self._nverts, self._ntris, self._changed = C.c_uint32(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+
+    def _out(self, verts, indices):
+        size = lambda a: 0 if a is None else (int(a.numel()) if hasattr(a, "numel") else int(a.size)) // 3  # noqa: E731
+        p = lambda c: C.cast(C.pointer(c), C.c_void_p)  # noqa: E731
+        return VoxelBlocksOut(_ptr(verts), size(verts), _ptr(indices), size(indices), C.cast(self._table, C.c_void_p), p(self._nblocks), p(self._nverts),
+                              p(self._ntris), p(self._changed))
+
+    @property
+    def blocks(self):
+        n = int(self._nblocks.value)
+        return np.ctypeslib.as_array(self._table)[:n].copy() if n else np.zeros(0, np.ctypeslib.as_array(self._table).dtype)
+
+    @property
+    def nverts(self):
+        return int(self._nverts.value)
+
+    @property
+    def ntris(self):
+        return int(self._ntris.value)
+
+    @property
+    def changed(self):
+        return int(self._changed.value)
+
+
 class HeightmapJob:
     """The host result of Context.proc_gen_heightmap_launch: info (HeightmapInfo) is filled by the poll that completes the job."""
 
@@ -542,7 +597,7 @@ class Context:
             raise TwError(rc, "tw_create failed (no CUDA device? this library has no CPU fallback)")
         self._h = h
         self.device = device
-        self.parent, self._shared, self._sets = None, [], []
+        self.parent, self._shared, self._sets, self._models = None, [], [], []
         self._check(lib.tw_set_sin_table(self._h, _ptr(sin_table)))
 
     def shared(self):
@@ -552,7 +607,7 @@ class Context:
         h = C.c_void_p()
         self._check(lib.tw_create_shared(self._h, C.byref(h)))
         s = Context.__new__(Context)
-        s._h, s.device, s.parent, s._shared, s._sets = h, self.device, self, [], []
+        s._h, s.device, s.parent, s._shared, s._sets, s._models = h, self.device, self, [], [], []
         self._shared.append(s)
         return s
 
@@ -560,13 +615,17 @@ class Context:
         """tw_tile_set_create: a TileSet of this context - the live tiles' zvals on the device and each light slot's cached mesh shadows."""
         return TileSet(self, zvsize, nlights)
 
+    def voxel_model(self, vpp, tables, zix_xy=None, bx=32, by=32):
+        """tw_voxel_model_create: a VoxelModel of this context - the field of grid vpp kept on the device, meshed per block of bx x by cube columns."""
+        return VoxelModel(self, vpp, tables, zix_xy, bx, by)
+
     def close(self):
         if getattr(self, "_h", None) and lib is not None:   # lib can already be gone at interpreter shutdown
             for s in getattr(self, "_shared", ()):         # tw_destroy(parent) destroys them: their handles must not be destroyed again
-                for ts in getattr(s, "_sets", ()):
+                for ts in list(getattr(s, "_sets", ())) + list(getattr(s, "_models", ())):
                     ts._h = None
                 s._h = None
-            for ts in getattr(self, "_sets", ()):           # and this context's tile sets
+            for ts in list(getattr(self, "_sets", ())) + list(getattr(self, "_models", ())):   # and this context's tile sets and voxel models
                 ts._h = None
             lib.tw_destroy(self._h)
             if getattr(self, "parent", None) is not None and self in self.parent._shared:
@@ -1006,6 +1065,72 @@ class Context:
         mm = MinMax()
         self._check(lib.tw_minmax_f32(self._h, _ptr(vals), int(np.prod(vals.shape)), C.byref(mm)))
         return mm.zmin, mm.zmax
+
+
+class VoxelModel:
+    """tw_voxel_model (include/tw3d.h): a voxel grid's raw field, outside flags and post-processed field kept on the device, meshed per block of bx x by
+    cube columns. build_launch and edit_launch are the context's asynchronous jobs, completed by Context.create_tiles_poll; they cannot be cancelled.
+    Context.close() destroys the model with the context."""
+
+    def __init__(self, ctx, vpp, tables, zix_xy, bx, by):
+        self.tables = tuple(np.ascontiguousarray(t, dt) for t, dt in zip(tables, (np.uint32, np.int32, np.uint32)))
+        z = None if zix_xy is None else (zix_xy if hasattr(zix_xy, "data_ptr") else np.ascontiguousarray(zix_xy, np.uint32))
+        h = C.c_void_p()
+        ctx._check(lib.tw_voxel_model_create(ctx._h, C.byref(vpp), _ptr(self.tables[0]), _ptr(self.tables[1]), _ptr(self.tables[2]), _ptr(z), int(bx), int(by),
+                                             C.byref(h)))
+        self._h, self.ctx, self.vpp, self.bx, self.by = h, ctx, vpp, int(bx), int(by)
+        self.nbx, self.nby = (max(int(vpp.nx) - 1, 0) + self.bx - 1) // self.bx, (max(int(vpp.ny) - 1, 0) + self.by - 1) // self.by
+        ctx._models.append(self)
+
+    @property
+    def nblocks(self):
+        return self.nbx * self.nby
+
+    def close(self):
+        if getattr(self, "_h", None) and lib is not None:
+            lib.tw_voxel_model_destroy(self._h)
+            if self in self.ctx._models:
+                self.ctx._models.remove(self)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def build_launch(self, fill=None, vals=None, rdata=None, verts=None, indices=None):
+        """tw_voxel_model_build_launch: the raw field from fill (VoxelParams) or vals (numpy or CUDA tensor, [ny, nx, nz] float32), its flags and
+        remove_unconnected, and every block's mesh into verts / indices (CUDA tensors or page-locked buffers, filled up to their sizes). Returns a
+        VoxelModelJob."""
+        job = VoxelModelJob(self.nblocks)
+        rd = None if rdata is None else np.ascontiguousarray(rdata, np.float32)
+        out = job._out(verts, indices)
+        self.ctx._check(lib.tw_voxel_model_build_launch(self._h, C.byref(fill) if fill is not None else None, _ptr(rd), _ptr(vals), C.byref(out)))
+        self.ctx._tiles_job = (vals, verts, indices, job)
+        return job
+
+    def edit_launch(self, boxes, values, verts=None, indices=None):
+        """tw_voxel_model_edit_launch: boxes = (x, y, z, w, h, d) tuples, values = their new raw values one box after another, each in the grid's order
+        (z fastest, then x, then y), copied during the launch. Re-meshes the blocks the edit changed; returns a VoxelModelJob listing them."""
+        b = (VoxelBox * max(len(boxes), 1))(*[VoxelBox(*[int(v) for v in t]) for t in boxes])
+        vals = np.ascontiguousarray(values, np.float32).ravel()
+        job = VoxelModelJob(self.nblocks)
+        out = job._out(verts, indices)
+        self.ctx._check(lib.tw_voxel_model_edit_launch(self._h, C.cast(b, C.c_void_p) if len(boxes) else None, len(boxes), _ptr(vals) if len(boxes) else None,
+                                                       C.byref(out)))
+        self.ctx._tiles_job = (verts, indices, job)
+        return job
+
+    def read(self, raw=None, vals=None, outside=None):
+        """tw_voxel_model_read (completes the pending job): (raw field, field after remove_unconnected, its flags), [ny, nx, nz] numpy arrays unless given."""
+        shape = (int(self.vpp.ny), int(self.vpp.nx), int(self.vpp.nz))
+        raw = np.empty(shape, np.float32) if raw is None else raw
+        vals = np.empty(shape, np.float32) if vals is None else vals
+        outside = np.empty(shape, np.uint8) if outside is None else outside
+        self.ctx._check(lib.tw_voxel_model_read(self._h, _ptr(raw), _ptr(vals), _ptr(outside)))
+        self.ctx._tiles_job = None
+        return raw, vals, outside
 
 
 class TileSet:

@@ -126,6 +126,14 @@ int poll_job(tw_ctx *ctx, int wait) {
 		if (j.host_mesh_nverts) {*j.host_mesh_nverts = st.nverts; *j.host_mesh_ntris = st.mesh_ntris;}
 		break;
 	}
+	case twi_job::VMODEL: {
+		twi_vmodel_stage st;
+		memcpy(&st, h, sizeof(st));
+		*j.host_nblocks = (uint32_t)st.nblocks; *j.host_mesh_nverts = st.nverts; *j.host_mesh_ntris = st.ntris;
+		if (j.host_changed) {*j.host_changed = st.changed;}
+		memcpy(j.host_blocks, h + 64, (size_t)st.nblocks*sizeof(tw_voxel_block_mesh));
+		break;
+	}
 	case twi_job::HMAP: { // tw_proc_gen_heightmap's order: the step count and info even when the pack fails, the image only when everything succeeded
 		twi_hmap_stage st;
 		memcpy(&st, h, sizeof(st));
@@ -319,6 +327,7 @@ int tw_create_shared(tw_ctx *parent, tw_ctx **out) {
 void tw_destroy(tw_ctx *ctx) {
 	if (!ctx) return;
 	while (!ctx->sets.empty()) tw_tile_set_destroy(ctx->sets.back()); // each completes the pending job and removes itself from the list
+	while (!ctx->models.empty()) tw_voxel_model_destroy(ctx->models.back()); // the same
 	while (!ctx->shared.empty()) tw_destroy(ctx->shared.back()); // each removes itself from the list
 	if (ctx->dist) tw_dist_finalize(ctx);
 	cudaSetDevice(ctx->device);
@@ -367,7 +376,7 @@ int tw_cancel(tw_ctx *ctx) {
 	int rc = check_ctx(ctx); if (rc) return rc;
 	twi_job const &j = ctx->async.job;
 	if (j.kind == twi_job::NONE) return TW_OK;
-	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "a job that touches a tile set cannot be cancelled: the set's state was committed at its launch");
+	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "a job that touches a tile set or a voxel model cannot be cancelled: its state was committed at its launch");
 	ctx->h_job->cancel = j.seq;
 	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->d_job_words->cancel, &ctx->h_job->cancel, sizeof(unsigned), cudaMemcpyHostToDevice, ctx->cancel_stream));
 	ctx->cancel_sent = true;

@@ -11,14 +11,16 @@
 
 // A voxel build's counts in ctx->h_pinned (tw_voxel_build_launch)
 struct twi_voxel_stage {unsigned long long ntris, changed, nverts, mesh_ntris;}; // nverts, mesh_ntris: the welded mesh (tw_voxel_build_launch_ex)
+// A voxel model job's counts in ctx->h_pinned, followed at byte 64 by the listed blocks' tw_voxel_block_mesh entries (tw_voxel_model_*_launch)
+struct twi_vmodel_stage {unsigned long long nblocks, nverts, ntris, changed;};
 
 // The one asynchronous job a context may have in flight, as the poll that reports its completion unpacks it: which kind it is, what it staged in
 // ctx->h_pinned and where that goes. A job is pending when its kind is not NONE. Only twi_launch_job makes a job pending and only poll_job (tw_api.cu)
 // takes it back.
 struct twi_job {
-	enum kind_t {NONE, TILES, VOXEL, HMAP};
+	enum kind_t {NONE, TILES, VOXEL, HMAP, VMODEL};
 	kind_t kind = NONE;
-	bool cancellable = false;             // tw_cancel may stop it (set by the launch; a job that touches a tile set is not)
+	bool cancellable = false;             // tw_cancel may stop it (set by the launch; a job that touches a tile set or a voxel model is not)
 	bool reads_image = false;             // it reads or writes the family's heightmap image: its work waits for the edits made before its launch (tw_update_heightmap)
 	unsigned seq = 0;                     // the context's number of the job (twi_launch_job), the one tw_cancel names
 	// TILES (tile jobs and frames; a 2-D grid is n = 1 with its min/max at offset 0; a relight stages nothing): n tiles' results at byte offsets into
@@ -34,6 +36,9 @@ struct twi_job {
 	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0, off_flags = 0;
 	// VOXEL: a twi_voxel_stage at ctx->h_pinned
 	uint64_t *host_ntris = nullptr, *host_changed = nullptr, *host_mesh_nverts = nullptr, *host_mesh_ntris = nullptr;
+	// VMODEL: a twi_vmodel_stage at ctx->h_pinned; host_mesh_nverts / host_mesh_ntris / host_changed take its counts
+	tw_voxel_block_mesh *host_blocks = nullptr;
+	uint32_t *host_nblocks = nullptr;
 	// HMAP (tw_proc_gen_heightmap_launch; tw_erode_launch, which fills only the stage's min_z, bad, fail and steps and has no host_info): a twi_hmap_stage at
 	// ctx->h_pinned
 	tw_heightmap_info *host_info = nullptr;
@@ -125,6 +130,7 @@ struct tw_ctx {
 	tw_ctx *parent = nullptr;
 	std::vector<tw_ctx *> shared; // the parent's live shared contexts
 	std::vector<tw_tile_set *> sets; // live tile sets (tw_tileset.cu), destroyed with the context
+	std::vector<tw_voxel_model *> models; // live voxel models (tw_voxel_post.cu), destroyed with the context
 };
 
 int  tw_set_error(tw_ctx *ctx, int status, const char *fmt, ...);

@@ -324,9 +324,15 @@ __device__ void mesh_edge_tables(const unsigned *__restrict__ etv, unsigned char
 	__syncthreads();
 }
 
-// cube (c[0], c[1], c[2]) makes triangles: inside the grid, not in the last layer of an axis, and not skip_under_mesh with its 4 low corners under the mesh
-__device__ __forceinline__ bool cube_valid(const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const int *c) {
+// A block of a voxel model (tw_voxel_model): the cubes x in [x0, x1), y in [y0, y1), every z. A cube's index within it is ((y - y0)*(x1 - x0) + x - x0)*nz + z.
+struct CubeRange {unsigned x0, x1, y0, y1;};
+
+// cube (c[0], c[1], c[2]) makes triangles: inside the grid (with BLK: inside R), not in the last layer of an axis, and not skip_under_mesh with its 4 low
+// corners under the mesh
+template<bool BLK = false>
+__device__ __forceinline__ bool cube_valid(const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const int *c, const CubeRange &R = CubeRange()) {
 	if (c[0] < 0 || c[1] < 0 || c[2] < 0 || (unsigned)c[0] + 1 >= P.nx || (unsigned)c[1] + 1 >= P.ny || (unsigned)c[2] + 1 >= P.nz) return false;
+	if (BLK && ((unsigned)c[0] < R.x0 || (unsigned)c[0] >= R.x1 || (unsigned)c[1] < R.y0 || (unsigned)c[1] >= R.y1)) return false;
 	if (!P.skip_under_mesh) return true;
 	for (unsigned k = 0; k < 4; ++k) {
 		size_t const ix = (unsigned)c[2] + ((size_t)(c[0] + (k & 1)) + (size_t)(c[1] + (k >> 1))*P.nx)*P.nz;
@@ -337,11 +343,11 @@ __device__ __forceinline__ bool cube_valid(const unsigned char *__restrict__ out
 
 // One cube of the welded mesh: the welded position of each of its crossing edges (vlist), each edge's owner (linear index) and local edge there (own, oj),
 // the edges it owns (mask) and the triangles whose welded positions have a nonzero normal (kept, bit k = the k-th triangle of tri_table). Returns the
-// number of kept triangles.
+// number of kept triangles. With BLK the cube is one of block R's, only R's cubes can own an edge, and own / ci are indices within R.
 struct MeshCube {float vlist[12][3]; unsigned own[12]; unsigned char oj[12], tri[5][3]; unsigned mask, kept;};
-template<bool EMIT>
+template<bool EMIT, bool BLK = false>
 __device__ unsigned cube_mesh(const float *__restrict__ vals, const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const McTables &T,
-	const unsigned char *s_edge, const unsigned char *s_look, unsigned x, unsigned y, unsigned z, unsigned ci, MeshCube &m)
+	const unsigned char *s_edge, const unsigned char *s_look, unsigned x, unsigned y, unsigned z, unsigned ci, MeshCube &m, const CubeRange &R = CubeRange())
 {
 	m.mask = 0; m.kept = 0;
 	unsigned const nx = P.nx, ny = P.ny, nz = P.nz;
@@ -374,9 +380,13 @@ __device__ unsigned cube_mesh(const float *__restrict__ vals, const unsigned cha
 			int c[3] = {g[0], g[1], g[2]};
 			c[p1] -= (int)d1; c[p2] -= (int)d2;
 			if (c[0] == (int)x && c[1] == (int)y && c[2] == (int)z) {m.mask |= 1u << i; break;} // no earlier cube makes triangles: this one owns it
-			if (cube_valid(outside, P, c)) {o[0] = c[0]; o[1] = c[1]; o[2] = c[2]; j = s_look[4*a + 2*d1 + d2]; break;}
+			if (cube_valid<BLK>(outside, P, c, R)) {o[0] = c[0]; o[1] = c[1]; o[2] = c[2]; j = s_look[4*a + 2*d1 + d2]; break;}
 		}
-		if (EMIT) {m.own[i] = (m.mask & (1u << i)) ? ci : (unsigned)o[2] + ((unsigned)o[0] + (unsigned)o[1]*nx)*nz; m.oj[i] = (unsigned char)j;}
+		if (EMIT) {
+			m.own[i] = (m.mask & (1u << i)) ? ci : BLK ? (((unsigned)o[1] - R.y0)*(R.x1 - R.x0) + (unsigned)o[0] - R.x0)*nz + (unsigned)o[2]
+			                                            : (unsigned)o[2] + ((unsigned)o[0] + (unsigned)o[1]*nx)*nz;
+			m.oj[i] = (unsigned char)j;
+		}
 		float v2[2], pts[2][3];
 #pragma unroll
 		for (unsigned d = 0; d < 2; ++d) { // the owner's interpolation: its corners, in its order
@@ -830,4 +840,445 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 		if (wm) {TW_CUDA(ctx, cudaMemcpyAsync(&st->nverts, S.totals, 2*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));}
 		return TW_OK;
 	});
+}
+
+// ------------------------------------------------------------------------------------------------ resident voxel models (tw_voxel_model_*)
+// The model's device state (one allocation): raw field and flags, the field and flags after remove_unconnected (post), a working copy of those (work),
+// zix_xy, the tables, one mark byte per block, and two block lists {count, blocks...}: every block in order (build) and the marked ones (edit).
+// A job meshes the blocks of a list with block_mesh_kernel: launch block k handles chunk k % chunks of the block in list slot k / chunks (chunks = MC_BLOCK-cube
+// chunks of the largest block), so the grid is sized for every block listed and the slots past the device-side count exit at once. Count, the two scans of
+// mesh_kernel (over slots x chunks, so a block's vertices and triangles are contiguous and in list order), emit, then the table of the listed blocks.
+struct tw_voxel_model {
+	tw_ctx *ctx = nullptr;
+	tw_voxel_post_params P;
+	unsigned bx = 1, by = 1, nbx = 0, nblocks = 0, chunks = 0;
+	bool built = false, have_zix = false;
+	char *mem = nullptr;
+	float *raw = nullptr, *post = nullptr, *work = nullptr;
+	unsigned char *raw_o = nullptr, *post_o = nullptr, *work_o = nullptr, *mark = nullptr;
+	unsigned *zix = nullptr, *all = nullptr, *marked = nullptr;
+	void *tables = nullptr;
+};
+
+namespace {
+
+struct BlockGrid {unsigned bx, by, nbx, chunks;};
+
+__device__ __forceinline__ CubeRange block_range(const tw_voxel_post_params &P, const BlockGrid &G, unsigned b) {
+	CubeRange R;
+	R.x0 = (b % G.nbx)*G.bx; R.y0 = (b / G.nbx)*G.by;
+	R.x1 = min(R.x0 + G.bx, P.nx - 1); R.y1 = min(R.y0 + G.by, P.ny - 1);
+	return R;
+}
+
+// the welded mesh of the blocks list[1 .. 1 + list[0]) (see above); words: slots x chunks x MC_BLOCK, the per-cube words of mesh_kernel at the block's local
+// cube index; vsums / tsums / voff / toff: one entry per launch block
+template<bool EMIT>
+__global__ void __launch_bounds__(MC_BLOCK)
+block_mesh_kernel(const float *__restrict__ vals, const unsigned char *__restrict__ outside, tw_voxel_post_params P, McTables T, BlockGrid G,
+	const unsigned *__restrict__ list, unsigned *__restrict__ words, unsigned *__restrict__ vsums, unsigned *__restrict__ tsums,
+	const unsigned long long *__restrict__ voff, const unsigned long long *__restrict__ toff, float *__restrict__ verts, unsigned long long vcap,
+	uint32_t *__restrict__ indices, unsigned long long tcap)
+{
+	unsigned const slot = blockIdx.x / G.chunks;
+	if (slot >= __ldg(list)) { // not listed: nothing to count (the scans read zeros), nothing to emit
+		if (!EMIT && threadIdx.x == 0) {vsums[blockIdx.x] = 0; tsums[blockIdx.x] = 0;}
+		return;
+	}
+	__shared__ unsigned warp_sums[MC_BLOCK/32];
+	__shared__ unsigned char s_edge[12], s_look[12];
+	mesh_edge_tables(T.edge_to_vals, s_edge, s_look);
+	CubeRange const R = block_range(P, G, __ldg(list + 1 + slot));
+	unsigned const w = R.x1 - R.x0, ncubes = (R.y1 - R.y0)*w*P.nz;
+	unsigned const l = (blockIdx.x - slot*G.chunks)*MC_BLOCK + threadIdx.x;
+	MeshCube m;
+	m.mask = 0;
+	unsigned cnt = 0;
+	if (l < ncubes) {
+		unsigned const xy = l / P.nz;
+		unsigned const nt = cube_mesh<EMIT, true>(vals, outside, P, T, s_edge, s_look, R.x0 + xy % w, R.y0 + xy / w, l - xy*P.nz, l, m, R);
+		cnt = ((unsigned)__popc(m.mask) << 16) | nt;
+	}
+	unsigned const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	unsigned incl = cnt;
+	for (int o = 1; o < 32; o <<= 1) {unsigned const v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= (unsigned)o) incl += v;}
+	if (lane == 31) {warp_sums[warp] = incl;}
+	__syncthreads();
+	if (warp == 0) {
+		unsigned w = warp_sums[lane], wi = w;
+		for (int o = 1; o < 32; o <<= 1) {unsigned const v = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= (unsigned)o) wi += v;}
+		warp_sums[lane] = wi - w;
+		if (!EMIT && lane == 31) {vsums[blockIdx.x] = wi >> 16; tsums[blockIdx.x] = wi & 0xffffu;}
+	}
+	__syncthreads();
+	unsigned const excl = warp_sums[warp] + (incl - cnt);
+	unsigned *const bw = words + (size_t)slot*G.chunks*MC_BLOCK;
+	if (!EMIT) {
+		if (l < ncubes) {bw[l] = (excl & 0xffff0000u) | m.mask;}
+		return;
+	}
+	if (l >= ncubes) return;
+	const unsigned long long *const bvoff = voff + (size_t)slot*G.chunks;
+	unsigned long long const vbase = voff[blockIdx.x] + (excl >> 16);
+	for (unsigned mk = m.mask; mk; mk &= mk - 1) {
+		unsigned const e = __ffs(mk) - 1;
+		unsigned long long const s = vbase + __popc(m.mask & ((1u << e) - 1));
+		if (s < vcap) {float *o = verts + 3*s; o[0] = m.vlist[e][0]; o[1] = m.vlist[e][1]; o[2] = m.vlist[e][2];}
+	}
+	unsigned long long const tbase = toff[blockIdx.x] + (excl & 0xffffu);
+	for (unsigned k = 0; k < (cnt & 0xffffu); ++k) {
+		unsigned long long const s = tbase + k;
+		if (s >= tcap) break;
+		for (unsigned v = 0; v < 3; ++v) {
+			unsigned const e = m.tri[k][v], owner = m.own[e], ow = bw[owner];
+			indices[3*s + v] = (uint32_t)(bvoff[owner / MC_BLOCK] - bvoff[0] + (ow >> 16) + __popc(ow & 0xfffu & ((1u << m.oj[e]) - 1)));
+		}
+	}
+}
+
+// the listed blocks' ranges: entry s of slot s < list[0] (nslots: the grid's slots; offsets past the last are the totals)
+__global__ void block_table_kernel(const unsigned *__restrict__ list, unsigned chunks, unsigned nslots, const unsigned long long *__restrict__ voff,
+	const unsigned long long *__restrict__ toff, const unsigned long long *__restrict__ totals, tw_voxel_block_mesh *__restrict__ table)
+{
+	unsigned const s = blockIdx.x*blockDim.x + threadIdx.x;
+	if (s >= list[0]) return;
+	size_t const a = (size_t)s*chunks, b = a + chunks;
+	unsigned long long const v1 = (s + 1 < nslots) ? voff[b] : totals[0], t1 = (s + 1 < nslots) ? toff[b] : totals[1];
+	tw_voxel_block_mesh e;
+	e.block = list[1 + s]; e.pad = 0; e.voff = voff[a]; e.nverts = v1 - voff[a]; e.toff = toff[a]; e.ntris = t1 - toff[a];
+	table[s] = e;
+}
+
+// list = {count, the marked blocks in ascending order}; clears the marks (one block)
+__global__ void __launch_bounds__(1024) list_marked_kernel(unsigned char *__restrict__ mark, unsigned nblocks, unsigned *__restrict__ list) {
+	__shared__ unsigned warp_sums[32];
+	__shared__ unsigned carry;
+	if (threadIdx.x == 0) {carry = 0;}
+	__syncthreads();
+	unsigned const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	for (unsigned base = 0; base < nblocks; base += 1024) {
+		unsigned const i = base + threadIdx.x;
+		bool const f = (i < nblocks) && mark[i];
+		if (f) {mark[i] = 0;}
+		unsigned const bal = __ballot_sync(0xffffffffu, f);
+		if (lane == 0) {warp_sums[warp] = __popc(bal);}
+		__syncthreads();
+		if (warp == 0) {
+			unsigned w = warp_sums[lane], wi = w;
+			for (int o = 1; o < 32; o <<= 1) {unsigned const v = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= (unsigned)o) wi += v;}
+			warp_sums[lane] = wi - w;
+		}
+		__syncthreads();
+		if (f) {list[1 + carry + warp_sums[warp] + __popc(bal & ((1u << lane) - 1))] = i;}
+		__syncthreads();
+		if (threadIdx.x == 1023) {carry += warp_sums[31] + __popc(bal);}
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) {list[0] = carry;}
+}
+
+// every block whose cubes read voxel column (x, y): the cubes x-1, x and y-1, y that exist
+__device__ __forceinline__ void mark_readers(unsigned char *mark, const tw_voxel_post_params &P, const BlockGrid &G, unsigned x, unsigned y) {
+	for (unsigned cy = (y ? y - 1 : 0); cy <= y && cy + 1 < P.ny; ++cy) {
+		for (unsigned cx = (x ? x - 1 : 0); cx <= x && cx + 1 < P.nx; ++cx) {mark[(cy / G.by)*G.nbx + cx / G.bx] = 1;}
+	}
+}
+
+// an edit's box and the index of its first value among the packed values; later: a later box overlaps it
+struct twi_box {unsigned x, y, z, w, h, d; unsigned long long off; unsigned later, pad;};
+
+// the edit's values into the raw field, with the raw flags of outside_kernel; post (rm == 0, where the post field is the raw one): also compared with the
+// model's field and flags, which take the new values, marking the blocks that read a changed voxel
+__global__ void box_scatter_kernel(const twi_box *__restrict__ boxes, unsigned nboxes, const float *__restrict__ values, unsigned long long total,
+	tw_voxel_post_params P, const unsigned *__restrict__ zix_xy, BlockGrid G, float *__restrict__ raw, unsigned char *__restrict__ raw_o, float *post,
+	unsigned char *post_o, unsigned char *mark)
+{
+	unsigned long long const stride = (unsigned long long)gridDim.x*blockDim.x;
+	for (unsigned long long t = (unsigned long long)blockIdx.x*blockDim.x + threadIdx.x; t < total; t += stride) {
+		unsigned lo = 0, hi = nboxes - 1;
+		while (lo < hi) {unsigned const mid = (lo + hi + 1) >> 1; if (boxes[mid].off <= t) lo = mid; else hi = mid - 1;}
+		twi_box const B = boxes[lo];
+		unsigned long long const r = t - B.off, xy = r / B.d;
+		unsigned const z = B.z + (unsigned)(r - xy*B.d), x = B.x + (unsigned)(xy % B.w), y = B.y + (unsigned)(xy / B.w);
+		bool overwritten = false;
+		for (unsigned k = lo + 1; B.later && k < nboxes && !overwritten; ++k) {
+			twi_box const &C = boxes[k];
+			overwritten = (x - C.x < C.w && y - C.y < C.h && z - C.z < C.d);
+		}
+		if (overwritten) continue;
+		size_t const i = z + ((size_t)x + (size_t)y*P.nx)*P.nz;
+		float const val = values[t];
+		bool const on_edge = (P.make_closed_surface && ((x == 0 || x == P.nx-1) || (y == 0 || y == P.ny-1) || (z == 0 || z == P.nz-1)));
+		unsigned char o = on_edge ? (unsigned char)TW_VOX_ON_EDGE : (unsigned char)((val == P.isolevel) ? 1 : (((val < P.isolevel) != (P.invert != 0)) ? 1 : 0));
+		if (zix_xy && z < __ldg(zix_xy + (size_t)y*P.nx + x)) {o |= TW_VOX_UNDER_MESH;}
+		raw[i] = val; raw_o[i] = o;
+		if (post && (__float_as_uint(post[i]) != __float_as_uint(val) || post_o[i] != o)) {post[i] = val; post_o[i] = o; mark_readers(mark, P, G, x, y);}
+	}
+}
+
+// the model's field and flags (ov, oo) take the new ones (nv, no) where they differ, marking the blocks that read a changed voxel
+__global__ void diff_kernel(const float *__restrict__ nv, const unsigned char *__restrict__ no, float *__restrict__ ov, unsigned char *__restrict__ oo,
+	tw_voxel_post_params P, BlockGrid G, unsigned char *__restrict__ mark, size_t n)
+{
+	size_t const stride = (size_t)gridDim.x*blockDim.x;
+	for (size_t i = (size_t)blockIdx.x*blockDim.x + threadIdx.x; i < n; i += stride) {
+		float const v = nv[i];
+		unsigned char const o = no[i];
+		if (__float_as_uint(v) == __float_as_uint(ov[i]) && o == oo[i]) continue;
+		ov[i] = v; oo[i] = o;
+		size_t const xy = i / P.nz;
+		mark_readers(mark, P, G, (unsigned)(xy % P.nx), (unsigned)(xy / P.nx));
+	}
+}
+
+BlockGrid block_grid(const tw_voxel_model *m) {BlockGrid G; G.bx = m->bx; G.by = m->by; G.nbx = m->nbx; G.chunks = m->chunks; return G;}
+McTables model_tables(const tw_voxel_model *m) {
+	McTables T;
+	T.edge_table = (const unsigned *)m->tables; T.tri_table = (const int *)((const char *)m->tables + 1024);
+	T.edge_to_vals = (const unsigned *)((const char *)m->tables + 1024 + 16384);
+	return T;
+}
+
+// A model job's slot-0 scratch: [counters (64 B) | changed (64 B) | pad to 256 | frontiers (remove_unconnected > 0) | mesh scratch | table | boxes | values]
+// and pinned staging: [twi_vmodel_stage (64 B) | table | boxes | values | fill coefficients]
+struct ModelScratch {unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values; char *h_boxes, *h_values, *h_rdata;};
+int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X) {
+	tw_ctx *ctx = m->ctx;
+	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz, ng = (size_t)m->nblocks*m->chunks;
+	size_t const fb = (m->P.remove_unconnected > 0) ? al256((n + 16)*sizeof(unsigned)) : 0, mb = mesh_scratch_bytes(ng*MC_BLOCK, (unsigned)ng);
+	size_t const tb = al256((size_t)m->nblocks*sizeof(tw_voxel_block_mesh)), bb = al256(nboxes*sizeof(twi_box)), vb = al256(nvalues*sizeof(float));
+	size_t const rb = al256(TW_N3D_RDATA*sizeof(float));
+	int rc = tw_reserve(ctx, 0, 256 + 2*fb + mb + tb + bb + vb); if (rc) return rc;
+	rc = tw_reserve_pinned(ctx, 64 + tb + bb + vb + rb); if (rc) return rc;
+	char *sp = (char *)ctx->d_scratch[0], *h = (char *)ctx->h_pinned;
+	X->cnt = (unsigned *)sp; X->changed = (unsigned long long *)(sp + 64); sp += 256;
+	X->f0 = (unsigned *)sp; X->f1 = (unsigned *)(sp + fb); sp += 2*fb;
+	X->S = mesh_scratch(sp, ng*MC_BLOCK, (unsigned)ng); sp += mb;
+	X->table = (tw_voxel_block_mesh *)sp; sp += tb;
+	X->boxes = (twi_box *)sp; sp += bb;
+	X->values = (float *)sp;
+	X->h_boxes = h + 64 + tb; X->h_values = X->h_boxes + bb; X->h_rdata = X->h_values + vb;
+	return TW_OK;
+}
+
+int validate_blocks_out(tw_ctx *ctx, const tw_voxel_blocks_out *o, float **d_vt, uint32_t **d_ix) {
+	if (!o || !o->blocks || !o->nblocks || !o->nverts || !o->ntris) return tw_set_error(ctx, TW_ERR_ARG, "the block meshes need blocks, nblocks, nverts and ntris");
+	if ((o->vcapacity && !o->verts) || (o->tcapacity && !o->indices)) return tw_set_error(ctx, TW_ERR_ARG, "a mesh capacity without its buffer");
+	*d_vt = nullptr; *d_ix = nullptr;
+	if (o->verts && !(*d_vt = (float *)device_view(o->verts))) return tw_set_error(ctx, TW_ERR_ARG, "verts must be device or page-locked host memory");
+	if (o->indices && !(*d_ix = (uint32_t *)device_view(o->indices))) return tw_set_error(ctx, TW_ERR_ARG, "indices must be device or page-locked host memory");
+	return TW_OK;
+}
+
+// the meshes of the blocks in d_list, their table and the job's counts into the pinned stage
+int enqueue_block_meshes(tw_voxel_model *m, const unsigned *d_list, const ModelScratch &X, float *d_vt, uint64_t vcap, uint32_t *d_ix, uint64_t tcap) {
+	tw_ctx *ctx = m->ctx;
+	char *h = (char *)ctx->h_pinned;
+	twi_vmodel_stage *const st = (twi_vmodel_stage *)h;
+	if (m->nblocks) {
+		unsigned const ng = m->nblocks*m->chunks;
+		McTables const T = model_tables(m);
+		BlockGrid const G = block_grid(m);
+		MeshScratch const &S = X.S;
+		block_mesh_kernel<false><<<ng, MC_BLOCK, 0, ctx->stream>>>(m->post, m->post_o, m->P, T, G, d_list, S.words, S.vsums, S.tsums, nullptr, nullptr, nullptr, 0, nullptr, 0);
+		TW_LAUNCH_CHECK(ctx);
+		scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(S.vsums, ng, S.voff, S.totals);
+		TW_LAUNCH_CHECK(ctx);
+		scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(S.tsums, ng, S.toff, S.totals + 1);
+		TW_LAUNCH_CHECK(ctx);
+		if (vcap || tcap) {
+			block_mesh_kernel<true><<<ng, MC_BLOCK, 0, ctx->stream>>>(m->post, m->post_o, m->P, T, G, d_list, S.words, nullptr, nullptr, S.voff, S.toff, d_vt, vcap, d_ix, tcap);
+			TW_LAUNCH_CHECK(ctx);
+		}
+		block_table_kernel<<<(m->nblocks + 255)/256, 256, 0, ctx->stream>>>(d_list, m->chunks, m->nblocks, S.voff, S.toff, S.totals, X.table);
+		TW_LAUNCH_CHECK(ctx);
+		TW_CUDA(ctx, cudaMemcpyAsync(&st->nblocks, d_list, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream)); // the low word (little-endian)
+		TW_CUDA(ctx, cudaMemcpyAsync(&st->nverts, S.totals, 2*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+		TW_CUDA(ctx, cudaMemcpyAsync(h + 64, X.table, (size_t)m->nblocks*sizeof(tw_voxel_block_mesh), cudaMemcpyDeviceToHost, ctx->stream));
+	}
+	TW_CUDA(ctx, cudaMemcpyAsync(&st->changed, X.changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+	return TW_OK;
+}
+
+twi_job model_job(const tw_voxel_blocks_out *o) {
+	twi_job j;
+	j.kind = twi_job::VMODEL; j.cancellable = false;
+	j.host_blocks = o->blocks; j.host_nblocks = o->nblocks; j.host_mesh_nverts = o->nverts; j.host_mesh_ntris = o->ntris; j.host_changed = o->changed;
+	return j;
+}
+
+int model_begin(tw_voxel_model *m) {
+	if (!m) return TW_ERR_ARG;
+	TW_CUDA(m->ctx, cudaSetDevice(m->ctx->device));
+	return twi_finish_pending(m->ctx);
+}
+
+} // namespace
+
+extern "C" int tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp, const uint32_t *edge_table256, const int32_t *tri_table256x16,
+                                     const uint32_t *edge_to_vals12x2, const uint32_t *zix_xy, uint32_t bx, uint32_t by, tw_voxel_model **out)
+{
+	if (!ctx) return TW_ERR_ARG;
+	if (!out || !edge_table256 || !tri_table256x16 || !edge_to_vals12x2) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_create: null argument");
+	*out = nullptr;
+	TW_CUDA(ctx, cudaSetDevice(ctx->device));
+	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int rc = validate(ctx, vp); if (rc) return rc;
+	if (bx == 0 || by == 0) return tw_set_error(ctx, TW_ERR_ARG, "block sizes must be >= 1");
+	tw_voxel_post_params const P = *vp;
+	unsigned const ncx = P.nx - 1, ncy = P.ny - 1, bw = (bx < ncx) ? bx : ncx, bh = (by < ncy) ? by : ncy;
+	if (3ull*(bw + 1)*(bh + 1)*P.nz >= 0x100000000ull) return tw_set_error(ctx, TW_ERR_ARG, "a block's indices are 32-bit: 3*(bx+1)*(by+1)*nz must be below 2^32");
+	size_t const n = (size_t)P.nx*P.ny*P.nz, nxy = (size_t)P.nx*P.ny;
+	unsigned const nbx = (ncx + bx - 1)/bx, nby = (ncy + by - 1)/by, nblocks = nbx*nby;
+	size_t const fb = al256(n*sizeof(float)), ob = al256(n + 4), zb = zix_xy ? al256(nxy*sizeof(unsigned)) : 0, tb = al256(1024 + 16384 + 96);
+	size_t const mkb = al256(nblocks + 1), lb = al256(((size_t)nblocks + 1)*sizeof(unsigned));
+	tw_voxel_model *m = new (std::nothrow) tw_voxel_model();
+	if (!m) return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");
+	try {ctx->models.push_back(m);} catch (...) {delete m; return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");}
+	m->ctx = ctx; m->P = P; m->bx = bx; m->by = by; m->nbx = nbx; m->nblocks = nblocks; m->chunks = (unsigned)(((size_t)bw*bh*P.nz + MC_BLOCK - 1)/MC_BLOCK);
+	m->have_zix = (zix_xy != nullptr);
+	if (cudaMalloc(&m->mem, 3*fb + 3*ob + zb + tb + mkb + 2*lb) != cudaSuccess) {
+		cudaGetLastError(); m->mem = nullptr; tw_voxel_model_destroy(m);
+		return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: no device memory for %zu voxels", n);
+	}
+	char *p = m->mem;
+	m->raw = (float *)p; p += fb; m->post = (float *)p; p += fb; m->work = (float *)p; p += fb;
+	m->raw_o = (unsigned char *)p; p += ob; m->post_o = (unsigned char *)p; p += ob; m->work_o = (unsigned char *)p; p += ob;
+	m->zix = zix_xy ? (unsigned *)p : nullptr; p += zb;
+	m->tables = p; p += tb;
+	m->mark = (unsigned char *)p; p += mkb;
+	m->all = (unsigned *)p; p += lb; m->marked = (unsigned *)p;
+	std::vector<unsigned> all((size_t)nblocks + 1);
+	all[0] = nblocks;
+	for (unsigned b = 0; b < nblocks; ++b) {all[1 + b] = b;}
+	rc = TW_OK;
+	auto up = [&](void *dst, const void *src, size_t len) {if (rc == TW_OK && cudaMemcpyAsync(dst, src, len, cudaMemcpyDefault, ctx->stream) != cudaSuccess) rc = TW_ERR_CUDA;};
+	up(m->tables, edge_table256, 1024); up((char *)m->tables + 1024, tri_table256x16, 16384); up((char *)m->tables + 1024 + 16384, edge_to_vals12x2, 96);
+	if (zix_xy) {up(m->zix, zix_xy, nxy*sizeof(unsigned));}
+	up(m->all, all.data(), all.size()*sizeof(unsigned));
+	if (rc == TW_OK && cudaMemsetAsync(m->mark, 0, nblocks + 1, ctx->stream) != cudaSuccess) rc = TW_ERR_CUDA;
+	if (rc == TW_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = TW_ERR_CUDA;
+	if (rc != TW_OK) {
+		cudaStreamSynchronize(ctx->stream);
+		char msg[256]; snprintf(msg, sizeof(msg), "tw_voxel_model_create: upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+		tw_voxel_model_destroy(m);
+		return tw_set_error(ctx, TW_ERR_CUDA, "%s", msg);
+	}
+	*out = m;
+	return TW_OK;
+}
+
+extern "C" void tw_voxel_model_destroy(tw_voxel_model *m) {
+	if (!m) return;
+	tw_ctx *ctx = m->ctx;
+	cudaSetDevice(ctx->device);
+	twi_finish_pending(ctx); // the job may still read or write the model
+	if (m->mem) cudaFree(m->mem);
+	for (size_t i = 0; i < ctx->models.size(); ++i) {if (ctx->models[i] == m) {ctx->models.erase(ctx->models.begin() + i); break;}}
+	delete m;
+}
+
+extern "C" int tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_params *fill, const float *rdata420, const float *vals, const tw_voxel_blocks_out *out) {
+	int rc = model_begin(m); if (rc) return rc;
+	tw_ctx *ctx = m->ctx;
+	if ((fill != nullptr) == (vals != nullptr)) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_build_launch: give either fill or vals");
+	float *d_vt; uint32_t *d_ix;
+	rc = validate_blocks_out(ctx, out, &d_vt, &d_ix); if (rc) return rc;
+	tw_voxel_blocks_out const O = *out;
+	tw_voxel_post_params const &P = m->P;
+	size_t tab_bytes = 0;
+	tw_voxel_params F;
+	if (fill) {
+		F = *fill;
+		if (F.nx != P.nx || F.ny != P.ny || F.nz != P.nz) return tw_set_error(ctx, TW_ERR_ARG, "the fill's grid %ux%ux%u differs from the model's %ux%ux%u", F.nx, F.ny, F.nz, P.nx, P.ny, P.nz);
+		rc = twi_voxel_fill_check(ctx, &F, &tab_bytes); if (rc) return rc;
+		if (tab_bytes) {rc = tw_reserve(ctx, 1, tab_bytes); if (rc) return rc;}
+		if (F.gen_mode != TW_MGEN_SINE) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
+	}
+	bool const rm = (P.remove_unconnected > 0);
+	unsigned blocks = 0;
+	if (rm) {rc = flood_blocks(ctx, &blocks); if (rc) return rc;}
+	ModelScratch X;
+	rc = model_scratch(m, 0, 0, &X); if (rc) return rc;
+	size_t const n = (size_t)P.nx*P.ny*P.nz;
+	memset(ctx->h_pinned, 0, sizeof(twi_vmodel_stage));
+	m->built = true; // the job commits the model's state
+	return twi_launch_job(ctx, model_job(&O), [&]() -> int {
+		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
+		if (fill) {int const r = twi_voxel_fill(ctx, &F, rdata420, m->raw, X.h_rdata); if (r) return r;}
+		else {TW_CUDA(ctx, cudaMemcpyAsync(m->raw, vals, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+		outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(m->raw, P, m->zix, m->raw_o, n);
+		TW_LAUNCH_CHECK(ctx);
+		TW_CUDA(ctx, cudaMemcpyAsync(m->post, m->raw, n*sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+		TW_CUDA(ctx, cudaMemcpyAsync(m->post_o, m->raw_o, n, cudaMemcpyDeviceToDevice, ctx->stream));
+		if (rm) {int const r = enqueue_remove_unconnected(ctx, blocks, m->post, m->post_o, &P, X.f0, X.f1, X.cnt, X.changed); if (r) return r;}
+		return enqueue_block_meshes(m, m->all, X, d_vt, O.vcapacity, d_ix, O.tcapacity);
+	});
+}
+
+extern "C" int tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out) {
+	int rc = model_begin(m); if (rc) return rc;
+	tw_ctx *ctx = m->ctx;
+	if (nboxes && (!boxes || !values)) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_edit_launch: null boxes or values");
+	float *d_vt; uint32_t *d_ix;
+	rc = validate_blocks_out(ctx, out, &d_vt, &d_ix); if (rc) return rc;
+	tw_voxel_blocks_out const O = *out;
+	tw_voxel_post_params const &P = m->P;
+	unsigned long long total = 0;
+	std::vector<twi_box> B(nboxes);
+	for (uint32_t k = 0; k < nboxes; ++k) {
+		tw_voxel_box const &b = boxes[k];
+		if (b.w == 0 || b.h == 0 || b.d == 0) return tw_set_error(ctx, TW_ERR_ARG, "box %u is empty", k);
+		if (b.x >= P.nx || b.w > P.nx - b.x || b.y >= P.ny || b.h > P.ny - b.y || b.z >= P.nz || b.d > P.nz - b.z)
+			return tw_set_error(ctx, TW_ERR_ARG, "box %u reaches outside the %ux%ux%u grid", k, P.nx, P.ny, P.nz);
+		twi_box &t = B[k];
+		t.x = b.x; t.y = b.y; t.z = b.z; t.w = b.w; t.h = b.h; t.d = b.d; t.off = total; t.later = 0; t.pad = 0;
+		total += (unsigned long long)b.w*b.h*b.d;
+	}
+	for (uint32_t k = 0; k < nboxes; ++k) { // overlaps: the later box's value wins
+		for (uint32_t j = k + 1; j < nboxes && !B[k].later; ++j) {
+			const twi_box &a = B[k], &b = B[j];
+			B[k].later = (a.x < b.x + b.w && b.x < a.x + a.w && a.y < b.y + b.h && b.y < a.y + a.h && a.z < b.z + b.d && b.z < a.z + a.d);
+		}
+	}
+	if (!m->built) return tw_set_error(ctx, TW_ERR_STATE, "the voxel model has no field yet (tw_voxel_model_build_launch)");
+	bool const rm = (P.remove_unconnected > 0);
+	unsigned blocks = 0;
+	if (rm && total) {rc = flood_blocks(ctx, &blocks); if (rc) return rc;}
+	ModelScratch X;
+	rc = model_scratch(m, nboxes, total, &X); if (rc) return rc;
+	size_t const n = (size_t)P.nx*P.ny*P.nz;
+	memset(ctx->h_pinned, 0, sizeof(twi_vmodel_stage));
+	if (nboxes) {memcpy(X.h_boxes, B.data(), nboxes*sizeof(twi_box)); memcpy(X.h_values, values, total*sizeof(float));}
+	return twi_launch_job(ctx, model_job(&O), [&]() -> int {
+		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
+		if (total) {
+			TW_CUDA(ctx, cudaMemcpyAsync(X.boxes, X.h_boxes, nboxes*sizeof(twi_box), cudaMemcpyHostToDevice, ctx->stream));
+			TW_CUDA(ctx, cudaMemcpyAsync(X.values, X.h_values, total*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+			box_scatter_kernel<<<stream_grid(ctx, total), 256, 0, ctx->stream>>>(X.boxes, nboxes, X.values, total, P, m->zix, block_grid(m), m->raw, m->raw_o,
+			                                                                     rm ? nullptr : m->post, rm ? nullptr : m->post_o, m->mark);
+			TW_LAUNCH_CHECK(ctx);
+			if (rm) {
+				TW_CUDA(ctx, cudaMemcpyAsync(m->work, m->raw, n*sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+				TW_CUDA(ctx, cudaMemcpyAsync(m->work_o, m->raw_o, n, cudaMemcpyDeviceToDevice, ctx->stream));
+				int const r = enqueue_remove_unconnected(ctx, blocks, m->work, m->work_o, &P, X.f0, X.f1, X.cnt, X.changed); if (r) return r;
+				diff_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(m->work, m->work_o, m->post, m->post_o, P, block_grid(m), m->mark, n);
+				TW_LAUNCH_CHECK(ctx);
+			}
+		}
+		if (m->nblocks) {list_marked_kernel<<<1, 1024, 0, ctx->stream>>>(m->mark, m->nblocks, m->marked); TW_LAUNCH_CHECK(ctx);}
+		return enqueue_block_meshes(m, m->marked, X, d_vt, O.vcapacity, d_ix, O.tcapacity);
+	});
+}
+
+extern "C" int tw_voxel_model_read(tw_voxel_model *m, float *raw, float *vals, uint8_t *outside) {
+	int rc = model_begin(m); if (rc) return rc;
+	tw_ctx *ctx = m->ctx;
+	if (!m->built) return tw_set_error(ctx, TW_ERR_STATE, "the voxel model has no field yet (tw_voxel_model_build_launch)");
+	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz;
+	if (raw) {TW_CUDA(ctx, cudaMemcpyAsync(raw, m->raw, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+	if (vals) {TW_CUDA(ctx, cudaMemcpyAsync(vals, m->post, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+	if (outside) {TW_CUDA(ctx, cudaMemcpyAsync(outside, m->post_o, n, cudaMemcpyDefault, ctx->stream));}
+	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return TW_OK;
 }

@@ -6,6 +6,7 @@
 //   tw3d::noise_gen_3d           <->  noise_gen_3d::{set_rand_seeds,gen_sines}        src/upsurface.h:39-50
 //   tw3d::create_procedural      <->  voxel_manager::create_procedural               src/voxels.h:196, src/voxels.cpp:278-346
 //   tw3d::voxel_mesh             <->  voxel_model::create_block's welded tri_verts    src/voxels.cpp:495-566,1077-1108
+//   tw3d::voxel_model            <->  voxel_model's brush edits + per-block create_block src/voxels.cpp:1077-1108,2139-2245
 //   tw3d::create_zvals_batch     <->  the height fill + erosion of tile_t::create_zvals for many tiles   src/tiled_mesh.cpp:467-515
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
@@ -976,6 +977,56 @@ inline tiles_job voxel_build_async(voxel_grid_view const &v, tw_voxel_params con
 	if (rc != TW_OK) {detail::fail(rc, "voxel_build_async", c);}
 	return tiles_job(c, &jobs, number);
 }
+
+// A voxel model edited with brushes (src/voxels.cpp:2139-2245) and meshed per block, as create_block keeps one mesh and vertex cache per block (:1077-1108),
+// kept on the device by the thread's context (tw_voxel_model_*). build_async takes the field from fill or from vals (v.data is not read) and meshes every
+// block; edit_async writes boxes of new raw values (one box after another, each z fastest, then x, then y) and re-meshes only the blocks whose cubes read a
+// voxel that changed. Both return a tiles_job of the context; out (verts / indices in device or page-locked memory, the host block table and counts) is
+// complete once it is ready. The jobs cannot be cancelled. read() completes the pending job and copies the raw field, the field after remove_unconnected
+// and its flags. Not copyable; destroyed with the context's pending job completed.
+class voxel_model {
+	tw_voxel_model *m = nullptr;
+	tw_ctx *c = nullptr;
+	size_t n = 0;
+	tiles_job job_of(int rc, const char *what) {
+		std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+		uint64_t const number = ++jobs;
+		if (rc != TW_OK) {--jobs; detail::fail(rc, what, c);}
+		return tiles_job(c, &jobs, number);
+	}
+public:
+	voxel_model(voxel_grid_view const &v, float isolevel, bool invert, bool make_closed_surface, unsigned remove_unconnected, bool keep_at_edge,
+	            bool sphere_mode_or_no_mesh, bool skip_under_mesh, const uint32_t *zix_xy, const unsigned *edge_table, const int *tri_table,
+	            const unsigned *edge_to_vals, unsigned bx, unsigned by)
+	{
+		tw_voxel_post_params vp;
+		memset(&vp, 0, sizeof(vp));
+		vp.nx = v.nx; vp.ny = v.ny; vp.nz = v.nz;
+		for (int d = 0; d < 3; ++d) {vp.lo_pos[d] = v.lo_pos[d]; vp.vsz[d] = v.vsz[d];}
+		vp.isolevel = isolevel; vp.invert = invert; vp.make_closed_surface = make_closed_surface; vp.remove_unconnected = (int)remove_unconnected;
+		vp.keep_at_edge = keep_at_edge; vp.centre_seed = sphere_mode_or_no_mesh; vp.skip_under_mesh = skip_under_mesh;
+		c = ctx();
+		n = (size_t)v.nx*v.ny*v.nz;
+		int const rc = tw_voxel_model_create(c, &vp, edge_table, tri_table, edge_to_vals, zix_xy, bx, by, &m);
+		if (rc != TW_OK) {detail::fail(rc, "voxel_model", c);}
+	}
+	~voxel_model() {tw_voxel_model_destroy(m);}
+	voxel_model(voxel_model const &) = delete;
+	voxel_model &operator=(voxel_model const &) = delete;
+	tiles_job build_async(tw_voxel_params const *fill, const float *vals, tw_voxel_blocks_out const &out) {
+		return job_of(tw_voxel_model_build_launch(m, fill, nullptr, vals, &out), "voxel_model::build_async");
+	}
+	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out) {
+		return job_of(tw_voxel_model_edit_launch(m, boxes.data(), (uint32_t)boxes.size(), values, &out), "voxel_model::edit_async");
+	}
+	void read(std::vector<float> *raw, std::vector<float> *vals, std::vector<unsigned char> *outside) {
+		if (raw) raw->resize(n);
+		if (vals) vals->resize(n);
+		if (outside) outside->resize(n);
+		int const rc = tw_voxel_model_read(m, raw ? raw->data() : nullptr, vals ? vals->data() : nullptr, outside ? outside->data() : nullptr);
+		if (rc != TW_OK) {detail::fail(rc, "voxel_model::read", c);}
+	}
+};
 
 // ------------------------------------------------------------------------------------------------ all GPUs of the box (include/tw3d.h "Multi-GPU")
 // One object per process: per-device contexts with the current tables, NUMA-local pinned output bands, the tile loop of tile_draw_t::update

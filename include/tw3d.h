@@ -593,6 +593,69 @@ TW_API int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b);
  * for a mesh without tables or counts, a capacity without its buffer, pageable verts / indices and 3*nx*ny*nz >= 2^32. */
 TW_API int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, const tw_voxel_mesh *mesh);
 
+/* ---- resident voxel models: the field kept on the device, edited in place, re-meshed per block ----
+ * What voxel_model does with brushes (src/voxels.cpp:2139-2245): it keeps one mesh per block, each with its own vertex cache (create_block, :1077-1108), and an
+ * edit re-creates only the blocks it modified. Blocks: with block sizes bx, by >= 1 (in cubes), block (i, j) covers the cubes x in [i*bx, min((i+1)*bx, nx-1)),
+ * y in [j*by, min((j+1)*by, ny-1)) and every z; its number is j*nbx + i with nbx = ceil((nx-1)/bx), nby = ceil((ny-1)/by) (y-major, the (y, x, z) cube order of
+ * create_block). Each block is welded on its own with the owner rule of tw_voxel_mesh_welded restricted to the block's cubes: an edge's owner is the
+ * lowest-index valid cube OF THE BLOCK containing it, vertices are ordered by owner then local edge, indices are local to the block, and triangles whose welded
+ * positions give a zero normal are dropped. A vertex on a block face therefore appears once in every block that uses it, as with per-block caches. One block
+ * covering the grid (bx >= nx-1, by >= ny-1) gives tw_voxel_mesh_welded's mesh bit for bit. Not confirmed: that this partition is create_block's for more
+ * than one block (the reference build pinned here has one block); the caller chooses bx, by to match its own block layout.
+ * Outputs of a model job: the meshes of the listed blocks, one after another in ascending block order, in one vertex and one index buffer. */
+typedef struct tw_voxel_block_mesh {
+	uint32_t block, pad;     /* block number j*nbx + i */
+	uint64_t voff, nverts;   /* the block's vertices: verts[voff .. voff + nverts) */
+	uint64_t toff, ntris;    /* its triangles: indices[toff .. toff + ntris), local to the block (0 = verts[voff]) */
+} tw_voxel_block_mesh;
+typedef struct tw_voxel_blocks_out {
+	float    *verts;         /* vcapacity*3 floats, device or page-locked host memory (NULL with vcapacity 0) */
+	uint64_t  vcapacity;
+	uint32_t *indices;       /* tcapacity*3 indices, device or page-locked host memory (NULL with tcapacity 0) */
+	uint64_t  tcapacity;
+	tw_voxel_block_mesh *blocks; /* HOST, required: room for nbx*nby entries; the listed blocks' ranges, filled by the completing poll */
+	uint32_t *nblocks;       /* HOST, required: blocks listed */
+	uint64_t *nverts, *ntris;/* HOST, required: totals over the listed blocks (may exceed the capacities: nothing is written beyond them) */
+	uint64_t *changed;       /* optional HOST: voxels flipped by remove_unconnected */
+} tw_voxel_blocks_out;
+/* A box of voxels [x, x+w) x [y, y+h) x [z, z+d) */
+typedef struct tw_voxel_box {uint32_t x, y, z, w, h, d;} tw_voxel_box;
+typedef struct tw_voxel_model tw_voxel_model;
+/* A model of the grid *vp with its marching-cubes tables and zix_xy (optional, as tw_voxel_outside; host or device, copied here). It keeps on the device:
+ * the raw field (as the caller gave it or the fill made it), its outside flags, the field and flags after remove_unconnected, and a working copy of those
+ * for the edit's comparison: 15 bytes per voxel (about 2 GB at 512^3), plus the blocks' words. While a job runs, the context's scratch also holds the
+ * flood's frontiers (8 bytes per voxel with remove_unconnected > 0) and the mesh's per-cube words (4 bytes per cube of the listed blocks' worst case).
+ * A model belongs to the context that created it: its jobs are that context's pending job (tw_create_tiles_poll completes them), every model call first
+ * completes the pending job, and tw_destroy(ctx) destroys the context's live models first (their handles are invalid after).
+ * Model jobs commit the model's state at launch, so they cannot be cancelled: tw_cancel returns TW_ERR_STATE, as for tile-set jobs.
+ * TW_ERR_ARG (nothing allocated): NULL arguments, bx or by == 0, an empty grid or 2^32 voxels or more, 3*(bx+1)*(by+1)*nz >= 2^32 with the block sizes
+ * clamped to the grid (the block's indices are 32-bit). */
+TW_API int  tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp, const uint32_t *edge_table256, const int32_t *tri_table256x16,
+                                  const uint32_t *edge_to_vals12x2, const uint32_t *zix_xy, uint32_t bx, uint32_t by, tw_voxel_model **out);
+/* Completes the context's pending job, then frees the model. */
+TW_API void tw_voxel_model_destroy(tw_voxel_model *m);
+/* The build as the context's asynchronous job: the raw field from fill (as tw_voxel_fill(fill, rdata420)) or from vals (n floats, host or device, read
+ * during the job), then tw_voxel_outside, tw_voxel_remove_unconnected, and the mesh of every block, listed in order. The model keeps the results. Rules and
+ * lifetimes as tw_voxel_build_launch. TW_ERR_ARG (nothing enqueued): NULL arguments, both or neither of fill and vals, a fill grid that differs, a capacity
+ * without its buffer, pageable verts / indices; TW_ERR_STATE where tw_voxel_fill returns it. */
+TW_API int  tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_params *fill, const float *rdata420, const float *vals, const tw_voxel_blocks_out *out);
+/* An edit as the context's asynchronous job, without the host reading anything back before the end:
+ *   1. each box's new raw values (values: the boxes' voxels one box after another, each packed in the grid's order - z fastest, then x, then y; host
+ *      memory, copied during the launch) go into the raw field; where boxes overlap, the later box's value wins;
+ *   2. the raw flags are recomputed inside the boxes (they depend only on the voxel's value, its position and zix_xy);
+ *   3. with remove_unconnected > 0, tw_voxel_remove_unconnected runs again on the whole raw field (an edit can disconnect ground far from the box);
+ *   4. every block whose cubes read a voxel whose value or flags after step 3 differ from the model's previous ones is marked (a voxel on a block face marks
+ *      every block that reads it); the model keeps the new field and flags;
+ *   5. the marked blocks - and only those - are meshed, listed in ascending order.
+ * After the completing poll the model's field and flags equal tw_voxel_outside then tw_voxel_remove_unconnected on the edited raw field, and the listed blocks'
+ * meshes equal a fresh build's. nboxes == 0 (boxes and values may then be NULL) changes nothing and lists no block. TW_ERR_ARG (nothing enqueued): NULL
+ * arguments, an empty box or one reaching outside the grid (no clipping), and the output errors of tw_voxel_model_build_launch; TW_ERR_STATE before the
+ * model's first build. */
+TW_API int  tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out);
+/* Synchronous, after completing the pending job: the raw field, the field after remove_unconnected and its flags (each optional; n elements, host or
+ * device). TW_ERR_STATE before the model's first build. */
+TW_API int  tw_voxel_model_read(tw_voxel_model *m, float *raw, float *vals, uint8_t *outside);
+
 /* ---- mesh shadows of tiles (SURVEY.md 8f row N4): calc_mesh_shadows (src/visibility.cpp:411-517) for a batch of tiles with the neighbour chaining of
  * tile_t::calc_shadows_for_light (src/tiled_mesh.cpp:664-692) ---- */
 typedef struct tw_shadow_params {

@@ -55,9 +55,6 @@ int twi_ensure_aux_streams(tw_ctx *ctx) {
 
 namespace {
 
-// slot-2 layout (small device scalars)
-constexpr size_t OFF_MM = 0, OFF_BAD = 64, OFF_TILES = 4096;
-
 int check_ctx(tw_ctx *ctx) { // NOTE: makes ctx->device the calling thread's current CUDA device and leaves it so (documented in tw3d.h: one context per thread);
                              // a shared context takes its parent's current tables
 	if (!ctx) return TW_ERR_ARG;
@@ -429,10 +426,10 @@ int tw_heightgen_2d_launch(tw_ctx *ctx, const tw_grid2d *g, const tw_height_para
 	bool const dev_out = tw_is_device_ptr(out);
 	float *d_out = out;
 	if (!dev_out) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc; d_out = (float *)ctx->d_scratch[0];}
-	rc = tw_reserve(ctx, 2, OFF_TILES); if (rc) return rc;
+	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
 	if (mm) {rc = tw_reserve_pinned(ctx, 2*sizeof(unsigned)); if (rc) return rc;}
 	if (!dev_out) {rc = twi_ensure_aux_streams(ctx); if (rc) return rc;}
-	unsigned *d_mm = mm ? (unsigned *)((char *)ctx->d_scratch[2] + OFF_MM) : nullptr;
+	unsigned *d_mm = mm ? twi_slot2(ctx)->mm : nullptr;
 	twi_job pending; // the tile unpack of one min/max at offset 0
 	pending.kind = twi_job::TILES; pending.n = 1; pending.host_mm = mm; pending.cancellable = true;
 	return twi_launch_job(ctx, pending, [&]() -> int {
@@ -468,18 +465,15 @@ int tw_tile_weights_batch(tw_ctx *ctx, const float *zvals, const int32_t *origin
 	uint32_t const stride = zvsize - 1;
 	size_t const zn = (size_t)ntiles*zvsize*zvsize, tn = (size_t)ntiles*stride*stride;
 	bool const dev_z = tw_is_device_ptr(zvals), dev_w = tw_is_device_ptr(weights), dev_f = has_any_grass && tw_is_device_ptr(has_any_grass), dev_p = tw_is_device_ptr(tile_params);
-	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
-	rc = tw_reserve(ctx, 0, al(tn*sizeof(float)) + (dev_z ? 0 : al(zn*sizeof(float))) + (dev_w ? 0 : al(tn*4)) + al(ntiles) + (dev_p ? 0 : al((size_t)ntiles*8*sizeof(float))) + 256);
-	if (rc) return rc;
-	char *q = (char *)ctx->d_scratch[0];
-	float *d_rand = (float *)q; q += al(tn*sizeof(float));
-	const float *d_z = zvals;
-	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(q, zvals, zn*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const float *)q; q += al(zn*sizeof(float));}
-	uint8_t *d_w = weights;
-	if (!dev_w) {d_w = (uint8_t *)q; q += al(tn*4);}
-	uint8_t *d_f = dev_f ? has_any_grass : (uint8_t *)q; q += al(ntiles);
-	const float *d_p = tile_params;
-	if (!dev_p) {TW_CUDA(ctx, cudaMemcpyAsync(q, tile_params, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_p = (const float *)q;}
+	float *d_rand, *s_z = nullptr, *s_p = nullptr;
+	uint8_t *d_w = weights, *d_f = has_any_grass;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_rand = c.take<float>(tn); if (!dev_z) {s_z = c.take<float>(zn);} if (!dev_w) {d_w = c.take<uint8_t>(tn*4);} if (!dev_f) {d_f = c.take<uint8_t>(ntiles);}
+		if (!dev_p) {s_p = c.take<float>((size_t)ntiles*8);}
+	}); if (rc) return rc;
+	const float *d_z = dev_z ? zvals : s_z, *d_p = dev_p ? tile_params : s_p;
+	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, zn*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	if (!dev_p) {TW_CUDA(ctx, cudaMemcpyAsync(s_p, tile_params, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
 	if (has_any_grass) {TW_CUDA(ctx, cudaMemsetAsync(d_f, 0, ntiles, ctx->stream));}
 	// height_gen.build_arrays((x1 - MESH_X_SIZE/2), (y1 - MESH_Y_SIZE/2), MESH_NOISE_FREQ*DX_VAL, MESH_NOISE_FREQ*DY_VAL, tsize, tsize, 0, 1) (src/tiled_mesh.cpp:1103)
 	float const MESH_NOISE_FREQ = 80.0f;
@@ -513,10 +507,9 @@ int tw_heightgen_tiles(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, 
 	bool const dev_out = tw_is_device_ptr(out);
 	float *d_out = out;
 	if (!dev_out) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc; d_out = (float *)ctx->d_scratch[0];}
-	size_t const mm_bytes = (size_t)ntiles*2*sizeof(unsigned), org_bytes = (size_t)ntiles*sizeof(float2);
-	rc = tw_reserve(ctx, 2, OFF_TILES + mm_bytes + org_bytes); if (rc) return rc;
-	unsigned *d_mm = mm ? (unsigned *)((char *)ctx->d_scratch[2] + OFF_TILES) : nullptr;
-	float2 *d_org = (float2 *)((char *)ctx->d_scratch[2] + OFF_TILES + mm_bytes);
+	unsigned *d_mm = nullptr; float2 *d_org;
+	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {c.take<twi_slot2_words>(1); if (mm) {d_mm = c.take<unsigned>((size_t)ntiles*2);} d_org = c.take<float2>(ntiles);});
+	if (rc) return rc;
 	if (d_mm) {rc = twi_init_minmax(ctx, d_mm, ntiles); if (rc) return rc;}
 	// setup_height_gen_async: build_arrays((x0 - MESH_X_SIZE/2), (y0 - MESH_Y_SIZE/2), dx, dy, ...): int -> float, then mx0 = dx*x0 (src/tiled_mesh.cpp:461, src/mesh_gen.cpp:591)
 	if (p->gen_mode != TW_MGEN_SINE) {
@@ -525,7 +518,7 @@ int tw_heightgen_tiles(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, 
 			float const x0 = (float)(origins_xy[2*t] - mesh_x_size/2), y0 = (float)(origins_xy[2*t+1] - mesh_y_size/2);
 			org[t] = make_float2(dx*x0, dy*y0);
 		}
-		TW_CUDA(ctx, cudaMemcpyAsync(d_org, org.data(), org_bytes, cudaMemcpyHostToDevice, ctx->stream));
+		TW_CUDA(ctx, cudaMemcpyAsync(d_org, org.data(), (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
 		TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // org is a local vector
 		uint32_t const zmax = 65535;
 		for (uint32_t t0 = 0; t0 < ntiles; t0 += zmax) { // gridDim.z limit
@@ -557,15 +550,14 @@ int tw_tile_bounds_batch(tw_ctx *ctx, const float *zvals, uint32_t ntiles, uint3
 	if (4*(zvsize/4) >= zvsize) return tw_set_error(ctx, TW_ERR_ARG, "zvsize %u: the last sub-block would end at cell %u (the reference asserts x_end < zvsize, src/tiled_mesh.cpp:520)", zvsize, 4*(zvsize/4));
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
 	size_t const n = (size_t)ntiles*zvsize*zvsize;
-	size_t const sub_bytes = (size_t)ntiles*16*sizeof(Sub);
-	const float *d_z = zvals;
 	bool const dev = tw_is_device_ptr(zvals);
-	rc = tw_reserve(ctx, 0, (dev ? 0 : n*sizeof(float)) + sub_bytes + 256); if (rc) return rc;
-	char *s0 = (char *)ctx->d_scratch[0];
-	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(s0, zvals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const float *)s0; s0 += (n*sizeof(float) + 255) & ~(size_t)255;}
-	rc = twi_tile_bounds(ctx, ctx->stream, d_z, ntiles, zvsize, wpz_max, s0); if (rc) return rc;
+	float *s_z = nullptr; Sub *d_sub;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {s_z = c.take<float>(n);} d_sub = c.take<Sub>((size_t)ntiles*16);}); if (rc) return rc;
+	const float *d_z = dev ? zvals : s_z;
+	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	rc = twi_tile_bounds(ctx, ctx->stream, d_z, ntiles, zvsize, wpz_max, d_sub); if (rc) return rc;
 	std::vector<Sub> sub((size_t)ntiles*16);
-	TW_CUDA(ctx, cudaMemcpyAsync(sub.data(), s0, sub_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+	TW_CUDA(ctx, cudaMemcpyAsync(sub.data(), d_sub, sub.size()*sizeof(Sub), cudaMemcpyDeviceToHost, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	combine_bounds(sub.data(), ntiles, dx_val, dy_val, size, out);
 	return TW_OK;
@@ -584,8 +576,8 @@ int tw_glaciate_mesh(tw_ctx *ctx, float *mesh, int nx, int ny, int xoff2, int yo
 		d_mesh = (float *)ctx->d_scratch[0];
 		TW_CUDA(ctx, cudaMemcpyAsync(d_mesh, mesh, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 	}
-	rc = tw_reserve(ctx, 2, OFF_TILES); if (rc) return rc;
-	unsigned *d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_MM);
+	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
+	unsigned *d_mm = twi_slot2(ctx)->mm;
 	rc = twi_init_minmax(ctx, d_mm, 1); if (rc) return rc;
 	rc = twi_glaciate_mesh(ctx, d_mesh, nx, ny, xoff2, yoff2, mesh_x_size, mesh_y_size, p, d_mm); if (rc) return rc;
 	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(mesh, d_mesh, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
@@ -613,8 +605,7 @@ int tw_erode_tiles(tw_ctx *ctx, float *maps, uint32_t ntiles, int xsize, int ysi
 	}
 	float *d_minz = nullptr;
 	if (min_zvals) {
-		rc = tw_reserve(ctx, 2, OFF_TILES + (size_t)ntiles*sizeof(float)); if (rc) return rc;
-		d_minz = (float *)((char *)ctx->d_scratch[2] + OFF_TILES);
+		rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {c.take<twi_slot2_words>(1); d_minz = c.take<float>(ntiles);}); if (rc) return rc;
 		TW_CUDA(ctx, cudaMemcpyAsync(d_minz, min_zvals, (size_t)ntiles*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 		TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	}
@@ -684,7 +675,6 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	bool const dev_out = o->zvals && tw_is_device_ptr(o->zvals), host_out = o->zvals && !dev_out, dev_nrm = want_normals && tw_is_device_ptr(o->normals_rgba);
 	bool const dev_ao = want_ao && tw_is_device_ptr(sh->ao), dev_w = want_w && tw_is_device_ptr(sh->weights), dev_f = want_f && tw_is_device_ptr(sh->has_any_grass);
 	bool const dev_tp = want_w && tw_is_device_ptr(sh->tile_params);
-	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
 	if (tail) {rc = tail->prepare(ctx); if (rc) return rc;}
 	rc = twi_ensure_aux_streams(ctx); if (rc) return rc;
 	// The pipeline. Work per tile is heavy-tailed (ocean tiles: 1000 droplets x 1 move; mountain tiles: 1e5 moves in one serial chain), and a chain
@@ -707,21 +697,30 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		if (want_w) {jorg[t] = make_float2(gj.dx*x0, gj.dy*y0);}
 	}
 	twi_sine_batch sb_ctx, sb_jit; // sine tables of the sine-mode contexts and of the jitter grids: one plan (distinct columns / rows) each
-	size_t const ctab_bytes = (want_ao && sine) ? al(twi_sine_tiles_plan(&gc, corg.data(), ntiles, &sb_ctx)) : 0, jtab_bytes = want_w ? al(twi_sine_tiles_plan(&gj, jorg.data(), ntiles, &sb_jit)) : 0;
-	// slot 0: device staging of the host-bound arrays [zvals | normal maps | AO maps | weights | has_any_grass], then [tile_params | sine tables | context /
-	// jitter grid buffers]. All but the buffers is reserved before the erosion budget is taken, so the budget sees that memory as used.
-	size_t const z_bytes = dev_out ? 0 : al(n*sizeof(float)), nrm_bytes = (want_normals && !dev_nrm) ? al(ntiles*nrm_elems*4) : 0;
-	size_t const ao_bytes = (want_ao && !dev_ao) ? al(ntiles*nrm_elems) : 0, w_bytes = (want_w && !dev_w) ? al(ntiles*nrm_elems*4) : 0, f_bytes = (want_f && !dev_f) ? al(ntiles) : 0;
-	size_t const tp_bytes = (want_w && !dev_tp) ? al((size_t)ntiles*8*sizeof(float)) : 0;
-	// mesh shadows, reused light after light: [mask staging (host smask) | 64-bit keys | x edges | y edges (outputs, then caller rows) | plan of every light]
-	size_t const edge = (size_t)ntiles*zvsize, plan_bytes = al(twi_shadow_plan_ints(ntiles)*sizeof(int));
+	size_t const ctab_bytes = (want_ao && sine) ? twi_sine_tiles_plan(&gc, corg.data(), ntiles, &sb_ctx) : 0, jtab_bytes = want_w ? twi_sine_tiles_plan(&gj, jorg.data(), ntiles, &sb_jit) : 0;
+	// slot 0: device staging of the host-bound arrays [zvals | normal maps | AO maps | weights | has_any_grass], then [tile_params | sine tables | mesh shadows |
+	// tail], then the ring of context / jitter grid buffers. All but the ring is reserved before the erosion budget is taken, so the budget sees that memory as
+	// used. Mesh shadows, reused light after light: [mask staging (host smask) | 64-bit keys | x edges | y edges (outputs, then caller rows) | plan of every light].
+	size_t const edge = (size_t)ntiles*zvsize;
 	bool sh_host_m = false, sh_in_x = false, sh_in_y = false;
 	for (uint32_t l = 0; l < nl; ++l) {sh_host_m |= !sdev_m[l]; sh_in_x |= (lights[l].sh_in_x != nullptr); sh_in_y |= (lights[l].sh_in_y != nullptr);}
-	size_t const shm_bytes = sh_host_m ? al(n + 4) : 0, shk_bytes = nl ? al(2*edge*sizeof(unsigned long long)) : 0;
-	size_t const shx_bytes = nl ? al((sh_in_x ? 2 : 1)*edge*sizeof(float)) : 0, shy_bytes = nl ? al((sh_in_y ? 2 : 1)*edge*sizeof(float)) : 0;
-	size_t const sh_bytes = shm_bytes + shk_bytes + shx_bytes + shy_bytes + nl*plan_bytes, tail_bytes = tail ? al(tail->dev_bytes) : 0;
-	size_t const fixed_bytes = z_bytes + nrm_bytes + ao_bytes + w_bytes + f_bytes + tp_bytes + ctab_bytes + jtab_bytes + sh_bytes + tail_bytes;
-	if (fixed_bytes) {rc = tw_reserve(ctx, 0, fixed_bytes); if (rc) return rc;}
+	float *d_out = dev_out ? o->zvals : nullptr, *d_shx = nullptr, *d_shy = nullptr;
+	unsigned char *d_rgba = dev_nrm ? o->normals_rgba : nullptr, *d_shm = nullptr, *d_ao = dev_ao ? sh->ao : nullptr, *d_w = dev_w ? sh->weights : nullptr;
+	uint8_t *d_f = dev_f ? sh->has_any_grass : nullptr;
+	const float *d_tp = dev_tp ? sh->tile_params : nullptr;
+	char *d_ctab = nullptr, *d_jtab = nullptr, *d_tail = nullptr;
+	unsigned long long *d_shk = nullptr;
+	std::vector<int *> d_shp(nl);
+	auto slot0 = [&](twi_carve &c) {
+		if (!dev_out) {d_out = c.take<float>(n);} if (want_normals && !dev_nrm) {d_rgba = c.take<unsigned char>(ntiles*nrm_elems*4);}
+		if (want_ao && !dev_ao) {d_ao = c.take<uint8_t>(ntiles*nrm_elems);} if (want_w && !dev_w) {d_w = c.take<uint8_t>(ntiles*nrm_elems*4);}
+		if (want_f && !dev_f) {d_f = c.take<uint8_t>(ntiles);} if (want_w && !dev_tp) {d_tp = c.take<float>((size_t)ntiles*8);}
+		if (want_ao && sine) {d_ctab = c.take<char>(ctab_bytes);} if (want_w) {d_jtab = c.take<char>(jtab_bytes);} if (sh_host_m) {d_shm = c.take<unsigned char>(n + 4);}
+		if (nl) {d_shk = c.take<unsigned long long>(2*edge); d_shx = c.take<float>((sh_in_x ? 2 : 1)*edge); d_shy = c.take<float>((sh_in_y ? 2 : 1)*edge);}
+		for (uint32_t l = 0; l < nl; ++l) {d_shp[l] = c.take<int>(twi_shadow_plan_ints(ntiles));} if (tail) {d_tail = c.take<char>(tail->dev_bytes);}
+	};
+	twi_carve fixed; slot0(fixed);
+	rc = tw_reserve(ctx, 0, fixed.bytes); if (rc) return rc;
 	// AO context grids and weights jitter grids are per chunk (schedule order): written on the main stream, read on the chunk's erosion stream. The buffers
 	// hold about 2 GB of context grids (or jitter grids without AO) in all, the bound tw_tile_ao_batch keeps; a chunk holds at most a third of that. When
 	// the batch needs more chunks than buffers, chunk 0 (every long droplet chain) keeps its buffer and the later chunks take turns in the others: before the
@@ -730,7 +729,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	size_t const bound_tile = want_ao ? ctx_elems*sizeof(float) : nrm_elems*sizeof(float);
 	size_t const ring_max = ring_tile ? std::min((RING/bound_tile)*ring_tile, (size_t)ntiles*ring_tile) + 2*65536 : 0; // what the buffers can take, for the erosion budget
 	uint32_t nchunks = 0, chunk = 0;
-	size_t sbytes = 0;
+	size_t sbytes = 0; // one erosion lane's scratch (a multiple of 256 bytes): lane l's is at l*sbytes in slot 1
 	if (erode) {
 		size_t free_b = 0, total_b = 0;
 		TW_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
@@ -757,96 +756,90 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	bool const reorder = (erode && nchunks > 1 && !sine && !getenv("TW_PIPE_NO_REORDER"));
 	int const nes = (nchunks > 2) ? 3 : (int)nchunks; // aux streams / erosion scratch buffers
 	uint32_t const nbuf = ring_tile ? (uint32_t)std::min<size_t>(nchunks, std::max<size_t>(3, RING/((size_t)chunk*bound_tile))) : 0;
-	size_t const cz_bytes = want_ao ? al((size_t)chunk*ctx_elems*sizeof(float)) : 0, rand_bytes = want_w ? al((size_t)chunk*nrm_elems*sizeof(float)) : 0;
-	size_t const ring_bytes = nbuf*(cz_bytes + rand_bytes);
-	if (ring_bytes) {rc = tw_reserve(ctx, 0, fixed_bytes + ring_bytes); if (rc) return rc;}
-	char *s0 = (char *)ctx->d_scratch[0];
-	float *d_out = dev_out ? o->zvals : (float *)s0; s0 += z_bytes;
-	unsigned char *d_rgba = !want_normals ? nullptr : (dev_nrm ? o->normals_rgba : (unsigned char *)s0); s0 += nrm_bytes;
-	uint8_t *d_ao = !want_ao ? nullptr : (dev_ao ? sh->ao : (uint8_t *)s0); s0 += ao_bytes;
-	uint8_t *d_w = !want_w ? nullptr : (dev_w ? sh->weights : (uint8_t *)s0); s0 += w_bytes;
-	uint8_t *d_f = !want_f ? nullptr : (dev_f ? sh->has_any_grass : (uint8_t *)s0); s0 += f_bytes;
-	const float *d_tp = !want_w ? nullptr : (dev_tp ? sh->tile_params : (const float *)s0); s0 += tp_bytes;
-	char *d_ctab = s0; s0 += ctab_bytes;
-	char *d_jtab = s0; s0 += jtab_bytes;
-	unsigned char *d_shm = (unsigned char *)s0; s0 += shm_bytes;
-	unsigned long long *d_shk = (unsigned long long *)s0; s0 += shk_bytes;
-	float *d_shx = (float *)s0; s0 += shx_bytes;
-	float *d_shy = (float *)s0; s0 += shy_bytes;
-	char *d_shp = s0; s0 += nl*plan_bytes;
-	char *d_tail = s0; s0 += tail_bytes;
-	char *d_ring = s0;
+	std::vector<float *> ring_cz(nbuf), ring_rand(nbuf);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		slot0(c);
+		for (uint32_t b = 0; b < nbuf; ++b) {ring_cz[b] = want_ao ? c.take<float>((size_t)chunk*ctx_elems) : nullptr; ring_rand[b] = want_w ? c.take<float>((size_t)chunk*nrm_elems) : nullptr;}
+	}); if (rc) return rc;
 	if (erode) {
-		sbytes = al(twi_erode_scratch_bytes(ctx, chunk, (int)zvsize, (int)zvsize));
+		sbytes = twi_erode_scratch_bytes(ctx, chunk, (int)zvsize, (int)zvsize);
 		rc = tw_reserve(ctx, 1, sbytes*nes); if (rc) return rc; // before the sine tables claim the same slot: it is never re-allocated under the erosion
 	}
-	// slot 2: [small scalars | per-tile min/max | origins | sorted origins | work | order | hist(256) | coarse samples | sub-block bounds | min_normal_z |
+	// slot 2: [fixed words | per-tile min/max | origins | sorted origins | work | order | hist(256) | coarse samples | sub-block bounds | min_normal_z |
 	// context origins | sorted context origins]
 	bool const ctx_org = want_ao && !sine; // the paired noise kernels read the context origins from the device
 	uint32_t const CS = 8, cstep = (zvsize >= CS) ? zvsize/CS : 1;
-	size_t const mm_bytes = al((size_t)ntiles*2*sizeof(unsigned)), org_bytes = al((size_t)ntiles*sizeof(float2));
-	size_t const u_bytes = al((size_t)ntiles*sizeof(unsigned)), coarse_bytes = reorder ? al((size_t)ntiles*CS*CS*sizeof(float)) : 0;
-	size_t const sub_bytes = want_bounds ? al((size_t)ntiles*16*sizeof(Sub)) : 0, mnz_bytes = want_mnz ? u_bytes : 0, corg_bytes = ctx_org ? org_bytes : 0;
-	rc = tw_reserve(ctx, 2, OFF_TILES + mm_bytes + 2*org_bytes + 2*u_bytes + 1024 + coarse_bytes + sub_bytes + mnz_bytes + 2*corg_bytes); if (rc) return rc;
-	char *s2 = (char *)ctx->d_scratch[2] + OFF_TILES;
-	unsigned *d_mm = (unsigned *)s2; s2 += mm_bytes;
-	float2 *d_org = (float2 *)s2; s2 += org_bytes;
-	float2 *d_org_sorted = (float2 *)s2; s2 += org_bytes;
-	unsigned *d_work = (unsigned *)s2; s2 += u_bytes;
-	unsigned *d_order = (unsigned *)s2; s2 += u_bytes;
-	unsigned *d_hist = (unsigned *)s2; s2 += 1024;
-	float *d_coarse = (float *)s2; s2 += coarse_bytes;
-	Sub *d_sub = (Sub *)s2; s2 += sub_bytes;
-	unsigned *d_mnz = want_mnz ? (unsigned *)s2 : nullptr; s2 += mnz_bytes;
-	float2 *d_corg = (float2 *)s2; s2 += corg_bytes;
-	float2 *d_corg_sorted = (float2 *)s2;
-	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
+	twi_slot2_words *words;
+	unsigned *d_mm, *d_work, *d_order, *d_hist, *d_mnz = nullptr;
+	float2 *d_org, *d_org_sorted, *d_corg = nullptr, *d_corg_sorted = nullptr;
+	float *d_coarse = nullptr;
+	Sub *d_sub = nullptr;
+	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {
+		words = c.take<twi_slot2_words>(1); d_mm = c.take<unsigned>((size_t)ntiles*2); d_org = c.take<float2>(ntiles); d_org_sorted = c.take<float2>(ntiles);
+		d_work = c.take<unsigned>(ntiles); d_order = c.take<unsigned>(ntiles); d_hist = c.take<unsigned>(256);
+		if (reorder) {d_coarse = c.take<float>((size_t)ntiles*CS*CS);} if (want_bounds) {d_sub = c.take<Sub>((size_t)ntiles*16);}
+		if (want_mnz) {d_mnz = c.take<unsigned>(ntiles);} if (ctx_org) {d_corg = c.take<float2>(ntiles); d_corg_sorted = c.take<float2>(ntiles);}
+	}); if (rc) return rc;
+	unsigned long long *d_steps = &words->steps;
 	// pinned staging: inputs [origins | sine-mode index tables | context origins or their sine tables | jitter sine tables | tile_params | per light: shadow plan,
 	// host sh_in_x, host sh_in_y], then the small results [steps | min/max | sub-block bounds | min_normal_z | has_any_grass] that the completing poll unpacks.
 	// Every sine batch has its own region, and the caller's origins, tile_params, tile_xy and host sh_in rows may be reused as soon as this function returns.
-	size_t const in_org = al((size_t)ntiles*sizeof(float2)), in_sine = sine ? al(twi_sine_tiles_stage_bytes(ntiles)) : 0;
-	size_t const in_ctx = !want_ao ? 0 : (sine ? al(twi_sine_tiles_stage_bytes(ntiles)) : in_org), in_jit = want_w ? al(twi_sine_tiles_stage_bytes(ntiles)) : 0;
-	size_t const in_tp = tp_bytes, off_ctx = in_org + in_sine, off_jit = off_ctx + in_ctx, off_tp = off_jit + in_jit, off_sh = off_tp + in_tp;
-	std::vector<size_t> off_six(nl), off_siy(nl);
-	size_t in_sh = nl*plan_bytes;
-	for (uint32_t l = 0; l < nl; ++l) {
-		off_six[l] = off_sh + in_sh; in_sh += (lights[l].sh_in_x && !sdev_ix[l]) ? al(edge*sizeof(float)) : 0;
-		off_siy[l] = off_sh + in_sh; in_sh += (lights[l].sh_in_y && !sdev_iy[l]) ? al(edge*sizeof(float)) : 0;
-	}
-	size_t const off_steps = off_sh + in_sh, off_mm = off_steps + 256, off_sub = off_mm + (want_mm ? mm_bytes : 0), off_mnz = off_sub + sub_bytes, off_f = off_mnz + mnz_bytes;
-	size_t const off_tail = off_f + (want_f ? al(ntiles) : 0);
-	rc = tw_reserve_pinned(ctx, off_tail + (tail ? tail->pin_bytes : 0)); if (rc) return rc;
-	char *h_stage = (char *)ctx->h_pinned;
-	float2 *h_org = (float2 *)h_stage;
-	if (hs) {memcpy(h_stage, origins_xy, (size_t)ntiles*2*sizeof(int32_t));} // the sampler reads the int (x1, y1) origins (d_org then holds int2)
+	float2 *h_org;
+	char *h_sine = nullptr, *h_ctx = nullptr, *h_jit = nullptr, *h_tail = nullptr;
+	float *h_tp = nullptr;
+	std::vector<int *> h_shp(nl);
+	std::vector<float *> h_six(nl), h_siy(nl);
+	unsigned long long *h_steps;
+	unsigned *h_mm = nullptr, *h_mnz = nullptr;
+	Sub *h_sub = nullptr;
+	uint8_t *h_f = nullptr;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
+		h_org = c.take<float2>(ntiles);
+		if (sine) {h_sine = c.take<char>(twi_sine_tiles_stage_bytes(ntiles));}
+		if (want_ao) {h_ctx = c.take<char>(sine ? twi_sine_tiles_stage_bytes(ntiles) : ntiles*sizeof(float2));}
+		if (want_w) {h_jit = c.take<char>(twi_sine_tiles_stage_bytes(ntiles));}
+		if (want_w && !dev_tp) {h_tp = c.take<float>((size_t)ntiles*8);}
+		for (uint32_t l = 0; l < nl; ++l) {h_shp[l] = c.take<int>(twi_shadow_plan_ints(ntiles));}
+		for (uint32_t l = 0; l < nl; ++l) {
+			h_six[l] = (lights[l].sh_in_x && !sdev_ix[l]) ? c.take<float>(edge) : nullptr; h_siy[l] = (lights[l].sh_in_y && !sdev_iy[l]) ? c.take<float>(edge) : nullptr;
+		}
+		h_steps = c.take<unsigned long long>(1);
+		if (want_mm) {h_mm = c.take<unsigned>((size_t)ntiles*2);}
+		if (want_bounds) {h_sub = c.take<Sub>((size_t)ntiles*16);}
+		if (want_mnz) {h_mnz = c.take<unsigned>(ntiles);}
+		if (want_f) {h_f = c.take<uint8_t>(ntiles);}
+		if (tail) {h_tail = c.take<char>(tail->pin_bytes);}
+	}); if (rc) return rc;
+	if (hs) {memcpy(h_org, origins_xy, (size_t)ntiles*2*sizeof(int32_t));} // the sampler reads the int (x1, y1) origins (d_org then holds int2)
 	else {
 		for (uint32_t t = 0; t < ntiles; ++t) { // build_arrays((x1 - MESH_X_SIZE/2), (y1 - MESH_Y_SIZE/2), ...): int -> float, mx0 = dx*x0 (src/tiled_mesh.cpp:461, src/mesh_gen.cpp:591)
 			float const x0 = (float)(origins_xy[2*t] - mesh_x_size/2), y0 = (float)(origins_xy[2*t+1] - mesh_y_size/2);
 			h_org[t] = make_float2(dx*x0, dy*y0);
 		}
 	}
+	auto off = [&](const void *h) {return h ? (size_t)((const char *)h - (const char *)ctx->h_pinned) : 0;};
 	twi_job pending;
 	pending.kind = twi_job::TILES; pending.n = ntiles; pending.host_steps = erode ? &ctx->last_erosion_steps : nullptr;
 	pending.cancellable = (tail == nullptr); // a tail commits a tile set's state
 	pending.reads_image = (hs != nullptr);
 	pending.host_mm = o->mm; pending.host_bounds = o->bounds; pending.host_min_nz = o->min_normal_z; pending.host_flags = (want_f && !dev_f) ? sh->has_any_grass : nullptr;
 	pending.dx = dx; pending.dy = dy; pending.size = size;
-	pending.off_steps = off_steps; pending.off_mm = off_mm; pending.off_sub = off_sub; pending.off_min_nz = off_mnz; pending.off_flags = off_f;
+	pending.off_steps = off(h_steps); pending.off_mm = off(h_mm); pending.off_sub = off(h_sub); pending.off_min_nz = off(h_mnz); pending.off_flags = off(h_f);
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		if (!sine) {TW_CUDA(ctx, cudaMemcpyAsync(d_org, h_org, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));}
 		if (ctx_org) {
-			memcpy(h_stage + off_ctx, corg.data(), (size_t)ntiles*sizeof(float2));
-			TW_CUDA(ctx, cudaMemcpyAsync(d_corg, h_stage + off_ctx, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+			memcpy(h_ctx, corg.data(), (size_t)ntiles*sizeof(float2));
+			TW_CUDA(ctx, cudaMemcpyAsync(d_corg, h_ctx, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
 		}
-		if (tp_bytes) {
-			memcpy(h_stage + off_tp, sh->tile_params, (size_t)ntiles*8*sizeof(float));
-			TW_CUDA(ctx, cudaMemcpyAsync((void *)d_tp, h_stage + off_tp, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+		if (h_tp) {
+			memcpy(h_tp, sh->tile_params, (size_t)ntiles*8*sizeof(float));
+			TW_CUDA(ctx, cudaMemcpyAsync((void *)d_tp, h_tp, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 		}
 		for (uint32_t l = 0; l < nl; ++l) { // the plans go up now; host sh_in rows wait in the staging until their light's pass copies them into the edge buffers
-			twi_shadow_plan_pack(splan[l], (int *)(h_stage + off_sh + l*plan_bytes));
-			TW_CUDA(ctx, cudaMemcpyAsync(d_shp + l*plan_bytes, h_stage + off_sh + l*plan_bytes, twi_shadow_plan_ints(ntiles)*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-			if (lights[l].sh_in_x && !sdev_ix[l]) {memcpy(h_stage + off_six[l], lights[l].sh_in_x, edge*sizeof(float));}
-			if (lights[l].sh_in_y && !sdev_iy[l]) {memcpy(h_stage + off_siy[l], lights[l].sh_in_y, edge*sizeof(float));}
+			twi_shadow_plan_pack(splan[l], h_shp[l]);
+			TW_CUDA(ctx, cudaMemcpyAsync(d_shp[l], h_shp[l], twi_shadow_plan_ints(ntiles)*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+			if (h_six[l]) {memcpy(h_six[l], lights[l].sh_in_x, edge*sizeof(float));}
+			if (h_siy[l]) {memcpy(h_siy[l], lights[l].sh_in_y, edge*sizeof(float));}
 		}
 		if (want_f) {TW_CUDA(ctx, cudaMemsetAsync(d_f, 0, ntiles, ctx->stream));}
 		if (erode) {TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, sizeof(unsigned long long), ctx->stream));} // the aux streams see it through the chunk events
@@ -869,12 +862,12 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 			if (ctx_org) {rc = twi_gather_origins(ctx, d_corg, d_order, ntiles, d_corg_sorted); if (rc) return rc; d_gen_corg = d_corg_sorted;}
 			d_gen_org = d_org_sorted; d_perm = d_order;
 		}
-		if (sine) {rc = twi_heightgen_sine_tiles(ctx, &g, p, 1, 0, h_org, ntiles, d_out, nullptr, h_stage + in_org); if (rc) return rc;}
-		if (want_ao && sine) {rc = twi_sine_tiles_setup(ctx, &gc, p, 1, 0, corg.data(), ntiles, d_ctab, h_stage + off_ctx, &sb_ctx); if (rc) return rc;}
+		if (sine) {rc = twi_heightgen_sine_tiles(ctx, &g, p, 1, 0, h_org, ntiles, d_out, nullptr, h_sine); if (rc) return rc;}
+		if (want_ao && sine) {rc = twi_sine_tiles_setup(ctx, &gc, p, 1, 0, corg.data(), ntiles, d_ctab, h_ctx, &sb_ctx); if (rc) return rc;}
 		if (want_w) { // force_sine_mode: gen_mode = MGEN_SINE, gen_shape = 0 (src/mesh_gen.cpp:592-593); no glaciate, start index >= 50 (src/tiled_mesh.cpp:1103)
 			tw_height_params ps = *p;
 			ps.gen_mode = TW_MGEN_SINE; ps.gen_shape = 0;
-			rc = twi_sine_tiles_setup(ctx, &gj, &ps, 0, 50, jorg.data(), ntiles, d_jtab, h_stage + off_jit, &sb_jit); if (rc) return rc;
+			rc = twi_sine_tiles_setup(ctx, &gj, &ps, 0, 50, jorg.data(), ntiles, d_jtab, h_jit, &sb_jit); if (rc) return rc;
 		}
 		auto chain = [](cudaStream_t from, cudaStream_t to) -> bool { // `to` waits for what `from` has enqueued so far
 			cudaEvent_t ev = nullptr;
@@ -892,7 +885,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 			size_t const r0 = d_perm ? 0 : t0; // first result slot the chunk's kernels address directly
 			const unsigned *perm_k = d_perm ? d_perm + t0 : nullptr;
 			uint32_t const b = (k < nbuf) ? k : 1 + (k - 1) % (nbuf - 1); // buffer 0 stays chunk 0's
-			float *d_cz = (float *)(d_ring + b*(cz_bytes + rand_bytes)), *d_rand = (float *)(d_ring + b*(cz_bytes + rand_bytes) + cz_bytes);
+			float *d_cz = nbuf ? ring_cz[b] : nullptr, *d_rand = nbuf ? ring_rand[b] : nullptr;
 			bool const reuse = (nbuf && ring_ev[b]); // the main stream waits right before its first write into the buffer
 			if (ctx_mode && reuse && cudaStreamWaitEvent(ctx->stream, ring_ev[b], 0) != cudaSuccess) {status = tw_set_error(ctx, TW_ERR_CUDA, "ring event"); break;}
 			if (ctx_mode) { // contexts in schedule order, zvals cut from their interiors into the caller-visible slots
@@ -953,24 +946,24 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		for (uint32_t l = 0; l < nl; ++l) {
 			tw_tile_light const &L = lights[l];
 			unsigned char *d_m = sdev_m[l] ? L.smask : d_shm;
-			if (L.sh_in_x) {TW_CUDA(ctx, cudaMemcpyAsync(d_shx + edge, sdev_ix[l] ? (const void *)L.sh_in_x : h_stage + off_six[l], edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
-			if (L.sh_in_y) {TW_CUDA(ctx, cudaMemcpyAsync(d_shy + edge, sdev_iy[l] ? (const void *)L.sh_in_y : h_stage + off_siy[l], edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
-			rc = twi_shadow_enqueue(ctx, ctx->stream, splan[l], d_out, ntiles, zvsize, d_m, d_shk, d_shx, d_shy, (const int *)(d_shp + l*plan_bytes), true); if (rc) return rc;
+			if (L.sh_in_x) {TW_CUDA(ctx, cudaMemcpyAsync(d_shx + edge, sdev_ix[l] ? (const void *)L.sh_in_x : h_six[l], edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+			if (L.sh_in_y) {TW_CUDA(ctx, cudaMemcpyAsync(d_shy + edge, sdev_iy[l] ? (const void *)L.sh_in_y : h_siy[l], edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
+			rc = twi_shadow_enqueue(ctx, ctx->stream, splan[l], d_out, ntiles, zvsize, d_m, d_shk, d_shx, d_shy, d_shp[l], true); if (rc) return rc;
 			if (!sdev_m[l]) {TW_CUDA(ctx, cudaMemcpyAsync(L.smask, d_m, n, cudaMemcpyDeviceToHost, ctx->stream));}
 			if (L.sh_out_x) {TW_CUDA(ctx, cudaMemcpyAsync(L.sh_out_x, d_shx, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 			if (L.sh_out_y) {TW_CUDA(ctx, cudaMemcpyAsync(L.sh_out_y, d_shy, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 		}
-		if (tail) {rc = tail->enqueue(ctx, d_out, d_tail, h_stage + off_tail); if (rc) return rc;} // the tail's work reads the final zvals
+		if (tail) {rc = tail->enqueue(ctx, d_out, d_tail, h_tail); if (rc) return rc;} // the tail's work reads the final zvals
 		// every host-bound result is copied once, at the end: the schedule order scatters a chunk over the whole batch
 		if (host_out && d_perm) {TW_CUDA(ctx, cudaMemcpyAsync(o->zvals, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 		if (want_normals && !dev_nrm) {TW_CUDA(ctx, cudaMemcpyAsync(o->normals_rgba, d_rgba, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
 		if (want_ao && !dev_ao) {TW_CUDA(ctx, cudaMemcpyAsync(sh->ao, d_ao, (size_t)ntiles*nrm_elems, cudaMemcpyDeviceToHost, ctx->stream));}
 		if (want_w && !dev_w) {TW_CUDA(ctx, cudaMemcpyAsync(sh->weights, d_w, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
-		if (erode) {TW_CUDA(ctx, cudaMemcpyAsync(h_stage + off_steps, d_steps, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_mm) {TW_CUDA(ctx, cudaMemcpyAsync(h_stage + off_mm, d_mm, (size_t)ntiles*2*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_bounds) {TW_CUDA(ctx, cudaMemcpyAsync(h_stage + off_sub, d_sub, (size_t)ntiles*16*sizeof(Sub), cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_mnz) {TW_CUDA(ctx, cudaMemcpyAsync(h_stage + off_mnz, d_mnz, (size_t)ntiles*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_f && !dev_f) {TW_CUDA(ctx, cudaMemcpyAsync(h_stage + off_f, d_f, ntiles, cudaMemcpyDeviceToHost, ctx->stream));}
+		if (erode) {TW_CUDA(ctx, cudaMemcpyAsync(h_steps, d_steps, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));}
+		if (want_mm) {TW_CUDA(ctx, cudaMemcpyAsync(h_mm, d_mm, (size_t)ntiles*2*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
+		if (want_bounds) {TW_CUDA(ctx, cudaMemcpyAsync(h_sub, d_sub, (size_t)ntiles*16*sizeof(Sub), cudaMemcpyDeviceToHost, ctx->stream));}
+		if (want_mnz) {TW_CUDA(ctx, cudaMemcpyAsync(h_mnz, d_mnz, (size_t)ntiles*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
+		if (want_f && !dev_f) {TW_CUDA(ctx, cudaMemcpyAsync(h_f, d_f, ntiles, cudaMemcpyDeviceToHost, ctx->stream));}
 		return TW_OK;
 	});
 }
@@ -1021,7 +1014,9 @@ int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, con
 	}
 	if (tw_is_device_ptr(src16)) return tw_set_error(ctx, TW_ERR_ARG, "src16 must be host memory");
 	if (nrows > 0xffffffffu) return tw_set_error(ctx, TW_ERR_ARG, "too many rows in one edit");
-	size_t const rows_bytes = (nrows*sizeof(twi_hmap_row) + 255) & ~(size_t)255, need = rows_bytes + 2*texels;
+	twi_carve rows_region;
+	rows_region.take<twi_hmap_row>(nrows);
+	size_t const rows_bytes = rows_region.bytes, need = rows_bytes + 2*texels;
 	if (!ctx->img_stream) {
 		TW_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->img_stream, cudaStreamNonBlocking));
 		TW_CUDA(ctx, cudaEventCreateWithFlags(&ctx->img_ev, cudaEventDisableTiming));
@@ -1139,16 +1134,15 @@ int tw_heightmap_sample_tiles(tw_ctx *ctx, const uint8_t *data16, const tw_hmap_
 	if (!data16 || !hs || !origins_xy || !out || ntiles == 0 || zvsize == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	if (hs->width <= 0 || hs->height <= 0 || hs->edge_mode < 0 || hs->edge_mode > 2) return tw_set_error(ctx, TW_ERR_ARG, "bad heightmap sampler");
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
-	size_t const img_bytes = ((size_t)2*hs->width*hs->height + 255) & ~(size_t)255, org_bytes = ((size_t)ntiles*8 + 255) & ~(size_t)255;
-	size_t const out_bytes = (size_t)ntiles*zvsize*zvsize*sizeof(float);
+	size_t const img_bytes = (size_t)2*hs->width*hs->height, out_bytes = (size_t)ntiles*zvsize*zvsize*sizeof(float);
 	bool const dev_img = tw_is_device_ptr(data16), dev_out = tw_is_device_ptr(out);
-	rc = tw_reserve(ctx, 0, org_bytes + (dev_img ? 0 : img_bytes) + (dev_out ? 0 : out_bytes) + 256); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0];
-	void *d_org = sp; sp += org_bytes;
+	int32_t *d_org; uint8_t *s_img = nullptr; float *d_out = out;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_org = c.take<int32_t>((size_t)ntiles*2); if (!dev_img) {s_img = c.take<uint8_t>(img_bytes);} if (!dev_out) {d_out = c.take<float>((size_t)ntiles*zvsize*zvsize);}
+	}); if (rc) return rc;
 	TW_CUDA(ctx, cudaMemcpyAsync(d_org, origins_xy, (size_t)ntiles*8, cudaMemcpyHostToDevice, ctx->stream));
-	const uint8_t *d_img = data16;
-	if (!dev_img) {TW_CUDA(ctx, cudaMemcpyAsync(sp, data16, (size_t)2*hs->width*hs->height, cudaMemcpyHostToDevice, ctx->stream)); d_img = (const uint8_t *)sp; sp += img_bytes;}
-	float *d_out = dev_out ? out : (float *)sp;
+	const uint8_t *d_img = dev_img ? data16 : s_img;
+	if (!dev_img) {TW_CUDA(ctx, cudaMemcpyAsync(s_img, data16, img_bytes, cudaMemcpyHostToDevice, ctx->stream));}
 	rc = twi_hmap_sample_tiles(ctx, d_img, hs, d_org, ntiles, zvsize, d_out); if (rc) return rc;
 	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // origins_xy is the caller's buffer
@@ -1163,13 +1157,12 @@ int tw_tile_normals_batch(tw_ctx *ctx, const float *zvals, uint32_t ntiles, uint
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
 	size_t const n = (size_t)ntiles*zvsize*zvsize, stride = zvsize - 1, out_bytes = (size_t)ntiles*stride*stride*4;
 	bool const dev_in = tw_is_device_ptr(zvals), dev_out = tw_is_device_ptr(rgba);
-	size_t const in_bytes = (n*sizeof(float) + 255) & ~(size_t)255, mn_bytes = ((size_t)ntiles*sizeof(unsigned) + 255) & ~(size_t)255;
-	rc = tw_reserve(ctx, 0, (dev_in ? 0 : in_bytes) + (dev_out ? 0 : out_bytes) + mn_bytes + 256); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0];
-	unsigned *d_mn = (unsigned *)sp; sp += mn_bytes;
-	const float *d_z = zvals;
-	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(sp, zvals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const float *)sp; sp += in_bytes;}
-	unsigned char *d_rgba = dev_out ? rgba : (unsigned char *)sp;
+	unsigned *d_mn; float *s_z = nullptr; unsigned char *d_rgba = rgba;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_mn = c.take<unsigned>(ntiles); if (!dev_in) {s_z = c.take<float>(n);} if (!dev_out) {d_rgba = c.take<unsigned char>(out_bytes);}
+	}); if (rc) return rc;
+	const float *d_z = dev_in ? zvals : s_z;
+	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
 	{
 		std::vector<unsigned> init(ntiles, tw_f2ord(1.0f)); // min_normal_z = 1.0, src/tiled_mesh.cpp:868
 		TW_CUDA(ctx, cudaMemcpyAsync(d_mn, init.data(), ntiles*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));
@@ -1209,17 +1202,17 @@ int tw_tile_ao_batch(tw_ctx *ctx, const float *zvals, const int32_t *origins_xy,
 	// chunk of tiles whose context grids fit in ~2 GB
 	uint32_t chunk = (uint32_t)std::min<size_t>(ntiles, std::max<size_t>(1, ((size_t)2 << 30)/(ctx_elems*sizeof(float))));
 	if (chunk > 65535) chunk = 65535;
-	size_t const in_bytes = ((size_t)chunk*tile_elems*sizeof(float) + 255) & ~(size_t)255, cz_bytes = ((size_t)chunk*ctx_elems*sizeof(float) + 255) & ~(size_t)255;
-	size_t const ao_bytes = ((size_t)chunk*ao_elems + 255) & ~(size_t)255;
-	rc = tw_reserve(ctx, 0, (dev_in ? 0 : in_bytes) + cz_bytes + (dev_out ? 0 : ao_bytes) + 256); if (rc) return rc;
+	float *d_cz, *s_z = nullptr; unsigned char *s_ao = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_cz = c.take<float>((size_t)chunk*ctx_elems); if (!dev_in) {s_z = c.take<float>((size_t)chunk*tile_elems);}
+		if (!dev_out) {s_ao = c.take<unsigned char>((size_t)chunk*ao_elems);}
+	}); if (rc) return rc;
 	std::vector<int32_t> org(2*(size_t)chunk);
 	for (uint32_t t0 = 0; t0 < ntiles; t0 += chunk) {
 		uint32_t const nt = (ntiles - t0 < chunk) ? ntiles - t0 : chunk;
-		char *sp = (char *)ctx->d_scratch[0];
-		float *d_cz = (float *)sp; sp += cz_bytes;
 		const float *d_z = zvals + (size_t)t0*tile_elems;
-		if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(sp, d_z, (size_t)nt*tile_elems*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const float *)sp; sp += in_bytes;}
-		unsigned char *d_ao = dev_out ? ao + (size_t)t0*ao_elems : (unsigned char *)sp;
+		if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, d_z, (size_t)nt*tile_elems*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = s_z;}
+		unsigned char *d_ao = dev_out ? ao + (size_t)t0*ao_elems : s_ao;
 		rc = gen_ao_contexts(ctx, origins_xy + 2*(size_t)t0, nt, mesh_x_size, mesh_y_size, dx, dy, zvsize, p, !ctx_inside, org, d_cz);
 		if (rc) return rc;
 		rc = twi_tile_ao(ctx, ctx->stream, d_z, d_cz, nt, zvsize, half_dxy, ctx_inside, d_ao); if (rc) return rc;
@@ -1253,16 +1246,11 @@ int tw_eval_points(tw_ctx *ctx, const float *xy, size_t n, const tw_height_param
 	if (n == 0) return TW_OK;
 	if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
 	bool const dev_in = tw_is_device_ptr(xy), dev_out = tw_is_device_ptr(out);
-	size_t const in_bytes = (2*n*sizeof(float) + 255) & ~(size_t)255, out_bytes = n*sizeof(float);
-	size_t const need = (dev_in ? 0 : in_bytes) + (dev_out ? 0 : out_bytes);
-	if (need) {rc = tw_reserve(ctx, 0, need); if (rc) return rc;}
-	const float *d_xy = xy; float *d_out = out;
-	char *sp = (char *)ctx->d_scratch[0];
-	if (!dev_in) {
-		d_xy = (const float *)sp; sp += in_bytes;
-		TW_CUDA(ctx, cudaMemcpyAsync((void *)d_xy, xy, 2*n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	}
-	if (!dev_out) {d_out = (float *)sp;}
+	size_t const out_bytes = n*sizeof(float);
+	float *s_xy = nullptr, *d_out = out;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_in) {s_xy = c.take<float>(2*n);} if (!dev_out) {d_out = c.take<float>(n);}}); if (rc) return rc;
+	const float *d_xy = dev_in ? xy : s_xy;
+	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_xy, xy, 2*n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
 	rc = twi_eval_points(ctx, d_xy, n, p, q, d_out);
 	if (rc) return rc;
 	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
@@ -1327,13 +1315,13 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 	bool const openmp = (job->mode == TW_EROSION_OPENMP), spec = erode && !openmp && !sweeps && twi_erode_spec_eligible(1, xsize, ysize, job->num_iters);
 	float *const user = image ? job->vals : job->heightmap; // the caller's floats: the map, or the image's optional eroded floats
 	bool const user_dev = (user && tw_is_device_ptr(user));
-	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
-	// slot 0: the floats (unless the caller's are on the device); slot 1: the erosion's scratch; slot 2: [ordered min/max, droplet counter | stage]
-	if (erode && !user_dev) {rc = tw_reserve(ctx, 0, al(n*sizeof(float))); if (rc) return rc;}
+	// slot 0: the floats (unless the caller's are on the device); slot 1: the erosion's scratch; slot 2: [fixed words (ordered min/max, droplet counter) | stage]
+	if (erode && !user_dev) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc;}
 	size_t const ebytes = !erode ? 0 : openmp ? twi_erode_parallel_scratch_bytes(xsize, ysize) : sweeps ? twi_erode_sweeps_scratch_bytes(xsize, ysize)
 	                                 : spec ? twi_erode_spec_scratch_bytes(xsize, ysize) : twi_erode_scratch_bytes(ctx, 1, xsize, ysize);
 	if (ebytes) {rc = tw_reserve(ctx, 1, ebytes); if (rc) return rc;}
-	rc = tw_reserve(ctx, 2, OFF_TILES + 64 + al(sizeof(twi_hmap_stage))); if (rc) return rc;
+	twi_slot2_words *words; twi_hmap_stage *d_st;
+	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {words = c.take<twi_slot2_words>(1); d_st = c.take<twi_hmap_stage>(1);}); if (rc) return rc;
 	rc = tw_reserve_pinned(ctx, sizeof(twi_hmap_stage)); if (rc) return rc;
 	if (image) { // the shared contexts' jobs may read the image; the context has none until the completing poll
 		rc = begin_table_change(ctx); if (rc) return rc;
@@ -1341,8 +1329,7 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 	}
 	tw_erosion_params const ep = *job->ep;
 	float *const d_vals = user_dev ? user : (float *)ctx->d_scratch[0];
-	unsigned *const d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_TILES);
-	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
+	unsigned *const d_mm = words->mm;
 	twi_job pending;
 	pending.kind = twi_job::HMAP; pending.image_w = image ? xsize : 0; pending.image_h = image ? ysize : 0; pending.cancellable = true; pending.reads_image = image;
 	return twi_launch_job(ctx, pending, [&]() -> int {
@@ -1358,7 +1345,7 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 			}
 			else if (!user_dev) {TW_CUDA(ctx, cudaMemcpyAsync(d_vals, user, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
 			int r;
-			if (openmp) {r = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, job->num_threads, &d_st->steps, d_mm + 2);}
+			if (openmp) {r = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, job->num_threads, &d_st->steps, &words->next);}
 			else if (sweeps) {r = twi_erode_sweeps_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, sw->sweep, sw->halo, &d_st->steps);}
 			else if (spec) {r = twi_erode_spec_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps, &d_st->fail, false);}
 			else {r = twi_erode_enqueue(ctx, ctx->stream, 0, ctx->d_scratch[1], 1, d_vals, 1, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps);}
@@ -1396,14 +1383,12 @@ int tw_heightmap_from_floats_u16(tw_ctx *ctx, const float *vals, size_t n, float
 	if (!vals || !out2n || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	bool const dev_in = tw_is_device_ptr(vals), dev_out = tw_is_device_ptr(out2n);
 	size_t const in_bytes = n*sizeof(float), out_bytes = 2*n;
-	size_t const need = (dev_in ? 0 : in_bytes) + (dev_out ? 0 : out_bytes);
-	if (need) {rc = tw_reserve(ctx, 0, need + 256); if (rc) return rc;}
-	rc = tw_reserve(ctx, 2, OFF_TILES); if (rc) return rc;
-	const float *d_in = vals; uint8_t *d_out = out2n;
-	char *s = (char *)ctx->d_scratch[0];
-	if (!dev_in) {d_in = (const float *)s; TW_CUDA(ctx, cudaMemcpyAsync(s, vals, in_bytes, cudaMemcpyHostToDevice, ctx->stream)); s += (in_bytes + 255) & ~(size_t)255;}
-	if (!dev_out) {d_out = (uint8_t *)s;}
-	unsigned *d_bad = (unsigned *)((char *)ctx->d_scratch[2] + OFF_BAD);
+	float *s_in = nullptr; uint8_t *d_out = out2n;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_in) {s_in = c.take<float>(n);} if (!dev_out) {d_out = c.take<uint8_t>(out_bytes);}}); if (rc) return rc;
+	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
+	const float *d_in = dev_in ? vals : s_in;
+	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_in, vals, in_bytes, cudaMemcpyHostToDevice, ctx->stream));}
+	unsigned *d_bad = &twi_slot2(ctx)->bad;
 	TW_CUDA(ctx, cudaMemsetAsync(d_bad, 0, sizeof(unsigned), ctx->stream));
 	rc = twi_from_floats_u16(ctx, d_in, n, val_mult, val_add, d_out, d_bad);
 	if (rc) return rc;
@@ -1421,12 +1406,10 @@ int tw_heightmap_to_floats_u16(tw_ctx *ctx, const uint8_t *data2n, size_t n, flo
 	if (!vals || !data2n || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	bool const dev_in = tw_is_device_ptr(data2n), dev_out = tw_is_device_ptr(vals);
 	size_t const in_bytes = 2*n, out_bytes = n*sizeof(float);
-	size_t const need = (dev_in ? 0 : in_bytes) + (dev_out ? 0 : out_bytes);
-	if (need) {rc = tw_reserve(ctx, 0, need + 256); if (rc) return rc;}
-	const uint8_t *d_in = data2n; float *d_out = vals;
-	char *s = (char *)ctx->d_scratch[0];
-	if (!dev_out) {d_out = (float *)s; s += (out_bytes + 255) & ~(size_t)255;}
-	if (!dev_in) {d_in = (const uint8_t *)s; TW_CUDA(ctx, cudaMemcpyAsync(s, data2n, in_bytes, cudaMemcpyHostToDevice, ctx->stream));}
+	uint8_t *s_in = nullptr; float *d_out = vals;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_out) {d_out = c.take<float>(n);} if (!dev_in) {s_in = c.take<uint8_t>(in_bytes);}}); if (rc) return rc;
+	const uint8_t *d_in = dev_in ? data2n : s_in;
+	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_in, data2n, in_bytes, cudaMemcpyHostToDevice, ctx->stream));}
 	rc = twi_to_floats_u16(ctx, d_in, n, val_mult, val_add, d_out);
 	if (rc) return rc;
 	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(vals, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
@@ -1451,15 +1434,16 @@ int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, f
 	bool const erode = (erosion_iters > 0 && ep && ep->erode_amount > 0.0); // run_erosion (src/heightmap.cpp:153-156, src/erosion.cpp:16)
 	bool const spec = erode && twi_erode_spec_eligible(1, (int)width, (int)height, erosion_iters);
 	bool const vals_dev = (out->vals && tw_is_device_ptr(out->vals)), img_dev = (out->data16 && tw_is_device_ptr(out->data16));
-	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
 	// slot 0: [vals (unless on the device)] [image (unless on the device or the context's)]; slot 1: the sine tables, then the erosion's scratch;
-	// slot 2: [ordered min/max | stage]
-	size_t const vbytes = vals_dev ? 0 : al(n*sizeof(float)), ibytes = (img_dev || out->set_image) ? 0 : al(2*n);
-	rc = tw_reserve(ctx, 0, vbytes + ibytes + 256); if (rc) return rc;
+	// slot 2: [fixed words (ordered min/max) | stage]
+	float *d_vals = out->vals; uint8_t *s_img = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!vals_dev) {d_vals = c.take<float>(n);} if (!img_dev && !out->set_image) {s_img = c.take<uint8_t>(2*n);}}); if (rc) return rc;
 	size_t const ebytes = !erode ? 0 : (spec ? twi_erode_spec_scratch_bytes((int)width, (int)height) : twi_erode_scratch_bytes(ctx, 1, (int)width, (int)height));
 	size_t const s1 = std::max(ebytes, twi_heightgen_slot1_bytes(&g, p));
 	if (s1) {rc = tw_reserve(ctx, 1, s1); if (rc) return rc;}
-	rc = tw_reserve(ctx, 2, OFF_TILES + 64 + al(sizeof(twi_hmap_stage))); if (rc) return rc;
+	twi_slot2_words *words; twi_hmap_stage *d_st;
+	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {words = c.take<twi_slot2_words>(1); d_st = c.take<twi_hmap_stage>(1);}); if (rc) return rc;
+	unsigned *const d_mm = words->mm;
 	rc = tw_reserve_pinned(ctx, sizeof(twi_hmap_stage)); if (rc) return rc;
 	if (out->set_image) { // the old image goes now; the context has none until the completing poll
 		rc = begin_table_change(ctx); if (rc) return rc;
@@ -1469,11 +1453,7 @@ int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, f
 		ctx->hmap_w = ctx->hmap_h = 0;
 		if (!ctx->d_hmap) {TW_CUDA(ctx, cudaMalloc(&ctx->d_hmap, bytes));}
 	}
-	char *s0 = (char *)ctx->d_scratch[0];
-	float *const d_vals = vals_dev ? out->vals : (float *)s0;
-	uint8_t *const d_img = out->set_image ? ctx->d_hmap : (img_dev ? out->data16 : (uint8_t *)(s0 + vbytes));
-	unsigned *const d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_TILES);
-	twi_hmap_stage *const d_st = (twi_hmap_stage *)((char *)ctx->d_scratch[2] + OFF_TILES + 64);
+	uint8_t *const d_img = out->set_image ? ctx->d_hmap : (img_dev ? out->data16 : s_img);
 	twi_job pending;
 	pending.kind = twi_job::HMAP; pending.host_info = out->info; pending.image_w = out->set_image ? (int)width : 0; pending.image_h = out->set_image ? (int)height : 0;
 	pending.cancellable = true; pending.reads_image = (out->set_image != 0);
@@ -1520,8 +1500,8 @@ int tw_minmax_f32(tw_ctx *ctx, const float *vals, size_t n, tw_minmax *mm) {
 		TW_CUDA(ctx, cudaMemcpyAsync(ctx->d_scratch[0], vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 		d_in = (const float *)ctx->d_scratch[0];
 	}
-	rc = tw_reserve(ctx, 2, OFF_TILES); if (rc) return rc;
-	unsigned *d_mm = (unsigned *)((char *)ctx->d_scratch[2] + OFF_MM);
+	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
+	unsigned *d_mm = twi_slot2(ctx)->mm;
 	rc = twi_init_minmax(ctx, d_mm, 1); if (rc) return rc;
 	rc = twi_minmax(ctx, d_in, n, d_mm); if (rc) return rc;
 	return read_minmax(ctx, d_mm, mm, 1);

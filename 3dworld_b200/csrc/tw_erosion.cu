@@ -805,11 +805,15 @@ int twi_ensure_heavy(tw_ctx *ctx, int lane) {
 	return TW_OK;
 }
 
+// twi_erode_enqueue's scratch for `capacity` padded maps: the maps, then the schedule's [work | hist | order] words
+static void erode_layout(twi_carve &c, uint32_t capacity, int xsize, int ysize, float *&d_pad, unsigned *&d_work) {
+	d_pad = c.take<float>((size_t)capacity*(xsize + 2*PAD)*(ysize + 2*PAD)); d_work = c.take<unsigned>((size_t)capacity*2 + WORK_BINS);
+}
+
 size_t twi_erode_scratch_bytes(const tw_ctx *ctx, uint32_t chunk, int xsize, int ysize) {
 	if (plan_whole(ctx->num_sms, chunk, xsize, ysize)) return 256; // no padded copy
-	size_t const padded_elems = (size_t)(xsize + 2*PAD)*(ysize + 2*PAD);
-	size_t const pad_bytes = ((size_t)chunk*padded_elems*sizeof(float) + 255) & ~(size_t)255;
-	return pad_bytes + (((size_t)chunk*2 + WORK_BINS)*sizeof(unsigned) + 255 & ~(size_t)255);
+	twi_carve c; float *d_pad; unsigned *d_work; erode_layout(c, chunk, xsize, ysize, d_pad, d_work);
+	return c.bytes;
 }
 
 // Enqueue the erosion of nt <= 65535 heightmaps on `st`, using `scratch` (twi_erode_scratch_bytes(capacity,..) bytes). `lane` (0..2) selects
@@ -832,9 +836,8 @@ int twi_erode_enqueue(tw_ctx *ctx, cudaStream_t st, int lane, void *scratch, uin
 		TW_LAUNCH_CHECK(ctx);
 		return TW_OK;
 	}
-	size_t const pad_bytes = ((size_t)capacity*padded_elems*sizeof(float) + 255) & ~(size_t)255;
-	float *d_pad = (float *)scratch;
-	unsigned *d_work = (unsigned *)((char *)scratch + pad_bytes), *d_hist = d_work + capacity, *d_order = d_hist + WORK_BINS;
+	twi_carve c{(char *)scratch}; float *d_pad; unsigned *d_work; erode_layout(c, capacity, xsize, ysize, d_pad, d_work);
+	unsigned *d_hist = d_work + capacity, *d_order = d_hist + WORK_BINS;
 	bool const schedule = (nt > ctx->num_sms*4u); // with few heightmaps everything is resident at once anyway
 	if (schedule) {TW_CUDA(ctx, cudaMemsetAsync(d_work, 0, ((size_t)capacity + WORK_BINS)*sizeof(unsigned), st));}
 	pad_kernel<<<dim3((NX + 255)/256, NY, nt), 256, 0, st>>>(maps, d_pad, xsize, ysize, NX, NY, A.E.wpz_minus_half_dxy, schedule ? d_work : nullptr, d_perm);
@@ -927,13 +930,13 @@ int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float mi
 	if (num_iters == 0 || p->erode_amount <= 0.0) return TW_OK; // erosion disabled, src/erosion.cpp:16
 	if (xsize <= 0 || ysize <= 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_erode_parallel: empty heightmap");
 	if (!ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
-	int rc = tw_reserve(ctx, 2, 4096);
+	int rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words));
 	if (rc) return rc;
-	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
+	unsigned long long *d_steps = &twi_slot2(ctx)->steps;
 	TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, sizeof(unsigned long long), ctx->stream));
 	rc = tw_reserve(ctx, 1, twi_erode_parallel_scratch_bytes(xsize, ysize));
 	if (rc) return rc;
-	rc = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_map, xsize, ysize, nullptr, min_zval, num_iters, p, num_threads, d_steps, (unsigned *)(d_steps + 1));
+	rc = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_map, xsize, ysize, nullptr, min_zval, num_iters, p, num_threads, d_steps, &twi_slot2(ctx)->next);
 	if (rc) return rc;
 	cudaStream_t const st = ctx->stream;
 	unsigned long long h_steps = 0;
@@ -1038,8 +1041,8 @@ bool spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters) {
 }
 } // namespace
 
-// M_SPEC's window: sizes from the TW_SPEC_* overrides, arrays carved from `scratch` (nullptr: sizes only); returns the scratch bytes
-static size_t spec_layout(int xsize, int ysize, void *scratch, SpecArgs &S, float *&d_pad, size_t &ntile) {
+// M_SPEC's window: sizes from the TW_SPEC_* overrides, arrays carved by c
+static void spec_layout(twi_carve &c, int xsize, int ysize, SpecArgs &S, float *&d_pad, size_t &ntile) {
 	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
 	memset(&S, 0, sizeof(S));
 	S.B = (unsigned)std::max(32, std::min(env_int("TW_SPEC_WINDOW", 256), (int)SPEC_MAX_SLOTS)); S.B &= ~31u; // <= 256: the round kernel is one cluster with a warp per slot
@@ -1049,22 +1052,11 @@ static size_t spec_layout(int xsize, int ysize, void *scratch, SpecArgs &S, floa
 	S.TNX = ((NX - 1) >> SP_TILE_SHIFT) + 1;
 	S.cap = (unsigned)std::max(1, env_int("TW_SPEC_MOVES", 64));
 	ntile = (size_t)S.TNX*(((NY - 1) >> SP_TILE_SHIFT) + 1);
-	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
-	size_t const pad_b = al((size_t)NX*NY*sizeof(float)), slot_b = al((size_t)S.B*sizeof(unsigned));
-	size_t const total = pad_b + 7*slot_b + 2*al((size_t)S.B*S.W*4) + al((size_t)S.B*S.T*4) + al((size_t)S.B*S.R*12) + al((size_t)S.B*SP_STATE_WORDS*4) + al(ntile*4) + 256;
-	if (!scratch) return total;
-	char *q = (char *)scratch;
-	d_pad = (float *)q; q += pad_b;
+	d_pad = c.take<float>((size_t)NX*NY);
 	unsigned **slot_arrays[7] = {&S.it, &S.status, &S.nlog, &S.ntiles, &S.nseg, &S.minw, &S.steps};
-	for (auto a : slot_arrays) {*a = (unsigned *)q; q += slot_b;}
-	S.cells = (unsigned *)q; q += al((size_t)S.B*S.W*4);
-	S.vals = (float *)q; q += al((size_t)S.B*S.W*4);
-	S.tiles = (unsigned *)q; q += al((size_t)S.B*S.T*4);
-	S.seg = (unsigned *)q; q += al((size_t)S.B*S.R*12);
-	S.state = (unsigned *)q; q += al((size_t)S.B*SP_STATE_WORDS*4);
-	S.stamps = (unsigned *)q; q += al(ntile*4);
-	S.ctl = (unsigned *)q; // 256 bytes
-	return total;
+	for (auto a : slot_arrays) {*a = c.take<unsigned>(S.B);}
+	S.cells = c.take<unsigned>((size_t)S.B*S.W); S.vals = c.take<float>((size_t)S.B*S.W); S.tiles = c.take<unsigned>((size_t)S.B*S.T);
+	S.seg = c.take<unsigned>((size_t)S.B*S.R*3); S.state = c.take<unsigned>((size_t)S.B*SP_STATE_WORDS); S.stamps = c.take<unsigned>(ntile); S.ctl = c.take<unsigned>(64);
 }
 
 // The rounds as one CUDA graph: a conditional WHILE node whose body is the walker launch and the round kernel, which clears the condition. The graph's kernel
@@ -1106,8 +1098,8 @@ static int spec_loop_graph(tw_ctx *ctx, cudaStream_t st, DArgs const &W, unsigne
 bool twi_erode_spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters) {return spec_eligible(nt, xsize, ysize, num_iters);}
 
 size_t twi_erode_spec_scratch_bytes(int xsize, int ysize) {
-	SpecArgs S; float *d_pad; size_t ntile;
-	return spec_layout(xsize, ysize, nullptr, S, d_pad, ntile);
+	twi_carve c; SpecArgs S; float *d_pad; size_t ntile; spec_layout(c, xsize, ysize, S, d_pad, ntile);
+	return c.bytes;
 }
 
 // One heightmap, the reference's serial droplet order, bit for bit (see M_SPEC at the top), on ctx->stream: pad, window set-up, the rounds, unpad with the lower
@@ -1124,7 +1116,7 @@ int twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, 
 	SpecArgs S;
 	float *d_pad = nullptr;
 	size_t ntile = 0;
-	spec_layout(xsize, ysize, scratch, S, d_pad, ntile);
+	twi_carve c{(char *)scratch}; spec_layout(c, xsize, ysize, S, d_pad, ntile);
 	DArgs A;
 	memset(&A, 0, sizeof(A));
 	A.E = make_eparams(p);
@@ -1180,14 +1172,14 @@ int twi_erode(tw_ctx *ctx, float *d_maps, uint32_t ntiles, int xsize, int ysize,
 	if (num_iters == 0 || p->erode_amount <= 0.0) return TW_OK; // erosion disabled, src/erosion.cpp:16
 	if (xsize <= 0 || ysize <= 0 || ntiles == 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_erode: empty heightmap");
 	if (!ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
-	int rc = tw_reserve(ctx, 2, 4096);
+	int rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words));
 	if (rc) return rc;
-	unsigned long long *d_steps = (unsigned long long *)((char *)ctx->d_scratch[2] + 2048);
+	unsigned long long *d_steps = &twi_slot2(ctx)->steps;
 	TW_CUDA(ctx, cudaMemsetAsync(d_steps, 0, sizeof(unsigned long long), ctx->stream));
 	if (spec_eligible(ntiles, xsize, ysize, num_iters)) { // one big map: the serial order, walked speculatively in parallel and committed in order (M_SPEC)
 		rc = tw_reserve(ctx, 1, twi_erode_spec_scratch_bytes(xsize, ysize));
 		if (rc) return rc;
-		unsigned *d_fail = (unsigned *)(d_steps + 2);
+		unsigned *d_fail = &twi_slot2(ctx)->fail;
 		rc = twi_erode_spec_enqueue(ctx, ctx->d_scratch[1], d_maps, xsize, ysize, d_min_zvals, min_zval_all, num_iters, p, d_steps, d_fail, true);
 		if (rc) return rc;
 		unsigned long long h_steps = 0;
@@ -1302,12 +1294,13 @@ __global__ void sweep_advance_kernel(unsigned *it0, unsigned sweep, unsigned num
 	if (cancel) {twi_mark_stopped(jw);}
 	if (last || cancel) {cudaGraphSetConditional(loop, 0u);}
 }
-size_t al256(size_t b) {return (b + 255) & ~(size_t)255;}
+// the sweeps job's scratch: the padded map (n cells), its fixed-point deltas and the sweep word
+void sweeps_layout(twi_carve &c, size_t n, float *&P, long long *&D, unsigned *&ctl) {P = c.take<float>(n); D = c.take<long long>(n); ctl = c.take<unsigned>(1);}
 } // namespace
 
 size_t twi_erode_sweeps_scratch_bytes(int xsize, int ysize) {
-	size_t const n = (size_t)(xsize + 2*PAD)*(ysize + 2*PAD);
-	return al256(n*sizeof(float)) + al256(n*sizeof(long long)) + 256;
+	twi_carve c; float *P; long long *D; unsigned *ctl; sweeps_layout(c, (size_t)(xsize + 2*PAD)*(ysize + 2*PAD), P, D, ctl);
+	return c.bytes;
 }
 
 // The sweeps as one CUDA graph: a conditional WHILE node whose body is the walk of a sweep, the apply and sweep_advance_kernel, which clears the condition.
@@ -1356,9 +1349,7 @@ int twi_erode_sweeps_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize
 	cudaStream_t const st = ctx->stream;
 	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
 	size_t const n = (size_t)NX*NY;
-	float *P = (float *)scratch;
-	long long *D = (long long *)((char *)scratch + al256(n*sizeof(float)));
-	unsigned *ctl = (unsigned *)((char *)D + al256(n*sizeof(long long)));
+	twi_carve c{(char *)scratch}; float *P; long long *D; unsigned *ctl; sweeps_layout(c, n, P, D, ctl);
 	TW_CUDA(ctx, cudaMemsetAsync(D, 0, n*sizeof(long long), st));
 	TW_CUDA(ctx, cudaMemsetAsync(ctl, 0, sizeof(unsigned), st));
 	pad_kernel<<<dim3((NX + 255)/256, NY, 1), 256, 0, st>>>(d_map, P, xsize, ysize, NX, NY, 0.0f, nullptr, nullptr); // = sweep_pad_kernel of the one band

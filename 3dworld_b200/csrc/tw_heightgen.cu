@@ -772,11 +772,13 @@ int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, in
 size_t twi_sine_tiles_stage_bytes(uint32_t ntiles) {return (size_t)ntiles*(2*sizeof(float) + sizeof(uint2) + sizeof(float2));} // distinct origins (<= 2 per tile), table indices, origins
 
 namespace {
-struct SineTilesLayout {size_t tab_bytes, org_bytes, tt_bytes, to_bytes;};
-SineTilesLayout sine_tiles_layout(const tw_grid2d *g, size_t nux, size_t nuy, uint32_t ntiles) {
+// a sine batch's device memory: the tables (nux X tables, then nuy Y tables), the distinct origins, the tiles' table indices and origins
+struct SineTilesMem {float *Xt, *uorg; uint2 *tabs; float2 *torg;};
+SineTilesMem sine_tiles_layout(twi_carve &c, const tw_grid2d *g, size_t nux, size_t nuy, uint32_t ntiles) {
 	size_t const xstride = (size_t)(F_TABLE + 1)*((g->nx + 63) & ~63u), ystride = (size_t)(F_TABLE + 1)*((g->ny + 63) & ~63u);
-	return SineTilesLayout{((nux*xstride + nuy*ystride)*sizeof(float) + 255) & ~(size_t)255, ((nux + nuy)*sizeof(float) + 255) & ~(size_t)255,
-	                       ((size_t)ntiles*sizeof(uint2) + 255) & ~(size_t)255, ((size_t)ntiles*sizeof(float2) + 255) & ~(size_t)255};
+	SineTilesMem M;
+	M.Xt = c.take<float>(nux*xstride + nuy*ystride); M.uorg = c.take<float>(nux + nuy); M.tabs = c.take<uint2>(ntiles); M.torg = c.take<float2>(ntiles);
+	return M;
 }
 } // namespace
 
@@ -793,8 +795,8 @@ size_t twi_sine_tiles_plan(const tw_grid2d *g, const float2 *h_org, uint32_t nti
 	}
 	b->nux = (unsigned)b->uorg.size(); b->nuy = (unsigned)uy.size();
 	b->uorg.insert(b->uorg.end(), uy.begin(), uy.end()); // [distinct x origins | distinct y origins]
-	SineTilesLayout const L = sine_tiles_layout(g, b->nux, b->nuy, ntiles);
-	return L.tab_bytes + L.org_bytes + L.tt_bytes + L.to_bytes;
+	twi_carve c; sine_tiles_layout(c, g, b->nux, b->nuy, ntiles);
+	return c.bytes;
 }
 
 int twi_sine_tiles_setup(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, int enable_glaciate, int min_start_sin, const float2 *h_org, uint32_t ntiles,
@@ -807,17 +809,11 @@ int twi_sine_tiles_setup(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params
 	if (nux + nuy > 65535) return tw_set_error(ctx, TW_ERR_ARG, "more than 65535 distinct tile rows + columns in one batch"); // gridDim.z of the table launch
 	unsigned const xpitch = (nx + 63) & ~63u, ypitch = (ny + 63) & ~63u;
 	size_t const xstride = (size_t)(F_TABLE + 1)*xpitch, ystride = (size_t)(F_TABLE + 1)*ypitch;
-	SineTilesLayout const L = sine_tiles_layout(g, nux, nuy, ntiles);
-	if (!d_mem) {
-		int const rc = tw_reserve(ctx, 1, L.tab_bytes + L.org_bytes + L.tt_bytes + L.to_bytes);
-		if (rc) return rc;
-		d_mem = ctx->d_scratch[1];
-	}
-	char *sp = (char *)d_mem;
-	float *Xt = (float *)sp, *Yt = Xt + nux*xstride; sp += L.tab_bytes;
-	float *d_uorg = (float *)sp; sp += L.org_bytes;
-	uint2 *d_tabs = (uint2 *)sp; sp += L.tt_bytes;
-	float2 *d_torg = (float2 *)sp;
+	SineTilesMem M;
+	auto layout = [&](twi_carve &c) {M = sine_tiles_layout(c, g, nux, nuy, ntiles);};
+	if (d_mem) {twi_carve c{(char *)d_mem}; layout(c);}
+	else {int const rc = twi_reserve_carve(ctx, 1, layout); if (rc) return rc;}
+	float *Xt = M.Xt, *Yt = Xt + nux*xstride, *d_uorg = M.uorg; uint2 *d_tabs = M.tabs; float2 *d_torg = M.torg;
 	std::vector<float> const &uorg = b->uorg;
 	const void *src_uorg = uorg.data(), *src_tabs = b->tabs.data(), *src_org = h_org;
 	if (h_stage) { // pinned copies that outlive this call: nothing below has to wait for the uploads

@@ -142,6 +142,27 @@ int  tw_reserve(tw_ctx *ctx, int slot, size_t bytes);           // grow d_scratc
 int  tw_reserve_pinned(tw_ctx *ctx, size_t bytes);
 bool tw_is_device_ptr(const void *p);
 
+// A layout of scratch or pinned staging: regions carved one after another from `base`, each starting on a 256-byte boundary. A layout is written once, as
+// code that takes a twi_carve &, and run twice: with base == nullptr it only counts `bytes` (the size to reserve), then on the reserved memory. An absent
+// region is written `want ? c.take<T>(n) : nullptr`, never take(0), which returns an address.
+struct twi_carve {
+	char *base = nullptr; size_t bytes = 0;
+	template <typename T> T *take(size_t count) {T *p = base ? (T *)(base + bytes) : nullptr; bytes += (count*sizeof(T) + 255) & ~(size_t)255; return p;}
+};
+// Counts `layout`, reserves its bytes of scratch slot `slot` (TWI_PINNED: of the pinned staging), then carves it from that memory. Reserve before anything is
+// enqueued: tw_reserve synchronises ctx->stream and may re-allocate the slot, so a pointer carved before a later reserve of the same slot is stale after it.
+constexpr int TWI_PINNED = -1;
+template <typename Layout> int twi_reserve_carve(tw_ctx *ctx, int slot, Layout &&layout) {
+	twi_carve c; layout(c);
+	int const rc = (slot == TWI_PINNED) ? tw_reserve_pinned(ctx, c.bytes) : tw_reserve(ctx, slot, c.bytes); if (rc) return rc;
+	c = twi_carve{(char *)((slot == TWI_PINNED) ? ctx->h_pinned : ctx->d_scratch[slot])}; layout(c);
+	return TW_OK;
+}
+// The fixed words at the start of scratch slot 2 (a layout of slot 2 takes them first): one grid's ordered min/max, the 16-bit packing's count of values out
+// of range, the erosion's droplet moves, its droplet counter (tw_erode_parallel) and the speculative erosion's no-progress word
+struct twi_slot2_words {unsigned mm[2], bad, pad_; unsigned long long steps; unsigned next, fail;};
+inline twi_slot2_words *twi_slot2(tw_ctx *ctx) {return (twi_slot2_words *)ctx->d_scratch[2];}
+
 #define TW_CUDA(ctx, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
 	return tw_set_error((ctx), TW_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
 #define TW_LAUNCH_CHECK(ctx) do { (ctx)->launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { \

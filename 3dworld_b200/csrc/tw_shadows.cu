@@ -237,18 +237,13 @@ static int tile_shadows(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy,
 	if (!twi_shadow_plan_make(tile_xy, ntiles, sp, sh_in_x != nullptr, sh_in_y != nullptr, &P) && ex) return tw_set_error(ctx, TW_ERR_ARG, "tile_xy names a tile twice");
 	bool const dev_z = tw_is_device_ptr(zvals), dev_m = tw_is_device_ptr(smask);
 	if (dev_m && ((size_t)smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)");
-	auto al = [](size_t b) {return (b + 255) & ~(size_t)255;};
-	size_t const zb = al(cells*sizeof(float)), mb = al(cells + 4), kb = al(2*edge*sizeof(unsigned long long));
-	size_t const fbx = al((sh_in_x ? 2 : 1)*edge*sizeof(float)), fby = al((sh_in_y ? 2 : 1)*edge*sizeof(float)), ib = al(twi_shadow_plan_ints(ntiles)*sizeof(int));
-	int rc = tw_reserve(ctx, 0, (dev_z ? 0 : zb) + (dev_m ? 0 : mb) + kb + fbx + fby + ib + 256); if (rc) return rc;
-	char *p = (char *)ctx->d_scratch[0];
-	const float *d_z = zvals; unsigned char *d_m = smask;
-	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(p, zvals, cells*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const float *)p; p += zb;}
-	if (!dev_m) {d_m = (unsigned char *)p; p += mb;}
-	unsigned long long *d_keys = (unsigned long long *)p; p += kb;
-	float *d_ox = (float *)p; p += fbx;
-	float *d_oy = (float *)p; p += fby;
-	int *d_plan = (int *)p;
+	float *s_z = nullptr, *d_ox, *d_oy; unsigned char *d_m = smask; unsigned long long *d_keys; int *d_plan;
+	int rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		if (!dev_z) {s_z = c.take<float>(cells);} if (!dev_m) {d_m = c.take<unsigned char>(cells + 4);} d_keys = c.take<unsigned long long>(2*edge);
+		d_ox = c.take<float>((sh_in_x ? 2 : 1)*edge); d_oy = c.take<float>((sh_in_y ? 2 : 1)*edge); d_plan = c.take<int>(twi_shadow_plan_ints(ntiles));
+	}); if (rc) return rc;
+	const float *d_z = zvals;
+	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, cells*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = s_z;}
 	std::vector<int> plan(twi_shadow_plan_ints(ntiles));
 	twi_shadow_plan_pack(P, plan.data());
 	TW_CUDA(ctx, cudaMemcpyAsync(d_plan, plan.data(), plan.size()*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));

@@ -59,8 +59,6 @@ int copy_tiles(tw_ctx *ctx, void *dst, const int *dst_idx, const void *src, cons
 	return TW_OK;
 }
 
-size_t al(size_t b) {return (b + 255) & ~(size_t)255;}
-
 int begin_call(tw_tile_set *s) { // the context's device, its tables, and its pending job completed
 	TW_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
 	return twi_finish_pending(s->ctx);
@@ -148,32 +146,44 @@ int frame_keys(tw_ctx *ctx, const tw_tile_set *s, const int32_t *remove_xy, uint
 }
 
 // A relight planned on the host against a set state: per light the batch B (invalid requested tiles + their invalid upstream closure), its plan, and the
-// slab slots it reads and writes. Its scratch is [B's zvals | mask | 64-bit keys | x edges (outputs, then caller rows) | y edges | host-bound output staging |
-// int region], the int region ([requested tiles' slots | per light: plan, B's slots, x and y caller-row sources]) staged in pinned memory.
+// slab slots it reads and writes. Its int region ([requested tiles' slots | per light: plan, B's slots, x and y caller-row sources]) is staged in pinned memory
+// and goes up in one copy.
 struct relight_t {
 	struct batch_t {
 		bool reset = false;                      // the slot's params differ: every tile of it is invalid
 		std::vector<twts::key> B;
 		twi_shadow_plan P;
 		std::vector<int> ints;                   // [plan (3*nB) | B's slots | x caller-row sources | y caller-row sources]
-		size_t off_ints = 0, off_out = 0;        // byte offsets into the int region / the output staging
+		size_t off_ints = 0;                     // byte offset into the int region
 	};
-	uint32_t n = 0, nl = 0;
+	uint32_t n = 0, nl = 0, zv = 0, maxB = 0;
 	std::vector<tw_tile_set_light> lights;
 	std::vector<int> req_slot;
 	std::vector<char> dev_m, dev_x, dev_y;
 	std::vector<batch_t> jobs;
-	size_t zb = 0, mb = 0, kb = 0, fb = 0, off_out = 0, off_ints = 0, ints_bytes = 0;
-	size_t dev_bytes() const {return off_ints + ints_bytes;}
+	size_t ints_bytes = 0;
+	// the device scratch: [B's zvals | mask | 64-bit keys | x edges (outputs, then caller rows) | y edges | per light: staging of the host-bound smask, sh_out_x
+	// and sh_out_y (nullptr: none) | int region]
+	struct dev_t {float *zB, *ox, *oy; unsigned char *mB; unsigned long long *keys; std::vector<unsigned char *> om; std::vector<float *> sx, sy; char *ints;};
+	void dev_layout(twi_carve &c, dev_t &D) const {
+		size_t const zt = (size_t)zv*zv, e2 = 2*(size_t)maxB*zv;
+		D.zB = c.take<float>(maxB*zt); D.mB = c.take<unsigned char>(maxB*zt + 4); D.keys = c.take<unsigned long long>(e2); D.ox = c.take<float>(e2); D.oy = c.take<float>(e2);
+		D.om.resize(nl); D.sx.resize(nl); D.sy.resize(nl);
+		for (uint32_t l = 0; l < nl; ++l) {
+			D.om[l] = dev_m[l] ? nullptr : c.take<unsigned char>(n*zt);
+			D.sx[l] = (lights[l].sh_out_x && !dev_x[l]) ? c.take<float>((size_t)n*zv) : nullptr; D.sy[l] = (lights[l].sh_out_y && !dev_y[l]) ? c.take<float>((size_t)n*zv) : nullptr;
+		}
+		D.ints = c.take<char>(ints_bytes);
+	}
+	size_t dev_bytes() const {twi_carve c; dev_t D; dev_layout(c, D); return c.bytes;}
 };
 
 // validates req against st (TW_ERR_ARG on ctx; nothing changes) and plans it
 int relight_plan(tw_ctx *ctx, const tw_tile_set *s, twts::state const &st, const tw_tile_set_request *req, relight_t &R) {
 	if (!req || !req->tile_xy || req->n == 0 || !req->lights || req->nlights == 0 || req->nlights > s->nlights)
 		return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: needs tile_xy, n >= 1 and 1 .. %u lights", s->nlights);
-	uint32_t const n = req->n, nl = req->nlights, zv = s->zvsize;
-	size_t const zt = (size_t)zv*zv, eb = (size_t)zv*sizeof(float);
-	R.n = n; R.nl = nl;
+	uint32_t const n = req->n, nl = req->nlights;
+	R.n = n; R.nl = nl; R.zv = s->zvsize;
 	R.lights.assign(req->lights, req->lights + nl);
 	std::vector<twts::key> keys;
 	if (!read_keys(req->tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set relight: tile_xy names a tile twice");
@@ -192,8 +202,7 @@ int relight_plan(tw_ctx *ctx, const tw_tile_set *s, twts::state const &st, const
 		R.dev_x[l] = Lr.sh_out_x && tw_is_device_ptr(Lr.sh_out_x); R.dev_y[l] = Lr.sh_out_y && tw_is_device_ptr(Lr.sh_out_y);
 	}
 	R.jobs.resize(nl);
-	uint32_t maxB = 0;
-	size_t ints_bytes = al(n*sizeof(int)), out_bytes = 0;    // the int region starts with the requested tiles' slots
+	twi_carve ints; ints.take<int>(n);                       // the int region's offsets: it starts with the requested tiles' slots
 	for (uint32_t l = 0; l < nl; ++l) {
 		tw_tile_set::slot_t const &S = s->L[l];
 		relight_t::batch_t &J = R.jobs[l];
@@ -204,7 +213,7 @@ int relight_plan(tw_ctx *ctx, const tw_tile_set *s, twts::state const &st, const
 		std::vector<uint8_t> const &valid = J.reset ? none : st.valid[l];
 		J.B = twts::recompute_batch(st.where, valid, keys, sx, sy);
 		uint32_t const nB = (uint32_t)J.B.size();
-		maxB = std::max(maxB, nB);
+		R.maxB = std::max(R.maxB, nB);
 		if (nB) {
 			std::vector<int32_t> bxy(2*(size_t)nB);
 			for (uint32_t t = 0; t < nB; ++t) {bxy[2*t] = J.B[t].first; bxy[2*t+1] = J.B[t].second;}
@@ -219,12 +228,9 @@ int relight_plan(tw_ctx *ctx, const tw_tile_set *s, twts::state const &st, const
 				ry[t] = cached(twts::key(J.B[t].first + sx, J.B[t].second)); // sh_in_y row: the sh_out_y of (tx + sx, ty)
 			}
 		}
-		J.off_ints = ints_bytes; ints_bytes += al(J.ints.size()*sizeof(int));
-		J.off_out = out_bytes;
-		out_bytes += (R.dev_m[l] ? 0 : al(n*zt)) + ((R.lights[l].sh_out_x && !R.dev_x[l]) ? al(n*eb) : 0) + ((R.lights[l].sh_out_y && !R.dev_y[l]) ? al(n*eb) : 0);
+		J.off_ints = ints.bytes; ints.take<int>(J.ints.size());
 	}
-	R.zb = al((size_t)maxB*zt*sizeof(float)); R.mb = al((size_t)maxB*zt + 4); R.kb = al(2*(size_t)maxB*eb*2); R.fb = al(2*(size_t)maxB*eb);
-	R.off_out = R.zb + R.mb + R.kb + 2*R.fb; R.off_ints = R.off_out + out_bytes; R.ints_bytes = ints_bytes;
+	R.ints_bytes = ints.bytes;
 	return TW_OK;
 }
 
@@ -234,11 +240,9 @@ int relight_plan(tw_ctx *ctx, const tw_tile_set *s, twts::state const &st, const
 int relight_enqueue(tw_ctx *ctx, tw_tile_set *s, relight_t const &R, char *d, char *h) {
 	uint32_t const n = R.n, zv = s->zvsize;
 	size_t const zt = (size_t)zv*zv, eb = (size_t)zv*sizeof(float);
-	float *d_zB = (float *)d;
-	unsigned char *d_mB = (unsigned char *)(d + R.zb);
-	unsigned long long *d_keys = (unsigned long long *)(d + R.zb + R.mb);
-	float *d_ox = (float *)(d + R.zb + R.mb + R.kb), *d_oy = (float *)(d + R.zb + R.mb + R.kb + R.fb);
-	char *d_ints = d + R.off_ints;
+	twi_carve c{d};
+	relight_t::dev_t D; R.dev_layout(c, D);
+	float *d_zB = D.zB, *d_ox = D.ox, *d_oy = D.oy; unsigned char *d_mB = D.mB; unsigned long long *d_keys = D.keys; char *d_ints = D.ints;
 	memcpy(h, R.req_slot.data(), n*sizeof(int));
 	for (relight_t::batch_t const &J : R.jobs) {memcpy(h + J.off_ints, J.ints.data(), J.ints.size()*sizeof(int));}
 	uint32_t minz_bits; {float const m = TW_MESH_MIN_Z; memcpy(&minz_bits, &m, 4);}
@@ -259,10 +263,10 @@ int relight_enqueue(tw_ctx *ctx, tw_tile_set *s, relight_t const &R, char *d, ch
 			r = copy_tiles(ctx, S.d_ox, d_bs, d_ox, nullptr, eb, nB); if (r) return r;
 			r = copy_tiles(ctx, S.d_oy, d_bs, d_oy, nullptr, eb, nB); if (r) return r;
 		}
-		char *st = d + R.off_out + J.off_out; // the requested tiles' outputs, in request order
-		unsigned char *om = R.dev_m[l] ? Lr.smask : (unsigned char *)st; st += R.dev_m[l] ? 0 : al(n*zt);
-		float *ox = !Lr.sh_out_x ? nullptr : (R.dev_x[l] ? Lr.sh_out_x : (float *)st); st += (Lr.sh_out_x && !R.dev_x[l]) ? al(n*eb) : 0;
-		float *oy = !Lr.sh_out_y ? nullptr : (R.dev_y[l] ? Lr.sh_out_y : (float *)st);
+		// the requested tiles' outputs, in request order
+		unsigned char *om = R.dev_m[l] ? Lr.smask : D.om[l];
+		float *ox = !Lr.sh_out_x ? nullptr : (R.dev_x[l] ? Lr.sh_out_x : D.sx[l]);
+		float *oy = !Lr.sh_out_y ? nullptr : (R.dev_y[l] ? Lr.sh_out_y : D.sy[l]);
 		int r = copy_tiles(ctx, om, nullptr, S.d_m, d_req, zt, n); if (r) return r;
 		if (ox) {r = copy_tiles(ctx, ox, nullptr, S.d_ox, d_req, eb, n); if (r) return r;}
 		if (oy) {r = copy_tiles(ctx, oy, nullptr, S.d_oy, d_req, eb, n); if (r) return r;}
@@ -270,10 +274,9 @@ int relight_enqueue(tw_ctx *ctx, tw_tile_set *s, relight_t const &R, char *d, ch
 	TW_CUDA(ctx, cudaEventRecord(s->ev, ctx->stream));
 	for (uint32_t l = 0; l < R.nl; ++l) { // host outputs: one copy each, at the end
 		tw_tile_set_light const &Lr = R.lights[l];
-		char *st = d + R.off_out + R.jobs[l].off_out;
-		if (!R.dev_m[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.smask, st, n*zt, cudaMemcpyDeviceToHost, ctx->stream)); st += al(n*zt);}
-		if (Lr.sh_out_x && !R.dev_x[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_x, st, n*eb, cudaMemcpyDeviceToHost, ctx->stream)); st += al(n*eb);}
-		if (Lr.sh_out_y && !R.dev_y[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_y, st, n*eb, cudaMemcpyDeviceToHost, ctx->stream));}
+		if (D.om[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.smask, D.om[l], n*zt, cudaMemcpyDeviceToHost, ctx->stream));}
+		if (D.sx[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_x, D.sx[l], n*eb, cudaMemcpyDeviceToHost, ctx->stream));}
+		if (D.sy[l]) {TW_CUDA(ctx, cudaMemcpyAsync(Lr.sh_out_y, D.sy[l], n*eb, cudaMemcpyDeviceToHost, ctx->stream));}
 	}
 	return TW_OK;
 }
@@ -303,9 +306,13 @@ struct frame_tail : twi_job_tail {
 	twts::state post;                // the set's host state after the frame's removes and puts
 	std::vector<int> idx;            // the put tiles' slab slots, in tile_xy order
 	uint32_t ntiles = 0;
-	size_t idx_bytes = 0;
 	bool relight = false;
 	relight_t R;
+	// [put tiles' slots | the relight's memory] of the device scratch (d) and of the pinned staging (h)
+	void layout(twi_carve &d, twi_carve &h, int *&d_idx, int *&h_idx, char *&d_rl, char *&h_rl) const {
+		d_idx = d.take<int>(ntiles); h_idx = h.take<int>(ntiles);
+		d_rl = relight ? d.take<char>(R.dev_bytes()) : nullptr; h_rl = relight ? h.take<char>(R.ints_bytes) : nullptr;
+	}
 	int prepare(tw_ctx *ctx) override {return grow(s, post.used, ctx);}
 	// once this starts the slabs may be partly written, so every failure from here on is reported as TW_ERR_CUDA (the code that selects the error state)
 	int enqueue(tw_ctx *ctx, const float *d_zvals, char *d, char *h) override {
@@ -313,12 +320,13 @@ struct frame_tail : twi_job_tail {
 		return (rc && rc != TW_ERR_CUDA) ? TW_ERR_CUDA : rc;
 	}
 	int enqueue_tail(tw_ctx *ctx, const float *d_zvals, char *d, char *h) {
-		memcpy(h, idx.data(), ntiles*sizeof(int));
-		int *d_idx = (int *)d;
-		TW_CUDA(ctx, cudaMemcpyAsync(d_idx, h, ntiles*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+		twi_carve dc{d}, hc{h}; int *d_idx, *h_idx; char *d_rl, *h_rl;
+		layout(dc, hc, d_idx, h_idx, d_rl, h_rl);
+		memcpy(h_idx, idx.data(), ntiles*sizeof(int));
+		TW_CUDA(ctx, cudaMemcpyAsync(d_idx, h_idx, ntiles*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
 		TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0));
 		int rc = copy_tiles(ctx, s->d_z, d_idx, d_zvals, nullptr, (size_t)s->zvsize*s->zvsize*sizeof(float), ntiles); if (rc) return rc;
-		if (relight) return relight_enqueue(ctx, s, R, d + idx_bytes, h + idx_bytes);
+		if (relight) return relight_enqueue(ctx, s, R, d_rl, h_rl);
 		TW_CUDA(ctx, cudaEventRecord(s->ev, ctx->stream));
 		return TW_OK;
 	}
@@ -371,11 +379,9 @@ int tw_tile_set_put(tw_tile_set *s, const int32_t *tile_xy, uint32_t n, const fl
 	rc = grow(s, next, ctx); if (rc) return rc;
 	size_t const tb = (size_t)s->zvsize*s->zvsize*sizeof(float);
 	bool const dev = tw_is_device_ptr(zvals);
-	size_t const zb = dev ? 0 : al(n*tb);
-	rc = tw_reserve(ctx, 0, zb + al(n*sizeof(int))); if (rc) return rc;
-	char *p = (char *)ctx->d_scratch[0];
+	char *p = nullptr; int *d_idx;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {p = c.take<char>(n*tb);} d_idx = c.take<int>(n);}); if (rc) return rc;
 	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(p, zvals, n*tb, cudaMemcpyHostToDevice, ctx->stream));}
-	int *d_idx = (int *)(p + zb);
 	TW_CUDA(ctx, cudaMemcpyAsync(d_idx, idx.data(), n*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
 	TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0)); // a frame's job on another context may still read these slots
 	rc = copy_tiles(ctx, s->d_z, d_idx, dev ? (const void *)zvals : (const void *)p, nullptr, tb, n); if (rc) return rc;
@@ -464,9 +470,8 @@ int tw_tile_set_create_tiles_launch(tw_ctx *ctx, tw_tile_set *s, const int32_t *
 		twts::put_tiles(T.post, pk, T.idx, free_left, used, sg);
 	}
 	if (frame->relight) {rc = relight_plan(ctx, s, T.post, frame->relight, T.R); if (rc) return rc; T.relight = true;}
-	T.ntiles = ntiles; T.idx_bytes = al((size_t)ntiles*sizeof(int));
-	T.dev_bytes = T.idx_bytes + (T.relight ? T.R.dev_bytes() : 0);
-	T.pin_bytes = T.idx_bytes + (T.relight ? T.R.ints_bytes : 0);
+	T.ntiles = ntiles;
+	{twi_carve dc, hc; int *d_idx, *h_idx; char *d_rl, *h_rl; T.layout(dc, hc, d_idx, h_idx, d_rl, h_rl); T.dev_bytes = dc.bytes; T.pin_bytes = hc.bytes;}
 	tw_tile_outputs const none = {nullptr, nullptr, nullptr, nullptr, nullptr};
 	rc = twi_create_tiles_launch(ctx, frame->hs, origins_xy, ntiles, mesh_x_size, mesh_y_size, dx, dy, s->zvsize, p, erosion_iters, ep, min_zval, wpz_max, size,
 	                             out ? out : &none, shading, &T);

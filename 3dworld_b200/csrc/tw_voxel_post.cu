@@ -298,7 +298,6 @@ scan_blocks_kernel(const unsigned *__restrict__ sums, unsigned nblocks, unsigned
 // The cube's 12 edges as grid edges, from edge_to_vals: s_edge[i] = axis | ox << 2 | oy << 3 | oz << 4 (axis 0 x, 1 y, 2 z; o = the edge's low corner in
 // the cube); s_look[4*axis + 2*o1 + o2] = the local edge along axis whose low corner is at o1, o2 on the axis' other two (perp() order).
 // edge_to_vals must name each edge of the cube once (Bourke's table does).
-size_t al256(size_t b) {return (b + 255) & ~(size_t)255;}
 __device__ __forceinline__ void perp(unsigned a, unsigned &p1, unsigned &p2) {p1 = (a == 1) ? 0u : 1u; p2 = (a == 2) ? 0u : 2u;} // y > x > z in index weight
 __device__ void mesh_edge_tables(const unsigned *__restrict__ etv, unsigned char *s_edge, unsigned char *s_look) {
 	unsigned const t = threadIdx.x;
@@ -488,15 +487,14 @@ int enqueue_mesh(tw_ctx *ctx, const float *d_v, const unsigned char *d_o, const 
 	}
 	return TW_OK;
 }
-size_t mesh_scratch_bytes(size_t n, unsigned nblocks) {return al256(n*sizeof(unsigned)) + 2*al256((size_t)nblocks*sizeof(unsigned)) + 2*al256((size_t)nblocks*8) + 256;}
-MeshScratch mesh_scratch(char *sp, size_t n, unsigned nblocks) {
+MeshScratch mesh_scratch(twi_carve &c, size_t n, unsigned nblocks) {
 	MeshScratch S;
-	S.words = (unsigned *)sp; sp += al256(n*sizeof(unsigned));
-	S.vsums = (unsigned *)sp; sp += al256((size_t)nblocks*sizeof(unsigned));
-	S.tsums = (unsigned *)sp; sp += al256((size_t)nblocks*sizeof(unsigned));
-	S.voff = (unsigned long long *)sp; sp += al256((size_t)nblocks*8);
-	S.toff = (unsigned long long *)sp; sp += al256((size_t)nblocks*8);
-	S.totals = (unsigned long long *)sp;
+	S.words = c.take<unsigned>(n);
+	S.vsums = c.take<unsigned>(nblocks);
+	S.tsums = c.take<unsigned>(nblocks);
+	S.voff = c.take<unsigned long long>(nblocks);
+	S.toff = c.take<unsigned long long>(nblocks);
+	S.totals = c.take<unsigned long long>(2);
 	return S;
 }
 
@@ -564,13 +562,13 @@ extern "C" int tw_voxel_outside(tw_ctx *ctx, const float *vals, const tw_voxel_p
 	int rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz, nxy = (size_t)vp->nx*vp->ny;
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_z = (zix_xy && tw_is_device_ptr(zix_xy));
-	size_t const vb = (n*sizeof(float) + 255) & ~(size_t)255, ob = (n + 255) & ~(size_t)255, zb = (nxy*sizeof(unsigned) + 255) & ~(size_t)255;
-	rc = tw_reserve(ctx, 0, (dev_v ? 0 : vb) + (dev_o ? 0 : ob) + ((zix_xy && !dev_z) ? zb : 0) + 256); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0];
-	const float *d_v = vals; uint8_t *d_o = outside; const unsigned *d_z = zix_xy;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(sp, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_v = (const float *)sp; sp += vb;}
-	if (!dev_o) {d_o = (uint8_t *)sp; sp += ob;}
-	if (zix_xy && !dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(sp, zix_xy, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream)); d_z = (const unsigned *)sp;}
+	float *s_v = nullptr; uint8_t *d_o = outside; unsigned *s_z = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		if (!dev_v) {s_v = c.take<float>(n);} if (!dev_o) {d_o = c.take<uint8_t>(n);} if (zix_xy && !dev_z) {s_z = c.take<unsigned>(nxy);}
+	}); if (rc) return rc;
+	const float *d_v = dev_v ? vals : s_v; const unsigned *d_z = s_z ? s_z : zix_xy;
+	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(s_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	if (s_z) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zix_xy, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));}
 	outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(d_v, *vp, d_z, d_o, n);
 	TW_LAUNCH_CHECK(ctx);
 	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(outside, d_o, n, cudaMemcpyDeviceToHost, ctx->stream));}
@@ -592,15 +590,13 @@ extern "C" int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *ou
 	bool const stage_o = !dev_o || (n & 3);
 	unsigned blocks = 0;
 	rc = flood_blocks(ctx, &blocks); if (rc) return rc;
-	size_t const vb = al256(n*sizeof(float)), ob = al256(n + 4), fb = al256((n + 16)*sizeof(unsigned));
-	rc = tw_reserve(ctx, 0, (dev_v ? 0 : vb) + (stage_o ? ob : 0) + 2*fb + 512); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0];
-	float *d_v = vals; unsigned char *d_o = outside;
-	if (!dev_v) {d_v = (float *)sp; sp += vb; TW_CUDA(ctx, cudaMemcpyAsync(d_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (stage_o) {d_o = (unsigned char *)sp; sp += ob; TW_CUDA(ctx, cudaMemcpyAsync(d_o, outside, n, dev_o ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));}
-	unsigned *f0 = (unsigned *)sp, *f1 = (unsigned *)(sp + fb); sp += 2*fb;
-	unsigned *cnt = (unsigned *)sp;
-	unsigned long long *d_changed = (unsigned long long *)(sp + 64);
+	float *d_v = vals; unsigned char *d_o = outside; unsigned *f0, *f1, *cnt; unsigned long long *d_changed;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		if (!dev_v) {d_v = c.take<float>(n);} if (stage_o) {d_o = c.take<unsigned char>(n + 4);} f0 = c.take<unsigned>(n + 16); f1 = c.take<unsigned>(n + 16);
+		cnt = c.take<unsigned>(8); d_changed = c.take<unsigned long long>(1);
+	}); if (rc) return rc;
+	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	if (stage_o) {TW_CUDA(ctx, cudaMemcpyAsync(d_o, outside, n, dev_o ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));}
 	TW_CUDA(ctx, cudaMemsetAsync(d_changed, 0, sizeof(unsigned long long), ctx->stream));
 	rc = enqueue_remove_unconnected(ctx, blocks, d_v, d_o, vp, f0, f1, cnt, d_changed);
 	if (rc) {cudaStreamSynchronize(ctx->stream); return rc;}
@@ -623,22 +619,19 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_t = (tris && tw_is_device_ptr(tris));
-	size_t const vb = (n*sizeof(float) + 255) & ~(size_t)255, ob = (n + 255) & ~(size_t)255, tb = 256*4 + 256*16*4 + 24*4 + 256;
-	size_t const sb = ((size_t)nblocks*sizeof(unsigned) + 255) & ~(size_t)255, ofb = ((size_t)nblocks*sizeof(unsigned long long) + 255) & ~(size_t)255;
-	rc = tw_reserve(ctx, 0, (dev_v ? 0 : vb) + (dev_o ? 0 : ob) + tb + sb + ofb + 512); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0];
-	const float *d_v = vals; const unsigned char *d_o = outside;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(sp, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_v = (const float *)sp; sp += vb;}
-	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(sp, outside, n, cudaMemcpyHostToDevice, ctx->stream)); d_o = (const unsigned char *)sp; sp += ob;}
+	float *s_v = nullptr; unsigned char *s_o = nullptr, *sp; unsigned *d_sums; unsigned long long *d_offsets, *d_total;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		if (!dev_v) {s_v = c.take<float>(n);} if (!dev_o) {s_o = c.take<unsigned char>(n);} sp = c.take<unsigned char>(1024 + 16384 + 96);
+		d_sums = c.take<unsigned>(nblocks); d_offsets = c.take<unsigned long long>(nblocks); d_total = c.take<unsigned long long>(1);
+	}); if (rc) return rc;
+	const float *d_v = dev_v ? vals : s_v; const unsigned char *d_o = dev_o ? outside : s_o;
+	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(s_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(s_o, outside, n, cudaMemcpyHostToDevice, ctx->stream));}
 	McTables T;
 	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384);
 	TW_CUDA(ctx, cudaMemcpyAsync(sp, edge_table256, 1024, cudaMemcpyDefault, ctx->stream));
 	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024, tri_table256x16, 16384, cudaMemcpyDefault, ctx->stream));
 	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024 + 16384, edge_to_vals12x2, 96, cudaMemcpyDefault, ctx->stream));
-	sp += tb;
-	unsigned *d_sums = (unsigned *)sp; sp += sb;
-	unsigned long long *d_offsets = (unsigned long long *)sp; sp += ofb;
-	unsigned long long *d_total = (unsigned long long *)sp;
 	mc_kernel<false><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, *vp, T, n, d_sums, nullptr, nullptr, 0);
 	TW_LAUNCH_CHECK(ctx);
 	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(d_sums, nblocks, d_offsets, d_total);
@@ -687,19 +680,18 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside);
-	size_t const vb = dev_v ? 0 : al256(n*sizeof(float)), ob = dev_o ? 0 : al256(n), tb = al256(1024 + 16384 + 96);
-	rc = tw_reserve(ctx, 0, vb + ob + tb + mesh_scratch_bytes(n, nblocks)); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0];
-	const float *d_v = vals; const unsigned char *d_o = outside;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(sp, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_v = (const float *)sp; sp += vb;}
-	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(sp, outside, n, cudaMemcpyHostToDevice, ctx->stream)); d_o = (const unsigned char *)sp; sp += ob;}
+	float *s_v = nullptr; unsigned char *s_o = nullptr, *sp; MeshScratch S;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		if (!dev_v) {s_v = c.take<float>(n);} if (!dev_o) {s_o = c.take<unsigned char>(n);} sp = c.take<unsigned char>(1024 + 16384 + 96); S = mesh_scratch(c, n, nblocks);
+	}); if (rc) return rc;
+	const float *d_v = dev_v ? vals : s_v; const unsigned char *d_o = dev_o ? outside : s_o;
+	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(s_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(s_o, outside, n, cudaMemcpyHostToDevice, ctx->stream));}
 	McTables T;
 	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384);
 	TW_CUDA(ctx, cudaMemcpyAsync(sp, edge_table256, 1024, cudaMemcpyDefault, ctx->stream));
 	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024, tri_table256x16, 16384, cudaMemcpyDefault, ctx->stream));
 	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024 + 16384, edge_to_vals12x2, 96, cudaMemcpyDefault, ctx->stream));
-	sp += tb;
-	MeshScratch const S = mesh_scratch(sp, n, nblocks);
 	// count and scan first: the emit pass writes at most min(count, capacity) of each, so host outputs are staged at that size
 	rc = enqueue_mesh(ctx, d_v, d_o, *vp, T, S, nullptr, 0, nullptr, 0); if (rc) return rc;
 	unsigned long long tot[2] = {0, 0};
@@ -709,10 +701,10 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
 	uint64_t const nv = (tot[0] < M.vcapacity) ? tot[0] : M.vcapacity, nt = (tot[1] < M.tcapacity) ? tot[1] : M.tcapacity;
 	if (nv == 0 && nt == 0) return TW_OK;
 	bool const dev_vt = nv && tw_is_device_ptr(M.verts), dev_ix = nt && tw_is_device_ptr(M.indices);
-	size_t const svb = dev_vt ? 0 : al256((size_t)nv*12), sib = dev_ix ? 0 : al256((size_t)nt*12);
-	if (svb + sib) {rc = tw_reserve(ctx, 1, svb + sib); if (rc) return rc;}
-	float *d_vt = dev_vt ? M.verts : (float *)ctx->d_scratch[1];
-	uint32_t *d_ix = dev_ix ? M.indices : (uint32_t *)((char *)ctx->d_scratch[1] + svb);
+	float *d_vt = M.verts; uint32_t *d_ix = M.indices;
+	rc = twi_reserve_carve(ctx, 1, [&](twi_carve &c) {
+		if (!dev_vt) {d_vt = c.take<float>((size_t)nv*3);} if (!dev_ix) {d_ix = c.take<uint32_t>((size_t)nt*3);}
+	}); if (rc) return rc;
 	mesh_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, *vp, T, n, S.words, nullptr, nullptr, S.voff, S.toff, d_vt, nv, d_ix, nt);
 	TW_LAUNCH_CHECK(ctx);
 	if (nv && !dev_vt) {TW_CUDA(ctx, cudaMemcpyAsync(M.verts, d_vt, (size_t)nv*12, cudaMemcpyDeviceToHost, ctx->stream));}
@@ -725,9 +717,9 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
 // fill (optional) -> outside -> remove_unconnected -> marching cubes (count, block scan, emit with the caller's capacity) on ctx->stream; nothing is read back
 // before the end: the triangle count and the flipped voxels go to pinned staging that the completing poll unpacks. Every buffer is reserved before anything is
 // enqueued, so no re-allocation synchronises in the middle.
-//   device slot 0: [counters (256 B) | field (unless vals is device memory) | padded flags | 2 frontiers (remove_unconnected > 0) | tables | block sums | block
+//   device slot 0: [counters | field (unless vals is device memory) | padded flags | 2 frontiers (remove_unconnected > 0) | tables | block sums | block
 //                  offsets | zix_xy (host input)]
-//   pinned:        [twi_voxel_stage (64 B) | sine coefficients | tables | zix_xy (host input)]
+//   pinned:        [twi_voxel_stage | sine coefficients | tables | zix_xy (host input)]
 //   with a welded mesh, device slot 0 ends with the mesh's scratch (mesh_scratch)
 extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {return tw_voxel_build_launch_ex(ctx, b, nullptr);}
 
@@ -777,45 +769,48 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
 	bool const dev_v = b->vals && tw_is_device_ptr(b->vals), dev_z = b->zix_xy && tw_is_device_ptr(b->zix_xy);
 	size_t const TAB = 1024 + 16384 + 96;
-	bool const tabs = (ntab == 3);
-	size_t const vb = dev_v ? 0 : al256(n*sizeof(float)), ob = al256(n + 4), fb = rm ? al256((n + 16)*sizeof(unsigned)) : 0, tb = tabs ? al256(TAB) : 0;
-	size_t const sb = mc ? al256((size_t)nblocks*sizeof(unsigned)) : 0, ofb = mc ? al256((size_t)nblocks*sizeof(unsigned long long)) : 0;
-	size_t const zb = (b->zix_xy && !dev_z) ? al256(nxy*sizeof(unsigned)) : 0, mb = wm ? mesh_scratch_bytes(n, nblocks) : 0;
-	rc = tw_reserve(ctx, 0, 256 + vb + ob + 2*fb + tb + sb + ofb + zb + mb); if (rc) return rc;
-	if (tab_bytes) {rc = tw_reserve(ctx, 1, tab_bytes); if (rc) return rc;}
-	size_t const off_rdata = 64, off_tab = off_rdata + al256(TW_N3D_RDATA*sizeof(float)), off_zix = off_tab + (tabs ? al256(TAB) : 0);
-	rc = tw_reserve_pinned(ctx, off_zix + zb); if (rc) return rc;
-	if (fill && F.gen_mode != TW_MGEN_SINE) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
-	char *sp = (char *)ctx->d_scratch[0], *h = (char *)ctx->h_pinned;
-	unsigned *cnt = (unsigned *)sp;
-	unsigned long long *d_changed = (unsigned long long *)(sp + 64), *d_total = (unsigned long long *)(sp + 128);
-	sp += 256;
-	float *d_v = dev_v ? b->vals : (float *)sp; sp += vb;
-	unsigned char *d_o = (unsigned char *)sp; sp += ob;
-	unsigned *f0 = (unsigned *)sp, *f1 = (unsigned *)(sp + fb); sp += 2*fb;
-	McTables T;
-	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384); sp += tb;
-	unsigned *d_sums = (unsigned *)sp; sp += sb;
-	unsigned long long *d_offsets = (unsigned long long *)sp; sp += ofb;
-	const unsigned *d_z = dev_z ? b->zix_xy : (b->zix_xy ? (const unsigned *)sp : nullptr); sp += zb;
+	bool const tabs = (ntab == 3), stage_z = (b->zix_xy && !dev_z);
+	unsigned *cnt, *f0 = nullptr, *f1 = nullptr, *d_sums = nullptr, *s_z = nullptr;
+	float *d_v = b->vals;
+	unsigned char *d_o, *tab = nullptr;
+	unsigned long long *d_offsets = nullptr;
 	MeshScratch S;
-	if (wm) {S = mesh_scratch(sp, n, nblocks);}
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		cnt = c.take<unsigned>(64); // [flood counters | changed at byte 64 | triangle total at byte 128], zeroed together
+		if (!dev_v) {d_v = c.take<float>(n);}
+		d_o = c.take<unsigned char>(n + 4);
+		if (rm) {f0 = c.take<unsigned>(n + 16); f1 = c.take<unsigned>(n + 16);}
+		if (tabs) {tab = c.take<unsigned char>(TAB);}
+		if (mc) {d_sums = c.take<unsigned>(nblocks); d_offsets = c.take<unsigned long long>(nblocks);}
+		if (stage_z) {s_z = c.take<unsigned>(nxy);}
+		if (wm) S = mesh_scratch(c, n, nblocks);
+	}); if (rc) return rc;
+	if (tab_bytes) {rc = tw_reserve(ctx, 1, tab_bytes); if (rc) return rc;}
+	twi_voxel_stage *st; float *h_rdata; unsigned char *h_tab = nullptr; unsigned *h_z = nullptr;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
+		st = c.take<twi_voxel_stage>(1); h_rdata = c.take<float>(TW_N3D_RDATA); if (tabs) {h_tab = c.take<unsigned char>(TAB);} if (stage_z) {h_z = c.take<unsigned>(nxy);}
+	}); if (rc) return rc;
+	if (fill && F.gen_mode != TW_MGEN_SINE) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
+	unsigned long long *d_changed = (unsigned long long *)(cnt + 16), *d_total = (unsigned long long *)(cnt + 32);
+	McTables T = {};
+	if (tabs) {T.edge_table = (const unsigned *)tab; T.tri_table = (const int *)(tab + 1024); T.edge_to_vals = (const unsigned *)(tab + 1024 + 16384);}
+	const unsigned *d_z = dev_z ? b->zix_xy : s_z;
 	twi_job pending;
 	pending.kind = twi_job::VOXEL; pending.host_ntris = mc ? b->ntris : nullptr; pending.host_changed = b->changed; pending.cancellable = true;
 	pending.host_mesh_nverts = M.nverts; pending.host_mesh_ntris = M.ntris;
 	return twi_launch_job(ctx, pending, [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(cnt, 0, 256, ctx->stream));
-		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h + off_rdata); if (r) return r;}
+		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h_rdata); if (r) return r;}
 		else if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, b->vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-		if (zb) {memcpy(h + off_zix, b->zix_xy, nxy*sizeof(unsigned)); TW_CUDA(ctx, cudaMemcpyAsync((void *)d_z, h + off_zix, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));}
+		if (stage_z) {memcpy(h_z, b->zix_xy, nxy*sizeof(unsigned)); TW_CUDA(ctx, cudaMemcpyAsync(s_z, h_z, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));}
 		if (tabs) {
 			const void *src[3] = {b->edge_table256, b->tri_table256x16, b->edge_to_vals12x2};
 			size_t const off[3] = {0, 1024, 1024 + 16384}, len[3] = {1024, 16384, 96};
 			for (int k = 0; k < 3; ++k) {
 				// host tables are copied during the launch; device tables are read by the job
-				if (tw_is_device_ptr(src[k])) {TW_CUDA(ctx, cudaMemcpyAsync((char *)T.edge_table + off[k], src[k], len[k], cudaMemcpyDeviceToDevice, ctx->stream)); continue;}
-				memcpy(h + off_tab + off[k], src[k], len[k]);
-				TW_CUDA(ctx, cudaMemcpyAsync((char *)T.edge_table + off[k], h + off_tab + off[k], len[k], cudaMemcpyHostToDevice, ctx->stream));
+				if (tw_is_device_ptr(src[k])) {TW_CUDA(ctx, cudaMemcpyAsync(tab + off[k], src[k], len[k], cudaMemcpyDeviceToDevice, ctx->stream)); continue;}
+				memcpy(h_tab + off[k], src[k], len[k]);
+				TW_CUDA(ctx, cudaMemcpyAsync(tab + off[k], h_tab + off[k], len[k], cudaMemcpyHostToDevice, ctx->stream));
 			}
 		}
 		outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(d_v, P, d_z, d_o, n);
@@ -834,7 +829,6 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 		if (wm) {int const r = enqueue_mesh(ctx, d_v, d_o, P, T, S, d_mv, M.vcapacity, d_mi, M.tcapacity); if (r) return r;}
 		if (b->vals && !dev_v && (fill || rm)) {TW_CUDA(ctx, cudaMemcpyAsync(b->vals, d_v, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 		if (b->outside) {TW_CUDA(ctx, cudaMemcpyAsync(b->outside, d_o, n, cudaMemcpyDefault, ctx->stream));}
-		twi_voxel_stage *const st = (twi_voxel_stage *)h;
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->ntris, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->changed, d_changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		if (wm) {TW_CUDA(ctx, cudaMemcpyAsync(&st->nverts, S.totals, 2*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));}
@@ -1039,25 +1033,23 @@ McTables model_tables(const tw_voxel_model *m) {
 	return T;
 }
 
-// A model job's slot-0 scratch: [counters (64 B) | changed (64 B) | pad to 256 | frontiers (remove_unconnected > 0) | mesh scratch | table | boxes | values]
-// and pinned staging: [twi_vmodel_stage (64 B) | table | boxes | values | fill coefficients]
+// A model job's slot-0 scratch: [counters (changed at byte 64), zeroed together | frontiers (remove_unconnected > 0) | mesh scratch | table | boxes | values]
+// and pinned staging: [twi_vmodel_stage (64 B), then the table | boxes | values | fill coefficients]
 struct ModelScratch {unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values; char *h_boxes, *h_values, *h_rdata;};
 int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X) {
 	tw_ctx *ctx = m->ctx;
 	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz, ng = (size_t)m->nblocks*m->chunks;
-	size_t const fb = (m->P.remove_unconnected > 0) ? al256((n + 16)*sizeof(unsigned)) : 0, mb = mesh_scratch_bytes(ng*MC_BLOCK, (unsigned)ng);
-	size_t const tb = al256((size_t)m->nblocks*sizeof(tw_voxel_block_mesh)), bb = al256(nboxes*sizeof(twi_box)), vb = al256(nvalues*sizeof(float));
-	size_t const rb = al256(TW_N3D_RDATA*sizeof(float));
-	int rc = tw_reserve(ctx, 0, 256 + 2*fb + mb + tb + bb + vb); if (rc) return rc;
-	rc = tw_reserve_pinned(ctx, 64 + tb + bb + vb + rb); if (rc) return rc;
-	char *sp = (char *)ctx->d_scratch[0], *h = (char *)ctx->h_pinned;
-	X->cnt = (unsigned *)sp; X->changed = (unsigned long long *)(sp + 64); sp += 256;
-	X->f0 = (unsigned *)sp; X->f1 = (unsigned *)(sp + fb); sp += 2*fb;
-	X->S = mesh_scratch(sp, ng*MC_BLOCK, (unsigned)ng); sp += mb;
-	X->table = (tw_voxel_block_mesh *)sp; sp += tb;
-	X->boxes = (twi_box *)sp; sp += bb;
-	X->values = (float *)sp;
-	X->h_boxes = h + 64 + tb; X->h_values = X->h_boxes + bb; X->h_rdata = X->h_values + vb;
+	X->f0 = X->f1 = nullptr;
+	int rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		X->cnt = c.take<unsigned>(64); if (m->P.remove_unconnected > 0) {X->f0 = c.take<unsigned>(n + 16); X->f1 = c.take<unsigned>(n + 16);}
+		X->S = mesh_scratch(c, ng*MC_BLOCK, (unsigned)ng); X->table = c.take<tw_voxel_block_mesh>(m->nblocks); X->boxes = c.take<twi_box>(nboxes);
+		X->values = c.take<float>(nvalues);
+	}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
+		c.take<char>(64 + (size_t)m->nblocks*sizeof(tw_voxel_block_mesh)); X->h_boxes = c.take<char>(nboxes*sizeof(twi_box));
+		X->h_values = c.take<char>(nvalues*sizeof(float)); X->h_rdata = c.take<char>(TW_N3D_RDATA*sizeof(float));
+	}); if (rc) return rc;
+	X->changed = (unsigned long long *)(X->cnt + 16);
 	return TW_OK;
 }
 
@@ -1130,24 +1122,25 @@ extern "C" int tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp
 	if (3ull*(bw + 1)*(bh + 1)*P.nz >= 0x100000000ull) return tw_set_error(ctx, TW_ERR_ARG, "a block's indices are 32-bit: 3*(bx+1)*(by+1)*nz must be below 2^32");
 	size_t const n = (size_t)P.nx*P.ny*P.nz, nxy = (size_t)P.nx*P.ny;
 	unsigned const nbx = (ncx + bx - 1)/bx, nby = (ncy + by - 1)/by, nblocks = nbx*nby;
-	size_t const fb = al256(n*sizeof(float)), ob = al256(n + 4), zb = zix_xy ? al256(nxy*sizeof(unsigned)) : 0, tb = al256(1024 + 16384 + 96);
-	size_t const mkb = al256(nblocks + 1), lb = al256(((size_t)nblocks + 1)*sizeof(unsigned));
 	tw_voxel_model *m = new (std::nothrow) tw_voxel_model();
 	if (!m) return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");
 	try {ctx->models.push_back(m);} catch (...) {delete m; return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");}
 	m->ctx = ctx; m->P = P; m->bx = bx; m->by = by; m->nbx = nbx; m->nblocks = nblocks; m->chunks = (unsigned)(((size_t)bw*bh*P.nz + MC_BLOCK - 1)/MC_BLOCK);
 	m->have_zix = (zix_xy != nullptr);
-	if (cudaMalloc(&m->mem, 3*fb + 3*ob + zb + tb + mkb + 2*lb) != cudaSuccess) {
+	auto layout = [&](twi_carve &c) {
+		m->raw = c.take<float>(n); m->post = c.take<float>(n); m->work = c.take<float>(n);
+		m->raw_o = c.take<unsigned char>(n + 4); m->post_o = c.take<unsigned char>(n + 4); m->work_o = c.take<unsigned char>(n + 4);
+		m->zix = zix_xy ? c.take<unsigned>(nxy) : nullptr; m->tables = c.take<char>(1024 + 16384 + 96); m->mark = c.take<unsigned char>((size_t)nblocks + 1);
+		m->all = c.take<unsigned>((size_t)nblocks + 1); m->marked = c.take<unsigned>((size_t)nblocks + 1);
+	};
+	twi_carve c;
+	layout(c);
+	if (cudaMalloc(&m->mem, c.bytes) != cudaSuccess) {
 		cudaGetLastError(); m->mem = nullptr; tw_voxel_model_destroy(m);
 		return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: no device memory for %zu voxels", n);
 	}
-	char *p = m->mem;
-	m->raw = (float *)p; p += fb; m->post = (float *)p; p += fb; m->work = (float *)p; p += fb;
-	m->raw_o = (unsigned char *)p; p += ob; m->post_o = (unsigned char *)p; p += ob; m->work_o = (unsigned char *)p; p += ob;
-	m->zix = zix_xy ? (unsigned *)p : nullptr; p += zb;
-	m->tables = p; p += tb;
-	m->mark = (unsigned char *)p; p += mkb;
-	m->all = (unsigned *)p; p += lb; m->marked = (unsigned *)p;
+	c = twi_carve{m->mem};
+	layout(c);
 	std::vector<unsigned> all((size_t)nblocks + 1);
 	all[0] = nblocks;
 	for (unsigned b = 0; b < nblocks; ++b) {all[1 + b] = b;}

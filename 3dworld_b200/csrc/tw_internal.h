@@ -5,44 +5,20 @@
 #include <stddef.h>
 #include <stdio.h>
 #include <string.h>
+#include <functional>
 #include <utility>
 #include <vector>
 #include "../../include/tw3d.h"
 
-// A voxel build's counts in ctx->h_pinned (tw_voxel_build_launch)
-struct twi_voxel_stage {unsigned long long ntris, changed, nverts, mesh_ntris;}; // nverts, mesh_ntris: the welded mesh (tw_voxel_build_launch_ex)
-// A voxel model job's counts in ctx->h_pinned, followed at byte 64 by the listed blocks' tw_voxel_block_mesh entries (tw_voxel_model_*_launch)
-struct twi_vmodel_stage {unsigned long long nblocks, nverts, ntris, changed;};
-
-// The one asynchronous job a context may have in flight, as the poll that reports its completion unpacks it: which kind it is, what it staged in
-// ctx->h_pinned and where that goes. A job is pending when its kind is not NONE. Only twi_launch_job makes a job pending and only poll_job (tw_api.cu)
-// takes it back.
+// The one asynchronous job a context may have in flight. Its launch supplies `complete`, which unpacks what that launch staged in ctx->h_pinned into the
+// caller's outputs and returns the status of the completed work; it captures by value the destinations and the pinned regions it reads. The poll that sees
+// the job done calls it, unless a cancellation point acted. A job is pending while it has a completion (a relight, which stages nothing, has an empty one).
+// Only twi_launch_job makes a job pending and only poll_job (tw_api.cu) takes it back.
 struct twi_job {
-	enum kind_t {NONE, TILES, VOXEL, HMAP, VMODEL};
-	kind_t kind = NONE;
+	std::function<int(tw_ctx *)> complete;
 	bool cancellable = false;             // tw_cancel may stop it (set by the launch; a job that touches a tile set or a voxel model is not)
 	bool reads_image = false;             // it reads or writes the family's heightmap image: its work waits for the edits made before its launch (tw_update_heightmap)
 	unsigned seq = 0;                     // the context's number of the job (twi_launch_job), the one tw_cancel names
-	// TILES (tile jobs and frames; a 2-D grid is n = 1 with its min/max at offset 0; a relight stages nothing): n tiles' results at byte offsets into
-	// ctx->h_pinned, each unpacked only when its destination is set
-	uint32_t n = 0;
-	uint64_t *host_steps = nullptr;       // the erosion step count (&ctx->last_erosion_steps when the job eroded)
-	tw_minmax *host_mm = nullptr;
-	tw_tile_bounds *host_bounds = nullptr;
-	float *host_min_nz = nullptr;
-	uint8_t *host_flags = nullptr;        // has_any_grass
-	float dx = 0.0f, dy = 0.0f;           // what the bounds combination needs
-	uint32_t size = 0;
-	size_t off_steps = 0, off_mm = 0, off_sub = 0, off_min_nz = 0, off_flags = 0;
-	// VOXEL: a twi_voxel_stage at ctx->h_pinned
-	uint64_t *host_ntris = nullptr, *host_changed = nullptr, *host_mesh_nverts = nullptr, *host_mesh_ntris = nullptr;
-	// VMODEL: a twi_vmodel_stage at ctx->h_pinned; host_mesh_nverts / host_mesh_ntris / host_changed take its counts
-	tw_voxel_block_mesh *host_blocks = nullptr;
-	uint32_t *host_nblocks = nullptr;
-	// HMAP (tw_proc_gen_heightmap_launch; tw_erode_launch, which fills only the stage's min_z, bad, fail and steps and has no host_info): a twi_hmap_stage at
-	// ctx->h_pinned
-	tw_heightmap_info *host_info = nullptr;
-	int image_w = 0, image_h = 0;         // > 0: the packed image becomes (again) the context's tw_set_heightmap image when the job completes
 };
 
 // One edit's staging (tw_update_heightmap): pinned host memory and device memory of `bytes` each, holding [row table | packed texels], reused once `ev` (recorded
@@ -134,6 +110,8 @@ struct tw_ctx {
 };
 
 int  tw_set_error(tw_ctx *ctx, int status, const char *fmt, ...);
+int  twi_begin(tw_ctx *ctx);                                    // an entry point's prologue: TW_ERR_ARG for a null ctx, else its device made current, its
+                                                                // parent's tables borrowed and its pending job completed (twi_finish_pending)
 int  twi_finish_pending(tw_ctx *ctx);                           // completes the context's pending asynchronous job (if any) before other work reuses its scratch
 void twi_borrow_tables(tw_ctx *ctx);                            // a shared context takes its parent's current tables (no-op on any other context)
 int  twi_ensure_simplex_lut(tw_ctx *ctx);                       // builds ctx->d_simplex_lut on ctx->stream if absent (tw_heightgen.cu)
@@ -183,7 +161,7 @@ int twi_hmap_scatter(tw_ctx *ctx, cudaStream_t st, const twi_hmap_row *d_rows, u
 // joined into ctx->stream, between the job's start and end in the device words, and ctx->async.done is recorded behind it. When any step fails, the call
 // waits for every stream of the context, so none of the job still runs on the scratch or the pinned staging when the error is returned, and no job is pending.
 // A job that reads or writes the image (job.reads_image) first waits on the device for the edits made before its launch.
-template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, const twi_job &job, Enqueue &&enqueue) {
+template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, twi_job job, Enqueue &&enqueue) {
 	unsigned seq = 0;
 	int rc = job.reads_image ? twi_wait_image_edits(ctx) : TW_OK;
 	if (rc == TW_OK) {rc = twi_job_start(ctx, &seq);}
@@ -201,7 +179,7 @@ template <typename Enqueue> int twi_launch_job(tw_ctx *ctx, const twi_job &job, 
 		for (cudaStream_t s : ctx->heavy_stream) {if (s) cudaStreamSynchronize(s);}
 		return rc;
 	}
-	ctx->async.job = job;
+	ctx->async.job = std::move(job);
 	ctx->async.job.seq = seq;
 	return TW_OK;
 }

@@ -122,8 +122,7 @@ extern "C" int tw_dist_allreduce_minmax(tw_ctx *ctx, tw_minmax *inout) {
 	if (!d) return tw_set_error(ctx, TW_ERR_STATE, "tw_dist_init() has not been called");
 	std::string err;
 	NcclApi *N = nccl_api(err);
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int const rc = twi_begin(ctx); if (rc) return rc;
 	float h[2] = {-inout->zmin, inout->zmax}; // one MAX reduction gives both ends of the range
 	TW_CUDA(ctx, cudaMemcpyAsync(d->d_buf, h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
 	ncclResult_t const r = N->AllReduce(d->d_buf, d->d_buf, 2, ncclFloat, ncclMax, d->comm, ctx->stream);
@@ -466,8 +465,7 @@ extern "C" int tw_erode_sweeps(tw_ctx *ctx, float *heightmap, int xsize, int ysi
                                uint32_t sweep, int halo, uint64_t *moves)
 {
 	if (!ctx || !heightmap || !p) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int const rc = twi_begin(ctx); if (rc) return rc;
 	float *bands[1] = {heightmap};
 	tw_ctx *ctxs[1] = {ctx};
 	return erode_sweeps_core(1, ctxs, nullptr, bands, xsize, ysize, min_zval, num_iters, p, sweep, halo, moves, ctx->err, sizeof(ctx->err));
@@ -477,8 +475,7 @@ extern "C" int tw_erode_sweeps_banded(tw_ctx *ctx, float *const *bands, int nban
                                       uint32_t sweep, int halo, uint64_t *moves)
 {
 	if (!ctx || !bands || !p || nbands < 1 || nbands > 1024) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int const rc = twi_begin(ctx); if (rc) return rc;
 	std::vector<tw_ctx *> ctxs((size_t)nbands, ctx);
 	return erode_sweeps_core(nbands, ctxs.data(), nullptr, bands, xsize, ysize, min_zval, num_iters, p, sweep, halo, moves, ctx->err, sizeof(ctx->err));
 }

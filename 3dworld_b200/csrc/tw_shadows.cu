@@ -229,8 +229,7 @@ static int tile_shadows(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy,
                         const float *sh_in_y, uint8_t *smask, float *sh_out_x, float *sh_out_y, bool ex)
 {
 	if (!ctx || !zvals || !tile_xy || !sp || !smask || ntiles == 0 || zvsize < 2) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!ex && ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
 	size_t const cells = (size_t)ntiles*zvsize*zvsize, edge = (size_t)ntiles*zvsize;
 	twi_shadow_plan P;
@@ -238,7 +237,7 @@ static int tile_shadows(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy,
 	bool const dev_z = tw_is_device_ptr(zvals), dev_m = tw_is_device_ptr(smask);
 	if (dev_m && ((size_t)smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)");
 	float *s_z = nullptr, *d_ox, *d_oy; unsigned char *d_m = smask; unsigned long long *d_keys; int *d_plan;
-	int rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
 		if (!dev_z) {s_z = c.take<float>(cells);} if (!dev_m) {d_m = c.take<unsigned char>(cells + 4);} d_keys = c.take<unsigned long long>(2*edge);
 		d_ox = c.take<float>((sh_in_x ? 2 : 1)*edge); d_oy = c.take<float>((sh_in_y ? 2 : 1)*edge); d_plan = c.take<int>(twi_shadow_plan_ints(ntiles));
 	}); if (rc) return rc;

@@ -59,11 +59,6 @@ int copy_tiles(tw_ctx *ctx, void *dst, const int *dst_idx, const void *src, cons
 	return TW_OK;
 }
 
-int begin_call(tw_tile_set *s) { // the context's device, its tables, and its pending job completed
-	TW_CUDA(s->ctx, cudaSetDevice(s->ctx->device));
-	return twi_finish_pending(s->ctx);
-}
-
 // unique keys of n (x, y) pairs, or false when one is named twice
 bool read_keys(const int32_t *tile_xy, uint32_t n, std::vector<twts::key> &keys) {
 	keys.resize(n);
@@ -372,7 +367,7 @@ int tw_tile_set_put(tw_tile_set *s, const int32_t *tile_xy, uint32_t n, const fl
 	if (!tile_xy || !zvals || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "tile set put: null or empty argument");
 	std::vector<twts::key> keys;
 	if (!read_keys(tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set put: tile_xy names a tile twice");
-	int rc = begin_call(s); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
 	std::vector<uint32_t> free_left;
 	std::vector<int> idx;
 	uint32_t const next = twts::put_slots(s->st, keys, free_left, idx);
@@ -398,7 +393,7 @@ int tw_tile_set_remove(tw_tile_set *s, const int32_t *tile_xy, uint32_t n) {
 	std::vector<twts::key> keys;
 	if (!read_keys(tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set remove: tile_xy names a tile twice");
 	for (twts::key const &k : keys) {if (!s->st.where.count(k)) return tw_set_error(ctx, TW_ERR_ARG, "tile set remove: tile (%d, %d) is not resident", k.first, k.second);}
-	int rc = begin_call(s); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
 	// host state only: the next writer of a freed slot waits on the set's event
 	twts::remove_tiles(s->st, keys, slot_signs(s));
 	return TW_OK;
@@ -437,9 +432,9 @@ int tw_tile_set_shadows_launch(tw_tile_set *s, const tw_tile_set_request *req) {
 	// everything is reserved before anything is enqueued (tw_reserve synchronises the stream and may re-allocate)
 	rc = tw_reserve(ctx, 0, R.dev_bytes()); if (rc) return rc;
 	rc = tw_reserve_pinned(ctx, R.ints_bytes); if (rc) return rc;
-	twi_job pending; // a relight stages nothing for the poll
-	pending.kind = twi_job::TILES;
-	rc = twi_launch_job(ctx, pending, [&]() -> int {
+	twi_job pending;
+	pending.complete = [](tw_ctx *) {return TW_OK;}; // a relight stages nothing for the poll
+	rc = twi_launch_job(ctx, std::move(pending), [&]() -> int {
 		TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0)); // a frame's job on another context may still use the slabs
 		return relight_enqueue(ctx, s, R, (char *)ctx->d_scratch[0], (char *)ctx->h_pinned);
 	});

@@ -557,9 +557,8 @@ int enqueue_remove_unconnected(tw_ctx *ctx, unsigned blocks, float *d_v, unsigne
 
 extern "C" int tw_voxel_outside(tw_ctx *ctx, const float *vals, const tw_voxel_post_params *vp, const uint32_t *zix_xy, uint8_t *outside) {
 	if (!ctx || !vals || !outside) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
-	int rc = validate(ctx, vp); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
+	rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz, nxy = (size_t)vp->nx*vp->ny;
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_z = (zix_xy && tw_is_device_ptr(zix_xy));
 	float *s_v = nullptr; uint8_t *d_o = outside; unsigned *s_z = nullptr;
@@ -578,9 +577,8 @@ extern "C" int tw_voxel_outside(tw_ctx *ctx, const float *vals, const tw_voxel_p
 
 extern "C" int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *outside, const tw_voxel_post_params *vp, uint64_t *changed) {
 	if (!ctx || !vals || !outside) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
-	int rc = validate(ctx, vp); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
+	rc = validate(ctx, vp); if (rc) return rc;
 	if (changed) *changed = 0;
 	if (vp->remove_unconnected <= 0) return TW_OK;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
@@ -613,9 +611,8 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
                                   const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, float *tris, uint64_t capacity, uint64_t *ntris)
 {
 	if (!ctx || !vals || !outside || !edge_table256 || !tri_table256x16 || !edge_to_vals12x2 || !ntris || (capacity && !tris)) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
-	int rc = validate(ctx, vp); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
+	rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
 	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_t = (tris && tw_is_device_ptr(tris));
@@ -672,9 +669,8 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
                                     const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, const tw_voxel_mesh *out)
 {
 	if (!ctx || !vals || !outside || !edge_table256 || !tri_table256x16 || !edge_to_vals12x2 || !out) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
-	int rc = validate(ctx, vp); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
+	rc = validate(ctx, vp); if (rc) return rc;
 	tw_voxel_mesh const M = *out;
 	rc = validate_mesh(ctx, vp, &M); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
@@ -714,6 +710,9 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
 }
 
 // ------------------------------------------------------------------------------------------------ the whole build as one asynchronous job
+// The counts the build stages; nverts, mesh_ntris: the welded mesh (tw_voxel_build_launch_ex)
+struct twi_voxel_stage {unsigned long long ntris, changed, nverts, mesh_ntris;};
+
 // fill (optional) -> outside -> remove_unconnected -> marching cubes (count, block scan, emit with the caller's capacity) on ctx->stream; nothing is read back
 // before the end: the triangle count and the flipped voxels go to pinned staging that the completing poll unpacks. Every buffer is reserved before anything is
 // enqueued, so no re-allocation synchronises in the middle.
@@ -724,12 +723,10 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
 extern "C" int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b) {return tw_voxel_build_launch_ex(ctx, b, nullptr);}
 
 extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, const tw_voxel_mesh *mesh) {
-	if (!ctx) return TW_ERR_ARG;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
+	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!b || !b->post) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_build_launch: null argument");
 	tw_voxel_post_params const P = *b->post;
-	int rc = validate(ctx, &P); if (rc) return rc;
+	rc = validate(ctx, &P); if (rc) return rc;
 	bool const fill = (b->fill != nullptr);
 	tw_voxel_params F;
 	size_t tab_bytes = 0;
@@ -796,9 +793,14 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 	if (tabs) {T.edge_table = (const unsigned *)tab; T.tri_table = (const int *)(tab + 1024); T.edge_to_vals = (const unsigned *)(tab + 1024 + 16384);}
 	const unsigned *d_z = dev_z ? b->zix_xy : s_z;
 	twi_job pending;
-	pending.kind = twi_job::VOXEL; pending.host_ntris = mc ? b->ntris : nullptr; pending.host_changed = b->changed; pending.cancellable = true;
-	pending.host_mesh_nverts = M.nverts; pending.host_mesh_ntris = M.ntris;
-	return twi_launch_job(ctx, pending, [&]() -> int {
+	pending.cancellable = true;
+	pending.complete = [st, ntris = mc ? b->ntris : nullptr, changed = b->changed, nverts = M.nverts, mesh_ntris = M.ntris](tw_ctx *) -> int {
+		if (ntris) {*ntris = st->ntris;}
+		if (changed) {*changed = st->changed;}
+		if (nverts) {*nverts = st->nverts; *mesh_ntris = st->mesh_ntris;}
+		return TW_OK;
+	};
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(cnt, 0, 256, ctx->stream));
 		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h_rdata); if (r) return r;}
 		else if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, b->vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
@@ -1033,9 +1035,15 @@ McTables model_tables(const tw_voxel_model *m) {
 	return T;
 }
 
+// A model job's counts in its pinned staging
+struct twi_vmodel_stage {unsigned long long nblocks, nverts, ntris, changed;};
+
 // A model job's slot-0 scratch: [counters (changed at byte 64), zeroed together | frontiers (remove_unconnected > 0) | mesh scratch | table | boxes | values]
 // and pinned staging: [twi_vmodel_stage (64 B), then the table | boxes | values | fill coefficients]
-struct ModelScratch {unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values; char *h_boxes, *h_values, *h_rdata;};
+struct ModelScratch {
+	unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values;
+	twi_vmodel_stage *h_stage; tw_voxel_block_mesh *h_table; char *h_boxes, *h_values, *h_rdata;
+};
 int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X) {
 	tw_ctx *ctx = m->ctx;
 	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz, ng = (size_t)m->nblocks*m->chunks;
@@ -1045,10 +1053,12 @@ int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch
 		X->S = mesh_scratch(c, ng*MC_BLOCK, (unsigned)ng); X->table = c.take<tw_voxel_block_mesh>(m->nblocks); X->boxes = c.take<twi_box>(nboxes);
 		X->values = c.take<float>(nvalues);
 	}); if (rc) return rc;
+	char *h_head;
 	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
-		c.take<char>(64 + (size_t)m->nblocks*sizeof(tw_voxel_block_mesh)); X->h_boxes = c.take<char>(nboxes*sizeof(twi_box));
+		h_head = c.take<char>(64 + (size_t)m->nblocks*sizeof(tw_voxel_block_mesh)); X->h_boxes = c.take<char>(nboxes*sizeof(twi_box));
 		X->h_values = c.take<char>(nvalues*sizeof(float)); X->h_rdata = c.take<char>(TW_N3D_RDATA*sizeof(float));
 	}); if (rc) return rc;
+	X->h_stage = (twi_vmodel_stage *)h_head; X->h_table = (tw_voxel_block_mesh *)(h_head + 64);
 	X->changed = (unsigned long long *)(X->cnt + 16);
 	return TW_OK;
 }
@@ -1065,8 +1075,7 @@ int validate_blocks_out(tw_ctx *ctx, const tw_voxel_blocks_out *o, float **d_vt,
 // the meshes of the blocks in d_list, their table and the job's counts into the pinned stage
 int enqueue_block_meshes(tw_voxel_model *m, const unsigned *d_list, const ModelScratch &X, float *d_vt, uint64_t vcap, uint32_t *d_ix, uint64_t tcap) {
 	tw_ctx *ctx = m->ctx;
-	char *h = (char *)ctx->h_pinned;
-	twi_vmodel_stage *const st = (twi_vmodel_stage *)h;
+	twi_vmodel_stage *const st = X.h_stage;
 	if (m->nblocks) {
 		unsigned const ng = m->nblocks*m->chunks;
 		McTables const T = model_tables(m);
@@ -1086,24 +1095,25 @@ int enqueue_block_meshes(tw_voxel_model *m, const unsigned *d_list, const ModelS
 		TW_LAUNCH_CHECK(ctx);
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->nblocks, d_list, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream)); // the low word (little-endian)
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->nverts, S.totals, 2*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-		TW_CUDA(ctx, cudaMemcpyAsync(h + 64, X.table, (size_t)m->nblocks*sizeof(tw_voxel_block_mesh), cudaMemcpyDeviceToHost, ctx->stream));
+		TW_CUDA(ctx, cudaMemcpyAsync(X.h_table, X.table, (size_t)m->nblocks*sizeof(tw_voxel_block_mesh), cudaMemcpyDeviceToHost, ctx->stream));
 	}
 	TW_CUDA(ctx, cudaMemcpyAsync(&st->changed, X.changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 	return TW_OK;
 }
 
-twi_job model_job(const tw_voxel_blocks_out *o) {
+// a model job (not cancellable: it commits the model's state) whose completion unpacks X's stage and table into o
+twi_job model_job(const ModelScratch &X, const tw_voxel_blocks_out &o) {
 	twi_job j;
-	j.kind = twi_job::VMODEL; j.cancellable = false;
-	j.host_blocks = o->blocks; j.host_nblocks = o->nblocks; j.host_mesh_nverts = o->nverts; j.host_mesh_ntris = o->ntris; j.host_changed = o->changed;
+	j.complete = [st = X.h_stage, table = X.h_table, o](tw_ctx *) -> int {
+		*o.nblocks = (uint32_t)st->nblocks; *o.nverts = st->nverts; *o.ntris = st->ntris;
+		if (o.changed) {*o.changed = st->changed;}
+		memcpy(o.blocks, table, (size_t)st->nblocks*sizeof(tw_voxel_block_mesh));
+		return TW_OK;
+	};
 	return j;
 }
 
-int model_begin(tw_voxel_model *m) {
-	if (!m) return TW_ERR_ARG;
-	TW_CUDA(m->ctx, cudaSetDevice(m->ctx->device));
-	return twi_finish_pending(m->ctx);
-}
+int model_begin(tw_voxel_model *m) {return m ? twi_begin(m->ctx) : TW_ERR_ARG;}
 
 } // namespace
 
@@ -1113,9 +1123,8 @@ extern "C" int tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp
 	if (!ctx) return TW_ERR_ARG;
 	if (!out || !edge_table256 || !tri_table256x16 || !edge_to_vals12x2) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_create: null argument");
 	*out = nullptr;
-	TW_CUDA(ctx, cudaSetDevice(ctx->device));
-	{int const rc_ = twi_finish_pending(ctx); if (rc_) return rc_;}
-	int rc = validate(ctx, vp); if (rc) return rc;
+	int rc = twi_begin(ctx); if (rc) return rc;
+	rc = validate(ctx, vp); if (rc) return rc;
 	if (bx == 0 || by == 0) return tw_set_error(ctx, TW_ERR_ARG, "block sizes must be >= 1");
 	tw_voxel_post_params const P = *vp;
 	unsigned const ncx = P.nx - 1, ncy = P.ny - 1, bw = (bx < ncx) ? bx : ncx, bh = (by < ncy) ? by : ncy;
@@ -1194,9 +1203,9 @@ extern "C" int tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_par
 	ModelScratch X;
 	rc = model_scratch(m, 0, 0, &X); if (rc) return rc;
 	size_t const n = (size_t)P.nx*P.ny*P.nz;
-	memset(ctx->h_pinned, 0, sizeof(twi_vmodel_stage));
+	memset(X.h_stage, 0, sizeof(twi_vmodel_stage));
 	m->built = true; // the job commits the model's state
-	return twi_launch_job(ctx, model_job(&O), [&]() -> int {
+	return twi_launch_job(ctx, model_job(X, O), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
 		if (fill) {int const r = twi_voxel_fill(ctx, &F, rdata420, m->raw, X.h_rdata); if (r) return r;}
 		else {TW_CUDA(ctx, cudaMemcpyAsync(m->raw, vals, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
@@ -1241,9 +1250,9 @@ extern "C" int tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box 
 	ModelScratch X;
 	rc = model_scratch(m, nboxes, total, &X); if (rc) return rc;
 	size_t const n = (size_t)P.nx*P.ny*P.nz;
-	memset(ctx->h_pinned, 0, sizeof(twi_vmodel_stage));
+	memset(X.h_stage, 0, sizeof(twi_vmodel_stage));
 	if (nboxes) {memcpy(X.h_boxes, B.data(), nboxes*sizeof(twi_box)); memcpy(X.h_values, values, total*sizeof(float));}
-	return twi_launch_job(ctx, model_job(&O), [&]() -> int {
+	return twi_launch_job(ctx, model_job(X, O), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
 		if (total) {
 			TW_CUDA(ctx, cudaMemcpyAsync(X.boxes, X.h_boxes, nboxes*sizeof(twi_box), cudaMemcpyHostToDevice, ctx->stream));

@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(_HERE, "lib3dworld_b200.so")
 MGEN_SINE, MGEN_SIMPLEX, MGEN_PERLIN, MGEN_SIMPLEX_GPU, MGEN_DWARP_GPU = range(5)
 TW_OK, TW_ERR_NO_DEVICE, TW_ERR_CUDA, TW_ERR_ARG, TW_ERR_STATE, TW_ERR_NOT_READY, TW_ERR_CANCELED = 0, -1, -2, -3, -4, -5, -6
 TW_EROSION_SERIAL, TW_EROSION_OPENMP, TW_EROSION_SWEEPS = 0, 1, 2
-PQ_SIN_TERMS, PQ_SIN_TERMS_SCALED, PQ_EXACT_ZVAL = 0, 1, 2   # tw_point_query.kind
+PQ_SIN_TERMS, PQ_SIN_TERMS_SCALED, PQ_EXACT_ZVAL, PQ_HMAP = 0, 1, 2, 3   # tw_point_query.kind (PQ_HMAP: tw_points_launch only)
 
 
 class TwError(RuntimeError):
@@ -160,6 +160,11 @@ class HmapSampler(C.Structure):
                 ("mesh_file_scale", C.c_float), ("mesh_file_tz", C.c_float), ("mesh_scale_z_inv", C.c_float)]
 
 
+class PointsJobArgs(C.Structure):
+    """tw_points_job (include/tw3d.h): the points, the query and, for PQ_HMAP, the heightmap sampler of one tw_points_launch, and where the heights go."""
+    _fields_ = [("xy", C.c_void_p), ("n", C.c_size_t), ("p", C.c_void_p), ("q", C.c_void_p), ("hs", C.c_void_p), ("out", C.c_void_p)]
+
+
 class HmapRect(C.Structure):
     """tw_hmap_rect (include/tw3d.h): texels [x, x + w) x [y, y + h) of the heightmap image."""
     _fields_ = [("x", C.c_int), ("y", C.c_int), ("w", C.c_int), ("h", C.c_int)]
@@ -212,7 +217,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_tile_set_create_tiles_launch", "tw_tile_set_stale_after", "tw_voxel_build_launch",
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
                "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
-               "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read"]
+               "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
+               "tw_points_launch"]
 
 
 def _load():
@@ -272,6 +278,7 @@ def _load():
     L.tw_update_heightmap.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32]
     L.tw_hmap_tiles_touched.argtypes = [C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
+    L.tw_points_launch.argtypes = [vp, C.POINTER(PointsJobArgs)]
     L.tw_erode_parallel.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_uint32, C.POINTER(ErosionParams), C.c_uint32]
     L.tw_erode_launch.argtypes = [vp, C.POINTER(ErosionJobArgs)]
     L.tw_erode_launch_ex.argtypes = [vp, C.POINTER(ErosionJobArgs), C.POINTER(SweepParams)]
@@ -587,6 +594,16 @@ class ErosionJob:
         self.heightmap, self.vals = heightmap, vals
 
 
+class PointsJob:
+    """What Context.points_launch returns: poll(wait) completes the job (the context's pending job) and returns out, or None while it runs (wait=False)."""
+
+    def __init__(self, ctx, out):
+        self._ctx, self.out = ctx, out
+
+    def poll(self, wait=False):
+        return self.out if self._ctx.create_tiles_poll(wait) else None
+
+
 class Context:
     """One tw_ctx (device + stream + uploaded tables). All compute goes through the C ABI."""
 
@@ -860,6 +877,20 @@ class Context:
             out = np.empty(n, np.float32)
         self._check(lib.tw_eval_points(self._h, _ptr(xy), n, C.byref(hp), C.byref(pq), _ptr(out)))
         return out
+
+    def points_launch(self, xy, hp=None, pq=None, hs=None, out=None):
+        """tw_points_launch: eval_points (hp, pq of a PQ_* procedural kind) or, with pq.kind = PQ_HMAP and hs (HmapSampler), the heights of the set_heightmap
+        image at cells xy, as this context's asynchronous job. xy = [n, 2] float32 numpy array or torch tensor (host xy is copied during the launch, CUDA xy
+        stays referenced until the job completes); out = n floats (numpy array or torch tensor, host or CUDA; default a new numpy array). Returns a PointsJob."""
+        n = int(xy.shape[0])
+        if out is None:
+            out = np.empty(n, np.float32)
+        ref = lambda s: C.cast(C.pointer(s), C.c_void_p) if s is not None else None  # noqa: E731
+        a = PointsJobArgs(_ptr(xy), n, ref(hp), ref(pq), ref(hs), _ptr(out))
+        self._check(lib.tw_points_launch(self._h, C.byref(a)))
+        job = PointsJob(self, out)
+        self._tiles_job = (xy, out, hp, pq, hs, job)
+        return job
 
     def erode(self, h, min_zval, num_iters, ep):
         """In place on h (numpy [ys, xs] or CUDA tensor)."""

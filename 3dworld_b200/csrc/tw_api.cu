@@ -44,6 +44,12 @@ bool tw_is_device_ptr(const void *p) {
 	return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged);
 }
 
+bool twi_is_page_locked(const void *p) {
+	cudaPointerAttributes a;
+	if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {cudaGetLastError(); return false;}
+	return a.type == cudaMemoryTypeHost;
+}
+
 int twi_ensure_aux_streams(tw_ctx *ctx) {
 	if (ctx->aux_stream[0]) return TW_OK;
 	int lo = 0, hi = 0; // the latency-bound droplet kernels / band copies get the higher priority
@@ -350,7 +356,8 @@ int tw_cancel(tw_ctx *ctx) {
 	int rc = check_ctx(ctx); if (rc) return rc;
 	twi_job const &j = ctx->async.job;
 	if (!j.complete) return TW_OK;
-	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "a job that touches a tile set or a voxel model cannot be cancelled: its state was committed at its launch");
+	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "the pending job cannot be cancelled: a job that touches a tile set or a voxel model committed its state at "
+	                                                           "its launch, and a points job is a single kernel");
 	ctx->h_job->cancel = j.seq;
 	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->d_job_words->cancel, &ctx->h_job->cancel, sizeof(unsigned), cudaMemcpyHostToDevice, ctx->cancel_stream));
 	ctx->cancel_sent = true;
@@ -1225,6 +1232,50 @@ int tw_eval_points(tw_ctx *ctx, const float *xy, size_t n, const tw_height_param
 	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
+}
+
+// tw_eval_points, or get_clamped_height of the context's image (TW_PQ_HMAP), as the context's asynchronous job: host xy is copied into the pinned staging
+// during the launch and goes up from there; the results go to device or page-locked out directly, and to pageable out through the staging, which the
+// completion copies. Device scratch slot 0: [xy (host xy) | out (host out)]; pinned staging: [xy (host xy) | out (pageable out)].
+int tw_points_launch(tw_ctx *ctx, const tw_points_job *job) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!job) return tw_set_error(ctx, TW_ERR_ARG, "null job");
+	size_t const n = job->n;
+	if (n == 0) return TW_OK;
+	if (!job->xy || !job->q || !job->out) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+	bool const hmap = (job->q->kind == TW_PQ_HMAP);
+	if (hmap) {
+		rc = validate_hmap(ctx, job->hs, nullptr); if (rc) return rc;
+		if (n > (size_t)0x7fffffff*256) return tw_set_error(ctx, TW_ERR_ARG, "tw_points_launch: too many points");
+	}
+	else {
+		if (!job->p) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+		if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
+		rc = twi_eval_points_check(ctx, n, job->p, job->q); if (rc) return rc;
+	}
+	bool const dev_in = tw_is_device_ptr(job->xy), dev_out = tw_is_device_ptr(job->out), locked_out = !dev_out && twi_is_page_locked(job->out);
+	float *s_xy = nullptr, *d_out = job->out, *h_xy = nullptr, *h_out = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_in) {s_xy = c.take<float>(2*n);} if (!dev_out) {d_out = c.take<float>(n);}}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {if (!dev_in) {h_xy = c.take<float>(2*n);} if (!dev_out && !locked_out) {h_out = c.take<float>(n);}}); if (rc) return rc;
+	float *const out = job->out;
+	twi_job pending;
+	pending.reads_image = hmap; // one kernel: not cancellable
+	pending.complete = [h_out, out, n](tw_ctx *) -> int {if (h_out) {memcpy(out, h_out, n*sizeof(float));} return TW_OK;};
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
+		if (!dev_in) {
+			memcpy(h_xy, job->xy, 2*n*sizeof(float));
+			TW_CUDA(ctx, cudaMemcpyAsync(s_xy, h_xy, 2*n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+		}
+		const float *d_xy = dev_in ? job->xy : s_xy;
+		if (hmap) {
+			int const r = twi_hmap_points(ctx, ctx->d_hmap, job->hs, d_xy, n, d_out); if (r) return r;
+			TW_CUDA(ctx, cudaEventRecord(ctx->async.image_free, ctx->stream)); // a later edit waits for this kernel only
+			ctx->async.image_free_set = true;
+		}
+		else {int const r = twi_eval_points(ctx, d_xy, n, job->p, job->q, d_out); if (r) return r;}
+		if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(locked_out ? out : h_out, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+		return TW_OK;
+	});
 }
 
 int tw_erode(tw_ctx *ctx, float *heightmap, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p) {

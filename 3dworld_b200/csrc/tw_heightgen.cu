@@ -937,17 +937,26 @@ static void launch_points(int shape, unsigned grid, cudaStream_t st, const float
 	}
 }
 
-int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out) {
+int twi_eval_points_check(tw_ctx *ctx, size_t n, const tw_height_params *p, const tw_point_query *q) {
 	if (q->kind < TW_PQ_SIN_TERMS || q->kind > TW_PQ_EXACT_ZVAL) return tw_set_error(ctx, TW_ERR_ARG, "tw_eval_points: bad kind %d", q->kind);
 	bool const sine_mode = (p->gen_mode == TW_MGEN_SINE || q->kind == TW_PQ_SIN_TERMS);
 	if (sine_mode && !ctx->have_sine_params) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sine_params() has not been called");
 	if (p->start_eval_sin < 0 || p->start_eval_sin > F_TABLE) return tw_set_error(ctx, TW_ERR_ARG, "start_eval_sin %d out of range", p->start_eval_sin);
 	if (n > (size_t)0x7fffffff*256) return tw_set_error(ctx, TW_ERR_ARG, "tw_eval_points: too many points");
+	NoiseParams N;
+	bool simplex = true;
+	if (!sine_mode && !make_noise_params(p, N, simplex)) return tw_set_error(ctx, TW_ERR_ARG, "start_eval_sin out of range");
+	return TW_OK;
+}
+
+int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out) {
+	int const rc = twi_eval_points_check(ctx, n, p, q); if (rc) return rc;
+	bool const sine_mode = (p->gen_mode == TW_MGEN_SINE || q->kind == TW_PQ_SIN_TERMS);
 	PostParams const P = make_post_params(p, 1, 0.0f, 0.0f);
 	NoiseParams N;
 	bool simplex = true;
 	memset(&N, 0, sizeof(N));
-	if (!sine_mode && !make_noise_params(p, N, simplex)) return tw_set_error(ctx, TW_ERR_ARG, "start_eval_sin out of range");
+	if (!sine_mode) {make_noise_params(p, N, simplex);}
 	PointParams Q;
 	memset(&Q, 0, sizeof(Q));
 	Q.kind = q->kind; Q.sine_mode = sine_mode; Q.start = p->start_eval_sin; Q.glaciate = (p->glaciate != 0);

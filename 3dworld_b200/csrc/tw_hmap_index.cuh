@@ -1,6 +1,6 @@
 // tw_hmap_index.cuh - the texel index arithmetic of get_clamped_height (src/heightmap.cpp:309-341,385-402): which texels a cell of a heightmap-texture tile
 // reads. Shared by hmap_sample_tiles_kernel (tw_streaming.cu) and the host-only tw_hmap_tiles_touched, so that the texels the host names as read are the ones
-// the kernel reads, expression for expression (both are compiled without FMA contraction).
+// the kernel reads, expression for expression (both are compiled without FMA contraction); hmap_points_kernel uses the float forms below.
 #pragma once
 #include "../../include/tw3d.h"
 #include <math.h>
@@ -36,6 +36,18 @@ TWH_HD int near_index(float mesh_scale, int x) {return round_fp(mesh_scale*((flo
 // mesh_scale < 1: interpolate_height's scaled coordinate and its two taps floor / ceil, before clamp_no_scale (src/heightmap.cpp:394-402)
 TWH_HD float lerp_index(float mesh_scale, int x, int &lo, int &hi) {
 	float const s = mesh_scale*(float)x;
+	lo = (int)floorf(s); hi = (int)ceilf(s);
+	return s;
+}
+
+// The same at a fractional cell (hmap_points_kernel: an object between cells), the library's extension of the integer-cell function. At an integer x with
+// |mesh_scale*x| < 2^30 (every |x| < 2^24 at a mesh_scale below 64) both forms give the int forms' results bit for bit: (float)x is then exact and the
+// arithmetic is the same. The scaled coordinate is held to [-2^30, 2^30] (NaN goes to -2^30), so the texel index and clamp_no_scale's
+// x + width/2 stay inside int range for any float a caller passes.
+TWH_HD float clamp_scaled(float s) {return fminf(fmaxf(s, -1073741824.0f), 1073741824.0f);}
+TWH_HD int near_index(float mesh_scale, float x) {return round_fp(clamp_scaled(mesh_scale*(x + 0.0f)));}
+TWH_HD float lerp_index(float mesh_scale, float x, int &lo, int &hi) {
+	float const s = clamp_scaled(mesh_scale*x);
 	lo = (int)floorf(s); hi = (int)ceilf(s);
 	return s;
 }

@@ -119,6 +119,7 @@ int  twi_ensure_glm3_lut(tw_ctx *ctx);                          // builds ctx->d
 int  tw_reserve(tw_ctx *ctx, int slot, size_t bytes);           // grow d_scratch[slot]; returns TW_OK / TW_ERR_CUDA
 int  tw_reserve_pinned(tw_ctx *ctx, size_t bytes);
 bool tw_is_device_ptr(const void *p);
+bool twi_is_page_locked(const void *p);                         // host memory the device can copy to without staging (cudaHostAlloc / cudaHostRegister)
 
 // A layout of scratch or pinned staging: regions carved one after another from `base`, each starting on a 256-byte boundary. A layout is written once, as
 // code that takes a twi_carve &, and run twice: with base == nullptr it only counts `bytes` (the size to reserve), then on the reserved memory. An absent
@@ -291,6 +292,10 @@ int twi_create_tiles_launch(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_
                             uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
                             const tw_tile_outputs *out, const tw_tile_shading *shading, twi_job_tail *tail);
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
+// twi_eval_points' refusals (TW_ERR_ARG / TW_ERR_STATE), without enqueuing anything
+int twi_eval_points_check(tw_ctx *ctx, size_t n, const tw_height_params *p, const tw_point_query *q);
+// get_clamped_height of the image d_data16 under hs at n cells d_xy (x, y pairs, fractional allowed) into d_out, on ctx->stream (tw_streaming.cu)
+int twi_hmap_points(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const float *d_xy, size_t n, float *d_out);
 // M_SPEC (one big map, the reference's serial droplet order) in parts: whether twi_erode takes it, its scratch, and the enqueue - with host_rounds = false
 // one that ends on the device (*d_fail = the rounds run when the window stopped making progress, else 0), with true tw_erode's host-driven rounds
 bool   twi_erode_spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters);

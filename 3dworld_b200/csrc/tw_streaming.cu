@@ -140,7 +140,40 @@ hmap_sample_tiles_kernel(const uint8_t *__restrict__ data16, tw_hmap_sampler H, 
 	}
 	out[(size_t)tile*zvsize*zvsize + i] = z;
 }
+
+// get_clamped_height at n arbitrary cells (x, y) of the tiles' index space, one thread per point: hmap_sample_tiles_kernel's expressions with the float index
+// forms, so an integer cell gives that kernel's value bit for bit and a fractional one takes the float directly
+__global__ void __launch_bounds__(256)
+hmap_points_kernel(const uint8_t *__restrict__ data16, tw_hmap_sampler H, const float2 *__restrict__ xy, size_t n, float *__restrict__ out) {
+	size_t const i = (size_t)blockIdx.x*blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	float2 const pt = __ldg(xy + i);
+	float z;
+	if (H.mesh_scale < 1.0f) {
+		int xlo, ylo, xhi, yhi;
+		float const sx = twh::lerp_index(H.mesh_scale, pt.x, xlo, xhi), sy = twh::lerp_index(H.mesh_scale, pt.y, ylo, yhi);
+		float const xv = sx - (float)xlo, yv = sy - (float)ylo;
+		bool const ok_lo = twh::clamp_no_scale(xlo, ylo, H);
+		bool const ok = ok_lo && twh::clamp_no_scale(xhi, yhi, H);
+		if (!ok) {z = hmap_scale_val(0.0f, H);}
+		else {
+			z = yv*(xv*hmap_raw_height(data16, xhi, yhi, H) + (1.0f - xv)*hmap_raw_height(data16, xlo, yhi, H)) +
+			    (1.0f - yv)*(xv*hmap_raw_height(data16, xhi, ylo, H) + (1.0f - xv)*hmap_raw_height(data16, xlo, ylo, H));
+		}
+	}
+	else {
+		int x = twh::near_index(H.mesh_scale, pt.x), y = twh::near_index(H.mesh_scale, pt.y);
+		z = twh::clamp_no_scale(x, y, H) ? hmap_raw_height(data16, x, y, H) : hmap_scale_val(0.0f, H);
+	}
+	out[i] = z;
+}
 } // namespace
+
+int twi_hmap_points(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const float *d_xy, size_t n, float *d_out) {
+	hmap_points_kernel<<<(unsigned)((n + 255)/256), 256, 0, ctx->stream>>>(d_data16, *hs, reinterpret_cast<const float2 *>(d_xy), n, d_out);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
 
 int twi_hmap_sample_tiles(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler *hs, const void *d_origins, uint32_t ntiles, uint32_t zvsize, float *d_out,
                           cudaStream_t st, const unsigned *d_perm, uint32_t cstep) {

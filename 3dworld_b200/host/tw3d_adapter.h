@@ -11,6 +11,7 @@
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //   tw3d::update_heightmap, tw3d::hmap_tiles_touched  <->  terrain_hmap_manager_t's brush edits and re-applied modmap, and the tiles they change   src/heightmap.cpp:36-58,243-308
+//   tw3d::get_exact_zvals_async, tw3d::heightmap_heights_async  <->  get_exact_zval / get_clamped_height per placed object, without stalling the frame   src/mesh_gen.cpp:816-847, src/heightmap.cpp:385-402
 //   tw3d::set_deferred_gens, tw3d::tile_job_pool  <->  several of them in flight at once, as tile_draw_t::update keeps up to 8   src/tiled_mesh.cpp:2367-2417
 //   tw3d::tile_set               <->  the live tiles' calc_shadows_for_light when the light moves or new tiles appear   src/tiled_mesh.cpp:664-692
 //
@@ -261,12 +262,19 @@ inline void apply_erosion(float *heightmap, int xsize, int ysize, float min_zval
 // float get_exact_zval(float xval, float yval, bool no_xyoff=0) / eval_mesh_sin_terms(xv, yv) / eval_mesh_sin_terms_scaled(xval, yval, xy_scale)
 // (src/function_registry.h:340-341, src/mesh_gen.cpp:797-847) for n points at once: xy = n (x, y) pairs. The single-point forms below cost a
 // kernel launch per call - callers that place many objects (buildings, scenery) should collect their points and use the batch forms.
+namespace detail {
+	inline tw_point_query point_query(int kind, float xy_scale, bool no_xyoff) {
+		scene_globals const &g = globals();
+		tw_point_query q;
+		q.kind = kind; q.xy_scale = xy_scale; q.mesh_x_size = g.MESH_X_SIZE; q.mesh_y_size = g.MESH_Y_SIZE;
+		q.x_scene_size = g.X_SCENE_SIZE; q.y_scene_size = g.Y_SCENE_SIZE; q.xoff2 = g.xoff2; q.yoff2 = g.yoff2; q.no_xyoff = no_xyoff;
+		return q;
+	}
+}
 inline void eval_points(int kind, const float *xy, size_t n, float *out, float xy_scale = 1.0f, bool no_xyoff = false) {
 	scene_globals const &g = globals();
 	tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
-	tw_point_query q;
-	q.kind = kind; q.xy_scale = xy_scale; q.mesh_x_size = g.MESH_X_SIZE; q.mesh_y_size = g.MESH_Y_SIZE;
-	q.x_scene_size = g.X_SCENE_SIZE; q.y_scene_size = g.Y_SCENE_SIZE; q.xoff2 = g.xoff2; q.yoff2 = g.yoff2; q.no_xyoff = no_xyoff;
+	tw_point_query const q = detail::point_query(kind, xy_scale, no_xyoff);
 	tw_ctx *c = ctx();
 	int const rc = tw_eval_points(c, xy, n, &p, &q, out);
 	if (rc != TW_OK) {detail::fail(rc, "eval_points", c);}
@@ -439,6 +447,33 @@ inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, un
 	return detail::launch_tiles(c, detail::tls().tile_jobs, &hs, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
 }
 
+// Object placement without stalling the frame (tw_points_launch): get_exact_zvals_async is get_exact_zvals as a job, and heightmap_heights_async gives, for
+// a heightmap-texture terrain, get_clamped_height at n cells (x, y) of the tiles' index space (a tile's cell (i, j) is (x1 + i, y1 + j)) from the image
+// set_heightmap() keeps on this thread's device, with every update_heightmap made before the call and none made after; a fractional cell takes the
+// sampler's expressions at the float (an object between cells). Both return at once with a tiles_job; out holds the heights once it is ready. xy / cells
+// (host memory is copied during the call, device memory is read until the job is ready) and out (device, page-locked or pageable host memory) as
+// tw_points_job; cancel() throws (TW_ERR_STATE: the job is one kernel). tile_job_pool has the same two calls for several jobs in flight.
+namespace detail {
+	inline tiles_job launch_points(tw_ctx *c, std::atomic<uint64_t> &jobs, const float *xy, size_t n, float *out, int kind, bool no_xyoff, int tex_edge_mode,
+	                               const char *what) {
+		scene_globals const &g = globals();
+		tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
+		tw_point_query const q = point_query(kind, 1.0f, no_xyoff);
+		tw_hmap_sampler const hs = hmap_sampler(tls().hmap_w, tls().hmap_h, tex_edge_mode);
+		tw_points_job const job = {xy, n, &p, &q, kind == TW_PQ_HMAP ? &hs : nullptr, out};
+		uint64_t const number = ++jobs;
+		int const rc = tw_points_launch(c, &job);
+		if (rc != TW_OK) {fail(rc, what, c);}
+		return tiles_job(c, &jobs, number);
+	}
+}
+inline tiles_job get_exact_zvals_async(const float *xy, size_t n, float *zvals_out, bool no_xyoff = false) {
+	return detail::launch_points(ctx(), detail::tls().tile_jobs, xy, n, zvals_out, TW_PQ_EXACT_ZVAL, no_xyoff, 0, "get_exact_zvals_async");
+}
+inline tiles_job heightmap_heights_async(const float *cells, size_t n, float *heights_out, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	return detail::launch_points(ctx(), detail::tls().tile_jobs, cells, n, heights_out, TW_PQ_HMAP, false, tex_edge_mode, "heightmap_heights_async");
+}
+
 // terrain_hmap_manager_t::proc_gen_heightmap (heightmap_t::proc_gen, src/heightmap.cpp:130-215): the globals' height function on a width x height grid
 // (cell size dx, dy), run_erosion with erosion_iters droplets, the z range, the texture scalars (info: get_mh_texture_mult/add, mesh_file_scale / _tz, the
 // droplet moves) and the 16-bit image data16 (2*width*height bytes). data16 and vals (optional, width*height floats) are host or device memory.
@@ -590,6 +625,15 @@ public:
 		slot &s = next();
 		tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
 		return detail::launch_tiles(s.c, s.jobs, &hs, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
+	}
+	// object placement (get_exact_zvals_async / heightmap_heights_async above) on a slot, beside the frames in flight on the others
+	tiles_job get_exact_zvals_async(const float *xy, size_t n, float *zvals_out, bool no_xyoff = false) {
+		slot &s = next();
+		return detail::launch_points(s.c, s.jobs, xy, n, zvals_out, TW_PQ_EXACT_ZVAL, no_xyoff, 0, "get_exact_zvals_async");
+	}
+	tiles_job heightmap_heights_async(const float *cells, size_t n, float *heights_out, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+		slot &s = next();
+		return detail::launch_points(s.c, s.jobs, cells, n, heights_out, TW_PQ_HMAP, false, tex_edge_mode, "heightmap_heights_async");
 	}
 };
 

@@ -268,6 +268,38 @@ typedef struct tw_point_query {
 	int   xoff2, yoff2, no_xyoff;     /* current mesh scroll offset, and the no_xyoff argument (exact) */
 } tw_point_query;
 TW_API int tw_eval_points(tw_ctx *ctx, const float *xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *out);
+/* Heights at many points as the context's ASYNCHRONOUS job, so that object placement does not stall the frame: the procedural kinds of tw_eval_points, and
+ * TW_PQ_HMAP, the height of the context's tw_set_heightmap image.
+ * - TW_PQ_SIN_TERMS .. TW_PQ_EXACT_ZVAL: after the completing poll out equals tw_eval_points(ctx, xy, n, p, q, out) bit for bit (same kernel).
+ * - TW_PQ_HMAP: xy holds cells of the heightmap tiles' index space (a tile's cell (x, y) is (x1 + x, y1 + y), tw_create_tiles_launch_hmap); out[i] is
+ *   get_clamped_height there under hs, scaled by scale_mh_texture_val, with the expressions of tw_heightmap_sample_tiles: mesh_scale < 1 interpolate_height
+ *   at mesh_scale*x with its floor and ceil taps, otherwise the nearest texel round_fp(mesh_scale*x); outside the image clamp_no_scale in hs->edge_mode (cliff:
+ *   scale_mh_texture_val(0)). At an integer cell with |mesh_scale*x|, |mesh_scale*y| < 2^30 (every |x|, |y| < 2^24 at a mesh_scale below 64) the result equals,
+ *   bit for bit, the tw_heightmap_sample_tiles value of any tile containing the cell. At a fractional cell (an object between cells) the same expressions
+ *   take the float directly: the library's extension of the reference's integer-cell function. Scaled coordinates beyond +-2^30, and NaN, are held to
+ *   -2^30 .. 2^30. p is not read.
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it (wait = 0 returns TW_ERR_NOT_READY while it runs), every
+ *   other entry point and tw_destroy complete it first. On a shared context it runs beside the other contexts' jobs. tw_cancel returns TW_ERR_STATE: the
+ *   job is one kernel.
+ * - TW_PQ_HMAP sees the image as it was when its launch returned: every tw_update_heightmap made before the launch, none made after it. A later edit waits
+ *   on the device only for this job's kernel. While an erosion of the image or a set_image heightmap job is pending the launch returns TW_ERR_STATE, as
+ *   tw_create_tiles_launch_hmap does.
+ * - Host xy (pageable or page-locked) is copied into the context's pinned staging during the launch, so the caller may reuse it as soon as the call returns;
+ *   device xy is read until the completing poll. out is device, page-locked or pageable host memory; pageable out is filled by the completing poll. With
+ *   device or page-locked xy and out the launch never waits for the device, except when the context's scratch or staging first has to grow.
+ * - Errors, nothing enqueued: TW_ERR_ARG for what tw_eval_points refuses, a NULL job, a NULL q, xy or out with n > 0, TW_PQ_HMAP without hs, hs sized
+ *   unlike the image and edge_mode outside 0..2; TW_ERR_STATE without the sin table or (sine mode, TW_PQ_SIN_TERMS) the sine params, and TW_PQ_HMAP
+ *   without an image. n == 0 is TW_OK and enqueues nothing. tw_eval_points refuses TW_PQ_HMAP as any other unknown kind. */
+#define TW_PQ_HMAP 3
+typedef struct tw_points_job {
+	const float            *xy;   /* n (x, y) pairs: host (copied during the launch) or device (read until the completing poll) */
+	size_t                  n;
+	const tw_height_params *p;    /* procedural kinds, as tw_eval_points */
+	const tw_point_query   *q;    /* required; q->kind selects TW_PQ_SIN_TERMS .. TW_PQ_EXACT_ZVAL or TW_PQ_HMAP */
+	const struct tw_hmap_sampler *hs; /* TW_PQ_HMAP only: required, sized like the context's image (declared below) */
+	float                  *out;  /* n floats: device, page-locked or pageable host memory (the last is filled by the completing poll) */
+} tw_points_job;
+TW_API int tw_points_launch(tw_ctx *ctx, const tw_points_job *job);
 
 /* ---- hydraulic erosion ----
  * Replaces apply_erosion(float *heightmap, int xsize, int ysize, float min_zval, unsigned num_iters) (src/function_registry.h:354,

@@ -406,19 +406,18 @@ int tw_heightgen_2d_launch(tw_ctx *ctx, const tw_grid2d *g, const tw_height_para
 	int rc = twi_begin(ctx); if (rc) return rc;
 	rc = validate_height(ctx, g, p, out); if (rc) return rc;
 	size_t const n = (size_t)g->nx*g->ny;
-	bool const dev_out = tw_is_device_ptr(out);
-	float *d_out = out;
-	if (!dev_out) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc; d_out = (float *)ctx->d_scratch[0];}
+	twi_user<float> o(out, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {o.take(c);}); if (rc) return rc;
 	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
 	if (mm) {rc = tw_reserve_pinned(ctx, 2*sizeof(unsigned)); if (rc) return rc;}
-	if (!dev_out) {rc = twi_ensure_aux_streams(ctx); if (rc) return rc;}
+	if (!o.dev) {rc = twi_ensure_aux_streams(ctx); if (rc) return rc;}
 	unsigned *d_mm = mm ? twi_slot2(ctx)->mm : nullptr, *h_mm = (unsigned *)ctx->h_pinned;
 	twi_job pending;
 	pending.cancellable = true;
 	pending.complete = [mm, h_mm](tw_ctx *) -> int {if (mm) {unpack_minmax(h_mm, 1, mm);} return TW_OK;};
 	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
 		if (d_mm) {rc = twi_init_minmax(ctx, d_mm, 1); if (rc) return rc;}
-		rc = twi_heightgen(ctx, g, p, enable_glaciate, min_start_sin, nullptr, 1, d_out, d_mm, dev_out ? nullptr : out); // host out: band-wise D2H overlapped with compute
+		rc = twi_heightgen(ctx, g, p, enable_glaciate, min_start_sin, nullptr, 1, o.d, d_mm, o.dev ? nullptr : out); // host out: band-wise D2H overlapped with compute
 		if (rc) return rc;
 		if (mm) {TW_CUDA(ctx, cudaMemcpyAsync(h_mm, d_mm, 2*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
 		return TW_OK;
@@ -447,17 +446,13 @@ int tw_tile_weights_batch(tw_ctx *ctx, const float *zvals, const int32_t *origin
 	rc = validate_weights(ctx, wp, W); if (rc) return rc;
 	uint32_t const stride = zvsize - 1;
 	size_t const zn = (size_t)ntiles*zvsize*zvsize, tn = (size_t)ntiles*stride*stride;
-	bool const dev_z = tw_is_device_ptr(zvals), dev_w = tw_is_device_ptr(weights), dev_f = has_any_grass && tw_is_device_ptr(has_any_grass), dev_p = tw_is_device_ptr(tile_params);
-	float *d_rand, *s_z = nullptr, *s_p = nullptr;
-	uint8_t *d_w = weights, *d_f = has_any_grass;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		d_rand = c.take<float>(tn); if (!dev_z) {s_z = c.take<float>(zn);} if (!dev_w) {d_w = c.take<uint8_t>(tn*4);} if (!dev_f) {d_f = c.take<uint8_t>(ntiles);}
-		if (!dev_p) {s_p = c.take<float>((size_t)ntiles*8);}
-	}); if (rc) return rc;
-	const float *d_z = dev_z ? zvals : s_z, *d_p = dev_p ? tile_params : s_p;
-	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, zn*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (!dev_p) {TW_CUDA(ctx, cudaMemcpyAsync(s_p, tile_params, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (has_any_grass) {TW_CUDA(ctx, cudaMemsetAsync(d_f, 0, ntiles, ctx->stream));}
+	twi_user<const float> z(zvals, zn), tp(tile_params, (size_t)ntiles*8);
+	twi_user<uint8_t> w(weights, tn*4), f(has_any_grass, ntiles);
+	float *d_rand;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {d_rand = c.take<float>(tn); z.take(c); w.take(c); f.take(c); tp.take(c);}); if (rc) return rc;
+	rc = z.in(ctx); if (rc) return rc;
+	rc = tp.in(ctx); if (rc) return rc;
+	if (has_any_grass) {TW_CUDA(ctx, cudaMemsetAsync(f.d, 0, ntiles, ctx->stream));}
 	// height_gen.build_arrays((x1 - MESH_X_SIZE/2), (y1 - MESH_Y_SIZE/2), MESH_NOISE_FREQ*DX_VAL, MESH_NOISE_FREQ*DY_VAL, tsize, tsize, 0, 1) (src/tiled_mesh.cpp:1103)
 	float const MESH_NOISE_FREQ = 80.0f;
 	tw_grid2d g; g.x0 = 0; g.y0 = 0; g.dx = MESH_NOISE_FREQ*dx; g.dy = MESH_NOISE_FREQ*dy; g.nx = stride; g.ny = stride;
@@ -470,10 +465,10 @@ int tw_tile_weights_batch(tw_ctx *ctx, const float *zvals, const int32_t *origin
 	ps.gen_mode = TW_MGEN_SINE; ps.gen_shape = 0; // force_sine_mode: gen_mode = MGEN_SINE, gen_shape = 0 (src/mesh_gen.cpp:592-593)
 	rc = twi_heightgen_sine_tiles(ctx, &g, &ps, 0, 50, org.data(), ntiles, d_rand, nullptr);
 	if (rc) return rc;
-	rc = twi_tile_weights(ctx, ctx->stream, d_z, d_rand, ntiles, zvsize, d_p, &W, d_w, has_any_grass ? d_f : nullptr);
+	rc = twi_tile_weights(ctx, ctx->stream, z.d, d_rand, ntiles, zvsize, tp.d, &W, w.d, has_any_grass ? f.d : nullptr);
 	if (rc) return rc;
-	if (!dev_w) {TW_CUDA(ctx, cudaMemcpyAsync(weights, d_w, tn*4, cudaMemcpyDeviceToHost, ctx->stream));}
-	if (has_any_grass && !dev_f) {TW_CUDA(ctx, cudaMemcpyAsync(has_any_grass, d_f, ntiles, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = w.out(ctx); if (rc) return rc;
+	rc = f.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -486,9 +481,8 @@ int tw_heightgen_tiles(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, 
 	tw_grid2d g; g.x0 = 0; g.y0 = 0; g.dx = dx; g.dy = dy; g.nx = zvsize; g.ny = zvsize;
 	rc = validate_height(ctx, &g, p, out); if (rc) return rc;
 	size_t const tile_elems = (size_t)zvsize*zvsize, n = tile_elems*ntiles;
-	bool const dev_out = tw_is_device_ptr(out);
-	float *d_out = out;
-	if (!dev_out) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc; d_out = (float *)ctx->d_scratch[0];}
+	twi_user<float> o(out, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {o.take(c);}); if (rc) return rc;
 	unsigned *d_mm = nullptr; float2 *d_org;
 	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {c.take<twi_slot2_words>(1); if (mm) {d_mm = c.take<unsigned>((size_t)ntiles*2);} d_org = c.take<float2>(ntiles);});
 	if (rc) return rc;
@@ -505,7 +499,7 @@ int tw_heightgen_tiles(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, 
 		uint32_t const zmax = 65535;
 		for (uint32_t t0 = 0; t0 < ntiles; t0 += zmax) { // gridDim.z limit
 			uint32_t const nt = (ntiles - t0 < zmax) ? ntiles - t0 : zmax;
-			rc = twi_heightgen(ctx, &g, p, 1, 0, d_org + t0, nt, d_out + (size_t)t0*tile_elems, d_mm ? d_mm + 2*(size_t)t0 : nullptr);
+			rc = twi_heightgen(ctx, &g, p, 1, 0, d_org + t0, nt, o.d + (size_t)t0*tile_elems, d_mm ? d_mm + 2*(size_t)t0 : nullptr);
 			if (rc) return rc;
 		}
 	}
@@ -515,10 +509,10 @@ int tw_heightgen_tiles(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles, 
 			float const x0 = (float)(origins_xy[2*t] - mesh_x_size/2), y0 = (float)(origins_xy[2*t+1] - mesh_y_size/2);
 			org[t] = make_float2(dx*x0, dy*y0);
 		}
-		rc = twi_heightgen_sine_tiles(ctx, &g, p, 1, 0, org.data(), ntiles, d_out, d_mm);
+		rc = twi_heightgen_sine_tiles(ctx, &g, p, 1, 0, org.data(), ntiles, o.d, d_mm);
 		if (rc) return rc;
 	}
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = o.out(ctx); if (rc) return rc;
 	if (mm) {rc = read_minmax(ctx, d_mm, mm, ntiles); if (rc) return rc;}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
@@ -531,12 +525,11 @@ int tw_tile_bounds_batch(tw_ctx *ctx, const float *zvals, uint32_t ntiles, uint3
 	if (4*(zvsize/4) >= zvsize) return tw_set_error(ctx, TW_ERR_ARG, "zvsize %u: the last sub-block would end at cell %u (the reference asserts x_end < zvsize, src/tiled_mesh.cpp:520)", zvsize, 4*(zvsize/4));
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
 	size_t const n = (size_t)ntiles*zvsize*zvsize;
-	bool const dev = tw_is_device_ptr(zvals);
-	float *s_z = nullptr; Sub *d_sub;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {s_z = c.take<float>(n);} d_sub = c.take<Sub>((size_t)ntiles*16);}); if (rc) return rc;
-	const float *d_z = dev ? zvals : s_z;
-	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	rc = twi_tile_bounds(ctx, ctx->stream, d_z, ntiles, zvsize, wpz_max, d_sub); if (rc) return rc;
+	twi_user<const float> z(zvals, n);
+	Sub *d_sub;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {z.take(c); d_sub = c.take<Sub>((size_t)ntiles*16);}); if (rc) return rc;
+	rc = z.in(ctx); if (rc) return rc;
+	rc = twi_tile_bounds(ctx, ctx->stream, z.d, ntiles, zvsize, wpz_max, d_sub); if (rc) return rc;
 	std::vector<Sub> sub((size_t)ntiles*16);
 	TW_CUDA(ctx, cudaMemcpyAsync(sub.data(), d_sub, sub.size()*sizeof(Sub), cudaMemcpyDeviceToHost, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -549,18 +542,14 @@ int tw_glaciate_mesh(tw_ctx *ctx, float *mesh, int nx, int ny, int xoff2, int yo
 	if (!mesh || !p || nx <= 0 || ny <= 0 || ny > 65535) return tw_set_error(ctx, TW_ERR_ARG, "bad argument");
 	if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
 	size_t const n = (size_t)nx*ny;
-	bool const dev = tw_is_device_ptr(mesh);
-	float *d_mesh = mesh;
-	if (!dev) {
-		rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc;
-		d_mesh = (float *)ctx->d_scratch[0];
-		TW_CUDA(ctx, cudaMemcpyAsync(d_mesh, mesh, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	}
+	twi_user<float> m(mesh, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {m.take(c);}); if (rc) return rc;
+	rc = m.in(ctx); if (rc) return rc;
 	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
 	unsigned *d_mm = twi_slot2(ctx)->mm;
 	rc = twi_init_minmax(ctx, d_mm, 1); if (rc) return rc;
-	rc = twi_glaciate_mesh(ctx, d_mesh, nx, ny, xoff2, yoff2, mesh_x_size, mesh_y_size, p, d_mm); if (rc) return rc;
-	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(mesh, d_mesh, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = twi_glaciate_mesh(ctx, m.d, nx, ny, xoff2, yoff2, mesh_x_size, mesh_y_size, p, d_mm); if (rc) return rc;
+	rc = m.out(ctx); if (rc) return rc;
 	if (zbottom_ztop) {return read_minmax(ctx, d_mm, zbottom_ztop, 1);}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
@@ -575,22 +564,18 @@ int tw_erode_tiles(tw_ctx *ctx, float *maps, uint32_t ntiles, int xsize, int ysi
 	if (xsize <= 0 || ysize <= 0 || ntiles == 0) return tw_set_error(ctx, TW_ERR_ARG, "empty heightmap");
 	if (num_iters == 0 || p->erode_amount <= 0.0) {ctx->last_erosion_steps = 0; return TW_OK;} // src/erosion.cpp:16
 	size_t const n = (size_t)xsize*ysize*ntiles;
-	bool const dev = tw_is_device_ptr(maps);
-	float *d_maps = maps;
-	if (!dev) {
-		rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc;
-		d_maps = (float *)ctx->d_scratch[0];
-		TW_CUDA(ctx, cudaMemcpyAsync(d_maps, maps, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	}
+	twi_user<float> m(maps, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {m.take(c);}); if (rc) return rc;
+	rc = m.in(ctx); if (rc) return rc;
 	float *d_minz = nullptr;
 	if (min_zvals) {
 		rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {c.take<twi_slot2_words>(1); d_minz = c.take<float>(ntiles);}); if (rc) return rc;
 		TW_CUDA(ctx, cudaMemcpyAsync(d_minz, min_zvals, (size_t)ntiles*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 		TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	}
-	rc = twi_erode(ctx, d_maps, ntiles, xsize, ysize, d_minz, min_zval_all, num_iters, p);
+	rc = twi_erode(ctx, m.d, ntiles, xsize, ysize, d_minz, min_zval_all, num_iters, p);
 	if (rc) return rc;
-	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(maps, d_maps, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = m.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -651,9 +636,9 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	bool const ctx_mode = want_ao && p->gen_mode >= TW_MGEN_SIMPLEX_GPU;
 	uint32_t const stride = zvsize - 1, ray = 36, csz = stride + 2*ray; // AO_RAY_LEN, context_sz (src/tiled_mesh.cpp:43,601)
 	size_t const tile_elems = (size_t)zvsize*zvsize, n = tile_elems*ntiles, nrm_elems = (size_t)stride*stride, ctx_elems = (size_t)csz*csz;
-	bool const dev_out = o->zvals && tw_is_device_ptr(o->zvals), host_out = o->zvals && !dev_out, dev_nrm = want_normals && tw_is_device_ptr(o->normals_rgba);
-	bool const dev_ao = want_ao && tw_is_device_ptr(sh->ao), dev_w = want_w && tw_is_device_ptr(sh->weights), dev_f = want_f && tw_is_device_ptr(sh->has_any_grass);
-	bool const dev_tp = want_w && tw_is_device_ptr(sh->tile_params);
+	bool const dev_out = o->zvals && tw_is_device_ptr(o->zvals), host_out = o->zvals && !dev_out, dev_f = want_f && tw_is_device_ptr(sh->has_any_grass);
+	twi_user<uint8_t> nrm(o->normals_rgba, ntiles*nrm_elems*4), ao(want_ao ? sh->ao : nullptr, ntiles*nrm_elems), wt(want_w ? sh->weights : nullptr, ntiles*nrm_elems*4);
+	twi_user<const float> tp(want_w ? sh->tile_params : nullptr, (size_t)ntiles*8);
 	if (tail) {rc = tail->prepare(ctx); if (rc) return rc;}
 	rc = twi_ensure_aux_streams(ctx); if (rc) return rc;
 	// The pipeline. Work per tile is heavy-tailed (ocean tiles: 1000 droplets x 1 move; mountain tiles: 1e5 moves in one serial chain), and a chain
@@ -684,16 +669,15 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	bool sh_host_m = false, sh_in_x = false, sh_in_y = false;
 	for (uint32_t l = 0; l < nl; ++l) {sh_host_m |= !sdev_m[l]; sh_in_x |= (lights[l].sh_in_x != nullptr); sh_in_y |= (lights[l].sh_in_y != nullptr);}
 	float *d_out = dev_out ? o->zvals : nullptr, *d_shx = nullptr, *d_shy = nullptr;
-	unsigned char *d_rgba = dev_nrm ? o->normals_rgba : nullptr, *d_shm = nullptr, *d_ao = dev_ao ? sh->ao : nullptr, *d_w = dev_w ? sh->weights : nullptr;
+	unsigned char *d_shm = nullptr;
 	uint8_t *d_f = dev_f ? sh->has_any_grass : nullptr;
-	const float *d_tp = dev_tp ? sh->tile_params : nullptr;
 	char *d_ctab = nullptr, *d_jtab = nullptr, *d_tail = nullptr;
 	unsigned long long *d_shk = nullptr;
 	std::vector<int *> d_shp(nl);
 	auto slot0 = [&](twi_carve &c) {
-		if (!dev_out) {d_out = c.take<float>(n);} if (want_normals && !dev_nrm) {d_rgba = c.take<unsigned char>(ntiles*nrm_elems*4);}
-		if (want_ao && !dev_ao) {d_ao = c.take<uint8_t>(ntiles*nrm_elems);} if (want_w && !dev_w) {d_w = c.take<uint8_t>(ntiles*nrm_elems*4);}
-		if (want_f && !dev_f) {d_f = c.take<uint8_t>(ntiles);} if (want_w && !dev_tp) {d_tp = c.take<float>((size_t)ntiles*8);}
+		if (!dev_out) {d_out = c.take<float>(n);} if (want_normals) {nrm.take(c);}
+		if (want_ao) {ao.take(c);} if (want_w) {wt.take(c);}
+		if (want_f && !dev_f) {d_f = c.take<uint8_t>(ntiles);} if (want_w) {tp.take(c);}
 		if (want_ao && sine) {d_ctab = c.take<char>(ctab_bytes);} if (want_w) {d_jtab = c.take<char>(jtab_bytes);} if (sh_host_m) {d_shm = c.take<unsigned char>(n + 4);}
 		if (nl) {d_shk = c.take<unsigned long long>(2*edge); d_shx = c.take<float>((sh_in_x ? 2 : 1)*edge); d_shy = c.take<float>((sh_in_y ? 2 : 1)*edge);}
 		for (uint32_t l = 0; l < nl; ++l) {d_shp[l] = c.take<int>(twi_shadow_plan_ints(ntiles));} if (tail) {d_tail = c.take<char>(tail->dev_bytes);}
@@ -765,7 +749,6 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 	// Every sine batch has its own region, and the caller's origins, tile_params, tile_xy and host sh_in rows may be reused as soon as this function returns.
 	float2 *h_org;
 	char *h_sine = nullptr, *h_ctx = nullptr, *h_jit = nullptr, *h_tail = nullptr;
-	float *h_tp = nullptr;
 	std::vector<int *> h_shp(nl);
 	std::vector<float *> h_six(nl), h_siy(nl);
 	unsigned long long *h_steps;
@@ -777,7 +760,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		if (sine) {h_sine = c.take<char>(twi_sine_tiles_stage_bytes(ntiles));}
 		if (want_ao) {h_ctx = c.take<char>(sine ? twi_sine_tiles_stage_bytes(ntiles) : ntiles*sizeof(float2));}
 		if (want_w) {h_jit = c.take<char>(twi_sine_tiles_stage_bytes(ntiles));}
-		if (want_w && !dev_tp) {h_tp = c.take<float>((size_t)ntiles*8);}
+		tp.take_pinned(c);
 		for (uint32_t l = 0; l < nl; ++l) {h_shp[l] = c.take<int>(twi_shadow_plan_ints(ntiles));}
 		for (uint32_t l = 0; l < nl; ++l) {
 			h_six[l] = (lights[l].sh_in_x && !sdev_ix[l]) ? c.take<float>(edge) : nullptr; h_siy[l] = (lights[l].sh_in_y && !sdev_iy[l]) ? c.take<float>(edge) : nullptr;
@@ -814,10 +797,7 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 			memcpy(h_ctx, corg.data(), (size_t)ntiles*sizeof(float2));
 			TW_CUDA(ctx, cudaMemcpyAsync(d_corg, h_ctx, (size_t)ntiles*sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
 		}
-		if (h_tp) {
-			memcpy(h_tp, sh->tile_params, (size_t)ntiles*8*sizeof(float));
-			TW_CUDA(ctx, cudaMemcpyAsync((void *)d_tp, h_tp, (size_t)ntiles*8*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-		}
+		rc = tp.in(ctx); if (rc) return rc;
 		for (uint32_t l = 0; l < nl; ++l) { // the plans go up now; host sh_in rows wait in the staging until their light's pass copies them into the edge buffers
 			twi_shadow_plan_pack(splan[l], h_shp[l]);
 			TW_CUDA(ctx, cudaMemcpyAsync(d_shp[l], h_shp[l], twi_shadow_plan_ints(ntiles)*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
@@ -908,10 +888,10 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 			if (want_w) {status = twi_sine_tiles_grid(ctx, &sb_jit, t0, nt, d_perm, d_rand, nullptr); if (status) break;}
 			if (want_mm) {status = twi_minmax_tiles(ctx, es, maps, tile_elems, nt, d_mm + 2*r0, perm_k); if (status) break;}
 			if (want_bounds) {status = twi_tile_bounds(ctx, es, maps, nt, zvsize, wpz_max, d_sub + 16*r0, perm_k); if (status) break;}
-			if (want_normals) {status = twi_tile_normals(ctx, es, maps, nt, zvsize, dx, dy, d_rgba + r0*nrm_elems*4, d_mnz ? d_mnz + r0 : nullptr, perm_k); if (status) break;}
+			if (want_normals) {status = twi_tile_normals(ctx, es, maps, nt, zvsize, dx, dy, nrm.d + r0*nrm_elems*4, d_mnz ? d_mnz + r0 : nullptr, perm_k); if (status) break;}
 			if (((want_ao && !ctx_mode) || want_w) && !chain(ctx->stream, es)) {status = tw_set_error(ctx, TW_ERR_CUDA, "chunk event"); break;}
-			if (want_ao) {status = twi_tile_ao(ctx, es, maps, d_cz, nt, zvsize, sh->half_dxy, ctx_mode, d_ao + r0*nrm_elems, perm_k); if (status) break;}
-			if (want_w) {status = twi_tile_weights(ctx, es, maps, d_rand, nt, zvsize, d_tp + r0*8, &W, d_w + r0*nrm_elems*4, d_f ? d_f + r0 : nullptr, perm_k); if (status) break;}
+			if (want_ao) {status = twi_tile_ao(ctx, es, maps, d_cz, nt, zvsize, sh->half_dxy, ctx_mode, ao.d + r0*nrm_elems, perm_k); if (status) break;}
+			if (want_w) {status = twi_tile_weights(ctx, es, maps, d_rand, nt, zvsize, tp.d + r0*8, &W, wt.d + r0*nrm_elems*4, d_f ? d_f + r0 : nullptr, perm_k); if (status) break;}
 			if (nbuf) {
 				if (!ring_ev[b] && cudaEventCreateWithFlags(&ring_ev[b], cudaEventDisableTiming) != cudaSuccess) {ring_ev[b] = nullptr; status = tw_set_error(ctx, TW_ERR_CUDA, "ring event"); break;}
 				if (cudaEventRecord(ring_ev[b], es) != cudaSuccess) {status = tw_set_error(ctx, TW_ERR_CUDA, "ring event"); break;}
@@ -939,9 +919,9 @@ static int tiles_launch(tw_ctx *ctx, const int32_t *origins_xy, uint32_t ntiles,
 		if (tail) {rc = tail->enqueue(ctx, d_out, d_tail, h_tail); if (rc) return rc;} // the tail's work reads the final zvals
 		// every host-bound result is copied once, at the end: the schedule order scatters a chunk over the whole batch
 		if (host_out && d_perm) {TW_CUDA(ctx, cudaMemcpyAsync(o->zvals, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_normals && !dev_nrm) {TW_CUDA(ctx, cudaMemcpyAsync(o->normals_rgba, d_rgba, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_ao && !dev_ao) {TW_CUDA(ctx, cudaMemcpyAsync(sh->ao, d_ao, (size_t)ntiles*nrm_elems, cudaMemcpyDeviceToHost, ctx->stream));}
-		if (want_w && !dev_w) {TW_CUDA(ctx, cudaMemcpyAsync(sh->weights, d_w, (size_t)ntiles*nrm_elems*4, cudaMemcpyDeviceToHost, ctx->stream));}
+		rc = nrm.out(ctx); if (rc) return rc;
+		rc = ao.out(ctx); if (rc) return rc;
+		rc = wt.out(ctx); if (rc) return rc;
 		if (erode) {TW_CUDA(ctx, cudaMemcpyAsync(h_steps, d_steps, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));}
 		if (want_mm) {TW_CUDA(ctx, cudaMemcpyAsync(h_mm, d_mm, (size_t)ntiles*2*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
 		if (want_bounds) {TW_CUDA(ctx, cudaMemcpyAsync(h_sub, d_sub, (size_t)ntiles*16*sizeof(Sub), cudaMemcpyDeviceToHost, ctx->stream));}
@@ -1113,17 +1093,14 @@ int tw_heightmap_sample_tiles(tw_ctx *ctx, const uint8_t *data16, const tw_hmap_
 	if (!data16 || !hs || !origins_xy || !out || ntiles == 0 || zvsize == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	if (hs->width <= 0 || hs->height <= 0 || hs->edge_mode < 0 || hs->edge_mode > 2) return tw_set_error(ctx, TW_ERR_ARG, "bad heightmap sampler");
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
-	size_t const img_bytes = (size_t)2*hs->width*hs->height, out_bytes = (size_t)ntiles*zvsize*zvsize*sizeof(float);
-	bool const dev_img = tw_is_device_ptr(data16), dev_out = tw_is_device_ptr(out);
-	int32_t *d_org; uint8_t *s_img = nullptr; float *d_out = out;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		d_org = c.take<int32_t>((size_t)ntiles*2); if (!dev_img) {s_img = c.take<uint8_t>(img_bytes);} if (!dev_out) {d_out = c.take<float>((size_t)ntiles*zvsize*zvsize);}
-	}); if (rc) return rc;
+	twi_user<const uint8_t> img(data16, (size_t)2*hs->width*hs->height);
+	twi_user<float> o(out, (size_t)ntiles*zvsize*zvsize);
+	int32_t *d_org;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {d_org = c.take<int32_t>((size_t)ntiles*2); img.take(c); o.take(c);}); if (rc) return rc;
 	TW_CUDA(ctx, cudaMemcpyAsync(d_org, origins_xy, (size_t)ntiles*8, cudaMemcpyHostToDevice, ctx->stream));
-	const uint8_t *d_img = dev_img ? data16 : s_img;
-	if (!dev_img) {TW_CUDA(ctx, cudaMemcpyAsync(s_img, data16, img_bytes, cudaMemcpyHostToDevice, ctx->stream));}
-	rc = twi_hmap_sample_tiles(ctx, d_img, hs, d_org, ntiles, zvsize, d_out); if (rc) return rc;
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = img.in(ctx); if (rc) return rc;
+	rc = twi_hmap_sample_tiles(ctx, img.d, hs, d_org, ntiles, zvsize, o.d); if (rc) return rc;
+	rc = o.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // origins_xy is the caller's buffer
 	return TW_OK;
 }
@@ -1133,21 +1110,19 @@ int tw_tile_normals_batch(tw_ctx *ctx, const float *zvals, uint32_t ntiles, uint
 	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!zvals || !rgba || ntiles == 0 || zvsize < 2) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
 	if (ntiles > 65535) return tw_set_error(ctx, TW_ERR_ARG, "at most 65535 tiles per call");
-	size_t const n = (size_t)ntiles*zvsize*zvsize, stride = zvsize - 1, out_bytes = (size_t)ntiles*stride*stride*4;
-	bool const dev_in = tw_is_device_ptr(zvals), dev_out = tw_is_device_ptr(rgba);
-	unsigned *d_mn; float *s_z = nullptr; unsigned char *d_rgba = rgba;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		d_mn = c.take<unsigned>(ntiles); if (!dev_in) {s_z = c.take<float>(n);} if (!dev_out) {d_rgba = c.take<unsigned char>(out_bytes);}
-	}); if (rc) return rc;
-	const float *d_z = dev_in ? zvals : s_z;
-	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	size_t const stride = zvsize - 1;
+	twi_user<const float> z(zvals, (size_t)ntiles*zvsize*zvsize);
+	twi_user<uint8_t> o(rgba, (size_t)ntiles*stride*stride*4);
+	unsigned *d_mn;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {d_mn = c.take<unsigned>(ntiles); z.take(c); o.take(c);}); if (rc) return rc;
+	rc = z.in(ctx); if (rc) return rc;
 	{
 		std::vector<unsigned> init(ntiles, tw_f2ord(1.0f)); // min_normal_z = 1.0, src/tiled_mesh.cpp:868
 		TW_CUDA(ctx, cudaMemcpyAsync(d_mn, init.data(), ntiles*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));
 		TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	}
-	rc = twi_tile_normals(ctx, ctx->stream, d_z, ntiles, zvsize, dx_val, dy_val, d_rgba, d_mn); if (rc) return rc;
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(rgba, d_rgba, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = twi_tile_normals(ctx, ctx->stream, z.d, ntiles, zvsize, dx_val, dy_val, o.d, d_mn); if (rc) return rc;
+	rc = o.out(ctx); if (rc) return rc;
 	std::vector<unsigned> mn(ntiles);
 	if (min_normal_z) {TW_CUDA(ctx, cudaMemcpyAsync(mn.data(), d_mn, ntiles*sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1221,15 +1196,13 @@ int tw_eval_points(tw_ctx *ctx, const float *xy, size_t n, const tw_height_param
 	if (!xy || !p || !q || !out) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
 	if (n == 0) return TW_OK;
 	if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
-	bool const dev_in = tw_is_device_ptr(xy), dev_out = tw_is_device_ptr(out);
-	size_t const out_bytes = n*sizeof(float);
-	float *s_xy = nullptr, *d_out = out;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_in) {s_xy = c.take<float>(2*n);} if (!dev_out) {d_out = c.take<float>(n);}}); if (rc) return rc;
-	const float *d_xy = dev_in ? xy : s_xy;
-	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_xy, xy, 2*n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	rc = twi_eval_points(ctx, d_xy, n, p, q, d_out);
+	twi_user<const float> pts(xy, 2*n);
+	twi_user<float> o(out, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {pts.take(c); o.take(c);}); if (rc) return rc;
+	rc = pts.in(ctx); if (rc) return rc;
+	rc = twi_eval_points(ctx, pts.d, n, p, q, o.d);
 	if (rc) return rc;
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = o.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -1253,26 +1226,23 @@ int tw_points_launch(tw_ctx *ctx, const tw_points_job *job) {
 		if (!ctx->have_sin) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
 		rc = twi_eval_points_check(ctx, n, job->p, job->q); if (rc) return rc;
 	}
-	bool const dev_in = tw_is_device_ptr(job->xy), dev_out = tw_is_device_ptr(job->out), locked_out = !dev_out && twi_is_page_locked(job->out);
-	float *s_xy = nullptr, *d_out = job->out, *h_xy = nullptr, *h_out = nullptr;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_in) {s_xy = c.take<float>(2*n);} if (!dev_out) {d_out = c.take<float>(n);}}); if (rc) return rc;
-	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {if (!dev_in) {h_xy = c.take<float>(2*n);} if (!dev_out && !locked_out) {h_out = c.take<float>(n);}}); if (rc) return rc;
+	twi_user<const float> pts(job->xy, 2*n);
+	bool const dev_out = tw_is_device_ptr(job->out), locked_out = !dev_out && twi_is_page_locked(job->out);
+	float *d_out = job->out, *h_out = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {pts.take(c); if (!dev_out) {d_out = c.take<float>(n);}}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {pts.take_pinned(c); if (!dev_out && !locked_out) {h_out = c.take<float>(n);}}); if (rc) return rc;
 	float *const out = job->out;
 	twi_job pending;
 	pending.reads_image = hmap; // one kernel: not cancellable
 	pending.complete = [h_out, out, n](tw_ctx *) -> int {if (h_out) {memcpy(out, h_out, n*sizeof(float));} return TW_OK;};
 	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
-		if (!dev_in) {
-			memcpy(h_xy, job->xy, 2*n*sizeof(float));
-			TW_CUDA(ctx, cudaMemcpyAsync(s_xy, h_xy, 2*n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-		}
-		const float *d_xy = dev_in ? job->xy : s_xy;
+		rc = pts.in(ctx); if (rc) return rc;
 		if (hmap) {
-			int const r = twi_hmap_points(ctx, ctx->d_hmap, job->hs, d_xy, n, d_out); if (r) return r;
+			int const r = twi_hmap_points(ctx, ctx->d_hmap, job->hs, pts.d, n, d_out); if (r) return r;
 			TW_CUDA(ctx, cudaEventRecord(ctx->async.image_free, ctx->stream)); // a later edit waits for this kernel only
 			ctx->async.image_free_set = true;
 		}
-		else {int const r = twi_eval_points(ctx, d_xy, n, job->p, job->q, d_out); if (r) return r;}
+		else {int const r = twi_eval_points(ctx, pts.d, n, job->p, job->q, d_out); if (r) return r;}
 		if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(locked_out ? out : h_out, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 		return TW_OK;
 	});
@@ -1288,16 +1258,12 @@ int tw_erode_parallel(tw_ctx *ctx, float *heightmap, int xsize, int ysize, float
 	if (xsize <= 0 || ysize <= 0) return tw_set_error(ctx, TW_ERR_ARG, "empty heightmap");
 	if (num_iters == 0 || p->erode_amount <= 0.0) {ctx->last_erosion_steps = 0; return TW_OK;} // src/erosion.cpp:16
 	size_t const n = (size_t)xsize*ysize;
-	bool const dev = tw_is_device_ptr(heightmap);
-	float *d_map = heightmap;
-	if (!dev) {
-		rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc;
-		d_map = (float *)ctx->d_scratch[0];
-		TW_CUDA(ctx, cudaMemcpyAsync(d_map, heightmap, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-	}
-	rc = twi_erode_parallel(ctx, d_map, xsize, ysize, min_zval, num_iters, p, num_threads);
+	twi_user<float> m(heightmap, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {m.take(c);}); if (rc) return rc;
+	rc = m.in(ctx); if (rc) return rc;
+	rc = twi_erode_parallel(ctx, m.d, xsize, ysize, min_zval, num_iters, p, num_threads);
 	if (rc) return rc;
-	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(heightmap, d_map, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = m.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -1331,10 +1297,9 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 	bool const erode = (job->num_iters > 0 && job->ep->erode_amount > 0.0); // src/erosion.cpp:16
 	if (erode && !ctx->d_dir_table) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sin_table() has not been called");
 	bool const openmp = (job->mode == TW_EROSION_OPENMP), spec = erode && !openmp && !sweeps && twi_erode_spec_eligible(1, xsize, ysize, job->num_iters);
-	float *const user = image ? job->vals : job->heightmap; // the caller's floats: the map, or the image's optional eroded floats
-	bool const user_dev = (user && tw_is_device_ptr(user));
+	twi_user<float> u(image ? job->vals : job->heightmap, n); // the caller's floats: the map, or the image's optional eroded floats
 	// slot 0: the floats (unless the caller's are on the device); slot 1: the erosion's scratch; slot 2: [fixed words (ordered min/max, droplet counter) | stage]
-	if (erode && !user_dev) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc;}
+	if (erode) {rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {u.take(c);}); if (rc) return rc;}
 	size_t const ebytes = !erode ? 0 : openmp ? twi_erode_parallel_scratch_bytes(xsize, ysize) : sweeps ? twi_erode_sweeps_scratch_bytes(xsize, ysize)
 	                                 : spec ? twi_erode_spec_scratch_bytes(xsize, ysize) : twi_erode_scratch_bytes(ctx, 1, xsize, ysize);
 	if (ebytes) {rc = tw_reserve(ctx, 1, ebytes); if (rc) return rc;}
@@ -1347,7 +1312,7 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 		ctx->hmap_w = ctx->hmap_h = 0;
 	}
 	tw_erosion_params const ep = *job->ep;
-	float *const d_vals = user_dev ? user : (float *)ctx->d_scratch[0];
+	float *const d_vals = u.d;
 	unsigned *const d_mm = words->mm;
 	twi_job pending;
 	pending.cancellable = true; pending.reads_image = image;
@@ -1363,7 +1328,7 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 				r = twi_ord_min(ctx, d_mm, &d_st->min_z); if (r) return r;
 				d_min = &d_st->min_z;
 			}
-			else if (!user_dev) {TW_CUDA(ctx, cudaMemcpyAsync(d_vals, user, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+			else {int const r = u.in(ctx); if (r) return r;} // the image's floats are an output only
 			int r;
 			if (openmp) {r = twi_erode_parallel_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, job->num_threads, &d_st->steps, &words->next);}
 			else if (sweeps) {r = twi_erode_sweeps_enqueue(ctx, ctx->d_scratch[1], d_vals, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, sw->sweep, sw->halo, &d_st->steps);}
@@ -1371,7 +1336,7 @@ int tw_erode_launch_ex(tw_ctx *ctx, const tw_erosion_job *job, const tw_sweep_pa
 			else {r = twi_erode_enqueue(ctx, ctx->stream, 0, ctx->d_scratch[1], 1, d_vals, 1, xsize, ysize, d_min, job->min_zval, job->num_iters, &ep, &d_st->steps);}
 			if (r) return r;
 			if (image) {r = twi_from_floats_u16(ctx, d_vals, n, job->val_mult, job->val_add, ctx->d_hmap, &d_st->bad); if (r) return r;}
-			if (user && !user_dev) {TW_CUDA(ctx, cudaMemcpyAsync(user, d_vals, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+			r = u.out(ctx); if (r) return r;
 		}
 		TW_CUDA(ctx, cudaMemcpyAsync(h_st, d_st, sizeof(twi_hmap_stage), cudaMemcpyDeviceToHost, ctx->stream));
 		return TW_OK;
@@ -1385,12 +1350,11 @@ int tw_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420,
 	size_t tab_bytes = 0;
 	rc = twi_voxel_fill_check(ctx, vp, &tab_bytes); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
-	bool const dev_out = tw_is_device_ptr(out);
-	float *d_out = out;
-	if (!dev_out) {rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc; d_out = (float *)ctx->d_scratch[0];}
-	rc = twi_voxel_fill(ctx, vp, rdata420, d_out);
+	twi_user<float> o(out, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {o.take(c);}); if (rc) return rc;
+	rc = twi_voxel_fill(ctx, vp, rdata420, o.d);
 	if (rc) return rc;
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out, d_out, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = o.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -1399,18 +1363,16 @@ int tw_voxel_fill(tw_ctx *ctx, const tw_voxel_params *vp, const float *rdata420,
 int tw_heightmap_from_floats_u16(tw_ctx *ctx, const float *vals, size_t n, float val_mult, float val_add, uint8_t *out2n) {
 	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!vals || !out2n || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
-	bool const dev_in = tw_is_device_ptr(vals), dev_out = tw_is_device_ptr(out2n);
-	size_t const in_bytes = n*sizeof(float), out_bytes = 2*n;
-	float *s_in = nullptr; uint8_t *d_out = out2n;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_in) {s_in = c.take<float>(n);} if (!dev_out) {d_out = c.take<uint8_t>(out_bytes);}}); if (rc) return rc;
+	twi_user<const float> v(vals, n);
+	twi_user<uint8_t> o(out2n, 2*n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {v.take(c); o.take(c);}); if (rc) return rc;
 	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
-	const float *d_in = dev_in ? vals : s_in;
-	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_in, vals, in_bytes, cudaMemcpyHostToDevice, ctx->stream));}
+	rc = v.in(ctx); if (rc) return rc;
 	unsigned *d_bad = &twi_slot2(ctx)->bad;
 	TW_CUDA(ctx, cudaMemsetAsync(d_bad, 0, sizeof(unsigned), ctx->stream));
-	rc = twi_from_floats_u16(ctx, d_in, n, val_mult, val_add, d_out, d_bad);
+	rc = twi_from_floats_u16(ctx, v.d, n, val_mult, val_add, o.d, d_bad);
 	if (rc) return rc;
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(out2n, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = o.out(ctx); if (rc) return rc;
 	unsigned bad = 0;
 	TW_CUDA(ctx, cudaMemcpyAsync(&bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1421,15 +1383,13 @@ int tw_heightmap_from_floats_u16(tw_ctx *ctx, const float *vals, size_t n, float
 int tw_heightmap_to_floats_u16(tw_ctx *ctx, const uint8_t *data2n, size_t n, float val_mult, float val_add, float *vals) {
 	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!vals || !data2n || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
-	bool const dev_in = tw_is_device_ptr(data2n), dev_out = tw_is_device_ptr(vals);
-	size_t const in_bytes = 2*n, out_bytes = n*sizeof(float);
-	uint8_t *s_in = nullptr; float *d_out = vals;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev_out) {d_out = c.take<float>(n);} if (!dev_in) {s_in = c.take<uint8_t>(in_bytes);}}); if (rc) return rc;
-	const uint8_t *d_in = dev_in ? data2n : s_in;
-	if (!dev_in) {TW_CUDA(ctx, cudaMemcpyAsync(s_in, data2n, in_bytes, cudaMemcpyHostToDevice, ctx->stream));}
-	rc = twi_to_floats_u16(ctx, d_in, n, val_mult, val_add, d_out);
+	twi_user<const uint8_t> img(data2n, 2*n);
+	twi_user<float> o(vals, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {o.take(c); img.take(c);}); if (rc) return rc;
+	rc = img.in(ctx); if (rc) return rc;
+	rc = twi_to_floats_u16(ctx, img.d, n, val_mult, val_add, o.d);
 	if (rc) return rc;
-	if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(vals, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = o.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -1510,16 +1470,13 @@ int tw_proc_gen_heightmap(tw_ctx *ctx, uint32_t width, uint32_t height, float dx
 int tw_minmax_f32(tw_ctx *ctx, const float *vals, size_t n, tw_minmax *mm) {
 	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!vals || !mm || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");
-	const float *d_in = vals;
-	if (!tw_is_device_ptr(vals)) {
-		rc = tw_reserve(ctx, 0, n*sizeof(float)); if (rc) return rc;
-		TW_CUDA(ctx, cudaMemcpyAsync(ctx->d_scratch[0], vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-		d_in = (const float *)ctx->d_scratch[0];
-	}
+	twi_user<const float> v(vals, n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {v.take(c);}); if (rc) return rc;
+	rc = v.in(ctx); if (rc) return rc;
 	rc = tw_reserve(ctx, 2, sizeof(twi_slot2_words)); if (rc) return rc;
 	unsigned *d_mm = twi_slot2(ctx)->mm;
 	rc = twi_init_minmax(ctx, d_mm, 1); if (rc) return rc;
-	rc = twi_minmax(ctx, d_in, n, d_mm); if (rc) return rc;
+	rc = twi_minmax(ctx, v.d, n, d_mm); if (rc) return rc;
 	return read_minmax(ctx, d_mm, mm, 1);
 }
 

@@ -147,6 +147,28 @@ inline twi_slot2_words *twi_slot2(tw_ctx *ctx) {return (twi_slot2_words *)ctx->d
 #define TW_LAUNCH_CHECK(ctx) do { (ctx)->launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { \
 	return tw_set_error((ctx), TW_ERR_CUDA, "%s:%d kernel launch: %s", __FILE__, __LINE__, cudaGetErrorString(e_)); } } while (0)
 
+// A caller's array of n elements of T, in device or host memory, or null. `d` is what the device work reads or writes: the caller's array when it is device
+// memory, else the region take() carved for it in a layout (also for a null array, which the work may fill without copying it anywhere), else nullptr.
+// take_pinned() carves a pinned bounce region for a host input in a job's staging layout: in() then copies the array there first, so the caller may reuse
+// it once the launch returns. in() (host -> d) and out() (d -> host) enqueue on ctx->stream and do nothing for a device, null or empty array.
+template <typename T> struct twi_user {
+	T *user; size_t n; bool dev; T *d, *h = nullptr;
+	twi_user(T *p, size_t count) : user(p), n(count), dev(p && tw_is_device_ptr(p)), d(dev ? p : nullptr) {}
+	void take(twi_carve &c) {if (!dev) d = c.take<T>(n);}
+	void take_pinned(twi_carve &c) {if (user && !dev) h = c.take<T>(n);}
+	int in(tw_ctx *ctx) const {
+		if (!user || dev || !n) return TW_OK;
+		if (h) memcpy((void *)h, user, n*sizeof(T));
+		TW_CUDA(ctx, cudaMemcpyAsync((void *)d, h ? h : user, n*sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+		return TW_OK;
+	}
+	int out(tw_ctx *ctx) const {
+		if (!user || dev || !n) return TW_OK;
+		TW_CUDA(ctx, cudaMemcpyAsync(user, d, n*sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+		return TW_OK;
+	}
+};
+
 // The job's number in the device words, on ctx->stream, before its work (twi_job_start sets *seq) / after it: `stopped` to the pinned staging, `job` cleared
 int twi_job_start(tw_ctx *ctx, unsigned *seq);
 int twi_job_end(tw_ctx *ctx);

@@ -234,22 +234,22 @@ static int tile_shadows(tw_ctx *ctx, const float *zvals, const int32_t *tile_xy,
 	size_t const cells = (size_t)ntiles*zvsize*zvsize, edge = (size_t)ntiles*zvsize;
 	twi_shadow_plan P;
 	if (!twi_shadow_plan_make(tile_xy, ntiles, sp, sh_in_x != nullptr, sh_in_y != nullptr, &P) && ex) return tw_set_error(ctx, TW_ERR_ARG, "tile_xy names a tile twice");
-	bool const dev_z = tw_is_device_ptr(zvals), dev_m = tw_is_device_ptr(smask);
-	if (dev_m && ((size_t)smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)");
-	float *s_z = nullptr, *d_ox, *d_oy; unsigned char *d_m = smask; unsigned long long *d_keys; int *d_plan;
+	twi_user<const float> z(zvals, cells);
+	twi_user<uint8_t> m(smask, cells); // a carved region covers the 32-bit word of its last byte: regions are whole 256-byte blocks
+	if (m.dev && ((size_t)smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)");
+	float *d_ox, *d_oy; unsigned long long *d_keys; int *d_plan;
 	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		if (!dev_z) {s_z = c.take<float>(cells);} if (!dev_m) {d_m = c.take<unsigned char>(cells + 4);} d_keys = c.take<unsigned long long>(2*edge);
+		z.take(c); m.take(c); d_keys = c.take<unsigned long long>(2*edge);
 		d_ox = c.take<float>((sh_in_x ? 2 : 1)*edge); d_oy = c.take<float>((sh_in_y ? 2 : 1)*edge); d_plan = c.take<int>(twi_shadow_plan_ints(ntiles));
 	}); if (rc) return rc;
-	const float *d_z = zvals;
-	if (!dev_z) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zvals, cells*sizeof(float), cudaMemcpyHostToDevice, ctx->stream)); d_z = s_z;}
+	rc = z.in(ctx); if (rc) return rc;
 	std::vector<int> plan(twi_shadow_plan_ints(ntiles));
 	twi_shadow_plan_pack(P, plan.data());
 	TW_CUDA(ctx, cudaMemcpyAsync(d_plan, plan.data(), plan.size()*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
 	if (sh_in_x) {TW_CUDA(ctx, cudaMemcpyAsync(d_ox + edge, sh_in_x, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	if (sh_in_y) {TW_CUDA(ctx, cudaMemcpyAsync(d_oy + edge, sh_in_y, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
-	rc = twi_shadow_enqueue(ctx, ctx->stream, P, d_z, ntiles, zvsize, d_m, d_keys, d_ox, d_oy, d_plan, false); if (rc) return rc; // the call blocks anyway
-	if (!dev_m) {TW_CUDA(ctx, cudaMemcpyAsync(smask, d_m, cells, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = twi_shadow_enqueue(ctx, ctx->stream, P, z.d, ntiles, zvsize, m.d, d_keys, d_ox, d_oy, d_plan, false); if (rc) return rc; // the call blocks anyway
+	rc = m.out(ctx); if (rc) return rc;
 	if (sh_out_x) {TW_CUDA(ctx, cudaMemcpyAsync(sh_out_x, d_ox, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	if (sh_out_y) {TW_CUDA(ctx, cudaMemcpyAsync(sh_out_y, d_oy, edge*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

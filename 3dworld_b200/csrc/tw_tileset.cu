@@ -373,13 +373,13 @@ int tw_tile_set_put(tw_tile_set *s, const int32_t *tile_xy, uint32_t n, const fl
 	uint32_t const next = twts::put_slots(s->st, keys, free_left, idx);
 	rc = grow(s, next, ctx); if (rc) return rc;
 	size_t const tb = (size_t)s->zvsize*s->zvsize*sizeof(float);
-	bool const dev = tw_is_device_ptr(zvals);
-	char *p = nullptr; int *d_idx;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {p = c.take<char>(n*tb);} d_idx = c.take<int>(n);}); if (rc) return rc;
-	if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(p, zvals, n*tb, cudaMemcpyHostToDevice, ctx->stream));}
+	twi_user<const float> z(zvals, (size_t)n*s->zvsize*s->zvsize);
+	int *d_idx;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {z.take(c); d_idx = c.take<int>(n);}); if (rc) return rc;
+	rc = z.in(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaMemcpyAsync(d_idx, idx.data(), n*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
 	TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, s->ev, 0)); // a frame's job on another context may still read these slots
-	rc = copy_tiles(ctx, s->d_z, d_idx, dev ? (const void *)zvals : (const void *)p, nullptr, tb, n); if (rc) return rc;
+	rc = copy_tiles(ctx, s->d_z, d_idx, z.d, nullptr, tb, n); if (rc) return rc;
 	TW_CUDA(ctx, cudaEventRecord(s->ev, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // zvals (and idx) have been read
 	twts::put_tiles(s->st, keys, idx, free_left, next, slot_signs(s));

@@ -156,6 +156,22 @@ __global__ void flood_finish_kernel(float *__restrict__ vals, unsigned char *__r
 // ---- marching cubes ----
 struct McTables {const unsigned *edge_table; const int *tri_table; const unsigned *edge_to_vals;};
 constexpr int MC_BLOCK = 1024;
+// The three tables in one device region of MC_TAB_BYTES: [edge_table 1024 B | tri_table 16384 B | edge_to_vals 96 B]
+constexpr size_t MC_TAB_OFF[3] = {0, 1024, 1024 + 16384}, MC_TAB_LEN[3] = {1024, 16384, 96}, MC_TAB_BYTES = MC_TAB_OFF[2] + MC_TAB_LEN[2];
+McTables mc_tables(const void *tab) {
+	const char *t = (const char *)tab;
+	return McTables{(const unsigned *)t, (const int *)(t + MC_TAB_OFF[1]), (const unsigned *)(t + MC_TAB_OFF[2])};
+}
+// Copies the caller's tables into the region `tab` on ctx->stream. h_bounce (optional): MC_TAB_BYTES of pinned staging that host tables are copied into
+// first, so the caller may reuse them once this returns (device tables are read when the copy runs).
+int mc_tables_upload(tw_ctx *ctx, void *tab, const uint32_t *edge_table256, const int32_t *tri_table256x16, const uint32_t *edge_to_vals12x2, char *h_bounce = nullptr) {
+	const void *src[3] = {edge_table256, tri_table256x16, edge_to_vals12x2};
+	for (int k = 0; k < 3; ++k) {
+		if (h_bounce && !tw_is_device_ptr(src[k])) {memcpy(h_bounce + MC_TAB_OFF[k], src[k], MC_TAB_LEN[k]); src[k] = h_bounce + MC_TAB_OFF[k];}
+		TW_CUDA(ctx, cudaMemcpyAsync((char *)tab + MC_TAB_OFF[k], src[k], MC_TAB_LEN[k], cudaMemcpyDefault, ctx->stream));
+	}
+	return TW_OK;
+}
 
 __device__ __forceinline__ void interpolate_pt(float isolevel, const float *pt1, const float *pt2, float val1, float val2, float *pt) { // src/voxels.cpp:485-493
 	if (fabsf(isolevel - val1) < VOX_TOLERANCE) {pt[0] = pt1[0]; pt[1] = pt1[1]; pt[2] = pt1[2]; return;}
@@ -560,17 +576,15 @@ extern "C" int tw_voxel_outside(tw_ctx *ctx, const float *vals, const tw_voxel_p
 	int rc = twi_begin(ctx); if (rc) return rc;
 	rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz, nxy = (size_t)vp->nx*vp->ny;
-	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_z = (zix_xy && tw_is_device_ptr(zix_xy));
-	float *s_v = nullptr; uint8_t *d_o = outside; unsigned *s_z = nullptr;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		if (!dev_v) {s_v = c.take<float>(n);} if (!dev_o) {d_o = c.take<uint8_t>(n);} if (zix_xy && !dev_z) {s_z = c.take<unsigned>(nxy);}
-	}); if (rc) return rc;
-	const float *d_v = dev_v ? vals : s_v; const unsigned *d_z = s_z ? s_z : zix_xy;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(s_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (s_z) {TW_CUDA(ctx, cudaMemcpyAsync(s_z, zix_xy, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));}
-	outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(d_v, *vp, d_z, d_o, n);
+	twi_user<const float> v(vals, n);
+	twi_user<uint8_t> o(outside, n);
+	twi_user<const uint32_t> z(zix_xy, nxy);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {v.take(c); o.take(c); if (zix_xy) {z.take(c);}}); if (rc) return rc;
+	rc = v.in(ctx); if (rc) return rc;
+	rc = z.in(ctx); if (rc) return rc;
+	outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(v.d, *vp, z.d, o.d, n);
 	TW_LAUNCH_CHECK(ctx);
-	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(outside, d_o, n, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = o.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -582,25 +596,26 @@ extern "C" int tw_voxel_remove_unconnected(tw_ctx *ctx, float *vals, uint8_t *ou
 	if (changed) *changed = 0;
 	if (vp->remove_unconnected <= 0) return TW_OK;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
-	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside);
+	twi_user<float> v(vals, n);
+	bool const dev_o = tw_is_device_ptr(outside);
 	if (dev_o && ((size_t)outside & 3)) return tw_set_error(ctx, TW_ERR_ARG, "outside must be 4-byte aligned (flag bytes are claimed with 32-bit atomics)");
 	// the 32-bit word that holds the last flag byte reaches up to 3 bytes past a buffer of n % 4 != 0 bytes: such a device buffer is staged like a host one
 	bool const stage_o = !dev_o || (n & 3);
 	unsigned blocks = 0;
 	rc = flood_blocks(ctx, &blocks); if (rc) return rc;
-	float *d_v = vals; unsigned char *d_o = outside; unsigned *f0, *f1, *cnt; unsigned long long *d_changed;
+	unsigned char *d_o = outside; unsigned *f0, *f1, *cnt; unsigned long long *d_changed;
 	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		if (!dev_v) {d_v = c.take<float>(n);} if (stage_o) {d_o = c.take<unsigned char>(n + 4);} f0 = c.take<unsigned>(n + 16); f1 = c.take<unsigned>(n + 16);
+		v.take(c); if (stage_o) {d_o = c.take<unsigned char>(n + 4);} f0 = c.take<unsigned>(n + 16); f1 = c.take<unsigned>(n + 16);
 		cnt = c.take<unsigned>(8); d_changed = c.take<unsigned long long>(1);
 	}); if (rc) return rc;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+	rc = v.in(ctx); if (rc) return rc;
 	if (stage_o) {TW_CUDA(ctx, cudaMemcpyAsync(d_o, outside, n, dev_o ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));}
 	TW_CUDA(ctx, cudaMemsetAsync(d_changed, 0, sizeof(unsigned long long), ctx->stream));
-	rc = enqueue_remove_unconnected(ctx, blocks, d_v, d_o, vp, f0, f1, cnt, d_changed);
+	rc = enqueue_remove_unconnected(ctx, blocks, v.d, d_o, vp, f0, f1, cnt, d_changed);
 	if (rc) {cudaStreamSynchronize(ctx->stream); return rc;}
 	unsigned long long hc = 0;
 	TW_CUDA(ctx, cudaMemcpyAsync(&hc, d_changed, sizeof(hc), cudaMemcpyDeviceToHost, ctx->stream));
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(vals, d_v, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = v.out(ctx); if (rc) return rc;
 	if (stage_o) {TW_CUDA(ctx, cudaMemcpyAsync(outside, d_o, n, dev_o ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	if (changed) *changed = hc;
@@ -615,21 +630,18 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 	rc = validate(ctx, vp); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
-	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside), dev_t = (tris && tw_is_device_ptr(tris));
-	float *s_v = nullptr; unsigned char *s_o = nullptr, *sp; unsigned *d_sums; unsigned long long *d_offsets, *d_total;
+	twi_user<const float> v(vals, n);
+	twi_user<const uint8_t> o(outside, n);
+	char *tab; unsigned *d_sums; unsigned long long *d_offsets, *d_total;
 	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		if (!dev_v) {s_v = c.take<float>(n);} if (!dev_o) {s_o = c.take<unsigned char>(n);} sp = c.take<unsigned char>(1024 + 16384 + 96);
+		v.take(c); o.take(c); tab = c.take<char>(MC_TAB_BYTES);
 		d_sums = c.take<unsigned>(nblocks); d_offsets = c.take<unsigned long long>(nblocks); d_total = c.take<unsigned long long>(1);
 	}); if (rc) return rc;
-	const float *d_v = dev_v ? vals : s_v; const unsigned char *d_o = dev_o ? outside : s_o;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(s_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(s_o, outside, n, cudaMemcpyHostToDevice, ctx->stream));}
-	McTables T;
-	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384);
-	TW_CUDA(ctx, cudaMemcpyAsync(sp, edge_table256, 1024, cudaMemcpyDefault, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024, tri_table256x16, 16384, cudaMemcpyDefault, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024 + 16384, edge_to_vals12x2, 96, cudaMemcpyDefault, ctx->stream));
-	mc_kernel<false><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, *vp, T, n, d_sums, nullptr, nullptr, 0);
+	rc = v.in(ctx); if (rc) return rc;
+	rc = o.in(ctx); if (rc) return rc;
+	rc = mc_tables_upload(ctx, tab, edge_table256, tri_table256x16, edge_to_vals12x2); if (rc) return rc;
+	McTables const T = mc_tables(tab);
+	mc_kernel<false><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(v.d, o.d, *vp, T, n, d_sums, nullptr, nullptr, 0);
 	TW_LAUNCH_CHECK(ctx);
 	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(d_sums, nblocks, d_offsets, d_total);
 	TW_LAUNCH_CHECK(ctx);
@@ -639,11 +651,11 @@ extern "C" int tw_voxel_triangles(tw_ctx *ctx, const float *vals, const uint8_t 
 	*ntris = total;
 	if (capacity == 0 || total == 0) return TW_OK;
 	uint64_t const nw = (total < capacity) ? total : capacity;
-	float *d_t = tris;
-	if (!dev_t) {rc = tw_reserve(ctx, 1, (size_t)nw*9*sizeof(float)); if (rc) return rc; d_t = (float *)ctx->d_scratch[1];}
-	mc_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, *vp, T, n, nullptr, d_offsets, d_t, nw);
+	twi_user<float> t(tris, (size_t)nw*9);
+	rc = twi_reserve_carve(ctx, 1, [&](twi_carve &c) {t.take(c);}); if (rc) return rc;
+	mc_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(v.d, o.d, *vp, T, n, nullptr, d_offsets, t.d, nw);
 	TW_LAUNCH_CHECK(ctx);
-	if (!dev_t) {TW_CUDA(ctx, cudaMemcpyAsync(tris, d_t, (size_t)nw*9*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = t.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -675,36 +687,29 @@ extern "C" int tw_voxel_mesh_welded(tw_ctx *ctx, const float *vals, const uint8_
 	rc = validate_mesh(ctx, vp, &M); if (rc) return rc;
 	size_t const n = (size_t)vp->nx*vp->ny*vp->nz;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
-	bool const dev_v = tw_is_device_ptr(vals), dev_o = tw_is_device_ptr(outside);
-	float *s_v = nullptr; unsigned char *s_o = nullptr, *sp; MeshScratch S;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
-		if (!dev_v) {s_v = c.take<float>(n);} if (!dev_o) {s_o = c.take<unsigned char>(n);} sp = c.take<unsigned char>(1024 + 16384 + 96); S = mesh_scratch(c, n, nblocks);
-	}); if (rc) return rc;
-	const float *d_v = dev_v ? vals : s_v; const unsigned char *d_o = dev_o ? outside : s_o;
-	if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(s_v, vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-	if (!dev_o) {TW_CUDA(ctx, cudaMemcpyAsync(s_o, outside, n, cudaMemcpyHostToDevice, ctx->stream));}
-	McTables T;
-	T.edge_table = (const unsigned *)sp; T.tri_table = (const int *)(sp + 1024); T.edge_to_vals = (const unsigned *)(sp + 1024 + 16384);
-	TW_CUDA(ctx, cudaMemcpyAsync(sp, edge_table256, 1024, cudaMemcpyDefault, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024, tri_table256x16, 16384, cudaMemcpyDefault, ctx->stream));
-	TW_CUDA(ctx, cudaMemcpyAsync(sp + 1024 + 16384, edge_to_vals12x2, 96, cudaMemcpyDefault, ctx->stream));
+	twi_user<const float> v(vals, n);
+	twi_user<const uint8_t> o(outside, n);
+	char *tab; MeshScratch S;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {v.take(c); o.take(c); tab = c.take<char>(MC_TAB_BYTES); S = mesh_scratch(c, n, nblocks);}); if (rc) return rc;
+	rc = v.in(ctx); if (rc) return rc;
+	rc = o.in(ctx); if (rc) return rc;
+	rc = mc_tables_upload(ctx, tab, edge_table256, tri_table256x16, edge_to_vals12x2); if (rc) return rc;
+	McTables const T = mc_tables(tab);
 	// count and scan first: the emit pass writes at most min(count, capacity) of each, so host outputs are staged at that size
-	rc = enqueue_mesh(ctx, d_v, d_o, *vp, T, S, nullptr, 0, nullptr, 0); if (rc) return rc;
+	rc = enqueue_mesh(ctx, v.d, o.d, *vp, T, S, nullptr, 0, nullptr, 0); if (rc) return rc;
 	unsigned long long tot[2] = {0, 0};
 	TW_CUDA(ctx, cudaMemcpyAsync(tot, S.totals, sizeof(tot), cudaMemcpyDeviceToHost, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	*M.nverts = tot[0]; *M.ntris = tot[1];
 	uint64_t const nv = (tot[0] < M.vcapacity) ? tot[0] : M.vcapacity, nt = (tot[1] < M.tcapacity) ? tot[1] : M.tcapacity;
 	if (nv == 0 && nt == 0) return TW_OK;
-	bool const dev_vt = nv && tw_is_device_ptr(M.verts), dev_ix = nt && tw_is_device_ptr(M.indices);
-	float *d_vt = M.verts; uint32_t *d_ix = M.indices;
-	rc = twi_reserve_carve(ctx, 1, [&](twi_carve &c) {
-		if (!dev_vt) {d_vt = c.take<float>((size_t)nv*3);} if (!dev_ix) {d_ix = c.take<uint32_t>((size_t)nt*3);}
-	}); if (rc) return rc;
-	mesh_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, *vp, T, n, S.words, nullptr, nullptr, S.voff, S.toff, d_vt, nv, d_ix, nt);
+	twi_user<float> vt(M.verts, (size_t)nv*3);
+	twi_user<uint32_t> ix(M.indices, (size_t)nt*3);
+	rc = twi_reserve_carve(ctx, 1, [&](twi_carve &c) {vt.take(c); ix.take(c);}); if (rc) return rc;
+	mesh_kernel<true><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(v.d, o.d, *vp, T, n, S.words, nullptr, nullptr, S.voff, S.toff, vt.d, nv, ix.d, nt);
 	TW_LAUNCH_CHECK(ctx);
-	if (nv && !dev_vt) {TW_CUDA(ctx, cudaMemcpyAsync(M.verts, d_vt, (size_t)nv*12, cudaMemcpyDeviceToHost, ctx->stream));}
-	if (nt && !dev_ix) {TW_CUDA(ctx, cudaMemcpyAsync(M.indices, d_ix, (size_t)nt*12, cudaMemcpyDeviceToHost, ctx->stream));}
+	rc = vt.out(ctx); if (rc) return rc;
+	rc = ix.out(ctx); if (rc) return rc;
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
 }
@@ -764,34 +769,33 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 	if (rm) {rc = flood_blocks(ctx, &blocks); if (rc) return rc;}
 	size_t const n = (size_t)P.nx*P.ny*P.nz, nxy = (size_t)P.nx*P.ny;
 	unsigned const nblocks = (unsigned)((n + MC_BLOCK - 1)/MC_BLOCK);
-	bool const dev_v = b->vals && tw_is_device_ptr(b->vals), dev_z = b->zix_xy && tw_is_device_ptr(b->zix_xy);
-	size_t const TAB = 1024 + 16384 + 96;
-	bool const tabs = (ntab == 3), stage_z = (b->zix_xy && !dev_z);
-	unsigned *cnt, *f0 = nullptr, *f1 = nullptr, *d_sums = nullptr, *s_z = nullptr;
-	float *d_v = b->vals;
-	unsigned char *d_o, *tab = nullptr;
+	twi_user<float> v(b->vals, n); // the fill's output when vals is null
+	twi_user<const uint32_t> z(b->zix_xy, nxy);
+	bool const tabs = (ntab == 3);
+	unsigned *cnt, *f0 = nullptr, *f1 = nullptr, *d_sums = nullptr;
+	unsigned char *d_o;
+	char *tab = nullptr;
 	unsigned long long *d_offsets = nullptr;
 	MeshScratch S;
 	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
 		cnt = c.take<unsigned>(64); // [flood counters | changed at byte 64 | triangle total at byte 128], zeroed together
-		if (!dev_v) {d_v = c.take<float>(n);}
+		v.take(c);
 		d_o = c.take<unsigned char>(n + 4);
 		if (rm) {f0 = c.take<unsigned>(n + 16); f1 = c.take<unsigned>(n + 16);}
-		if (tabs) {tab = c.take<unsigned char>(TAB);}
+		if (tabs) {tab = c.take<char>(MC_TAB_BYTES);}
 		if (mc) {d_sums = c.take<unsigned>(nblocks); d_offsets = c.take<unsigned long long>(nblocks);}
-		if (stage_z) {s_z = c.take<unsigned>(nxy);}
+		if (b->zix_xy) {z.take(c);}
 		if (wm) S = mesh_scratch(c, n, nblocks);
 	}); if (rc) return rc;
 	if (tab_bytes) {rc = tw_reserve(ctx, 1, tab_bytes); if (rc) return rc;}
-	twi_voxel_stage *st; float *h_rdata; unsigned char *h_tab = nullptr; unsigned *h_z = nullptr;
+	twi_voxel_stage *st; float *h_rdata; char *h_tab = nullptr;
 	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
-		st = c.take<twi_voxel_stage>(1); h_rdata = c.take<float>(TW_N3D_RDATA); if (tabs) {h_tab = c.take<unsigned char>(TAB);} if (stage_z) {h_z = c.take<unsigned>(nxy);}
+		st = c.take<twi_voxel_stage>(1); h_rdata = c.take<float>(TW_N3D_RDATA); if (tabs) {h_tab = c.take<char>(MC_TAB_BYTES);} z.take_pinned(c);
 	}); if (rc) return rc;
 	if (fill && F.gen_mode != TW_MGEN_SINE) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
 	unsigned long long *d_changed = (unsigned long long *)(cnt + 16), *d_total = (unsigned long long *)(cnt + 32);
-	McTables T = {};
-	if (tabs) {T.edge_table = (const unsigned *)tab; T.tri_table = (const int *)(tab + 1024); T.edge_to_vals = (const unsigned *)(tab + 1024 + 16384);}
-	const unsigned *d_z = dev_z ? b->zix_xy : s_z;
+	McTables const T = tabs ? mc_tables(tab) : McTables{};
+	float *const d_v = v.d;
 	twi_job pending;
 	pending.cancellable = true;
 	pending.complete = [st, ntris = mc ? b->ntris : nullptr, changed = b->changed, nverts = M.nverts, mesh_ntris = M.ntris](tw_ctx *) -> int {
@@ -802,22 +806,12 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 	};
 	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(cnt, 0, 256, ctx->stream));
-		if (fill) {int const r = twi_voxel_fill(ctx, &F, b->rdata420, d_v, h_rdata); if (r) return r;}
-		else if (!dev_v) {TW_CUDA(ctx, cudaMemcpyAsync(d_v, b->vals, n*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
-		if (stage_z) {memcpy(h_z, b->zix_xy, nxy*sizeof(unsigned)); TW_CUDA(ctx, cudaMemcpyAsync(s_z, h_z, nxy*sizeof(unsigned), cudaMemcpyHostToDevice, ctx->stream));}
-		if (tabs) {
-			const void *src[3] = {b->edge_table256, b->tri_table256x16, b->edge_to_vals12x2};
-			size_t const off[3] = {0, 1024, 1024 + 16384}, len[3] = {1024, 16384, 96};
-			for (int k = 0; k < 3; ++k) {
-				// host tables are copied during the launch; device tables are read by the job
-				if (tw_is_device_ptr(src[k])) {TW_CUDA(ctx, cudaMemcpyAsync(tab + off[k], src[k], len[k], cudaMemcpyDeviceToDevice, ctx->stream)); continue;}
-				memcpy(h_tab + off[k], src[k], len[k]);
-				TW_CUDA(ctx, cudaMemcpyAsync(tab + off[k], h_tab + off[k], len[k], cudaMemcpyHostToDevice, ctx->stream));
-			}
-		}
-		outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(d_v, P, d_z, d_o, n);
+		int r = fill ? twi_voxel_fill(ctx, &F, b->rdata420, d_v, h_rdata) : v.in(ctx); if (r) return r;
+		r = z.in(ctx); if (r) return r;
+		if (tabs) {r = mc_tables_upload(ctx, tab, b->edge_table256, b->tri_table256x16, b->edge_to_vals12x2, h_tab); if (r) return r;}
+		outside_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(d_v, P, z.d, d_o, n);
 		TW_LAUNCH_CHECK(ctx);
-		if (rm) {int const r = enqueue_remove_unconnected(ctx, blocks, d_v, d_o, &P, f0, f1, cnt, d_changed); if (r) return r;}
+		if (rm) {r = enqueue_remove_unconnected(ctx, blocks, d_v, d_o, &P, f0, f1, cnt, d_changed); if (r) return r;}
 		if (mc) {
 			mc_kernel<false><<<nblocks, MC_BLOCK, 0, ctx->stream>>>(d_v, d_o, P, T, n, d_sums, nullptr, nullptr, 0);
 			TW_LAUNCH_CHECK(ctx);
@@ -828,8 +822,8 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 				TW_LAUNCH_CHECK(ctx);
 			}
 		}
-		if (wm) {int const r = enqueue_mesh(ctx, d_v, d_o, P, T, S, d_mv, M.vcapacity, d_mi, M.tcapacity); if (r) return r;}
-		if (b->vals && !dev_v && (fill || rm)) {TW_CUDA(ctx, cudaMemcpyAsync(b->vals, d_v, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+		if (wm) {r = enqueue_mesh(ctx, d_v, d_o, P, T, S, d_mv, M.vcapacity, d_mi, M.tcapacity); if (r) return r;}
+		if (fill || rm) {r = v.out(ctx); if (r) return r;}
 		if (b->outside) {TW_CUDA(ctx, cudaMemcpyAsync(b->outside, d_o, n, cudaMemcpyDefault, ctx->stream));}
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->ntris, d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		TW_CUDA(ctx, cudaMemcpyAsync(&st->changed, d_changed, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1028,12 +1022,6 @@ __global__ void diff_kernel(const float *__restrict__ nv, const unsigned char *_
 }
 
 BlockGrid block_grid(const tw_voxel_model *m) {BlockGrid G; G.bx = m->bx; G.by = m->by; G.nbx = m->nbx; G.chunks = m->chunks; return G;}
-McTables model_tables(const tw_voxel_model *m) {
-	McTables T;
-	T.edge_table = (const unsigned *)m->tables; T.tri_table = (const int *)((const char *)m->tables + 1024);
-	T.edge_to_vals = (const unsigned *)((const char *)m->tables + 1024 + 16384);
-	return T;
-}
 
 // A model job's counts in its pinned staging
 struct twi_vmodel_stage {unsigned long long nblocks, nverts, ntris, changed;};
@@ -1078,7 +1066,7 @@ int enqueue_block_meshes(tw_voxel_model *m, const unsigned *d_list, const ModelS
 	twi_vmodel_stage *const st = X.h_stage;
 	if (m->nblocks) {
 		unsigned const ng = m->nblocks*m->chunks;
-		McTables const T = model_tables(m);
+		McTables const T = mc_tables(m->tables);
 		BlockGrid const G = block_grid(m);
 		MeshScratch const &S = X.S;
 		block_mesh_kernel<false><<<ng, MC_BLOCK, 0, ctx->stream>>>(m->post, m->post_o, m->P, T, G, d_list, S.words, S.vsums, S.tsums, nullptr, nullptr, nullptr, 0, nullptr, 0);
@@ -1139,7 +1127,7 @@ extern "C" int tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp
 	auto layout = [&](twi_carve &c) {
 		m->raw = c.take<float>(n); m->post = c.take<float>(n); m->work = c.take<float>(n);
 		m->raw_o = c.take<unsigned char>(n + 4); m->post_o = c.take<unsigned char>(n + 4); m->work_o = c.take<unsigned char>(n + 4);
-		m->zix = zix_xy ? c.take<unsigned>(nxy) : nullptr; m->tables = c.take<char>(1024 + 16384 + 96); m->mark = c.take<unsigned char>((size_t)nblocks + 1);
+		m->zix = zix_xy ? c.take<unsigned>(nxy) : nullptr; m->tables = c.take<char>(MC_TAB_BYTES); m->mark = c.take<unsigned char>((size_t)nblocks + 1);
 		m->all = c.take<unsigned>((size_t)nblocks + 1); m->marked = c.take<unsigned>((size_t)nblocks + 1);
 	};
 	twi_carve c;
@@ -1153,9 +1141,8 @@ extern "C" int tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp
 	std::vector<unsigned> all((size_t)nblocks + 1);
 	all[0] = nblocks;
 	for (unsigned b = 0; b < nblocks; ++b) {all[1 + b] = b;}
-	rc = TW_OK;
+	rc = mc_tables_upload(ctx, m->tables, edge_table256, tri_table256x16, edge_to_vals12x2);
 	auto up = [&](void *dst, const void *src, size_t len) {if (rc == TW_OK && cudaMemcpyAsync(dst, src, len, cudaMemcpyDefault, ctx->stream) != cudaSuccess) rc = TW_ERR_CUDA;};
-	up(m->tables, edge_table256, 1024); up((char *)m->tables + 1024, tri_table256x16, 16384); up((char *)m->tables + 1024 + 16384, edge_to_vals12x2, 96);
 	if (zix_xy) {up(m->zix, zix_xy, nxy*sizeof(unsigned));}
 	up(m->all, all.data(), all.size()*sizeof(unsigned));
 	if (rc == TW_OK && cudaMemsetAsync(m->mark, 0, nblocks + 1, ctx->stream) != cudaSuccess) rc = TW_ERR_CUDA;

@@ -120,6 +120,13 @@ struct NoiseParams {
 	float hmap_scale;            // get_hmap_scale(mode)
 	float freq_last, rsum_last;  // freq / (rx+ry) of the last octave: bound of the lattice coordinates (paired-path range guard)
 };
+// Windowed domain-warp kernel (twn2::DWARP_WIN_OCTAVES, dwarp_windows()): per fBm stage, the box {x_lo, y_lo, x_hi, y_hi} of fBm input coordinates the
+// windows hold for, and per stage and windowed octave the table-base shifts {-128*c_x, -16*c_y} as denormals (bits = the byte offsets). A kernel
+// parameter of its own, so that the other kernels taking NoiseParams keep their parameter layout.
+struct DwarpWindows {
+	float4 box[5];
+	float2 win[5][twn2::DWARP_WIN_OCTAVES];
+};
 
 template<bool SIMPLEX, int SHAPE>
 __device__ __forceinline__ float gen_noise(float xv, float yv, const NoiseParams &N) { // src/mesh_gen.cpp:706-730
@@ -190,13 +197,19 @@ noise_grid_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y_
 #ifndef TW_NOISE2_THREADS
 #define TW_NOISE2_THREADS 512    // threads per block (256 x 3 blocks = 24 warps per SM at 80 registers: 0.7 % slower on the headline, results/h100/launch_shape.txt)
 #endif
+#ifndef TW_DWARP_WIN_THREADS
+#define TW_DWARP_WIN_THREADS ((TW_DWARP_WIN_OCTAVES > 5) ? 1024 : 512)   // windowed domain-warp kernel: one block of 1024 threads per SM holds the 161 KB of
+                                                                       // tables at 7 windowed octaves, two blocks of 512 the 101 KB at 5
+#endif
 #ifndef TW_NOISE2_BLOCK_CELLS
 // Cells per block in every mode, walked as chunks of 2*TW_NOISE2_THREADS cells: the 74 KB table fill is paid once per block (the plain modes run
 // only 8 evaluations per cell), and a 258^2 tile (66564 cells) leaves 1.5 % of the cells of its last block idle. One H100, 8192^2 headline at
 // 256 threads: 512 -> 9.76 ms, 1024 -> 9.31, 2048 -> 9.13, 4096 -> 9.15 (results/h100/warp_chunks.txt)
 #define TW_NOISE2_BLOCK_CELLS 2048
 #endif
-static_assert(TW_NOISE2_BLOCK_CELLS % (2*TW_NOISE2_THREADS) == 0, "a block walks whole chunks of 2 cells per thread");
+static_assert(TW_NOISE2_BLOCK_CELLS % (2*TW_NOISE2_THREADS) == 0 && TW_NOISE2_BLOCK_CELLS % (2*TW_DWARP_WIN_THREADS) == 0, "a block walks whole chunks of 2 cells per thread");
+template<bool WIN> __host__ __device__ constexpr int noise2_threads() {return WIN ? TW_DWARP_WIN_THREADS : TW_NOISE2_THREADS;}
+template<bool WIN> __host__ __device__ constexpr int noise2_min_blocks() {return WIN ? 1024/TW_DWARP_WIN_THREADS : TW_NOISE2_MIN_BLOCKS;} // 32 warps per SM either way
 // ---- paired variant: two horizontally adjacent cells per thread (see tw_noise2.cuh) ----
 // |lattice coordinate| < 2^22 for every octave of this fBm call (needed by the division-free mod); NaN-safe
 __device__ __forceinline__ bool noise_lattice_in_range(float2 xv, float2 yv, const NoiseParams &N) {
@@ -208,35 +221,63 @@ __device__ __forceinline__ bool noise_lattice_in_range(float2 xv, float2 yv, con
 // repaid by the 40 evaluations per cell of that mode; plain simplex, 8 evaluations per cell, measured 8 % slower with the earlier (37 KB) form of it
 // at one block per 2048 cells (as tile batches launch).
 template<bool SIMPLEX, bool WARP> __host__ __device__ constexpr bool noise2_hash() {return SIMPLEX && WARP && TW_SIMPLEX_HASH_TABLE;}
-// entries of the table a block stages: the gradient table, and the hash table behind it
-template<bool HASH> __host__ __device__ constexpr int lut_entries() {return twn2::SIMPLEX_LUT_N + (HASH ? twn2::SIMPLEX_HASH_N : 0);}
+// entries of the gradient table a block stages, and of the hash table behind it (WIN: the windowed kernel's repeating tables, tw_noise2.cuh)
+template<bool WIN> __host__ __device__ constexpr int lut_grad_n() {return WIN ? twn2::SIMPLEX_WLUT_N : twn2::SIMPLEX_LUT_N;}
+template<bool HASH, bool WIN> __host__ __device__ constexpr int lut_hash_n() {return !HASH ? 0 : WIN ? twn2::SIMPLEX_WHASH_N : twn2::SIMPLEX_HASH_N;}
+template<bool HASH> __host__ __device__ constexpr int lut_entries() {return lut_grad_n<false>() + lut_hash_n<HASH, false>();}
 // float4 slots a block stages: 8 copies of the gradient table, then SIMPLEX_HASH_COPIES of the hash table
-template<bool HASH> __host__ __device__ constexpr int lut_slots() {return twn2::SIMPLEX_LUT_N*twn2::SIMPLEX_LUT_COPIES + (HASH ? twn2::SIMPLEX_HASH_N*twn2::SIMPLEX_HASH_COPIES : 0);}
+template<bool HASH, bool WIN = false> __host__ __device__ constexpr int lut_slots() {return lut_grad_n<WIN>()*twn2::SIMPLEX_LUT_COPIES + lut_hash_n<HASH, WIN>()*twn2::SIMPLEX_HASH_COPIES;}
+// byte distance from the gradient table to the hash table in shared memory
+template<bool WIN> __host__ __device__ constexpr unsigned lut_hash_offset() {return lut_grad_n<WIN>()*twn2::LUT_ENTRY_BYTES;}
 
-// one octave of gen_noise for two cells
-template<bool SIMPLEX, int SHAPE, bool HASH>
+// one octave of gen_noise for two cells (H: see lut_hash_offset)
+template<bool SIMPLEX, int SHAPE, bool HASH, unsigned H = twn2::SIMPLEX_HASH_OFFSET>
 __device__ __forceinline__ float2 noise2_octave(float2 xv, float2 yv, float4 o, unsigned L, float2 zval) {
 	float2 const px = twn2::add2(twn2::mul2(xv, o.x), o.y), py = twn2::add2(twn2::mul2(yv, o.x), o.z); // o = {freq, rx, ry, mag}
-	float2 noise = SIMPLEX ? ((TW_SIMPLEX_LUT > 0) ? twn2::simplex2_lut<HASH>(px, py, L) : twn2::simplex2(px, py)) : ((TW_SIMPLEX_LUT > 0) ? twn2::perlin2_lut(px, py, L) : twn2::perlin2(px, py));
+	float2 noise = SIMPLEX ? ((TW_SIMPLEX_LUT > 0) ? twn2::simplex2_lut<HASH, H>(px, py, L) : twn2::simplex2(px, py)) : ((TW_SIMPLEX_LUT > 0) ? twn2::perlin2_lut(px, py, L) : twn2::perlin2(px, py));
 	if (SHAPE == 1) {noise = make_float2((float)((double)fabsf(noise.x) - 0.40), (float)((double)fabsf(noise.y) - 0.40));}
 	if (SHAPE == 2) {noise = make_float2((float)(0.45 - (double)fabsf(noise.x)), (float)(0.45 - (double)fabsf(noise.y)));}
 	return twn2::fma2(noise, o.w, zval); // mag is a power of two: exact product
 }
 
-template<bool SIMPLEX, int SHAPE, bool HASH>
-__device__ __forceinline__ float2 gen_noise2(float2 xv, float2 yv, const NoiseParams &N, unsigned L) { // gen_noise (src/mesh_gen.cpp:706-730) for two cells; L: simplex table base (twn2::simplex_lut_base) or 0
+// one windowed octave (shape 0, 8 octaves; see twn2::DWARP_WIN_OCTAVES): gb, hb = the thread's gradient / hash table bases as denormals, w = the
+// stage's and octave's shifts; both cells share the stage, so the two exact adds serve the pair
+template<unsigned H>
+__device__ __forceinline__ float2 noise2_octave_win(float2 xv, float2 yv, float4 o, unsigned L, float gb, float hb, float2 w, float2 zval) {
+	float2 const px = twn2::add2(twn2::mul2(xv, o.x), o.y), py = twn2::add2(twn2::mul2(yv, o.x), o.z);
+	float2 const noise = twn2::simplex2_lut<true, H, true>(px, py, L, make_float2(__fadd_rn(gb, w.x), __fadd_rn(hb, w.y)));
+	return twn2::fma2(noise, o.w, zval);
+}
+
+// WIN: the windowed domain-warp kernel; s = the fBm stage of the domain warp (selects the box and the windows)
+template<bool SIMPLEX, int SHAPE, bool HASH, bool WIN = false>
+__device__ __forceinline__ float2 gen_noise2(float2 xv, float2 yv, const NoiseParams &N, unsigned L, const DwarpWindows *W = nullptr, int s = 0) { // gen_noise (src/mesh_gen.cpp:706-730) for two cells; L: simplex table base (twn2::simplex_lut_base) or 0
+	constexpr unsigned H = lut_hash_offset<WIN>();
 	float2 zval = make_float2(0.0f, 0.0f);
+	if (WIN) {
+		static_assert(!WIN || (SIMPLEX && HASH && SHAPE == 0), "windows exist for the domain-warp simplex kernel at shape 0");
+		float4 const b = W->box[s];
+		if (xv.x >= b.x && xv.y >= b.x && yv.x >= b.y && yv.y >= b.y && xv.x <= b.z && xv.y <= b.z && yv.x <= b.w && yv.y <= b.w) { // inside the stage's box (NaN: outside)
+			float const gb = __uint_as_float(L), hb = __uint_as_float(L - (threadIdx.x & (twn2::SIMPLEX_LUT_COPIES - 1))*16u);
+#pragma unroll
+			for (int i = 0; i < 8; ++i) {
+				if (i < twn2::DWARP_WIN_OCTAVES) {zval = noise2_octave_win<H>(xv, yv, N.oct[i], L, gb, hb, W->win[s][i < twn2::DWARP_WIN_OCTAVES ? i : 0], zval);}
+				else {zval = noise2_octave<SIMPLEX, SHAPE, HASH, H>(xv, yv, N.oct[i], L, zval);}
+			}
+			return zval;
+		}
+	}
 	bool const in_range = noise_lattice_in_range(xv, yv, N);
-	if (HASH && SHAPE == 0 && N.octaves == 8 && in_range) {
+	if (!WIN && HASH && SHAPE == 0 && N.octaves == 8 && in_range) {
 		// The domain-warp kernel at 8 octaves (mesh_freq_filter 1: the headline, config 5, the tile jobs) runs the same octaves in the same order
 		// fully unrolled: with a constant index the octave constants need no counter, address arithmetic or branch (164 instead of 169 instructions
 		// per octave). Shapes 1 and 2 keep the rolled loop: their double-precision shaping pushes the unrolled kernel past 64 registers (spills).
 #pragma unroll
 		for (int i = 0; i < 8; ++i) {zval = noise2_octave<SIMPLEX, SHAPE, HASH>(xv, yv, N.oct[i], L, zval);}
 	}
-	else if (in_range) {
+	else if (in_range) { // (windowed kernel: a pair outside its box, which a sound margin never leaves)
 #pragma unroll 1
-		for (int i = 0; i < N.octaves; ++i) {zval = noise2_octave<SIMPLEX, SHAPE, HASH>(xv, yv, N.oct[i], L, zval);}
+		for (int i = 0; i < N.octaves; ++i) {zval = noise2_octave<SIMPLEX, SHAPE, HASH, H>(xv, yv, N.oct[i], L, zval);}
 	}
 	else {zval = make_float2(gen_noise<SIMPLEX, SHAPE>(xv.x, yv.x, N), gen_noise<SIMPLEX, SHAPE>(xv.y, yv.y, N));} // astronomically far out: scalar path with the literal division
 	return zval;
@@ -270,18 +311,20 @@ __device__ __forceinline__ void gen_noise2_dual(float2 xa, float2 ya, float2 xb,
 __device__ __forceinline__ float dadd(float a, double b) {return (float)((double)a + b);} // float + double literal, rounded back (src/mesh_gen.cpp:742-745)
 __constant__ double2 warp_offsets[4] = {{0.0, 0.0}, {5.2, 1.3}, {1.7, 9.2}, {8.3, 2.8}}; // the domain warp's offsets per stage (src/mesh_gen.cpp:742-745)
 
-template<bool SIMPLEX, bool WARP, int SHAPE>
-__global__ void __launch_bounds__(TW_NOISE2_THREADS, TW_NOISE2_MIN_BLOCKS)
+// WIN: the windowed domain-warp kernel (single grids, shape 0, 8 octaves; dwarp_windows() on the host)
+template<bool SIMPLEX, bool WARP, int SHAPE, bool WIN = false>
+__global__ void __launch_bounds__(noise2_threads<WIN>(), noise2_min_blocks<WIN>())
 noise_grid2_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y_off, unsigned y_end, float mx0_single, float my0_single, const float2 *__restrict__ tile_origins,
-	NoiseParams N, PostParams P, const float *__restrict__ sin_tab, unsigned *__restrict__ mm, const float4 *__restrict__ simplex_lut)
+	NoiseParams N, PostParams P, const float *__restrict__ sin_tab, unsigned *__restrict__ mm, const float4 *__restrict__ simplex_lut, DwarpWindows W)
 {
 	constexpr bool HASH = noise2_hash<SIMPLEX, WARP>();
+	static_assert(!WIN || !TW_NOISE2_DUAL, "the windowed kernel runs the five fBm calls as one stage loop");
 	unsigned L = 0;
 	if (TW_SIMPLEX_LUT > 0) { // hash/gradient table (simplex or Perlin flavour) -> shared memory, 8 interleaved copies (see tw_noise2.cuh)
-		extern __shared__ float4 lut_s[]; // lut_slots<HASH>() entries (dynamic: 74 KB at level 3, + 4.6 KB of hash table)
-		constexpr int G = twn2::SIMPLEX_LUT_N*twn2::SIMPLEX_LUT_COPIES;
-		for (int e = threadIdx.x; e < lut_slots<HASH>(); e += blockDim.x) {
-			lut_s[e] = __ldg(simplex_lut + ((e < G) ? e/twn2::SIMPLEX_LUT_COPIES : twn2::SIMPLEX_LUT_N + (e - G)/twn2::SIMPLEX_HASH_COPIES));
+		extern __shared__ float4 lut_s[]; // lut_slots<HASH, WIN>() entries (dynamic: 74 KB at level 3, + 4.6 KB of hash table; windowed: see tw_noise2.cuh)
+		constexpr int G = lut_grad_n<WIN>()*twn2::SIMPLEX_LUT_COPIES;
+		for (int e = threadIdx.x; e < lut_slots<HASH, WIN>(); e += blockDim.x) {
+			lut_s[e] = __ldg(simplex_lut + ((e < G) ? e/twn2::SIMPLEX_LUT_COPIES : lut_grad_n<WIN>() + (e - G)/twn2::SIMPLEX_HASH_COPIES));
 		}
 		__syncthreads();
 		L = twn2::simplex_lut_base(lut_s, threadIdx.x);
@@ -327,7 +370,7 @@ noise_grid2_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y
 				                            // dx2 = noise(wx + 1.7, wy + 9.2), dy2 = noise(wx + 8.3, wy + 2.8), z = noise(v + scale*(dx2, dy2))
 				float2 sx = xv, sy = yv;
 				if (s < 4) {double2 const o = warp_offsets[s]; sx = make_float2(dadd(bx.x, o.x), dadd(bx.y, o.x)); sy = make_float2(dadd(by.x, o.y), dadd(by.y, o.y));}
-				float2 const r = gen_noise2<SIMPLEX, SHAPE, HASH>(sx, sy, N, L);
+				float2 const r = gen_noise2<SIMPLEX, SHAPE, HASH, WIN>(sx, sy, N, L, &W, s);
 				if (s == 1) {bx = add2(xv, mul2(d, scale)); by = add2(yv, mul2(r, scale));} // wx, wy
 				if (s == 3) {xv = add2(xv, mul2(d, scale)); yv = add2(yv, mul2(r, scale));}
 				d = r; // dx1 / dx2 for the next stage; the last stage's is the result
@@ -369,6 +412,14 @@ noise_grid2_kernel(float *__restrict__ out, unsigned nx, unsigned ny, unsigned y
 	if (mm) {block_minmax(lo, hi, mm + 2*tile);}
 }
 
+void launch_noise2_win(dim3 grid, dim3 block, cudaStream_t st, float *out, unsigned nx, unsigned ny, unsigned y_off, unsigned y_end, float mx0, float my0,
+	const NoiseParams &N, const PostParams &P, const float *tab, unsigned *mm, const float4 *lut, const DwarpWindows &W)
+{
+	size_t const lut_bytes = (size_t)lut_slots<true, true>()*sizeof(float4);
+	cudaFuncSetAttribute(noise_grid2_kernel<true, true, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lut_bytes); // per launch, see launch_noise2
+	noise_grid2_kernel<true, true, 0, true><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, nullptr, N, P, tab, mm, lut, W);
+}
+
 template<bool SIMPLEX, bool WARP>
 void launch_noise2(int shape, dim3 grid, dim3 block, cudaStream_t st, float *out, unsigned nx, unsigned ny, unsigned y_off, unsigned y_end, float mx0, float my0,
 	const float2 *origins, const NoiseParams &N, const PostParams &P, const float *tab, unsigned *mm, const float4 *lut)
@@ -384,24 +435,29 @@ void launch_noise2(int shape, dim3 grid, dim3 block, cudaStream_t st, float *out
 		}
 	}
 	switch (shape) {
-	case 1:  noise_grid2_kernel<SIMPLEX, WARP, 1><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, origins, N, P, tab, mm, lut); break;
-	case 2:  noise_grid2_kernel<SIMPLEX, WARP, 2><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, origins, N, P, tab, mm, lut); break;
-	default: noise_grid2_kernel<SIMPLEX, WARP, 0><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, origins, N, P, tab, mm, lut); break;
+	case 1:  noise_grid2_kernel<SIMPLEX, WARP, 1><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, origins, N, P, tab, mm, lut, DwarpWindows()); break;
+	case 2:  noise_grid2_kernel<SIMPLEX, WARP, 2><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, origins, N, P, tab, mm, lut, DwarpWindows()); break;
+	default: noise_grid2_kernel<SIMPLEX, WARP, 0><<<grid, block, lut_bytes, st>>>(out, nx, ny, y_off, y_end, mx0, my0, origins, N, P, tab, mm, lut, DwarpWindows()); break;
 	}
 }
 
 constexpr int PERLIN_LUT_OFFSET = lut_entries<true>();
-__global__ void simplex_lut_kernel(float4 *__restrict__ lut) { // [0, N): simplex table, [N, N + H): simplex hash table, [N + H, 2N + H): Perlin table
+constexpr int WIN_LUT_OFFSET = PERLIN_LUT_OFFSET + twn2::SIMPLEX_LUT_N;
+// [0, N): simplex table, [N, N + H): simplex hash table, [N + H, 2N + H): Perlin table, then the windowed kernel's repeating simplex and hash tables
+__global__ void simplex_lut_kernel(float4 *__restrict__ lut) {
 	int const k = blockIdx.x*blockDim.x + threadIdx.x;
 	if (k < twn2::SIMPLEX_LUT_N) {lut[k] = twn2::simplex_lut_entry((float)k); lut[PERLIN_LUT_OFFSET + k] = twn2::perlin_lut_entry((float)k);}
 	if (k < twn2::SIMPLEX_HASH_N) {lut[twn2::SIMPLEX_LUT_N + k] = twn2::simplex_hash_entry((float)k);}
+	if (k < twn2::SIMPLEX_WLUT_N) {lut[WIN_LUT_OFFSET + k] = twn2::simplex_lut_entry((float)(k % 289));}
+	if (k < twn2::SIMPLEX_WHASH_N) {lut[WIN_LUT_OFFSET + twn2::SIMPLEX_WLUT_N + k] = twn2::simplex_hash_entry((float)(k % 289));} // permute(288 + 1) is exact: = permute(0)
 }
 } // namespace
 int twi_ensure_simplex_lut(tw_ctx *ctx) {
 	if (ctx->d_simplex_lut) return TW_OK;
-	static_assert(twn2::SIMPLEX_HASH_N <= twn2::SIMPLEX_LUT_N, "simplex_lut_kernel's grid covers the gradient tables");
-	TW_CUDA(ctx, cudaMalloc(&ctx->d_simplex_lut, (PERLIN_LUT_OFFSET + twn2::SIMPLEX_LUT_N)*sizeof(float4)));
-	simplex_lut_kernel<<<(twn2::SIMPLEX_LUT_N + 127)/128, 128, 0, ctx->stream>>>((float4 *)ctx->d_simplex_lut);
+	static_assert(twn2::SIMPLEX_HASH_N <= twn2::SIMPLEX_LUT_N && twn2::SIMPLEX_WHASH_N <= twn2::SIMPLEX_WLUT_N && twn2::SIMPLEX_LUT_N <= twn2::SIMPLEX_WLUT_N,
+	              "simplex_lut_kernel's grid covers the windowed gradient table");
+	TW_CUDA(ctx, cudaMalloc(&ctx->d_simplex_lut, (WIN_LUT_OFFSET + twn2::SIMPLEX_WLUT_N + twn2::SIMPLEX_WHASH_N)*sizeof(float4)));
+	simplex_lut_kernel<<<(twn2::SIMPLEX_WLUT_N + 127)/128, 128, 0, ctx->stream>>>((float4 *)ctx->d_simplex_lut);
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }
@@ -678,6 +734,47 @@ static bool make_noise_params(const tw_height_params *p, NoiseParams &N, bool &s
 	return true;
 }
 
+// Windows of the domain-warp kernel (twn2::DWARP_WIN_OCTAVES) for the cells [0, nx) x [r0, r1) of one grid: per fBm stage, the box of its input
+// coordinates (stages 0 and 1: the cells' exact extent plus the stage offset; stages 2-4 also read the warp, whose displacement |0.2*d| stays below
+// WARP_MARGIN: |simplex| <= 1 and the octave weights sum to < 2), and per windowed octave the lattice window at the box's corners. Each step from
+// (x, y) to the lattice indices - px = f*x + rx, s = px*Cy + py*Cy, floor(p + s), all rounded as the kernel rounds them - is monotone non-decreasing
+// in both coordinates (f, Cy > 0), so the two corners bound every cell inside the box exactly; the kernel checks each pair against the box and
+// takes the reducing loop outside it. false: a window is wider than the tables (large grids, far-out origins) or not finite - keep the reducing kernel.
+#ifndef TW_DWARP_WARP_MARGIN
+#define TW_DWARP_WARP_MARGIN 0.45f   // a build with a margin below the displacement sends pairs of stages 2-4 outside their box (the path the tests check it with)
+#endif
+static bool dwarp_windows(DwarpWindows &W, const NoiseParams &N, const PostParams &P, unsigned nx, unsigned r0, unsigned r1, float mx0, float my0) {
+	constexpr float WARP_MARGIN = TW_DWARP_WARP_MARGIN, Cy = 0.366025403784439f;
+	auto coord = [&](unsigned i, float md, float m0, float inv) {return (((float)i*md + m0)*inv)*N.xy_scale;}; // xv, yv as the kernel computes them
+	float const xa = coord(0, P.mdx, mx0, P.dx_inv), xb = coord(nx - 1, P.mdx, mx0, P.dx_inv), ya = coord(r0, P.mdy, my0, P.dy_inv), yb = coord(r1 - 1, P.mdy, my0, P.dy_inv);
+	static const double off[5][2] = {{0.0, 0.0}, {5.2, 1.3}, {1.7, 9.2}, {8.3, 2.8}, {0.0, 0.0}}; // warp_offsets, stage 4 none
+	for (int s = 0; s < 5; ++s) {
+		float const m = (s >= 2) ? WARP_MARGIN : 0.0f;
+		float4 &b = W.box[s];
+		b.x = (float)((double)(std::min(xa, xb) - m) + off[s][0]); b.z = (float)((double)(std::max(xa, xb) + m) + off[s][0]); // dadd(), monotone
+		b.y = (float)((double)(std::min(ya, yb) - m) + off[s][1]); b.w = (float)((double)(std::max(ya, yb) + m) + off[s][1]);
+		for (int o = 0; o < twn2::DWARP_WIN_OCTAVES; ++o) {
+			float4 const c = N.oct[o];
+			float lo[2], hi[2];
+			for (int k = 0; k < 2; ++k) {
+				float const x = k ? b.z : b.x, y = k ? b.w : b.y;
+				float const px = c.x*x + c.y, py = c.x*y + c.z, sk = px*Cy + py*Cy;
+				float *i = k ? hi : lo;
+				i[0] = floorf(px + sk); i[1] = floorf(py + sk);
+			}
+			long sh[2];
+			for (int a = 0; a < 2; ++a) {
+				if (!(fabsf(lo[a]) < 32768.0f && fabsf(hi[a]) < 32768.0f && hi[a] - lo[a] <= (float)twn2::DWARP_WIN_SPAN)) return false; // NaN fails too
+				long const l = (long)lo[a];
+				sh[a] = (a ? -16L : -128L)*289L*((l >= 0) ? l/289 : -((288 - l)/289)); // -128*c_x, -16*c_y; c = 289*floor(lo/289), |shift| < 2^23
+			}
+			auto denorm = [](long v) {uint32_t const u = (v < 0) ? (0x80000000u | (uint32_t)(-v)) : (uint32_t)v; float f; memcpy(&f, &u, 4); return f;}; // bits = |v|, sign
+			W.win[s][o] = make_float2(denorm(sh[0]), denorm(sh[1]));
+		}
+	}
+	return true;
+}
+
 size_t twi_heightgen_slot1_bytes(const tw_grid2d *g, const tw_height_params *p) { // the sine-table mode's X / Y tables below
 	if (p->gen_mode != TW_MGEN_SINE) return 0;
 	unsigned const xpitch = (g->nx + 63) & ~63u, ypitch = (g->ny + 63) & ~63u;
@@ -715,6 +812,15 @@ int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, in
 #if TW_NOISE2_PERSISTENT
 				{unsigned const wave = ctx->num_sms*TW_NOISE2_MIN_BLOCKS*TW_NOISE2_PERSISTENT; if (ntiles == 1 && gx > wave) gx = wave;} // TW_NOISE2_PERSISTENT waves' worth of resident blocks
 #endif
+				DwarpWindows W;
+				if (warp && !d_tile_origins && p->gen_shape == 0 && N.octaves == 8 && !TW_NOISE2_DUAL && dwarp_windows(W, N, P, nx, r0, r1, mx0, my0)) {
+					unsigned const wave = ctx->num_sms*noise2_min_blocks<true>()*TW_NOISE2_PERSISTENT;
+					launch_noise2_win(dim3((TW_NOISE2_PERSISTENT && gx > wave) ? wave : gx), dim3(noise2_threads<true>()), ctx->stream, d_out, nx, ny, r0, r1, mx0, my0, N, P,
+					                  ctx->d_sin_table, d_mm_ord, (const float4 *)ctx->d_simplex_lut + WIN_LUT_OFFSET, W);
+					TW_LAUNCH_CHECK(ctx);
+					if (h_out_bands) {int const rc = band_copy(ctx, h_out_bands, d_out, nx, r0, r1); if (rc) return rc;}
+					continue;
+				}
 				dim3 const block(TW_NOISE2_THREADS, 1, 1), grid(gx, 1, ntiles);
 				if (p->gen_mode == TW_MGEN_PERLIN) {launch_noise2<false, false>(p->gen_shape, grid, block, ctx->stream, d_out, nx, ny, r0, r1, mx0, my0, d_tile_origins, N, P, ctx->d_sin_table, d_mm_ord, lut);}
 				else if (warp) {launch_noise2<true, true >(p->gen_shape, grid, block, ctx->stream, d_out, nx, ny, r0, r1, mx0, my0, d_tile_origins, N, P, ctx->d_sin_table, d_mm_ord, lut);}

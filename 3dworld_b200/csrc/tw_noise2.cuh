@@ -191,23 +191,46 @@ template<unsigned OFF> __device__ __forceinline__ float lut_load_f32(unsigned ad
 	return v;
 }
 
-// gradient-table offsets of the three corners of two cells from the simplex hash table (ix, iy: lattice indices after mod_int289_lazy)
-__device__ __forceinline__ void simplex_hash_offsets(f2 ix, f2 iy, f2 i1y, unsigned Lb, f2 &k0, f2 &k1, f2 &k2) {
-	constexpr unsigned H = SIMPLEX_HASH_OFFSET, PITCH = 16u*SIMPLEX_HASH_COPIES;
-	unsigned const base = Lb - (threadIdx.x & (SIMPLEX_LUT_COPIES - 1))*16u; // Lb without the lane's copy offset: the hash table's one copy
-	f2 const j0 = raw_fma(iy, splat(__uint_as_float(PITCH)), splat(__uint_as_float(base))); // address of entry iy of the hash table, less H (exact, as lut_offsets)
-	f2 const j1 = raw_fma(i1y, splat(__uint_as_float(PITCH - 4)), j0);                       // + pitch - 4 bytes when i1.y = 1 (see simplex_hash_entry)
+// Domain-warp windows (the headline kernel, tw_heightgen.cu): one launch of the domain-warp kernel only reaches a small window of lattice indices
+// per fBm stage and octave, [ix_lo, ix_lo + span] x [iy_lo, iy_lo + span], which the host evaluates exactly. With c = 289*floor(lo/289), the shifted
+// index i - c lies in [0, 288 + span]; tables that repeat themselves every 289 entries then give, at i - c, the bits the 580-entry tables give at
+// mod 289 of i, and the octave needs no reduction (12 instructions per cell pair: FMUL, FRND, FFMA per coordinate and cell). The shift is folded into
+// the table bases (one exact denormal add each, shared by the two cells). Octaves 0 .. DWARP_WIN_OCTAVES-1 take this form; the last octaves' windows
+// would need larger tables and keep the reduction.
+//   gradient table: entry k = simplex_lut_entry(k mod 289), k <= P + (i - c) + 1 <= 577 + span
+//   hash table:     entry r = simplex_hash_entry(r mod 289), r <= (i - c) + 1 <= 289 + span
+// Both are built from k mod 289: permute() is exact only while (34k + 1)k < 2^24.
+// TW_DWARP_WIN_OCTAVES 7: 161 KB of tables, one block of 1024 threads per SM; 5: 101 KB, two blocks of 512 (both 32 warps at 64 registers).
+#ifndef TW_DWARP_WIN_OCTAVES
+#define TW_DWARP_WIN_OCTAVES 7
+#endif
+constexpr int DWARP_WIN_OCTAVES = TW_DWARP_WIN_OCTAVES;
+constexpr int DWARP_WIN_SPAN = (DWARP_WIN_OCTAVES > 5) ? 600 : 170;   // widest window the tables hold (8192^2 headline: 576 at octave 6, 157 at octave 4)
+constexpr int SIMPLEX_WLUT_N = 578 + DWARP_WIN_SPAN;
+constexpr int SIMPLEX_WHASH_N = 290 + DWARP_WIN_SPAN;
+static_assert(DWARP_WIN_OCTAVES >= 1 && DWARP_WIN_OCTAVES <= 8, "windowed octaves of the 8-octave body");
+
+// gradient-table offsets of the three corners of two cells from the simplex hash table (ix, iy: lattice indices after mod_int289_lazy, or shifted into
+// a window). H: byte distance from the gradient table to the hash table; gb: denormal whose bits are the address of the lane's copy of gradient
+// entry 0 (Lb), hb: the same for hash entry 0, less H; a window's shift is folded into both.
+template<unsigned H>
+__device__ __forceinline__ void simplex_hash_offsets(f2 ix, f2 iy, f2 i1y, float gb, float hb, f2 &k0, f2 &k1, f2 &k2) {
+	constexpr unsigned PITCH = 16u*SIMPLEX_HASH_COPIES;
+	f2 const j0 = raw_fma(iy, splat(__uint_as_float(PITCH)), splat(hb));   // address of entry iy of the hash table, less H (exact, as lut_offsets)
+	f2 const j1 = raw_fma(i1y, splat(__uint_as_float(PITCH - 4)), j0);     // + pitch - 4 bytes when i1.y = 1 (see simplex_hash_entry)
 	unsigned const ja = __float_as_uint(j0.x), jb = __float_as_uint(j0.y), j1a = __float_as_uint(j1.x), j1b = __float_as_uint(j1.y);
-	f2 const bx = lut_offsets(ix, Lb);
+	f2 const bx = raw_fma(ix, splat(__uint_as_float(LUT_ENTRY_BYTES)), splat(gb));
 	k0 = add2(make_float2(lut_load_f32<H>(ja), lut_load_f32<H>(jb)), bx);
 	k1 = add2(make_float2(lut_load_f32<H + 4>(j1a), lut_load_f32<H + 4>(j1b)), bx);
 	k2 = add2(make_float2(lut_load_f32<H + 8>(ja), lut_load_f32<H + 8>(jb)), bx);
 }
 
-// glm::simplex(vec2) for two positions with the table; Lb = simplex_lut_base(); HASH: the block staged the simplex hash table too
-template<bool HASH>
-__device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
+// glm::simplex(vec2) for two positions with the table; Lb = simplex_lut_base(); HASH: the block staged the simplex hash table too, H bytes behind
+// the gradient table; WIN: ix, iy stay unreduced and wb = {gb, hb} of simplex_hash_offsets with the octave's window shift folded in
+template<bool HASH, unsigned H = SIMPLEX_HASH_OFFSET, bool WIN = false>
+__device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb, f2 wb = f2()) {
 	static_assert(!HASH || TW_SIMPLEX_HASH_TABLE, "the hash table exists at level 3 with the denormal addressing only");
+	static_assert(!WIN || HASH, "the windowed form addresses through the hash table");
 	float const Cx = 0.211324865405187f, Cy = 0.366025403784439f, Cz = -0.577350269189626f;
 	f2 const s = sumprod2(vx, Cy, vy, Cy);
 	f2 ix = floor2(add2(vx, s)), iy = floor2(add2(vy, s));
@@ -217,7 +240,11 @@ __device__ __forceinline__ f2 simplex2_lut(f2 vx, f2 vy, unsigned Lb) {
 	f2 const i1y = rsub2(1.0f, i1x); // (1,0) or (0,1)
 	f2 const x12x = sub2(add2(x0x, Cx), i1x), x12y = sub2(add2(x0y, Cx), i1y), x12z = add2(x0x, Cz), x12w = add2(x0y, Cz);
 	f2 k0, k1, k2;
-	if constexpr (HASH) {simplex_hash_offsets(mod_int289_lazy(ix), mod_int289_lazy(iy), i1y, Lb, k0, k1, k2);}
+	if constexpr (WIN) {simplex_hash_offsets<H>(ix, iy, i1y, wb.x, wb.y, k0, k1, k2);}
+	else if constexpr (HASH) { // the hash table's one copy starts at Lb without the lane's copy offset
+		unsigned const base = Lb - (threadIdx.x & (SIMPLEX_LUT_COPIES - 1))*16u;
+		simplex_hash_offsets<H>(mod_int289_lazy(ix), mod_int289_lazy(iy), i1y, __uint_as_float(Lb), __uint_as_float(base), k0, k1, k2);
+	}
 	else {
 	f2 p0, p1, p2;
 #if TW_SIMPLEX_LUT >= 2

@@ -3,7 +3,7 @@
 # then prints the command that runs the parity tests once and the kernel-only bench for every variant, to be run on the GPU machine.
 #   tools/ab_variants.sh base "" t256 "-DTW_NOISE2_THREADS=256 -DTW_NOISE2_MIN_BLOCKS=3" lut2 "-DTW_SIMPLEX_LUT=2 -DTW_NOISE2_THREADS=256 -DTW_NOISE2_MIN_BLOCKS=5"
 # Knobs that exist today: TW_SIMPLEX_LUT (0 no table, 1 gradient, 2 + first hash, 3 + second hash folded = shipped), TW_NOISE2_MIN_BLOCKS,
-# TW_NOISE2_THREADS, TW_NOISE2_BLOCK_CELLS, TW_NOISE2_PERSISTENT (tw_heightgen.cu); run-time: TW_NOISE_SCALAR=1 (scalar kernel), TW_EROSION_LANES, TW_PIPE_CHUNKS.
+# TW_NOISE2_THREADS, TW_NOISE2_BLOCK_CELLS, TW_NOISE2_PERSISTENT, TW_DWARP_WIN_OCTAVES, TW_DWARP_WIN_THREADS, TW_DWARP_WARP_MARGIN (tw_heightgen.cu); run-time: TW_NOISE_SCALAR=1 (scalar kernel), TW_EROSION_LANES, TW_PIPE_CHUNKS.
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p tools/ab

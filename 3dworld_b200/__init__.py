@@ -187,6 +187,19 @@ class ErosionJobArgs(C.Structure):
                 ("num_iters", C.c_uint32), ("ep", C.c_void_p), ("mode", C.c_int), ("num_threads", C.c_uint32), ("vals", C.c_void_p)]
 
 
+class GenMeshInfo(C.Structure):
+    """tw_gen_mesh_info (include/tw3d.h): the z globals gen_mesh leaves and the erosion's droplet moves, filled by the poll that completes the job."""
+    _fields_ = [(n, C.c_float) for n in ("zmin", "zmax", "zmax_est", "zbottom", "ztop", "water_plane_z")] + [("erosion_moves", C.c_uint64)]
+
+
+class GenMeshJobArgs(C.Structure):
+    """tw_gen_mesh_job (include/tw3d.h): the arguments of one tw_gen_mesh_launch."""
+    _fields_ = [("mesh_x_size", C.c_int), ("mesh_y_size", C.c_int), ("xoff2", C.c_int), ("yoff2", C.c_int), ("dx_val", C.c_float), ("dy_val", C.c_float),
+                ("x_scene_size", C.c_float), ("y_scene_size", C.c_float), ("p", C.c_void_p), ("erosion_iters", C.c_uint32), ("ep", C.c_void_p),
+                ("water_h_off", C.c_float), ("water_h_off_rel", C.c_float), ("prev_zbottom", C.c_float), ("prev_ztop", C.c_float),
+                ("prev_water_plane_z", C.c_float), ("mesh", C.c_void_p), ("info", C.c_void_p)]
+
+
 class SweepParams(C.Structure):
     """tw_sweep_params (include/tw3d.h): tw_erode_sweeps' sweep and halo for tw_erode_launch_ex's TW_EROSION_SWEEPS mode."""
     _fields_ = [("sweep", C.c_uint32), ("halo", C.c_int)]
@@ -218,7 +231,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
                "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
-               "tw_points_launch"]
+               "tw_points_launch", "tw_gen_mesh_launch"]
 
 
 def _load():
@@ -279,6 +292,7 @@ def _load():
     L.tw_hmap_tiles_touched.argtypes = [C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_points_launch.argtypes = [vp, C.POINTER(PointsJobArgs)]
+    L.tw_gen_mesh_launch.argtypes = [vp, C.POINTER(GenMeshJobArgs)]
     L.tw_erode_parallel.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_uint32, C.POINTER(ErosionParams), C.c_uint32]
     L.tw_erode_launch.argtypes = [vp, C.POINTER(ErosionJobArgs)]
     L.tw_erode_launch_ex.argtypes = [vp, C.POINTER(ErosionJobArgs), C.POINTER(SweepParams)]
@@ -604,6 +618,19 @@ class PointsJob:
         return self.out if self._ctx.create_tiles_poll(wait) else None
 
 
+class GenMeshJob:
+    """What Context.gen_mesh_launch returns: poll(wait) completes the job (the context's pending job) and returns (mesh, info dict with the keys of
+    scene.gen_mesh's plus erosion_moves), or None while it runs (wait=False)."""
+
+    def __init__(self, ctx, mesh):
+        self._ctx, self.mesh, self.info = ctx, mesh, GenMeshInfo()
+
+    def poll(self, wait=False):
+        if not self._ctx.create_tiles_poll(wait):
+            return None
+        return self.mesh, {n: (int if n == "erosion_moves" else float)(getattr(self.info, n)) for n, _ in GenMeshInfo._fields_}
+
+
 class Context:
     """One tw_ctx (device + stream + uploaded tables). All compute goes through the C ABI."""
 
@@ -890,6 +917,26 @@ class Context:
         self._check(lib.tw_points_launch(self._h, C.byref(a)))
         job = PointsJob(self, out)
         self._tiles_job = (xy, out, hp, pq, hs, job)
+        return job
+
+    def gen_mesh_launch(self, mesh_size, hp, ep, erosion_iters=0, xoff2=0, yoff2=0, dx_val=None, dy_val=None, scene_size=(4.0, 4.0), water_h_off=0.0,
+                        water_h_off_rel=0.0, prev=(0.0, 0.0, 0.0), mesh=None):
+        """tw_gen_mesh_launch: gen_mesh in ground mode after its sine table (set_sine_params first) as this context's asynchronous job. mesh_size =
+        (MESH_X_SIZE, MESH_Y_SIZE); hp (its zmax_est is ignored) and ep (erode_amount, half_dxy, relh_adj_tex, clip_hd1 are read) are copied during the
+        launch; dx_val / dy_val default to 1/hp.dx_val_inv, 1/hp.dy_val_inv; scene_size = (X_SCENE_SIZE, Y_SCENE_SIZE); prev = (zbottom, ztop, water_plane_z)
+        before the call, which a flat mesh keeps. mesh = [MY, MX] floats (numpy array or torch tensor, host or CUDA; default a new numpy array).
+        Returns a GenMeshJob."""
+        MX, MY = int(mesh_size[0]), int(mesh_size[1])
+        if mesh is None:
+            mesh = np.empty((MY, MX), np.float32)
+        dx = float(np.float32(1.0) / np.float32(hp.dx_val_inv)) if dx_val is None else dx_val
+        dy = float(np.float32(1.0) / np.float32(hp.dy_val_inv)) if dy_val is None else dy_val
+        job = GenMeshJob(self, mesh)
+        a = GenMeshJobArgs(MX, MY, xoff2, yoff2, dx, dy, scene_size[0], scene_size[1], C.cast(C.pointer(hp), C.c_void_p), erosion_iters,
+                           C.cast(C.pointer(ep), C.c_void_p), water_h_off, water_h_off_rel, prev[0], prev[1], prev[2], _ptr(mesh),
+                           C.cast(C.pointer(job.info), C.c_void_p))
+        self._check(lib.tw_gen_mesh_launch(self._h, C.byref(a)))
+        self._tiles_job = (mesh, job)
         return job
 
     def erode(self, h, min_zval, num_iters, ep):

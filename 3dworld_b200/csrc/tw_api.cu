@@ -1467,6 +1467,70 @@ int tw_proc_gen_heightmap(tw_ctx *ctx, uint32_t width, uint32_t height, float dx
 	return poll_job(ctx, 1);
 }
 
+// gen_mesh in ground mode as the context's asynchronous job: the mesh and the probe are generated, then one-thread kernels turn the data's min/max and the
+// probe's max |z| into the record's z values (twi_gen_mesh_zvals), glaciation reads zmax_est from the record and writes zbottom / ztop back, and the erosion
+// builds its parameters from the record (twi_erode_dev_enqueue); the record comes back through the pinned staging, which the completing poll unpacks.
+// Scratch slot 0: [mesh (unless on the device) | probe]; slot 1: the sine tables, then the erosion's scratch; slot 2: [fixed words | record];
+// pinned staging: [record | mesh (pageable mesh)].
+int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!job || !job->p || !job->ep || !job->mesh) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+	int const MX = job->mesh_x_size, MY = job->mesh_y_size;
+	if (MX <= 0 || MY <= 0 || MY > 65535) return tw_set_error(ctx, TW_ERR_ARG, "mesh size %d x %d", MX, MY);
+	tw_height_params const p = *job->p;
+	tw_erosion_params const ep = *job->ep;
+	tw_grid2d const grid = {(float)(job->xoff2 - MX/2), (float)(job->yoff2 - MY/2), job->dx_val, job->dy_val, (uint32_t)MX, (uint32_t)MY}; // gen_mesh_sine_table, src/mesh_gen.cpp:201-210
+	float const xy_scene_size(0.5f*(job->x_scene_size + job->y_scene_size));
+	float const rm_scale(1000.0*xy_scene_size/p.mesh_scale);
+	tw_grid2d const probe = {0.0f, 0.0f, rm_scale, rm_scale, 128, 128}; // estimate_zminmax's EST_RAND_PARAM grid, src/mesh_gen.cpp:468-472
+	rc = validate_gen(ctx, &grid, &p); if (rc) return rc;
+	if (p.gen_mode == TW_MGEN_SINE && !ctx->have_sine_params) return tw_set_error(ctx, TW_ERR_STATE, "tw_set_sine_params() has not been called");
+	size_t const n = (size_t)MX*MY, nprobe = (size_t)probe.nx*probe.ny;
+	uint32_t const iters = job->erosion_iters;
+	bool const erode = (iters > 0 && ep.erode_amount > 0.0); // apply_erosion, src/erosion.cpp:16
+	bool const dev = tw_is_device_ptr(job->mesh), locked = !dev && twi_is_page_locked(job->mesh);
+	float *d_mesh = job->mesh, *d_probe;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {d_mesh = c.take<float>(n);} d_probe = c.take<float>(nprobe);}); if (rc) return rc;
+	size_t const s1 = std::max(erode ? twi_erode_dev_scratch_bytes(ctx, MX, MY, iters) : 0, std::max(twi_heightgen_slot1_bytes(&grid, &p), twi_heightgen_slot1_bytes(&probe, &p)));
+	if (s1) {rc = tw_reserve(ctx, 1, s1); if (rc) return rc;}
+	twi_gen_mesh_rec *d_rec;
+	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {c.take<twi_slot2_words>(1); d_rec = c.take<twi_gen_mesh_rec>(1);}); if (rc) return rc;
+	twi_gen_mesh_rec *h_rec; float *h_mesh = nullptr;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {h_rec = c.take<twi_gen_mesh_rec>(1); if (!dev && !locked) {h_mesh = c.take<float>(n);}}); if (rc) return rc;
+	float const wpz = twi_water_rel(p.glaciate, p.custom_glaciate_exp, job->water_h_off_rel);
+	float *const mesh = job->mesh;
+	tw_gen_mesh_info *const info = job->info;
+	twi_job pending;
+	pending.cancellable = true;
+	pending.complete = [h_rec, h_mesh, mesh, n, info](tw_ctx *c) -> int {
+		twi_gen_mesh_rec const r = *h_rec;
+		if (r.fail) {c->last_erosion_steps = 0; return tw_set_error(c, TW_ERR_STATE, "speculative erosion made no progress (%u rounds)", r.fail);}
+		c->last_erosion_steps = r.steps;
+		if (info) {
+			info->zmin = r.zmin; info->zmax = r.zmax; info->zmax_est = r.zmax_est; info->zbottom = r.zbottom; info->ztop = r.ztop;
+			info->water_plane_z = r.water_plane_z; info->erosion_moves = r.steps;
+		}
+		if (h_mesh) {memcpy(mesh, h_mesh, n*sizeof(float));}
+		return TW_OK;
+	};
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
+		TW_CUDA(ctx, cudaMemsetAsync(d_rec, 0, sizeof(twi_gen_mesh_rec), ctx->stream));
+		int r = twi_init_minmax(ctx, d_rec->mm, 1); if (r) return r;
+		r = twi_heightgen(ctx, &grid, &p, 0, 0, nullptr, 1, d_mesh, d_rec->mm); if (r) return r;     // the mesh and calc_zminmax
+		r = twi_heightgen(ctx, &probe, &p, 0, 0, nullptr, 1, d_probe, nullptr); if (r) return r;
+		r = twi_gen_mesh_zvals(ctx, d_rec, d_probe, nprobe, p.gen_mode == TW_MGEN_SINE, wpz, job->water_h_off, job->prev_zbottom, job->prev_ztop,
+		                       job->prev_water_plane_z); if (r) return r;
+		if (p.glaciate) { // gen_terrain_map -> glaciate(): zbottom / ztop of the glaciated mesh
+			r = twi_glaciate_mesh_rec(ctx, d_mesh, MX, MY, job->xoff2, job->yoff2, MX, MY, &p, d_rec); if (r) return r;
+			r = twi_gen_mesh_zbottom(ctx, d_rec); if (r) return r;
+		}
+		if (erode) {r = twi_erode_dev_enqueue(ctx, ctx->d_scratch[1], d_mesh, MX, MY, iters, &ep, d_rec); if (r) return r;}
+		if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(locked ? mesh : h_mesh, d_mesh, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
+		TW_CUDA(ctx, cudaMemcpyAsync(h_rec, d_rec, sizeof(twi_gen_mesh_rec), cudaMemcpyDeviceToHost, ctx->stream));
+		return TW_OK;
+	});
+}
+
 int tw_minmax_f32(tw_ctx *ctx, const float *vals, size_t n, tw_minmax *mm) {
 	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!vals || !mm || n == 0) return tw_set_error(ctx, TW_ERR_ARG, "null/empty argument");

@@ -26,11 +26,8 @@ __device__ __forceinline__ float smin(float a, float b) {return (b < a) ? b : a;
 __device__ __forceinline__ float smax(float a, float b) {return (a < b) ? b : a;} // std::max
 __device__ __forceinline__ int clampi(int v, int hi) {return max(min(v, hi), 0);}
 
-struct EParams {
-	float erode_amount, wpz_minus_half_dxy, zmin, zrange, relh_adj_tex, clip_hd1;
-	float rock_min;   // get_bare_ls_tid(nh) == ROCK_TEX  <=>  nh >= rock_min (see make_eparams); rock_exact == 0: evaluate the reference expression per move
-	int   rock_exact;
-};
+// rock_min: get_bare_ls_tid(nh) == ROCK_TEX  <=>  nh >= rock_min (see make_eparams); rock_exact == 0: evaluate the reference expression per move
+using EParams = twi_eparams;
 
 // Also counts, per heightmap, the cells above the ocean-stop level (src/erosion.cpp:98): droplets that start below it die in one move, the
 // others walk downhill, so this count predicts the heightmap's total droplet work (correlation 0.95 on the BASELINE terrain) and is used to
@@ -195,6 +192,7 @@ struct DArgs {
 	twi_job_words *jw;          // in a job: the context's job words (tw_cancel), M_GLOBAL / M_ATOMIC / M_WINDOW / M_WHOLE start no droplet once it is cancelled; nullptr otherwise
 	const unsigned *sweep_it0;  // M_FROZEN in a job (twi_erode_sweeps_enqueue): the device word holding it0; the sweep is [it0, fz_end(it0, sweep, num_iters))
 	unsigned sweep;
+	const EParams *dE;          // DEV_E (the ground-mode mesh job): the parameters in device memory, read at the kernel's entry (A.E then holds erode_amount only)
 };
 
 // CANCEL: the variant with the cancellation point, for jobs (see launch_droplets); synchronous calls and short latency-mode walks run the one without it, whose
@@ -202,7 +200,7 @@ struct DArgs {
 // M_FROZEN's job variant (CANCEL = true) has no check in the walk: it reads its sweep's bounds from A.sweep_it0, so one graph body serves every sweep, and
 // the loop's cancellation point is sweep_advance_kernel. The flags are spelled out in the expressions below rather than named: even an unused constexpr local
 // changes how the front end orders the code, and the SASS of the other instantiations is meant to stay as it was.
-template<int G, int MODE, bool CANCEL>
+template<int G, int MODE, bool CANCEL, bool DEV_E = false>
 __global__ void __launch_bounds__(128)
 droplet_kernel(DArgs const A)
 {
@@ -230,7 +228,7 @@ droplet_kernel(DArgs const A)
 	float const Kq=10, Kw=0.001f, Kr=0.9f, Kd=0.02f, Ki=0.1f, minSlope=0.05f, g=20, Kg=g*2;
 	unsigned const MAX_PATH_LEN = 4u*(unsigned)NX*(unsigned)NY;
 	float const erode_amount = A.E.erode_amount;
-	EParams const E = A.E;
+	EParams const E = DEV_E ? *A.dE : A.E;
 	unsigned num_iters = A.num_iters;
 	unsigned long long steps = 0;
 	bool const have_tile = active;
@@ -646,12 +644,12 @@ droplet_kernel(DArgs const A)
 
 constexpr size_t SMEM_MAX_BLOCK = 227u*1024u; // sm_90: 227 KB of dynamic shared memory per block
 
-template<int G, int MODE, bool CANCEL>
+template<int G, int MODE, bool CANCEL, bool DEV_E = false>
 void launch_droplets_c(cudaStream_t st, DArgs const &A, unsigned warps_per_block, size_t smem_per_group) {
 	unsigned const groups_per_block = warps_per_block*(32/G);
 	size_t const smem = smem_per_group*groups_per_block;
-	if (smem > 48*1024) {cudaFuncSetAttribute(droplet_kernel<G, MODE, CANCEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);}
-	droplet_kernel<G, MODE, CANCEL><<<(A.nslots + groups_per_block - 1)/groups_per_block, 32*warps_per_block, smem, st>>>(A);
+	if (smem > 48*1024) {cudaFuncSetAttribute(droplet_kernel<G, MODE, CANCEL, DEV_E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);}
+	droplet_kernel<G, MODE, CANCEL, DEV_E><<<(A.nslots + groups_per_block - 1)/groups_per_block, 32*warps_per_block, smem, st>>>(A);
 }
 
 // The variant with the cancellation point runs for a job's erosion (A.jw set: twi_erode_enqueue / twi_erode_parallel_enqueue inside twi_launch_job) in the
@@ -1080,7 +1078,8 @@ static int spec_loop_graph(tw_ctx *ctx, cudaStream_t st, DArgs const &W, unsigne
 	}
 	if (e == cudaSuccess) {e = cudaStreamBeginCaptureToGraph(st, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed);}
 	if (e == cudaSuccess) {
-		launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));
+		if (W.dE) {launch_droplets_c<32, M_SPEC, false, true>(st, W, 4, (size_t)W.win_elems*sizeof(float));}
+		else {launch_droplets<32, M_SPEC>(st, W, 4, (size_t)W.win_elems*sizeof(float));}
 		spec_round_kernel<<<SPEC_CLUSTER, 1024, 0, st>>>(W.S, num_iters, d_pad, NX, d_steps, max_rounds, d_fail, h, true, W.jw);
 		cudaError_t const le = cudaGetLastError();
 		cudaGraph_t body = nullptr;
@@ -1107,8 +1106,9 @@ size_t twi_erode_spec_scratch_bytes(int xsize, int ysize) {
 // host_rounds = false: the rounds are one graph launch that ends on the device and nothing waits; *d_fail becomes the number of rounds run if the window stopped
 // making progress (0 otherwise). host_rounds = true (tw_erode): the rounds are queued from the host, which reads the "done" flag every 8 rounds and returns the
 // no-progress error itself; on the BASELINE 8192^2 map this was 1-2 % faster than the graph with 1000 droplets and equal with 1e5 (DESIGN.md section 4e).
+// d_E (graph rounds only): the walkers read their parameters from it on the device, and only p->erode_amount is read here.
 int twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zvals, float min_zval, uint32_t num_iters,
-                           const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds) {
+                           const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds, const twi_eparams *d_E) {
 	volatile unsigned *h_done = nullptr;
 	if (host_rounds) {int const rc = tw_reserve_pinned(ctx, 64); if (rc) return rc; h_done = (volatile unsigned *)ctx->h_pinned;}
 	cudaStream_t const st = ctx->stream;
@@ -1119,7 +1119,8 @@ int twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, 
 	twi_carve c{(char *)scratch}; spec_layout(c, xsize, ysize, S, d_pad, ntile);
 	DArgs A;
 	memset(&A, 0, sizeof(A));
-	A.E = make_eparams(p);
+	if (d_E) {A.E.erode_amount = p->erode_amount; A.dE = d_E;}
+	else {A.E = make_eparams(p);}
 	A.xsize = xsize; A.ysize = ysize; A.num_iters = num_iters; A.dir_table = ctx->d_dir_table;
 	A.padded = d_pad; A.slot0 = 0; A.jw = ctx->in_job ? ctx->d_job_words : nullptr; // the graph's round kernel reads them (tw_erode's host rounds never do)
 	pad_kernel<<<dim3((NX + 255)/256, NY, 1), 256, 0, st>>>(d_map, d_pad, xsize, ysize, NX, NY, A.E.wpz_minus_half_dxy, nullptr, nullptr);
@@ -1207,6 +1208,58 @@ int twi_erode(tw_ctx *ctx, float *d_maps, uint32_t ntiles, int xsize, int ysize,
 	TW_CUDA(ctx, cudaMemcpyAsync(&h_steps, d_steps, sizeof(h_steps), cudaMemcpyDeviceToHost, ctx->stream));
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	ctx->last_erosion_steps = h_steps;
+	return TW_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the ground-mode mesh job's erosion (tw_gen_mesh_launch)
+namespace {
+// make_eparams with the water level and z range the job derived on the device; rock_exact = 0 keeps the reference expression per move, which the host's
+// threshold equals by construction
+__global__ void gen_mesh_eparams_kernel(twi_gen_mesh_rec *rec, float erode_amount, float half_dxy, float relh_adj_tex, float clip_hd1) {
+	EParams E;
+	E.erode_amount = erode_amount;
+	E.wpz_minus_half_dxy = rec->water_plane_z - half_dxy;
+	E.zmin = rec->zmin; E.zrange = rec->zmax - rec->zmin;
+	E.relh_adj_tex = relh_adj_tex; E.clip_hd1 = clip_hd1;
+	E.rock_min = 0.0f; E.rock_exact = 0;
+	rec->E = E;
+}
+} // namespace
+
+size_t twi_erode_dev_scratch_bytes(const tw_ctx *ctx, int xsize, int ysize, uint32_t num_iters) {
+	return spec_eligible(1, xsize, ysize, num_iters) ? twi_erode_spec_scratch_bytes(xsize, ysize) : twi_erode_scratch_bytes(ctx, 1, xsize, ysize);
+}
+
+// twi_erode's single-map paths with DEV_E walkers: M_SPEC as the asynchronous jobs run it, else M_WHOLE, else M_GLOBAL (one map: no schedule, no window)
+int twi_erode_dev_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, uint32_t num_iters, const tw_erosion_params *ep, twi_gen_mesh_rec *d_rec) {
+	cudaStream_t const st = ctx->stream;
+	gen_mesh_eparams_kernel<<<1, 1, 0, st>>>(d_rec, ep->erode_amount, ep->half_dxy, ep->relh_adj_tex, ep->clip_hd1);
+	TW_LAUNCH_CHECK(ctx);
+	if (spec_eligible(1, xsize, ysize, num_iters)) {
+		return twi_erode_spec_enqueue(ctx, scratch, d_map, xsize, ysize, &d_rec->zbottom, 0.0f, num_iters, ep, &d_rec->steps, &d_rec->fail, false, &d_rec->E);
+	}
+	int const NX = xsize + 2*PAD, NY = ysize + 2*PAD;
+	DArgs A;
+	memset(&A, 0, sizeof(A));
+	A.E.erode_amount = ep->erode_amount; A.dE = &d_rec->E;
+	A.xsize = xsize; A.ysize = ysize; A.num_iters = num_iters; A.dir_table = ctx->d_dir_table; A.steps_out = &d_rec->steps;
+	A.min_zvals = &d_rec->zbottom; A.jw = ctx->in_job ? ctx->d_job_words : nullptr; A.slot0 = 0; A.nslots = 1;
+	if (plan_whole(ctx->num_sms, 1, xsize, ysize)) {
+		A.maps = d_map; A.WX = NX; A.WY = NY; A.P = whole_pitch(NX, NY); A.win_elems = (unsigned)A.P*NY;
+		size_t const smem = (size_t)A.win_elems*sizeof(float);
+		if (A.jw && num_iters >= CANCEL_MIN_DROPLETS) {launch_droplets_c<32, M_WHOLE, true, true>(st, A, 1, smem);}
+		else {launch_droplets_c<32, M_WHOLE, false, true>(st, A, 1, smem);}
+		TW_LAUNCH_CHECK(ctx);
+		return TW_OK;
+	}
+	twi_carve c{(char *)scratch}; float *d_pad; unsigned *d_work; erode_layout(c, 1, xsize, ysize, d_pad, d_work);
+	pad_kernel<<<dim3((NX + 255)/256, NY, 1), 256, 0, st>>>(d_map, d_pad, xsize, ysize, NX, NY, 0.0f, nullptr, nullptr);
+	TW_LAUNCH_CHECK(ctx);
+	A.padded = d_pad;
+	launch_droplets_c<32, M_GLOBAL, true, true>(st, A, 2, 0);
+	TW_LAUNCH_CHECK(ctx);
+	unpad_kernel<<<dim3((xsize + 255)/256, ysize, 1), 256, 0, st>>>(d_pad, d_map, xsize, ysize, NX, NY, &d_rec->zbottom, 0.0f, nullptr);
+	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }
 

@@ -40,6 +40,15 @@ void apply_mesh_rand_seed(rand_gen &rgen, int mesh_seed, int mesh_rgen_index, in
 
 } // namespace
 
+// the part of get_water_z_height that does not depend on zmax_est (tw_internal.h)
+float twi_water_rel(int glaciate, float custom_glaciate_exp, float water_h_off_rel) {
+	float const t(0.42f + water_h_off_rel); // W_PLANE_Z
+	float const lo((t < 1.0f) ? t : 1.0f);
+	float wpz((0.0f < lo) ? lo : 0.0f);       // CLIP_TO_01
+	if (glaciate) {wpz = ((custom_glaciate_exp == 0.0f) ? wpz*wpz*wpz : std::pow(wpz, custom_glaciate_exp));}
+	return wpz;
+}
+
 extern "C" {
 
 void tw_build_sin_table(float *tab) {
@@ -110,10 +119,7 @@ void tw_noise3d_gen_sines(int rs1, int rs2, float mag, float freq, float *rdata)
 }
 
 float tw_water_z_height(float zmax_est, int glaciate, float custom_glaciate_exp, float water_h_off, float water_h_off_rel) {
-	float const t(0.42f + water_h_off_rel); // W_PLANE_Z
-	float const lo((t < 1.0f) ? t : 1.0f);
-	float wpz((0.0f < lo) ? lo : 0.0f);       // CLIP_TO_01
-	if (glaciate) {wpz = ((custom_glaciate_exp == 0.0f) ? wpz*wpz*wpz : std::pow(wpz, custom_glaciate_exp));}
+	float const wpz = twi_water_rel(glaciate, custom_glaciate_exp, water_h_off_rel);
 	float const zmax_est2(2.0*zmax_est);
 	return wpz*zmax_est2 - zmax_est + water_h_off;
 }

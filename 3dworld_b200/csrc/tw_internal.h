@@ -322,8 +322,11 @@ int twi_hmap_points(tw_ctx *ctx, const uint8_t *d_data16, const tw_hmap_sampler 
 // one that ends on the device (*d_fail = the rounds run when the window stopped making progress, else 0), with true tw_erode's host-driven rounds
 bool   twi_erode_spec_eligible(uint32_t nt, int xsize, int ysize, uint32_t num_iters);
 size_t twi_erode_spec_scratch_bytes(int xsize, int ysize);
+// The droplet erosion's parameters as its kernels read them (make_eparams, tw_erosion.cu): rock_exact == 0 evaluates the reference's rock expression per move; d_E (graph rounds
+// only): the walkers read them on the device, and only p->erode_amount is read on the host
+struct twi_eparams {float erode_amount, wpz_minus_half_dxy, zmin, zrange, relh_adj_tex, clip_hd1, rock_min; int rock_exact;};
 int    twi_erode_spec_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, const float *d_min_zvals, float min_zval, uint32_t num_iters,
-                              const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds);
+                              const tw_erosion_params *p, unsigned long long *d_steps, unsigned *d_fail, bool host_rounds, const twi_eparams *d_E = nullptr);
 int twi_erode_parallel(tw_ctx *ctx, float *d_map, int xsize, int ysize, float min_zval, uint32_t num_iters, const tw_erosion_params *p, uint32_t num_threads);
 // tw_erode_parallel in parts: its padded scratch, and the enqueue (lower clamp *d_min_zval, or min_zval when it is nullptr; moves added to *d_steps)
 size_t twi_erode_parallel_scratch_bytes(int xsize, int ysize);
@@ -363,6 +366,32 @@ int twi_hmap_scales(tw_ctx *ctx, const unsigned *d_mm, float mesh_height_scale, 
 int twi_from_floats_u16_dev(tw_ctx *ctx, const float *d_vals, size_t n, const twi_hmap_stage *d_stage, uint8_t *d_out);
 // *d_min = the minimum of the ordered min/max d_mm as a float (tw_erode_launch's lower clamp of the image, left on the device)
 int twi_ord_min(tw_ctx *ctx, const unsigned *d_mm, float *d_min);
+// tw_gen_mesh_launch's record in device memory: every scalar the ground-mode chain derives from the data, written by one-thread kernels and read by the steps
+// after them, then copied whole into the pinned staging for the completing poll. The first six fields are tw_gen_mesh_info's.
+struct twi_gen_mesh_rec {
+	float zmin, zmax, zmax_est, zbottom, ztop, water_plane_z;
+	float zmax_est2, zmax_est2_inv;  // glaciation's, derived from zmax_est as twi_glaciate_mesh derives them
+	unsigned mm[2];                  // ordered min/max of the generated mesh, then of the glaciated mesh
+	unsigned absmax;                 // the probe's largest |z| (float bits; NaN skipped), 0 before the reduction
+	unsigned fail;                   // the speculative erosion's no-progress round count (0: none)
+	unsigned long long steps;        // droplet moves
+	twi_eparams E;                   // the erosion's parameters
+};
+// The ground-mode mesh's host-known part of get_water_z_height (tw_host.cpp): the relative water level wpz, glaciated, before it is scaled by zmax_est
+float twi_water_rel(int glaciate, float custom_glaciate_exp, float water_h_off_rel);
+// estimate_zminmax + set_zvals (tw_tiles.cu): max |z| of the n probe heights d_probe, then one thread derives zmax_est, zmin / zmax, zbottom / ztop and
+// water_plane_z from rec->mm and that maximum into *rec, as the host chain does (the flat mesh keeps the prev_* values)
+int twi_gen_mesh_zvals(tw_ctx *ctx, twi_gen_mesh_rec *d_rec, const float *d_probe, size_t n, bool sine_mode, float wpz, float water_h_off,
+                       float prev_zbottom, float prev_ztop, float prev_water_plane_z);
+// glaciate() with zmax_est / zmax_est2 / zmax_est2_inv read from *d_rec; min/max of the result into d_rec->mm (ordered, initialised by the caller)
+int twi_glaciate_mesh_rec(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, twi_gen_mesh_rec *d_rec);
+// d_rec->zbottom / ztop = the ordered min/max d_rec->mm (glaciate()'s calc_zminmax)
+int twi_gen_mesh_zbottom(tw_ctx *ctx, twi_gen_mesh_rec *d_rec);
+// The erosion of the ground-mode mesh job (tw_erode's serial order, the mode tw_erode picks for one map of this size, M_SPEC's rounds ending on the device) with
+// its parameters read on the device: one thread first builds d_rec->E as make_eparams does from d_rec's zmin / zmax / water_plane_z and ep's erode_amount,
+// half_dxy, relh_adj_tex and clip_hd1 (rock_exact = 0); the lower clamp is d_rec->zbottom; moves into d_rec->steps, no progress into d_rec->fail.
+size_t twi_erode_dev_scratch_bytes(const tw_ctx *ctx, int xsize, int ysize, uint32_t num_iters);
+int    twi_erode_dev_enqueue(tw_ctx *ctx, void *scratch, float *d_map, int xsize, int ysize, uint32_t num_iters, const tw_erosion_params *ep, twi_gen_mesh_rec *d_rec);
 // scratch slot 1 bytes twi_heightgen uses for this grid (the sine mode's tables; 0 otherwise)
 size_t twi_heightgen_slot1_bytes(const tw_grid2d *g, const tw_height_params *p);
 int twi_to_floats_u16(tw_ctx *ctx, const uint8_t *d_data, size_t n, float val_mult, float val_add, float *d_vals);

@@ -1,11 +1,14 @@
 // tw_tiles.cu - the pieces of the reference's callers that sit right next to the generators (sm_90a):
 //   tile_bounds_kernel     tail of tile_t::create_zvals (src/tiled_mesh.cpp:517-540): 4x4 sub-block min/max (inclusive ends), water bbox
 //   glaciate_mesh_kernel   glaciate() of the ground-mode mesh (src/mesh_gen.cpp:388-404): apply_glaciate + apply_mesh_sine per cell + zbottom/ztop
+//   probe_absmax_kernel,   the z estimate of gen_mesh (estimate_zminmax + set_zvals, src/mesh_gen.cpp:447-504) for tw_gen_mesh_launch, into its device record
+//   gen_mesh_zvals_kernel
 //   tile_normals_kernel    tile_t::upload_normal_texture (src/tiled_mesh.cpp:865-880, get_norm src/tiled_mesh.h:281-284): RGBA8 normal map + min_normal_z
 //   tile_ao_kernel         tile_t::calc_mesh_ao_lighting (src/tiled_mesh.cpp:586-662): 8 directions x 8 steps of growing stride over the
 //                          tile's zvals and the (stride+72)^2 context generated around it
 // All are single streaming passes over data that is already resident (4 B/cell read, glaciate also 4 B/cell written): HBM/L2-bound.
 #include "tw_internal.h"
+#include <algorithm>
 
 namespace {
 
@@ -67,8 +70,11 @@ __device__ __forceinline__ float volcano_height(float xi, float yi, const GlacPa
 	return P.volcano_height*smax(0.0f, (peak - hole))*P.mszi;
 }
 
+// REC (tw_gen_mesh_launch): zmax_est, zmax_est2 and zmax_est2_inv come from the job's device record instead of P
+template<bool REC>
 __global__ void __launch_bounds__(256)
-glaciate_mesh_kernel(float *__restrict__ mesh, GlacParams P, const float *__restrict__ tab, unsigned *__restrict__ mm) {
+glaciate_mesh_kernel(float *__restrict__ mesh, GlacParams P, const float *__restrict__ tab, unsigned *__restrict__ mm, const twi_gen_mesh_rec *__restrict__ rec) {
+	if (REC) {P.zmax_est = rec->zmax_est; P.zmax_est2 = rec->zmax_est2; P.zmax_est2_inv = rec->zmax_est2_inv;}
 	int const j = blockIdx.x*blockDim.x + threadIdx.x, i = blockIdx.y;
 	float vmin = INFINITY, vmax = -INFINITY;
 	if (j < P.nx) {
@@ -91,6 +97,42 @@ glaciate_mesh_kernel(float *__restrict__ mesh, GlacParams P, const float *__rest
 	}
 	if (mm && (threadIdx.x & 31) == 0 && vmin <= vmax) {atomicMin(mm, tw_f2ord(vmin)); atomicMax(mm + 1, tw_f2ord(vmax));}
 }
+
+// estimate_zminmax's loop over the probe (src/mesh_gen.cpp:474-478): zmax_est = (zmax_est < |z|) ? |z| : zmax_est, so a NaN never wins. |z| is never negative, so
+// its float bits order as integers and the largest non-NaN |z| is one atomicMax; folding that into zmax_est (> 0, or NaN) gives the loop's result.
+__global__ void __launch_bounds__(256)
+probe_absmax_kernel(const float *__restrict__ v, size_t n, unsigned *__restrict__ absmax) {
+	unsigned m = 0u;
+	size_t const stride = (size_t)gridDim.x*blockDim.x;
+	for (size_t i = (size_t)blockIdx.x*blockDim.x + threadIdx.x; i < n; i += stride) {float const a = fabsf(__ldg(v + i)); if (a == a) {m = max(m, __float_as_uint(a));}}
+	for (int o = 16; o > 0; o >>= 1) {m = max(m, __shfl_xor_sync(0xffffffffu, m, o));}
+	if ((threadIdx.x & 31) == 0 && m) {atomicMax(absmax, m);}
+}
+
+// calc_zminmax -> estimate_zminmax -> set_zvals of gen_mesh (src/mesh_gen.cpp:447-504) on one thread, with the host chain's operation types: the double products
+// rounded to float, and water_plane_z = get_water_z_height's tail, wpz (its zmax_est-free head) computed on the host
+__global__ void gen_mesh_zvals_kernel(twi_gen_mesh_rec *rec, bool sine_mode, float wpz, float water_h_off, float prev_zbottom, float prev_ztop, float prev_wpz) {
+	float const zmin = tw_ord2f(rec->mm[0]), zmax = tw_ord2f(rec->mm[1]);
+	float zmax_est = (zmax < -zmin) ? -zmin : zmax;                  // set_zmax_est(max(zmax, -zmin))
+	if (zmax == zmin) { // flat mesh: estimate_zminmax returns before set_zvals (src/mesh_gen.cpp:463-466)
+		zmax_est = (float)((double)zmax_est + 1.0E-6);
+		rec->zmin = zmin; rec->zmax = zmax; rec->zbottom = prev_zbottom; rec->ztop = prev_ztop; rec->water_plane_z = prev_wpz;
+	}
+	else {
+		float const a = __uint_as_float(rec->absmax);
+		zmax_est = (zmax_est < a) ? a : zmax_est;
+		if (!sine_mode) {zmax_est = (float)((double)zmax_est*1.2);}
+		zmax_est = (float)(1.1*(double)zmax_est);
+		rec->zbottom = zmin; rec->ztop = zmax; rec->zmin = -zmax_est; rec->zmax = zmax_est; // set_zvals
+		float const zmax_est2 = (float)(2.0*(double)zmax_est);           // get_water_z_height (src/mesh_gen.cpp:507-512)
+		rec->water_plane_z = wpz*zmax_est2 - zmax_est + water_h_off;
+	}
+	rec->zmax_est = zmax_est;
+	rec->zmax_est2 = (float)(2.0*(double)zmax_est); rec->zmax_est2_inv = (float)(1.0/(double)rec->zmax_est2); // set_zmax_est, as twi_glaciate_mesh derives them
+	rec->mm[0] = 0xffffffffu; rec->mm[1] = 0u; // for the glaciated mesh's min/max
+}
+
+__global__ void gen_mesh_zbottom_kernel(twi_gen_mesh_rec *rec) {rec->zbottom = tw_ord2f(rec->mm[0]); rec->ztop = tw_ord2f(rec->mm[1]);} // glaciate(), :399-403
 
 
 // One thread per cell of the stride^2 normal map (stride = zvsize-1). get_norm_not_normalized(ix) = (DY_VAL*(z[ix] - z[ix+1]),
@@ -158,7 +200,7 @@ int twi_tile_bounds(tw_ctx *ctx, cudaStream_t st, const float *d_zvals, uint32_t
 	return TW_OK;
 }
 
-int twi_glaciate_mesh(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, unsigned *d_mm) {
+static GlacParams glac_params(int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p) {
 	GlacParams P;
 	memset(&P, 0, sizeof(P));
 	P.glaciate = (p->glaciate != 0);
@@ -168,7 +210,33 @@ int twi_glaciate_mesh(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int
 	P.volcano_on = (p->hmap.volcano_width > 0.0f && p->hmap.volcano_height > 0.0f);
 	P.volcano_freq = P.volcano_on ? p->mesh_scale/p->hmap.volcano_width : 0.0f; P.volcano_height = p->hmap.volcano_height;
 	P.nx = nx; P.ny = ny; P.x_shift = xoff2 - MX/2; P.y_shift = yoff2 - MY/2;
-	glaciate_mesh_kernel<<<dim3((nx + 255)/256, ny), 256, 0, ctx->stream>>>(d_mesh, P, ctx->d_sin_table, d_mm);
+	return P;
+}
+
+int twi_glaciate_mesh(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, unsigned *d_mm) {
+	glaciate_mesh_kernel<false><<<dim3((nx + 255)/256, ny), 256, 0, ctx->stream>>>(d_mesh, glac_params(nx, ny, xoff2, yoff2, MX, MY, p), ctx->d_sin_table, d_mm, nullptr);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+int twi_glaciate_mesh_rec(tw_ctx *ctx, float *d_mesh, int nx, int ny, int xoff2, int yoff2, int MX, int MY, const tw_height_params *p, twi_gen_mesh_rec *d_rec) {
+	glaciate_mesh_kernel<true><<<dim3((nx + 255)/256, ny), 256, 0, ctx->stream>>>(d_mesh, glac_params(nx, ny, xoff2, yoff2, MX, MY, p), ctx->d_sin_table, d_rec->mm, d_rec);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+int twi_gen_mesh_zbottom(tw_ctx *ctx, twi_gen_mesh_rec *d_rec) {
+	gen_mesh_zbottom_kernel<<<1, 1, 0, ctx->stream>>>(d_rec);
+	TW_LAUNCH_CHECK(ctx);
+	return TW_OK;
+}
+
+int twi_gen_mesh_zvals(tw_ctx *ctx, twi_gen_mesh_rec *d_rec, const float *d_probe, size_t n, bool sine_mode, float wpz, float water_h_off,
+                       float prev_zbottom, float prev_ztop, float prev_water_plane_z) {
+	unsigned const blocks = (unsigned)std::min<size_t>((n + 255)/256, (size_t)ctx->num_sms*8);
+	probe_absmax_kernel<<<blocks ? blocks : 1, 256, 0, ctx->stream>>>(d_probe, n, &d_rec->absmax);
+	TW_LAUNCH_CHECK(ctx);
+	gen_mesh_zvals_kernel<<<1, 1, 0, ctx->stream>>>(d_rec, sine_mode, wpz, water_h_off, prev_zbottom, prev_ztop, prev_water_plane_z);
 	TW_LAUNCH_CHECK(ctx);
 	return TW_OK;
 }

@@ -11,6 +11,7 @@
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //   tw3d::update_heightmap, tw3d::hmap_tiles_touched  <->  terrain_hmap_manager_t's brush edits and re-applied modmap, and the tiles they change   src/heightmap.cpp:36-58,243-308
+//   tw3d::gen_mesh_async         <->  gen_mesh in ground mode at start-up and on every regeneration, without stalling the frame   src/mesh_gen.cpp:257-355
 //   tw3d::get_exact_zvals_async, tw3d::heightmap_heights_async  <->  get_exact_zval / get_clamped_height per placed object, without stalling the frame   src/mesh_gen.cpp:816-847, src/heightmap.cpp:385-402
 //   tw3d::set_deferred_gens, tw3d::tile_job_pool  <->  several of them in flight at once, as tile_draw_t::update keeps up to 8   src/tiled_mesh.cpp:2367-2417
 //   tw3d::tile_set               <->  the live tiles' calc_shadows_for_light when the light moves or new tiles appear   src/tiled_mesh.cpp:664-692
@@ -27,6 +28,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <stdexcept>
@@ -331,21 +333,33 @@ class tiles_job {
 	std::atomic<uint64_t> const *latest = nullptr; // the launch count of c's thread
 	uint64_t number = 0;
 	bool done = true, was_cancelled = false, cancel_asked = false;
+	std::function<void()> on_done; // run once when the job completes and was not cut short (gen_mesh_async: the derived globals)
 	bool poll(bool wait) {
 		if (done) return true;
-		if (latest->load() != number) {done = true; was_cancelled = cancel_asked; return true;} // a later launch on the same context completed this job before it started
-		int const rc = tw_create_tiles_poll(c, wait ? 1 : 0);
-		if (rc == TW_ERR_NOT_READY) return false;
-		done = true;
-		if (rc == TW_ERR_CANCELED) {was_cancelled = true; return true;}
-		if (rc != TW_OK) {detail::fail(rc, "create_tiles_async", c);}
+		if (latest->load() != number) {done = true; was_cancelled = cancel_asked;} // a later launch on the same context completed this job before it started
+		else {
+			int const rc = tw_create_tiles_poll(c, wait ? 1 : 0);
+			if (rc == TW_ERR_NOT_READY) return false;
+			done = true;
+			if (rc == TW_ERR_CANCELED) {was_cancelled = true;}
+			else if (rc != TW_OK) {on_done = nullptr; detail::fail(rc, "create_tiles_async", c);}
+		}
+		if (on_done && !was_cancelled) {std::function<void()> const f = std::move(on_done); on_done = nullptr; f();}
 		return true;
 	}
 public:
 	tiles_job() = default;
-	tiles_job(tw_ctx *ctx_, std::atomic<uint64_t> const *latest_, uint64_t number_) : c(ctx_), latest(latest_), number(number_), done(false) {}
-	tiles_job(tiles_job &&o) noexcept : c(o.c), latest(o.latest), number(o.number), done(o.done), was_cancelled(o.was_cancelled), cancel_asked(o.cancel_asked) {o.done = true;}
-	tiles_job &operator=(tiles_job &&o) {if (this != &o) {wait(); c = o.c; latest = o.latest; number = o.number; done = o.done; was_cancelled = o.was_cancelled; cancel_asked = o.cancel_asked; o.done = true;} return *this;}
+	tiles_job(tw_ctx *ctx_, std::atomic<uint64_t> const *latest_, uint64_t number_, std::function<void()> on_done_ = nullptr)
+		: c(ctx_), latest(latest_), number(number_), done(false), on_done(std::move(on_done_)) {}
+	tiles_job(tiles_job &&o) noexcept : c(o.c), latest(o.latest), number(o.number), done(o.done), was_cancelled(o.was_cancelled), cancel_asked(o.cancel_asked),
+		on_done(std::move(o.on_done)) {o.done = true; o.on_done = nullptr;}
+	tiles_job &operator=(tiles_job &&o) {
+		if (this != &o) {
+			wait(); c = o.c; latest = o.latest; number = o.number; done = o.done; was_cancelled = o.was_cancelled; cancel_asked = o.cancel_asked;
+			on_done = std::move(o.on_done); o.done = true; o.on_done = nullptr;
+		}
+		return *this;
+	}
 	tiles_job(tiles_job const &) = delete;
 	tiles_job &operator=(tiles_job const &) = delete;
 	~tiles_job() {try {wait();} catch (...) {}}
@@ -573,6 +587,9 @@ inline tiles_job erode_heightmap_sweeps_async(float val_mult, float val_add, uns
 // flight; when every slot is busy, on the slot launched on longest ago, whose job that launch completes first (its tiles_job then reports ready).
 // A launch never waits for another slot's job. Create and use the pool on one thread, let it outlive the jobs it returned, and destroy it before the
 // thread ends (its contexts are shared contexts of the thread's context); destroying it completes its jobs.
+// the z globals gen_mesh leaves (gen_mesh, gen_mesh_async below)
+struct gen_mesh_result {float zmin, zmax, zmax_est, zbottom, ztop, water_plane_z;};
+
 class tile_job_pool {
 	friend class tile_set; // its frame launches take a slot too
 	struct slot {tw_ctx *c = nullptr; std::atomic<uint64_t> jobs{0}; uint64_t launched = 0;};
@@ -626,6 +643,9 @@ public:
 		tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
 		return detail::launch_tiles(s.c, s.jobs, &hs, origins_xy, ntiles, zvsize, dx, dy, erosion_iters_tt, wpz_max, size, out, shading, shadows);
 	}
+	// gen_mesh_async (below) on a slot, beside the frames in flight on the others
+	tiles_job gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters, int xoff2 = 0, int yoff2 = 0,
+	                         float dx_val = 0.0f, float dy_val = 0.0f, float water_h_off = 0.0f, float water_h_off_rel = 0.0f, gen_mesh_result *result = nullptr);
 	// object placement (get_exact_zvals_async / heightmap_heights_async above) on a slot, beside the frames in flight on the others
 	tiles_job get_exact_zvals_async(const float *xy, size_t n, float *zvals_out, bool no_xyoff = false) {
 		slot &s = next();
@@ -804,7 +824,6 @@ inline void create_texture_weights(const float *zvals, const int32_t *origins_xy
 // the function-static generator state (pass the same tw_rng across calls), fills mesh_height, estimates zmax_est from a 128x128 probe of the
 // equation (estimate_zminmax, :447-485), sets the z globals (set_zvals, :494-504), glaciates (:388-404) and erodes (:443).
 // The derived globals are written back into scene_globals (zmax_est, zmin, zmax, water_plane_z) exactly as the reference leaves them.
-struct gen_mesh_result {float zmin, zmax, zmax_est, zbottom, ztop, water_plane_z;};
 
 inline gen_mesh_result gen_mesh(float *mesh_height /* MESH_Y_SIZE x MESH_X_SIZE, row-major */, tw_rng &sine_rng, float x_scene_size, float y_scene_size,
 	unsigned erosion_iters, int xoff2 = 0, int yoff2 = 0, float dx_val = 0.0f, float dy_val = 0.0f, float water_h_off = 0.0f, float water_h_off_rel = 0.0f)
@@ -855,6 +874,53 @@ inline gen_mesh_result gen_mesh(float *mesh_height /* MESH_Y_SIZE x MESH_X_SIZE,
 	}
 	apply_erosion(mesh_height, MX, MY, r.zbottom, erosion_iters);
 	return r;
+}
+
+// gen_mesh as a job that does not stall the frame (tw_gen_mesh_launch): the sine table is made from sine_rng and set as gen_mesh does, then the rest - the
+// fill, the z estimate, set_zvals, glaciation and erosion - is one job that returns at once. Once ready() (or wait()) returns, mesh_height, *result and
+// tw_last_erosion_steps() of the job's context are gen_mesh's, bit for bit, and the derived globals (zmax_est, zmin, zmax, water_plane_z, zbottom, ztop) have
+// been written into scene_globals as gen_mesh writes them; a cancelled job writes neither. mesh_height (MESH_Y_SIZE x MESH_X_SIZE) is device, page-locked or
+// pageable host memory (the last is filled when the job is ready) and must stay valid until then. tile_job_pool::gen_mesh_async runs it on a pool slot.
+namespace detail {
+	inline void gen_mesh_tables(tw_rng &sine_rng, float x_scene_size, float y_scene_size) { // gen_mesh's sine table, set as the thread's tables
+		scene_globals const g = globals();
+		std::vector<float> sinTable(TW_F_TABLE_SIZE*5);
+		tw_gen_sine_params(&sine_rng, g.MESH_HEIGHT*g.mesh_height_scale, g.MESH_X_SIZE, g.MESH_Y_SIZE, x_scene_size, y_scene_size, g.mesh_seed, g.mesh_rgen_index,
+		                   g.mesh_gen_mode, g.MESH_START_MAG, g.MESH_START_FREQ, g.MESH_MAG_MULT, g.MESH_FREQ_MULT, sinTable.data());
+		set_globals(g, nullptr, sinTable.data());
+	}
+	inline tiles_job launch_gen_mesh(tw_ctx *c, std::atomic<uint64_t> &jobs, float *mesh_height, float x_scene_size, float y_scene_size, unsigned erosion_iters,
+	                                 int xoff2, int yoff2, float dx_val, float dy_val, float water_h_off, float water_h_off_rel, gen_mesh_result *result) {
+		scene_globals const g = globals();
+		if (dx_val == 0.0f) {dx_val = 1.0f/g.DX_VAL_INV;}
+		if (dy_val == 0.0f) {dy_val = 1.0f/g.DY_VAL_INV;}
+		tw_height_params const p = height_params_from_globals(g.mesh_gen_mode, g.mesh_gen_shape);
+		tw_erosion_params const e = erosion_params_from_globals();
+		std::shared_ptr<tw_gen_mesh_info> const info = std::make_shared<tw_gen_mesh_info>();
+		tw_gen_mesh_job const job = {g.MESH_X_SIZE, g.MESH_Y_SIZE, xoff2, yoff2, dx_val, dy_val, x_scene_size, y_scene_size, &p, erosion_iters, &e,
+		                             water_h_off, water_h_off_rel, g.zbottom, g.ztop, g.water_plane_z, mesh_height, info.get()};
+		uint64_t const number = ++jobs;
+		int const rc = tw_gen_mesh_launch(c, &job);
+		if (rc != TW_OK) {--jobs; fail(rc, "gen_mesh_async", c);}
+		return tiles_job(c, &jobs, number, [info, result]() {
+			scene_globals g = globals();
+			g.zmax_est = info->zmax_est; g.zmin = info->zmin; g.zmax = info->zmax; g.water_plane_z = info->water_plane_z; g.zbottom = info->zbottom; g.ztop = info->ztop;
+			set_globals(g);
+			if (result) {*result = gen_mesh_result{info->zmin, info->zmax, info->zmax_est, info->zbottom, info->ztop, info->water_plane_z};}
+		});
+	}
+}
+inline tiles_job gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters, int xoff2 = 0, int yoff2 = 0,
+                                float dx_val = 0.0f, float dy_val = 0.0f, float water_h_off = 0.0f, float water_h_off_rel = 0.0f, gen_mesh_result *result = nullptr) {
+	detail::gen_mesh_tables(sine_rng, x_scene_size, y_scene_size);
+	return detail::launch_gen_mesh(ctx(), detail::tls().tile_jobs, mesh_height, x_scene_size, y_scene_size, erosion_iters, xoff2, yoff2, dx_val, dy_val,
+	                               water_h_off, water_h_off_rel, result);
+}
+inline tiles_job tile_job_pool::gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters, int xoff2, int yoff2,
+                                               float dx_val, float dy_val, float water_h_off, float water_h_off_rel, gen_mesh_result *result) {
+	detail::gen_mesh_tables(sine_rng, x_scene_size, y_scene_size); // before the slot is picked: the slots' jobs complete before the new tables go up
+	slot &s = next();
+	return detail::launch_gen_mesh(s.c, s.jobs, mesh_height, x_scene_size, y_scene_size, erosion_iters, xoff2, yoff2, dx_val, dy_val, water_h_off, water_h_off_rel, result);
 }
 
 // tail of tile_t::create_zvals for a batch of finished tiles (sub_zmin/sub_zmax, mzmin/mzmax, mesh_dz, radius, water bbox), src/tiled_mesh.cpp:517-541

@@ -177,3 +177,14 @@ def gen_mesh(ctx, cfg, erosion_iters=0, xoff2=0, yoff2=0, sine_rng=None):
     if erosion_iters > 0:
         ctx.erode(mesh, float(zbottom), erosion_iters, ep)
     return mesh, dict(zmin=float(zmin), zmax=float(zmax), zmax_est=float(zmax_est), zbottom=float(zbottom), ztop=float(ztop), water_plane_z=float(wpz)), sp
+
+
+def gen_mesh_async(ctx, cfg, erosion_iters=0, xoff2=0, yoff2=0, sine_rng=None, prev=(0.0, 0.0, 0.0), mesh=None):
+    """gen_mesh as one asynchronous job (Context.gen_mesh_launch): the sine table is made and set here, as gen_mesh does, and everything after it runs on
+    the device. prev = (zbottom, ztop, water_plane_z) before the call, which a flat mesh keeps. Returns (job, sine_params); job.poll(wait) gives (mesh[MY, MX],
+    info) once the job is complete, with gen_mesh's info for a mesh that is not flat. cfg.zmax_est is not updated: set it from info['zmax_est']."""
+    sp = cfg.sine_params(rng=sine_rng)
+    ctx.set_sine_params(sp)
+    job = ctx.gen_mesh_launch(cfg.mesh_size[:2], cfg.height_params(), cfg.erosion_params(), erosion_iters, xoff2, yoff2, float(cfg.dx_val), float(cfg.dy_val),
+                              cfg.scene_size[:2], cfg.water_h_off, cfg.water_h_off_rel, prev, mesh)
+    return job, sp

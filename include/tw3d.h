@@ -478,6 +478,47 @@ typedef struct tw_heightmap_outputs {
 } tw_heightmap_outputs;
 TW_API int tw_proc_gen_heightmap_launch(tw_ctx *ctx, uint32_t width, uint32_t height, float dx_val, float dy_val, const tw_height_params *p,
                                         uint32_t erosion_iters, const tw_erosion_params *ep, const tw_heightmap_outputs *out);
+/* gen_mesh() of the ground mode (src/mesh_gen.cpp:257-355) after its sine table, as the context's ASYNCHRONOUS job: the mesh fill (gen_mesh_sine_table,
+ * :201-210), calc_zminmax, the 128x128 probe of estimate_zminmax (:447-485), set_zvals (:494-504), glaciate() (:388-404) and apply_erosion(mesh, X, Y,
+ * zbottom, erosion_iters) (:443) are enqueued without the host reading anything back: every scalar a step takes from the data (zmax_est, zbottom, the
+ * erosion's zmin / zmax / water_plane_z) is derived on the device, and the speculative erosion's rounds end on the device. After the completing poll mesh,
+ * every field of info and tw_last_erosion_steps() equal, bit for bit, the synchronous chain tw_heightgen_2d of the mesh -> tw_heightgen_2d of the probe ->
+ * the host's zmax_est / set_zvals arithmetic -> tw_glaciate_mesh (p->glaciate) -> tw_erode(min_zval = zbottom) with these arguments (tw3d::gen_mesh).
+ * - Run tw_gen_sine_params and tw_set_sine_params first, as gen_mesh does: the job reads the context's tables like every other job.
+ * - p->zmax_est is ignored: the job derives it. ep's erode_amount, half_dxy, relh_adj_tex and clip_hd1 are read; its zmin, zmax and water_plane_z are the
+ *   ones set_zvals leaves (-zmax_est, zmax_est, get_water_z_height(zmax_est) from water_h_off / water_h_off_rel and p's glaciation). The probe's step is
+ *   rm_scale = 1000*XY_SCENE_SIZE/mesh_scale with XY_SCENE_SIZE = 0.5*(x_scene_size + y_scene_size) and p->mesh_scale.
+ * - A flat mesh (zmin == zmax) keeps what the reference keeps: estimate_zminmax returns before set_zvals, so zmin / zmax are the measured pair and zbottom,
+ *   ztop and water_plane_z are the caller's prev_* values (glaciation still replaces zbottom / ztop). The erosion then takes the per-move rock expression
+ *   with zmax - zmin = 0, as tw_erode does.
+ * - No erosion (erosion_iters == 0 or erode_amount <= 0, src/erosion.cpp:16): info->erosion_moves and tw_last_erosion_steps() are 0.
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it (wait = 0 returns TW_ERR_NOT_READY while it runs), every
+ *   other entry point and tw_destroy complete it first. On a shared context it runs beside the other contexts' jobs. tw_cancel stops the erosion at its
+ *   cancellation points (as for tw_erode_launch); the poll then returns TW_ERR_CANCELED and the outputs are unspecified.
+ * - mesh is device, page-locked or pageable host memory; pageable mesh is filled by the completing poll. With device or page-locked mesh the launch never
+ *   waits for the device, except when the context's scratch or staging first has to grow. Every buffer is reserved before anything is enqueued.
+ * - The erosion walks the map in the mode tw_erode picks for it (the serial order's result does not depend on the mode): M_SPEC's speculative rounds from
+ *   2^20 padded cells and 64 droplets on. A window that stops making progress makes the poll return TW_ERR_STATE with tw_erode's message.
+ * - Errors, nothing enqueued: TW_ERR_ARG for a NULL job, p, ep or mesh, a mesh size <= 0 (or a mesh_y_size above 65535), and what tw_heightgen_2d refuses
+ *   for either grid; TW_ERR_STATE without the sin table or, in sine mode, the sine params. */
+typedef struct tw_gen_mesh_info {
+	float    zmin, zmax, zmax_est, zbottom, ztop, water_plane_z; /* the z globals gen_mesh leaves */
+	uint64_t erosion_moves;                                      /* droplet moves of the erosion (tw_last_erosion_steps()) */
+} tw_gen_mesh_info;
+typedef struct tw_gen_mesh_job {
+	int                       mesh_x_size, mesh_y_size;  /* MESH_X_SIZE, MESH_Y_SIZE: the mesh is mesh_y_size rows of mesh_x_size floats */
+	int                       xoff2, yoff2;              /* the mesh's scroll offset */
+	float                     dx_val, dy_val;            /* DX_VAL, DY_VAL */
+	float                     x_scene_size, y_scene_size;/* X_SCENE_SIZE, Y_SCENE_SIZE: the probe's step */
+	const tw_height_params   *p;                         /* required, copied during the launch; zmax_est is ignored */
+	uint32_t                  erosion_iters;
+	const tw_erosion_params  *ep;                        /* required, copied during the launch: erode_amount, half_dxy, relh_adj_tex, clip_hd1 */
+	float                     water_h_off, water_h_off_rel;
+	float                     prev_zbottom, prev_ztop, prev_water_plane_z; /* zbottom, ztop, water_plane_z before the call: a flat mesh keeps them */
+	float                    *mesh;                      /* required: mesh_x_size*mesh_y_size floats, device, page-locked or pageable host memory */
+	tw_gen_mesh_info         *info;                      /* optional HOST: filled by the completing poll */
+} tw_gen_mesh_job;
+TW_API int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job);
 /* Heightmap-texture mode of tile_t::create_zvals (src/tiled_mesh.cpp:498-501; SURVEY.md 8f row N2): every cell of every tile is
  * terrain_hmap_manager_t::get_clamped_height(x1 + x, y1 + y) (src/heightmap.cpp:385-402) of a 16-bit heightmap image -
  *   mesh_scale < 1: bilinear interpolate_height(); otherwise the nearest texel round_fp(mesh_scale*x) (clamp_xy, :309-313);

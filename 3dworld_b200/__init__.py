@@ -219,6 +219,7 @@ def hmap_params(**kw):
 
 # every symbol include/tw3d.h declares (tests check the library exports exactly these)
 ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", "tw_last_error", "tw_sync", "tw_stream", "tw_launch_count",
+               "tw_dwarp_window_launches",
                "tw_build_sin_table", "tw_compute_scale", "tw_gen_sine_params", "tw_gen_rx_ry", "tw_noise3d_gen_sines",
                "tw_water_z_height", "tw_set_sin_table", "tw_set_sine_params", "tw_heightgen_2d", "tw_heightgen_2d_launch",
                "tw_heightgen_2d_poll", "tw_heightgen_tiles", "tw_create_zvals_batch", "tw_create_tiles_launch", "tw_create_tiles_launch_ex", "tw_create_tiles_poll", "tw_tile_bounds_batch", "tw_tile_normals_batch", "tw_tile_ao_batch", "tw_create_zvals_ao_batch", "tw_glaciate_mesh", "tw_eval_points", "tw_erode", "tw_erode_parallel", "tw_erode_tiles", "tw_last_erosion_steps", "tw_voxel_fill",
@@ -251,6 +252,8 @@ def _load():
     L.tw_stream.restype = vp
     L.tw_launch_count.argtypes = [vp]
     L.tw_launch_count.restype = C.c_uint64
+    L.tw_dwarp_window_launches.argtypes = [vp]
+    L.tw_dwarp_window_launches.restype = C.c_uint64
     L.tw_cancel.argtypes = [vp]
     L.tw_build_sin_table.argtypes = [vp]
     L.tw_build_sin_table.restype = None
@@ -698,6 +701,11 @@ class Context:
     @property
     def launch_count(self):
         return int(lib.tw_launch_count(self._h))
+
+    @property
+    def dwarp_window_launches(self):
+        """Of launch_count, the launches of the domain-warp kernel with lattice windows (tw_dwarp_window_launches)"""
+        return int(lib.tw_dwarp_window_launches(self._h))
 
     def sync(self):
         self._check(lib.tw_sync(self._h))

@@ -349,6 +349,7 @@ void tw_destroy(tw_ctx *ctx) {
 const char *tw_last_error(const tw_ctx *ctx) {return ctx ? ctx->err : "null context";}
 void *tw_stream(tw_ctx *ctx) {return ctx ? (void *)ctx->stream : nullptr;}
 uint64_t tw_launch_count(const tw_ctx *ctx) {return ctx ? ctx->launches : 0;}
+uint64_t tw_dwarp_window_launches(const tw_ctx *ctx) {return ctx ? ctx->dwarp_win_launches : 0;}
 uint64_t tw_last_erosion_steps(const tw_ctx *ctx) {return ctx ? ctx->last_erosion_steps : 0;}
 
 // "cancel job k" into the device words, by a copy on the context's cancel stream: nothing waits, nothing goes to ctx->stream

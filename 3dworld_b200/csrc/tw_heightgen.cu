@@ -741,7 +741,8 @@ static bool make_noise_params(const tw_height_params *p, NoiseParams &N, bool &s
 // in both coordinates (f, Cy > 0), so the two corners bound every cell inside the box exactly; the kernel checks each pair against the box and
 // takes the reducing loop outside it. false: a window is wider than the tables (large grids, far-out origins) or not finite - keep the reducing kernel.
 #ifndef TW_DWARP_WARP_MARGIN
-#define TW_DWARP_WARP_MARGIN 0.45f   // a build with a margin below the displacement sends pairs of stages 2-4 outside their box (the path the tests check it with)
+#define TW_DWARP_WARP_MARGIN 0.45f   // a build with a margin below the displacement sends pairs of stages 2-4 outside their box: tests/test_gpu_dwarp_windows_paths.py
+                                     // builds margins 0 and 0.05 to check that path
 #endif
 static bool dwarp_windows(DwarpWindows &W, const NoiseParams &N, const PostParams &P, unsigned nx, unsigned r0, unsigned r1, float mx0, float my0) {
 	constexpr float WARP_MARGIN = TW_DWARP_WARP_MARGIN, Cy = 0.366025403784439f;
@@ -818,6 +819,7 @@ int twi_heightgen(tw_ctx *ctx, const tw_grid2d *g, const tw_height_params *p, in
 					launch_noise2_win(dim3((TW_NOISE2_PERSISTENT && gx > wave) ? wave : gx), dim3(noise2_threads<true>()), ctx->stream, d_out, nx, ny, r0, r1, mx0, my0, N, P,
 					                  ctx->d_sin_table, d_mm_ord, (const float4 *)ctx->d_simplex_lut + WIN_LUT_OFFSET, W);
 					TW_LAUNCH_CHECK(ctx);
+					ctx->dwarp_win_launches++;
 					if (h_out_bands) {int const rc = band_copy(ctx, h_out_bands, d_out, nx, r0, r1); if (rc) return rc;}
 					continue;
 				}

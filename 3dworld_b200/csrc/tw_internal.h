@@ -64,6 +64,7 @@ struct tw_ctx {
 	const unsigned *tile_perm = nullptr; // set around twi_heightgen by the tile pipeline: output slot of each generated tile
 	char err[512] = {0};
 	uint64_t launches = 0;
+	uint64_t dwarp_win_launches = 0;   // of those, launches of the windowed domain-warp kernel (tw_dwarp_window_launches)
 	uint64_t last_erosion_steps = 0;
 	// uploaded tables
 	float  *d_sin_table = nullptr;     // [65536]  sin_table (src/sinf.h:11)

@@ -144,6 +144,8 @@ TW_API const char *tw_last_error(const tw_ctx *ctx);
 TW_API int  tw_sync(tw_ctx *ctx);                         /* cudaStreamSynchronize on the context stream */
 TW_API void *tw_stream(tw_ctx *ctx);                      /* the cudaStream_t all work of this context is issued on */
 TW_API uint64_t tw_launch_count(const tw_ctx *ctx);       /* kernels launched by this context so far (bench.py gpu_launches) */
+TW_API uint64_t tw_dwarp_window_launches(const tw_ctx *ctx); /* of those, launches of the domain-warp kernel with lattice windows (one per grid or
+                                                            * row band whose windows fit its tables; every other launch of that mode reduces mod 289) */
 /* Asks the context's pending asynchronous job to stop, for work the caller no longer wants (a map reloaded or the scene quit while it is eroded, tiles
  * that went out of range, a voxel model replaced while its fills run). Returns at once: it never waits for the device and enqueues nothing on the
  * context's stream. Called by the thread that owns the context, like every other entry point.

@@ -200,6 +200,11 @@ class GenMeshJobArgs(C.Structure):
                 ("prev_water_plane_z", C.c_float), ("mesh", C.c_void_p), ("info", C.c_void_p)]
 
 
+class MeshShadowsJobArgs(C.Structure):
+    """tw_mesh_shadows_job (include/tw3d.h): one mesh and the lights tw_mesh_shadows_launch traces over it."""
+    _fields_ = [("mesh", C.c_void_p), ("xsize", C.c_int), ("ysize", C.c_int), ("nlights", C.c_uint32), ("lights", C.c_void_p)]
+
+
 class SweepParams(C.Structure):
     """tw_sweep_params (include/tw3d.h): tw_erode_sweeps' sweep and halo for tw_erode_launch_ex's TW_EROSION_SWEEPS mode."""
     _fields_ = [("sweep", C.c_uint32), ("halo", C.c_int)]
@@ -232,7 +237,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
                "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
-               "tw_points_launch", "tw_gen_mesh_launch"]
+               "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows"]
 
 
 def _load():
@@ -296,6 +301,9 @@ def _load():
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_points_launch.argtypes = [vp, C.POINTER(PointsJobArgs)]
     L.tw_gen_mesh_launch.argtypes = [vp, C.POINTER(GenMeshJobArgs)]
+    L.tw_gen_mesh_launch_shadows.argtypes = [vp, C.POINTER(GenMeshJobArgs), C.c_uint32, vp]
+    L.tw_mesh_shadows.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
+    L.tw_mesh_shadows_launch.argtypes = [vp, C.POINTER(MeshShadowsJobArgs)]
     L.tw_erode_parallel.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_uint32, C.POINTER(ErosionParams), C.c_uint32]
     L.tw_erode_launch.argtypes = [vp, C.POINTER(ErosionJobArgs)]
     L.tw_erode_launch_ex.argtypes = [vp, C.POINTER(ErosionJobArgs), C.POINTER(SweepParams)]
@@ -623,15 +631,47 @@ class PointsJob:
 
 class GenMeshJob:
     """What Context.gen_mesh_launch returns: poll(wait) completes the job (the context's pending job) and returns (mesh, info dict with the keys of
-    scene.gen_mesh's plus erosion_moves), or None while it runs (wait=False)."""
+    scene.gen_mesh's plus erosion_moves), or None while it runs (wait=False). With lights it returns (mesh, info, shadows), shadows as MeshShadowsJob's."""
 
-    def __init__(self, ctx, mesh):
-        self._ctx, self.mesh, self.info = ctx, mesh, GenMeshInfo()
+    def __init__(self, ctx, mesh, lights=None):
+        self._ctx, self.mesh, self.info, self.lights = ctx, mesh, GenMeshInfo(), lights
 
     def poll(self, wait=False):
         if not self._ctx.create_tiles_poll(wait):
             return None
-        return self.mesh, {n: (int if n == "erosion_moves" else float)(getattr(self.info, n)) for n, _ in GenMeshInfo._fields_}
+        info = {n: (int if n == "erosion_moves" else float)(getattr(self.info, n)) for n, _ in GenMeshInfo._fields_}
+        if self.lights is None:
+            return self.mesh, info
+        return self.mesh, info, [(r.smask, r.sh_out_x, r.sh_out_y) for r in self.lights]
+
+
+class MeshShadowsJob:
+    """What Context.mesh_shadows_launch returns: poll(wait) completes the job (the context's pending job) and returns one (smask, sh_out_x, sh_out_y) per
+    light, or None while it runs (wait=False)."""
+
+    def __init__(self, ctx, lights):
+        self._ctx, self.lights = ctx, lights
+
+    def poll(self, wait=False):
+        if not self._ctx.create_tiles_poll(wait):
+            return None
+        return [(r.smask, r.sh_out_x, r.sh_out_y) for r in self.lights]
+
+
+def _mesh_lights(lights, xsize, ysize):
+    """Light records for a whole xsize x ysize mesh and their TileLight array: each light is a Light, a (ShadowParams, smask, sh_out_x, sh_out_y, sh_in_x,
+    sh_in_y) tuple, or a bare ShadowParams, whose smask [ysize, xsize] uint8, sh_out_x [xsize] and sh_out_y [ysize] float32 are new numpy arrays."""
+    recs = []
+    for lt in lights:
+        if isinstance(lt, ShadowParams):
+            lt = Light(lt, np.empty((ysize, xsize), np.uint8), np.empty(xsize, np.float32), np.empty(ysize, np.float32))
+        elif not isinstance(lt, Light):
+            lt = Light(*lt)
+        recs.append(Light(lt.sp, lt.smask, lt.sh_out_x, lt.sh_out_y, _edge(lt.sh_in_x), _edge(lt.sh_in_y)))
+    arr = (TileLight * max(1, len(recs)))()
+    for i, r in enumerate(recs):
+        arr[i] = TileLight(r.sp, _ptr(r.sh_in_x), _ptr(r.sh_in_y), _ptr(r.smask), _ptr(r.sh_out_x), _ptr(r.sh_out_y))
+    return recs, arr
 
 
 class Context:
@@ -928,23 +968,50 @@ class Context:
         return job
 
     def gen_mesh_launch(self, mesh_size, hp, ep, erosion_iters=0, xoff2=0, yoff2=0, dx_val=None, dy_val=None, scene_size=(4.0, 4.0), water_h_off=0.0,
-                        water_h_off_rel=0.0, prev=(0.0, 0.0, 0.0), mesh=None):
+                        water_h_off_rel=0.0, prev=(0.0, 0.0, 0.0), mesh=None, lights=None):
         """tw_gen_mesh_launch: gen_mesh in ground mode after its sine table (set_sine_params first) as this context's asynchronous job. mesh_size =
         (MESH_X_SIZE, MESH_Y_SIZE); hp (its zmax_est is ignored) and ep (erode_amount, half_dxy, relh_adj_tex, clip_hd1 are read) are copied during the
         launch; dx_val / dy_val default to 1/hp.dx_val_inv, 1/hp.dy_val_inv; scene_size = (X_SCENE_SIZE, Y_SCENE_SIZE); prev = (zbottom, ztop, water_plane_z)
         before the call, which a flat mesh keeps. mesh = [MY, MX] floats (numpy array or torch tensor, host or CUDA; default a new numpy array).
-        Returns a GenMeshJob."""
+        lights (tw_gen_mesh_launch_shadows): a list of lights as mesh_shadows_launch takes them, traced over the final mesh with the job's own zmin / zmax
+        in place of each ShadowParams' (the GenMeshJob's poll then also returns the shadows). Returns a GenMeshJob."""
         MX, MY = int(mesh_size[0]), int(mesh_size[1])
         if mesh is None:
             mesh = np.empty((MY, MX), np.float32)
         dx = float(np.float32(1.0) / np.float32(hp.dx_val_inv)) if dx_val is None else dx_val
         dy = float(np.float32(1.0) / np.float32(hp.dy_val_inv)) if dy_val is None else dy_val
-        job = GenMeshJob(self, mesh)
+        recs, arr = _mesh_lights(lights, MX, MY) if lights is not None else (None, None)
+        job = GenMeshJob(self, mesh, recs)
         a = GenMeshJobArgs(MX, MY, xoff2, yoff2, dx, dy, scene_size[0], scene_size[1], C.cast(C.pointer(hp), C.c_void_p), erosion_iters,
                            C.cast(C.pointer(ep), C.c_void_p), water_h_off, water_h_off_rel, prev[0], prev[1], prev[2], _ptr(mesh),
                            C.cast(C.pointer(job.info), C.c_void_p))
-        self._check(lib.tw_gen_mesh_launch(self._h, C.byref(a)))
-        self._tiles_job = (mesh, job)
+        if lights is None:
+            self._check(lib.tw_gen_mesh_launch(self._h, C.byref(a)))
+        else:
+            self._check(lib.tw_gen_mesh_launch_shadows(self._h, C.byref(a), len(recs), C.cast(arr, C.c_void_p)))
+        self._tiles_job = (mesh, job, arr)
+        return job
+
+    def mesh_shadows(self, mesh, sp, sh_in_x=None, sh_in_y=None):
+        """tw_mesh_shadows: calc_mesh_shadows on the whole mesh [ysize, xsize] (numpy or CUDA) for one light: returns (smask [ysize, xsize] uint8,
+        sh_out_x [xsize] float32, sh_out_y [ysize] float32). sh_in_x [xsize] / sh_in_y [ysize] (numpy or CUDA): incoming heights."""
+        ysize, xsize = int(mesh.shape[0]), int(mesh.shape[1])
+        out, ox, oy = np.empty((ysize, xsize), np.uint8), np.empty(xsize, np.float32), np.empty(ysize, np.float32)
+        ix, iy = _edge(sh_in_x), _edge(sh_in_y)
+        self._check(lib.tw_mesh_shadows(self._h, _ptr(mesh), xsize, ysize, C.byref(sp), _ptr(ix), _ptr(iy), _ptr(out), _ptr(ox), _ptr(oy)))
+        return out, ox, oy
+
+    def mesh_shadows_launch(self, mesh, lights):
+        """tw_mesh_shadows_launch: calc_mesh_shadows on the whole mesh [ysize, xsize] (numpy or CUDA) for every light, as this context's asynchronous job.
+        lights: Light records, (ShadowParams, smask, sh_out_x, sh_out_y, sh_in_x, sh_in_y) tuples - smask [ysize, xsize] uint8 required, sh_*_x [xsize]
+        and sh_*_y [ysize] float32 or None - or bare ShadowParams (outputs allocated here). A host mesh and host sh_in rows are copied during the launch;
+        the outputs and device inputs are kept referenced here until the job completes. Returns a MeshShadowsJob."""
+        ysize, xsize = int(mesh.shape[0]), int(mesh.shape[1])
+        recs, arr = _mesh_lights(lights, xsize, ysize)
+        a = MeshShadowsJobArgs(_ptr(mesh), xsize, ysize, len(recs), C.cast(arr, C.c_void_p))
+        self._check(lib.tw_mesh_shadows_launch(self._h, C.byref(a)))
+        job = MeshShadowsJob(self, recs)
+        self._tiles_job = (mesh, job, arr)
         return job
 
     def erode(self, h, min_zval, num_iters, ep):

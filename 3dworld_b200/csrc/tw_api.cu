@@ -1471,13 +1471,17 @@ int tw_proc_gen_heightmap(tw_ctx *ctx, uint32_t width, uint32_t height, float dx
 // gen_mesh in ground mode as the context's asynchronous job: the mesh and the probe are generated, then one-thread kernels turn the data's min/max and the
 // probe's max |z| into the record's z values (twi_gen_mesh_zvals), glaciation reads zmax_est from the record and writes zbottom / ztop back, and the erosion
 // builds its parameters from the record (twi_erode_dev_enqueue); the record comes back through the pinned staging, which the completing poll unpacks.
-// Scratch slot 0: [mesh (unless on the device) | probe]; slot 1: the sine tables, then the erosion's scratch; slot 2: [fixed words | record];
-// pinned staging: [record | mesh (pageable mesh)].
-int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job) {
+// With lights, a mesh shadow pass (twi_mesh_pass) follows on the final mesh, its clip z range read from the record.
+// Scratch slot 0: [mesh (unless on the device) | probe | the shadow pass's]; slot 1: the sine tables, then the erosion's scratch; slot 2: [fixed words |
+// record]; pinned staging: [record | mesh (pageable mesh) | the shadow pass's].
+int tw_gen_mesh_launch_shadows(tw_ctx *ctx, const tw_gen_mesh_job *job, uint32_t nlights, const tw_tile_light *lights) {
 	int rc = twi_begin(ctx); if (rc) return rc;
 	if (!job || !job->p || !job->ep || !job->mesh) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
 	int const MX = job->mesh_x_size, MY = job->mesh_y_size;
 	if (MX <= 0 || MY <= 0 || MY > 65535) return tw_set_error(ctx, TW_ERR_ARG, "mesh size %d x %d", MX, MY);
+	if (nlights && !lights) return tw_set_error(ctx, TW_ERR_ARG, "nlights > 0 without lights");
+	twi_mesh_pass pass;
+	if (nlights) {rc = pass.make(ctx, MX, MY, nlights, lights); if (rc) return rc;}
 	tw_height_params const p = *job->p;
 	tw_erosion_params const ep = *job->ep;
 	tw_grid2d const grid = {(float)(job->xoff2 - MX/2), (float)(job->yoff2 - MY/2), job->dx_val, job->dy_val, (uint32_t)MX, (uint32_t)MY}; // gen_mesh_sine_table, src/mesh_gen.cpp:201-210
@@ -1491,19 +1495,20 @@ int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job) {
 	bool const erode = (iters > 0 && ep.erode_amount > 0.0); // apply_erosion, src/erosion.cpp:16
 	bool const dev = tw_is_device_ptr(job->mesh), locked = !dev && twi_is_page_locked(job->mesh);
 	float *d_mesh = job->mesh, *d_probe;
-	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {d_mesh = c.take<float>(n);} d_probe = c.take<float>(nprobe);}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {if (!dev) {d_mesh = c.take<float>(n);} d_probe = c.take<float>(nprobe); pass.carve_dev(c);}); if (rc) return rc;
 	size_t const s1 = std::max(erode ? twi_erode_dev_scratch_bytes(ctx, MX, MY, iters) : 0, std::max(twi_heightgen_slot1_bytes(&grid, &p), twi_heightgen_slot1_bytes(&probe, &p)));
 	if (s1) {rc = tw_reserve(ctx, 1, s1); if (rc) return rc;}
 	twi_gen_mesh_rec *d_rec;
 	rc = twi_reserve_carve(ctx, 2, [&](twi_carve &c) {c.take<twi_slot2_words>(1); d_rec = c.take<twi_gen_mesh_rec>(1);}); if (rc) return rc;
 	twi_gen_mesh_rec *h_rec; float *h_mesh = nullptr;
-	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {h_rec = c.take<twi_gen_mesh_rec>(1); if (!dev && !locked) {h_mesh = c.take<float>(n);}}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {h_rec = c.take<twi_gen_mesh_rec>(1); if (!dev && !locked) {h_mesh = c.take<float>(n);} pass.carve_pin(c);});
+	if (rc) return rc;
 	float const wpz = twi_water_rel(p.glaciate, p.custom_glaciate_exp, job->water_h_off_rel);
 	float *const mesh = job->mesh;
 	tw_gen_mesh_info *const info = job->info;
 	twi_job pending;
 	pending.cancellable = true;
-	pending.complete = [h_rec, h_mesh, mesh, n, info](tw_ctx *c) -> int {
+	pending.complete = [h_rec, h_mesh, mesh, n, info, pass](tw_ctx *c) -> int {
 		twi_gen_mesh_rec const r = *h_rec;
 		if (r.fail) {c->last_erosion_steps = 0; return tw_set_error(c, TW_ERR_STATE, "speculative erosion made no progress (%u rounds)", r.fail);}
 		c->last_erosion_steps = r.steps;
@@ -1512,6 +1517,7 @@ int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job) {
 			info->water_plane_z = r.water_plane_z; info->erosion_moves = r.steps;
 		}
 		if (h_mesh) {memcpy(mesh, h_mesh, n*sizeof(float));}
+		pass.complete();
 		return TW_OK;
 	};
 	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
@@ -1526,10 +1532,45 @@ int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job) {
 			r = twi_gen_mesh_zbottom(ctx, d_rec); if (r) return r;
 		}
 		if (erode) {r = twi_erode_dev_enqueue(ctx, ctx->d_scratch[1], d_mesh, MX, MY, iters, &ep, d_rec); if (r) return r;}
+		r = pass.enqueue(ctx, d_mesh, d_rec); if (r) return r; // calc_mesh_shadows per light on the final mesh, with the record's zmin / zmax
 		if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(locked ? mesh : h_mesh, d_mesh, n*sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));}
 		TW_CUDA(ctx, cudaMemcpyAsync(h_rec, d_rec, sizeof(twi_gen_mesh_rec), cudaMemcpyDeviceToHost, ctx->stream));
 		return TW_OK;
 	});
+}
+
+int tw_gen_mesh_launch(tw_ctx *ctx, const tw_gen_mesh_job *job) {return tw_gen_mesh_launch_shadows(ctx, job, 0, nullptr);}
+
+// calc_mesh_shadows over one whole mesh for every light of the job, as the context's pending job (twi_mesh_pass). Scratch slot 0: [mesh (unless on the device)
+// | the pass's]; pinned staging: [host mesh | the pass's].
+int tw_mesh_shadows_launch(tw_ctx *ctx, const tw_mesh_shadows_job *job) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!job || !job->mesh) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+	twi_mesh_pass pass;
+	rc = pass.make(ctx, job->xsize, job->ysize, job->nlights, job->lights); if (rc) return rc;
+	twi_user<const float> z(job->mesh, (size_t)job->xsize*job->ysize);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {z.take(c); pass.carve_dev(c);}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {z.take_pinned(c); pass.carve_pin(c);}); if (rc) return rc;
+	twi_job pending;
+	pending.cancellable = true;
+	pending.complete = [pass](tw_ctx *) -> int {pass.complete(); return TW_OK;};
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
+		int r = z.in(ctx); if (r) return r;
+		return pass.enqueue(ctx, z.d, nullptr);
+	});
+}
+
+int tw_mesh_shadows(tw_ctx *ctx, const float *mesh, int xsize, int ysize, const tw_shadow_params *sp, const float *sh_in_x, const float *sh_in_y, uint8_t *smask,
+                    float *sh_out_x, float *sh_out_y)
+{
+	if (!ctx) return TW_ERR_ARG;
+	if (!sp) return tw_set_error(ctx, TW_ERR_ARG, "null argument");
+	tw_tile_light L;
+	L.sp = *sp; L.sh_in_x = sh_in_x; L.sh_in_y = sh_in_y; L.smask = smask; L.sh_out_x = sh_out_x; L.sh_out_y = sh_out_y;
+	tw_mesh_shadows_job const job = {mesh, xsize, ysize, 1, &L};
+	int const rc = tw_mesh_shadows_launch(ctx, &job);
+	if (rc) return rc;
+	return poll_job(ctx, 1);
 }
 
 int tw_minmax_f32(tw_ctx *ctx, const float *vals, size_t n, tw_minmax *mm) {

@@ -295,11 +295,45 @@ struct twi_shadow_plan {
 	twi_shadow_dev S;
 	bool trace = false, all_shadowed = false;
 };
+// S from sp: scene sizes, clip z range, and the light direction, ray length, dim and dir_ratio (mesh_shadow_gen::run, :492-496) on the host with the
+// reference's operations; returns whether rays are traced at all (not no_shadow, lpos.xy != 0)
+bool   twi_shadow_light(const tw_shadow_params *sp, twi_shadow_dev *S);
 bool   twi_shadow_plan_make(const int32_t *tile_xy, uint32_t ntiles, const tw_shadow_params *sp, bool has_in_x, bool has_in_y, twi_shadow_plan *P);
 size_t twi_shadow_plan_ints(uint32_t ntiles);
 void   twi_shadow_plan_pack(const twi_shadow_plan &P, int *out); // [wave_tiles | nbx | nby]
 int    twi_shadow_enqueue(tw_ctx *ctx, cudaStream_t st, const twi_shadow_plan &P, const float *d_z, uint32_t ntiles, uint32_t n, unsigned char *d_m,
                           unsigned long long *d_keys, float *d_ox, float *d_oy, const int *d_plan, bool use_graph);
+struct twi_gen_mesh_rec;
+// Mesh shadows of one whole xsize x ysize mesh for nlights lights (tw_mesh_shadows_launch, tw_gen_mesh_launch_shadows; tw_shadows.cu), all lights in one
+// launch of each kernel. Each light has a device record: its twi_shadow_dev, whose zmin / zmax are the data-dependent part (the caller's, or written on the
+// device from a gen_mesh record), and where its mask, keys, edges and incoming rows are. all_shadowed is decided on the device from that zmin.
+struct twi_mesh_light {
+	twi_shadow_dev S;
+	float lz; int no_shadow, trace;                 // lpos.z and no_shadow (all_shadowed), and twi_shadow_light's result
+	unsigned char *smask;                           // xsize*ysize bytes, 4-byte aligned
+	const float *in_x, *in_y;                       // incoming rows (xsize / ysize floats) or nullptr
+	unsigned long long *keys; float *out;           // [x edge (xsize) | y edge (ysize)]: 64-bit last-writer keys, then the unpacked sh_out
+};
+// A pass is made on the host (make: TW_ERR_ARG for a light without smask or a misaligned device smask; nothing reserved or enqueued), then its device regions
+// (slot 0) and pinned regions are carved into the caller's layouts, enqueue runs it on ctx->stream over d_mesh (d_rec: zmin / zmax from that record), and the
+// completing poll calls complete, which copies the outputs staged for pageable host memory.
+struct twi_mesh_pass {
+	struct slot {
+		tw_tile_light L;
+		int km = 0, ki[2] = {0, 0}, ko[2] = {0, 0};          // where smask, sh_in_x / _y and sh_out_x / _y are (tw_shadows.cu's mem_kind)
+		unsigned char *d_m = nullptr, *h_m = nullptr;       // the mask on the device (the caller's, or scratch); pinned staging for a pageable mask
+		const float *d_in[2] = {nullptr, nullptr}; float *h_in[2] = {nullptr, nullptr}; // incoming rows on the device; pinned bounce of host rows
+		unsigned long long *d_k = nullptr; float *d_o = nullptr, *h_o = nullptr; // keys and edges on the device; pinned staging for pageable sh_out
+	};
+	int xsize = 0, ysize = 0;
+	std::vector<slot> s;
+	twi_mesh_light *d_tab = nullptr, *h_tab = nullptr;
+	int  make(tw_ctx *ctx, int xsize, int ysize, uint32_t nlights, const tw_tile_light *lights);
+	void carve_dev(twi_carve &c);   // [per light: mask (unless the caller's is device memory) | keys | edges | incoming rows from host] [records]
+	void carve_pin(twi_carve &c);   // [per light: incoming rows from host | pageable mask | pageable edges] [records]
+	int  enqueue(tw_ctx *ctx, const float *d_mesh, const twi_gen_mesh_rec *d_rec);
+	void complete() const;
+};
 // Work a caller adds to the end of the asynchronous tile job (tw_tile_set_create_tiles_launch: the tile set's put and relight). The job validates its
 // arguments, then calls prepare (nothing of the job is enqueued yet), reserves dev_bytes of slot-0 scratch and pin_bytes of pinned staging for the tail
 // together with its own (before the erosion budget is taken), and after the chunk join calls enqueue on ctx->stream with the job's caller-order zvals, the

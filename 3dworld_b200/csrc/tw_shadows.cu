@@ -112,6 +112,81 @@ __global__ void shadow_unpack_kernel(const unsigned long long *__restrict__ kx, 
 	oy[o] = b ? __uint_as_float((unsigned)b) : TW_MESH_MIN_Z;
 }
 
+// Mesh shadows of one whole xsize x ysize mesh (twi_mesh_pass): light = blockIdx.y, its record L[blockIdx.y]. Cell indices are 64-bit, so a mesh of more than
+// 2^31 cells is addressed correctly. The mask starts as calc_mesh_shadows sets it (:505-510): MESH_SHADOW everywhere when the light is below the record's zmin.
+__global__ void mesh_shadow_init_kernel(const twi_mesh_light *__restrict__ L, size_t ncells, int nedge) {
+	twi_mesh_light const &l = L[blockIdx.y];
+	unsigned const val = (!l.no_shadow && l.lz < l.S.zmin) ? TW_MESH_SHADOW*0x01010101u : 0u;
+	size_t const i = (size_t)blockIdx.x*blockDim.x + threadIdx.x, stride = (size_t)gridDim.x*blockDim.x;
+	for (size_t k = i; k < (ncells >> 2); k += stride) {((unsigned *)l.smask)[k] = val;} // the mask is 4-byte aligned
+	for (size_t k = (ncells & ~(size_t)3) + i; k < ncells; k += stride) {l.smask[k] = (unsigned char)val;}
+	for (size_t k = i; k < (size_t)nedge; k += stride) {l.keys[k] = 0ull;}
+}
+// one thread per ray: 2*ysize rays from the x edge (ray = y), then 2*xsize from the y edge (ray = 2*ysize + x), as shadow_rays_kernel for one tile of
+// xsize x ysize cells. In a cancelled job (tw_cancel) a block returns at entry.
+__global__ void mesh_shadow_rays_kernel(const float *__restrict__ mh, int xsize, int ysize, const twi_mesh_light *__restrict__ L, twi_job_words *jw) {
+	if (twi_cancelled(jw)) {if (threadIdx.x == 0) {twi_mark_stopped(jw);} return;}
+	twi_mesh_light const &l = L[blockIdx.y];
+	int const ray = blockIdx.x*blockDim.x + threadIdx.x;
+	if (!l.trace || ray >= 2*(xsize + ysize)) return;
+	ShadowDev const S = l.S;
+	const float *sh_in_x = l.in_x, *sh_in_y = l.in_y;
+	unsigned char *smask = l.smask;
+	unsigned long long *out_x = l.keys, *out_y = l.keys + xsize;
+	Pt v1;
+	if (ray < 2*ysize) {v1.x = -S.xs + S.dx*(float)((S.dirx > 0.0f) ? 0 : xsize); v1.y = (float)((double)(-S.ys) + 0.5*(double)S.dy*(double)ray); v1.z = 0.0f;}       // run_x, :478-481
+	else {int const x = ray - 2*ysize; v1.x = (float)((double)(-S.xs) + 0.5*(double)S.dx*(double)x); v1.y = -S.ys + S.dy*(float)((S.diry > 0.0f) ? 0 : ysize); v1.z = 0.0f;} // run_y, :482-485
+	Pt v2 = {v1.x + S.dirx*S.dist, v1.y + S.diry*S.dist, v1.z + 0.0f};
+	float const d[3][2] = {{-S.xs, -S.xs + S.dx*(float)xsize}, {-S.ys, -S.ys + S.dy*(float)ysize}, {S.zmin, S.zmax}};
+	if (!line_clip(v1, v2, d)) return;
+	int const xa = to_pos(v1.x, S.xs, S.dxi), ya = to_pos(v1.y, S.ys, S.dyi), xb = to_pos(v2.x, S.xs, S.dxi), yb = to_pos(v2.y, S.ys, S.dyi), ddx = xb - xa, ddy = yb - ya;
+	bool inited = false;
+	Pt cur = {0.0f, 0.0f, 0.0f};
+	int x = xa, y = ya, dx1 = 0, dy1 = 0, dx2 = 0, dy2 = 0; // Bresenham, :429-440
+	if (ddx < 0) {dx1 = -1; dx2 = -1;} else if (ddx > 0) {dx1 = 1; dx2 = 1;}
+	if (ddy < 0) {dy1 = -1;} else if (ddy > 0) {dy1 = 1;}
+	int longest = abs(ddx), shortest = abs(ddy);
+	if (longest <= shortest) {
+		int const t = longest; longest = shortest; shortest = t;
+		if (ddy < 0) {dy2 = -1;} else if (ddy > 0) {dy2 = 1;}
+		dx2 = 0;
+	}
+	int numerator = longest >> 1;
+	unsigned long long const seq = (unsigned long long)(ray + 1) << 32;
+	for (int i = 0; i <= longest; i++) {
+		if (x >= 0 && y >= 0 && x < xsize && y < ysize) {
+			size_t const c = (size_t)y*xsize + x;
+			Pt const pt = {-S.xs + S.dx*(float)x, -S.ys + S.dy*(float)y, __ldg(mh + c)};
+			if (sh_in_y != nullptr && x == xa && sh_in_y[y] > TW_MESH_MIN_Z) {cur.x = pt.x; cur.y = pt.y; cur.z = sh_in_y[y]; inited = true;}      // starting shadow height
+			else if (sh_in_x != nullptr && y == ya && sh_in_x[x] > TW_MESH_MIN_Z) {cur.x = pt.x; cur.y = pt.y; cur.z = sh_in_x[x]; inited = true;}
+			float const shadow_z = (float)((double)((S.dim ? pt.y : pt.x) - (S.dim ? cur.y : cur.x))*S.dir_ratio + (double)cur.z);
+			if (inited && shadow_z > pt.z) { // shadowed
+				atomicOr((unsigned *)(smask + (c & ~(size_t)3)), (unsigned)TW_MESH_SHADOW << ((unsigned)(c & 3)*8u));
+				if (x == xb) {atomicMax(out_y + y, seq | __float_as_uint(shadow_z));}
+				if (y == yb) {atomicMax(out_x + x, seq | __float_as_uint(shadow_z));}
+			}
+			else {cur = pt;}
+			inited = true;
+		}
+		numerator += shortest;
+		if (numerator >= longest) {numerator -= longest; x += dx1; y += dy1;} else {x += dx2; y += dy2;}
+	}
+}
+__global__ void mesh_shadow_unpack_kernel(const twi_mesh_light *__restrict__ L, int nedge) {
+	int const i = blockIdx.x*blockDim.x + threadIdx.x;
+	if (i >= nedge) return;
+	twi_mesh_light const &l = L[blockIdx.y];
+	unsigned long long const a = l.keys[i];
+	l.out[i] = a ? __uint_as_float((unsigned)a) : TW_MESH_MIN_Z;
+}
+// the clip z range of every light from a gen_mesh record (tw_gen_mesh_launch_shadows): the zmin / zmax that gen_mesh leaves, known only on the device
+__global__ void mesh_shadow_zrange_kernel(twi_mesh_light *L, unsigned nlights, const twi_gen_mesh_rec *rec) {
+	for (unsigned l = 0; l < nlights; ++l) {L[l].S.zmin = rec->zmin; L[l].S.zmax = rec->zmax;}
+}
+
+enum {MEM_NONE, MEM_DEV, MEM_LOCKED, MEM_PAGEABLE};
+int mem_kind(const void *p) {return !p ? MEM_NONE : tw_is_device_ptr(p) ? MEM_DEV : twi_is_page_locked(p) ? MEM_LOCKED : MEM_PAGEABLE;}
+
 } // namespace
 
 bool twi_shadow_plan_make(const int32_t *tile_xy, uint32_t ntiles, const tw_shadow_params *sp, bool has_in_x, bool has_in_y, twi_shadow_plan *P) {
@@ -152,24 +227,26 @@ bool twi_shadow_plan_make(const int32_t *tile_xy, uint32_t ntiles, const tw_shad
 	std::vector<int> fill(P->wave_start.begin(), P->wave_start.end() - 1);
 	for (uint32_t t = 0; t < ntiles; ++t) {P->wave_tiles[fill[level[t]]++] = (int)t;}
 	// light direction and ray length (mesh_shadow_gen::run, :492-496), on the host with the reference's operations
-	ShadowDev &S = P->S;
-	memset(&S, 0, sizeof(S));
-	S.xs = sp->x_scene_size; S.ys = sp->y_scene_size; S.dx = sp->dx_val; S.dy = sp->dy_val; S.dxi = sp->dx_val_inv; S.dyi = sp->dy_val_inv; S.zmin = sp->zmin; S.zmax = sp->zmax;
 	P->all_shadowed = (!sp->no_shadow && sp->lpos[2] < sp->zmin);
-	P->trace = !(sp->no_shadow || (sp->lpos[0] == 0.0f && sp->lpos[1] == 0.0f));
-	if (P->trace) {
-		volatile float m2 = sp->lpos[0]*sp->lpos[0]; volatile float m2b = sp->lpos[1]*sp->lpos[1]; volatile float m2c = sp->lpos[2]*sp->lpos[2];
-		volatile float ms = m2 + m2b; ms = ms + m2c;
-		float const vmag = sqrtf(ms);
-		float nx = sp->lpos[0], ny = sp->lpos[1], nz = sp->lpos[2];
-		if (!(vmag < 1.0E-12f)) {nx = sp->lpos[0]/vmag; ny = sp->lpos[1]/vmag; nz = sp->lpos[2]/vmag;} // get_norm
-		S.dirx = -nx; S.diry = -ny; S.dirz = -nz;
-		volatile float q1 = S.dirx*S.dirx; volatile float q2 = S.diry*S.diry; volatile float q = q1 + q2;
-		S.dist = (float)(2.0*sp->xy_sum_size/sqrtf(q));
-		S.dim = (fabsf(S.dirx) < fabsf(S.diry)) ? 1 : 0;
-		S.dir_ratio = (double)(S.dirz/(S.dim ? S.diry : S.dirx));
-	}
+	P->trace = twi_shadow_light(sp, &P->S);
 	return unique;
+}
+
+bool twi_shadow_light(const tw_shadow_params *sp, ShadowDev *S) {
+	memset(S, 0, sizeof(*S));
+	S->xs = sp->x_scene_size; S->ys = sp->y_scene_size; S->dx = sp->dx_val; S->dy = sp->dy_val; S->dxi = sp->dx_val_inv; S->dyi = sp->dy_val_inv; S->zmin = sp->zmin; S->zmax = sp->zmax;
+	if (sp->no_shadow || (sp->lpos[0] == 0.0f && sp->lpos[1] == 0.0f)) return false;
+	volatile float m2 = sp->lpos[0]*sp->lpos[0]; volatile float m2b = sp->lpos[1]*sp->lpos[1]; volatile float m2c = sp->lpos[2]*sp->lpos[2];
+	volatile float ms = m2 + m2b; ms = ms + m2c;
+	float const vmag = sqrtf(ms);
+	float nx = sp->lpos[0], ny = sp->lpos[1], nz = sp->lpos[2];
+	if (!(vmag < 1.0E-12f)) {nx = sp->lpos[0]/vmag; ny = sp->lpos[1]/vmag; nz = sp->lpos[2]/vmag;} // get_norm
+	S->dirx = -nx; S->diry = -ny; S->dirz = -nz;
+	volatile float q1 = S->dirx*S->dirx; volatile float q2 = S->diry*S->diry; volatile float q = q1 + q2;
+	S->dist = (float)(2.0*sp->xy_sum_size/sqrtf(q));
+	S->dim = (fabsf(S->dirx) < fabsf(S->diry)) ? 1 : 0;
+	S->dir_ratio = (double)(S->dirz/(S->dim ? S->diry : S->dirx));
+	return true;
 }
 
 size_t twi_shadow_plan_ints(uint32_t ntiles) {return (size_t)3*ntiles;}
@@ -266,4 +343,95 @@ extern "C" int tw_tile_shadows_batch_ex(tw_ctx *ctx, const float *zvals, const i
                                         const float *sh_in_x, const float *sh_in_y, uint8_t *smask, float *sh_out_x, float *sh_out_y)
 {
 	return tile_shadows(ctx, zvals, tile_xy, ntiles, zvsize, sp, sh_in_x, sh_in_y, smask, sh_out_x, sh_out_y, true);
+}
+
+// ---- mesh shadows of one whole mesh (twi_mesh_pass, tw_internal.h) ----
+int twi_mesh_pass::make(tw_ctx *ctx, int xs, int ys, uint32_t nlights, const tw_tile_light *lights) {
+	if (xs < 2 || ys < 2 || (long long)xs + ys >= (1ll << 30)) return tw_set_error(ctx, TW_ERR_ARG, "mesh shadows: mesh size %d x %d", xs, ys); // 2*(xs + ys) ray numbers fit an int
+	if (nlights == 0 || !lights) return tw_set_error(ctx, TW_ERR_ARG, "mesh shadows: no lights");
+	xsize = xs; ysize = ys;
+	s.assign(nlights, slot());
+	for (uint32_t l = 0; l < nlights; ++l) {
+		slot &q = s[l];
+		q.L = lights[l];
+		if (!q.L.smask) return tw_set_error(ctx, TW_ERR_ARG, "mesh shadows: light %u has no smask", l);
+		q.km = mem_kind(q.L.smask);
+		if (q.km == MEM_DEV && ((size_t)q.L.smask & 3)) return tw_set_error(ctx, TW_ERR_ARG, "smask must be 4-byte aligned (flag bytes are set with 32-bit atomics)");
+		q.ki[0] = mem_kind(q.L.sh_in_x); q.ki[1] = mem_kind(q.L.sh_in_y); q.ko[0] = mem_kind(q.L.sh_out_x); q.ko[1] = mem_kind(q.L.sh_out_y);
+	}
+	return TW_OK;
+}
+
+void twi_mesh_pass::carve_dev(twi_carve &c) {
+	if (s.empty()) return;
+	size_t const cells = (size_t)xsize*ysize, ne = (size_t)xsize + ysize;
+	for (slot &q : s) {
+		q.d_m = (q.km == MEM_DEV) ? q.L.smask : c.take<unsigned char>(cells);
+		q.d_k = c.take<unsigned long long>(ne); q.d_o = c.take<float>(ne);
+		const float *in[2] = {q.L.sh_in_x, q.L.sh_in_y};
+		for (int e = 0; e < 2; ++e) {q.d_in[e] = (q.ki[e] == MEM_NONE || q.ki[e] == MEM_DEV) ? in[e] : c.take<float>(e ? ysize : xsize);}
+	}
+	d_tab = c.take<twi_mesh_light>(s.size());
+}
+
+void twi_mesh_pass::carve_pin(twi_carve &c) {
+	if (s.empty()) return;
+	size_t const cells = (size_t)xsize*ysize, ne = (size_t)xsize + ysize;
+	for (slot &q : s) {
+		for (int e = 0; e < 2; ++e) {q.h_in[e] = (q.ki[e] == MEM_NONE || q.ki[e] == MEM_DEV) ? nullptr : c.take<float>(e ? ysize : xsize);} // host rows are copied during the launch
+		q.h_m = (q.km == MEM_PAGEABLE) ? c.take<unsigned char>(cells) : nullptr;
+		q.h_o = (q.ko[0] == MEM_PAGEABLE || q.ko[1] == MEM_PAGEABLE) ? c.take<float>(ne) : nullptr;
+	}
+	h_tab = c.take<twi_mesh_light>(s.size());
+}
+
+int twi_mesh_pass::enqueue(tw_ctx *ctx, const float *d_mesh, const twi_gen_mesh_rec *d_rec) {
+	if (s.empty()) return TW_OK;
+	unsigned const nl = (unsigned)s.size();
+	size_t const cells = (size_t)xsize*ysize, ne = (size_t)xsize + ysize;
+	for (unsigned l = 0; l < nl; ++l) {
+		slot const &q = s[l];
+		twi_mesh_light &R = h_tab[l];
+		memset(&R, 0, sizeof(R));
+		R.trace = twi_shadow_light(&q.L.sp, &R.S) ? 1 : 0;
+		R.lz = q.L.sp.lpos[2]; R.no_shadow = q.L.sp.no_shadow;
+		R.smask = q.d_m; R.in_x = q.d_in[0]; R.in_y = q.d_in[1]; R.keys = q.d_k; R.out = q.d_o;
+		const float *in[2] = {q.L.sh_in_x, q.L.sh_in_y};
+		for (int e = 0; e < 2; ++e) {
+			if (!q.h_in[e]) continue;
+			size_t const bytes = (e ? ysize : xsize)*sizeof(float);
+			memcpy(q.h_in[e], in[e], bytes);
+			TW_CUDA(ctx, cudaMemcpyAsync((void *)q.d_in[e], q.h_in[e], bytes, cudaMemcpyHostToDevice, ctx->stream));
+		}
+	}
+	TW_CUDA(ctx, cudaMemcpyAsync(d_tab, h_tab, nl*sizeof(twi_mesh_light), cudaMemcpyHostToDevice, ctx->stream));
+	if (d_rec) {mesh_shadow_zrange_kernel<<<1, 1, 0, ctx->stream>>>(d_tab, nl, d_rec); TW_LAUNCH_CHECK(ctx);}
+	unsigned const YMAX = 65535; // more lights than gridDim.y takes run in pieces
+	for (unsigned l0 = 0; l0 < nl; l0 += YMAX) {
+		unsigned const m = std::min(YMAX, nl - l0);
+		mesh_shadow_init_kernel<<<dim3(ctx->num_sms*4, m), 256, 0, ctx->stream>>>(d_tab + l0, cells, (int)ne);
+		TW_LAUNCH_CHECK(ctx);
+		mesh_shadow_rays_kernel<<<dim3((unsigned)((2*ne + 127)/128), m), 128, 0, ctx->stream>>>(d_mesh, xsize, ysize, d_tab + l0, ctx->d_job_words);
+		TW_LAUNCH_CHECK(ctx);
+		mesh_shadow_unpack_kernel<<<dim3((unsigned)((ne + 255)/256), m), 256, 0, ctx->stream>>>(d_tab + l0, (int)ne);
+		TW_LAUNCH_CHECK(ctx);
+	}
+	for (slot const &q : s) {
+		if (q.km != MEM_DEV) {TW_CUDA(ctx, cudaMemcpyAsync(q.h_m ? (void *)q.h_m : (void *)q.L.smask, q.d_m, cells, cudaMemcpyDeviceToHost, ctx->stream));}
+		float *out[2] = {q.L.sh_out_x, q.L.sh_out_y};
+		for (int e = 0; e < 2; ++e) {
+			if (!out[e]) continue;
+			size_t const off = e ? xsize : 0;
+			TW_CUDA(ctx, cudaMemcpyAsync(q.ko[e] == MEM_PAGEABLE ? q.h_o + off : out[e], q.d_o + off, (e ? ysize : xsize)*sizeof(float), cudaMemcpyDefault, ctx->stream));
+		}
+	}
+	return TW_OK;
+}
+
+void twi_mesh_pass::complete() const {
+	for (slot const &q : s) {
+		if (q.h_m) {memcpy(q.L.smask, q.h_m, (size_t)xsize*ysize);}
+		float *out[2] = {q.L.sh_out_x, q.L.sh_out_y};
+		for (int e = 0; e < 2; ++e) {if (q.ko[e] == MEM_PAGEABLE) memcpy(out[e], q.h_o + (e ? xsize : 0), (e ? ysize : xsize)*sizeof(float));}
+	}
 }

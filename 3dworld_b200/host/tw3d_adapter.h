@@ -12,6 +12,7 @@
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //   tw3d::update_heightmap, tw3d::hmap_tiles_touched  <->  terrain_hmap_manager_t's brush edits and re-applied modmap, and the tiles they change   src/heightmap.cpp:36-58,243-308
 //   tw3d::gen_mesh_async         <->  gen_mesh in ground mode at start-up and on every regeneration, without stalling the frame   src/mesh_gen.cpp:257-355
+//   tw3d::calc_mesh_shadows(lpos, mh, smask, xsize, ysize, ...), tw3d::mesh_shadows_async  <->  calc_mesh_shadows on the ground-mode mesh   src/visibility.cpp:411-517
 //   tw3d::get_exact_zvals_async, tw3d::heightmap_heights_async  <->  get_exact_zval / get_clamped_height per placed object, without stalling the frame   src/mesh_gen.cpp:816-847, src/heightmap.cpp:385-402
 //   tw3d::set_deferred_gens, tw3d::tile_job_pool  <->  several of them in flight at once, as tile_draw_t::update keeps up to 8   src/tiled_mesh.cpp:2367-2417
 //   tw3d::tile_set               <->  the live tiles' calc_shadows_for_light when the light moves or new tiles appear   src/tiled_mesh.cpp:664-692
@@ -646,6 +647,11 @@ public:
 	// gen_mesh_async (below) on a slot, beside the frames in flight on the others
 	tiles_job gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters, int xoff2 = 0, int yoff2 = 0,
 	                         float dx_val = 0.0f, float dy_val = 0.0f, float water_h_off = 0.0f, float water_h_off_rel = 0.0f, gen_mesh_result *result = nullptr);
+	tiles_job gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters, std::vector<tw_tile_light> const &lights,
+	                         int xoff2 = 0, int yoff2 = 0, float dx_val = 0.0f, float dy_val = 0.0f, float water_h_off = 0.0f, float water_h_off_rel = 0.0f,
+	                         gen_mesh_result *result = nullptr);
+	// mesh_shadows_async (below) on a slot
+	tiles_job mesh_shadows_async(const float *mh, int xsize, int ysize, std::vector<tw_tile_light> const &lights);
 	// object placement (get_exact_zvals_async / heightmap_heights_async above) on a slot, beside the frames in flight on the others
 	tiles_job get_exact_zvals_async(const float *xy, size_t n, float *zvals_out, bool no_xyoff = false) {
 		slot &s = next();
@@ -712,6 +718,41 @@ inline void calc_mesh_shadows(const float lpos[3], const float *zvals, const int
 	tw_ctx *c = ctx();
 	int const rc = tw_tile_shadows_batch_ex(c, zvals, tile_xy, ntiles, zvsize, &sp, sh_in_x, sh_in_y, smask, sh_out_x, sh_out_y);
 	if (rc != TW_OK) {detail::fail(rc, "calc_mesh_shadows", c);}
+}
+
+// calc_mesh_shadows(l, lpos, mh, smask, xsize, ysize, sh_in_x, sh_in_y, sh_out_x, sh_out_y) itself on one whole mesh (tw_mesh_shadows), in the reference's
+// argument order: ground mode's calc_visibility (src/visibility.cpp:411-517) calls it with mesh_height, shadow_mask[l], MESH_X_SIZE, MESH_Y_SIZE and no
+// incoming or outgoing heights, for each light. smask = xsize*ysize bytes; sh_in_* / sh_out_* optional (xsize resp. ysize floats). Globals read: those of
+// mesh_shadow_params.
+inline tw_shadow_params mesh_shadow_params(const float lpos[3], bool no_shadow = false) { // shadow_params with DX_VAL = 1/DX_VAL_INV, DY_VAL = 1/DY_VAL_INV
+	scene_globals const &g = globals();
+	return shadow_params(lpos, 1.0f/g.DX_VAL_INV, 1.0f/g.DY_VAL_INV, no_shadow);
+}
+inline void calc_mesh_shadows(const float lpos[3], const float *mh, unsigned char *smask, int xsize, int ysize, const float *sh_in_x = nullptr, const float *sh_in_y = nullptr,
+                              float *sh_out_x = nullptr, float *sh_out_y = nullptr, bool no_shadow = false) {
+	tw_shadow_params const sp = mesh_shadow_params(lpos, no_shadow);
+	tw_ctx *c = ctx();
+	int const rc = tw_mesh_shadows(c, mh, xsize, ysize, &sp, sh_in_x, sh_in_y, smask, sh_out_x, sh_out_y);
+	if (rc != TW_OK) {detail::fail(rc, "calc_mesh_shadows", c);}
+}
+// The same for several lights over one mesh as a job that does not stall the frame (tw_mesh_shadows_launch): the relight when the sun or moon moves. Each
+// light is a tw_tile_light sized for the mesh (sp from mesh_shadow_params); its outputs hold calc_mesh_shadows' results once the tiles_job is ready. mh and
+// the outputs must stay valid until then (a host mh is copied during the call). tile_job_pool::mesh_shadows_async runs it on a pool slot.
+namespace detail {
+	inline tiles_job launch_mesh_shadows(tw_ctx *c, std::atomic<uint64_t> &jobs, const float *mh, int xsize, int ysize, std::vector<tw_tile_light> const &lights) {
+		tw_mesh_shadows_job const job = {mh, xsize, ysize, (uint32_t)lights.size(), lights.data()};
+		uint64_t const number = ++jobs;
+		int const rc = tw_mesh_shadows_launch(c, &job);
+		if (rc != TW_OK) {--jobs; fail(rc, "mesh_shadows_async", c);}
+		return tiles_job(c, &jobs, number);
+	}
+}
+inline tiles_job mesh_shadows_async(const float *mh, int xsize, int ysize, std::vector<tw_tile_light> const &lights) {
+	return detail::launch_mesh_shadows(ctx(), detail::tls().tile_jobs, mh, xsize, ysize, lights);
+}
+inline tiles_job tile_job_pool::mesh_shadows_async(const float *mh, int xsize, int ysize, std::vector<tw_tile_light> const &lights) {
+	slot &s = next();
+	return detail::launch_mesh_shadows(s.c, s.jobs, mh, xsize, ysize, lights);
 }
 
 // The live tiles of tile_draw_t on the device (tw_tile_set, include/tw3d.h), for the two relights of calc_shadows_for_light the engine otherwise does itself
@@ -881,6 +922,8 @@ inline gen_mesh_result gen_mesh(float *mesh_height /* MESH_Y_SIZE x MESH_X_SIZE,
 // tw_last_erosion_steps() of the job's context are gen_mesh's, bit for bit, and the derived globals (zmax_est, zmin, zmax, water_plane_z, zbottom, ztop) have
 // been written into scene_globals as gen_mesh writes them; a cancelled job writes neither. mesh_height (MESH_Y_SIZE x MESH_X_SIZE) is device, page-locked or
 // pageable host memory (the last is filled when the job is ready) and must stay valid until then. tile_job_pool::gen_mesh_async runs it on a pool slot.
+// The overloads with lights also trace each light's calc_mesh_shadows over the final mesh in the same job (tw_gen_mesh_launch_shadows): lights are sized as
+// for mesh_shadows_async, and each sp's zmin / zmax are replaced by the ones the job leaves - what calc_visibility reads after gen_mesh.
 namespace detail {
 	inline void gen_mesh_tables(tw_rng &sine_rng, float x_scene_size, float y_scene_size) { // gen_mesh's sine table, set as the thread's tables
 		scene_globals const g = globals();
@@ -890,7 +933,8 @@ namespace detail {
 		set_globals(g, nullptr, sinTable.data());
 	}
 	inline tiles_job launch_gen_mesh(tw_ctx *c, std::atomic<uint64_t> &jobs, float *mesh_height, float x_scene_size, float y_scene_size, unsigned erosion_iters,
-	                                 int xoff2, int yoff2, float dx_val, float dy_val, float water_h_off, float water_h_off_rel, gen_mesh_result *result) {
+	                                 int xoff2, int yoff2, float dx_val, float dy_val, float water_h_off, float water_h_off_rel, gen_mesh_result *result,
+	                                 std::vector<tw_tile_light> const &lights = {}) {
 		scene_globals const g = globals();
 		if (dx_val == 0.0f) {dx_val = 1.0f/g.DX_VAL_INV;}
 		if (dy_val == 0.0f) {dy_val = 1.0f/g.DY_VAL_INV;}
@@ -900,7 +944,7 @@ namespace detail {
 		tw_gen_mesh_job const job = {g.MESH_X_SIZE, g.MESH_Y_SIZE, xoff2, yoff2, dx_val, dy_val, x_scene_size, y_scene_size, &p, erosion_iters, &e,
 		                             water_h_off, water_h_off_rel, g.zbottom, g.ztop, g.water_plane_z, mesh_height, info.get()};
 		uint64_t const number = ++jobs;
-		int const rc = tw_gen_mesh_launch(c, &job);
+		int const rc = tw_gen_mesh_launch_shadows(c, &job, (uint32_t)lights.size(), lights.empty() ? nullptr : lights.data());
 		if (rc != TW_OK) {--jobs; fail(rc, "gen_mesh_async", c);}
 		return tiles_job(c, &jobs, number, [info, result]() {
 			scene_globals g = globals();
@@ -921,6 +965,21 @@ inline tiles_job tile_job_pool::gen_mesh_async(float *mesh_height, tw_rng &sine_
 	detail::gen_mesh_tables(sine_rng, x_scene_size, y_scene_size); // before the slot is picked: the slots' jobs complete before the new tables go up
 	slot &s = next();
 	return detail::launch_gen_mesh(s.c, s.jobs, mesh_height, x_scene_size, y_scene_size, erosion_iters, xoff2, yoff2, dx_val, dy_val, water_h_off, water_h_off_rel, result);
+}
+inline tiles_job gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters, std::vector<tw_tile_light> const &lights,
+                                int xoff2 = 0, int yoff2 = 0, float dx_val = 0.0f, float dy_val = 0.0f, float water_h_off = 0.0f, float water_h_off_rel = 0.0f,
+                                gen_mesh_result *result = nullptr) {
+	detail::gen_mesh_tables(sine_rng, x_scene_size, y_scene_size);
+	return detail::launch_gen_mesh(ctx(), detail::tls().tile_jobs, mesh_height, x_scene_size, y_scene_size, erosion_iters, xoff2, yoff2, dx_val, dy_val,
+	                               water_h_off, water_h_off_rel, result, lights);
+}
+inline tiles_job tile_job_pool::gen_mesh_async(float *mesh_height, tw_rng &sine_rng, float x_scene_size, float y_scene_size, unsigned erosion_iters,
+                                               std::vector<tw_tile_light> const &lights, int xoff2, int yoff2, float dx_val, float dy_val, float water_h_off,
+                                               float water_h_off_rel, gen_mesh_result *result) {
+	detail::gen_mesh_tables(sine_rng, x_scene_size, y_scene_size);
+	slot &s = next();
+	return detail::launch_gen_mesh(s.c, s.jobs, mesh_height, x_scene_size, y_scene_size, erosion_iters, xoff2, yoff2, dx_val, dy_val, water_h_off, water_h_off_rel,
+	                               result, lights);
 }
 
 // tail of tile_t::create_zvals for a batch of finished tiles (sub_zmin/sub_zmax, mzmin/mzmax, mesh_dz, radius, water bbox), src/tiled_mesh.cpp:517-541

@@ -9,7 +9,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import (ErosionParams, Grid2D, HeightParams, Rng, VoxelParams, compute_scale, gen_rx_ry, gen_sine_params, hmap_params,
+from . import (ErosionParams, Grid2D, HeightParams, Rng, ShadowParams, VoxelParams, compute_scale, gen_rx_ry, gen_sine_params, hmap_params,
                water_z_height, MGEN_SINE)
 
 f32 = np.float32
@@ -179,12 +179,29 @@ def gen_mesh(ctx, cfg, erosion_iters=0, xoff2=0, yoff2=0, sine_rng=None):
     return mesh, dict(zmin=float(zmin), zmax=float(zmax), zmax_est=float(zmax_est), zbottom=float(zbottom), ztop=float(ztop), water_plane_z=float(wpz)), sp
 
 
-def gen_mesh_async(ctx, cfg, erosion_iters=0, xoff2=0, yoff2=0, sine_rng=None, prev=(0.0, 0.0, 0.0), mesh=None):
+def gen_mesh_async(ctx, cfg, erosion_iters=0, xoff2=0, yoff2=0, sine_rng=None, prev=(0.0, 0.0, 0.0), mesh=None, lights=None):
     """gen_mesh as one asynchronous job (Context.gen_mesh_launch): the sine table is made and set here, as gen_mesh does, and everything after it runs on
     the device. prev = (zbottom, ztop, water_plane_z) before the call, which a flat mesh keeps. Returns (job, sine_params); job.poll(wait) gives (mesh[MY, MX],
-    info) once the job is complete, with gen_mesh's info for a mesh that is not flat. cfg.zmax_est is not updated: set it from info['zmax_est']."""
+    info) once the job is complete, with gen_mesh's info for a mesh that is not flat. cfg.zmax_est is not updated: set it from info['zmax_est'].
+    lights (mesh_shadow_params per light, or the records Context.mesh_shadows_launch takes) adds calc_mesh_shadows of the final mesh per light, with the
+    job's zmin / zmax: the poll then gives (mesh, info, [(smask, sh_out_x, sh_out_y) per light])."""
     sp = cfg.sine_params(rng=sine_rng)
     ctx.set_sine_params(sp)
     job = ctx.gen_mesh_launch(cfg.mesh_size[:2], cfg.height_params(), cfg.erosion_params(), erosion_iters, xoff2, yoff2, float(cfg.dx_val), float(cfg.dy_val),
-                              cfg.scene_size[:2], cfg.water_h_off, cfg.water_h_off_rel, prev, mesh)
+                              cfg.scene_size[:2], cfg.water_h_off, cfg.water_h_off_rel, prev, mesh, lights)
     return job, sp
+
+
+def mesh_shadow_params(cfg, lpos, zmin=0.0, zmax=0.0, no_shadow=False):
+    """The ShadowParams of calc_mesh_shadows on the ground-mode mesh for the light at lpos, built as the C++ adapter's shadow_params: X/Y_SCENE_SIZE,
+    DX/DY_VAL and DX/DY_VAL_INV = 1/DX_VAL (set_scene_constants), XY_SUM_SIZE = MESH_X_SIZE + MESH_Y_SIZE, the clip range zmin / zmax (what gen_mesh left:
+    info['zmin'] / info['zmax']; gen_mesh_async's lights take the job's own) and no_shadow (the moon with combined_gu)."""
+    sp = ShadowParams()
+    for d in range(3):
+        sp.lpos[d] = float(lpos[d])
+    sp.x_scene_size, sp.y_scene_size = float(cfg.scene_size[0]), float(cfg.scene_size[1])
+    sp.dx_val, sp.dy_val = float(cfg.dx_val), float(cfg.dy_val)
+    sp.dx_val_inv, sp.dy_val_inv = float(f32(1.0) / cfg.dx_val), float(f32(1.0) / cfg.dy_val)
+    sp.xy_sum_size = int(cfg.mesh_size[0]) + int(cfg.mesh_size[1])
+    sp.zmin, sp.zmax, sp.no_shadow = float(zmin), float(zmax), int(bool(no_shadow))
+    return sp

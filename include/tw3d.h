@@ -801,6 +801,51 @@ TW_API int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, c
                           float dx, float dy, uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
                           float wpz_max, uint32_t size, const tw_tile_outputs *out, const tw_tile_shading *shading, const tw_tile_shadows *shadows);
 
+/* ---- mesh shadows of the ground-mode mesh: calc_mesh_shadows (src/visibility.cpp:411-517) on one whole xsize x ysize mesh ----
+ * In ground mode the engine calls calc_mesh_shadows(l, light_pos, mesh_height, shadow_mask[l], MESH_X_SIZE, MESH_Y_SIZE) - the whole mesh, no incoming
+ * heights - for each light after every regeneration of the mesh and whenever the sun or moon moves (calc_visibility). tw_mesh_shadows is that call, for any
+ * xsize x ysize, with the optional incoming and outgoing edges of the tile path:
+ *   mesh      xsize*ysize floats (ysize rows of xsize), host or device
+ *   sh_in_x   optional, xsize floats: incoming shadow heights along the y edge; sh_in_y optional, ysize floats along the x edge (entries <= TW_MESH_MIN_Z:
+ *             no incoming height)
+ *   smask     xsize*ysize bytes = 0 / MESH_SHADOW per cell, host or device (device: 4-byte aligned)
+ *   sh_out_x  optional, xsize floats; sh_out_y optional, ysize floats: the outgoing heights, MESH_MIN_Z where no shadowed ray wrote one. As in the reference,
+ *             only a ray whose clipped end lies on a cell of that edge writes it, and where two rays write one entry the later ray of the sequential order
+ *             (2*ysize rays from the x edge by y, then 2*xsize from the y edge by x) wins.
+ * sp->zmin / zmax are the globals the line clip reads; lpos.z < zmin shadows every cell. The results equal the reference's function bit for bit (one thread per
+ * ray, the same fp32 / double steps). Cell indices are 64-bit: a mesh of more than 2^31 cells is supported. tw_mesh_shadows completes the context's pending
+ * job first and blocks until its outputs are written; it is tw_mesh_shadows_launch for one light followed by a waiting poll.
+ * Errors (TW_ERR_ARG, nothing enqueued): a NULL mesh, sp or smask, xsize < 2 or ysize < 2, xsize + ysize >= 2^30, a device smask that is not 4-byte aligned. */
+TW_API int tw_mesh_shadows(tw_ctx *ctx, const float *mesh, int xsize, int ysize, const tw_shadow_params *sp, const float *sh_in_x, const float *sh_in_y,
+                          uint8_t *smask, float *sh_out_x, float *sh_out_y);
+/* The same for nlights lights over one mesh as the context's asynchronous job (a relight when the sun or moon moves): every light's results equal its own
+ * tw_mesh_shadows call. Each light is a tw_tile_light sized for the mesh: smask xsize*ysize bytes, sh_in_x / sh_out_x xsize floats, sh_in_y / sh_out_y ysize
+ * floats. All lights run in one launch of each kernel.
+ * - tw_create_tiles_poll / tw_heightgen_2d_poll complete the job (wait = 0 returns TW_ERR_NOT_READY while it runs); every other entry point and tw_destroy
+ *   complete it first. On a shared context it runs beside the other contexts' jobs. tw_cancel stops its rays at their cancellation point (the kernel's
+ *   entry); the poll then returns TW_ERR_CANCELED and the outputs are unspecified.
+ * - The job, the lights array and HOST mesh and sh_in rows are copied during the launch; a device mesh and device sh_in rows are read until the completing
+ *   poll. Outputs in device or page-locked memory are written by the device; pageable ones are filled by the completing poll. Every buffer is reserved
+ *   before anything is enqueued, and with device or page-locked outputs the launch never waits for the device, except when the context's scratch or staging
+ *   first has to grow.
+ * - Errors (TW_ERR_ARG, nothing enqueued): those of tw_mesh_shadows for each light, and nlights == 0 or NULL lights. */
+typedef struct tw_mesh_shadows_job {
+	const float         *mesh;          /* required: xsize*ysize floats, host or device */
+	int                  xsize, ysize;  /* MESH_X_SIZE, MESH_Y_SIZE: >= 2 each */
+	uint32_t             nlights;       /* >= 1 */
+	const tw_tile_light *lights;
+} tw_mesh_shadows_job;
+TW_API int tw_mesh_shadows_launch(tw_ctx *ctx, const tw_mesh_shadows_job *job);
+/* tw_gen_mesh_launch plus one mesh shadow pass per light on the job's final mesh (after glaciation and erosion): mesh, z values and shadows, all on the device
+ * in one job. Each light's results equal tw_mesh_shadows_launch on that mesh with the light's sp, except that sp->zmin / zmax are ignored and replaced by
+ * the zmin / zmax the job leaves - those tw_gen_mesh_info reports, read on the device. Every other sp field is the caller's (xy_sum_size = mesh_x_size +
+ * mesh_y_size in the reference). The contract is that the engine's calc_visibility reads the zmin / zmax gen_mesh leaves; an engine that changes them
+ * first uses tw_mesh_shadows_launch with explicit params instead. Lights are sized for the mesh as in tw_mesh_shadows_launch and follow its buffer rules;
+ * the mesh, info and tw_last_erosion_steps() are those of tw_gen_mesh_launch, which is tw_gen_mesh_launch_shadows(ctx, job, 0, NULL). Errors (TW_ERR_ARG,
+ * nothing enqueued): those of tw_gen_mesh_launch, nlights > 0 with NULL lights, and with lights those of tw_mesh_shadows for each light (a mesh size
+ * below 2 x 2, a light without smask, a misaligned device smask). */
+TW_API int tw_gen_mesh_launch_shadows(tw_ctx *ctx, const tw_gen_mesh_job *job, uint32_t nlights, const tw_tile_light *lights);
+
 /* ---- tile sets: the live tiles kept on the device, relit with cached, chained mesh shadows ----
  * What tile_draw_t::update does for every live tile when the light moves, and for the existing tiles behind new ones (src/tiled_mesh.cpp:664-692): a tile set
  * holds the zvals of the resident tiles in device memory the set owns, keyed by their grid coordinates (x1/size, y1/size), and per light slot the mesh shadows

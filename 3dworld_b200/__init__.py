@@ -170,6 +170,11 @@ class HmapRect(C.Structure):
     _fields_ = [("x", C.c_int), ("y", C.c_int), ("w", C.c_int), ("h", C.c_int)]
 
 
+class HmapReadArgs(C.Structure):
+    """tw_hmap_read (include/tw3d.h): the rects of one tw_read_heightmap_launch and where their texels go (texel (x, y) -> dst16 + y*dst_pitch + 2*x)."""
+    _fields_ = [("rects", C.c_void_p), ("nrects", C.c_uint32), ("dst16", C.c_void_p), ("dst_pitch", C.c_size_t)]
+
+
 class HeightmapInfo(C.Structure):
     _fields_ = [("min_z", C.c_float), ("max_z", C.c_float), ("val_mult", C.c_float), ("val_add", C.c_float), ("mesh_file_scale", C.c_float),
                 ("mesh_file_tz", C.c_float), ("erosion_moves", C.c_uint64)]
@@ -237,7 +242,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
                "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
-               "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows"]
+               "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows",
+               "tw_read_heightmap_launch", "tw_read_heightmap"]
 
 
 def _load():
@@ -297,6 +303,8 @@ def _load():
     L.tw_heightmap_sample_tiles.argtypes = [vp, vp, C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp]
     L.tw_set_heightmap.argtypes = [vp, vp, C.c_int, C.c_int]
     L.tw_update_heightmap.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32]
+    L.tw_read_heightmap_launch.argtypes = [vp, C.POINTER(HmapReadArgs)]
+    L.tw_read_heightmap.argtypes = [vp, C.POINTER(HmapReadArgs)]
     L.tw_hmap_tiles_touched.argtypes = [C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_points_launch.argtypes = [vp, C.POINTER(PointsJobArgs)]
@@ -629,6 +637,11 @@ class PointsJob:
         return self.out if self._ctx.create_tiles_poll(wait) else None
 
 
+class HmapReadJob(PointsJob):
+    """What Context.read_heightmap_launch returns: poll(wait) completes the job (the context's pending job) and returns out, or None while it runs
+    (wait=False)."""
+
+
 class GenMeshJob:
     """What Context.gen_mesh_launch returns: poll(wait) completes the job (the context's pending job) and returns (mesh, info dict with the keys of
     scene.gen_mesh's plus erosion_moves), or None while it runs (wait=False). With lights it returns (mesh, info, shadows), shadows as MeshShadowsJob's."""
@@ -886,12 +899,14 @@ class Context:
         (numpy or CUDA tensor), None releases it."""
         if data16 is None:
             self._check(lib.tw_set_heightmap(self._h, None, 0, 0))
+            self._hmap_size = None
             return
         if not hasattr(data16, "data_ptr"):
             data16 = np.ascontiguousarray(data16, np.uint8)
         if len(data16.shape) != 3 or data16.shape[2] != 2:
             raise ValueError("set_heightmap: data16 must have shape [h, w, 2]")
         self._check(lib.tw_set_heightmap(self._h, _ptr(data16), int(data16.shape[1]), int(data16.shape[0])))
+        self._hmap_size = (int(data16.shape[1]), int(data16.shape[0]))
 
     def update_heightmap(self, data16, rects):
         """tw_update_heightmap: texels rects ([n, 4] x, y, w, h) of the set_heightmap image become those of data16 (uint8 [h, w, 2] host array, the whole
@@ -906,6 +921,46 @@ class Context:
             ptr, pitch = C.c_void_p(data16.ctypes.data), int(data16.strides[0])
         arr, n = _rects(rects)
         self._check(lib.tw_update_heightmap(self._h, ptr, pitch, arr, n))
+
+    def image_size(self):
+        """(width, height) of the set_heightmap image this context reads (a shared context: its parent's), as the last set_heightmap or set_image
+        heightmap job on the root gave it; None without one."""
+        root = self.parent or self
+        return getattr(root, "_hmap_size", None)
+
+    def read_heightmap_launch(self, rects=None, out=None):
+        """tw_read_heightmap_launch: the set_heightmap image's texels back, as this context's asynchronous job (also on a shared context, which reads its
+        parent's image). rects = [n, 4] (x, y, w, h), default the whole image. out = uint8 [rows, cols, 2] with contiguous rows: a numpy array or a torch
+        tensor, host (pageable or pinned) or CUDA, whose texel (x, y) is out[y, x] (its row pitch may exceed 2*cols); default a new numpy [h, w, 2] array.
+        The job sees every update_heightmap made before the launch and none after it. Returns a HmapReadJob whose poll returns out."""
+        size = self.image_size()
+        if rects is None:
+            if size is None:
+                raise TwError(TW_ERR_STATE, "read_heightmap: the context has no heightmap image")
+            rects = [(0, 0, size[0], size[1])]
+        if out is None:
+            if size is None:
+                raise TwError(TW_ERR_STATE, "read_heightmap: the context has no heightmap image")
+            out = np.zeros((size[1], size[0], 2), np.uint8)
+        if hasattr(out, "data_ptr"):
+            import torch
+            if out.dtype != torch.uint8 or out.dim() != 3 or out.shape[2] != 2 or tuple(out.stride())[1:] != (2, 1):
+                raise ValueError("read_heightmap: out must be uint8 [rows, cols, 2] with contiguous rows")
+            ptr, pitch = C.c_void_p(out.data_ptr()), int(out.stride(0))
+        else:
+            if not isinstance(out, np.ndarray) or out.dtype != np.uint8 or out.ndim != 3 or out.shape[2] != 2 or out.strides[1:] != (2, 1):
+                raise ValueError("read_heightmap: out must be uint8 [rows, cols, 2] with contiguous rows")
+            ptr, pitch = C.c_void_p(out.ctypes.data), int(out.strides[0])
+        arr, n = _rects(rects)
+        a = HmapReadArgs(C.cast(arr, C.c_void_p) if n else None, n, ptr, pitch)
+        self._check(lib.tw_read_heightmap_launch(self._h, C.byref(a)))
+        job = HmapReadJob(self, out)
+        self._tiles_job = (out, job)
+        return job
+
+    def read_heightmap(self, rects=None, out=None):
+        """tw_read_heightmap: read_heightmap_launch(rects, out) completed at once; returns out (default the whole image as a new uint8 [h, w, 2] array)."""
+        return self.read_heightmap_launch(rects, out).poll(wait=True)
 
     def tile_normals(self, tiles, dx_val, dy_val, out=None):
         """tile_t::upload_normal_texture for a batch: returns (rgba [nt, stride, stride, 4] uint8, min_normal_z [nt])."""
@@ -1211,6 +1266,8 @@ class Context:
         job = HeightmapJob()
         o = HeightmapOutputs(_ptr(data16), _ptr(vals), C.cast(C.pointer(job.info), C.c_void_p), 1 if set_image else 0)
         self._check(lib.tw_proc_gen_heightmap_launch(self._h, width, height, dx_val, dy_val, C.byref(hp), erosion_iters, C.byref(ep), C.byref(o)))
+        if set_image:
+            self._hmap_size = (int(width), int(height))
         self._tiles_job = (data16, vals, job)
         return job
 

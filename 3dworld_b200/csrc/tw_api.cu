@@ -217,6 +217,34 @@ int validate_weights(tw_ctx *ctx, const tw_weight_params *wp, tw_weight_params &
 	return TW_OK;
 }
 
+// The rects of an edit or a read of the context's image (tw_update_heightmap, tw_read_heightmap_launch): TW_ERR_ARG unless every rect lies inside the image
+// and pitch >= 2*(x + w); *nrows = their rows, *texels = the packed staging's texels (each row may start up to 7 texels on, to keep its phase)
+int check_hmap_rects(tw_ctx *ctx, const tw_hmap_rect *rects, uint32_t nrects, size_t pitch, const char *pitch_name, size_t *nrows, size_t *texels) {
+	int const W = ctx->hmap_w, H = ctx->hmap_h;
+	*nrows = *texels = 0;
+	for (uint32_t r = 0; r < nrects; ++r) {
+		tw_hmap_rect const &R = rects[r];
+		if (R.w <= 0 || R.h <= 0 || R.x < 0 || R.y < 0 || R.x > W - R.w || R.y > H - R.h)
+			return tw_set_error(ctx, TW_ERR_ARG, "rect %u (%d, %d, %d x %d) is empty or reaches outside the %d x %d image", r, R.x, R.y, R.w, R.h, W, H);
+		if (pitch < (size_t)2*((size_t)R.x + (size_t)R.w)) return tw_set_error(ctx, TW_ERR_ARG, "%s %zu < 2*(x + w) for rect %u", pitch_name, pitch, r);
+		*nrows += (size_t)R.h; *texels += (size_t)R.w*R.h + 7*(size_t)R.h;
+	}
+	if (*nrows > 0xffffffffu) return tw_set_error(ctx, TW_ERR_ARG, "too many rows in one call");
+	return TW_OK;
+}
+
+// Each row of the rects in order: row(rect, y, img), where img = y*width + x is the row's first texel in the image
+template <typename Row> void for_hmap_rows(size_t width, const tw_hmap_rect *rects, uint32_t nrects, Row &&row) {
+	for (uint32_t r = 0; r < nrects; ++r) {
+		for (int y = rects[r].y; y < rects[r].y + rects[r].h; ++y) {row(rects[r], y, (size_t)y*width + (size_t)rects[r].x);}
+	}
+}
+
+// The next row of w texels of packed staging whose next free texel is `at`: its first texel, placed at the phase of texel `phase_of` modulo 8 texels (16 bytes)
+inline size_t pack_hmap_row(size_t &at, size_t phase_of, unsigned w) {size_t const p = at + ((phase_of - at) & 7); at = p + w; return p;}
+
+inline void set_hmap_row(twi_hmap_row &row, size_t dst, size_t src, int w) {row.dst = dst; row.src = src; row.w = (unsigned)w; row.pad = 0;}
+
 } // namespace
 
 int twi_begin(tw_ctx *ctx) {int const rc = check_ctx(ctx); return rc ? rc : finish_pending(ctx);}
@@ -358,7 +386,7 @@ int tw_cancel(tw_ctx *ctx) {
 	twi_job const &j = ctx->async.job;
 	if (!j.complete) return TW_OK;
 	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "the pending job cannot be cancelled: a job that touches a tile set or a voxel model committed its state at "
-	                                                           "its launch, and a points job is a single kernel");
+	                                                           "its launch, and a points job or a heightmap read has no cancellation point");
 	ctx->h_job->cancel = j.seq;
 	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->d_job_words->cancel, &ctx->h_job->cancel, sizeof(unsigned), cudaMemcpyHostToDevice, ctx->cancel_stream));
 	ctx->cancel_sent = true;
@@ -966,17 +994,9 @@ int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, con
 	if (nrects && (!src16 || !rects)) return tw_set_error(ctx, TW_ERR_ARG, "null src16 or rects");
 	if (nrects == 0) return TW_OK;
 	if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "the context has no heightmap image (tw_set_heightmap, or a job that sets it is pending)");
-	int const W = ctx->hmap_w, H = ctx->hmap_h;
-	size_t nrows = 0, texels = 0;
-	for (uint32_t r = 0; r < nrects; ++r) {
-		tw_hmap_rect const &R = rects[r];
-		if (R.w <= 0 || R.h <= 0 || R.x < 0 || R.y < 0 || R.x > W - R.w || R.y > H - R.h)
-			return tw_set_error(ctx, TW_ERR_ARG, "rect %u (%d, %d, %d x %d) is empty or reaches outside the %d x %d image", r, R.x, R.y, R.w, R.h, W, H);
-		if (src_pitch < (size_t)2*((size_t)R.x + (size_t)R.w)) return tw_set_error(ctx, TW_ERR_ARG, "src_pitch %zu < 2*(x + w) for rect %u", src_pitch, r);
-		nrows += (size_t)R.h; texels += (size_t)R.w*R.h + 7*(size_t)R.h;
-	}
+	size_t nrows, texels;
+	rc = check_hmap_rects(ctx, rects, nrects, src_pitch, "src_pitch", &nrows, &texels); if (rc) return rc;
 	if (tw_is_device_ptr(src16)) return tw_set_error(ctx, TW_ERR_ARG, "src16 must be host memory");
-	if (nrows > 0xffffffffu) return tw_set_error(ctx, TW_ERR_ARG, "too many rows in one edit");
 	twi_carve rows_region;
 	rows_region.take<twi_hmap_row>(nrows);
 	size_t const rows_bytes = rows_region.bytes, need = rows_bytes + 2*texels;
@@ -1011,15 +1031,11 @@ int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, con
 	twi_hmap_row *rows = (twi_hmap_row *)g->h;
 	uint8_t *data = (uint8_t *)g->h + rows_bytes;
 	size_t k = 0, at = 0; // row, next free texel of the packed data
-	for (uint32_t r = 0; r < nrects; ++r) {
-		tw_hmap_rect const &R = rects[r];
-		for (int y = R.y; y < R.y + R.h; ++y, ++k) {
-			size_t const dst = (size_t)y*W + R.x, src = at + ((dst - at) & 7); // src = dst modulo 8 texels (16 bytes)
-			memcpy(data + 2*src, src16 + (size_t)y*src_pitch + 2*(size_t)R.x, 2*(size_t)R.w);
-			rows[k].dst = dst; rows[k].src = src; rows[k].w = (unsigned)R.w; rows[k].pad = 0;
-			at = src + R.w;
-		}
-	}
+	for_hmap_rows((size_t)ctx->hmap_w, rects, nrects, [&](tw_hmap_rect const &R, int y, size_t img) {
+		size_t const packed = pack_hmap_row(at, img, (unsigned)R.w);
+		memcpy(data + 2*packed, src16 + (size_t)y*src_pitch + 2*(size_t)R.x, 2*(size_t)R.w);
+		set_hmap_row(rows[k++], img, packed, R.w);
+	});
 	// behind the image work of the family's pending jobs that read or write the image: a heightmap tile job's sampling, the whole of an image erosion or a
 	// set_image job (a job that does not complete before its poll is still pending)
 	std::vector<tw_ctx *> family(1, ctx);
@@ -1032,6 +1048,85 @@ int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, con
 	TW_CUDA(ctx, cudaEventRecord(g->ev, ctx->img_stream));
 	TW_CUDA(ctx, cudaEventRecord(ctx->img_ev, ctx->img_stream));
 	return TW_OK;
+}
+
+// A read of the image, the inverse of an edit, as the context's job, on the edit's kernel run the other way (a row copy between two buffers whose rows share
+// their phase modulo 16 bytes). The row tables go up from the pinned staging in one copy. A device dst16 whose rows all have their image rows' phase is
+// written by one kernel straight from the image. Otherwise the kernel packs the rows into device staging, each at its image phase:
+//   host dst16: one copy brings the staging down to the pinned staging, and the completion moves each row to dst16;
+//   device dst16: the rows are packed in groups by their phase shift d (0..7 texels), one copy per group moves it d texels on into a second staging, where
+//                 each row has its destination's phase, and a second run of the kernel writes the rows to dst16.
+// So the work enqueued does not grow with the number of rects. The image is free for later edits after the first kernel.
+// Slot 0: [row tables | staging | second staging (device dst16 out of phase)]; pinned staging: [row tables | staging (host dst16)].
+int tw_read_heightmap_launch(tw_ctx *ctx, const tw_hmap_read *r) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!r) return tw_set_error(ctx, TW_ERR_ARG, "null read");
+	uint32_t const nrects = r->nrects;
+	if (nrects && (!r->rects || !r->dst16)) return tw_set_error(ctx, TW_ERR_ARG, "null rects or dst16");
+	if (nrects == 0) return TW_OK;
+	if (!ctx->hmap_w) return tw_set_error(ctx, TW_ERR_STATE, "the context has no heightmap image (tw_set_heightmap, or a job that sets it is pending)");
+	size_t nrows, texels;
+	rc = check_hmap_rects(ctx, r->rects, nrects, r->dst_pitch, "dst_pitch", &nrows, &texels); if (rc) return rc;
+	uint8_t *const dst16 = r->dst16;
+	size_t const pitch = r->dst_pitch, W = (size_t)ctx->hmap_w;
+	bool const dev = tw_is_device_ptr(dst16);
+	if (dev && ((reinterpret_cast<uintptr_t>(dst16) | pitch) & 1)) return tw_set_error(ctx, TW_ERR_ARG, "a device dst16 must be 2-byte aligned and dst_pitch even: its texels are 16-bit words");
+	// a device dst16 as texel offsets from the 16-byte boundary at or below it, and each row's phase shift from its image row
+	uint8_t *const base = dev ? dst16 - (reinterpret_cast<uintptr_t>(dst16) & 15) : nullptr;
+	size_t const lead = dev ? (size_t)(dst16 - base)/2 : 0;
+	auto out_of = [&](tw_hmap_rect const &R, int y) {return lead + (size_t)y*(pitch/2) + (size_t)R.x;};
+	auto shift_of = [&](tw_hmap_rect const &R, int y, size_t img) {return dev ? (unsigned)((out_of(R, y) - img) & 7) : 0u;};
+	size_t group[8] = {0, 0, 0, 0, 0, 0, 0, 0}; // texels of each shift's rows in the staging
+	for_hmap_rows(W, r->rects, nrects, [&](tw_hmap_rect const &R, int y, size_t img) {group[shift_of(R, y, img)] += (size_t)R.w + 7;});
+	bool const shifted = dev && group[0] < texels, direct = dev && !shifted;
+	size_t const ntab = shifted ? 2*nrows : nrows, stage = texels + 64; // each group starts on an 8-texel boundary
+	twi_hmap_row *d_rows, *h_rows;
+	uint8_t *d_s1 = nullptr, *d_s2 = nullptr, *h_data = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_rows = c.take<twi_hmap_row>(ntab);
+		if (!direct) {d_s1 = c.take<uint8_t>(2*stage);}
+		if (shifted) {d_s2 = c.take<uint8_t>(2*stage + 16);}
+	}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {h_rows = c.take<twi_hmap_row>(ntab); if (!dev) {h_data = c.take<uint8_t>(2*stage);}}); if (rc) return rc;
+	size_t g0[8], at[8]; // each group's first texel and next free texel in the staging
+	for (size_t d = 0, o = 0; d < 8; o += (group[d] + 7) & ~(size_t)7, ++d) {g0[d] = at[d] = o;}
+	size_t k = 0;
+	for_hmap_rows(W, r->rects, nrects, [&](tw_hmap_rect const &R, int y, size_t img) {
+		if (direct) {set_hmap_row(h_rows[k++], out_of(R, y), img, R.w); return;}
+		unsigned const d = shift_of(R, y, img);
+		size_t const packed = pack_hmap_row(at[d], img, (unsigned)R.w);
+		set_hmap_row(h_rows[k], packed, img, R.w);
+		if (shifted) {set_hmap_row(h_rows[nrows + k], out_of(R, y), packed + d, R.w);} // in the second staging, the row has its destination's phase
+		++k;
+	});
+	twi_job pending;
+	pending.reads_image = true; // no cancellation point
+	pending.complete = [dev, h_rows, h_data, nrows, W, dst16, pitch](tw_ctx *) -> int {
+		for (size_t i = 0; i < nrows && !dev; ++i) {
+			twi_hmap_row const &R = h_rows[i];
+			memcpy(dst16 + (R.src/W)*pitch + 2*(R.src % W), h_data + 2*R.dst, 2*(size_t)R.w);
+		}
+		return TW_OK;
+	};
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
+		TW_CUDA(ctx, cudaMemcpyAsync(d_rows, h_rows, ntab*sizeof(twi_hmap_row), cudaMemcpyHostToDevice, ctx->stream));
+		int g = twi_hmap_scatter(ctx, ctx->stream, d_rows, (uint32_t)nrows, ctx->d_hmap, direct ? base : d_s1); if (g) return g;
+		TW_CUDA(ctx, cudaEventRecord(ctx->async.image_free, ctx->stream)); // a later edit waits for this kernel only
+		ctx->async.image_free_set = true;
+		if (shifted) {
+			for (size_t d = 0; d < 8; ++d) {
+				if (at[d] > g0[d]) {TW_CUDA(ctx, cudaMemcpyAsync(d_s2 + 2*(g0[d] + d), d_s1 + 2*g0[d], 2*(at[d] - g0[d]), cudaMemcpyDeviceToDevice, ctx->stream));}
+			}
+			g = twi_hmap_scatter(ctx, ctx->stream, d_rows + nrows, (uint32_t)nrows, d_s2, base); if (g) return g;
+		}
+		if (!dev) {TW_CUDA(ctx, cudaMemcpyAsync(h_data, d_s1, 2*at[0], cudaMemcpyDeviceToHost, ctx->stream));}
+		return TW_OK;
+	});
+}
+
+int tw_read_heightmap(tw_ctx *ctx, const tw_hmap_read *r) {
+	int const rc = tw_read_heightmap_launch(ctx, r);
+	return rc ? rc : poll_job(ctx, 1);
 }
 
 int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,

@@ -24,7 +24,8 @@ struct twi_job {
 // One edit's staging (tw_update_heightmap): pinned host memory and device memory of `bytes` each, holding [row table | packed texels], reused once `ev` (recorded
 // after the edit's scatter kernel) has completed
 struct twi_img_stage {void *h = nullptr; void *d = nullptr; size_t bytes = 0; cudaEvent_t ev = nullptr;};
-// one row of an edit: w texels from texel src of the staging's packed texels to texel dst of the image (src and dst have the same phase modulo 8 texels)
+// one row of an edit: w texels from texel src of the staging's packed texels to texel dst of the image (src and dst have the same phase modulo 8 texels);
+// a read runs the same kernel the other way, from texel src of the image (or of its own staging) to texel dst of its staging or of the caller's device dst16
 struct twi_hmap_row {unsigned long long dst, src; unsigned w, pad;};
 
 struct tw_async_state {
@@ -178,7 +179,8 @@ int twi_wait_image_edits(tw_ctx *ctx);
 // Before the root's image is freed or replaced (tw_set_heightmap, a set_image job, tw_destroy): waits for the pending edits (the caller has completed every job
 // of the family they could wait for) and frees their staging
 int twi_image_settle(tw_ctx *root);
-// the scatter kernel of an edit on `st`: nrows rows (d_rows) of packed texels d_data into the image d_img
+// the scatter kernel of an edit on `st`: nrows rows (d_rows) of packed texels d_data into the image d_img (a read: of texels d_data into d_img, its destination;
+// d_data and d_img 16-byte aligned, each row's src and dst of the same phase modulo 8 texels)
 int twi_hmap_scatter(tw_ctx *ctx, cudaStream_t st, const twi_hmap_row *d_rows, uint32_t nrows, const uint8_t *d_data, uint8_t *d_img);
 
 // Makes `job` the context's pending job (the previous one has been completed): enqueue() puts the job's work on ctx->stream, with every other stream it used

@@ -11,6 +11,7 @@
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //   tw3d::update_heightmap, tw3d::hmap_tiles_touched  <->  terrain_hmap_manager_t's brush edits and re-applied modmap, and the tiles they change   src/heightmap.cpp:36-58,243-308
+//   tw3d::read_heightmap(_async)  <->  heightmap_t::data brought back in line with the device's image before brushes, write_heightmap_png and saved edits   src/heightmap.cpp:243-308,365-378
 //   tw3d::gen_mesh_async         <->  gen_mesh in ground mode at start-up and on every regeneration, without stalling the frame   src/mesh_gen.cpp:257-355
 //   tw3d::calc_mesh_shadows(lpos, mh, smask, xsize, ysize, ...), tw3d::mesh_shadows_async  <->  calc_mesh_shadows on the ground-mode mesh   src/visibility.cpp:411-517
 //   tw3d::get_exact_zvals_async, tw3d::heightmap_heights_async  <->  get_exact_zval / get_clamped_height per placed object, without stalling the frame   src/mesh_gen.cpp:816-847, src/heightmap.cpp:385-402
@@ -448,6 +449,28 @@ inline void update_heightmap(const uint8_t *hmap16, int width, int height, const
 	int const rc = tw_update_heightmap(c, hmap16, 2*(size_t)width, rects, n);
 	if (rc != TW_OK) {detail::fail(rc, "update_heightmap", c);}
 }
+// The inverse of update_heightmap (tw_read_heightmap): after an erosion of the image (erode_heightmap_async) or a set_image proc_gen_heightmap_async without
+// data16, the engine's CPU image hmap16 (width x height texels, the layout set_heightmap took) no longer holds the device's map. read_heightmap_async copies
+// the rects' texels (rects = nullptr: the whole image) into hmap16 once its tiles_job is ready; read_heightmap blocks until they are there. Only then do
+// brushes, update_heightmap, write_heightmap_png and the saved edits work on the map the device has. The read sees every update_heightmap made before the
+// call and none made after it; hmap16 is host or device memory (2-byte aligned) and must stay valid until the job is ready. tile_job_pool has the same call on a slot.
+namespace detail {
+	inline tiles_job launch_read_heightmap(tw_ctx *c, std::atomic<uint64_t> &jobs, uint8_t *hmap16, int width, int height, const tw_hmap_rect *rects, unsigned n) {
+		if (width != tls().hmap_w || height != tls().hmap_h) {fail(TW_ERR_ARG, "read_heightmap: the image size differs from set_heightmap's", nullptr);}
+		tw_hmap_rect const whole = {0, 0, width, height};
+		tw_hmap_read const r = {rects ? rects : &whole, rects ? n : 1u, hmap16, 2*(size_t)width};
+		uint64_t const number = ++jobs;
+		int const rc = tw_read_heightmap_launch(c, &r);
+		if (rc != TW_OK) {--jobs; fail(rc, "read_heightmap_async", c);}
+		return tiles_job(c, &jobs, number);
+	}
+}
+inline tiles_job read_heightmap_async(uint8_t *hmap16, int width, int height, const tw_hmap_rect *rects = nullptr, unsigned n = 0) {
+	return detail::launch_read_heightmap(ctx(), detail::tls().tile_jobs, hmap16, width, height, rects, n);
+}
+inline void read_heightmap(uint8_t *hmap16, int width, int height, const tw_hmap_rect *rects = nullptr, unsigned n = 0) {
+	read_heightmap_async(hmap16, width, height, rects, n).wait();
+}
 inline void hmap_tiles_touched(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const tw_hmap_rect *rects, unsigned n, uint8_t *touched,
                                int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
 	tw_hmap_sampler const hs = hmap_sampler(detail::tls().hmap_w, detail::tls().hmap_h, tex_edge_mode);
@@ -660,6 +683,11 @@ public:
 	tiles_job heightmap_heights_async(const float *cells, size_t n, float *heights_out, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
 		slot &s = next();
 		return detail::launch_points(s.c, s.jobs, cells, n, heights_out, TW_PQ_HMAP, false, tex_edge_mode, "heightmap_heights_async");
+	}
+	// read_heightmap_async (above) on a slot
+	tiles_job read_heightmap_async(uint8_t *hmap16, int width, int height, const tw_hmap_rect *rects = nullptr, unsigned n = 0) {
+		slot &s = next();
+		return detail::launch_read_heightmap(s.c, s.jobs, hmap16, width, height, rects, n);
 	}
 };
 

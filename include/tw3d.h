@@ -567,6 +567,34 @@ typedef struct tw_hmap_rect { int x, y, w, h; } tw_hmap_rect;
  * w <= 0 or h <= 0 or reaching outside the image (no clipping), src_pitch < 2*(x + w) for some rect, and a device src16; TW_ERR_STATE without an image,
  * which includes the time an erosion of the image or a set_image heightmap job is pending. nrects == 0 is TW_OK and does nothing. */
 TW_API int tw_update_heightmap(tw_ctx *ctx, const uint8_t *src16, size_t src_pitch, const tw_hmap_rect *rects, uint32_t nrects);
+/* Reads the context's image back, the inverse of tw_update_heightmap: for each rect, the two bytes of texel (x, y) go to dst16 + y*dst_pitch + 2*x, so a read
+ * of rects followed by tw_update_heightmap of the same rects from the same buffer changes no byte. The whole image is the one rect {0, 0, width, height}
+ * with dst_pitch = 2*width. This is how an engine's CPU copy catches up with what the device wrote: an erosion of the image, a set_image heightmap job (with
+ * or without data16), before its brushes, its PNG or its saved edits read the CPU copy.
+ * - What it sees: the image as it was when the launch returned - every tw_update_heightmap made before the launch, none made after it - on the root context
+ *   and on every shared context (a shared context reads its parent's image, as TW_PQ_HMAP points do). On the root the launch first completes the pending
+ *   job, as every entry point does, so a read launched after an erosion of the image or a set_image job sees their result; on a shared context while such a
+ *   job is pending there is no image (TW_ERR_STATE).
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it. A later edit waits on the device for its first kernel
+ *   only. tw_cancel returns TW_ERR_STATE: the job has no cancellation point.
+ * - The copies run on tw_update_heightmap's row kernel. dst16 in device memory (2-byte aligned, even dst_pitch: texels are 16-bit words) is written at the
+ *   caller's pitch: straight from the image when every row has its image row's phase modulo 16 bytes (a buffer laid out like the image), otherwise through
+ *   device staging, with one device copy per phase shift (at most 8) and a second run of the kernel. dst16 in host memory (page-locked or pageable)
+ *   receives the rows from the context's pinned staging in the completing poll. Either way the launch never waits for the device, except when the
+ *   context's scratch or staging first has to grow, and what it enqueues does not grow with nrects: one row-table copy and one kernel, plus one copy down
+ *   for host dst16, or the shift copies and the second kernel for a device dst16 out of phase. dst16 must stay valid until the completing poll.
+ * - Errors, nothing enqueued: TW_ERR_ARG for a NULL ctx or r, NULL rects or dst16 with nrects > 0, a rect with w <= 0 or h <= 0 or reaching outside the
+ *   image (no clipping), dst_pitch < 2*(x + w) for some rect, a device dst16 at an odd address or with an odd dst_pitch; TW_ERR_STATE without an image.
+ *   nrects == 0 is TW_OK and does nothing.
+ * tw_read_heightmap is the launch followed by a poll with wait = 1. */
+typedef struct tw_hmap_read {
+	const tw_hmap_rect *rects;   /* nrects rects of the image, as tw_update_heightmap's */
+	uint32_t nrects;
+	uint8_t *dst16;              /* texel (x, y) of each rect -> dst16 + y*dst_pitch + 2*x */
+	size_t   dst_pitch;          /* >= 2*(x + w) for every rect; 2*width for an engine's whole image */
+} tw_hmap_read;
+TW_API int tw_read_heightmap_launch(tw_ctx *ctx, const tw_hmap_read *r);
+TW_API int tw_read_heightmap(tw_ctx *ctx, const tw_hmap_read *r);
 /* Host only, no context: touched[t] = 1 exactly when some cell of tile t (origin origins_xy[2t], origins_xy[2t + 1], zvsize^2 cells), as the heightmap-texture
  * tiles sample it under hs, reads a texel inside one of the rects - the live tiles an edit changes. A texel counts as read even where its bilinear weight is 0;
  * cells that read nothing (off the texture in cliff mode) read no texel. Exact, and O(zvsize) per distinct tile column and row: the sampler's index

@@ -93,6 +93,11 @@ class VoxelBlocksOut(C.Structure):
                 ("nblocks", C.c_void_p), ("nverts", C.c_void_p), ("ntris", C.c_void_p), ("changed", C.c_void_p)]
 
 
+class VoxelChanges(C.Structure):
+    """tw_voxel_changes (include/tw3d.h): the voxels an edit changed - index, value and flags buffers, their capacity, and the host count."""
+    _fields_ = [("index", C.c_void_p), ("vals", C.c_void_p), ("outside", C.c_void_p), ("capacity", C.c_uint64), ("nchanged", C.c_void_p)]
+
+
 class VoxelBox(C.Structure):
     """tw_voxel_box (include/tw3d.h): the voxels [x, x+w) x [y, y+h) x [z, z+d)."""
     _fields_ = [(n, C.c_uint32) for n in ("x", "y", "z", "w", "h", "d")]
@@ -242,6 +247,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
                "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
+               "tw_voxel_model_edit_launch_ex",
                "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows",
                "tw_read_heightmap_launch", "tw_read_heightmap"]
 
@@ -359,6 +365,7 @@ def _load():
     L.tw_voxel_model_build_launch.argtypes = [vp, C.POINTER(VoxelParams), vp, vp, C.POINTER(VoxelBlocksOut)]
     L.tw_voxel_model_edit_launch.argtypes = [vp, vp, C.c_uint32, vp, C.POINTER(VoxelBlocksOut)]
     L.tw_voxel_model_read.argtypes = [vp, vp, vp, vp]
+    L.tw_voxel_model_edit_launch_ex.argtypes = [vp, vp, C.c_uint32, vp, C.POINTER(VoxelBlocksOut), C.POINTER(VoxelChanges)]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
@@ -582,11 +589,31 @@ class VoxelBuildJob:
 
 class VoxelModelJob:
     """The host results of a VoxelModel job, filled by the poll that completes it: blocks (numpy structured array of the listed blocks' VoxelBlockMesh
-    rows: block, voff, nverts, toff, ntris), nverts, ntris and changed."""
+    rows: block, voff, nverts, toff, ntris), nverts, ntris and changed; for an edit launched with a change list, nchanged and changes."""
 
     def __init__(self, nblocks_max):
         self._table = (VoxelBlockMesh * max(nblocks_max, 1))()
         self._nblocks, self._nverts, self._ntris, self._changed = C.c_uint32(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._nchanged, self._change_bufs = C.c_uint64(0), None
+
+    def _changes(self, changes):
+        """VoxelChanges of (index, vals, outside) buffers, each None or a CUDA tensor / page-locked buffer; the capacity is index's length."""
+        index, vals, outside = changes
+        self._change_bufs = (index, vals, outside)
+        cap = 0 if index is None else (int(index.numel()) if hasattr(index, "numel") else int(index.size))
+        return VoxelChanges(_ptr(index), _ptr(vals), _ptr(outside), cap, C.cast(C.pointer(self._nchanged), C.c_void_p))
+
+    @property
+    def nchanged(self):
+        """Voxels whose value or flags the edit changed (may exceed the change list's capacity)."""
+        return int(self._nchanged.value)
+
+    @property
+    def changes(self):
+        """(index, vals, outside): the caller's buffers cut to the listed entries, min(capacity, nchanged); None where no buffer was given."""
+        index = self._change_bufs[0]
+        k = min(self.nchanged, 0 if index is None else (int(index.numel()) if hasattr(index, "numel") else int(index.size)))
+        return tuple(None if b is None else b[:k] for b in self._change_bufs)
 
     def _out(self, verts, indices):
         size = lambda a: 0 if a is None else (int(a.numel()) if hasattr(a, "numel") else int(a.size)) // 3  # noqa: E731
@@ -1320,16 +1347,19 @@ class VoxelModel:
         self.ctx._tiles_job = (vals, verts, indices, job)
         return job
 
-    def edit_launch(self, boxes, values, verts=None, indices=None):
+    def edit_launch(self, boxes, values, verts=None, indices=None, changes=None):
         """tw_voxel_model_edit_launch: boxes = (x, y, z, w, h, d) tuples, values = their new raw values one box after another, each in the grid's order
-        (z fastest, then x, then y), copied during the launch. Re-meshes the blocks the edit changed; returns a VoxelModelJob listing them."""
+        (z fastest, then x, then y), copied during the launch. Re-meshes the blocks the edit changed; returns a VoxelModelJob listing them.
+        changes = (index, vals, outside) (tw_voxel_model_edit_launch_ex): buffers for the list of the voxels the edit changed, each None or a CUDA tensor /
+        page-locked buffer (uint32, float32, uint8) of the list's capacity; the job's nchanged and changes hold the list once it completes."""
         b = (VoxelBox * max(len(boxes), 1))(*[VoxelBox(*[int(v) for v in t]) for t in boxes])
         vals = np.ascontiguousarray(values, np.float32).ravel()
         job = VoxelModelJob(self.nblocks)
         out = job._out(verts, indices)
-        self.ctx._check(lib.tw_voxel_model_edit_launch(self._h, C.cast(b, C.c_void_p) if len(boxes) else None, len(boxes), _ptr(vals) if len(boxes) else None,
-                                                       C.byref(out)))
-        self.ctx._tiles_job = (verts, indices, job)
+        ch = None if changes is None else job._changes(changes)
+        self.ctx._check(lib.tw_voxel_model_edit_launch_ex(self._h, C.cast(b, C.c_void_p) if len(boxes) else None, len(boxes), _ptr(vals) if len(boxes) else None,
+                                                          C.byref(out), C.byref(ch) if ch is not None else None))
+        self.ctx._tiles_job = (verts, indices, changes, job)
         return job
 
     def read(self, raw=None, vals=None, outside=None):

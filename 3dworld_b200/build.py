@@ -9,6 +9,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib3dworld_b200.so")
 SOURCES = ["tw_api.cu", "tw_heightgen.cu", "tw_erosion.cu", "tw_voxel.cu", "tw_streaming.cu", "tw_tiles.cu", "tw_multi.cu", "tw_voxel_post.cu", "tw_shadows.cu", "tw_tileset.cu", "tw_host.cpp"]
+# device code the library loads at run time (cudaLibraryLoadFromFile), each built as <name>.cubin beside the library: the change list of a voxel model
+# edit (tw_voxel_post.cu loads it)
+MODULES = ["tw_voxel_changes.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fno-fast-math,-fvisibility=hidden", "--use_fast_math=false"]
 
@@ -20,10 +23,14 @@ def nvcc():
     raise RuntimeError("nvcc not found")
 
 
+def module_path(lib, src):
+    return os.path.join(os.path.dirname(lib), src.rsplit(".", 1)[0] + ".cubin")
+
+
 def needs_build():
-    if not os.path.exists(LIB):
+    if not os.path.exists(LIB) or not all(os.path.exists(module_path(LIB, m)) for m in MODULES):
         return True
-    t = os.path.getmtime(LIB)
+    t = min([os.path.getmtime(LIB)] + [os.path.getmtime(module_path(LIB, m)) for m in MODULES])
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "tw3d.h"), __file__]
     return any(os.path.getmtime(d) > t for d in deps)
 
@@ -43,6 +50,9 @@ def build(force=False, verbose=False, lib=None, objdir=None):
         cmd = [nvcc()] + flags + (["-Xptxas", "-v"] if verbose else []) + ["-x", "cu", "-c", os.path.join(CSRC, src), "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(obj)
+    for src in MODULES:
+        cmd = [nvcc()] + flags + (["-Xptxas", "-v"] if verbose else []) + ["-cubin", os.path.join(CSRC, src), "-o", module_path(lib, src) + ".tmp"]
+        procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     for src, p in procs:
         out, _ = p.communicate()
         if verbose and out:
@@ -51,6 +61,8 @@ def build(force=False, verbose=False, lib=None, objdir=None):
             raise RuntimeError("nvcc failed for %s:\n%s" % (src, out))
     cmd = [nvcc(), "-shared", "-Wno-deprecated-gpu-targets", "-o", lib + ".tmp"] + objs + ["-Xlinker", "--no-undefined", "-lcudart_static", "-lpthread", "-ldl", "-lrt"]
     subprocess.check_call(cmd)
+    for src in MODULES:
+        os.replace(module_path(lib, src) + ".tmp", module_path(lib, src))
     os.replace(lib + ".tmp", lib)   # atomic: a concurrent snapshot of the tree never sees a half-written library
     return lib
 

@@ -11,6 +11,10 @@
 //                       reference's emission order without atomics (pass 1: counts only; pass 2: write).
 // All fp32 arithmetic is the reference's (separate multiply and add: the TU is compiled with -fmad=false), std::min/max argument order kept.
 #include "tw_internal.h"
+#include "tw_voxel_edit.cuh"
+#include <dlfcn.h>
+#include <mutex>
+#include <string>
 #include <vector>
 
 namespace {
@@ -852,7 +856,6 @@ struct tw_voxel_model {
 
 namespace {
 
-struct BlockGrid {unsigned bx, by, nbx, chunks;};
 
 __device__ __forceinline__ CubeRange block_range(const tw_voxel_post_params &P, const BlockGrid &G, unsigned b) {
 	CubeRange R;
@@ -967,43 +970,11 @@ __global__ void __launch_bounds__(1024) list_marked_kernel(unsigned char *__rest
 	if (threadIdx.x == 0) {list[0] = carry;}
 }
 
-// every block whose cubes read voxel column (x, y): the cubes x-1, x and y-1, y that exist
-__device__ __forceinline__ void mark_readers(unsigned char *mark, const tw_voxel_post_params &P, const BlockGrid &G, unsigned x, unsigned y) {
-	for (unsigned cy = (y ? y - 1 : 0); cy <= y && cy + 1 < P.ny; ++cy) {
-		for (unsigned cx = (x ? x - 1 : 0); cx <= x && cx + 1 < P.nx; ++cx) {mark[(cy / G.by)*G.nbx + cx / G.bx] = 1;}
-	}
-}
-
-// an edit's box and the index of its first value among the packed values; later: a later box overlaps it
-struct twi_box {unsigned x, y, z, w, h, d; unsigned long long off; unsigned later, pad;};
-
-// the edit's values into the raw field, with the raw flags of outside_kernel; post (rm == 0, where the post field is the raw one): also compared with the
-// model's field and flags, which take the new values, marking the blocks that read a changed voxel
 __global__ void box_scatter_kernel(const twi_box *__restrict__ boxes, unsigned nboxes, const float *__restrict__ values, unsigned long long total,
 	tw_voxel_post_params P, const unsigned *__restrict__ zix_xy, BlockGrid G, float *__restrict__ raw, unsigned char *__restrict__ raw_o, float *post,
 	unsigned char *post_o, unsigned char *mark)
 {
-	unsigned long long const stride = (unsigned long long)gridDim.x*blockDim.x;
-	for (unsigned long long t = (unsigned long long)blockIdx.x*blockDim.x + threadIdx.x; t < total; t += stride) {
-		unsigned lo = 0, hi = nboxes - 1;
-		while (lo < hi) {unsigned const mid = (lo + hi + 1) >> 1; if (boxes[mid].off <= t) lo = mid; else hi = mid - 1;}
-		twi_box const B = boxes[lo];
-		unsigned long long const r = t - B.off, xy = r / B.d;
-		unsigned const z = B.z + (unsigned)(r - xy*B.d), x = B.x + (unsigned)(xy % B.w), y = B.y + (unsigned)(xy / B.w);
-		bool overwritten = false;
-		for (unsigned k = lo + 1; B.later && k < nboxes && !overwritten; ++k) {
-			twi_box const &C = boxes[k];
-			overwritten = (x - C.x < C.w && y - C.y < C.h && z - C.z < C.d);
-		}
-		if (overwritten) continue;
-		size_t const i = z + ((size_t)x + (size_t)y*P.nx)*P.nz;
-		float const val = values[t];
-		bool const on_edge = (P.make_closed_surface && ((x == 0 || x == P.nx-1) || (y == 0 || y == P.ny-1) || (z == 0 || z == P.nz-1)));
-		unsigned char o = on_edge ? (unsigned char)TW_VOX_ON_EDGE : (unsigned char)((val == P.isolevel) ? 1 : (((val < P.isolevel) != (P.invert != 0)) ? 1 : 0));
-		if (zix_xy && z < __ldg(zix_xy + (size_t)y*P.nx + x)) {o |= TW_VOX_UNDER_MESH;}
-		raw[i] = val; raw_o[i] = o;
-		if (post && (__float_as_uint(post[i]) != __float_as_uint(val) || post_o[i] != o)) {post[i] = val; post_o[i] = o; mark_readers(mark, P, G, x, y);}
-	}
+	box_scatter<false>(boxes, nboxes, values, total, P, zix_xy, G, raw, raw_o, post, post_o, mark, nullptr);
 }
 
 // the model's field and flags (ov, oo) take the new ones (nv, no) where they differ, marking the blocks that read a changed voxel
@@ -1024,23 +995,30 @@ __global__ void diff_kernel(const float *__restrict__ nv, const unsigned char *_
 BlockGrid block_grid(const tw_voxel_model *m) {BlockGrid G; G.bx = m->bx; G.by = m->by; G.nbx = m->nbx; G.chunks = m->chunks; return G;}
 
 // A model job's counts in its pinned staging
-struct twi_vmodel_stage {unsigned long long nblocks, nverts, ntris, changed;};
+struct twi_vmodel_stage {unsigned long long nblocks, nverts, ntris, changed, nchanged;};
 
-// A model job's slot-0 scratch: [counters (changed at byte 64), zeroed together | frontiers (remove_unconnected > 0) | mesh scratch | table | boxes | values]
+// A model job's slot-0 scratch: [counters (changed at byte 64, the change list's total at byte 128), zeroed together | frontiers (remove_unconnected > 0) |
+// mesh scratch | table | boxes | values | change list (list: bits, chunk sums, chunk offsets)]
 // and pinned staging: [twi_vmodel_stage (64 B), then the table | boxes | values | fill coefficients]
+struct ChangeScratch {unsigned *bits, *sums; unsigned long long *offsets, *total; size_t nwords; unsigned nchunks;};
 struct ModelScratch {
-	unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values;
+	unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values; ChangeScratch L;
 	twi_vmodel_stage *h_stage; tw_voxel_block_mesh *h_table; char *h_boxes, *h_values, *h_rdata;
 };
-int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X) {
+int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X, bool list = false) {
 	tw_ctx *ctx = m->ctx;
 	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz, ng = (size_t)m->nblocks*m->chunks;
 	X->f0 = X->f1 = nullptr;
+	ChangeScratch &L = X->L;
+	L = ChangeScratch{};
+	L.nwords = list ? (n + 31)/32 : 0; L.nchunks = (unsigned)((L.nwords + CL_BLOCK - 1)/CL_BLOCK);
 	int rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
 		X->cnt = c.take<unsigned>(64); if (m->P.remove_unconnected > 0) {X->f0 = c.take<unsigned>(n + 16); X->f1 = c.take<unsigned>(n + 16);}
 		X->S = mesh_scratch(c, ng*MC_BLOCK, (unsigned)ng); X->table = c.take<tw_voxel_block_mesh>(m->nblocks); X->boxes = c.take<twi_box>(nboxes);
 		X->values = c.take<float>(nvalues);
+		if (list) {L.bits = c.take<unsigned>(L.nwords); L.sums = c.take<unsigned>(L.nchunks); L.offsets = c.take<unsigned long long>(L.nchunks);}
 	}); if (rc) return rc;
+	L.total = (unsigned long long *)(X->cnt + 32);
 	char *h_head;
 	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
 		h_head = c.take<char>(64 + (size_t)m->nblocks*sizeof(tw_voxel_block_mesh)); X->h_boxes = c.take<char>(nboxes*sizeof(twi_box));
@@ -1089,12 +1067,14 @@ int enqueue_block_meshes(tw_voxel_model *m, const unsigned *d_list, const ModelS
 	return TW_OK;
 }
 
-// a model job (not cancellable: it commits the model's state) whose completion unpacks X's stage and table into o
-twi_job model_job(const ModelScratch &X, const tw_voxel_blocks_out &o) {
+// a model job (not cancellable: it commits the model's state) whose completion unpacks X's stage and table into o, and the change list's count into
+// nchanged (optional)
+twi_job model_job(const ModelScratch &X, const tw_voxel_blocks_out &o, uint64_t *nchanged = nullptr) {
 	twi_job j;
-	j.complete = [st = X.h_stage, table = X.h_table, o](tw_ctx *) -> int {
+	j.complete = [st = X.h_stage, table = X.h_table, o, nchanged](tw_ctx *) -> int {
 		*o.nblocks = (uint32_t)st->nblocks; *o.nverts = st->nverts; *o.ntris = st->ntris;
 		if (o.changed) {*o.changed = st->changed;}
+		if (nchanged) {*nchanged = st->nchanged;}
 		memcpy(o.blocks, table, (size_t)st->nblocks*sizeof(tw_voxel_block_mesh));
 		return TW_OK;
 	};
@@ -1205,13 +1185,91 @@ extern "C" int tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_par
 	});
 }
 
+namespace {
+// the change list's outputs as the device addresses them
+struct ChangeOut {uint32_t *index; float *vals; uint8_t *outside; unsigned long long capacity; uint64_t *nchanged;};
+int validate_changes(tw_ctx *ctx, const tw_voxel_changes *ch, ChangeOut *d) {
+	if (!ch->nchanged) return tw_set_error(ctx, TW_ERR_ARG, "the change list needs nchanged");
+	if (ch->capacity && !ch->index) return tw_set_error(ctx, TW_ERR_ARG, "a change list capacity without index");
+	if ((ch->vals || ch->outside) && !ch->index) return tw_set_error(ctx, TW_ERR_ARG, "change list vals or outside without index");
+	d->index = nullptr; d->vals = nullptr; d->outside = nullptr; d->capacity = ch->capacity; d->nchanged = ch->nchanged;
+	if (ch->index && !(d->index = (uint32_t *)device_view(ch->index))) return tw_set_error(ctx, TW_ERR_ARG, "change list index must be device or page-locked host memory");
+	if (ch->vals && !(d->vals = (float *)device_view(ch->vals))) return tw_set_error(ctx, TW_ERR_ARG, "change list vals must be device or page-locked host memory");
+	if (ch->outside && !(d->outside = (uint8_t *)device_view(ch->outside))) return tw_set_error(ctx, TW_ERR_ARG, "change list outside must be device or page-locked host memory");
+	return TW_OK;
+}
+
+// The change-list kernels (tw_voxel_changes.cu) live in their own module, tw_voxel_changes.cubin beside this library, loaded once per process on first
+// use (cudaLibraryLoadFromFile loads it into each device's context as needed). A missing or unloadable module is an error.
+struct ChangeKernels {cudaKernel_t box_bits, diff_bits, count, emit;};
+int change_kernels(tw_ctx *ctx, ChangeKernels *K) {
+	static std::mutex mu;
+	static cudaLibrary_t lib = nullptr;
+	static ChangeKernels loaded;
+	std::lock_guard<std::mutex> g(mu);
+	if (!lib) {
+		Dl_info info;
+		if (!dladdr((void *)&tw_voxel_model_edit_launch_ex, &info) || !info.dli_fname) return tw_set_error(ctx, TW_ERR_CUDA, "cannot locate the library's file");
+		std::string const lib_path = info.dli_fname, path = lib_path.substr(0, lib_path.rfind('/') + 1) + "tw_voxel_changes.cubin";
+		cudaLibrary_t l = nullptr;
+		cudaError_t e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+		ChangeKernels k;
+		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.box_bits, l, "tw_box_scatter_bits_kernel");
+		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.diff_bits, l, "tw_diff_bits_kernel");
+		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.count, l, "tw_change_count_kernel");
+		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.emit, l, "tw_change_emit_kernel");
+		if (e != cudaSuccess) {
+			cudaGetLastError();
+			if (l) cudaLibraryUnload(l);
+			return tw_set_error(ctx, TW_ERR_CUDA, "cannot load the change-list kernels from %s: %s", path.c_str(), cudaGetErrorString(e));
+		}
+		lib = l; loaded = k;
+	}
+	*K = loaded;
+	return TW_OK;
+}
+// one launch of a module kernel on ctx->stream; the arguments must have the kernel's parameter types exactly
+template<typename... A>
+int launch_module_kernel(tw_ctx *ctx, cudaKernel_t k, unsigned grid, unsigned block, A... a) {
+	void *args[] = {(void *)&a...};
+	TW_CUDA(ctx, cudaLaunchKernel((const void *)k, dim3(grid), dim3(block), args, 0, ctx->stream));
+	ctx->launches++;
+	return TW_OK;
+}
+
+// the list of the voxels whose bits are set (bits: every word written), its total into the pinned stage
+int enqueue_change_list(tw_voxel_model *m, const ModelScratch &X, const ChangeOut &C, const ChangeKernels &K) {
+	tw_ctx *ctx = m->ctx;
+	ChangeScratch const &L = X.L;
+	int rc = launch_module_kernel(ctx, K.count, L.nchunks, CL_BLOCK, (const unsigned *)L.bits, L.nwords, L.sums); if (rc) return rc;
+	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(L.sums, L.nchunks, L.offsets, L.total);
+	TW_LAUNCH_CHECK(ctx);
+	if (C.capacity) {
+		rc = launch_module_kernel(ctx, K.emit, L.nchunks, CL_BLOCK, (const unsigned *)L.bits, L.nwords, (const unsigned long long *)L.offsets, (const float *)m->post,
+		                          (const unsigned char *)m->post_o, C.index, C.vals, C.outside, C.capacity);
+		if (rc) return rc;
+	}
+	TW_CUDA(ctx, cudaMemcpyAsync(&X.h_stage->nchanged, L.total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+	return TW_OK;
+}
+} // namespace
+
 extern "C" int tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out) {
+	return tw_voxel_model_edit_launch_ex(m, boxes, nboxes, values, out, nullptr);
+}
+
+extern "C" int tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out,
+                                             const tw_voxel_changes *ch)
+{
 	int rc = model_begin(m); if (rc) return rc;
 	tw_ctx *ctx = m->ctx;
 	if (nboxes && (!boxes || !values)) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_edit_launch: null boxes or values");
 	float *d_vt; uint32_t *d_ix;
 	rc = validate_blocks_out(ctx, out, &d_vt, &d_ix); if (rc) return rc;
 	tw_voxel_blocks_out const O = *out;
+	ChangeOut CO;
+	ChangeKernels K;
+	if (ch) {rc = validate_changes(ctx, ch, &CO); if (rc) return rc;}
 	tw_voxel_post_params const &P = m->P;
 	unsigned long long total = 0;
 	std::vector<twi_box> B(nboxes);
@@ -1234,26 +1292,45 @@ extern "C" int tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box 
 	bool const rm = (P.remove_unconnected > 0);
 	unsigned blocks = 0;
 	if (rm && total) {rc = flood_blocks(ctx, &blocks); if (rc) return rc;}
+	// the change list: only an edit with boxes can change a voxel, so without them the count stays the stage's 0
+	bool const list = ch && total;
+	if (list) {rc = change_kernels(ctx, &K); if (rc) return rc;}
 	ModelScratch X;
-	rc = model_scratch(m, nboxes, total, &X); if (rc) return rc;
+	rc = model_scratch(m, nboxes, total, &X, list); if (rc) return rc;
 	size_t const n = (size_t)P.nx*P.ny*P.nz;
 	memset(X.h_stage, 0, sizeof(twi_vmodel_stage));
 	if (nboxes) {memcpy(X.h_boxes, B.data(), nboxes*sizeof(twi_box)); memcpy(X.h_values, values, total*sizeof(float));}
-	return twi_launch_job(ctx, model_job(X, O), [&]() -> int {
+	return twi_launch_job(ctx, model_job(X, O, ch ? CO.nchanged : nullptr), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
 		if (total) {
 			TW_CUDA(ctx, cudaMemcpyAsync(X.boxes, X.h_boxes, nboxes*sizeof(twi_box), cudaMemcpyHostToDevice, ctx->stream));
 			TW_CUDA(ctx, cudaMemcpyAsync(X.values, X.h_values, total*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-			box_scatter_kernel<<<stream_grid(ctx, total), 256, 0, ctx->stream>>>(X.boxes, nboxes, X.values, total, P, m->zix, block_grid(m), m->raw, m->raw_o,
-			                                                                     rm ? nullptr : m->post, rm ? nullptr : m->post_o, m->mark);
-			TW_LAUNCH_CHECK(ctx);
+			if (list && !rm) { // the boxes' voxels set their bits one by one
+				TW_CUDA(ctx, cudaMemsetAsync(X.L.bits, 0, X.L.nwords*sizeof(unsigned), ctx->stream));
+				int const r = launch_module_kernel(ctx, K.box_bits, stream_grid(ctx, total), 256u, (const twi_box *)X.boxes, (unsigned)nboxes, (const float *)X.values, total,
+				                                   P, (const unsigned *)m->zix, block_grid(m), m->raw, m->raw_o, m->post, m->post_o, m->mark, X.L.bits);
+				if (r) return r;
+			}
+			else {
+				box_scatter_kernel<<<stream_grid(ctx, total), 256, 0, ctx->stream>>>(X.boxes, nboxes, X.values, total, P, m->zix, block_grid(m), m->raw, m->raw_o,
+				                                                                     rm ? nullptr : m->post, rm ? nullptr : m->post_o, m->mark);
+				TW_LAUNCH_CHECK(ctx);
+			}
 			if (rm) {
 				TW_CUDA(ctx, cudaMemcpyAsync(m->work, m->raw, n*sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
 				TW_CUDA(ctx, cudaMemcpyAsync(m->work_o, m->raw_o, n, cudaMemcpyDeviceToDevice, ctx->stream));
 				int const r = enqueue_remove_unconnected(ctx, blocks, m->work, m->work_o, &P, X.f0, X.f1, X.cnt, X.changed); if (r) return r;
-				diff_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(m->work, m->work_o, m->post, m->post_o, P, block_grid(m), m->mark, n);
-				TW_LAUNCH_CHECK(ctx);
+				if (list) {
+					int const r2 = launch_module_kernel(ctx, K.diff_bits, stream_grid(ctx, n), 256u, (const float *)m->work, (const unsigned char *)m->work_o, m->post, m->post_o,
+					                                    P, block_grid(m), m->mark, n, X.L.bits);
+					if (r2) return r2;
+				}
+				else {
+					diff_kernel<<<stream_grid(ctx, n), 256, 0, ctx->stream>>>(m->work, m->work_o, m->post, m->post_o, P, block_grid(m), m->mark, n);
+					TW_LAUNCH_CHECK(ctx);
+				}
 			}
+			if (list) {int const r = enqueue_change_list(m, X, CO, K); if (r) return r;}
 		}
 		if (m->nblocks) {list_marked_kernel<<<1, 1024, 0, ctx->stream>>>(m->mark, m->nblocks, m->marked); TW_LAUNCH_CHECK(ctx);}
 		return enqueue_block_meshes(m, m->marked, X, d_vt, O.vcapacity, d_ix, O.tcapacity);

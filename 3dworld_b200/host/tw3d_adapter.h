@@ -1180,7 +1180,10 @@ inline tiles_job voxel_build_async(voxel_grid_view const &v, tw_voxel_params con
 // block; edit_async writes boxes of new raw values (one box after another, each z fastest, then x, then y) and re-meshes only the blocks whose cubes read a
 // voxel that changed. Both return a tiles_job of the context; out (verts / indices in device or page-locked memory, the host block table and counts) is
 // complete once it is ready. The jobs cannot be cancelled. read() completes the pending job and copies the raw field, the field after remove_unconnected
-// and its flags. Not copyable; destroyed with the context's pending job completed.
+// and its flags. edit_async with a tw_voxel_changes also lists the voxels the edit changed (their index, and optionally their new value and flags after
+// remove_unconnected, ascending), so the engine can patch its voxel_manager field and outside flags once the job is ready instead of reading the grid back:
+// apply_changes does that for host vectors, and returns false when the list overflowed its capacity (read() the grid then). Not copyable; destroyed
+// with the context's pending job completed.
 class voxel_model {
 	tw_voxel_model *m = nullptr;
 	tw_ctx *c = nullptr;
@@ -1215,6 +1218,18 @@ public:
 	}
 	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out) {
 		return job_of(tw_voxel_model_edit_launch(m, boxes.data(), (uint32_t)boxes.size(), values, &out), "voxel_model::edit_async");
+	}
+	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out, tw_voxel_changes const &changes) {
+		return job_of(tw_voxel_model_edit_launch_ex(m, boxes.data(), (uint32_t)boxes.size(), values, &out, &changes), "voxel_model::edit_async");
+	}
+	// the list of a ready edit (host-addressable index / vals / outside, e.g. page-locked) into copies of the field and flags; false when it overflowed
+	static bool apply_changes(tw_voxel_changes const &ch, std::vector<float> *vals, std::vector<unsigned char> *outside) {
+		if (*ch.nchanged > ch.capacity) return false;
+		for (uint64_t k = 0; k < *ch.nchanged; ++k) {
+			if (vals && ch.vals) (*vals)[ch.index[k]] = ch.vals[k];
+			if (outside && ch.outside) (*outside)[ch.index[k]] = ch.outside[k];
+		}
+		return true;
 	}
 	void read(std::vector<float> *raw, std::vector<float> *vals, std::vector<unsigned char> *outside) {
 		if (raw) raw->resize(n);

@@ -755,6 +755,25 @@ TW_API int  tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_params
  * arguments, an empty box or one reaching outside the grid (no clipping), and the output errors of tw_voxel_model_build_launch; TW_ERR_STATE before the
  * model's first build. */
 TW_API int  tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out);
+/* The voxels an edit changed, so a copy of the field on the host can follow the model without reading the grid back. A voxel is listed when its value
+ * after remove_unconnected (bitwise) or its flags differ between the launch and the completion: exactly the voxels that mark blocks in step 4.
+ * After the completing poll *nchanged holds their count, and the first min(capacity, *nchanged) of them are written in ascending index order: the linear
+ * index z + (x + y*nx)*nz, and optionally the new value and flags. Patching a copy of tw_voxel_model_read's (vals, outside) taken before the edit with
+ * the list gives the read after it, byte for byte, whenever *nchanged <= capacity; otherwise the caller can fall back to a read. */
+typedef struct tw_voxel_changes {
+	uint32_t *index;     /* capacity entries, device or page-locked host memory (NULL with capacity 0) */
+	float    *vals;      /* optional, capacity entries: the field after remove_unconnected at index[i] */
+	uint8_t  *outside;   /* optional, capacity entries: its flags at index[i] */
+	uint64_t  capacity;
+	uint64_t *nchanged;  /* HOST, required: filled by the completing poll; may exceed capacity */
+} tw_voxel_changes;
+/* tw_voxel_model_edit_launch with the list of changed voxels (ch, optional; copied during the launch). tw_voxel_model_edit_launch(m, ...) is
+ * tw_voxel_model_edit_launch_ex(m, ..., NULL). The job keeps one bit per voxel in the context's scratch (n/8 bytes) while it runs. TW_ERR_ARG (nothing
+ * enqueued): the errors of tw_voxel_model_edit_launch, a missing nchanged, a capacity without index, vals or outside without index, and pageable buffers.
+ * The list's kernels are a module of their own, tw_voxel_changes.cubin, shipped beside the library and loaded by the first edit with a list: TW_ERR_CUDA
+ * (nothing enqueued) when it is missing or cannot be loaded. */
+TW_API int  tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out,
+                                          const tw_voxel_changes *ch);
 /* Synchronous, after completing the pending job: the raw field, the field after remove_unconnected and its flags (each optional; n elements, host or
  * device). TW_ERR_STATE before the model's first build. */
 TW_API int  tw_voxel_model_read(tw_voxel_model *m, float *raw, float *vals, uint8_t *outside);

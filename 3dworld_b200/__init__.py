@@ -247,7 +247,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_proc_gen_heightmap_launch", "tw_erode_launch", "tw_cancel", "tw_erode_launch_ex",
                "tw_update_heightmap", "tw_hmap_tiles_touched", "tw_voxel_mesh_welded", "tw_voxel_build_launch_ex",
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
-               "tw_voxel_model_edit_launch_ex",
+               "tw_voxel_model_edit_launch_ex", "tw_voxel_model_build_launch_on", "tw_voxel_model_edit_launch_on", "tw_voxel_model_read_launch",
                "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows",
                "tw_read_heightmap_launch", "tw_read_heightmap"]
 
@@ -366,6 +366,9 @@ def _load():
     L.tw_voxel_model_edit_launch.argtypes = [vp, vp, C.c_uint32, vp, C.POINTER(VoxelBlocksOut)]
     L.tw_voxel_model_read.argtypes = [vp, vp, vp, vp]
     L.tw_voxel_model_edit_launch_ex.argtypes = [vp, vp, C.c_uint32, vp, C.POINTER(VoxelBlocksOut), C.POINTER(VoxelChanges)]
+    L.tw_voxel_model_build_launch_on.argtypes = [vp] + L.tw_voxel_model_build_launch.argtypes
+    L.tw_voxel_model_edit_launch_on.argtypes = [vp] + L.tw_voxel_model_edit_launch_ex.argtypes
+    L.tw_voxel_model_read_launch.argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
@@ -667,6 +670,11 @@ class PointsJob:
 class HmapReadJob(PointsJob):
     """What Context.read_heightmap_launch returns: poll(wait) completes the job (the context's pending job) and returns out, or None while it runs
     (wait=False)."""
+
+
+class VoxelReadJob(PointsJob):
+    """What VoxelModel.read_launch returns: poll(wait) completes the job (the pending job of the Context it was launched on) and returns (raw, vals,
+    outside), or None while it runs (wait=False)."""
 
 
 class GenMeshJob:
@@ -1306,8 +1314,9 @@ class Context:
 
 class VoxelModel:
     """tw_voxel_model (include/tw3d.h): a voxel grid's raw field, outside flags and post-processed field kept on the device, meshed per block of bx x by
-    cube columns. build_launch and edit_launch are the context's asynchronous jobs, completed by Context.create_tiles_poll; they cannot be cancelled.
-    Context.close() destroys the model with the context."""
+    cube columns. build_launch, edit_launch and read_launch are asynchronous jobs, completed by create_tiles_poll of the Context they run on; they cannot be
+    cancelled. They run on the model's Context by default, or on ctx: its parent or a shared Context of that parent, so several strokes and reads are in
+    flight at once, ordered on the device in launch order. Context.close() destroys the model with the context."""
 
     def __init__(self, ctx, vpp, tables, zix_xy, bx, by):
         self.tables = tuple(np.ascontiguousarray(t, dt) for t, dt in zip(tables, (np.uint32, np.int32, np.uint32)))
@@ -1336,30 +1345,51 @@ class VoxelModel:
         except Exception:
             pass
 
-    def build_launch(self, fill=None, vals=None, rdata=None, verts=None, indices=None):
-        """tw_voxel_model_build_launch: the raw field from fill (VoxelParams) or vals (numpy or CUDA tensor, [ny, nx, nz] float32), its flags and
-        remove_unconnected, and every block's mesh into verts / indices (CUDA tensors or page-locked buffers, filled up to their sizes). Returns a
-        VoxelModelJob."""
+    def build_launch(self, fill=None, vals=None, rdata=None, verts=None, indices=None, ctx=None):
+        """tw_voxel_model_build_launch(_on): the raw field from fill (VoxelParams) or vals (numpy or CUDA tensor, [ny, nx, nz] float32), its flags and
+        remove_unconnected, and every block's mesh into verts / indices (CUDA tensors or page-locked buffers, filled up to their sizes). Runs on ctx (default
+        the model's Context). Returns a VoxelModelJob."""
+        c = self.ctx if ctx is None else ctx
         job = VoxelModelJob(self.nblocks)
         rd = None if rdata is None else np.ascontiguousarray(rdata, np.float32)
         out = job._out(verts, indices)
-        self.ctx._check(lib.tw_voxel_model_build_launch(self._h, C.byref(fill) if fill is not None else None, _ptr(rd), _ptr(vals), C.byref(out)))
-        self.ctx._tiles_job = (vals, verts, indices, job)
+        c._check(lib.tw_voxel_model_build_launch_on(c._h, self._h, C.byref(fill) if fill is not None else None, _ptr(rd), _ptr(vals), C.byref(out)))
+        c._tiles_job = (vals, verts, indices, job)
         return job
 
-    def edit_launch(self, boxes, values, verts=None, indices=None, changes=None):
-        """tw_voxel_model_edit_launch: boxes = (x, y, z, w, h, d) tuples, values = their new raw values one box after another, each in the grid's order
-        (z fastest, then x, then y), copied during the launch. Re-meshes the blocks the edit changed; returns a VoxelModelJob listing them.
+    def edit_launch(self, boxes, values, verts=None, indices=None, changes=None, ctx=None):
+        """tw_voxel_model_edit_launch(_on): boxes = (x, y, z, w, h, d) tuples, values = their new raw values one box after another, each in the grid's
+        order (z fastest, then x, then y), copied during the launch. Re-meshes the blocks the edit changed; returns a VoxelModelJob listing them.
         changes = (index, vals, outside) (tw_voxel_model_edit_launch_ex): buffers for the list of the voxels the edit changed, each None or a CUDA tensor /
-        page-locked buffer (uint32, float32, uint8) of the list's capacity; the job's nchanged and changes hold the list once it completes."""
+        page-locked buffer (uint32, float32, uint8) of the list's capacity; the job's nchanged and changes hold the list once it completes. Runs on ctx
+        (default the model's Context)."""
+        c = self.ctx if ctx is None else ctx
         b = (VoxelBox * max(len(boxes), 1))(*[VoxelBox(*[int(v) for v in t]) for t in boxes])
         vals = np.ascontiguousarray(values, np.float32).ravel()
         job = VoxelModelJob(self.nblocks)
         out = job._out(verts, indices)
         ch = None if changes is None else job._changes(changes)
-        self.ctx._check(lib.tw_voxel_model_edit_launch_ex(self._h, C.cast(b, C.c_void_p) if len(boxes) else None, len(boxes), _ptr(vals) if len(boxes) else None,
-                                                          C.byref(out), C.byref(ch) if ch is not None else None))
-        self.ctx._tiles_job = (verts, indices, changes, job)
+        c._check(lib.tw_voxel_model_edit_launch_on(c._h, self._h, C.cast(b, C.c_void_p) if len(boxes) else None, len(boxes), _ptr(vals) if len(boxes) else None,
+                                                   C.byref(out), C.byref(ch) if ch is not None else None))
+        c._tiles_job = (verts, indices, changes, job)
+        return job
+
+    def read_launch(self, boxes=None, raw=None, vals=None, outside=None, ctx=None):
+        """tw_voxel_model_read_launch: (raw field, field after remove_unconnected, its flags) as they are after every job launched on the model before
+        this call, on any Context, as a job on ctx (default the model's Context). boxes = None: the whole grid, as new [ny, nx, nz] numpy arrays by default;
+        else (x, y, z, w, h, d) tuples whose voxels are packed one box after another as edit_launch's values, as new flat numpy arrays by default. Each of
+        raw / vals / outside may be given (numpy, page-locked or CUDA, float32 / float32 / uint8 of that size) or False to skip it; a numpy destination is
+        staged in ctx's pinned staging, which grows to its size. Returns a VoxelReadJob."""
+        c = self.ctx if ctx is None else ctx
+        if boxes is None:
+            shape, b, nb = (int(self.vpp.ny), int(self.vpp.nx), int(self.vpp.nz)), None, 0
+        else:
+            shape, nb = (sum(int(t[3]) * int(t[4]) * int(t[5]) for t in boxes),), len(boxes)
+            b = (VoxelBox * max(nb, 1))(*[VoxelBox(*[int(v) for v in t]) for t in boxes])
+        outs = [np.empty(shape, dt) if a is None else (None if a is False else a) for a, dt in ((raw, np.float32), (vals, np.float32), (outside, np.uint8))]
+        c._check(lib.tw_voxel_model_read_launch(c._h, self._h, C.cast(b, C.c_void_p) if b is not None else None, nb, *[_ptr(a) for a in outs]))
+        job = VoxelReadJob(c, tuple(outs))
+        c._tiles_job = (b, outs, job)
         return job
 
     def read(self, raw=None, vals=None, outside=None):

@@ -842,8 +842,10 @@ extern "C" int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, co
 // A job meshes the blocks of a list with block_mesh_kernel: launch block k handles chunk k % chunks of the block in list slot k / chunks (chunks = MC_BLOCK-cube
 // chunks of the largest block), so the grid is sized for every block listed and the slots past the device-side count exit at once. Count, the two scans of
 // mesh_kernel (over slots x chunks, so a block's vertices and triangles are contiguous and in list order), emit, then the table of the listed blocks.
+// A job may run on any context of the model's family (model_begin); `ev` orders their device work on the model's memory, as a tile set's event does.
 struct tw_voxel_model {
-	tw_ctx *ctx = nullptr;
+	tw_ctx *ctx = nullptr;                   // the context that created it (it owns the model)
+	cudaEvent_t ev = nullptr;                // recorded after the last model job's device work, on whichever context launched it; the next one waits on it
 	tw_voxel_post_params P;
 	unsigned bx = 1, by = 1, nbx = 0, nblocks = 0, chunks = 0;
 	bool built = false, have_zix = false;
@@ -1005,8 +1007,7 @@ struct ModelScratch {
 	unsigned *cnt, *f0, *f1; unsigned long long *changed; MeshScratch S; tw_voxel_block_mesh *table; twi_box *boxes; float *values; ChangeScratch L;
 	twi_vmodel_stage *h_stage; tw_voxel_block_mesh *h_table; char *h_boxes, *h_values, *h_rdata;
 };
-int model_scratch(tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X, bool list = false) {
-	tw_ctx *ctx = m->ctx;
+int model_scratch(tw_ctx *ctx, const tw_voxel_model *m, size_t nboxes, size_t nvalues, ModelScratch *X, bool list = false) {
 	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz, ng = (size_t)m->nblocks*m->chunks;
 	X->f0 = X->f1 = nullptr;
 	ChangeScratch &L = X->L;
@@ -1039,8 +1040,7 @@ int validate_blocks_out(tw_ctx *ctx, const tw_voxel_blocks_out *o, float **d_vt,
 }
 
 // the meshes of the blocks in d_list, their table and the job's counts into the pinned stage
-int enqueue_block_meshes(tw_voxel_model *m, const unsigned *d_list, const ModelScratch &X, float *d_vt, uint64_t vcap, uint32_t *d_ix, uint64_t tcap) {
-	tw_ctx *ctx = m->ctx;
+int enqueue_block_meshes(tw_ctx *ctx, const tw_voxel_model *m, const unsigned *d_list, const ModelScratch &X, float *d_vt, uint64_t vcap, uint32_t *d_ix, uint64_t tcap) {
 	twi_vmodel_stage *const st = X.h_stage;
 	if (m->nblocks) {
 		unsigned const ng = m->nblocks*m->chunks;
@@ -1081,7 +1081,46 @@ twi_job model_job(const ModelScratch &X, const tw_voxel_blocks_out &o, uint64_t 
 	return j;
 }
 
-int model_begin(tw_voxel_model *m) {return m ? twi_begin(m->ctx) : TW_ERR_ARG;}
+// A model call on ctx: TW_ERR_ARG unless ctx and m are set and ctx is m's context, its parent or a shared context of that parent; then ctx's pending job is
+// completed (never another context's)
+int model_begin(tw_ctx *ctx, tw_voxel_model *m) {
+	if (!ctx || !m) return TW_ERR_ARG;
+	tw_ctx const *root = ctx->parent ? ctx->parent : ctx, *owner = m->ctx->parent ? m->ctx->parent : m->ctx;
+	if (root != owner || ctx->device != m->ctx->device) return tw_set_error(ctx, TW_ERR_ARG, "the voxel model belongs to another family of contexts");
+	return twi_begin(ctx);
+}
+
+// A model job on ctx: its device work waits for the model's earlier jobs on any context of the family, and the model's event is recorded behind it
+template <typename Enqueue> int launch_model_job(tw_ctx *ctx, tw_voxel_model *m, twi_job job, Enqueue &&enqueue) {
+	return twi_launch_job(ctx, std::move(job), [&]() -> int {
+		TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, m->ev, 0));
+		int const r = enqueue(); if (r) return r;
+		TW_CUDA(ctx, cudaEventRecord(m->ev, ctx->stream));
+		return TW_OK;
+	});
+}
+
+// The boxes of an edit or a read (TW_ERR_ARG for an empty one or one reaching outside the grid) with their values' offsets and overlaps; *total = their voxels
+int model_boxes(tw_ctx *ctx, const tw_voxel_post_params &P, const tw_voxel_box *boxes, uint32_t nboxes, std::vector<twi_box> &B, unsigned long long *total) {
+	*total = 0;
+	B.resize(nboxes);
+	for (uint32_t k = 0; k < nboxes; ++k) {
+		tw_voxel_box const &b = boxes[k];
+		if (b.w == 0 || b.h == 0 || b.d == 0) return tw_set_error(ctx, TW_ERR_ARG, "box %u is empty", k);
+		if (b.x >= P.nx || b.w > P.nx - b.x || b.y >= P.ny || b.h > P.ny - b.y || b.z >= P.nz || b.d > P.nz - b.z)
+			return tw_set_error(ctx, TW_ERR_ARG, "box %u reaches outside the %ux%ux%u grid", k, P.nx, P.ny, P.nz);
+		twi_box &t = B[k];
+		t.x = b.x; t.y = b.y; t.z = b.z; t.w = b.w; t.h = b.h; t.d = b.d; t.off = *total; t.later = 0; t.pad = 0;
+		*total += (unsigned long long)b.w*b.h*b.d;
+	}
+	for (uint32_t k = 0; k < nboxes; ++k) { // overlaps: the later box's value wins
+		for (uint32_t j = k + 1; j < nboxes && !B[k].later; ++j) {
+			const twi_box &a = B[k], &b = B[j];
+			B[k].later = (a.x < b.x + b.w && b.x < a.x + a.w && a.y < b.y + b.h && b.y < a.y + a.h && a.z < b.z + b.d && b.z < a.z + a.d);
+		}
+	}
+	return TW_OK;
+}
 
 } // namespace
 
@@ -1101,7 +1140,9 @@ extern "C" int tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp
 	unsigned const nbx = (ncx + bx - 1)/bx, nby = (ncy + by - 1)/by, nblocks = nbx*nby;
 	tw_voxel_model *m = new (std::nothrow) tw_voxel_model();
 	if (!m) return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");
-	try {ctx->models.push_back(m);} catch (...) {delete m; return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");}
+	cudaError_t const ee = cudaEventCreateWithFlags(&m->ev, cudaEventDisableTiming);
+	if (ee != cudaSuccess) {delete m; return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: event: %s", cudaGetErrorString(ee));}
+	try {ctx->models.push_back(m);} catch (...) {cudaEventDestroy(m->ev); delete m; return tw_set_error(ctx, TW_ERR_CUDA, "tw_voxel_model_create: out of host memory");}
 	m->ctx = ctx; m->P = P; m->bx = bx; m->by = by; m->nbx = nbx; m->nblocks = nblocks; m->chunks = (unsigned)(((size_t)bw*bh*P.nz + MC_BLOCK - 1)/MC_BLOCK);
 	m->have_zix = (zix_xy != nullptr);
 	auto layout = [&](twi_carve &c) {
@@ -1142,14 +1183,20 @@ extern "C" void tw_voxel_model_destroy(tw_voxel_model *m) {
 	tw_ctx *ctx = m->ctx;
 	cudaSetDevice(ctx->device);
 	twi_finish_pending(ctx); // the job may still read or write the model
+	cudaEventSynchronize(m->ev); // and so may a job on another context of the family
+	cudaEventDestroy(m->ev);
 	if (m->mem) cudaFree(m->mem);
 	for (size_t i = 0; i < ctx->models.size(); ++i) {if (ctx->models[i] == m) {ctx->models.erase(ctx->models.begin() + i); break;}}
 	delete m;
 }
 
 extern "C" int tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_params *fill, const float *rdata420, const float *vals, const tw_voxel_blocks_out *out) {
-	int rc = model_begin(m); if (rc) return rc;
-	tw_ctx *ctx = m->ctx;
+	return tw_voxel_model_build_launch_on(m ? m->ctx : nullptr, m, fill, rdata420, vals, out);
+}
+
+extern "C" int tw_voxel_model_build_launch_on(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_params *fill, const float *rdata420, const float *vals,
+                                              const tw_voxel_blocks_out *out) {
+	int rc = model_begin(ctx, m); if (rc) return rc;
 	if ((fill != nullptr) == (vals != nullptr)) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_build_launch: give either fill or vals");
 	float *d_vt; uint32_t *d_ix;
 	rc = validate_blocks_out(ctx, out, &d_vt, &d_ix); if (rc) return rc;
@@ -1168,11 +1215,11 @@ extern "C" int tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_par
 	unsigned blocks = 0;
 	if (rm) {rc = flood_blocks(ctx, &blocks); if (rc) return rc;}
 	ModelScratch X;
-	rc = model_scratch(m, 0, 0, &X); if (rc) return rc;
+	rc = model_scratch(ctx, m, 0, 0, &X); if (rc) return rc;
 	size_t const n = (size_t)P.nx*P.ny*P.nz;
 	memset(X.h_stage, 0, sizeof(twi_vmodel_stage));
 	m->built = true; // the job commits the model's state
-	return twi_launch_job(ctx, model_job(X, O), [&]() -> int {
+	return launch_model_job(ctx, m, model_job(X, O), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
 		if (fill) {int const r = twi_voxel_fill(ctx, &F, rdata420, m->raw, X.h_rdata); if (r) return r;}
 		else {TW_CUDA(ctx, cudaMemcpyAsync(m->raw, vals, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
@@ -1181,7 +1228,7 @@ extern "C" int tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_par
 		TW_CUDA(ctx, cudaMemcpyAsync(m->post, m->raw, n*sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
 		TW_CUDA(ctx, cudaMemcpyAsync(m->post_o, m->raw_o, n, cudaMemcpyDeviceToDevice, ctx->stream));
 		if (rm) {int const r = enqueue_remove_unconnected(ctx, blocks, m->post, m->post_o, &P, X.f0, X.f1, X.cnt, X.changed); if (r) return r;}
-		return enqueue_block_meshes(m, m->all, X, d_vt, O.vcapacity, d_ix, O.tcapacity);
+		return enqueue_block_meshes(ctx, m, m->all, X, d_vt, O.vcapacity, d_ix, O.tcapacity);
 	});
 }
 
@@ -1238,8 +1285,7 @@ int launch_module_kernel(tw_ctx *ctx, cudaKernel_t k, unsigned grid, unsigned bl
 }
 
 // the list of the voxels whose bits are set (bits: every word written), its total into the pinned stage
-int enqueue_change_list(tw_voxel_model *m, const ModelScratch &X, const ChangeOut &C, const ChangeKernels &K) {
-	tw_ctx *ctx = m->ctx;
+int enqueue_change_list(tw_ctx *ctx, const tw_voxel_model *m, const ModelScratch &X, const ChangeOut &C, const ChangeKernels &K) {
 	ChangeScratch const &L = X.L;
 	int rc = launch_module_kernel(ctx, K.count, L.nchunks, CL_BLOCK, (const unsigned *)L.bits, L.nwords, L.sums); if (rc) return rc;
 	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(L.sums, L.nchunks, L.offsets, L.total);
@@ -1261,8 +1307,13 @@ extern "C" int tw_voxel_model_edit_launch(tw_voxel_model *m, const tw_voxel_box 
 extern "C" int tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out,
                                              const tw_voxel_changes *ch)
 {
-	int rc = model_begin(m); if (rc) return rc;
-	tw_ctx *ctx = m->ctx;
+	return tw_voxel_model_edit_launch_on(m ? m->ctx : nullptr, m, boxes, nboxes, values, out, ch);
+}
+
+extern "C" int tw_voxel_model_edit_launch_on(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values,
+                                             const tw_voxel_blocks_out *out, const tw_voxel_changes *ch)
+{
+	int rc = model_begin(ctx, m); if (rc) return rc;
 	if (nboxes && (!boxes || !values)) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_edit_launch: null boxes or values");
 	float *d_vt; uint32_t *d_ix;
 	rc = validate_blocks_out(ctx, out, &d_vt, &d_ix); if (rc) return rc;
@@ -1272,22 +1323,8 @@ extern "C" int tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_b
 	if (ch) {rc = validate_changes(ctx, ch, &CO); if (rc) return rc;}
 	tw_voxel_post_params const &P = m->P;
 	unsigned long long total = 0;
-	std::vector<twi_box> B(nboxes);
-	for (uint32_t k = 0; k < nboxes; ++k) {
-		tw_voxel_box const &b = boxes[k];
-		if (b.w == 0 || b.h == 0 || b.d == 0) return tw_set_error(ctx, TW_ERR_ARG, "box %u is empty", k);
-		if (b.x >= P.nx || b.w > P.nx - b.x || b.y >= P.ny || b.h > P.ny - b.y || b.z >= P.nz || b.d > P.nz - b.z)
-			return tw_set_error(ctx, TW_ERR_ARG, "box %u reaches outside the %ux%ux%u grid", k, P.nx, P.ny, P.nz);
-		twi_box &t = B[k];
-		t.x = b.x; t.y = b.y; t.z = b.z; t.w = b.w; t.h = b.h; t.d = b.d; t.off = total; t.later = 0; t.pad = 0;
-		total += (unsigned long long)b.w*b.h*b.d;
-	}
-	for (uint32_t k = 0; k < nboxes; ++k) { // overlaps: the later box's value wins
-		for (uint32_t j = k + 1; j < nboxes && !B[k].later; ++j) {
-			const twi_box &a = B[k], &b = B[j];
-			B[k].later = (a.x < b.x + b.w && b.x < a.x + a.w && a.y < b.y + b.h && b.y < a.y + a.h && a.z < b.z + b.d && b.z < a.z + a.d);
-		}
-	}
+	std::vector<twi_box> B;
+	rc = model_boxes(ctx, P, boxes, nboxes, B, &total); if (rc) return rc;
 	if (!m->built) return tw_set_error(ctx, TW_ERR_STATE, "the voxel model has no field yet (tw_voxel_model_build_launch)");
 	bool const rm = (P.remove_unconnected > 0);
 	unsigned blocks = 0;
@@ -1296,11 +1333,11 @@ extern "C" int tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_b
 	bool const list = ch && total;
 	if (list) {rc = change_kernels(ctx, &K); if (rc) return rc;}
 	ModelScratch X;
-	rc = model_scratch(m, nboxes, total, &X, list); if (rc) return rc;
+	rc = model_scratch(ctx, m, nboxes, total, &X, list); if (rc) return rc;
 	size_t const n = (size_t)P.nx*P.ny*P.nz;
 	memset(X.h_stage, 0, sizeof(twi_vmodel_stage));
 	if (nboxes) {memcpy(X.h_boxes, B.data(), nboxes*sizeof(twi_box)); memcpy(X.h_values, values, total*sizeof(float));}
-	return twi_launch_job(ctx, model_job(X, O, ch ? CO.nchanged : nullptr), [&]() -> int {
+	return launch_model_job(ctx, m, model_job(X, O, ch ? CO.nchanged : nullptr), [&]() -> int {
 		TW_CUDA(ctx, cudaMemsetAsync(X.cnt, 0, 256, ctx->stream));
 		if (total) {
 			TW_CUDA(ctx, cudaMemcpyAsync(X.boxes, X.h_boxes, nboxes*sizeof(twi_box), cudaMemcpyHostToDevice, ctx->stream));
@@ -1330,21 +1367,63 @@ extern "C" int tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_b
 					TW_LAUNCH_CHECK(ctx);
 				}
 			}
-			if (list) {int const r = enqueue_change_list(m, X, CO, K); if (r) return r;}
+			if (list) {int const r = enqueue_change_list(ctx, m, X, CO, K); if (r) return r;}
 		}
 		if (m->nblocks) {list_marked_kernel<<<1, 1024, 0, ctx->stream>>>(m->mark, m->nblocks, m->marked); TW_LAUNCH_CHECK(ctx);}
-		return enqueue_block_meshes(m, m->marked, X, d_vt, O.vcapacity, d_ix, O.tcapacity);
+		return enqueue_block_meshes(ctx, m, m->marked, X, d_vt, O.vcapacity, d_ix, O.tcapacity);
 	});
 }
 
 extern "C" int tw_voxel_model_read(tw_voxel_model *m, float *raw, float *vals, uint8_t *outside) {
-	int rc = model_begin(m); if (rc) return rc;
-	tw_ctx *ctx = m->ctx;
+	tw_ctx *ctx = m ? m->ctx : nullptr;
+	int rc = model_begin(ctx, m); if (rc) return rc;
 	if (!m->built) return tw_set_error(ctx, TW_ERR_STATE, "the voxel model has no field yet (tw_voxel_model_build_launch)");
 	size_t const n = (size_t)m->P.nx*m->P.ny*m->P.nz;
+	TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, m->ev, 0)); // the model's jobs on the other contexts of the family
 	if (raw) {TW_CUDA(ctx, cudaMemcpyAsync(raw, m->raw, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	if (vals) {TW_CUDA(ctx, cudaMemcpyAsync(vals, m->post, n*sizeof(float), cudaMemcpyDefault, ctx->stream));}
 	if (outside) {TW_CUDA(ctx, cudaMemcpyAsync(outside, m->post_o, n, cudaMemcpyDefault, ctx->stream));}
 	TW_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return TW_OK;
+}
+
+// The read as a job: each requested array is copied from the model straight into device or page-locked memory, or into the launching context's pinned
+// staging for a pageable destination, which the completing poll copies out. A box is one strided 3-D copy per array: rows of d voxels along z, w rows per
+// slice (x), h slices (y), packed as the edit packs its values.
+extern "C" int tw_voxel_model_read_launch(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, float *raw, float *vals, uint8_t *outside) {
+	int rc = model_begin(ctx, m); if (rc) return rc;
+	if (nboxes && !boxes) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_read_launch: null boxes with nboxes > 0");
+	tw_voxel_post_params const &P = m->P;
+	unsigned long long total = 0;
+	std::vector<twi_box> B;
+	rc = model_boxes(ctx, P, boxes, nboxes, B, &total); if (rc) return rc;
+	if (!m->built) return tw_set_error(ctx, TW_ERR_STATE, "the voxel model has no field yet (tw_voxel_model_build_launch)");
+	size_t const n = boxes ? (size_t)total : (size_t)P.nx*P.ny*P.nz;
+	struct Arr {void *user; const void *src; size_t es; char *h;};
+	Arr A[3] = {{raw, m->raw, sizeof(float), nullptr}, {vals, m->post, sizeof(float), nullptr}, {outside, m->post_o, 1, nullptr}};
+	bool stage[3];
+	for (int k = 0; k < 3; ++k) {stage[k] = A[k].user && n && !device_view(A[k].user);}
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {for (int k = 0; k < 3; ++k) {A[k].h = stage[k] ? c.take<char>(n*A[k].es) : nullptr;}}); if (rc) return rc;
+	twi_job pending;
+	pending.complete = [A0 = A[0], A1 = A[1], A2 = A[2], n](tw_ctx *) -> int {
+		for (Arr const &a : {A0, A1, A2}) {if (a.h) memcpy(a.user, a.h, n*a.es);}
+		return TW_OK;
+	};
+	return launch_model_job(ctx, m, std::move(pending), [&]() -> int {
+		for (Arr const &a : A) {
+			if (!a.user || !n) continue;
+			char *dst = a.h ? a.h : (char *)a.user;
+			if (!boxes) {TW_CUDA(ctx, cudaMemcpyAsync(dst, a.src, n*a.es, cudaMemcpyDefault, ctx->stream)); continue;}
+			for (twi_box const &b : B) {
+				cudaMemcpy3DParms q = {};
+				q.srcPtr = make_cudaPitchedPtr(const_cast<void *>(a.src), (size_t)P.nz*a.es, P.nz, P.nx);
+				q.srcPos = make_cudaPos((size_t)b.z*a.es, b.x, b.y);
+				q.dstPtr = make_cudaPitchedPtr(dst + b.off*a.es, (size_t)b.d*a.es, b.d, b.w);
+				q.extent = make_cudaExtent((size_t)b.d*a.es, b.w, b.h);
+				q.kind = cudaMemcpyDefault;
+				TW_CUDA(ctx, cudaMemcpy3DAsync(&q, ctx->stream));
+			}
+		}
+		return TW_OK;
+	});
 }

@@ -616,6 +616,7 @@ struct gen_mesh_result {float zmin, zmax, zmax_est, zbottom, ztop, water_plane_z
 
 class tile_job_pool {
 	friend class tile_set; // its frame launches take a slot too
+	friend class voxel_model; // and so do a voxel model's jobs
 	struct slot {tw_ctx *c = nullptr; std::atomic<uint64_t> jobs{0}; uint64_t launched = 0;};
 	std::vector<std::unique_ptr<slot>> slots; // stable addresses: a tiles_job keeps a pointer to its slot's launch count
 	uint64_t clock = 0;
@@ -1178,21 +1179,28 @@ inline tiles_job voxel_build_async(voxel_grid_view const &v, tw_voxel_params con
 // A voxel model edited with brushes (src/voxels.cpp:2139-2245) and meshed per block, as create_block keeps one mesh and vertex cache per block (:1077-1108),
 // kept on the device by the thread's context (tw_voxel_model_*). build_async takes the field from fill or from vals (v.data is not read) and meshes every
 // block; edit_async writes boxes of new raw values (one box after another, each z fastest, then x, then y) and re-meshes only the blocks whose cubes read a
-// voxel that changed. Both return a tiles_job of the context; out (verts / indices in device or page-locked memory, the host block table and counts) is
-// complete once it is ready. The jobs cannot be cancelled. read() completes the pending job and copies the raw field, the field after remove_unconnected
-// and its flags. edit_async with a tw_voxel_changes also lists the voxels the edit changed (their index, and optionally their new value and flags after
+// voxel that changed. Both return a tiles_job; out (verts / indices in device or page-locked memory, the host block table and counts) is complete once it
+// is ready. The jobs cannot be cancelled. read() completes the pending job and copies the raw field, the field after remove_unconnected and its flags.
+// edit_async with a tw_voxel_changes also lists the voxels the edit changed (their index, and optionally their new value and flags after
 // remove_unconnected, ascending), so the engine can patch its voxel_manager field and outside flags once the job is ready instead of reading the grid back:
-// apply_changes does that for host vectors, and returns false when the list overflowed its capacity (read() the grid then). Not copyable; destroyed
-// with the context's pending job completed.
+// apply_changes does that for host vectors, and returns false when the list overflowed its capacity (read_async() the grid then). read_async() is the read
+// as a job: the whole grid (no boxes) or the boxes' voxels packed as edit_async's values, into device, page-locked or pageable memory, as the model is after
+// every job launched before it. With a `pool` (a tile_job_pool of this thread's context) each job runs on a free slot instead of the thread's context, so a
+// stroke never waits for the previous one or for the frame's tile jobs; the model orders its jobs on the device in launch order. Not copyable; destroyed
+// with the context's pending job completed and the model's jobs on pool slots done.
 class voxel_model {
 	tw_voxel_model *m = nullptr;
 	tw_ctx *c = nullptr;
 	size_t n = 0;
-	tiles_job job_of(int rc, const char *what) {
-		std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
-		uint64_t const number = ++jobs;
-		if (rc != TW_OK) {--jobs; detail::fail(rc, what, c);}
-		return tiles_job(c, &jobs, number);
+	// launch(lc) on this model's context, or on a slot of pool
+	template <typename Launch> tiles_job job_on(tile_job_pool *pool, const char *what, Launch &&launch) {
+		tw_ctx *lc = c;
+		std::atomic<uint64_t> *jobs = &detail::tls().tile_jobs;
+		if (pool) {tile_job_pool::slot &sl = pool->next(); lc = sl.c; jobs = &sl.jobs;}
+		uint64_t const number = ++*jobs;
+		int const rc = launch(lc);
+		if (rc != TW_OK) {--*jobs; detail::fail(rc, what, lc);}
+		return tiles_job(lc, jobs, number);
 	}
 public:
 	voxel_model(voxel_grid_view const &v, float isolevel, bool invert, bool make_closed_surface, unsigned remove_unconnected, bool keep_at_edge,
@@ -1213,14 +1221,26 @@ public:
 	~voxel_model() {tw_voxel_model_destroy(m);}
 	voxel_model(voxel_model const &) = delete;
 	voxel_model &operator=(voxel_model const &) = delete;
-	tiles_job build_async(tw_voxel_params const *fill, const float *vals, tw_voxel_blocks_out const &out) {
-		return job_of(tw_voxel_model_build_launch(m, fill, nullptr, vals, &out), "voxel_model::build_async");
+	tiles_job build_async(tw_voxel_params const *fill, const float *vals, tw_voxel_blocks_out const &out, tile_job_pool *pool = nullptr) {
+		return job_on(pool, "voxel_model::build_async", [&](tw_ctx *lc) {return tw_voxel_model_build_launch_on(lc, m, fill, nullptr, vals, &out);});
 	}
-	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out) {
-		return job_of(tw_voxel_model_edit_launch(m, boxes.data(), (uint32_t)boxes.size(), values, &out), "voxel_model::edit_async");
+	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out, tile_job_pool *pool = nullptr) {
+		return job_on(pool, "voxel_model::edit_async", [&](tw_ctx *lc) {
+			return tw_voxel_model_edit_launch_on(lc, m, boxes.data(), (uint32_t)boxes.size(), values, &out, nullptr);
+		});
 	}
-	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out, tw_voxel_changes const &changes) {
-		return job_of(tw_voxel_model_edit_launch_ex(m, boxes.data(), (uint32_t)boxes.size(), values, &out, &changes), "voxel_model::edit_async");
+	tiles_job edit_async(std::vector<tw_voxel_box> const &boxes, const float *values, tw_voxel_blocks_out const &out, tw_voxel_changes const &changes,
+	                     tile_job_pool *pool = nullptr) {
+		return job_on(pool, "voxel_model::edit_async", [&](tw_ctx *lc) {
+			return tw_voxel_model_edit_launch_on(lc, m, boxes.data(), (uint32_t)boxes.size(), values, &out, &changes);
+		});
+	}
+	// raw / vals / outside (each optional): the whole grid's n elements when boxes is empty, else the boxes' voxels one box after another
+	// (page-locked for whole grids: a pageable destination grows the slot's pinned staging to the read's size, once, with a blocking allocation)
+	tiles_job read_async(std::vector<tw_voxel_box> const &boxes, float *raw, float *vals, unsigned char *outside, tile_job_pool *pool = nullptr) {
+		return job_on(pool, "voxel_model::read_async", [&](tw_ctx *lc) {
+			return tw_voxel_model_read_launch(lc, m, boxes.empty() ? nullptr : boxes.data(), (uint32_t)boxes.size(), raw, vals, outside);
+		});
 	}
 	// the list of a ready edit (host-addressable index / vals / outside, e.g. page-locked) into copies of the field and flags; false when it overflowed
 	static bool apply_changes(tw_voxel_changes const &ch, std::vector<float> *vals, std::vector<unsigned char> *outside) {

@@ -728,20 +728,32 @@ typedef struct tw_voxel_model tw_voxel_model;
  * the raw field (as the caller gave it or the fill made it), its outside flags, the field and flags after remove_unconnected, and a working copy of those
  * for the edit's comparison: 15 bytes per voxel (about 2 GB at 512^3), plus the blocks' words. While a job runs, the context's scratch also holds the
  * flood's frontiers (8 bytes per voxel with remove_unconnected > 0) and the mesh's per-cube words (4 bytes per cube of the listed blocks' worst case).
- * A model belongs to the context that created it: its jobs are that context's pending job (tw_create_tiles_poll completes them), every model call first
- * completes the pending job, and tw_destroy(ctx) destroys the context's live models first (their handles are invalid after).
+ * A model belongs to the context that created it: tw_destroy(ctx) destroys the context's live models before its shared contexts (their handles are invalid
+ * after). Its jobs run on that context or, through the _on / read_launch calls, on any context of its family - the parent or a shared context of that
+ * parent - so several brush strokes and reads are in flight at once:
+ * - A model job is the pending job of the context it was launched on (tw_create_tiles_poll on that context completes it); the launch first completes that
+ *   context's earlier job and never waits for a job of another context. Its scratch, pinned staging and kernel launches are the launching context's.
+ * - Model state is committed at launch, in launch order. On the device, every model job waits for the model's earlier jobs on any context before it
+ *   touches the model, so each job sees exactly the jobs launched before it. tw_voxel_model_read and tw_voxel_model_destroy also wait for them.
+ * - Threads: one thread at a time across a model and every context it is used on.
  * Model jobs commit the model's state at launch, so they cannot be cancelled: tw_cancel returns TW_ERR_STATE, as for tile-set jobs.
  * TW_ERR_ARG (nothing allocated): NULL arguments, bx or by == 0, an empty grid or 2^32 voxels or more, 3*(bx+1)*(by+1)*nz >= 2^32 with the block sizes
  * clamped to the grid (the block's indices are 32-bit). */
 TW_API int  tw_voxel_model_create(tw_ctx *ctx, const tw_voxel_post_params *vp, const uint32_t *edge_table256, const int32_t *tri_table256x16,
                                   const uint32_t *edge_to_vals12x2, const uint32_t *zix_xy, uint32_t bx, uint32_t by, tw_voxel_model **out);
-/* Completes the context's pending job, then frees the model. */
+/* Completes the model's context's pending job and waits for the device work of the model's jobs on every other context, then frees the model. Those jobs
+ * stay the pending jobs of their contexts; their polls still complete them (with TW_OK). */
 TW_API void tw_voxel_model_destroy(tw_voxel_model *m);
 /* The build as the context's asynchronous job: the raw field from fill (as tw_voxel_fill(fill, rdata420)) or from vals (n floats, host or device, read
  * during the job), then tw_voxel_outside, tw_voxel_remove_unconnected, and the mesh of every block, listed in order. The model keeps the results. Rules and
  * lifetimes as tw_voxel_build_launch. TW_ERR_ARG (nothing enqueued): NULL arguments, both or neither of fill and vals, a fill grid that differs, a capacity
  * without its buffer, pageable verts / indices; TW_ERR_STATE where tw_voxel_fill returns it. */
 TW_API int  tw_voxel_model_build_launch(tw_voxel_model *m, const tw_voxel_params *fill, const float *rdata420, const float *vals, const tw_voxel_blocks_out *out);
+/* tw_voxel_model_build_launch as the pending job of ctx: the model's context, its parent or a shared context of that parent (see the model rules above).
+ * tw_voxel_model_build_launch(m, ...) is tw_voxel_model_build_launch_on(m's context, m, ...). TW_ERR_ARG (nothing enqueued) also for a NULL ctx or model and
+ * a context of another family or device. */
+TW_API int  tw_voxel_model_build_launch_on(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_params *fill, const float *rdata420, const float *vals,
+                                           const tw_voxel_blocks_out *out);
 /* An edit as the context's asynchronous job, without the host reading anything back before the end:
  *   1. each box's new raw values (values: the boxes' voxels one box after another, each packed in the grid's order - z fastest, then x, then y; host
  *      memory, copied during the launch) go into the raw field; where boxes overlap, the later box's value wins;
@@ -774,9 +786,23 @@ typedef struct tw_voxel_changes {
  * (nothing enqueued) when it is missing or cannot be loaded. */
 TW_API int  tw_voxel_model_edit_launch_ex(tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values, const tw_voxel_blocks_out *out,
                                           const tw_voxel_changes *ch);
-/* Synchronous, after completing the pending job: the raw field, the field after remove_unconnected and its flags (each optional; n elements, host or
- * device). TW_ERR_STATE before the model's first build. */
+/* tw_voxel_model_edit_launch_ex as the pending job of ctx, a context of the model's family (as tw_voxel_model_build_launch_on). tw_voxel_model_edit_launch_ex(m,
+ * ...) is tw_voxel_model_edit_launch_on(m's context, m, ...). The change list's bits are in ctx's scratch. */
+TW_API int  tw_voxel_model_edit_launch_on(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, const float *values,
+                                          const tw_voxel_blocks_out *out, const tw_voxel_changes *ch);
+/* Synchronous, after completing the pending job of the model's context and waiting for the model's jobs on the other contexts: the raw field, the field
+ * after remove_unconnected and its flags (each optional; n elements, host or device). TW_ERR_STATE before the model's first build. */
 TW_API int  tw_voxel_model_read(tw_voxel_model *m, float *raw, float *vals, uint8_t *outside);
+/* The read as the pending job of ctx, a context of the model's family: what the model holds after every model job launched before this call and none
+ * launched after it, on any context. raw (the raw field), vals (the field after remove_unconnected) and outside (its flags) are each optional, in device,
+ * page-locked or pageable host memory; pageable ones are filled by the completing poll, the others by the device before it. A pageable destination
+ * is staged in the launching context's pinned staging, which grows to the read's size (671 MB for a whole 512^3 read of all three arrays) with a blocking
+ * cudaMallocHost the first time and stays allocated for the context's life: read whole grids into page-locked memory (cudaHostRegister the engine's arrays). boxes == NULL (with nboxes 0):
+ * the whole grid, n elements in the grid's order; otherwise the boxes' voxels one box after another, each packed as tw_voxel_model_edit_launch's values
+ * (z fastest, then x, then y) - one strided copy per box and array, no kernel. The boxes are read during the launch. TW_ERR_ARG (nothing enqueued): a NULL
+ * ctx or model, a context of another family or device, NULL boxes with nboxes > 0, an empty box or one reaching outside the grid; TW_ERR_STATE before the
+ * model's first build has been launched. */
+TW_API int  tw_voxel_model_read_launch(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, float *raw, float *vals, uint8_t *outside);
 
 /* ---- mesh shadows of tiles (SURVEY.md 8f row N4): calc_mesh_shadows (src/visibility.cpp:411-517) for a batch of tiles with the neighbour chaining of
  * tile_t::calc_shadows_for_light (src/tiled_mesh.cpp:664-692) ---- */

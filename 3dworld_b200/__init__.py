@@ -249,7 +249,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
                "tw_voxel_model_edit_launch_ex", "tw_voxel_model_build_launch_on", "tw_voxel_model_edit_launch_on", "tw_voxel_model_read_launch",
                "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows",
-               "tw_read_heightmap_launch", "tw_read_heightmap"]
+               "tw_read_heightmap_launch", "tw_read_heightmap", "tw_voxel_build_batch_launch"]
 
 
 def _load():
@@ -359,6 +359,7 @@ def _load():
     L.tw_voxel_build_launch.argtypes = [vp, C.POINTER(VoxelBuild)]
     L.tw_voxel_mesh_welded.argtypes = [vp, vp, vp, C.POINTER(VoxelPostParams), vp, vp, vp, C.POINTER(VoxelMesh)]
     L.tw_voxel_build_launch_ex.argtypes = [vp, C.POINTER(VoxelBuild), C.POINTER(VoxelMesh)]
+    L.tw_voxel_build_batch_launch.argtypes = [vp, C.POINTER(VoxelBuild), C.POINTER(VoxelMesh), C.c_uint32]
     L.tw_voxel_model_create.argtypes = [vp, C.POINTER(VoxelPostParams), vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
     L.tw_voxel_model_destroy.argtypes = [vp]
     L.tw_voxel_model_destroy.restype = None
@@ -588,6 +589,30 @@ class VoxelBuildJob:
     @property
     def changed(self):
         return int(self._changed.value)
+
+
+class VoxelBuildBatchJob:
+    """The host results of Context.voxel_build_batch_launch, filled by the poll that completes the job: per grid, the welded mesh's nverts / ntris and the
+    voxels remove_unconnected flipped (changed)."""
+
+    def __init__(self, n):
+        self._counts = (C.c_uint64 * (3 * n))()
+        self.n = n
+
+    def _col(self, k):
+        return [int(self._counts[3 * i + k]) for i in range(self.n)]
+
+    @property
+    def nverts(self):
+        return self._col(0)
+
+    @property
+    def ntris(self):
+        return self._col(1)
+
+    @property
+    def changed(self):
+        return self._col(2)
 
 
 class VoxelModelJob:
@@ -1270,6 +1295,32 @@ class Context:
                           C.cast(C.pointer(job._mesh_ntris), C.c_void_p))
             self._check(lib.tw_voxel_build_launch_ex(self._h, C.byref(b), C.byref(m)))
         self._tiles_job = (keep, tabs, z, job)
+        return job
+
+    def voxel_build_batch_launch(self, grids, tables):
+        """tw_voxel_build_batch_launch: many small grids (nx*ny*nz <= 2^18 each) built in one asynchronous job, each exactly as voxel_build_launch with
+        mesh=(verts, indices) and soup=False would build it alone; create_tiles_poll completes it. grids: a list of dicts with the keys of voxel_build_launch -
+        vpp (required), vals, outside, fill, rdata, zix_xy - and mesh = (verts, indices) (each a CUDA tensor, a page-locked buffer or None). tables (edge_table,
+        tri_table, edge_to_vals) are shared by every grid. Returns a VoxelBuildBatchJob whose per-grid nverts / ntris / changed are valid once the job is
+        complete. The outputs and device inputs stay referenced here until then."""
+        n = len(grids)
+        job = VoxelBuildBatchJob(max(n, 1))
+        tabs = tuple(t if hasattr(t, "data_ptr") else np.ascontiguousarray(t, dt) for t, dt in zip(tables, (np.uint32, np.int32, np.uint32)))
+        bs, ms, keep = (VoxelBuild * max(n, 1))(), (VoxelMesh * max(n, 1))(), [tabs]
+        size = lambda a: 0 if a is None else (int(a.numel()) if hasattr(a, "numel") else int(a.size)) // 3
+        base = C.addressof(job._counts)
+        for i, g in enumerate(grids):
+            z = g.get("zix_xy")
+            z = None if z is None else (z if hasattr(z, "data_ptr") else np.ascontiguousarray(z, np.uint32))
+            rd = None if g.get("rdata") is None else np.ascontiguousarray(g["rdata"], np.float32)
+            vpp, fill = g["vpp"], g.get("fill")
+            verts, indices = g.get("mesh", (None, None))
+            keep.append((g, z, rd))
+            bs[i] = VoxelBuild(C.cast(C.pointer(fill), C.c_void_p) if fill is not None else None, _ptr(rd), C.cast(C.pointer(vpp), C.c_void_p), _ptr(z),
+                               _ptr(tabs[0]), _ptr(tabs[1]), _ptr(tabs[2]), _ptr(g.get("vals")), _ptr(g.get("outside")), None, 0, None, base + (24 * i + 16))
+            ms[i] = VoxelMesh(_ptr(verts), size(verts), _ptr(indices), size(indices), base + 24 * i, base + (24 * i + 8))
+        self._check(lib.tw_voxel_build_batch_launch(self._h, bs, ms, n))
+        self._tiles_job = (keep, job)
         return job
 
     def from_floats_u16(self, vals, val_mult, val_add, out=None):

@@ -12,17 +12,15 @@
 // All fp32 arithmetic is the reference's (separate multiply and add: the TU is compiled with -fmad=false), std::min/max argument order kept.
 #include "tw_internal.h"
 #include "tw_voxel_edit.cuh"
+#include "tw_voxel_mc.cuh"
+#include "tw_voxel_batch.h"
 #include <dlfcn.h>
+#include <algorithm>
 #include <mutex>
 #include <string>
 #include <vector>
 
 namespace {
-
-constexpr float VOX_TOLERANCE = 1.0E-12f; // TOLERANCE, src/3DWorld.h:50
-
-__device__ __forceinline__ float smin(float a, float b) {return (b < a) ? b : a;} // std::min
-__device__ __forceinline__ float smax(float a, float b) {return (a < b) ? b : a;} // std::max
 
 __global__ void outside_kernel(const float *__restrict__ vals, tw_voxel_post_params P, const unsigned *__restrict__ zix_xy, unsigned char *__restrict__ outside, size_t n) {
 	size_t const stride = (size_t)gridDim.x*blockDim.x;
@@ -30,11 +28,7 @@ __global__ void outside_kernel(const float *__restrict__ vals, tw_voxel_post_par
 		unsigned const z = (unsigned)(i % P.nz);
 		size_t const xy = i / P.nz;
 		unsigned const x = (unsigned)(xy % P.nx), y = (unsigned)(xy / P.nx);
-		bool const on_edge = (P.make_closed_surface && ((x == 0 || x == P.nx-1) || (y == 0 || y == P.ny-1) || (z == 0 || z == P.nz-1)));
-		float const val = __ldg(vals + i);
-		unsigned char ival = on_edge ? (unsigned char)TW_VOX_ON_EDGE : (unsigned char)((val == P.isolevel) ? 1 : (((val < P.isolevel) != (P.invert != 0)) ? 1 : 0)); // val_is_outside
-		if (zix_xy && z < __ldg(zix_xy + (size_t)y*P.nx + x)) {ival |= TW_VOX_UNDER_MESH;}
-		outside[i] = ival;
+		outside[i] = outside_flag(vals, i, x, y, z, P, zix_xy);
 	}
 }
 
@@ -158,8 +152,6 @@ __global__ void flood_finish_kernel(float *__restrict__ vals, unsigned char *__r
 }
 
 // ---- marching cubes ----
-struct McTables {const unsigned *edge_table; const int *tri_table; const unsigned *edge_to_vals;};
-constexpr int MC_BLOCK = 1024;
 // The three tables in one device region of MC_TAB_BYTES: [edge_table 1024 B | tri_table 16384 B | edge_to_vals 96 B]
 constexpr size_t MC_TAB_OFF[3] = {0, 1024, 1024 + 16384}, MC_TAB_LEN[3] = {1024, 16384, 96}, MC_TAB_BYTES = MC_TAB_OFF[2] + MC_TAB_LEN[2];
 McTables mc_tables(const void *tab) {
@@ -175,15 +167,6 @@ int mc_tables_upload(tw_ctx *ctx, void *tab, const uint32_t *edge_table256, cons
 		TW_CUDA(ctx, cudaMemcpyAsync((char *)tab + MC_TAB_OFF[k], src[k], MC_TAB_LEN[k], cudaMemcpyDefault, ctx->stream));
 	}
 	return TW_OK;
-}
-
-__device__ __forceinline__ void interpolate_pt(float isolevel, const float *pt1, const float *pt2, float val1, float val2, float *pt) { // src/voxels.cpp:485-493
-	if (fabsf(isolevel - val1) < VOX_TOLERANCE) {pt[0] = pt1[0]; pt[1] = pt1[1]; pt[2] = pt1[2]; return;}
-	if (fabsf(isolevel - val2) < VOX_TOLERANCE) {pt[0] = pt2[0]; pt[1] = pt2[1]; pt[2] = pt2[2]; return;}
-	if (fabsf(val1     - val2) < VOX_TOLERANCE) {pt[0] = pt1[0]; pt[1] = pt1[1]; pt[2] = pt1[2]; return;}
-	float const mu = smax(0.0f, smin(1.0f, __fdiv_rn(isolevel - val1, val2 - val1))); // CLIP_TO_01
-#pragma unroll
-	for (int i = 0; i < 3; ++i) {pt[i] = pt1[i] + mu*(pt2[i] - pt1[i]);}
 }
 
 // add_triangles_for_voxel(x, y, z) at lod 0 (src/voxels.cpp:495-566): returns the number of valid triangles, written to tri[k][9] when EMIT
@@ -314,124 +297,6 @@ scan_blocks_kernel(const unsigned *__restrict__ sums, unsigned nblocks, unsigned
 // reference creates vertices in owner order and, per owner, in local edge order, so a vertex's index is the owned-vertex prefix of its owner plus its rank
 // among the owner's owned edges. mesh_kernel<false> counts per cube and stores word[c] = (block-exclusive owned-vertex prefix << 16) | owned-edge mask;
 // mesh_kernel<true> reads the words of the owners it references. Per block <= 12*1024 vertices and 5*1024 triangles: both prefixes fit 16 bits.
-
-// The cube's 12 edges as grid edges, from edge_to_vals: s_edge[i] = axis | ox << 2 | oy << 3 | oz << 4 (axis 0 x, 1 y, 2 z; o = the edge's low corner in
-// the cube); s_look[4*axis + 2*o1 + o2] = the local edge along axis whose low corner is at o1, o2 on the axis' other two (perp() order).
-// edge_to_vals must name each edge of the cube once (Bourke's table does).
-__device__ __forceinline__ void perp(unsigned a, unsigned &p1, unsigned &p2) {p1 = (a == 1) ? 0u : 1u; p2 = (a == 2) ? 0u : 2u;} // y > x > z in index weight
-__device__ void mesh_edge_tables(const unsigned *__restrict__ etv, unsigned char *s_edge, unsigned char *s_look) {
-	unsigned const t = threadIdx.x;
-	if (t < 12) {
-		unsigned c[2][3];
-		for (unsigned d = 0; d < 2; ++d) {
-			unsigned const e = __ldg(etv + 2*t + d), yhi = (e & 2) >> 1;
-			c[d][0] = yhi ^ (e & 1); c[d][1] = yhi; c[d][2] = (e >> 2) & 1;
-		}
-		unsigned const a = (c[0][0] != c[1][0]) ? 0u : ((c[0][1] != c[1][1]) ? 1u : 2u);
-		s_edge[t] = (unsigned char)(a | (min(c[0][0], c[1][0]) << 2) | (min(c[0][1], c[1][1]) << 3) | (min(c[0][2], c[1][2]) << 4));
-	}
-	__syncthreads();
-	if (t < 12) {
-		unsigned char look = 0;
-		for (unsigned i = 0; i < 12; ++i) {
-			unsigned const e = s_edge[i], a = e & 3;
-			unsigned p1, p2; perp(a, p1, p2);
-			if (4*a + 2*((e >> (2 + p1)) & 1) + ((e >> (2 + p2)) & 1) == t) {look = (unsigned char)i;}
-		}
-		s_look[t] = look;
-	}
-	__syncthreads();
-}
-
-// A block of a voxel model (tw_voxel_model): the cubes x in [x0, x1), y in [y0, y1), every z. A cube's index within it is ((y - y0)*(x1 - x0) + x - x0)*nz + z.
-struct CubeRange {unsigned x0, x1, y0, y1;};
-
-// cube (c[0], c[1], c[2]) makes triangles: inside the grid (with BLK: inside R), not in the last layer of an axis, and not skip_under_mesh with its 4 low
-// corners under the mesh
-template<bool BLK = false>
-__device__ __forceinline__ bool cube_valid(const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const int *c, const CubeRange &R = CubeRange()) {
-	if (c[0] < 0 || c[1] < 0 || c[2] < 0 || (unsigned)c[0] + 1 >= P.nx || (unsigned)c[1] + 1 >= P.ny || (unsigned)c[2] + 1 >= P.nz) return false;
-	if (BLK && ((unsigned)c[0] < R.x0 || (unsigned)c[0] >= R.x1 || (unsigned)c[1] < R.y0 || (unsigned)c[1] >= R.y1)) return false;
-	if (!P.skip_under_mesh) return true;
-	for (unsigned k = 0; k < 4; ++k) {
-		size_t const ix = (unsigned)c[2] + ((size_t)(c[0] + (k & 1)) + (size_t)(c[1] + (k >> 1))*P.nx)*P.nz;
-		if (!(__ldg(outside + ix) & TW_VOX_UNDER_MESH)) return true;
-	}
-	return false;
-}
-
-// One cube of the welded mesh: the welded position of each of its crossing edges (vlist), each edge's owner (linear index) and local edge there (own, oj),
-// the edges it owns (mask) and the triangles whose welded positions have a nonzero normal (kept, bit k = the k-th triangle of tri_table). Returns the
-// number of kept triangles. With BLK the cube is one of block R's, only R's cubes can own an edge, and own / ci are indices within R.
-struct MeshCube {float vlist[12][3]; unsigned own[12]; unsigned char oj[12], tri[5][3]; unsigned mask, kept;};
-template<bool EMIT, bool BLK = false>
-__device__ unsigned cube_mesh(const float *__restrict__ vals, const unsigned char *__restrict__ outside, const tw_voxel_post_params &P, const McTables &T,
-	const unsigned char *s_edge, const unsigned char *s_look, unsigned x, unsigned y, unsigned z, unsigned ci, MeshCube &m, const CubeRange &R = CubeRange())
-{
-	m.mask = 0; m.kept = 0;
-	unsigned const nx = P.nx, ny = P.ny, nz = P.nz;
-	if (x + 1 >= nx || y + 1 >= ny || z + 1 >= nz) return 0; // last layer of an axis
-	unsigned cix = 0;
-	bool all_under_mesh = (P.skip_under_mesh != 0);
-#pragma unroll
-	for (unsigned yhi = 0; yhi < 2; ++yhi) {
-#pragma unroll
-		for (unsigned xhi = 0; xhi < 2; ++xhi) {
-			size_t const ix = z + ((size_t)(x + xhi) + (size_t)(y + yhi)*nx)*nz;
-			if (all_under_mesh) {all_under_mesh = ((__ldg(outside + ix) & TW_VOX_UNDER_MESH) != 0);}
-#pragma unroll
-			for (unsigned zhi = 0; zhi < 2; ++zhi) {if (__ldg(outside + ix + zhi) & 7) {cix |= 1u << ((xhi ^ yhi) + 2*yhi + 4*zhi);}}
-		}
-	}
-	if (all_under_mesh) return 0;
-	unsigned const edge_val = __ldg(T.edge_table + cix);
-	if (edge_val == 0) return 0;
-	for (unsigned i = 0; i < 12; ++i) {
-		if (EMIT) {m.own[i] = ci; m.oj[i] = (unsigned char)i;}
-		if (!(edge_val & (1u << i))) continue;
-		unsigned const e = s_edge[i], a = e & 3;
-		unsigned p1, p2; perp(a, p1, p2);
-		int const g[3] = {(int)(x + ((e >> 2) & 1)), (int)(y + ((e >> 3) & 1)), (int)(z + ((e >> 4) & 1))};
-		int o[3] = {(int)x, (int)y, (int)z};
-		unsigned j = i;
-		for (unsigned k = 0; k < 4; ++k) { // the edge's cubes in increasing index: (d1, d2) = (1, 1), (1, 0), (0, 1), (0, 0) below its low corner
-			unsigned const d1 = (k < 2), d2 = !(k & 1);
-			int c[3] = {g[0], g[1], g[2]};
-			c[p1] -= (int)d1; c[p2] -= (int)d2;
-			if (c[0] == (int)x && c[1] == (int)y && c[2] == (int)z) {m.mask |= 1u << i; break;} // no earlier cube makes triangles: this one owns it
-			if (cube_valid<BLK>(outside, P, c, R)) {o[0] = c[0]; o[1] = c[1]; o[2] = c[2]; j = s_look[4*a + 2*d1 + d2]; break;}
-		}
-		if (EMIT) {
-			m.own[i] = (m.mask & (1u << i)) ? ci : BLK ? (((unsigned)o[1] - R.y0)*(R.x1 - R.x0) + (unsigned)o[0] - R.x0)*nz + (unsigned)o[2]
-			                                            : (unsigned)o[2] + ((unsigned)o[0] + (unsigned)o[1]*nx)*nz;
-			m.oj[i] = (unsigned char)j;
-		}
-		float v2[2], pts[2][3];
-#pragma unroll
-		for (unsigned d = 0; d < 2; ++d) { // the owner's interpolation: its corners, in its order
-			unsigned const ev = __ldg(T.edge_to_vals + 2*j + d), yhi = (ev & 2) >> 1, xhi = yhi ^ (ev & 1), zhi = (ev >> 2) & 1;
-			unsigned const cx = (unsigned)o[0] + xhi, cy = (unsigned)o[1] + yhi, cz = (unsigned)o[2] + zhi;
-			size_t const ix = cz + ((size_t)cx + (size_t)cy*nx)*nz;
-			v2[d] = ((__ldg(outside + ix) & 7) == TW_VOX_ON_EDGE) ? P.isolevel : __ldg(vals + ix);
-			pts[d][0] = (float)cx*P.vsz[0] + P.lo_pos[0]; pts[d][1] = (float)cy*P.vsz[1] + P.lo_pos[1]; pts[d][2] = (float)cz*P.vsz[2] + P.lo_pos[2];
-		}
-		interpolate_pt(P.isolevel, pts[0], pts[1], v2[0], v2[1], m.vlist[i]);
-	}
-	const int *t = T.tri_table + 16*cix;
-	unsigned count = 0;
-	for (unsigned i = 0, k = 0; i < 15; i += 3, ++k) {
-		int const t0 = __ldg(t + i);
-		if (t0 < 0) break;
-		int const t1 = __ldg(t + i + 1), t2 = __ldg(t + i + 2);
-		const float *p0 = m.vlist[t0], *p1 = m.vlist[t1], *p2 = m.vlist[t2];
-		float const a0 = p1[0] - p0[0], a1 = p1[1] - p0[1], a2 = p1[2] - p0[2], b0 = p2[0] - p1[0], b1 = p2[1] - p1[1], b2 = p2[2] - p1[2]; // get_normal
-		float const cx = a1*b2 - a2*b1, cy = a2*b0 - a0*b2, cz = a0*b1 - a1*b0;
-		if (cx == 0.0f && cy == 0.0f && cz == 0.0f) continue; // degenerate in the welded positions: the reference tests the cached points
-		if (EMIT) {m.tri[count][0] = (unsigned char)t0; m.tri[count][1] = (unsigned char)t1; m.tri[count][2] = (unsigned char)t2;}
-		++count;
-	}
-	return count;
-}
 
 template<bool EMIT>
 __global__ void __launch_bounds__(MC_BLOCK)
@@ -1246,43 +1111,48 @@ int validate_changes(tw_ctx *ctx, const tw_voxel_changes *ch, ChangeOut *d) {
 	return TW_OK;
 }
 
-// The change-list kernels (tw_voxel_changes.cu) live in their own module, tw_voxel_changes.cubin beside this library, loaded once per process on first
-// use (cudaLibraryLoadFromFile loads it into each device's context as needed). A missing or unloadable module is an error.
-struct ChangeKernels {cudaKernel_t box_bits, diff_bits, count, emit;};
-int change_kernels(tw_ctx *ctx, ChangeKernels *K) {
+// Device code the library loads at run time (build.py's MODULES): the kernels `names` of the sm_90a module `file` beside this library, loaded once per
+// process on first use (cudaLibraryLoadFromFile loads it into each device's context as needed). A missing or unloadable module is an error.
+int module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int count, cudaKernel_t *out) {
 	static std::mutex mu;
-	static cudaLibrary_t lib = nullptr;
-	static ChangeKernels loaded;
+	static std::vector<std::pair<std::string, std::vector<cudaKernel_t>>> loaded; // per file, its kernels in the order of names
 	std::lock_guard<std::mutex> g(mu);
-	if (!lib) {
-		Dl_info info;
-		if (!dladdr((void *)&tw_voxel_model_edit_launch_ex, &info) || !info.dli_fname) return tw_set_error(ctx, TW_ERR_CUDA, "cannot locate the library's file");
-		std::string const lib_path = info.dli_fname, path = lib_path.substr(0, lib_path.rfind('/') + 1) + "tw_voxel_changes.cubin";
-		cudaLibrary_t l = nullptr;
-		cudaError_t e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-		ChangeKernels k;
-		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.box_bits, l, "tw_box_scatter_bits_kernel");
-		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.diff_bits, l, "tw_diff_bits_kernel");
-		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.count, l, "tw_change_count_kernel");
-		if (e == cudaSuccess) e = cudaLibraryGetKernel(&k.emit, l, "tw_change_emit_kernel");
-		if (e != cudaSuccess) {
-			cudaGetLastError();
-			if (l) cudaLibraryUnload(l);
-			return tw_set_error(ctx, TW_ERR_CUDA, "cannot load the change-list kernels from %s: %s", path.c_str(), cudaGetErrorString(e));
-		}
-		lib = l; loaded = k;
+	for (auto const &e : loaded) {if (e.first == file) {for (int k = 0; k < count; ++k) {out[k] = e.second[k];} return TW_OK;}}
+	Dl_info info;
+	if (!dladdr((void *)&tw_voxel_model_edit_launch_ex, &info) || !info.dli_fname) return tw_set_error(ctx, TW_ERR_CUDA, "cannot locate the library's file");
+	std::string const lib_path = info.dli_fname, path = lib_path.substr(0, lib_path.rfind('/') + 1) + file;
+	cudaLibrary_t l = nullptr;
+	cudaError_t e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+	std::vector<cudaKernel_t> k(count);
+	for (int i = 0; i < count && e == cudaSuccess; ++i) {e = cudaLibraryGetKernel(&k[i], l, names[i]);}
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		if (l) cudaLibraryUnload(l);
+		return tw_set_error(ctx, TW_ERR_CUDA, "cannot load the kernels of %s: %s", path.c_str(), cudaGetErrorString(e));
 	}
-	*K = loaded;
+	loaded.emplace_back(file, k);
+	for (int i = 0; i < count; ++i) {out[i] = k[i];}
 	return TW_OK;
 }
-// one launch of a module kernel on ctx->stream; the arguments must have the kernel's parameter types exactly
+// The change-list kernels (tw_voxel_changes.cu), from tw_voxel_changes.cubin
+struct ChangeKernels {cudaKernel_t box_bits, diff_bits, count, emit;};
+int change_kernels(tw_ctx *ctx, ChangeKernels *K) {
+	static const char *const names[] = {"tw_box_scatter_bits_kernel", "tw_diff_bits_kernel", "tw_change_count_kernel", "tw_change_emit_kernel"};
+	cudaKernel_t k[4];
+	int const rc = module_kernels(ctx, "tw_voxel_changes.cubin", names, 4, k); if (rc) return rc;
+	*K = ChangeKernels{k[0], k[1], k[2], k[3]};
+	return TW_OK;
+}
+// one launch of a module kernel on ctx->stream with smem bytes of dynamic shared memory; the arguments must have the kernel's parameter types exactly
 template<typename... A>
-int launch_module_kernel(tw_ctx *ctx, cudaKernel_t k, unsigned grid, unsigned block, A... a) {
+int launch_module_kernel_smem(tw_ctx *ctx, cudaKernel_t k, dim3 grid, unsigned block, size_t smem, A... a) {
 	void *args[] = {(void *)&a...};
-	TW_CUDA(ctx, cudaLaunchKernel((const void *)k, dim3(grid), dim3(block), args, 0, ctx->stream));
+	TW_CUDA(ctx, cudaLaunchKernel((const void *)k, grid, dim3(block), args, smem, ctx->stream));
 	ctx->launches++;
 	return TW_OK;
 }
+template<typename... A>
+int launch_module_kernel(tw_ctx *ctx, cudaKernel_t k, unsigned grid, unsigned block, A... a) {return launch_module_kernel_smem(ctx, k, dim3(grid), block, 0, a...);}
 
 // the list of the voxels whose bits are set (bits: every word written), its total into the pinned stage
 int enqueue_change_list(tw_ctx *ctx, const tw_voxel_model *m, const ModelScratch &X, const ChangeOut &C, const ChangeKernels &K) {
@@ -1424,6 +1294,177 @@ extern "C" int tw_voxel_model_read_launch(tw_ctx *ctx, tw_voxel_model *m, const 
 				TW_CUDA(ctx, cudaMemcpy3DAsync(&q, ctx->stream));
 			}
 		}
+		return TW_OK;
+	});
+}
+
+// ------------------------------------------------------------------------------------------------ many small grids in one job (tw_voxel_build_batch_launch)
+// The batch's kernels are the module tw_voxel_batch.cubin's (tw_voxel_batch.cu), each launched once over every grid through the device table of
+// twi_vbatch_grid: sine tables (sine grids only), fill and flags, the flood (remove_unconnected grids only), mesh count, per-grid scan, mesh emit (grids with
+// a capacity only). So a batch launches the same kernels for 1 grid as for 300.
+//   device slot 0: [grid table | counts (3 per grid) | tables | sine coefficients | per grid: field (unless vals is device memory), flags, sine tables, zix_xy
+//                  (host input), mesh words, block sums and offsets]
+//   pinned:        [grid table | counts | tables | sine coefficients | per grid: zix_xy (host input)]
+namespace {
+struct BatchKernels {cudaKernel_t tables, fill, flood, count, scan, emit;};
+int batch_kernels(tw_ctx *ctx, BatchKernels *K) {
+	static const char *const names[] = {"tw_vbatch_tables_kernel", "tw_vbatch_fill_kernel", "tw_vbatch_flood_kernel", "tw_vbatch_mesh_count_kernel",
+	                                    "tw_vbatch_mesh_scan_kernel", "tw_vbatch_mesh_emit_kernel"};
+	cudaKernel_t k[6];
+	int const rc = module_kernels(ctx, "tw_voxel_batch.cubin", names, 6, k); if (rc) return rc;
+	*K = BatchKernels{k[0], k[1], k[2], k[3], k[4], k[5]};
+	return TW_OK;
+}
+// a refusal of grid i: the helper's message prefixed with the grid's index
+int grid_error(tw_ctx *ctx, uint32_t i, int rc) {
+	std::string const msg = ctx->err;
+	return tw_set_error(ctx, rc, "grid %u: %s", i, msg.c_str());
+}
+} // namespace
+
+extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *grids, const tw_voxel_mesh *meshes, uint32_t n) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!grids || !meshes) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_build_batch_launch: null grids or meshes");
+	if (n == 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_build_batch_launch: an empty batch");
+	struct Grid {tw_voxel_build b; tw_voxel_post_params P; tw_voxel_params F; tw_voxel_mesh M; float *d_mv; uint32_t *d_mi; unsigned nvox, nb; bool fill, sine;};
+	std::vector<Grid> G(n);
+	bool any_glm = false, any_rm = false, any_cap = false;
+	unsigned nsine = 0, flood_words = 0, fill_blocks = 0, mesh_blocks = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		Grid &g = G[i];
+		g.b = grids[i];
+		if (!g.b.post) return tw_set_error(ctx, TW_ERR_ARG, "grid %u: post is required", i);
+		g.P = *g.b.post;
+		rc = validate(ctx, &g.P); if (rc) return grid_error(ctx, i, rc);
+		if ((unsigned long long)g.P.nx*g.P.ny*g.P.nz > TWI_VB_MAX_VOXELS)
+			return tw_set_error(ctx, TW_ERR_ARG, "grid %u: %ux%ux%u is more than 2^18 voxels (build it with tw_voxel_build_launch_ex)", i, g.P.nx, g.P.ny, g.P.nz);
+		g.nvox = g.P.nx*g.P.ny*g.P.nz; g.nb = (g.nvox + MC_BLOCK - 1)/MC_BLOCK;
+		g.fill = (g.b.fill != nullptr); g.sine = false;
+		if (g.fill) {
+			g.F = *g.b.fill;
+			if (g.F.nx != g.P.nx || g.F.ny != g.P.ny || g.F.nz != g.P.nz)
+				return tw_set_error(ctx, TW_ERR_ARG, "grid %u: the fill's grid %ux%ux%u differs from post's %ux%ux%u", i, g.F.nx, g.F.ny, g.F.nz, g.P.nx, g.P.ny, g.P.nz);
+			size_t tab_bytes = 0;
+			rc = twi_voxel_fill_check(ctx, &g.F, &tab_bytes); if (rc) return grid_error(ctx, i, rc);
+			g.sine = (g.F.gen_mode == TW_MGEN_SINE);
+			nsine += g.sine; any_glm = any_glm || !g.sine;
+		}
+		else if (!g.b.vals) return tw_set_error(ctx, TW_ERR_ARG, "grid %u: vals is the input field when there is no fill", i);
+		if (!g.b.edge_table256 || !g.b.tri_table256x16 || !g.b.edge_to_vals12x2) return tw_set_error(ctx, TW_ERR_ARG, "grid %u: the welded mesh needs the three marching-cubes tables", i);
+		if (g.b.edge_table256 != grids[0].edge_table256 || g.b.tri_table256x16 != grids[0].tri_table256x16 || g.b.edge_to_vals12x2 != grids[0].edge_to_vals12x2)
+			return tw_set_error(ctx, TW_ERR_ARG, "grid %u: its marching-cubes tables are not grid 0's (a batch shares one set)", i);
+		if (g.b.tris || g.b.capacity || g.b.ntris) return tw_set_error(ctx, TW_ERR_ARG, "grid %u: a batch builds no triangle soup (tris, capacity and ntris must be NULL / 0)", i);
+		g.M = meshes[i];
+		rc = validate_mesh(ctx, &g.P, &g.M); if (rc) return grid_error(ctx, i, rc);
+		g.d_mv = nullptr; g.d_mi = nullptr;
+		if (g.M.verts && !(g.d_mv = (float *)device_view(g.M.verts))) return tw_set_error(ctx, TW_ERR_ARG, "grid %u: mesh verts must be device or page-locked host memory", i);
+		if (g.M.indices && !(g.d_mi = (uint32_t *)device_view(g.M.indices))) return tw_set_error(ctx, TW_ERR_ARG, "grid %u: mesh indices must be device or page-locked host memory", i);
+		if (g.P.remove_unconnected > 0) {any_rm = true; flood_words = std::max(flood_words, (g.nvox + 31)/32);}
+		any_cap = any_cap || g.M.vcapacity || g.M.tcapacity;
+		fill_blocks += (g.nvox + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS; mesh_blocks += g.nb;
+	}
+	BatchKernels K;
+	rc = batch_kernels(ctx, &K); if (rc) return rc;
+	size_t const lut_bytes = any_glm ? (size_t)twn2::LUT3D_N*twn2::SIMPLEX_LUT_COPIES*sizeof(float4) : 0, flood_bytes = 6*sizeof(unsigned)*(size_t)flood_words;
+	if (lut_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lut_bytes, ctx->device));}
+	if (flood_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.flood, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)flood_bytes, ctx->device));}
+	if (any_glm) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
+	std::vector<twi_user<float>> V; std::vector<twi_user<const uint32_t>> Z;
+	V.reserve(n); Z.reserve(n);
+	for (Grid const &g : G) {V.emplace_back(g.b.vals, g.nvox); Z.emplace_back(g.b.zix_xy, (size_t)g.P.nx*g.P.ny);}
+	twi_vbatch_grid *d_tab; unsigned long long *d_counts; char *tab; float *d_rdata = nullptr;
+	std::vector<twi_vbatch_grid> D(n);
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_tab = c.take<twi_vbatch_grid>(n); d_counts = c.take<unsigned long long>(3*(size_t)n); tab = c.take<char>(MC_TAB_BYTES);
+		if (nsine) {d_rdata = c.take<float>((size_t)nsine*TW_N3D_RDATA);}
+		for (uint32_t i = 0; i < n; ++i) {
+			Grid const &g = G[i];
+			twi_vbatch_grid &d = D[i];
+			V[i].take(c); d.flags = c.take<unsigned char>((size_t)g.nvox + 4);
+			d.xt = d.yt = d.zt = nullptr; d.xp = d.yp = d.zp = 0;
+			if (g.sine) {
+				d.xp = (g.P.nx + 31) & ~31u; d.yp = (g.P.ny + 31) & ~31u; d.zp = (g.P.nz + 31) & ~31u;
+				d.xt = c.take<float>((size_t)NS*(d.xp + d.yp + d.zp)); d.yt = d.xt ? d.xt + (size_t)NS*d.xp : nullptr; d.zt = d.yt ? d.yt + (size_t)NS*d.yp : nullptr;
+			}
+			if (g.b.zix_xy) {Z[i].take(c);}
+			d.words = c.take<unsigned>(g.nvox); d.vsums = c.take<unsigned>(g.nb); d.tsums = c.take<unsigned>(g.nb);
+			d.voff = c.take<unsigned long long>(g.nb); d.toff = c.take<unsigned long long>(g.nb);
+		}
+	}); if (rc) return rc;
+	twi_vbatch_grid *h_tab; unsigned long long *h_counts; char *h_mc; float *h_rdata = nullptr;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
+		h_tab = c.take<twi_vbatch_grid>(n); h_counts = c.take<unsigned long long>(3*(size_t)n); h_mc = c.take<char>(MC_TAB_BYTES);
+		if (nsine) {h_rdata = c.take<float>((size_t)nsine*TW_N3D_RDATA);}
+		for (twi_user<const uint32_t> &z : Z) {z.take_pinned(c);}
+	}); if (rc) return rc;
+	// the table: fill parameters as twi_voxel_fill derives them, sine coefficients as it stages them, the blocks' prefix sums
+	unsigned fb = 0, mb = 0, si = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		Grid const &g = G[i];
+		twi_vbatch_grid &d = D[i];
+		d.P = g.P; d.n = g.nvox; d.fill_blk0 = fb; d.mesh_blk0 = mb;
+		fb += (g.nvox + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS; mb += g.nb;
+		d.mode = !g.fill ? TWI_VB_INPUT : g.sine ? TWI_VB_SINE : (g.F.gen_mode == TW_MGEN_PERLIN) ? TWI_VB_PERLIN : TWI_VB_SIMPLEX;
+		memset(&d.E, 0, sizeof(d.E)); memset(&d.G, 0, sizeof(d.G));
+		d.rdata = nullptr;
+		for (int k = 0; k < 3; ++k) {d.s[k] = 0.0f; d.step[k] = 0.0f;}
+		if (g.fill) {
+			tw_voxel_params const &F = g.F;
+			d.E.zscale = F.zscale; d.E.normalize = F.normalize_to_1;
+			d.E.atten_mode = F.atten_mode; d.E.atten_val = F.atten_val; d.E.inner_radius = F.atten_inner_radius;
+			d.E.nx = F.nx; d.E.ny = F.ny; d.E.nz = F.nz;
+			if (g.sine) {
+				float *const r = h_rdata + (size_t)si*TW_N3D_RDATA;
+				if (g.b.rdata420) {memcpy(r, g.b.rdata420, TW_N3D_RDATA*sizeof(float));} else {tw_noise3d_gen_sines(F.rseed1, F.rseed2, F.mag, F.freq, r);}
+				d.rdata = d_rdata + (size_t)si*TW_N3D_RDATA; ++si;
+				for (int k = 0; k < 3; ++k) {d.s[k] = F.lo_pos[k] + F.offset[k]; d.step[k] = F.vsz[k];} // (lo_pos + offset), src/voxels.cpp:289
+			}
+			else {
+				for (int k = 0; k < 3; ++k) {d.G.lo[k] = F.lo_pos[k]; d.G.vsz[k] = F.vsz[k]; d.G.off[k] = F.offset[k];}
+				d.G.mag = F.mag; d.G.nfreq0 = (float)(0.25*F.freq);
+				d.G.rx = F.rx; d.G.ry = F.ry; d.G.rz = F.rx - F.ry;
+				d.G.octaves = F.octaves; d.G.perlin = (F.gen_mode == TW_MGEN_PERLIN);
+			}
+		}
+		d.vals = V[i].d; d.zix = g.b.zix_xy ? Z[i].d : nullptr;
+		d.verts = g.d_mv; d.vcap = g.M.vcapacity; d.indices = g.d_mi; d.tcap = g.M.tcapacity;
+		d.counts = d_counts + 3*(size_t)i;
+	}
+	memcpy(h_tab, D.data(), (size_t)n*sizeof(twi_vbatch_grid));
+	struct Out {uint64_t *nverts, *ntris, *changed;};
+	std::vector<Out> outs(n);
+	for (uint32_t i = 0; i < n; ++i) {outs[i] = Out{G[i].M.nverts, G[i].M.ntris, G[i].b.changed};}
+	twi_job pending;
+	pending.cancellable = true; // no cancellation point: a cancel changes nothing
+	pending.complete = [h_counts, outs = std::move(outs)](tw_ctx *) -> int {
+		for (size_t i = 0; i < outs.size(); ++i) {
+			*outs[i].nverts = h_counts[3*i]; *outs[i].ntris = h_counts[3*i + 1];
+			if (outs[i].changed) {*outs[i].changed = h_counts[3*i + 2];}
+		}
+		return TW_OK;
+	};
+	McTables const T = mc_tables(tab);
+	twi_vbatch_grid const *const dt = d_tab;
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
+		TW_CUDA(ctx, cudaMemsetAsync(d_counts, 0, 3*(size_t)n*sizeof(unsigned long long), ctx->stream));
+		TW_CUDA(ctx, cudaMemcpyAsync(d_tab, h_tab, (size_t)n*sizeof(twi_vbatch_grid), cudaMemcpyHostToDevice, ctx->stream));
+		if (nsine) {TW_CUDA(ctx, cudaMemcpyAsync(d_rdata, h_rdata, (size_t)nsine*TW_N3D_RDATA*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));}
+		int r = mc_tables_upload(ctx, tab, grids[0].edge_table256, grids[0].tri_table256x16, grids[0].edge_to_vals12x2, h_mc); if (r) return r;
+		for (uint32_t i = 0; i < n; ++i) {
+			if (!G[i].fill) {r = V[i].in(ctx); if (r) return r;}
+			r = Z[i].in(ctx); if (r) return r;
+		}
+		if (nsine) {r = launch_module_kernel_smem(ctx, K.tables, dim3(3, n), 64u, 0, dt, (const float *)ctx->d_sin_table); if (r) return r;}
+		r = launch_module_kernel_smem(ctx, K.fill, dim3(fill_blocks), TWI_VB_FILL_THREADS, lut_bytes, dt, n, (const float4 *)ctx->d_glm3_lut); if (r) return r;
+		if (any_rm) {r = launch_module_kernel_smem(ctx, K.flood, dim3(n), TWI_VB_FLOOD_THREADS, flood_bytes, dt); if (r) return r;}
+		r = launch_module_kernel(ctx, K.count, mesh_blocks, (unsigned)MC_BLOCK, dt, n, T); if (r) return r;
+		r = launch_module_kernel(ctx, K.scan, n, 1024u, dt); if (r) return r;
+		if (any_cap) {r = launch_module_kernel(ctx, K.emit, mesh_blocks, (unsigned)MC_BLOCK, dt, n, T); if (r) return r;}
+		for (uint32_t i = 0; i < n; ++i) {
+			if (G[i].fill || G[i].P.remove_unconnected > 0) {r = V[i].out(ctx); if (r) return r;}
+			if (G[i].b.outside) {TW_CUDA(ctx, cudaMemcpyAsync(G[i].b.outside, D[i].flags, G[i].nvox, cudaMemcpyDefault, ctx->stream));}
+		}
+		TW_CUDA(ctx, cudaMemcpyAsync(h_counts, d_counts, 3*(size_t)n*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		return TW_OK;
 	});
 }

@@ -1175,6 +1175,17 @@ inline tiles_job voxel_build_async(voxel_grid_view const &v, tw_voxel_params con
 	if (rc != TW_OK) {detail::fail(rc, "voxel_build_async", c);}
 	return tiles_job(c, &jobs, number);
 }
+// Many small grids - rock and asteroid models (gen_voxel_rock) - built as one job (tw_voxel_build_batch_launch): grids[i] / meshes[i] as for the welded form
+// of voxel_build_async (no soup: tris, capacity and ntris NULL / 0; the same three table pointers for every grid; at most 2^18 voxels per grid); every grid
+// equals its own voxel_build_async byte for byte once the returned tiles_job is ready. The arrays are copied during the launch.
+inline tiles_job voxel_build_batch_async(tw_voxel_build const *grids, tw_voxel_mesh const *meshes, unsigned n) {
+	tw_ctx *c = ctx();
+	std::atomic<uint64_t> &jobs = detail::tls().tile_jobs;
+	uint64_t const number = ++jobs;
+	int const rc = tw_voxel_build_batch_launch(c, grids, meshes, n);
+	if (rc != TW_OK) {detail::fail(rc, "voxel_build_batch_async", c);}
+	return tiles_job(c, &jobs, number);
+}
 
 // A voxel model edited with brushes (src/voxels.cpp:2139-2245) and meshed per block, as create_block keeps one mesh and vertex cache per block (:1077-1108),
 // kept on the device by the thread's context (tw_voxel_model_*). build_async takes the field from fill or from vals (v.data is not read) and meshes every

@@ -695,6 +695,20 @@ TW_API int tw_voxel_build_launch(tw_ctx *ctx, const tw_voxel_build *b);
  * completing poll, and not on TW_ERR_CANCELED. The mesh struct is copied during the launch. Every rule of tw_voxel_build_launch applies; TW_ERR_ARG also
  * for a mesh without tables or counts, a capacity without its buffer, pageable verts / indices and 3*nx*ny*nz >= 2^32. */
 TW_API int tw_voxel_build_launch_ex(tw_ctx *ctx, const tw_voxel_build *b, const tw_voxel_mesh *mesh);
+/* Many small grids in ONE asynchronous job - an engine's rock and asteroid models (gen_voxel_rock: atten_to_sphere, centre_seed), at start-up or a frame's
+ * worth at a time. After the completing poll grid i's outputs are bit-identical to tw_voxel_build_launch_ex(ctx, &grids[i], &meshes[i]) run alone: vals and
+ * outside after remove_unconnected, *changed, the welded mesh's verts / indices up to their capacities and *nverts / *ntris. The job launches the same
+ * kernels whatever n is, each over every grid, and floods each grid's remove_unconnected inside one SM's shared memory (DESIGN.md section 4l).
+ * - Mesh only: meshes[i] is required for every grid, and there is no triangle soup (grids[i].tris, capacity and ntris must be NULL / 0).
+ * - Size limit: nx*ny*nz <= 2^18 (64^3, or 8x8x4096, or 512x512x1) per grid; larger grids belong on tw_voxel_build_launch_ex.
+ * - Every grid has its own fill (any gen mode and attenuation) or input vals (host or device), post params and zix_xy; all grids pass the same three
+ *   marching-cubes table pointers.
+ * - Job rules, lifetimes and memory kinds: those of tw_voxel_build_launch_ex, per grid (the grids and meshes arrays are copied during the launch).
+ * - The job has no cancellation point (its grids are small): tw_cancel returns TW_OK and changes nothing, as after a job's last cancellation point.
+ * - Errors, nothing enqueued and nothing changed: TW_ERR_ARG for NULL grids or meshes, n == 0, a grid above the limit, tables that differ from grid 0's,
+ *   soup fields set, and every refusal of tw_voxel_build_launch_ex for a grid; TW_ERR_STATE where it returns that. tw_last_error names the grid's index.
+ *   TW_ERR_CUDA when tw_voxel_batch.cubin, the batch's sm_90a module beside the library, cannot be loaded. */
+TW_API int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *grids, const tw_voxel_mesh *meshes, uint32_t n);
 
 /* ---- resident voxel models: the field kept on the device, edited in place, re-meshed per block ----
  * What voxel_model does with brushes (src/voxels.cpp:2139-2245): it keeps one mesh per block, each with its own vertex cache (create_block, :1077-1108), and an

@@ -98,6 +98,16 @@ class VoxelChanges(C.Structure):
     _fields_ = [("index", C.c_void_p), ("vals", C.c_void_p), ("outside", C.c_void_p), ("capacity", C.c_uint64), ("nchanged", C.c_void_p)]
 
 
+class VoxelModelBuild(C.Structure):
+    """tw_voxel_model_build (include/tw3d.h): one model of tw_voxel_model_build_batch_launch and the arguments of its tw_voxel_model_build_launch_on."""
+    _fields_ = [("model", C.c_void_p), ("fill", C.c_void_p), ("rdata420", C.c_void_p), ("vals", C.c_void_p), ("out", C.c_void_p)]
+
+
+class VoxelModelEdit(C.Structure):
+    """tw_voxel_model_edit (include/tw3d.h): one model of tw_voxel_model_edit_batch_launch and the arguments of its tw_voxel_model_edit_launch_on."""
+    _fields_ = [("model", C.c_void_p), ("boxes", C.c_void_p), ("nboxes", C.c_uint32), ("values", C.c_void_p), ("out", C.c_void_p), ("ch", C.c_void_p)]
+
+
 class VoxelBox(C.Structure):
     """tw_voxel_box (include/tw3d.h): the voxels [x, x+w) x [y, y+h) x [z, z+d)."""
     _fields_ = [(n, C.c_uint32) for n in ("x", "y", "z", "w", "h", "d")]
@@ -249,7 +259,8 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_voxel_model_create", "tw_voxel_model_destroy", "tw_voxel_model_build_launch", "tw_voxel_model_edit_launch", "tw_voxel_model_read",
                "tw_voxel_model_edit_launch_ex", "tw_voxel_model_build_launch_on", "tw_voxel_model_edit_launch_on", "tw_voxel_model_read_launch",
                "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows",
-               "tw_read_heightmap_launch", "tw_read_heightmap", "tw_voxel_build_batch_launch"]
+               "tw_read_heightmap_launch", "tw_read_heightmap", "tw_voxel_build_batch_launch",
+               "tw_voxel_model_build_batch_launch", "tw_voxel_model_edit_batch_launch"]
 
 
 def _load():
@@ -370,6 +381,8 @@ def _load():
     L.tw_voxel_model_build_launch_on.argtypes = [vp] + L.tw_voxel_model_build_launch.argtypes
     L.tw_voxel_model_edit_launch_on.argtypes = [vp] + L.tw_voxel_model_edit_launch_ex.argtypes
     L.tw_voxel_model_read_launch.argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp]
+    L.tw_voxel_model_build_batch_launch.argtypes = [vp, C.POINTER(VoxelModelBuild), C.c_uint32]
+    L.tw_voxel_model_edit_batch_launch.argtypes = [vp, C.POINTER(VoxelModelEdit), C.c_uint32]
     L.tw_tile_shadows_batch.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp]
     L.tw_tile_shadows_batch_ex.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, C.POINTER(ShadowParams), vp, vp, vp, vp, vp]
     L.tw_tile_set_create.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]
@@ -1322,6 +1335,49 @@ class Context:
         self._check(lib.tw_voxel_build_batch_launch(self._h, bs, ms, n))
         self._tiles_job = (keep, job)
         return job
+
+    def voxel_model_build_batch_launch(self, builds):
+        """tw_voxel_model_build_batch_launch: many small VoxelModels (nx*ny*nz <= 2^18 each) built in one asynchronous job on this Context, each exactly as
+        its build_launch(ctx=self) would build it alone; create_tiles_poll completes it. builds: a list of dicts with the keys model (required) and fill,
+        vals, rdata, verts, indices as VoxelModel.build_launch takes them. Returns one VoxelModelJob per entry, filled once the job is complete; the buffers
+        stay referenced here until then."""
+        n = len(builds)
+        es, jobs, keep = (VoxelModelBuild * max(n, 1))(), [], []
+        for i, b in enumerate(builds):
+            m = b["model"]
+            job = VoxelModelJob(m.nblocks)
+            out = job._out(b.get("verts"), b.get("indices"))
+            rd = None if b.get("rdata") is None else np.ascontiguousarray(b["rdata"], np.float32)
+            fill = b.get("fill")
+            keep.append((b, out, rd))
+            es[i] = VoxelModelBuild(m._h, C.cast(C.pointer(fill), C.c_void_p) if fill is not None else None, _ptr(rd), _ptr(b.get("vals")),
+                                    C.cast(C.pointer(out), C.c_void_p))
+            jobs.append(job)
+        self._check(lib.tw_voxel_model_build_batch_launch(self._h, es, n))
+        self._tiles_job = (keep, jobs)
+        return jobs
+
+    def voxel_model_edit_batch_launch(self, edits):
+        """tw_voxel_model_edit_batch_launch: edits of many small VoxelModels in one asynchronous job on this Context, each exactly as its
+        edit_launch(ctx=self) would edit it alone; create_tiles_poll completes it. edits: a list of dicts with the keys model (required) and boxes, values,
+        verts, indices, changes as VoxelModel.edit_launch takes them (boxes absent or empty: no change). Returns one VoxelModelJob per entry."""
+        n = len(edits)
+        es, jobs, keep = (VoxelModelEdit * max(n, 1))(), [], []
+        for i, e in enumerate(edits):
+            m, boxes = e["model"], e.get("boxes")
+            boxes = [] if boxes is None else boxes
+            b = (VoxelBox * max(len(boxes), 1))(*[VoxelBox(*[int(v) for v in t]) for t in boxes])
+            vals = np.ascontiguousarray(e.get("values", np.zeros(0, np.float32)), np.float32).ravel()
+            job = VoxelModelJob(m.nblocks)
+            out = job._out(e.get("verts"), e.get("indices"))
+            ch = None if e.get("changes") is None else job._changes(e["changes"])
+            keep.append((e, b, vals, out, ch))
+            es[i] = VoxelModelEdit(m._h, C.cast(b, C.c_void_p) if len(boxes) else None, len(boxes), _ptr(vals) if len(boxes) else None, C.cast(C.pointer(out), C.c_void_p),
+                                   C.cast(C.pointer(ch), C.c_void_p) if ch is not None else None)
+            jobs.append(job)
+        self._check(lib.tw_voxel_model_edit_batch_launch(self._h, es, n))
+        self._tiles_job = (keep, jobs)
+        return jobs
 
     def from_floats_u16(self, vals, val_mult, val_add, out=None):
         n = int(np.prod(vals.shape))

@@ -14,6 +14,7 @@
 #include "tw_voxel_edit.cuh"
 #include "tw_voxel_mc.cuh"
 #include "tw_voxel_batch.h"
+#include "tw_voxel_model_batch.h"
 #include <dlfcn.h>
 #include <algorithm>
 #include <mutex>
@@ -948,10 +949,14 @@ twi_job model_job(const ModelScratch &X, const tw_voxel_blocks_out &o, uint64_t 
 
 // A model call on ctx: TW_ERR_ARG unless ctx and m are set and ctx is m's context, its parent or a shared context of that parent; then ctx's pending job is
 // completed (never another context's)
-int model_begin(tw_ctx *ctx, tw_voxel_model *m) {
-	if (!ctx || !m) return TW_ERR_ARG;
+int model_family(tw_ctx *ctx, const tw_voxel_model *m) {
 	tw_ctx const *root = ctx->parent ? ctx->parent : ctx, *owner = m->ctx->parent ? m->ctx->parent : m->ctx;
 	if (root != owner || ctx->device != m->ctx->device) return tw_set_error(ctx, TW_ERR_ARG, "the voxel model belongs to another family of contexts");
+	return TW_OK;
+}
+int model_begin(tw_ctx *ctx, tw_voxel_model *m) {
+	if (!ctx || !m) return TW_ERR_ARG;
+	int const rc = model_family(ctx, m); if (rc) return rc;
 	return twi_begin(ctx);
 }
 
@@ -1315,10 +1320,50 @@ int batch_kernels(tw_ctx *ctx, BatchKernels *K) {
 	*K = BatchKernels{k[0], k[1], k[2], k[3], k[4], k[5]};
 	return TW_OK;
 }
-// a refusal of grid i: the helper's message prefixed with the grid's index
-int grid_error(tw_ctx *ctx, uint32_t i, int rc) {
+// a refusal of entry i of a batch: the helper's message prefixed with the entry's kind and index
+int entry_error(tw_ctx *ctx, const char *kind, uint32_t i, int rc) {
 	std::string const msg = ctx->err;
-	return tw_set_error(ctx, rc, "grid %u: %s", i, msg.c_str());
+	return tw_set_error(ctx, rc, "%s %u: %s", kind, i, msg.c_str());
+}
+int grid_error(tw_ctx *ctx, uint32_t i, int rc) {return entry_error(ctx, "grid", i, rc);}
+// grid d's fill as the batch module reads it (F: nullptr for an input field): the mode, the epilogue and GLM parameters as twi_voxel_fill derives them, and
+// in sine mode the coefficients as it stages them - at h_r (rdata420, or generated), read by the device at d_r
+void vbatch_fill_params(const tw_voxel_params *F, const float *rdata420, float *h_r, const float *d_r, twi_vbatch_grid &d) {
+	bool const sine = F && F->gen_mode == TW_MGEN_SINE;
+	d.mode = !F ? TWI_VB_INPUT : sine ? TWI_VB_SINE : (F->gen_mode == TW_MGEN_PERLIN) ? TWI_VB_PERLIN : TWI_VB_SIMPLEX;
+	memset(&d.E, 0, sizeof(d.E)); memset(&d.G, 0, sizeof(d.G));
+	d.rdata = nullptr;
+	for (int k = 0; k < 3; ++k) {d.s[k] = 0.0f; d.step[k] = 0.0f;}
+	if (!F) return;
+	d.E.zscale = F->zscale; d.E.normalize = F->normalize_to_1;
+	d.E.atten_mode = F->atten_mode; d.E.atten_val = F->atten_val; d.E.inner_radius = F->atten_inner_radius;
+	d.E.nx = F->nx; d.E.ny = F->ny; d.E.nz = F->nz;
+	if (sine) {
+		if (rdata420) {memcpy(h_r, rdata420, TW_N3D_RDATA*sizeof(float));} else {tw_noise3d_gen_sines(F->rseed1, F->rseed2, F->mag, F->freq, h_r);}
+		d.rdata = d_r;
+		for (int k = 0; k < 3; ++k) {d.s[k] = F->lo_pos[k] + F->offset[k]; d.step[k] = F->vsz[k];} // (lo_pos + offset), src/voxels.cpp:289
+	}
+	else {
+		for (int k = 0; k < 3; ++k) {d.G.lo[k] = F->lo_pos[k]; d.G.vsz[k] = F->vsz[k]; d.G.off[k] = F->offset[k];}
+		d.G.mag = F->mag; d.G.nfreq0 = (float)(0.25*F->freq);
+		d.G.rx = F->rx; d.G.ry = F->ry; d.G.rz = F->rx - F->ry;
+		d.G.octaves = F->octaves; d.G.perlin = (F->gen_mode == TW_MGEN_PERLIN);
+	}
+}
+// the sine mode's axis tables of grid P, carved from c (none for another mode)
+void vbatch_sine_tables(twi_carve &c, const tw_voxel_post_params &P, bool sine, twi_vbatch_grid &d) {
+	d.xt = d.yt = d.zt = nullptr; d.xp = d.yp = d.zp = 0;
+	if (!sine) return;
+	d.xp = (P.nx + 31) & ~31u; d.yp = (P.ny + 31) & ~31u; d.zp = (P.nz + 31) & ~31u;
+	d.xt = c.take<float>((size_t)NS*(d.xp + d.yp + d.zp)); d.yt = d.xt ? d.xt + (size_t)NS*d.xp : nullptr; d.zt = d.yt ? d.yt + (size_t)NS*d.yp : nullptr;
+}
+// the dynamic shared memory of the batch module's fill (the GLM tables, when a grid has a GLM fill) and flood (six bitsets of flood_words words)
+int vbatch_smem(tw_ctx *ctx, const BatchKernels &K, bool any_glm, unsigned flood_words, size_t *lut_bytes, size_t *flood_bytes) {
+	*lut_bytes = any_glm ? (size_t)twn2::LUT3D_N*twn2::SIMPLEX_LUT_COPIES*sizeof(float4) : 0; *flood_bytes = 6*sizeof(unsigned)*(size_t)flood_words;
+	if (*lut_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*lut_bytes, ctx->device));}
+	if (*flood_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.flood, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*flood_bytes, ctx->device));}
+	if (any_glm) {int const rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
+	return TW_OK;
 }
 } // namespace
 
@@ -1365,10 +1410,8 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 	}
 	BatchKernels K;
 	rc = batch_kernels(ctx, &K); if (rc) return rc;
-	size_t const lut_bytes = any_glm ? (size_t)twn2::LUT3D_N*twn2::SIMPLEX_LUT_COPIES*sizeof(float4) : 0, flood_bytes = 6*sizeof(unsigned)*(size_t)flood_words;
-	if (lut_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lut_bytes, ctx->device));}
-	if (flood_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.flood, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)flood_bytes, ctx->device));}
-	if (any_glm) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
+	size_t lut_bytes, flood_bytes;
+	rc = vbatch_smem(ctx, K, any_glm, flood_words, &lut_bytes, &flood_bytes); if (rc) return rc;
 	std::vector<twi_user<float>> V; std::vector<twi_user<const uint32_t>> Z;
 	V.reserve(n); Z.reserve(n);
 	for (Grid const &g : G) {V.emplace_back(g.b.vals, g.nvox); Z.emplace_back(g.b.zix_xy, (size_t)g.P.nx*g.P.ny);}
@@ -1381,11 +1424,7 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 			Grid const &g = G[i];
 			twi_vbatch_grid &d = D[i];
 			V[i].take(c); d.flags = c.take<unsigned char>((size_t)g.nvox + 4);
-			d.xt = d.yt = d.zt = nullptr; d.xp = d.yp = d.zp = 0;
-			if (g.sine) {
-				d.xp = (g.P.nx + 31) & ~31u; d.yp = (g.P.ny + 31) & ~31u; d.zp = (g.P.nz + 31) & ~31u;
-				d.xt = c.take<float>((size_t)NS*(d.xp + d.yp + d.zp)); d.yt = d.xt ? d.xt + (size_t)NS*d.xp : nullptr; d.zt = d.yt ? d.yt + (size_t)NS*d.yp : nullptr;
-			}
+			vbatch_sine_tables(c, g.P, g.sine, d);
 			if (g.b.zix_xy) {Z[i].take(c);}
 			d.words = c.take<unsigned>(g.nvox); d.vsums = c.take<unsigned>(g.nb); d.tsums = c.take<unsigned>(g.nb);
 			d.voff = c.take<unsigned long long>(g.nb); d.toff = c.take<unsigned long long>(g.nb);
@@ -1404,28 +1443,8 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 		twi_vbatch_grid &d = D[i];
 		d.P = g.P; d.n = g.nvox; d.fill_blk0 = fb; d.mesh_blk0 = mb;
 		fb += (g.nvox + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS; mb += g.nb;
-		d.mode = !g.fill ? TWI_VB_INPUT : g.sine ? TWI_VB_SINE : (g.F.gen_mode == TW_MGEN_PERLIN) ? TWI_VB_PERLIN : TWI_VB_SIMPLEX;
-		memset(&d.E, 0, sizeof(d.E)); memset(&d.G, 0, sizeof(d.G));
-		d.rdata = nullptr;
-		for (int k = 0; k < 3; ++k) {d.s[k] = 0.0f; d.step[k] = 0.0f;}
-		if (g.fill) {
-			tw_voxel_params const &F = g.F;
-			d.E.zscale = F.zscale; d.E.normalize = F.normalize_to_1;
-			d.E.atten_mode = F.atten_mode; d.E.atten_val = F.atten_val; d.E.inner_radius = F.atten_inner_radius;
-			d.E.nx = F.nx; d.E.ny = F.ny; d.E.nz = F.nz;
-			if (g.sine) {
-				float *const r = h_rdata + (size_t)si*TW_N3D_RDATA;
-				if (g.b.rdata420) {memcpy(r, g.b.rdata420, TW_N3D_RDATA*sizeof(float));} else {tw_noise3d_gen_sines(F.rseed1, F.rseed2, F.mag, F.freq, r);}
-				d.rdata = d_rdata + (size_t)si*TW_N3D_RDATA; ++si;
-				for (int k = 0; k < 3; ++k) {d.s[k] = F.lo_pos[k] + F.offset[k]; d.step[k] = F.vsz[k];} // (lo_pos + offset), src/voxels.cpp:289
-			}
-			else {
-				for (int k = 0; k < 3; ++k) {d.G.lo[k] = F.lo_pos[k]; d.G.vsz[k] = F.vsz[k]; d.G.off[k] = F.offset[k];}
-				d.G.mag = F.mag; d.G.nfreq0 = (float)(0.25*F.freq);
-				d.G.rx = F.rx; d.G.ry = F.ry; d.G.rz = F.rx - F.ry;
-				d.G.octaves = F.octaves; d.G.perlin = (F.gen_mode == TW_MGEN_PERLIN);
-			}
-		}
+		vbatch_fill_params(g.fill ? &g.F : nullptr, g.b.rdata420, h_rdata + (size_t)si*TW_N3D_RDATA, d_rdata + (size_t)si*TW_N3D_RDATA, d);
+		si += g.sine;
 		d.vals = V[i].d; d.zix = g.b.zix_xy ? Z[i].d : nullptr;
 		d.verts = g.d_mv; d.vcap = g.M.vcapacity; d.indices = g.d_mi; d.tcap = g.M.tcapacity;
 		d.counts = d_counts + 3*(size_t)i;
@@ -1467,4 +1486,300 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 		TW_CUDA(ctx, cudaMemcpyAsync(h_counts, d_counts, 3*(size_t)n*sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
 		return TW_OK;
 	});
+}
+
+// ------------------------------------------------------------------------------------------------ many small voxel models in one job (tw_voxel_model_*_batch_launch)
+// The fill, the flags and the flood are tw_voxel_batch.cubin's kernels on twi_vbatch_grid descriptors that point at each model's own memory (raw / raw_o for
+// the fill, post / post_o for the build's flood, work / work_o for an edit's); the rest is tw_voxel_model_batch.cubin's, each kernel launched once over
+// every model through the device table of twi_vmb_model. Each model costs one event wait and one record: the job waits for the model's earlier jobs on any
+// context of the family and orders its later ones.
+//   upload (pinned -> device slot 0, one copy): [model table | batch-module table | sine coefficients | per model: boxes, values (edit), host field (build)]
+//   download (device -> pinned, one copy):     [counts (8 words per model) | per model: the listed blocks' table]
+//   device only:                                [per model: mesh words (slots x chunks x MC_BLOCK), launch block sums and offsets, sine tables | change bits]
+namespace {
+struct ModelBatchKernels {cudaKernel_t copy, scatter, diff, changes, marked, count, scan, emit;};
+int model_batch_kernels(tw_ctx *ctx, ModelBatchKernels *K) {
+	static const char *const names[] = {"tw_vmb_copy_kernel", "tw_vmb_box_scatter_kernel", "tw_vmb_diff_kernel", "tw_vmb_change_list_kernel",
+	                                    "tw_vmb_list_marked_kernel", "tw_vmb_mesh_count_kernel", "tw_vmb_mesh_scan_kernel", "tw_vmb_mesh_emit_kernel"};
+	cudaKernel_t k[8];
+	int const rc = module_kernels(ctx, "tw_voxel_model_batch.cubin", names, 8, k); if (rc) return rc;
+	*K = ModelBatchKernels{k[0], k[1], k[2], k[3], k[4], k[5], k[6], k[7]};
+	return TW_OK;
+}
+
+// The refusals every entry shares: a model that is set, of ctx's family and device, at most TWI_VB_MAX_VOXELS, and not named by an earlier entry
+int batch_model_check(tw_ctx *ctx, const tw_voxel_model *m, uint32_t i, std::vector<const tw_voxel_model *> &seen) {
+	if (!m) return tw_set_error(ctx, TW_ERR_ARG, "model %u: model is required", i);
+	int const rc = model_family(ctx, m); if (rc) return entry_error(ctx, "model", i, rc);
+	tw_voxel_post_params const &P = m->P;
+	if ((unsigned long long)P.nx*P.ny*P.nz > TWI_VB_MAX_VOXELS)
+		return tw_set_error(ctx, TW_ERR_ARG, "model %u: %ux%ux%u is more than 2^18 voxels (use the single-model calls)", i, P.nx, P.ny, P.nz);
+	if (std::find(seen.begin(), seen.end(), m) != seen.end()) return tw_set_error(ctx, TW_ERR_ARG, "model %u: the model is named twice in the batch", i);
+	seen.push_back(m);
+	return TW_OK;
+}
+
+// One model of a batch as the host sees it: its descriptor, its outputs and where the completing poll finds its counts and table
+struct BatchModel {
+	tw_voxel_model *m; twi_vmb_model d; tw_voxel_blocks_out O; uint64_t *nchanged;
+	unsigned ng, nvb, nbb;                        // mesh, per-voxel and box launch blocks
+	size_t table_off;                             // the model's table in the download segment, in entries
+	const float *host_in;                         // a build's host field / an edit's values, staged in the upload
+	std::vector<twi_box> B;
+	bool sine;                                    // a build with a sine fill: its axis tables (vb) are in the device carve
+	twi_vbatch_grid vb;                           // a build's fill descriptor
+};
+
+// The carve of a batch (see above) over models M with nvb batch-module descriptors and nsine sine fills; dev: the device carve (else pinned). Returns the
+// upload's and download's bytes.
+struct BatchCarve {twi_vmb_model *tab; twi_vbatch_grid *vb; float *rdata; unsigned long long *counts; tw_voxel_block_mesh *tables; unsigned *bits;
+                   std::vector<char *> in; std::vector<twi_box *> boxes;};
+void batch_carve(twi_carve &c, std::vector<BatchModel> &M, unsigned nvb, unsigned nsine, size_t ntable, size_t nwords, bool dev, BatchCarve &X,
+                 size_t *up_bytes, size_t *down_bytes)
+{
+	size_t const n = M.size();
+	X.in.assign(n, nullptr); X.boxes.assign(n, nullptr);
+	X.tab = c.take<twi_vmb_model>(n); X.vb = nvb ? c.take<twi_vbatch_grid>(nvb) : nullptr; X.rdata = nsine ? c.take<float>((size_t)nsine*TW_N3D_RDATA) : nullptr;
+	for (size_t i = 0; i < n; ++i) {
+		BatchModel &b = M[i];
+		if (!b.B.empty()) {X.boxes[i] = c.take<twi_box>(b.B.size());}
+		if (b.host_in) {X.in[i] = c.take<char>((b.B.empty() ? (size_t)b.d.n : (size_t)b.d.total)*sizeof(float));}
+	}
+	*up_bytes = c.bytes;
+	X.counts = c.take<unsigned long long>(8*n); X.tables = ntable ? c.take<tw_voxel_block_mesh>(ntable) : nullptr;
+	*down_bytes = c.bytes - *up_bytes;
+	X.bits = nullptr;
+	if (!dev) return;
+	for (BatchModel &b : M) {
+		twi_vmb_model &d = b.d;
+		vbatch_sine_tables(c, d.P, b.sine, b.vb);
+		if (!b.ng) {d.words = d.vsums = d.tsums = nullptr; d.voff = d.toff = nullptr; continue;} // no block: the mesh kernels never reach the model
+		d.words = c.take<unsigned>((size_t)b.ng*MC_BLOCK); d.vsums = c.take<unsigned>(b.ng); d.tsums = c.take<unsigned>(b.ng);
+		d.voff = c.take<unsigned long long>(b.ng); d.toff = c.take<unsigned long long>(b.ng);
+	}
+	X.bits = nwords ? c.take<unsigned>(nwords) : nullptr;
+}
+
+// The shared part of both batch launches once the entries are validated: the models' launch blocks, the carve, the descriptors' scratch pointers, the job
+// that unpacks the counts and tables. `vbatch` fills the batch-module descriptors (pinned) given the device carve; `enqueue` the kernels.
+template <typename VBatch, typename Enqueue>
+int launch_model_batch(tw_ctx *ctx, std::vector<BatchModel> &M, unsigned nvb, unsigned nsine, const ModelBatchKernels &K, VBatch &&vbatch, Enqueue &&enqueue) {
+	size_t ntable = 0, nwords = 0;
+	unsigned vb0 = 0, bb0 = 0, mb0 = 0;
+	for (BatchModel &b : M) {
+		twi_vmb_model &d = b.d;
+		b.ng = d.nblocks*d.G.chunks; b.nvb = (d.n + TWI_VMB_VOX_PER_BLOCK - 1)/TWI_VMB_VOX_PER_BLOCK;
+		b.nbb = (unsigned)((d.total + TWI_VMB_BOX_PER_BLOCK - 1)/TWI_VMB_BOX_PER_BLOCK);
+		d.vox_blk0 = vb0; d.box_blk0 = bb0; d.mesh_blk0 = mb0;
+		vb0 += b.nvb; bb0 += b.nbb; mb0 += b.ng;
+		b.table_off = ntable; ntable += d.nblocks;
+		nwords += d.nwords;
+	}
+	BatchCarve D, H;
+	size_t up = 0, down = 0;
+	int rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {batch_carve(c, M, nvb, nsine, ntable, nwords, true, D, &up, &down);}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {batch_carve(c, M, nvb, nsine, ntable, nwords, false, H, &up, &down);}); if (rc) return rc;
+	size_t bo = 0;
+	for (size_t i = 0; i < M.size(); ++i) {
+		BatchModel &b = M[i];
+		twi_vmb_model &d = b.d;
+		d.counts = D.counts + 8*i; d.table = d.nblocks ? D.tables + b.table_off : nullptr;
+		if (d.nwords) {d.bits = D.bits + bo; bo += d.nwords;}
+		if (!b.B.empty()) {memcpy(H.boxes[i], b.B.data(), b.B.size()*sizeof(twi_box)); d.boxes = D.boxes[i];}
+		if (b.host_in) {
+			size_t const nv = b.B.empty() ? (size_t)d.n : (size_t)d.total;
+			memcpy(H.in[i], b.host_in, nv*sizeof(float));
+			if (b.B.empty()) {d.in = (const float *)D.in[i];} else {d.values = (const float *)D.in[i];}
+		}
+		H.tab[i] = d;
+	}
+	vbatch(D, H);
+	struct Out {tw_voxel_blocks_out O; uint64_t *nchanged; const unsigned long long *counts; const tw_voxel_block_mesh *table;};
+	std::vector<Out> outs(M.size());
+	for (size_t i = 0; i < M.size(); ++i) {outs[i] = Out{M[i].O, M[i].nchanged, H.counts + 8*i, M[i].d.nblocks ? H.tables + M[i].table_off : nullptr};}
+	twi_job job; // not cancellable: it commits the models' state
+	job.complete = [outs = std::move(outs)](tw_ctx *) -> int {
+		for (Out const &o : outs) { // as model_job unpacks one model
+			*o.O.nblocks = (uint32_t)o.counts[3]; *o.O.nverts = o.counts[0]; *o.O.ntris = o.counts[1];
+			if (o.O.changed) {*o.O.changed = o.counts[2];}
+			if (o.nchanged) {*o.nchanged = o.counts[4];}
+			if (o.counts[3]) {memcpy(o.O.blocks, o.table, (size_t)o.counts[3]*sizeof(tw_voxel_block_mesh));}
+		}
+		return TW_OK;
+	};
+	unsigned const nm = (unsigned)M.size();
+	for (BatchModel &b : M) {b.m->built = true;} // the job commits the models' state
+	return twi_launch_job(ctx, std::move(job), [&]() -> int {
+		for (BatchModel const &b : M) {TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, b.m->ev, 0));}
+		TW_CUDA(ctx, cudaMemsetAsync(D.counts, 0, 8*M.size()*sizeof(unsigned long long), ctx->stream));
+		if (nwords) {TW_CUDA(ctx, cudaMemsetAsync(D.bits, 0, nwords*sizeof(unsigned), ctx->stream));}
+		TW_CUDA(ctx, cudaMemcpyAsync(D.tab, H.tab, up, cudaMemcpyHostToDevice, ctx->stream));
+		int r = enqueue((const twi_vmb_model *)D.tab, nm, vb0, bb0, (const twi_vbatch_grid *)D.vb); if (r) return r;
+		twi_vmb_model const *const dt = D.tab;
+		if (mb0) {r = launch_module_kernel(ctx, K.count, mb0, (unsigned)MC_BLOCK, dt, nm); if (r) return r;}
+		r = launch_module_kernel(ctx, K.scan, nm, 1024u, dt); if (r) return r;
+		bool any_cap = false;
+		for (BatchModel const &b : M) {any_cap = any_cap || b.d.vcap || b.d.tcap;}
+		if (mb0 && any_cap) {r = launch_module_kernel(ctx, K.emit, mb0, (unsigned)MC_BLOCK, dt, nm); if (r) return r;}
+		TW_CUDA(ctx, cudaMemcpyAsync(H.counts, D.counts, down, cudaMemcpyDeviceToHost, ctx->stream));
+		for (BatchModel const &b : M) {TW_CUDA(ctx, cudaEventRecord(b.m->ev, ctx->stream));}
+		return TW_OK;
+	});
+}
+
+// the descriptor fields a model's build and edit share
+void model_desc(tw_voxel_model *m, const tw_voxel_blocks_out &O, float *d_vt, uint32_t *d_ix, twi_vmb_model &d) {
+	memset(&d, 0, sizeof(d));
+	d.P = m->P; d.G = block_grid(m); d.T = mc_tables(m->tables);
+	d.n = m->P.nx*m->P.ny*m->P.nz; d.nblocks = m->nblocks;
+	d.raw = m->raw; d.post = m->post; d.work = m->work; d.raw_o = m->raw_o; d.post_o = m->post_o; d.work_o = m->work_o; d.mark = m->mark;
+	d.zix = m->zix;
+	d.verts = d_vt; d.vcap = O.vcapacity; d.indices = d_ix; d.tcap = O.tcapacity;
+}
+// a batch-module descriptor of model d's field vals and flags (fill_blk0, the fill and the counts set by the caller)
+twi_vbatch_grid vbatch_desc(const twi_vmb_model &d, float *vals, unsigned char *flags) {
+	twi_vbatch_grid g;
+	memset(&g, 0, sizeof(g));
+	g.P = d.P; g.n = d.n; g.vals = vals; g.flags = flags; g.zix = d.zix; g.counts = d.counts;
+	return g;
+}
+} // namespace
+
+extern "C" int tw_voxel_model_build_batch_launch(tw_ctx *ctx, const tw_voxel_model_build *builds, uint32_t n) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!builds) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_build_batch_launch: null builds");
+	if (n == 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_build_batch_launch: an empty batch");
+	std::vector<BatchModel> M(n);
+	std::vector<tw_voxel_params> F(n);
+	std::vector<const tw_voxel_model *> seen;
+	bool any_glm = false;
+	unsigned nsine = 0, nflood = 0, flood_words = 0, fill_blocks = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		tw_voxel_model_build const &e = builds[i];
+		BatchModel &b = M[i];
+		b.m = e.model; b.nchanged = nullptr; b.host_in = nullptr; b.sine = false;
+		rc = batch_model_check(ctx, e.model, i, seen); if (rc) return rc;
+		if ((e.fill != nullptr) == (e.vals != nullptr)) return tw_set_error(ctx, TW_ERR_ARG, "model %u: give either fill or vals", i);
+		float *d_vt; uint32_t *d_ix;
+		rc = validate_blocks_out(ctx, e.out, &d_vt, &d_ix); if (rc) return entry_error(ctx, "model", i, rc);
+		b.O = *e.out;
+		tw_voxel_post_params const &P = e.model->P;
+		if (e.fill) {
+			F[i] = *e.fill;
+			if (F[i].nx != P.nx || F[i].ny != P.ny || F[i].nz != P.nz)
+				return tw_set_error(ctx, TW_ERR_ARG, "model %u: the fill's grid %ux%ux%u differs from the model's %ux%ux%u", i, F[i].nx, F[i].ny, F[i].nz, P.nx, P.ny, P.nz);
+			size_t tab_bytes = 0;
+			rc = twi_voxel_fill_check(ctx, &F[i], &tab_bytes); if (rc) return entry_error(ctx, "model", i, rc);
+			bool const sine = (F[i].gen_mode == TW_MGEN_SINE);
+			nsine += sine; any_glm = any_glm || !sine; b.sine = sine;
+		}
+		model_desc(e.model, b.O, d_vt, d_ix, b.d);
+		b.d.list = e.model->all;
+		if (e.vals) {if (tw_is_device_ptr(e.vals)) {b.d.in = e.vals;} else {b.host_in = e.vals;}}
+		if (P.remove_unconnected > 0) {++nflood; flood_words = std::max(flood_words, (b.d.n + 31)/32);}
+		fill_blocks += (b.d.n + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS;
+	}
+	BatchKernels VK; ModelBatchKernels K;
+	rc = batch_kernels(ctx, &VK); if (rc) return rc;
+	rc = model_batch_kernels(ctx, &K); if (rc) return rc;
+	size_t lut_bytes, flood_bytes;
+	rc = vbatch_smem(ctx, VK, any_glm, flood_words, &lut_bytes, &flood_bytes); if (rc) return rc;
+	bool const any_in = std::any_of(M.begin(), M.end(), [](const BatchModel &b) {return b.d.in || b.host_in;});
+	// batch-module descriptors: n for the fill (raw / raw_o), then one per flooded model (post / post_o)
+	auto vbatch = [&](BatchCarve &D, BatchCarve &H) {
+		unsigned fb = 0, si = 0, fl = 0;
+		for (uint32_t i = 0; i < n; ++i) {
+			twi_vmb_model const &d = M[i].d;
+			twi_vbatch_grid g = vbatch_desc(d, M[i].m->raw, M[i].m->raw_o);
+			g.counts = D.counts + 8*i;
+			bool const fill = (builds[i].fill != nullptr), sine = fill && F[i].gen_mode == TW_MGEN_SINE;
+			vbatch_fill_params(fill ? &F[i] : nullptr, builds[i].rdata420, H.rdata + (size_t)si*TW_N3D_RDATA, D.rdata + (size_t)si*TW_N3D_RDATA, g);
+			si += sine;
+			twi_vbatch_grid const &t = M[i].vb;
+			g.xt = t.xt; g.yt = t.yt; g.zt = t.zt; g.xp = t.xp; g.yp = t.yp; g.zp = t.zp;
+			g.fill_blk0 = fb; fb += (d.n + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS;
+			H.vb[i] = g;
+			if (d.P.remove_unconnected > 0) {
+				twi_vbatch_grid f = vbatch_desc(d, M[i].m->post, M[i].m->post_o);
+				f.counts = D.counts + 8*i;
+				H.vb[n + fl++] = f;
+			}
+		}
+	};
+	auto enqueue = [&](const twi_vmb_model *dt, unsigned nm, unsigned vox_blocks, unsigned, const twi_vbatch_grid *vb) -> int {
+		int r;
+		if (any_in) {r = launch_module_kernel(ctx, K.copy, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm, (int)TWI_VMB_COPY_IN); if (r) return r;}
+		if (nsine) {r = launch_module_kernel_smem(ctx, VK.tables, dim3(3, n), 64u, 0, vb, (const float *)ctx->d_sin_table); if (r) return r;}
+		r = launch_module_kernel_smem(ctx, VK.fill, dim3(fill_blocks), TWI_VB_FILL_THREADS, lut_bytes, vb, n, (const float4 *)ctx->d_glm3_lut); if (r) return r;
+		r = launch_module_kernel(ctx, K.copy, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm, (int)TWI_VMB_COPY_POST); if (r) return r;
+		if (nflood) {r = launch_module_kernel_smem(ctx, VK.flood, dim3(nflood), TWI_VB_FLOOD_THREADS, flood_bytes, vb + n); if (r) return r;}
+		return TW_OK;
+	};
+	return launch_model_batch(ctx, M, n + nflood, nsine, K, vbatch, enqueue);
+}
+
+extern "C" int tw_voxel_model_edit_batch_launch(tw_ctx *ctx, const tw_voxel_model_edit *edits, uint32_t n) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!edits) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_edit_batch_launch: null edits");
+	if (n == 0) return tw_set_error(ctx, TW_ERR_ARG, "tw_voxel_model_edit_batch_launch: an empty batch");
+	std::vector<BatchModel> M(n);
+	std::vector<const tw_voxel_model *> seen;
+	unsigned nflood = 0, flood_words = 0;
+	bool any_list = false;
+	for (uint32_t i = 0; i < n; ++i) {
+		tw_voxel_model_edit const &e = edits[i];
+		BatchModel &b = M[i];
+		b.m = e.model; b.nchanged = nullptr; b.host_in = nullptr; b.sine = false;
+		rc = batch_model_check(ctx, e.model, i, seen); if (rc) return rc;
+		if (e.nboxes && (!e.boxes || !e.values)) return tw_set_error(ctx, TW_ERR_ARG, "model %u: null boxes or values", i);
+		float *d_vt; uint32_t *d_ix;
+		rc = validate_blocks_out(ctx, e.out, &d_vt, &d_ix); if (rc) return entry_error(ctx, "model", i, rc);
+		b.O = *e.out;
+		ChangeOut CO;
+		if (e.ch) {rc = validate_changes(ctx, e.ch, &CO); if (rc) return entry_error(ctx, "model", i, rc);}
+		tw_voxel_model *const m = e.model;
+		unsigned long long total = 0;
+		rc = model_boxes(ctx, m->P, e.boxes, e.nboxes, b.B, &total); if (rc) return entry_error(ctx, "model", i, rc);
+		if (!m->built) return tw_set_error(ctx, TW_ERR_STATE, "model %u: the voxel model has no field yet (tw_voxel_model_build_launch)", i);
+		model_desc(m, b.O, d_vt, d_ix, b.d);
+		twi_vmb_model &d = b.d;
+		d.list = m->marked; d.nboxes = e.nboxes; d.total = total;
+		if (total) {b.host_in = e.values;}
+		d.flood = (m->P.remove_unconnected > 0 && total) ? 1 : 0;
+		if (d.flood) {++nflood; flood_words = std::max(flood_words, (d.n + 31)/32);}
+		if (e.ch) {
+			b.nchanged = CO.nchanged;
+			if (total) { // only an edit with boxes can change a voxel: without them the count stays 0
+				d.nwords = (d.n + 31)/32; any_list = true; // launch_model_batch carves the bits
+				d.ch_index = CO.index; d.ch_vals = CO.vals; d.ch_outside = CO.outside; d.ch_cap = CO.capacity;
+			}
+		}
+	}
+	BatchKernels VK; ModelBatchKernels K;
+	if (nflood) {rc = batch_kernels(ctx, &VK); if (rc) return rc;}
+	rc = model_batch_kernels(ctx, &K); if (rc) return rc;
+	size_t lut_bytes = 0, flood_bytes = 0;
+	if (nflood) {rc = vbatch_smem(ctx, VK, false, flood_words, &lut_bytes, &flood_bytes); if (rc) return rc;}
+	// batch-module descriptors: one per flooded model (work / work_o)
+	auto vbatch = [&](BatchCarve &D, BatchCarve &H) {
+		unsigned fl = 0;
+		for (uint32_t i = 0; i < n; ++i) {
+			if (!M[i].d.flood) continue;
+			twi_vbatch_grid f = vbatch_desc(M[i].d, M[i].m->work, M[i].m->work_o);
+			f.counts = D.counts + 8*i;
+			H.vb[fl++] = f;
+		}
+	};
+	auto enqueue = [&](const twi_vmb_model *dt, unsigned nm, unsigned vox_blocks, unsigned box_blocks, const twi_vbatch_grid *vb) -> int {
+		int r;
+		if (box_blocks) {r = launch_module_kernel(ctx, K.scatter, box_blocks, TWI_VMB_BOX_THREADS, dt, nm); if (r) return r;}
+		if (nflood) {
+			r = launch_module_kernel(ctx, K.copy, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm, (int)TWI_VMB_COPY_WORK); if (r) return r;
+			r = launch_module_kernel_smem(ctx, VK.flood, dim3(nflood), TWI_VB_FLOOD_THREADS, flood_bytes, vb); if (r) return r;
+			r = launch_module_kernel(ctx, K.diff, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm); if (r) return r;
+		}
+		if (any_list) {r = launch_module_kernel(ctx, K.changes, nm, 1024u, dt); if (r) return r;}
+		return launch_module_kernel(ctx, K.marked, nm, 1024u, dt);
+	};
+	return launch_model_batch(ctx, M, nflood, 0, K, vbatch, enqueue);
 }

@@ -1199,13 +1199,23 @@ inline tiles_job voxel_build_batch_async(tw_voxel_build const *grids, tw_voxel_m
 // every job launched before it. With a `pool` (a tile_job_pool of this thread's context) each job runs on a free slot instead of the thread's context, so a
 // stroke never waits for the previous one or for the frame's tile jobs; the model orders its jobs on the device in launch order. Not copyable; destroyed
 // with the context's pending job completed and the model's jobs on pool slots done.
+class voxel_model;
+// One model of voxel_model_build_batch_async / voxel_model_edit_batch_async and the arguments of its build_async / edit_async
+struct voxel_model_build_args {voxel_model *model; tw_voxel_params const *fill; const float *vals; tw_voxel_blocks_out const *out;};
+struct voxel_model_edit_args {voxel_model *model; std::vector<tw_voxel_box> boxes; const float *values; tw_voxel_blocks_out const *out; tw_voxel_changes const *changes;};
+tiles_job voxel_model_build_batch_async(std::vector<voxel_model_build_args> const &builds, tile_job_pool *pool);
+tiles_job voxel_model_edit_batch_async(std::vector<voxel_model_edit_args> const &edits, tile_job_pool *pool);
 class voxel_model {
 	tw_voxel_model *m = nullptr;
 	tw_ctx *c = nullptr;
 	size_t n = 0;
+	friend tiles_job voxel_model_build_batch_async(std::vector<voxel_model_build_args> const &, tile_job_pool *);
+	friend tiles_job voxel_model_edit_batch_async(std::vector<voxel_model_edit_args> const &, tile_job_pool *);
 	// launch(lc) on this model's context, or on a slot of pool
-	template <typename Launch> tiles_job job_on(tile_job_pool *pool, const char *what, Launch &&launch) {
-		tw_ctx *lc = c;
+	template <typename Launch> tiles_job job_on(tile_job_pool *pool, const char *what, Launch &&launch) {return job_on(c, pool, what, launch);}
+	// launch(lc) on home, or on a slot of pool
+	template <typename Launch> static tiles_job job_on(tw_ctx *home, tile_job_pool *pool, const char *what, Launch &&launch) {
+		tw_ctx *lc = home;
 		std::atomic<uint64_t> *jobs = &detail::tls().tile_jobs;
 		if (pool) {tile_job_pool::slot &sl = pool->next(); lc = sl.c; jobs = &sl.jobs;}
 		uint64_t const number = ++*jobs;
@@ -1270,6 +1280,26 @@ public:
 		if (rc != TW_OK) {detail::fail(rc, "voxel_model::read", c);}
 	}
 };
+// Many small voxel models (at most 2^18 voxels each) - rock and asteroid models - built or edited in ONE job (tw_voxel_model_build_batch_launch /
+// tw_voxel_model_edit_batch_launch), on the thread's context or on a slot of pool: entry i gives what its model's build_async / edit_async would give, byte
+// for byte, once the returned tiles_job is ready, and the models order the job against their other jobs as those do. The entries are read during the launch.
+inline tiles_job voxel_model_build_batch_async(std::vector<voxel_model_build_args> const &builds, tile_job_pool *pool = nullptr) {
+	std::vector<tw_voxel_model_build> e(builds.size());
+	for (size_t i = 0; i < builds.size(); ++i) {e[i] = {builds[i].model->m, builds[i].fill, nullptr, builds[i].vals, builds[i].out};}
+	return voxel_model::job_on(ctx(), pool, "voxel_model_build_batch_async", [&](tw_ctx *lc) {
+		return tw_voxel_model_build_batch_launch(lc, e.data(), (uint32_t)e.size());
+	});
+}
+inline tiles_job voxel_model_edit_batch_async(std::vector<voxel_model_edit_args> const &edits, tile_job_pool *pool = nullptr) {
+	std::vector<tw_voxel_model_edit> e(edits.size());
+	for (size_t i = 0; i < edits.size(); ++i) {
+		voxel_model_edit_args const &a = edits[i];
+		e[i] = {a.model->m, a.boxes.data(), (uint32_t)a.boxes.size(), a.values, a.out, a.changes};
+	}
+	return voxel_model::job_on(ctx(), pool, "voxel_model_edit_batch_async", [&](tw_ctx *lc) {
+		return tw_voxel_model_edit_batch_launch(lc, e.data(), (uint32_t)e.size());
+	});
+}
 
 // ------------------------------------------------------------------------------------------------ all GPUs of the box (include/tw3d.h "Multi-GPU")
 // One object per process: per-device contexts with the current tables, NUMA-local pinned output bands, the tile loop of tile_draw_t::update

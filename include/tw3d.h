@@ -817,6 +817,38 @@ TW_API int  tw_voxel_model_read(tw_voxel_model *m, float *raw, float *vals, uint
  * ctx or model, a context of another family or device, NULL boxes with nboxes > 0, an empty box or one reaching outside the grid; TW_ERR_STATE before the
  * model's first build has been launched. */
 TW_API int  tw_voxel_model_read_launch(tw_ctx *ctx, tw_voxel_model *m, const tw_voxel_box *boxes, uint32_t nboxes, float *raw, float *vals, uint8_t *outside);
+/* Many small models built, or edited, in ONE asynchronous job - an engine's rock and asteroid models, loaded together or hit by the same frame's brushes.
+ * Entry i names a model and the arguments of its single call: after the completing poll each entry gives what tw_voxel_model_build_launch_on(ctx, model,
+ * fill, rdata420, vals, out) or tw_voxel_model_edit_launch_on(ctx, model, boxes, nboxes, values, out, ch) would give for that model alone, bit for bit:
+ * the raw field, the field and flags after remove_unconnected, the block table, vertices and indices up to their capacities, *nblocks, *nverts, *ntris,
+ * *changed, the change list and *nchanged. The job launches the same kernels whatever n is, each over every model, and floods each model's
+ * remove_unconnected inside one SM's shared memory, as tw_voxel_build_batch_launch does (DESIGN.md section 4m); each model costs one event wait and one
+ * event record, not a launch.
+ * - Job and family rules: those of the _on calls. The job is ctx's pending job (tw_create_tiles_poll completes it); every model belongs to ctx's family and
+ *   device; the job waits for each model's earlier jobs on any context before it touches that model and orders its later ones. Model state is committed
+ *   at launch, so tw_cancel returns TW_ERR_STATE. The entries array, boxes and values are read during the launch.
+ * - Size limit: nx*ny*nz <= 2^18 per model; larger models stay on the single calls.
+ * - Errors, nothing enqueued and no model changed: TW_ERR_ARG for NULL arrays, n == 0, a NULL model, a model above the limit, a model named twice, a
+ *   model of another family or device, and every refusal of the single call for an entry; TW_ERR_STATE for an edit of a model never built, and where
+ *   the single call returns it. tw_last_error names the entry's index. TW_ERR_CUDA when tw_voxel_model_batch.cubin or tw_voxel_batch.cubin, the sm_90a
+ *   modules beside the library, cannot be loaded. */
+typedef struct tw_voxel_model_build {
+	tw_voxel_model            *model;     /* required */
+	const tw_voxel_params     *fill;      /* exactly one of fill / vals, as tw_voxel_model_build_launch */
+	const float               *rdata420;  /* optional, sine fill only */
+	const float               *vals;      /* n floats, host or device */
+	const tw_voxel_blocks_out *out;       /* required */
+} tw_voxel_model_build;
+TW_API int tw_voxel_model_build_batch_launch(tw_ctx *ctx, const tw_voxel_model_build *builds, uint32_t n);
+typedef struct tw_voxel_model_edit {
+	tw_voxel_model            *model;     /* required */
+	const tw_voxel_box        *boxes;     /* as tw_voxel_model_edit_launch; nboxes 0 = no change, no block listed */
+	uint32_t                   nboxes;
+	const float               *values;
+	const tw_voxel_blocks_out *out;       /* required */
+	const tw_voxel_changes    *ch;        /* optional, as tw_voxel_model_edit_launch_ex */
+} tw_voxel_model_edit;
+TW_API int tw_voxel_model_edit_batch_launch(tw_ctx *ctx, const tw_voxel_model_edit *edits, uint32_t n);
 
 /* ---- mesh shadows of tiles (SURVEY.md 8f row N4): calc_mesh_shadows (src/visibility.cpp:411-517) for a batch of tiles with the neighbour chaining of
  * tile_t::calc_shadows_for_light (src/tiled_mesh.cpp:664-692) ---- */

@@ -190,6 +190,13 @@ class HmapReadArgs(C.Structure):
     _fields_ = [("rects", C.c_void_p), ("nrects", C.c_uint32), ("dst16", C.c_void_p), ("dst_pitch", C.c_size_t)]
 
 
+class HmapAoJobArgs(C.Structure):
+    """tw_hmap_ao_job (include/tw3d.h): the tiles of one tw_hmap_tile_ao_launch, where their final zvals come from (zvals, or the resident tiles tile_xy of
+    a tile set) and where their AO maps go."""
+    _fields_ = [("hs", C.c_void_p), ("origins_xy", C.c_void_p), ("ntiles", C.c_uint32), ("zvsize", C.c_uint32), ("half_dxy", C.c_float),
+                ("zvals", C.c_void_p), ("set", C.c_void_p), ("tile_xy", C.c_void_p), ("ao", C.c_void_p)]
+
+
 class HeightmapInfo(C.Structure):
     _fields_ = [("min_z", C.c_float), ("max_z", C.c_float), ("val_mult", C.c_float), ("val_add", C.c_float), ("mesh_file_scale", C.c_float),
                 ("mesh_file_tz", C.c_float), ("erosion_moves", C.c_uint64)]
@@ -260,7 +267,7 @@ ABI_SYMBOLS = ["tw_abi_version", "tw_create", "tw_create_shared", "tw_destroy", 
                "tw_voxel_model_edit_launch_ex", "tw_voxel_model_build_launch_on", "tw_voxel_model_edit_launch_on", "tw_voxel_model_read_launch",
                "tw_points_launch", "tw_gen_mesh_launch", "tw_mesh_shadows", "tw_mesh_shadows_launch", "tw_gen_mesh_launch_shadows",
                "tw_read_heightmap_launch", "tw_read_heightmap", "tw_voxel_build_batch_launch",
-               "tw_voxel_model_build_batch_launch", "tw_voxel_model_edit_batch_launch"]
+               "tw_voxel_model_build_batch_launch", "tw_voxel_model_edit_batch_launch", "tw_hmap_tile_ao_launch", "tw_hmap_tile_ao"]
 
 
 def _load():
@@ -322,6 +329,8 @@ def _load():
     L.tw_update_heightmap.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32]
     L.tw_read_heightmap_launch.argtypes = [vp, C.POINTER(HmapReadArgs)]
     L.tw_read_heightmap.argtypes = [vp, C.POINTER(HmapReadArgs)]
+    L.tw_hmap_tile_ao_launch.argtypes = [vp, C.POINTER(HmapAoJobArgs)]
+    L.tw_hmap_tile_ao.argtypes = [vp, C.POINTER(HmapAoJobArgs)]
     L.tw_hmap_tiles_touched.argtypes = [C.POINTER(HmapSampler), vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.tw_eval_points.argtypes = [vp, vp, C.c_size_t, C.POINTER(HeightParams), C.POINTER(PointQuery), vp]
     L.tw_points_launch.argtypes = [vp, C.POINTER(PointsJobArgs)]
@@ -705,6 +714,11 @@ class PointsJob:
         return self.out if self._ctx.create_tiles_poll(wait) else None
 
 
+class HmapAoJob(PointsJob):
+    """What Context.hmap_tile_ao_launch and TileSet.hmap_ao_launch return: poll(wait) completes the job (the pending job of the Context it was launched
+    on) and returns the AO maps [nt, stride, stride] uint8, or None while it runs (wait=False)."""
+
+
 class HmapReadJob(PointsJob):
     """What Context.read_heightmap_launch returns: poll(wait) completes the job (the context's pending job) and returns out, or None while it runs
     (wait=False)."""
@@ -1030,6 +1044,32 @@ class Context:
         job = HmapReadJob(self, out)
         self._tiles_job = (out, job)
         return job
+
+    def _hmap_ao_launch(self, hs, origins_xy, zvsize, half_dxy, zvals=None, tset=None, tile_xy=None, out=None):
+        org = np.ascontiguousarray(origins_xy, np.int32).reshape(-1, 2)
+        nt, zv = len(org), int(zvsize)
+        if out is None:
+            out = np.empty((nt, zv - 1, zv - 1), np.uint8)
+        if zvals is not None and not hasattr(zvals, "data_ptr"):
+            zvals = np.ascontiguousarray(zvals, np.float32)
+        txy = None if tile_xy is None else TileSet._xy(tile_xy)
+        a = HmapAoJobArgs(C.cast(C.pointer(hs), C.c_void_p) if hs is not None else None, _ptr(org) if nt else None, nt, zv, half_dxy, _ptr(zvals),
+                          tset._h if tset is not None else None, _ptr(txy) if txy is not None and len(txy) else None, _ptr(out))
+        self._check(lib.tw_hmap_tile_ao_launch(self._h, C.byref(a)))
+        job = HmapAoJob(self, out)
+        self._tiles_job = (org, zvals, txy, out, hs, job)
+        return job
+
+    def hmap_tile_ao_launch(self, hs, origins_xy, zvals, half_dxy, out=None):
+        """tw_hmap_tile_ao_launch: the AO maps of heightmap-texture tiles (origins_xy [nt, 2] (x1, y1)) from their final zvals [nt, zv, zv] float32 (numpy
+        or torch, host or CUDA; host zvals are copied during the launch) and the set_heightmap image under hs (HmapSampler), as this context's
+        asynchronous job. out = [nt, zv - 1, zv - 1] uint8, host or CUDA (default a new numpy array). The job sees every update_heightmap made before the
+        launch and none after it. Returns a HmapAoJob whose poll returns out."""
+        return self._hmap_ao_launch(hs, origins_xy, int(zvals.shape[1]), half_dxy, zvals=zvals, out=out)
+
+    def hmap_tile_ao(self, hs, origins_xy, zvals, half_dxy, out=None):
+        """tw_hmap_tile_ao: hmap_tile_ao_launch completed at once; returns the AO maps."""
+        return self.hmap_tile_ao_launch(hs, origins_xy, zvals, half_dxy, out).poll(wait=True)
 
     def read_heightmap(self, rects=None, out=None):
         """tw_read_heightmap: read_heightmap_launch(rects, out) completed at once; returns out (default the whole image as a new uint8 [h, w, 2] array)."""
@@ -1576,6 +1616,13 @@ class TileSet:
         self.ctx._check(lib.tw_tile_set_shadows_launch(self._h, C.byref(req)))
         self.ctx._tiles_job = ([(r.smask, r.sh_out_x, r.sh_out_y) for r in recs], arr)
         return recomputed
+
+    def hmap_ao_launch(self, tile_xy, origins_xy, hs, half_dxy, out=None, ctx=None):
+        """tw_hmap_tile_ao_launch on the resident tiles tile_xy [n, 2] of this set (origins origins_xy [n, 2] (x1, y1)): their AO maps from the zvals the set
+        holds and the set_heightmap image under hs, as the asynchronous job of ctx - this set's Context (None), its parent or a shared Context of that
+        parent. The job is ordered after the set's earlier device work on any of them (a frame launched just before needs no poll). Returns a HmapAoJob."""
+        c = self.ctx if ctx is None else ctx
+        return c._hmap_ao_launch(hs, origins_xy, self.zvsize, half_dxy, tset=self, tile_xy=tile_xy, out=out)
 
     def stale_after(self, sps, remove_xy=None, put_xy=None):
         """tw_tile_set_stale_after: what stale(sps) would return after remove(remove_xy) and put(put_xy), without changing the set - the tiles to name in

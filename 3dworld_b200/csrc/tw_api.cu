@@ -1,6 +1,7 @@
 // tw_api.cu - the extern "C" boundary (include/tw3d.h): context management, host/device pointer staging, and dispatch to the kernels.
 // There is deliberately NO CPU path in this library: without a CUDA device tw_create fails and nothing else can be called.
 #include "tw_internal.h"
+#include "tw_hmap_ao.h"
 #include <algorithm>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -386,7 +387,7 @@ int tw_cancel(tw_ctx *ctx) {
 	twi_job const &j = ctx->async.job;
 	if (!j.complete) return TW_OK;
 	if (!j.cancellable) return tw_set_error(ctx, TW_ERR_STATE, "the pending job cannot be cancelled: a job that touches a tile set or a voxel model committed its state at "
-	                                                           "its launch, and a points job or a heightmap read has no cancellation point");
+	                                                           "its launch, and a points job, a heightmap read or a heightmap AO job has no cancellation point");
 	ctx->h_job->cancel = j.seq;
 	TW_CUDA(ctx, cudaMemcpyAsync(&ctx->d_job_words->cancel, &ctx->h_job->cancel, sizeof(unsigned), cudaMemcpyHostToDevice, ctx->cancel_stream));
 	ctx->cancel_sent = true;
@@ -1126,6 +1127,78 @@ int tw_read_heightmap_launch(tw_ctx *ctx, const tw_hmap_read *r) {
 
 int tw_read_heightmap(tw_ctx *ctx, const tw_hmap_read *r) {
 	int const rc = tw_read_heightmap_launch(ctx, r);
+	return rc ? rc : poll_job(ctx, 1);
+}
+
+// The AO of heightmap tiles as one launch of tw_hmap_ao.cubin's kernel: one CTA per (tile, sub-square), each with the heights its rays reach in shared
+// memory. Sub-squares have at most TWI_AO_MAX_SIDE cells a side; when the tiles would give fewer CTAs than the device has SMs (a frame's few new tiles), the
+// tiles are cut finer so that every SM gets work. Slot 0: [origins | set slots | zvals (host zvals) | ao (host ao)]; pinned staging: [origins | set slots |
+// zvals (host zvals) | ao (pageable ao)].
+int tw_hmap_tile_ao_launch(tw_ctx *ctx, const tw_hmap_ao_job *job) {
+	int rc = twi_begin(ctx); if (rc) return rc;
+	if (!job) return tw_set_error(ctx, TW_ERR_ARG, "null job");
+	if (!job->hs) return tw_set_error(ctx, TW_ERR_ARG, "null heightmap sampler");
+	if (job->hs->edge_mode < 0 || job->hs->edge_mode > 2) return tw_set_error(ctx, TW_ERR_ARG, "bad edge_mode %d", job->hs->edge_mode);
+	if (job->zvsize < 2) return tw_set_error(ctx, TW_ERR_ARG, "zvsize %u < 2", job->zvsize);
+	if (!job->zvals == !job->set) return tw_set_error(ctx, TW_ERR_ARG, "exactly one of zvals and set is required");
+	if (!job->ao) return tw_set_error(ctx, TW_ERR_ARG, "null ao");
+	uint32_t const n = job->ntiles, zv = job->zvsize, stride = zv - 1;
+	if (n && (!job->origins_xy || (job->set && !job->tile_xy))) return tw_set_error(ctx, TW_ERR_ARG, "null origins_xy, or a set without tile_xy, with ntiles > 0");
+	if (n == 0) return TW_OK;
+	rc = validate_hmap(ctx, job->hs, nullptr); if (rc) return rc;
+	std::vector<int> slots;
+	const float *slab = nullptr;
+	cudaEvent_t set_ev = nullptr;
+	if (job->set) {rc = twi_tile_set_tiles(ctx, job->set, job->tile_xy, n, zv, slots, &slab, &set_ev); if (rc) return rc;}
+	unsigned nsub = (stride + TWI_AO_MAX_SIDE - 1)/TWI_AO_MAX_SIDE;
+	while (nsub < stride && (size_t)n*nsub*nsub < ctx->num_sms) ++nsub;
+	unsigned const side = (stride + nsub - 1)/nsub;
+	nsub = (stride + side - 1)/side;
+	if ((size_t)n*nsub*nsub > 0x7fffffffu) return tw_set_error(ctx, TW_ERR_ARG, "too many tiles in one job");
+	size_t const ao_bytes = (size_t)n*stride*stride, smem = (size_t)(side + 2*TWI_AO_RAY_LEN)*(side + 2*TWI_AO_RAY_LEN)*sizeof(float);
+	static const char *const names[] = {"tw_hmap_ao_kernel"};
+	cudaKernel_t k;
+	rc = twi_module_kernels(ctx, "tw_hmap_ao.cubin", names, 1, &k); if (rc) return rc;
+	TW_CUDA(ctx, cudaKernelSetAttributeForDevice(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem, ctx->device));
+	twi_user<const float> z(job->zvals, job->set ? 0 : (size_t)n*zv*zv);
+	uint8_t *const ao = job->ao;
+	bool const dev_out = tw_is_device_ptr(ao), locked_out = !dev_out && twi_is_page_locked(ao);
+	int32_t *d_org, *h_org; int *d_slots = nullptr, *h_slots = nullptr;
+	uint8_t *d_ao = ao, *h_ao = nullptr;
+	rc = twi_reserve_carve(ctx, 0, [&](twi_carve &c) {
+		d_org = c.take<int32_t>(2*(size_t)n); if (job->set) {d_slots = c.take<int>(n);}
+		z.take(c); if (!dev_out) {d_ao = c.take<uint8_t>(ao_bytes);}
+	}); if (rc) return rc;
+	rc = twi_reserve_carve(ctx, TWI_PINNED, [&](twi_carve &c) {
+		h_org = c.take<int32_t>(2*(size_t)n); if (job->set) {h_slots = c.take<int>(n);}
+		z.take_pinned(c); if (!dev_out && !locked_out) {h_ao = c.take<uint8_t>(ao_bytes);}
+	}); if (rc) return rc;
+	memcpy(h_org, job->origins_xy, 2*(size_t)n*sizeof(int32_t));
+	if (job->set) {memcpy(h_slots, slots.data(), n*sizeof(int));}
+	twi_hmap_ao_args A;
+	A.img = ctx->d_hmap; A.origins = d_org; A.zvals = job->set ? slab : z.d; A.slots = d_slots; A.ao = d_ao; A.H = *job->hs;
+	A.zvsize = zv; A.side = side; A.nsub = nsub; A.dz = (float)(0.5*job->half_dxy); // src/tiled_mesh.cpp:612
+	twi_job pending;
+	pending.reads_image = true; // one kernel: no cancellation point
+	pending.complete = [h_ao, ao, ao_bytes](tw_ctx *) -> int {if (h_ao) {memcpy(ao, h_ao, ao_bytes);} return TW_OK;};
+	return twi_launch_job(ctx, std::move(pending), [&]() -> int {
+		TW_CUDA(ctx, cudaMemcpyAsync(d_org, h_org, 2*(size_t)n*sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+		if (job->set) {TW_CUDA(ctx, cudaMemcpyAsync(d_slots, h_slots, n*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));}
+		int r = z.in(ctx); if (r) return r;
+		if (job->set) {TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, set_ev, 0));} // a frame on another context may still write the slab
+		void *args[] = {&A};
+		TW_CUDA(ctx, cudaLaunchKernel((const void *)k, dim3(n*nsub*nsub), dim3(TWI_AO_THREADS), args, smem, ctx->stream));
+		ctx->launches++;
+		TW_CUDA(ctx, cudaEventRecord(ctx->async.image_free, ctx->stream)); // a later edit waits for this kernel only
+		ctx->async.image_free_set = true;
+		if (job->set) {TW_CUDA(ctx, cudaEventRecord(set_ev, ctx->stream));}
+		if (!dev_out) {TW_CUDA(ctx, cudaMemcpyAsync(locked_out ? ao : h_ao, d_ao, ao_bytes, cudaMemcpyDeviceToHost, ctx->stream));}
+		return TW_OK;
+	});
+}
+
+int tw_hmap_tile_ao(tw_ctx *ctx, const tw_hmap_ao_job *job) {
+	int const rc = tw_hmap_tile_ao_launch(ctx, job);
 	return rc ? rc : poll_job(ctx, 1);
 }
 

@@ -350,6 +350,13 @@ struct twi_job_tail {
 int twi_create_tiles_launch(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
                             uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
                             const tw_tile_outputs *out, const tw_tile_shading *shading, twi_job_tail *tail);
+// Device code the library loads at run time (build.py's MODULES; tw_voxel_post.cu): the kernels `names` of the sm_90a module `file` beside this library,
+// loaded once per process on first use (cudaLibraryLoadFromFile loads it into each device's context as needed). A missing or unloadable module is an error.
+int twi_module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int count, cudaKernel_t *out);
+// The resident tiles a job reads from a tile set (tw_hmap_tile_ao_launch; tw_tileset.cu): TW_ERR_ARG on ctx unless ctx is of the set's family and device,
+// zvsize is the set's and tile_xy names n distinct resident tiles. slots = their slab slots, *d_z = the zvals slab, *ev = the set's event, which the job
+// waits on before it reads the slab and records once it no longer does.
+int twi_tile_set_tiles(tw_ctx *ctx, tw_tile_set *s, const int32_t *tile_xy, uint32_t n, uint32_t zvsize, std::vector<int> &slots, const float **d_z, cudaEvent_t *ev);
 int twi_eval_points(tw_ctx *ctx, const float *d_xy, size_t n, const tw_height_params *p, const tw_point_query *q, float *d_out);
 // twi_eval_points' refusals (TW_ERR_ARG / TW_ERR_STATE), without enqueuing anything
 int twi_eval_points_check(tw_ctx *ctx, size_t n, const tw_height_params *p, const tw_point_query *q);

@@ -329,6 +329,22 @@ struct frame_tail : twi_job_tail {
 
 } // namespace
 
+int twi_tile_set_tiles(tw_ctx *ctx, tw_tile_set *s, const int32_t *tile_xy, uint32_t n, uint32_t zvsize, std::vector<int> &slots, const float **d_z, cudaEvent_t *ev) {
+	tw_ctx const *root = ctx->parent ? ctx->parent : ctx, *set_root = s->ctx->parent ? s->ctx->parent : s->ctx;
+	if (root != set_root || ctx->device != s->ctx->device) return tw_set_error(ctx, TW_ERR_ARG, "tile set: ctx is neither the set's context, its parent nor a shared context of that parent");
+	if (zvsize != s->zvsize) return tw_set_error(ctx, TW_ERR_ARG, "tile set: zvsize %u differs from the set's %u", zvsize, s->zvsize);
+	std::vector<twts::key> keys;
+	if (!read_keys(tile_xy, n, keys)) return tw_set_error(ctx, TW_ERR_ARG, "tile set: tile_xy names a tile twice");
+	slots.resize(n);
+	for (uint32_t i = 0; i < n; ++i) {
+		auto const it = s->st.where.find(keys[i]);
+		if (it == s->st.where.end()) return tw_set_error(ctx, TW_ERR_ARG, "tile set: tile (%d, %d) is not resident", keys[i].first, keys[i].second);
+		slots[i] = (int)it->second;
+	}
+	*d_z = s->d_z; *ev = s->ev;
+	return TW_OK;
+}
+
 extern "C" {
 
 int tw_tile_set_create(tw_ctx *ctx, uint32_t zvsize, uint32_t nlights, tw_tile_set **out) {

@@ -1116,9 +1116,9 @@ int validate_changes(tw_ctx *ctx, const tw_voxel_changes *ch, ChangeOut *d) {
 	return TW_OK;
 }
 
-// Device code the library loads at run time (build.py's MODULES): the kernels `names` of the sm_90a module `file` beside this library, loaded once per
-// process on first use (cudaLibraryLoadFromFile loads it into each device's context as needed). A missing or unloadable module is an error.
-int module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int count, cudaKernel_t *out) {
+} // namespace
+
+int twi_module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int count, cudaKernel_t *out) {
 	static std::mutex mu;
 	static std::vector<std::pair<std::string, std::vector<cudaKernel_t>>> loaded; // per file, its kernels in the order of names
 	std::lock_guard<std::mutex> g(mu);
@@ -1139,12 +1139,14 @@ int module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int 
 	for (int i = 0; i < count; ++i) {out[i] = k[i];}
 	return TW_OK;
 }
+
+namespace {
 // The change-list kernels (tw_voxel_changes.cu), from tw_voxel_changes.cubin
 struct ChangeKernels {cudaKernel_t box_bits, diff_bits, count, emit;};
 int change_kernels(tw_ctx *ctx, ChangeKernels *K) {
 	static const char *const names[] = {"tw_box_scatter_bits_kernel", "tw_diff_bits_kernel", "tw_change_count_kernel", "tw_change_emit_kernel"};
 	cudaKernel_t k[4];
-	int const rc = module_kernels(ctx, "tw_voxel_changes.cubin", names, 4, k); if (rc) return rc;
+	int const rc = twi_module_kernels(ctx, "tw_voxel_changes.cubin", names, 4, k); if (rc) return rc;
 	*K = ChangeKernels{k[0], k[1], k[2], k[3]};
 	return TW_OK;
 }
@@ -1316,7 +1318,7 @@ int batch_kernels(tw_ctx *ctx, BatchKernels *K) {
 	static const char *const names[] = {"tw_vbatch_tables_kernel", "tw_vbatch_fill_kernel", "tw_vbatch_flood_kernel", "tw_vbatch_mesh_count_kernel",
 	                                    "tw_vbatch_mesh_scan_kernel", "tw_vbatch_mesh_emit_kernel"};
 	cudaKernel_t k[6];
-	int const rc = module_kernels(ctx, "tw_voxel_batch.cubin", names, 6, k); if (rc) return rc;
+	int const rc = twi_module_kernels(ctx, "tw_voxel_batch.cubin", names, 6, k); if (rc) return rc;
 	*K = BatchKernels{k[0], k[1], k[2], k[3], k[4], k[5]};
 	return TW_OK;
 }
@@ -1502,7 +1504,7 @@ int model_batch_kernels(tw_ctx *ctx, ModelBatchKernels *K) {
 	static const char *const names[] = {"tw_vmb_copy_kernel", "tw_vmb_box_scatter_kernel", "tw_vmb_diff_kernel", "tw_vmb_change_list_kernel",
 	                                    "tw_vmb_list_marked_kernel", "tw_vmb_mesh_count_kernel", "tw_vmb_mesh_scan_kernel", "tw_vmb_mesh_emit_kernel"};
 	cudaKernel_t k[8];
-	int const rc = module_kernels(ctx, "tw_voxel_model_batch.cubin", names, 8, k); if (rc) return rc;
+	int const rc = twi_module_kernels(ctx, "tw_voxel_model_batch.cubin", names, 8, k); if (rc) return rc;
 	*K = ModelBatchKernels{k[0], k[1], k[2], k[3], k[4], k[5], k[6], k[7]};
 	return TW_OK;
 }

@@ -11,6 +11,7 @@
 //   tw3d::create_tiles_async     <->  a frame's new tiles launched in tile_draw_t::update and collected on a later frame   src/tiled_mesh.cpp:2367-2417
 //   tw3d::create_tiles_async_from_heightmap  <->  the same with heightmap-texture tiles (after tw3d::set_heightmap)   src/tiled_mesh.cpp:498-501
 //   tw3d::update_heightmap, tw3d::hmap_tiles_touched  <->  terrain_hmap_manager_t's brush edits and re-applied modmap, and the tiles they change   src/heightmap.cpp:36-58,243-308
+//   tw3d::hmap_tile_ao(_async), hmap_ao_tiles_touched  <->  tile_t::calc_mesh_ao_lighting of heightmap-texture tiles, and the tiles an edit re-shades   src/tiled_mesh.cpp:586-662
 //   tw3d::read_heightmap(_async)  <->  heightmap_t::data brought back in line with the device's image before brushes, write_heightmap_png and saved edits   src/heightmap.cpp:243-308,365-378
 //   tw3d::gen_mesh_async         <->  gen_mesh in ground mode at start-up and on every regeneration, without stalling the frame   src/mesh_gen.cpp:257-355
 //   tw3d::calc_mesh_shadows(lpos, mh, smask, xsize, ysize, ...), tw3d::mesh_shadows_async  <->  calc_mesh_shadows on the ground-mode mesh   src/visibility.cpp:411-517
@@ -477,6 +478,36 @@ inline void hmap_tiles_touched(const int32_t *origins_xy, unsigned ntiles, unsig
 	int const rc = tw_hmap_tiles_touched(&hs, origins_xy, ntiles, zvsize, rects, n, touched);
 	if (rc != TW_OK) {detail::fail(rc, "hmap_tiles_touched: bad argument (no set_heightmap image?)", nullptr);}
 }
+// calc_mesh_ao_lighting (src/tiled_mesh.cpp:586-662) of heightmap-texture tiles, as a job (tw_hmap_tile_ao_launch): ao_lighting = ntiles*stride^2 bytes
+// (host or device) from the tiles' final zvals (host or device, copied during the launch when on the host) and the image set_heightmap gave; the rays read
+// the zvals inside the tile and the image outside it. The job sees every update_heightmap made before the call and none after it; ao_lighting must stay
+// valid until it is ready. tile_set::hmap_ao_async reads the zvals from a tile set instead, and tile_job_pool has the same call on a slot.
+// hmap_ao_tiles_touched names the tiles whose AO an edit of rects can change (a tile's AO reads the texels of its window, 36 cells beyond the tile on each
+// side): re-run the AO of those after update_heightmap.
+namespace detail {
+	inline tiles_job launch_hmap_ao(tw_ctx *c, std::atomic<uint64_t> &jobs, const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const float *zvals,
+	                                tw_tile_set *set, const int32_t *tile_xy, uint8_t *ao_lighting, int tex_edge_mode, const char *what) {
+		tw_hmap_sampler const hs = hmap_sampler(tls().hmap_w, tls().hmap_h, tex_edge_mode);
+		tw_hmap_ao_job const j = {&hs, origins_xy, ntiles, zvsize, globals().HALF_DXY, zvals, set, tile_xy, ao_lighting};
+		uint64_t const number = ++jobs;
+		int const rc = tw_hmap_tile_ao_launch(c, &j);
+		if (rc != TW_OK) {--jobs; fail(rc, what, c);}
+		return tiles_job(c, &jobs, number);
+	}
+}
+inline tiles_job hmap_tile_ao_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const float *zvals, uint8_t *ao_lighting,
+                                    int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	return detail::launch_hmap_ao(ctx(), detail::tls().tile_jobs, origins_xy, ntiles, zvsize, zvals, nullptr, nullptr, ao_lighting, tex_edge_mode, "hmap_tile_ao_async");
+}
+inline void hmap_tile_ao(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const float *zvals, uint8_t *ao_lighting, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	hmap_tile_ao_async(origins_xy, ntiles, zvsize, zvals, ao_lighting, tex_edge_mode).wait();
+}
+inline void hmap_ao_tiles_touched(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const tw_hmap_rect *rects, unsigned n, uint8_t *touched,
+                                  int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+	std::vector<int32_t> win(2*(size_t)ntiles);
+	for (size_t i = 0; i < win.size(); ++i) {win[i] = origins_xy[i] - 36;} // AO_RAY_LEN
+	hmap_tiles_touched(win.data(), ntiles, zvsize - 1 + 72, rects, n, touched, tex_edge_mode);
+}
 inline tiles_job create_tiles_async_from_heightmap(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, float dx, float dy, unsigned erosion_iters_tt, float wpz_max,
                                                    unsigned size, tw_tile_outputs const &out, tw_tile_shading const &shading, tw_tile_shadows const &shadows,
                                                    int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
@@ -690,6 +721,11 @@ public:
 		slot &s = next();
 		return detail::launch_read_heightmap(s.c, s.jobs, hmap16, width, height, rects, n);
 	}
+	// hmap_tile_ao_async (above) on a slot
+	tiles_job hmap_tile_ao_async(const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, const float *zvals, uint8_t *ao_lighting, int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+		slot &s = next();
+		return detail::launch_hmap_ao(s.c, s.jobs, origins_xy, ntiles, zvsize, zvals, nullptr, nullptr, ao_lighting, tex_edge_mode, "tile_job_pool::hmap_tile_ao_async");
+	}
 };
 
 // tile_t::upload_normal_texture (src/tiled_mesh.cpp:865-880, minus the GL upload) and tile_t::calc_mesh_ao_lighting (:586-662) for a batch of
@@ -853,6 +889,16 @@ public:
 		                                               &out, &shading, &frame);
 		if (rc != TW_OK) {detail::fail(rc, "tile_set::create_tiles_async", lc);}
 		return tiles_job(lc, jobs, number);
+	}
+	// hmap_tile_ao_async with the zvals of the resident tiles tile_xy (origins origins_xy): ordered on the device after the set's earlier work on any context,
+	// so it may follow a frame's create_tiles_async at once. On this set's context, or on a slot of `pool`.
+	tiles_job hmap_ao_async(const int32_t *tile_xy, const int32_t *origins_xy, unsigned ntiles, unsigned zvsize, uint8_t *ao_lighting, tile_job_pool *pool = nullptr,
+	                        int tex_edge_mode = TW_HMAP_EDGE_MIRROR) {
+		if (pool) {
+			tile_job_pool::slot &sl = pool->next();
+			return detail::launch_hmap_ao(sl.c, sl.jobs, origins_xy, ntiles, zvsize, nullptr, s, tile_xy, ao_lighting, tex_edge_mode, "tile_set::hmap_ao_async");
+		}
+		return detail::launch_hmap_ao(c, detail::tls().tile_jobs, origins_xy, ntiles, zvsize, nullptr, s, tile_xy, ao_lighting, tex_edge_mode, "tile_set::hmap_ao_async");
 	}
 };
 

@@ -599,7 +599,10 @@ TW_API int tw_read_heightmap(tw_ctx *ctx, const tw_hmap_read *r);
  * tiles sample it under hs, reads a texel inside one of the rects - the live tiles an edit changes. A texel counts as read even where its bilinear weight is 0;
  * cells that read nothing (off the texture in cliff mode) read no texel. Exact, and O(zvsize) per distinct tile column and row: the sampler's index
  * arithmetic is separable per axis. TW_ERR_ARG for a NULL hs, a width or height <= 0, edge_mode outside 0..2, a NULL array with a nonzero count, or
- * zvsize < 2. */
+ * zvsize < 2.
+ * The tiles whose AO map (tw_hmap_tile_ao_launch) an edit can change: the AO of tile t reads the texels of its window, cells [x1 - 36, x1 + zvsize + 35) on
+ * each axis, so this call with origins (x1 - 36, y1 - 36) and zvsize + 71 (= stride + 72) flags them (the C++ adapter's tw3d::hmap_ao_tiles_touched). That is
+ * conservative: texels that only the window's corners read, where no ray goes, count too. */
 TW_API int tw_hmap_tiles_touched(const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, uint32_t zvsize, const tw_hmap_rect *rects,
                                  uint32_t nrects, uint8_t *touched);
 /* min/max over a float array (get_heightmap_z_range, src/map_view.cpp:399-407) */
@@ -913,8 +916,8 @@ TW_API int tw_create_tiles_launch_shadows(tw_ctx *ctx, const int32_t *origins_xy
  * Whether heightmap tiles are eroded is the caller's choice (erosion_iters_tt or 0): this library does not pin the reference's (its test harness cannot reach the heightmap branch of create_zvals, see
  * oracle/refbuild/ref_tiled_harness.inc). tw_create_tiles_poll
  * completes the job; the image must not be replaced before then (tw_set_heightmap completes the job first). p is read only by the weights' jitter noise and
- * may be NULL without weights. No tile limit. Not done: the AO map (calc_mesh_ao_lighting reads a (stride + 72)^2 context around the tile, and what the
- * reference reads outside the tile in this mode is not pinned here). Errors, nothing enqueued: TW_ERR_STATE without tw_set_heightmap; TW_ERR_ARG for hs NULL
+ * may be NULL without weights. No tile limit. Not done here: the AO map, which is its own job on the final zvals (tw_hmap_tile_ao_launch, after the tile set
+ * section). Errors, nothing enqueued: TW_ERR_STATE without tw_set_heightmap; TW_ERR_ARG for hs NULL
  * or sized unlike the image, edge_mode outside 0..2, shading->ao, weights without p, and every error of tw_create_tiles_launch_shadows. */
 TW_API int tw_create_tiles_launch_hmap(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size,
                           float dx, float dy, uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval,
@@ -1048,6 +1051,38 @@ TW_API int  tw_tile_set_create_tiles_launch(tw_ctx *ctx, tw_tile_set *set, const
  * tiles to name in a frame's relight request. TW_ERR_ARG for what stale, remove and put refuse, and a tile both removed and put. */
 TW_API int  tw_tile_set_stale_after(tw_tile_set *set, const tw_shadow_params *sps, uint32_t nlights, const int32_t *remove_xy, uint32_t nremove,
                           const int32_t *put_xy, uint32_t nput, int32_t *tile_xy_out, uint32_t capacity, uint32_t *nstale);
+
+/* ---- the AO map of heightmap-texture tiles: tile_t::calc_mesh_ao_lighting (src/tiled_mesh.cpp:586-662) in the heightmap-texture mode ----
+ * For tile t with origin (x1, y1), zvsize = stride + 1 and final zvals zvals_t (sampled, then eroded when the engine erodes heightmap tiles), ao_t is
+ *   czv_t = tw_heightmap_sample_tiles(image, hs, origin (x1 - 36, y1 - 36), zvsize' = stride + 72)   (get_clamped_height over the window)
+ *   ao_t  = tile_ao(zvals_t, czv_t, zvsize, half_dxy) with use_ao_zvals = 0                           (tw_tile_ao_batch's kernel, CPU-gen-mode flow)
+ * bit for bit: the rays read the tile's own final zvals inside the tile and the image outside it, and start at the final zval. This library defines that AO;
+ * it does not pin the reference's heightmap branch (its test harness cannot reach the heightmap branch of create_zvals, see oracle/refbuild/ref_tiled_harness.inc).
+ * - The job is the context's pending job: tw_create_tiles_poll / tw_heightgen_2d_poll complete it, and tw_hmap_tile_ao is the launch followed by a poll with
+ *   wait = 1. tw_cancel returns TW_ERR_STATE: the job has no cancellation point.
+ * - Image: the job sees the image as it was when its launch returned (every tw_update_heightmap made before it, none after it), and a later edit waits on
+ *   the device for its kernel only. A shared context reads its parent's image; while the root's erosion of the image or a set_image job is pending there is
+ *   no image (TW_ERR_STATE).
+ * - Heights: zvals (ntiles*zvsize^2 floats, device, page-locked or pageable host memory, copied during the launch when on the host), or, with zvals == NULL,
+ *   the resident tiles of `set` named by tile_xy. The job then waits on the device for the set's earlier work (a frame launched just before on any context
+ *   of the family) before it reads the slabs, and orders the set's later work after its reads, as a relight does; ctx may be any context of the set's family.
+ * - ao: ntiles*stride^2 bytes, tile t's at t*stride^2, device or host memory (pageable host memory receives it in the completing poll); it must stay
+ *   valid until then.
+ * - Errors, nothing enqueued: TW_ERR_ARG for a NULL ctx or job, NULL hs, edge_mode outside 0..2, zvsize < 2, both or neither of zvals and set, NULL ao, NULL
+ *   origins_xy (or, with set, tile_xy) with ntiles > 0, hs sized unlike the image, and with set: a context of another family or device, zvsize unlike the
+ *   set's, a tile of tile_xy that is not resident or is named twice; TW_ERR_STATE without an image. ntiles == 0 is TW_OK and does nothing. */
+typedef struct tw_hmap_ao_job {
+	const tw_hmap_sampler *hs;       /* sized like the context's image */
+	const int32_t *origins_xy;       /* ntiles (x1, y1) pairs, as tw_create_tiles_launch_hmap */
+	uint32_t ntiles, zvsize;
+	float half_dxy;                  /* HALF_DXY */
+	const float *zvals;              /* ntiles*zvsize^2, host or device; NULL => read from set */
+	tw_tile_set *set;                /* with zvals == NULL: the resident tiles named by tile_xy */
+	const int32_t *tile_xy;          /* ntiles (x1/size, y1/size) keys, required with set */
+	uint8_t *ao;                     /* ntiles*stride^2 bytes, host or device */
+} tw_hmap_ao_job;
+TW_API int tw_hmap_tile_ao_launch(tw_ctx *ctx, const tw_hmap_ao_job *job);  /* the context's pending job */
+TW_API int tw_hmap_tile_ao(tw_ctx *ctx, const tw_hmap_ao_job *job);         /* launch + waiting poll */
 
 /* ---- terrain weights texture of tiles (SURVEY.md 8f row N4): tile_t::create_texture (src/tiled_mesh.cpp:1071-1248), the terrain part ----
  * RGBA texel (x, y) of a tile, x, y < stride = zvsize - 1: the weights {sand, dirt, grass, rock} (snow = the rest) of the ground textures from the cell's relative

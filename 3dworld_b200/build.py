@@ -9,8 +9,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib3dworld_b200.so")
 SOURCES = ["tw_api.cu", "tw_heightgen.cu", "tw_erosion.cu", "tw_voxel.cu", "tw_streaming.cu", "tw_tiles.cu", "tw_multi.cu", "tw_voxel_post.cu", "tw_shadows.cu", "tw_tileset.cu", "tw_host.cpp"]
-# device code the library loads at run time (cudaLibraryLoadFromFile), each built as <name>.cubin beside the library: the change list of a voxel model
-# edit, the batch of small voxel grids and the batch of small voxel models (tw_voxel_post.cu loads them), and the AO map of heightmap tiles (tw_api.cu)
+# device code the library loads at run time (cudaLibraryLoadFromFile, twi_load_kernel in tw_api.cu), each built as <name>.cubin beside the library: the
+# change list of a voxel model edit, the batch of small voxel grids and the batch of small voxel models (launched by tw_voxel_post.cu), and the AO map of
+# heightmap tiles (launched by tw_api.cu)
 MODULES = ["tw_voxel_changes.cu", "tw_voxel_batch.cu", "tw_voxel_model_batch.cu", "tw_hmap_ao.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fno-fast-math,-fvisibility=hidden", "--use_fast_math=false"]

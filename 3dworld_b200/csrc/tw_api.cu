@@ -3,9 +3,12 @@
 #include "tw_internal.h"
 #include "tw_hmap_ao.h"
 #include <algorithm>
+#include <dlfcn.h>
 #include <stdarg.h>
 #include <stdlib.h>
+#include <mutex>
 #include <new>
+#include <string>
 #include <vector>
 #include <math.h>
 
@@ -57,6 +60,28 @@ int twi_ensure_aux_streams(tw_ctx *ctx) {
 	TW_CUDA(ctx, cudaDeviceGetStreamPriorityRange(&lo, &hi));
 	bool const prio = !(getenv("TW_PIPE_NOPRIO"));
 	for (int i = 0; i < 3; ++i) {TW_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->aux_stream[i], cudaStreamNonBlocking, prio ? hi : lo));}
+	return TW_OK;
+}
+
+int twi_load_kernel(tw_ctx *ctx, const char *file, const char *name, cudaKernel_t *k) {
+	struct Module {std::string file; cudaLibrary_t lib; std::vector<std::pair<std::string, cudaKernel_t>> kernels;}; // the kernels looked up so far
+	static std::mutex mu;
+	static std::vector<Module> loaded;
+	std::lock_guard<std::mutex> g(mu);
+	auto m = std::find_if(loaded.begin(), loaded.end(), [file](const Module &e) {return e.file == file;});
+	if (m == loaded.end()) {
+		Dl_info info;
+		if (!dladdr((void *)&twi_load_kernel, &info) || !info.dli_fname) return tw_set_error(ctx, TW_ERR_CUDA, "cannot locate the library's file");
+		std::string const lib_path = info.dli_fname, path = lib_path.substr(0, lib_path.rfind('/') + 1) + file;
+		cudaLibrary_t l = nullptr;
+		cudaError_t const e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+		if (e != cudaSuccess) {cudaGetLastError(); return tw_set_error(ctx, TW_ERR_CUDA, "cannot load %s: %s", path.c_str(), cudaGetErrorString(e));}
+		m = loaded.insert(loaded.end(), Module{file, l, {}});
+	}
+	for (auto const &e : m->kernels) {if (e.first == name) {*k = e.second; return TW_OK;}}
+	cudaError_t const e = cudaLibraryGetKernel(k, m->lib, name);
+	if (e != cudaSuccess) {cudaGetLastError(); return tw_set_error(ctx, TW_ERR_CUDA, "cannot find %s in %s: %s", name, file, cudaGetErrorString(e));}
+	m->kernels.emplace_back(name, *k);
 	return TW_OK;
 }
 
@@ -1156,10 +1181,9 @@ int tw_hmap_tile_ao_launch(tw_ctx *ctx, const tw_hmap_ao_job *job) {
 	nsub = (stride + side - 1)/side;
 	if ((size_t)n*nsub*nsub > 0x7fffffffu) return tw_set_error(ctx, TW_ERR_ARG, "too many tiles in one job");
 	size_t const ao_bytes = (size_t)n*stride*stride, smem = (size_t)(side + 2*TWI_AO_RAY_LEN)*(side + 2*TWI_AO_RAY_LEN)*sizeof(float);
-	static const char *const names[] = {"tw_hmap_ao_kernel"};
-	cudaKernel_t k;
-	rc = twi_module_kernels(ctx, "tw_hmap_ao.cubin", names, 1, &k); if (rc) return rc;
-	TW_CUDA(ctx, cudaKernelSetAttributeForDevice(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem, ctx->device));
+	TWI_KERNEL(k, "tw_hmap_ao.cubin", tw_hmap_ao_kernel);
+	rc = k.load(ctx); if (rc) return rc;
+	rc = k.max_dynamic_smem(ctx, smem); if (rc) return rc;
 	twi_user<const float> z(job->zvals, job->set ? 0 : (size_t)n*zv*zv);
 	uint8_t *const ao = job->ao;
 	bool const dev_out = tw_is_device_ptr(ao), locked_out = !dev_out && twi_is_page_locked(ao);
@@ -1186,9 +1210,7 @@ int tw_hmap_tile_ao_launch(tw_ctx *ctx, const tw_hmap_ao_job *job) {
 		if (job->set) {TW_CUDA(ctx, cudaMemcpyAsync(d_slots, h_slots, n*sizeof(int), cudaMemcpyHostToDevice, ctx->stream));}
 		int r = z.in(ctx); if (r) return r;
 		if (job->set) {TW_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, set_ev, 0));} // a frame on another context may still write the slab
-		void *args[] = {&A};
-		TW_CUDA(ctx, cudaLaunchKernel((const void *)k, dim3(n*nsub*nsub), dim3(TWI_AO_THREADS), args, smem, ctx->stream));
-		ctx->launches++;
+		r = k.launch(ctx, n*nsub*nsub, TWI_AO_THREADS, smem, A); if (r) return r;
 		TW_CUDA(ctx, cudaEventRecord(ctx->async.image_free, ctx->stream)); // a later edit waits for this kernel only
 		ctx->async.image_free_set = true;
 		if (job->set) {TW_CUDA(ctx, cudaEventRecord(set_ev, ctx->stream));}

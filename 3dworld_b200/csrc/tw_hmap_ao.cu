@@ -3,7 +3,7 @@
 // tw_hmap_ao.cubin beside the library) that the library loads on first use, so the library's own kernels - whose code the tests pin, kernel by kernel - stay
 // exactly as they are. For the same reason the sampler's device helpers are copied here from tw_streaming.cu (hmap_scale_val, hmap_raw_height and
 // hmap_sample_tiles_kernel's cell body) rather than shared; the index arithmetic is tw_hmap_index.cuh's, which the host-only tw_hmap_tiles_touched
-// also uses. The kernel is extern "C" so the loader finds it by name.
+// also uses. The kernel is extern "C" so the loader finds it by name, and declared in tw_hmap_ao.h.
 #include "tw_hmap_ao.h"
 #include "tw_hmap_index.cuh"
 

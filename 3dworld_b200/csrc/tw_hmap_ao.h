@@ -20,3 +20,6 @@ struct twi_hmap_ao_args {
 constexpr int TWI_AO_RAY_LEN = 36;          // AO_RAY_LEN: 8 steps of growing stride, 1 + 2 + ... + 8 cells
 constexpr unsigned TWI_AO_MAX_SIDE = 160;   // (160 + 72)^2 floats = 210.25 KB of shared memory, inside sm_90a's 227 KB opt-in
 constexpr unsigned TWI_AO_THREADS = 1024;
+
+// the module's kernel (tw_hmap_ao.cu), declared once for its definition and the host's launch (tw_api.cu)
+extern "C" __global__ void tw_hmap_ao_kernel(twi_hmap_ao_args A);

@@ -350,9 +350,32 @@ struct twi_job_tail {
 int twi_create_tiles_launch(tw_ctx *ctx, const tw_hmap_sampler *hs, const int32_t *origins_xy, uint32_t ntiles, int mesh_x_size, int mesh_y_size, float dx, float dy,
                             uint32_t zvsize, const tw_height_params *p, uint32_t erosion_iters, const tw_erosion_params *ep, float min_zval, float wpz_max, uint32_t size,
                             const tw_tile_outputs *out, const tw_tile_shading *shading, twi_job_tail *tail);
-// Device code the library loads at run time (build.py's MODULES; tw_voxel_post.cu): the kernels `names` of the sm_90a module `file` beside this library,
-// loaded once per process on first use (cudaLibraryLoadFromFile loads it into each device's context as needed). A missing or unloadable module is an error.
-int twi_module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int count, cudaKernel_t *out);
+// Device code the library loads at run time (build.py's MODULES; tw_api.cu): *k = the kernel `name` of the sm_90a module `file` beside this library. The
+// module is loaded once per process, on the first look-up of one of its kernels (cudaLibraryLoadFromFile loads it into each device's context as needed). A
+// missing or unloadable module, or a kernel it lacks, is TW_ERR_CUDA.
+int twi_load_kernel(tw_ctx *ctx, const char *file, const char *name, cudaKernel_t *k);
+// A module kernel as the host launches it. F is the type of the kernel's extern "C" __global__ declaration, in the header the module shares with the host,
+// so launch() takes the kernel's own parameter types: an argument converts to its parameter's type or does not compile. Declared with TWI_KERNEL, which
+// names the kernel once. load() looks the kernel up, before anything is enqueued; launch() enqueues it on ctx->stream.
+template <typename F> struct twi_kernel;
+template <typename... P> struct twi_kernel<void(P...)> {
+	const char *file, *name;
+	cudaKernel_t k = nullptr;
+	int load(tw_ctx *ctx) {return twi_load_kernel(ctx, file, name, &k);}
+	int max_dynamic_smem(tw_ctx *ctx, size_t bytes) const {
+		TW_CUDA(ctx, cudaKernelSetAttributeForDevice(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes, ctx->device));
+		return TW_OK;
+	}
+	int launch(tw_ctx *ctx, dim3 grid, dim3 block, size_t smem, P... a) const {
+		void *args[] = {(void *)&a...};
+		TW_CUDA(ctx, cudaLaunchKernel((const void *)k, grid, block, args, smem, ctx->stream));
+		ctx->launches++;
+		return TW_OK;
+	}
+};
+#define TWI_KERNEL(var, file, kernel) twi_kernel<decltype(kernel)> var{file, #kernel}
+// load() of each handle, up to the first error
+template <typename... K> int twi_load_kernels(tw_ctx *ctx, K &...k) {int rc = TW_OK; (void)(((rc = k.load(ctx)) == TW_OK) && ...); return rc;}
 // The resident tiles a job reads from a tile set (tw_hmap_tile_ao_launch; tw_tileset.cu): TW_ERR_ARG on ctx unless ctx is of the set's family and device,
 // zvsize is the set's and tile_xy names n distinct resident tiles. slots = their slab slots, *d_z = the zvals slab, *ev = the set's event, which the job
 // waits on before it reads the slab and records once it no longer does.

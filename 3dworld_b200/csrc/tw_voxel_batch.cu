@@ -1,8 +1,8 @@
 // tw_voxel_batch.cu - many small voxel grids built in one job (tw_voxel_build_batch_launch): fill and outside flags, remove_unconnected and the welded mesh of
 // every grid, each step one launch over all grids. Built as its own sm_90a module (build.py: tw_voxel_batch.cubin beside the library) that tw_voxel_post.cu
-// loads on first use, so the library's own kernels - whose code the tests pin - stay exactly as they are. The kernels are extern "C" so the loader finds
-// them by name; each walks the grids through the table of twi_vbatch_grid (tw_voxel_batch.h), finding a launch block's grid by a binary search over the
-// grids' first blocks. The arithmetic is the library's: the fill's epilogue, sine look-up and GLM fBm come from tw_voxel_fill.cuh, the outside flag and the
+// loads on first use, so the library's own kernels - whose code the tests pin - stay exactly as they are. The kernels, declared in tw_voxel_batch.h, are
+// extern "C" so the loader finds them by name; each walks the grids through that header's table of twi_vbatch_grid, finding a launch block's grid by a
+// binary search over the grids' first blocks. The arithmetic is the library's: the fill's epilogue, sine look-up and GLM fBm come from tw_voxel_fill.cuh, the outside flag and the
 // welded mesh's cube from tw_voxel_mc.cuh.
 //   tw_vbatch_tables_kernel  gen_xyz_vals of the sine-mode grids, one thread per (grid, axis, term)
 //   tw_vbatch_fill_kernel    per voxel: the fill (or the input field), the epilogue, the outside flag; blocks of TWI_VB_FILL_VOXELS consecutive voxels
@@ -10,7 +10,6 @@
 //   tw_vbatch_mesh_count_kernel / tw_vbatch_mesh_scan_kernel / tw_vbatch_mesh_emit_kernel   the welded mesh: mesh_kernel's count, the block scan of
 //                            each grid (one CTA per grid) and the emit
 #include "tw_voxel_batch.h"
-#include "tw_voxel_mc.cuh"
 #include "tw_voxel_batch_util.cuh"
 
 // gen_xyz_vals (tw_voxel.cu's xyz_tables_kernel) of grid blockIdx.y, axis blockIdx.x, term threadIdx.x: t[k*pitch + i] (x pre-multiplied by mag), i walked

@@ -3,6 +3,7 @@
 // depend on its size.
 #pragma once
 #include "tw_voxel_fill.cuh"
+#include "tw_voxel_mc.cuh"
 
 // the fill of a grid: none (vals holds the input field), the sine sum, or GLM fBm
 enum {TWI_VB_INPUT = 0, TWI_VB_SINE = 1, TWI_VB_SIMPLEX = 2, TWI_VB_PERLIN = 3};
@@ -26,3 +27,11 @@ struct twi_vbatch_grid {
 	uint32_t *indices; unsigned long long tcap;
 	unsigned long long *counts;                      // [vertices, triangles, voxels flipped by remove_unconnected], zeroed before the batch
 };
+
+// The module's kernels (tw_voxel_batch.cu), declared once for the module's definitions and the host's launches (tw_voxel_post.cu)
+extern "C" __global__ void tw_vbatch_tables_kernel(const twi_vbatch_grid *grids, const float *sin_tab);
+extern "C" __global__ void tw_vbatch_fill_kernel(const twi_vbatch_grid *grids, unsigned ngrids, const float4 *lut);
+extern "C" __global__ void tw_vbatch_flood_kernel(const twi_vbatch_grid *grids);
+extern "C" __global__ void tw_vbatch_mesh_count_kernel(const twi_vbatch_grid *grids, unsigned ngrids, McTables T);
+extern "C" __global__ void tw_vbatch_mesh_scan_kernel(const twi_vbatch_grid *grids);
+extern "C" __global__ void tw_vbatch_mesh_emit_kernel(const twi_vbatch_grid *grids, unsigned ngrids, McTables T);

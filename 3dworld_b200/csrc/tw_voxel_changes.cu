@@ -1,7 +1,7 @@
 // tw_voxel_changes.cu - the change list of a voxel model edit (tw_voxel_model_edit_launch_ex): one change bit per voxel, then the changed voxels in
 // ascending index order. Built as its own sm_90a module (build.py: tw_voxel_changes.cubin beside the library) that tw_voxel_post.cu loads on first use
 // with cudaLibraryLoadFromFile, so the library's own kernels - whose code the tests pin, kernel by kernel - stay exactly as they are. The kernels are
-// extern "C" so the loader finds them by name.
+// extern "C" so the loader finds them by name, and declared in tw_voxel_edit.cuh, which the host's launches also read.
 #include "tw_voxel_edit.cuh"
 
 // rm == 0: box_scatter_kernel that also sets each changed voxel's bit; post is the model's field, bits are zeroed before

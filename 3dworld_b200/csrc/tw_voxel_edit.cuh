@@ -1,6 +1,6 @@
 // tw_voxel_edit.cuh - the pieces of a voxel model edit shared by tw_voxel_post.cu (the library) and tw_voxel_changes.cu (the change-list module, which
 // tw_voxel_post.cu loads at run time): the block grid, the blocks that read a voxel, the edit's boxes and the box scatter. Included by each at file scope;
-// everything here has internal linkage, so each translation unit keeps its own copy and its own kernels' names.
+// everything here but the module's kernel declarations has internal linkage, so each translation unit keeps its own copy and its own kernels' names.
 #pragma once
 #include "../../include/tw3d.h"
 
@@ -55,3 +55,13 @@ __device__ __forceinline__ void box_scatter(const twi_box *__restrict__ boxes, u
 constexpr int CL_BLOCK = 256;
 
 } // namespace
+
+// The change-list module's kernels (tw_voxel_changes.cu), declared once for the module's definitions and the host's launches (tw_voxel_post.cu)
+extern "C" __global__ void tw_box_scatter_bits_kernel(const twi_box *boxes, unsigned nboxes, const float *values, unsigned long long total,
+	tw_voxel_post_params P, const unsigned *zix_xy, BlockGrid G, float *raw, unsigned char *raw_o, float *post, unsigned char *post_o, unsigned char *mark,
+	unsigned *bits);
+extern "C" __global__ void tw_diff_bits_kernel(const float *nv, const unsigned char *no, float *ov, unsigned char *oo, tw_voxel_post_params P, BlockGrid G,
+	unsigned char *mark, size_t n, unsigned *bits);
+extern "C" __global__ void tw_change_count_kernel(const unsigned *bits, size_t nwords, unsigned *sums);
+extern "C" __global__ void tw_change_emit_kernel(const unsigned *bits, size_t nwords, const unsigned long long *offsets, const float *post,
+	const unsigned char *post_o, uint32_t *index, float *vals, uint8_t *outside, unsigned long long capacity);

@@ -32,3 +32,13 @@ struct twi_vmb_model {
 	uint32_t *ch_index; float *ch_vals; uint8_t *ch_outside; unsigned long long ch_cap; // the change list's outputs
 	unsigned long long *counts;                       // [vertices, triangles, voxels flipped, blocks listed, voxels changed], zeroed before the job
 };
+
+// The module's kernels (tw_voxel_model_batch.cu), declared once for the module's definitions and the host's launches (tw_voxel_post.cu)
+extern "C" __global__ void tw_vmb_copy_kernel(const twi_vmb_model *models, unsigned nmodels, int what);
+extern "C" __global__ void tw_vmb_box_scatter_kernel(const twi_vmb_model *models, unsigned nmodels);
+extern "C" __global__ void tw_vmb_diff_kernel(const twi_vmb_model *models, unsigned nmodels);
+extern "C" __global__ void tw_vmb_change_list_kernel(const twi_vmb_model *models);
+extern "C" __global__ void tw_vmb_list_marked_kernel(const twi_vmb_model *models);
+extern "C" __global__ void tw_vmb_mesh_count_kernel(const twi_vmb_model *models, unsigned nmodels);
+extern "C" __global__ void tw_vmb_mesh_scan_kernel(const twi_vmb_model *models);
+extern "C" __global__ void tw_vmb_mesh_emit_kernel(const twi_vmb_model *models, unsigned nmodels);

@@ -15,9 +15,7 @@
 #include "tw_voxel_mc.cuh"
 #include "tw_voxel_batch.h"
 #include "tw_voxel_model_batch.h"
-#include <dlfcn.h>
 #include <algorithm>
-#include <mutex>
 #include <string>
 #include <vector>
 
@@ -1116,60 +1114,22 @@ int validate_changes(tw_ctx *ctx, const tw_voxel_changes *ch, ChangeOut *d) {
 	return TW_OK;
 }
 
-} // namespace
-
-int twi_module_kernels(tw_ctx *ctx, const char *file, const char *const *names, int count, cudaKernel_t *out) {
-	static std::mutex mu;
-	static std::vector<std::pair<std::string, std::vector<cudaKernel_t>>> loaded; // per file, its kernels in the order of names
-	std::lock_guard<std::mutex> g(mu);
-	for (auto const &e : loaded) {if (e.first == file) {for (int k = 0; k < count; ++k) {out[k] = e.second[k];} return TW_OK;}}
-	Dl_info info;
-	if (!dladdr((void *)&tw_voxel_model_edit_launch_ex, &info) || !info.dli_fname) return tw_set_error(ctx, TW_ERR_CUDA, "cannot locate the library's file");
-	std::string const lib_path = info.dli_fname, path = lib_path.substr(0, lib_path.rfind('/') + 1) + file;
-	cudaLibrary_t l = nullptr;
-	cudaError_t e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-	std::vector<cudaKernel_t> k(count);
-	for (int i = 0; i < count && e == cudaSuccess; ++i) {e = cudaLibraryGetKernel(&k[i], l, names[i]);}
-	if (e != cudaSuccess) {
-		cudaGetLastError();
-		if (l) cudaLibraryUnload(l);
-		return tw_set_error(ctx, TW_ERR_CUDA, "cannot load the kernels of %s: %s", path.c_str(), cudaGetErrorString(e));
-	}
-	loaded.emplace_back(file, k);
-	for (int i = 0; i < count; ++i) {out[i] = k[i];}
-	return TW_OK;
-}
-
-namespace {
 // The change-list kernels (tw_voxel_changes.cu), from tw_voxel_changes.cubin
-struct ChangeKernels {cudaKernel_t box_bits, diff_bits, count, emit;};
-int change_kernels(tw_ctx *ctx, ChangeKernels *K) {
-	static const char *const names[] = {"tw_box_scatter_bits_kernel", "tw_diff_bits_kernel", "tw_change_count_kernel", "tw_change_emit_kernel"};
-	cudaKernel_t k[4];
-	int const rc = twi_module_kernels(ctx, "tw_voxel_changes.cubin", names, 4, k); if (rc) return rc;
-	*K = ChangeKernels{k[0], k[1], k[2], k[3]};
-	return TW_OK;
-}
-// one launch of a module kernel on ctx->stream with smem bytes of dynamic shared memory; the arguments must have the kernel's parameter types exactly
-template<typename... A>
-int launch_module_kernel_smem(tw_ctx *ctx, cudaKernel_t k, dim3 grid, unsigned block, size_t smem, A... a) {
-	void *args[] = {(void *)&a...};
-	TW_CUDA(ctx, cudaLaunchKernel((const void *)k, grid, dim3(block), args, smem, ctx->stream));
-	ctx->launches++;
-	return TW_OK;
-}
-template<typename... A>
-int launch_module_kernel(tw_ctx *ctx, cudaKernel_t k, unsigned grid, unsigned block, A... a) {return launch_module_kernel_smem(ctx, k, dim3(grid), block, 0, a...);}
+struct ChangeKernels {
+	static constexpr const char *file = "tw_voxel_changes.cubin";
+	TWI_KERNEL(box_bits, file, tw_box_scatter_bits_kernel); TWI_KERNEL(diff_bits, file, tw_diff_bits_kernel);
+	TWI_KERNEL(count, file, tw_change_count_kernel); TWI_KERNEL(emit, file, tw_change_emit_kernel);
+	int load(tw_ctx *ctx) {return twi_load_kernels(ctx, box_bits, diff_bits, count, emit);}
+};
 
 // the list of the voxels whose bits are set (bits: every word written), its total into the pinned stage
 int enqueue_change_list(tw_ctx *ctx, const tw_voxel_model *m, const ModelScratch &X, const ChangeOut &C, const ChangeKernels &K) {
 	ChangeScratch const &L = X.L;
-	int rc = launch_module_kernel(ctx, K.count, L.nchunks, CL_BLOCK, (const unsigned *)L.bits, L.nwords, L.sums); if (rc) return rc;
+	int rc = K.count.launch(ctx, L.nchunks, CL_BLOCK, 0, L.bits, L.nwords, L.sums); if (rc) return rc;
 	scan_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(L.sums, L.nchunks, L.offsets, L.total);
 	TW_LAUNCH_CHECK(ctx);
 	if (C.capacity) {
-		rc = launch_module_kernel(ctx, K.emit, L.nchunks, CL_BLOCK, (const unsigned *)L.bits, L.nwords, (const unsigned long long *)L.offsets, (const float *)m->post,
-		                          (const unsigned char *)m->post_o, C.index, C.vals, C.outside, C.capacity);
+		rc = K.emit.launch(ctx, L.nchunks, CL_BLOCK, 0, L.bits, L.nwords, L.offsets, m->post, m->post_o, C.index, C.vals, C.outside, C.capacity);
 		if (rc) return rc;
 	}
 	TW_CUDA(ctx, cudaMemcpyAsync(&X.h_stage->nchanged, L.total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1208,7 +1168,7 @@ extern "C" int tw_voxel_model_edit_launch_on(tw_ctx *ctx, tw_voxel_model *m, con
 	if (rm && total) {rc = flood_blocks(ctx, &blocks); if (rc) return rc;}
 	// the change list: only an edit with boxes can change a voxel, so without them the count stays the stage's 0
 	bool const list = ch && total;
-	if (list) {rc = change_kernels(ctx, &K); if (rc) return rc;}
+	if (list) {rc = K.load(ctx); if (rc) return rc;}
 	ModelScratch X;
 	rc = model_scratch(ctx, m, nboxes, total, &X, list); if (rc) return rc;
 	size_t const n = (size_t)P.nx*P.ny*P.nz;
@@ -1221,8 +1181,8 @@ extern "C" int tw_voxel_model_edit_launch_on(tw_ctx *ctx, tw_voxel_model *m, con
 			TW_CUDA(ctx, cudaMemcpyAsync(X.values, X.h_values, total*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 			if (list && !rm) { // the boxes' voxels set their bits one by one
 				TW_CUDA(ctx, cudaMemsetAsync(X.L.bits, 0, X.L.nwords*sizeof(unsigned), ctx->stream));
-				int const r = launch_module_kernel(ctx, K.box_bits, stream_grid(ctx, total), 256u, (const twi_box *)X.boxes, (unsigned)nboxes, (const float *)X.values, total,
-				                                   P, (const unsigned *)m->zix, block_grid(m), m->raw, m->raw_o, m->post, m->post_o, m->mark, X.L.bits);
+				int const r = K.box_bits.launch(ctx, stream_grid(ctx, total), 256, 0, X.boxes, nboxes, X.values, total, P, m->zix, block_grid(m), m->raw, m->raw_o,
+				                                m->post, m->post_o, m->mark, X.L.bits);
 				if (r) return r;
 			}
 			else {
@@ -1235,8 +1195,7 @@ extern "C" int tw_voxel_model_edit_launch_on(tw_ctx *ctx, tw_voxel_model *m, con
 				TW_CUDA(ctx, cudaMemcpyAsync(m->work_o, m->raw_o, n, cudaMemcpyDeviceToDevice, ctx->stream));
 				int const r = enqueue_remove_unconnected(ctx, blocks, m->work, m->work_o, &P, X.f0, X.f1, X.cnt, X.changed); if (r) return r;
 				if (list) {
-					int const r2 = launch_module_kernel(ctx, K.diff_bits, stream_grid(ctx, n), 256u, (const float *)m->work, (const unsigned char *)m->work_o, m->post, m->post_o,
-					                                    P, block_grid(m), m->mark, n, X.L.bits);
+					int const r2 = K.diff_bits.launch(ctx, stream_grid(ctx, n), 256, 0, m->work, m->work_o, m->post, m->post_o, P, block_grid(m), m->mark, n, X.L.bits);
 					if (r2) return r2;
 				}
 				else {
@@ -1313,15 +1272,12 @@ extern "C" int tw_voxel_model_read_launch(tw_ctx *ctx, tw_voxel_model *m, const 
 //                  (host input), mesh words, block sums and offsets]
 //   pinned:        [grid table | counts | tables | sine coefficients | per grid: zix_xy (host input)]
 namespace {
-struct BatchKernels {cudaKernel_t tables, fill, flood, count, scan, emit;};
-int batch_kernels(tw_ctx *ctx, BatchKernels *K) {
-	static const char *const names[] = {"tw_vbatch_tables_kernel", "tw_vbatch_fill_kernel", "tw_vbatch_flood_kernel", "tw_vbatch_mesh_count_kernel",
-	                                    "tw_vbatch_mesh_scan_kernel", "tw_vbatch_mesh_emit_kernel"};
-	cudaKernel_t k[6];
-	int const rc = twi_module_kernels(ctx, "tw_voxel_batch.cubin", names, 6, k); if (rc) return rc;
-	*K = BatchKernels{k[0], k[1], k[2], k[3], k[4], k[5]};
-	return TW_OK;
-}
+struct BatchKernels {
+	static constexpr const char *file = "tw_voxel_batch.cubin";
+	TWI_KERNEL(tables, file, tw_vbatch_tables_kernel); TWI_KERNEL(fill, file, tw_vbatch_fill_kernel); TWI_KERNEL(flood, file, tw_vbatch_flood_kernel);
+	TWI_KERNEL(count, file, tw_vbatch_mesh_count_kernel); TWI_KERNEL(scan, file, tw_vbatch_mesh_scan_kernel); TWI_KERNEL(emit, file, tw_vbatch_mesh_emit_kernel);
+	int load(tw_ctx *ctx) {return twi_load_kernels(ctx, tables, fill, flood, count, scan, emit);}
+};
 // a refusal of entry i of a batch: the helper's message prefixed with the entry's kind and index
 int entry_error(tw_ctx *ctx, const char *kind, uint32_t i, int rc) {
 	std::string const msg = ctx->err;
@@ -1362,9 +1318,10 @@ void vbatch_sine_tables(twi_carve &c, const tw_voxel_post_params &P, bool sine, 
 // the dynamic shared memory of the batch module's fill (the GLM tables, when a grid has a GLM fill) and flood (six bitsets of flood_words words)
 int vbatch_smem(tw_ctx *ctx, const BatchKernels &K, bool any_glm, unsigned flood_words, size_t *lut_bytes, size_t *flood_bytes) {
 	*lut_bytes = any_glm ? (size_t)twn2::LUT3D_N*twn2::SIMPLEX_LUT_COPIES*sizeof(float4) : 0; *flood_bytes = 6*sizeof(unsigned)*(size_t)flood_words;
-	if (*lut_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*lut_bytes, ctx->device));}
-	if (*flood_bytes) {TW_CUDA(ctx, cudaKernelSetAttributeForDevice(K.flood, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*flood_bytes, ctx->device));}
-	if (any_glm) {int const rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
+	int rc;
+	if (*lut_bytes) {rc = K.fill.max_dynamic_smem(ctx, *lut_bytes); if (rc) return rc;}
+	if (*flood_bytes) {rc = K.flood.max_dynamic_smem(ctx, *flood_bytes); if (rc) return rc;}
+	if (any_glm) {rc = twi_ensure_glm3_lut(ctx); if (rc) return rc;}
 	return TW_OK;
 }
 } // namespace
@@ -1411,7 +1368,7 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 		fill_blocks += (g.nvox + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS; mesh_blocks += g.nb;
 	}
 	BatchKernels K;
-	rc = batch_kernels(ctx, &K); if (rc) return rc;
+	rc = K.load(ctx); if (rc) return rc;
 	size_t lut_bytes, flood_bytes;
 	rc = vbatch_smem(ctx, K, any_glm, flood_words, &lut_bytes, &flood_bytes); if (rc) return rc;
 	std::vector<twi_user<float>> V; std::vector<twi_user<const uint32_t>> Z;
@@ -1475,12 +1432,12 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 			if (!G[i].fill) {r = V[i].in(ctx); if (r) return r;}
 			r = Z[i].in(ctx); if (r) return r;
 		}
-		if (nsine) {r = launch_module_kernel_smem(ctx, K.tables, dim3(3, n), 64u, 0, dt, (const float *)ctx->d_sin_table); if (r) return r;}
-		r = launch_module_kernel_smem(ctx, K.fill, dim3(fill_blocks), TWI_VB_FILL_THREADS, lut_bytes, dt, n, (const float4 *)ctx->d_glm3_lut); if (r) return r;
-		if (any_rm) {r = launch_module_kernel_smem(ctx, K.flood, dim3(n), TWI_VB_FLOOD_THREADS, flood_bytes, dt); if (r) return r;}
-		r = launch_module_kernel(ctx, K.count, mesh_blocks, (unsigned)MC_BLOCK, dt, n, T); if (r) return r;
-		r = launch_module_kernel(ctx, K.scan, n, 1024u, dt); if (r) return r;
-		if (any_cap) {r = launch_module_kernel(ctx, K.emit, mesh_blocks, (unsigned)MC_BLOCK, dt, n, T); if (r) return r;}
+		if (nsine) {r = K.tables.launch(ctx, dim3(3, n), 64, 0, dt, ctx->d_sin_table); if (r) return r;}
+		r = K.fill.launch(ctx, fill_blocks, TWI_VB_FILL_THREADS, lut_bytes, dt, n, (const float4 *)ctx->d_glm3_lut); if (r) return r;
+		if (any_rm) {r = K.flood.launch(ctx, n, TWI_VB_FLOOD_THREADS, flood_bytes, dt); if (r) return r;}
+		r = K.count.launch(ctx, mesh_blocks, MC_BLOCK, 0, dt, n, T); if (r) return r;
+		r = K.scan.launch(ctx, n, 1024, 0, dt); if (r) return r;
+		if (any_cap) {r = K.emit.launch(ctx, mesh_blocks, MC_BLOCK, 0, dt, n, T); if (r) return r;}
 		for (uint32_t i = 0; i < n; ++i) {
 			if (G[i].fill || G[i].P.remove_unconnected > 0) {r = V[i].out(ctx); if (r) return r;}
 			if (G[i].b.outside) {TW_CUDA(ctx, cudaMemcpyAsync(G[i].b.outside, D[i].flags, G[i].nvox, cudaMemcpyDefault, ctx->stream));}
@@ -1499,15 +1456,13 @@ extern "C" int tw_voxel_build_batch_launch(tw_ctx *ctx, const tw_voxel_build *gr
 //   download (device -> pinned, one copy):     [counts (8 words per model) | per model: the listed blocks' table]
 //   device only:                                [per model: mesh words (slots x chunks x MC_BLOCK), launch block sums and offsets, sine tables | change bits]
 namespace {
-struct ModelBatchKernels {cudaKernel_t copy, scatter, diff, changes, marked, count, scan, emit;};
-int model_batch_kernels(tw_ctx *ctx, ModelBatchKernels *K) {
-	static const char *const names[] = {"tw_vmb_copy_kernel", "tw_vmb_box_scatter_kernel", "tw_vmb_diff_kernel", "tw_vmb_change_list_kernel",
-	                                    "tw_vmb_list_marked_kernel", "tw_vmb_mesh_count_kernel", "tw_vmb_mesh_scan_kernel", "tw_vmb_mesh_emit_kernel"};
-	cudaKernel_t k[8];
-	int const rc = twi_module_kernels(ctx, "tw_voxel_model_batch.cubin", names, 8, k); if (rc) return rc;
-	*K = ModelBatchKernels{k[0], k[1], k[2], k[3], k[4], k[5], k[6], k[7]};
-	return TW_OK;
-}
+struct ModelBatchKernels {
+	static constexpr const char *file = "tw_voxel_model_batch.cubin";
+	TWI_KERNEL(copy, file, tw_vmb_copy_kernel); TWI_KERNEL(scatter, file, tw_vmb_box_scatter_kernel); TWI_KERNEL(diff, file, tw_vmb_diff_kernel);
+	TWI_KERNEL(changes, file, tw_vmb_change_list_kernel); TWI_KERNEL(marked, file, tw_vmb_list_marked_kernel);
+	TWI_KERNEL(count, file, tw_vmb_mesh_count_kernel); TWI_KERNEL(scan, file, tw_vmb_mesh_scan_kernel); TWI_KERNEL(emit, file, tw_vmb_mesh_emit_kernel);
+	int load(tw_ctx *ctx) {return twi_load_kernels(ctx, copy, scatter, diff, changes, marked, count, scan, emit);}
+};
 
 // The refusals every entry shares: a model that is set, of ctx's family and device, at most TWI_VB_MAX_VOXELS, and not named by an earlier entry
 int batch_model_check(tw_ctx *ctx, const tw_voxel_model *m, uint32_t i, std::vector<const tw_voxel_model *> &seen) {
@@ -1618,11 +1573,11 @@ int launch_model_batch(tw_ctx *ctx, std::vector<BatchModel> &M, unsigned nvb, un
 		TW_CUDA(ctx, cudaMemcpyAsync(D.tab, H.tab, up, cudaMemcpyHostToDevice, ctx->stream));
 		int r = enqueue((const twi_vmb_model *)D.tab, nm, vb0, bb0, (const twi_vbatch_grid *)D.vb); if (r) return r;
 		twi_vmb_model const *const dt = D.tab;
-		if (mb0) {r = launch_module_kernel(ctx, K.count, mb0, (unsigned)MC_BLOCK, dt, nm); if (r) return r;}
-		r = launch_module_kernel(ctx, K.scan, nm, 1024u, dt); if (r) return r;
+		if (mb0) {r = K.count.launch(ctx, mb0, MC_BLOCK, 0, dt, nm); if (r) return r;}
+		r = K.scan.launch(ctx, nm, 1024, 0, dt); if (r) return r;
 		bool any_cap = false;
 		for (BatchModel const &b : M) {any_cap = any_cap || b.d.vcap || b.d.tcap;}
-		if (mb0 && any_cap) {r = launch_module_kernel(ctx, K.emit, mb0, (unsigned)MC_BLOCK, dt, nm); if (r) return r;}
+		if (mb0 && any_cap) {r = K.emit.launch(ctx, mb0, MC_BLOCK, 0, dt, nm); if (r) return r;}
 		TW_CUDA(ctx, cudaMemcpyAsync(H.counts, D.counts, down, cudaMemcpyDeviceToHost, ctx->stream));
 		for (BatchModel const &b : M) {TW_CUDA(ctx, cudaEventRecord(b.m->ev, ctx->stream));}
 		return TW_OK;
@@ -1682,8 +1637,8 @@ extern "C" int tw_voxel_model_build_batch_launch(tw_ctx *ctx, const tw_voxel_mod
 		fill_blocks += (b.d.n + TWI_VB_FILL_VOXELS - 1)/TWI_VB_FILL_VOXELS;
 	}
 	BatchKernels VK; ModelBatchKernels K;
-	rc = batch_kernels(ctx, &VK); if (rc) return rc;
-	rc = model_batch_kernels(ctx, &K); if (rc) return rc;
+	rc = VK.load(ctx); if (rc) return rc;
+	rc = K.load(ctx); if (rc) return rc;
 	size_t lut_bytes, flood_bytes;
 	rc = vbatch_smem(ctx, VK, any_glm, flood_words, &lut_bytes, &flood_bytes); if (rc) return rc;
 	bool const any_in = std::any_of(M.begin(), M.end(), [](const BatchModel &b) {return b.d.in || b.host_in;});
@@ -1710,11 +1665,11 @@ extern "C" int tw_voxel_model_build_batch_launch(tw_ctx *ctx, const tw_voxel_mod
 	};
 	auto enqueue = [&](const twi_vmb_model *dt, unsigned nm, unsigned vox_blocks, unsigned, const twi_vbatch_grid *vb) -> int {
 		int r;
-		if (any_in) {r = launch_module_kernel(ctx, K.copy, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm, (int)TWI_VMB_COPY_IN); if (r) return r;}
-		if (nsine) {r = launch_module_kernel_smem(ctx, VK.tables, dim3(3, n), 64u, 0, vb, (const float *)ctx->d_sin_table); if (r) return r;}
-		r = launch_module_kernel_smem(ctx, VK.fill, dim3(fill_blocks), TWI_VB_FILL_THREADS, lut_bytes, vb, n, (const float4 *)ctx->d_glm3_lut); if (r) return r;
-		r = launch_module_kernel(ctx, K.copy, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm, (int)TWI_VMB_COPY_POST); if (r) return r;
-		if (nflood) {r = launch_module_kernel_smem(ctx, VK.flood, dim3(nflood), TWI_VB_FLOOD_THREADS, flood_bytes, vb + n); if (r) return r;}
+		if (any_in) {r = K.copy.launch(ctx, vox_blocks, TWI_VMB_VOX_THREADS, 0, dt, nm, TWI_VMB_COPY_IN); if (r) return r;}
+		if (nsine) {r = VK.tables.launch(ctx, dim3(3, n), 64, 0, vb, ctx->d_sin_table); if (r) return r;}
+		r = VK.fill.launch(ctx, fill_blocks, TWI_VB_FILL_THREADS, lut_bytes, vb, n, (const float4 *)ctx->d_glm3_lut); if (r) return r;
+		r = K.copy.launch(ctx, vox_blocks, TWI_VMB_VOX_THREADS, 0, dt, nm, TWI_VMB_COPY_POST); if (r) return r;
+		if (nflood) {r = VK.flood.launch(ctx, nflood, TWI_VB_FLOOD_THREADS, flood_bytes, vb + n); if (r) return r;}
 		return TW_OK;
 	};
 	return launch_model_batch(ctx, M, n + nflood, nsine, K, vbatch, enqueue);
@@ -1758,8 +1713,8 @@ extern "C" int tw_voxel_model_edit_batch_launch(tw_ctx *ctx, const tw_voxel_mode
 		}
 	}
 	BatchKernels VK; ModelBatchKernels K;
-	if (nflood) {rc = batch_kernels(ctx, &VK); if (rc) return rc;}
-	rc = model_batch_kernels(ctx, &K); if (rc) return rc;
+	if (nflood) {rc = VK.load(ctx); if (rc) return rc;}
+	rc = K.load(ctx); if (rc) return rc;
 	size_t lut_bytes = 0, flood_bytes = 0;
 	if (nflood) {rc = vbatch_smem(ctx, VK, false, flood_words, &lut_bytes, &flood_bytes); if (rc) return rc;}
 	// batch-module descriptors: one per flooded model (work / work_o)
@@ -1774,14 +1729,14 @@ extern "C" int tw_voxel_model_edit_batch_launch(tw_ctx *ctx, const tw_voxel_mode
 	};
 	auto enqueue = [&](const twi_vmb_model *dt, unsigned nm, unsigned vox_blocks, unsigned box_blocks, const twi_vbatch_grid *vb) -> int {
 		int r;
-		if (box_blocks) {r = launch_module_kernel(ctx, K.scatter, box_blocks, TWI_VMB_BOX_THREADS, dt, nm); if (r) return r;}
+		if (box_blocks) {r = K.scatter.launch(ctx, box_blocks, TWI_VMB_BOX_THREADS, 0, dt, nm); if (r) return r;}
 		if (nflood) {
-			r = launch_module_kernel(ctx, K.copy, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm, (int)TWI_VMB_COPY_WORK); if (r) return r;
-			r = launch_module_kernel_smem(ctx, VK.flood, dim3(nflood), TWI_VB_FLOOD_THREADS, flood_bytes, vb); if (r) return r;
-			r = launch_module_kernel(ctx, K.diff, vox_blocks, TWI_VMB_VOX_THREADS, dt, nm); if (r) return r;
+			r = K.copy.launch(ctx, vox_blocks, TWI_VMB_VOX_THREADS, 0, dt, nm, TWI_VMB_COPY_WORK); if (r) return r;
+			r = VK.flood.launch(ctx, nflood, TWI_VB_FLOOD_THREADS, flood_bytes, vb); if (r) return r;
+			r = K.diff.launch(ctx, vox_blocks, TWI_VMB_VOX_THREADS, 0, dt, nm); if (r) return r;
 		}
-		if (any_list) {r = launch_module_kernel(ctx, K.changes, nm, 1024u, dt); if (r) return r;}
-		return launch_module_kernel(ctx, K.marked, nm, 1024u, dt);
+		if (any_list) {r = K.changes.launch(ctx, nm, 1024, 0, dt); if (r) return r;}
+		return K.marked.launch(ctx, nm, 1024, 0, dt);
 	};
 	return launch_model_batch(ctx, M, nflood, 0, K, vbatch, enqueue);
 }
